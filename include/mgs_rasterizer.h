@@ -16,8 +16,10 @@
  *  - geom/binning/image state buffers are opaque bytes owned by the caller between forward and backward
  *    (rasterizer_impl.h:29-65); their internal layout is private to this library.
  * Differences (supersets) from the reference:
- *  - F, the number of feature channels, is a RUN-TIME argument (0..32) instead of the compile-time
- *    NUM_CHANNELS_language_feature (config.h:16); include_feature == (F > 0 && feature != NULL);
+ *  - F, the number of feature channels, is a RUN-TIME argument (0..MGS_MAX_FEATURE_CHANNELS = 512) instead of the
+ *    compile-time NUM_CHANNELS_language_feature (config.h:16); include_feature == (F > 0 && feature != NULL).
+ *    F > 32 is blended in groups of 32 channels (each group walks the tile lists again, so the blend costs grow with
+ *    ceil(F / 32));
  *  - an optional depth plane (out_depth / dL_dpix_depth) renders view-space z as one more blended channel;
  *  - work is enqueued on `stream` (the reference uses the legacy default stream);
  *  - outputs are fully overwritten: callers need not zero-initialise them.
@@ -41,7 +43,7 @@ extern "C" {
 #define MGS_ERR_CUDA (-3)
 #define MGS_ERR_ALLOC (-4)
 
-#define MGS_MAX_FEATURE_CHANNELS 32
+#define MGS_MAX_FEATURE_CHANNELS 512
 
 /* Allocator callback: return a device pointer to at least `bytes` bytes (any alignment >= 16; the library
  * re-aligns to 128), or NULL.  Replaces std::function<char*(size_t)> (rasterizer.h:32-34). */
@@ -59,7 +61,8 @@ size_t mgs_binning_state_bytes(int num_rendered);
 /*
  * Forward.  Replaces CudaRasterizer::Rasterizer::forward (rasterizer.h:31-60, rasterizer_impl.cu:198-355).
  * Returns num_rendered (R, the number of Gaussian/tile instances), which the caller passes to mgs_backward.
- *   D = active SH degree, M = SH coefficients per Gaussian (0 when shs == NULL), F = feature channels.
+ *   D = active SH degree, M = SH coefficients per Gaussian (0 when shs == NULL), F = feature channels
+ *   (0..MGS_MAX_FEATURE_CHANNELS; larger F returns MGS_ERR_UNSUPPORTED, as do mgs_backward and the multi-view calls).
  *   out_color [3,H,W], out_feature [F,H,W] (ignored when F == 0), out_depth [H,W] or NULL, radii int32 [P].
  * One stream synchronisation happens inside (R is read back to size the binning state), as in the reference
  * (rasterizer_impl.cu:284).
@@ -220,8 +223,10 @@ typedef struct mgs_view {
 	 * [F,H,W], the cosine embedding head (:310-318, loss.py:18-23): loss_acc (device, 2 floats, zeroed by the call) receives
 	 * {sum (render - target)^2, sum_px cos_sim(embed, target)} -- loss_rgb = loss_acc[0] / (3 H W), loss_embed =
 	 * 1 - loss_acc[1] / (H W) -- and cot_color [3,H,W] / cot_feature [F,H,W] receive d loss_rgb / d render and
-	 * d loss_embed / d embed.  Backward: pass those planes as dL_dpix / dL_dpix_F; cot_scale (device, 2 floats, or NULL for 1)
-	 * holds the upstream gradients of the two scalar losses and multiplies the planes on load. */
+	 * d loss_embed / d embed.  With F > 32 a pixel's feature vector spans several channel groups, so the embedding head
+	 * runs in one small kernel behind the blend on the view's stream instead (same outputs).  Backward: pass those planes
+	 * as dL_dpix / dL_dpix_F; cot_scale (device, 2 floats, or NULL for 1) holds the upstream gradients of the two scalar
+	 * losses and multiplies the planes on load. */
 	const float* target_color;
 	const float* target_feature;
 	float* cot_color;

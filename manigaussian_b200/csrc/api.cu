@@ -19,6 +19,9 @@
 namespace mgs {
 
 static thread_local std::string g_err;
+#define MGS_STR_(x) #x
+#define MGS_STR(x) MGS_STR_(x)
+static const char* const bad_width_msg = "feature channel count must be in [0, " MGS_STR(MGS_MAX_FEATURE_CHANNELS) "]";
 
 static int fail(int code, const std::string& msg)
 {
@@ -399,7 +402,7 @@ static int enqueue_binning(const Cloud& c, const mgs_view& w, bool exact_capacit
 static BlendArgs blend_args(const ViewState& s, const mgs_view& w, int F, const float* feature)
 {
 	BlendArgs ba{};
-	ba.W = w.width; ba.H = w.height; ba.grid_x = s.gx; ba.grid_y = s.gy; ba.F = F;
+	ba.W = w.width; ba.H = w.height; ba.grid_x = s.gx; ba.grid_y = s.gy; ba.F = F; ba.groups = blend_groups(F);
 	ba.ranges = s.img.ranges; ba.tile_order = use_tile_order() ? s.img.tile_order : nullptr; ba.point_list = s.bin.point_list; ba.recs = s.bin.recs;
 	ba.rgbd = s.geom.rgbd; ba.feature = F > 0 ? feature : nullptr; ba.bg = w.background;
 	ba.final_T = s.img.final_T; ba.n_contrib = s.img.n_contrib; ba.pix_mask = s.bin.pix_mask; ba.mask_stride = s.bin.mask_stride;
@@ -415,14 +418,24 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, int debug)
 	BlendArgs ba = blend_args(carve_view(w, c.P), w, F, c.feature);
 	ba.want_depth = w.out_depth != nullptr;
 	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth;
+	// the cosine embedding head needs a pixel's whole feature vector: in the blend epilogue when one CTA holds it (F <= 32),
+	// else in a features-only pass of the loss-heads kernel over the planes the blend just wrote
+	const bool embed = w.target_color && w.target_feature && F > 0;
+	const bool embed_after = embed && ba.groups > 1;
 	if (w.target_color) {
-		if (!w.cot_color || !w.loss_acc || (w.target_feature && F > 0 && !w.cot_feature))
+		if (!w.cot_color || !w.loss_acc || (embed && !w.cot_feature))
 			return fail(MGS_ERR_INVALID_ARG, "view: loss heads need cot_color, loss_acc (and cot_feature with target_feature)");
-		ba.tgt_color = w.target_color; ba.tgt_feature = F > 0 ? w.target_feature : nullptr;
+		ba.tgt_color = w.target_color; ba.tgt_feature = (embed && !embed_after) ? w.target_feature : nullptr;
 		ba.cot_color = w.cot_color; ba.cot_feature = w.cot_feature; ba.loss_acc = w.loss_acc;
 		MGS_CUDA(cudaMemsetAsync(w.loss_acc, 0, 2 * sizeof(float), st));
 	}
-	{ StageTimer t_(ST_BLEND_FWD, st); launch_blend_fwd(ba, st); }
+	{
+		StageTimer t_(ST_BLEND_FWD, st);
+		launch_blend_fwd(ba, st);
+		if (embed_after)
+			launch_loss_heads(1, F, w.width * w.height, nullptr, w.out_feature, nullptr, w.target_feature, nullptr, w.cot_feature,
+				w.loss_acc, st);
+	}
 	MGS_STAGE("blend_fwd");
 	return 0;
 }
@@ -532,7 +545,7 @@ int mgs_forward(
 	if (P < 0 || width <= 0 || height <= 0) return fail(MGS_ERR_INVALID_ARG, "bad P/width/height");
 	if (!out_color || !background) return fail(MGS_ERR_INVALID_ARG, "out_color/background are required");
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F))
-		return fail(MGS_ERR_UNSUPPORTED, "feature channel count must be in [0, 32]");
+		return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	if (F > 0 && (!feature_precomp || !out_feature)) F = 0;  // include_feature == false
 	const size_t N = (size_t)width * height;
 	if (P == 0) {
@@ -592,7 +605,7 @@ int mgs_backward(
 {
 	if (P < 0 || width <= 0 || height <= 0 || R < 0) return fail(MGS_ERR_INVALID_ARG, "bad P/R/width/height");
 	if (P == 0) return 0;
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "feature channel count must be in [0, 32]");
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	if (F > 0 && (!feature_precomp || !dL_dpix_F || !dL_dfeature)) F = 0;
 	if (!geometry_state || !binning_state || !image_state || !blend_scratch)
 		return fail(MGS_ERR_INVALID_ARG, "state buffers and scratch are required");
@@ -623,7 +636,7 @@ int mgs_forward_views(
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
 	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours");
 	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, "feature channel count must be in [0, 32]");
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int v = 0; v < V; v++) {
 		const mgs_view& w = views[v];
 		if (!w.viewmatrix || !w.projmatrix || !w.background || !w.geometry_state || !w.binning_state || !w.image_state || !w.out_color || !w.radii)
@@ -669,7 +682,7 @@ int mgs_backward_views(
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !dL_dmean3D || !dL_dopacity) return fail(MGS_ERR_INVALID_ARG, "means3D, dL_dmean3D and dL_dopacity are required");
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "feature channel count must be in [0, 32]");
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	if (F > 0 && (!feature_precomp || !dL_dfeature)) F = 0;
 	for (int v = 0; v < V; v++) {
 		const mgs_view& w = views[v];

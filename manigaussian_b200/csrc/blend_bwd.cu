@@ -61,7 +61,8 @@ constexpr int BWD_MT = BWD_CH / 16;       // 16-row tiles of Gaussians
 static_assert(BWD_CH == 16 || BWD_CH == 32, "backward chunk size");
 static_assert(BWD_BATCH % 32 == 0, "backward record batch");
 
-template <int NFT, bool VEC>
+// GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic
+template <int NFT, bool VEC, bool GRP>
 __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendArgs a)
 {
 	constexpr int NT = NFT + 1;          // channel tiles of 8: NFT feature tiles + {r,g,b,depth, 4 x zero}
@@ -86,7 +87,11 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	const int lane = threadIdx.x;
 	const int gid = lane >> 2, tig = lane & 3;
 	const int sub = blockIdx.x & 7;
-	const int tile = a.tile_order ? (int)a.tile_order[blockIdx.x >> 3] : (int)(blockIdx.x >> 3);  // longest lists first
+	// channel group (BlendArgs::groups): dL/dalpha is linear in c . g, so it splits over the groups.  Group g takes its own
+	// (c . g)_g and S_g; only group 0 carries the {r,g,b,depth} cotangents and the background term.
+	const int grp = GRP ? (int)(blockIdx.x >> 3) % a.groups : 0;
+	const int rank = GRP ? (int)(blockIdx.x >> 3) / a.groups : (int)(blockIdx.x >> 3);
+	const int tile = a.tile_order ? (int)a.tile_order[rank] : rank;  // longest lists first
 	const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
 	const int bx0 = tile_x * TILE_X + (sub & 1) * WARP_BX;
 	const int by0 = tile_y * TILE_Y + (sub >> 1) * WARP_BY;
@@ -95,21 +100,26 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	const float fbx0 = (float)bx0, fby0 = (float)by0;
 	const size_t HW = (size_t)a.H * a.W;
 	const size_t pix = (size_t)a.W * pyi + pxi;
-	const int F = a.F;
+	const int F = a.F;                 // feature row stride
+	const int c0 = 32 * grp;           // first channel of the group
+	const int Fg = GRP ? min(F - c0, 32) : F;  // channels of the group
+	const bool first = grp == 0;
 
 	// ---- per-pixel state and cotangent rows ----
 	uint32_t nc = 0;
 	float T = 0.f, bgterm = 0.f;
 	{
-		float g4[4] = { 0.f, 0.f, 0.f, 0.f };
+		float g4[4] = { 0.f, 0.f, 0.f, 0.f };  // zero in groups >= 1: no colour / depth gradient, no background term
 		// upstream gradients of the fused loss heads (loss_heads.cuh): the cotangent planes were written for d loss = 1
 		const float sc_color = a.cot_scale ? a.cot_scale[0] : 1.f, sc_feat = a.cot_scale ? a.cot_scale[1] : 1.f;
 		if (inside) {
 			nc = a.n_contrib[pix];
 			T = a.final_T[pix];
+			if (first) {
 #pragma unroll
-			for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
-			if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
+				for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
+				if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
+			}
 		}
 		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2]);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
@@ -118,7 +128,7 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 		if (NFT > 0) {
 #pragma unroll
 			for (int i = 0; i < 8 * NFT; i++)
-				grow[2 * i] = (inside && i < F && a.dL_dfeature) ? sc_feat * a.dL_dfeature[(size_t)i * HW + pix] : 0.f;
+				grow[2 * i] = (inside && i < Fg && a.dL_dfeature) ? sc_feat * a.dL_dfeature[(size_t)(c0 + i) * HW + pix] : 0.f;
 		}
 	}
 	uint32_t maxc = nc;
@@ -169,7 +179,10 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				for (int it = 0; it < BWD_CH / RPI; it++) {
 					const int r = it * RPI + sub;
 					const uint32_t id = __shfl_sync(0xffffffffu, myid, r);
-					if (r < cnt) cp_async16(s_rows + r * RS + 4 * q, reinterpret_cast<const float4*>(a.feature + (size_t)id * (8 * NFT)) + q);
+					// a remainder group (Fg < 32) copies its 4-channel pieces only: the columns behind them hold finite leftovers
+					// of the wgt tile, and their cotangents are zero
+					const float* frow = a.feature + (GRP ? (size_t)id * F + c0 : (size_t)id * (8 * NFT));
+					if (r < cnt && (!GRP || 4 * q < Fg)) cp_async16(s_rows + r * RS + 4 * q, reinterpret_cast<const float4*>(frow) + q);
 				}
 			}
 			if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
@@ -180,9 +193,9 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			float* row = s_rows + lane * RS;
 			*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
 			if (NFT > 0) {
-				const float* f = a.feature + (size_t)id * F;
+				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
-				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < F) ? __ldg(f + i) : 0.f;
+				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < Fg) ? __ldg(f + i) : 0.f;
 			}
 		}
 		__syncwarp();
@@ -334,12 +347,14 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 				if (NFT > 0 && g < cnt && a.dL_dfeat) {
 					const uint32_t id = __float_as_uint(s_q[2 * g + 1].w);
-					float* df = a.dL_dfeat + (size_t)id * F;
+					float* df = a.dL_dfeat + (size_t)id * F + c0;
 					// column 2 tig + e of feature tile nt is feature NFT (2 tig + e) + nt
 					if (VEC) {
-						if (NFT == 4) {
-							red_add_v4(df + 8 * tig, dC[mt][0][2 * h], dC[mt][1][2 * h], dC[mt][2][2 * h], dC[mt][3][2 * h]);
-							red_add_v4(df + 8 * tig + 4, dC[mt][0][2 * h + 1], dC[mt][1][2 * h + 1], dC[mt][2][2 * h + 1], dC[mt][3][2 * h + 1]);
+						if (NFT == 4) {  // Fg % 4 == 0 here
+							if (!GRP || 8 * tig < Fg)
+								red_add_v4(df + 8 * tig, dC[mt][0][2 * h], dC[mt][1][2 * h], dC[mt][2][2 * h], dC[mt][3][2 * h]);
+							if (!GRP || 8 * tig + 4 < Fg)
+								red_add_v4(df + 8 * tig + 4, dC[mt][0][2 * h + 1], dC[mt][1][2 * h + 1], dC[mt][2][2 * h + 1], dC[mt][3][2 * h + 1]);
 						} else if (NFT == 2) {
 							red_add_v4(df + 4 * tig, dC[mt][0][2 * h], dC[mt][1 % NT][2 * h], dC[mt][0][2 * h + 1], dC[mt][1 % NT][2 * h + 1]);
 						} else {
@@ -352,7 +367,7 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 #pragma unroll
 							for (int e = 0; e < 2; e++) {
 								const int f = NFT * (2 * tig + e) + nt;
-								if (f < F) red_add(df + f, dC[mt][nt][2 * h + e]);
+								if (f < Fg) red_add(df + f, dC[mt][nt][2 * h + e]);
 							}
 						}
 					}
@@ -376,7 +391,7 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			float* gb = a.gb + (size_t)__float_as_uint(r1.w) * GB_STRIDE;
 			red_add_v4(gb, dmx, dmy, -0.5f * q_dxx, -0.5f * q_dxy);
 			red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
-			red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);
+			if (first) red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}: zero in the other groups
 		}
 		// the (< 32) survivors behind the chunk move to the head of the queue
 		const int left = qcount - cnt;
@@ -440,23 +455,24 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 
 bool feature_rows_vectorizable(const float* feature, int F);
 
-template <int NFT>
+template <int NFT, bool GRP>
 static void launch_bwd_t(const BlendArgs& a, cudaStream_t s)
 {
-	const int grid = a.grid_x * a.grid_y * 8;
-	const bool vec = (NFT == 0) || (a.F == 8 * NFT && feature_rows_vectorizable(a.feature, a.F) &&
+	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
+	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F) &&
 		(reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0);
-	if (vec) blend_bwd_kernel<NFT, true><<<grid, 32, 0, s>>>(a);
-	else blend_bwd_kernel<NFT, false><<<grid, 32, 0, s>>>(a);
+	if (vec) blend_bwd_kernel<NFT, true, GRP><<<grid, 32, 0, s>>>(a);
+	else blend_bwd_kernel<NFT, false, GRP><<<grid, 32, 0, s>>>(a);
 }
 
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
 {
+	if (a.groups > 1) { launch_bwd_t<4, true>(a, s); return; }
 	switch (nft_for(a.F)) {
-	case 0: launch_bwd_t<0>(a, s); break;
-	case 1: launch_bwd_t<1>(a, s); break;
-	case 2: launch_bwd_t<2>(a, s); break;
-	default: launch_bwd_t<4>(a, s); break;
+	case 0: launch_bwd_t<0, false>(a, s); break;
+	case 1: launch_bwd_t<1, false>(a, s); break;
+	case 2: launch_bwd_t<2, false>(a, s); break;
+	default: launch_bwd_t<4, false>(a, s); break;
 	}
 }
 

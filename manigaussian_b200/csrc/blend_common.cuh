@@ -1,7 +1,8 @@
 // Shared by the forward and backward blend kernels.
 //
 // Work decomposition: ONE WARP = ONE CTA = one 8x4 pixel block of a 16x16 tile (tile ids / work lists stay the
-// reference's 16x16 tiles; eight single-warp CTAs share a tile's list).  A warp streams the tile's sorted 32-byte
+// reference's 16x16 tiles; eight single-warp CTAs share a tile's list, 8 G with G channel groups of 32 features when
+// F > 32, BlendArgs::groups).  A warp streams the tile's sorted 32-byte
 // instance records through its own RING-deep shared-memory ring with 1-D TMA bulk copies (SASS UBLKCP), one copy per
 // batch of records tracked by an mbarrier, keeps the records whose footprint reaches its block (one bit per block in the
 // record, set by the binning stage) and works on the survivors.  No CTA-wide barrier exists anywhere: warps of a heavy

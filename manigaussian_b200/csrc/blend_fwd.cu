@@ -25,6 +25,7 @@
 //    (survivor 8 ks + tig + 4 e), so {a0..a3} of one 16-pixel tile is ONE LDS.128 and the hi/lo split writes the second
 //    quad; the B pair {b0, b1} (survivors g0, g1, feature 8 nt + gid) is two conflict-free scalar loads of the channel rows;
 //    with x = gid the output planes are written as full 32-byte sectors straight from the D fragments.
+#include "../../include/mgs_rasterizer.h"
 #include "blend_common.cuh"
 #include "blend_mma.cuh"
 #include "loss_heads.cuh"
@@ -45,7 +46,8 @@ constexpr int FWD_QCAP = FWD_CH + 32;     // survivor queue: a chunk plus the su
 constexpr int FWD_BATCH = MGS_FWD_BATCH;  // records per bulk copy (a multiple of the 32-record cull chunk)
 static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32 && FWD_BATCH % 32 == 0, "forward chunk size");
 
-template <int NFT, bool VEC>
+// GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic
+template <int NFT, bool VEC, bool GRP>
 __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendArgs a)
 {
 	using L = RowLayout<NFT>;
@@ -64,7 +66,10 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	const int lane = threadIdx.x;
 	const int gid = lane >> 2, tig = lane & 3;
 	const int sub = blockIdx.x & 7;
-	const int tile = a.tile_order ? (int)a.tile_order[blockIdx.x >> 3] : (int)(blockIdx.x >> 3);  // longest lists first
+	// channel group (BlendArgs::groups): the walk is deterministic, so every group's CTA derives the same weights w = alpha T
+	const int grp = GRP ? (int)(blockIdx.x >> 3) % a.groups : 0;
+	const int rank = GRP ? (int)(blockIdx.x >> 3) / a.groups : (int)(blockIdx.x >> 3);
+	const int tile = a.tile_order ? (int)a.tile_order[rank] : rank;  // longest lists first
 	const int tile_x = tile % a.grid_x, tile_y = tile / a.grid_x;
 	const int bx0 = tile_x * TILE_X + (sub & 1) * WARP_BX;
 	const int by0 = tile_y * TILE_Y + (sub >> 1) * WARP_BY;
@@ -73,7 +78,10 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	const bool inside = pxi < a.W && pyi < a.H;
 	if (__all_sync(0xffffffffu, !inside)) return;  // block entirely outside the image (ragged right/bottom tiles)
 	const float pfx = (float)pxi, pfy = (float)pyi;
-	const int F = a.F;
+	const int F = a.F;                 // feature row stride
+	const int c0 = 32 * grp;           // first channel of the group
+	const int Fg = GRP ? min(F - c0, 32) : F;  // channels of the group
+	const bool first = grp == 0;       // group 0 also blends {r,g,b,depth} and writes the per-pixel state
 
 	// rows beyond a short last chunk are multiplied by zero weights: they must hold finite numbers
 	for (int i = lane; i < FWD_CH * RS / 4; i += 32) reinterpret_cast<float4*>(s_rows)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -117,19 +125,21 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				for (int it = 0; it < FWD_CH / RPI; it++) {
 					const int r = it * RPI + sub;
 					const uint32_t id = __shfl_sync(0xffffffffu, myid, r);
-					if (r < cnt) cp_async16(s_rows + r * RS + 4 * q, reinterpret_cast<const float4*>(a.feature + (size_t)id * (8 * NFT)) + q);
+					// a remainder group (Fg < 32) copies its 4-channel pieces only: the rest of the row keeps the zeros of the clear
+					const float* frow = a.feature + (GRP ? (size_t)id * F + c0 : (size_t)id * (8 * NFT));
+					if (r < cnt && (!GRP || 4 * q < Fg)) cp_async16(s_rows + r * RS + 4 * q, reinterpret_cast<const float4*>(frow) + q);
 				}
 			}
-			if (lane < cnt) cp_async16(s_rows + lane * RS + L::RGBD, a.rgbd + myid);
+			if (lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD, a.rgbd + myid);
 			cp_async_commit();
 		} else if (lane < cnt) {  // feature rows that are not whole 8-wide tiles (e.g. F = 3): plain loads, zero padded
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
-			*reinterpret_cast<float4*>(row + L::RGBD) = a.rgbd[id];
+			if (first) *reinterpret_cast<float4*>(row + L::RGBD) = a.rgbd[id];
 			if (NFT > 0) {
-				const float* f = a.feature + (size_t)id * F;
+				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
-				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < F) ? __ldg(f + i) : 0.f;
+				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < Fg) ? __ldg(f + i) : 0.f;
 			}
 		}
 		// ---- walk: one k-step (8 survivors) per trip, in two passes so that the eight footprint evaluations (independent:
@@ -168,7 +178,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			// The backward reads the masks of the queued survivors at positions <= max n_contrib of the block, and every one of
 			// them is walked here: a k-step is only skipped once every pixel has terminated, i.e. behind every pixel's last
 			// contributor.  So the array needs no clearing.
-			if (lane < 8 && 8 * ks + lane < cnt) mrow[__float_as_uint(q4[2 * lane + 1].z) - 1u] = s_pm[8 * ks + lane];
+			if (first && lane < 8 && 8 * ks + lane < cnt) mrow[__float_as_uint(q4[2 * lane + 1].z) - 1u] = s_pm[8 * ks + lane];
 		}
 		const int nk = ks;  // k-steps to contract
 		if (VEC) cp_async_wait<0>();
@@ -196,7 +206,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				mma_3xtf32(acc[0][nt], ahi[0], alo[0], bh0, bh1, bl0, bl1);
 				mma_3xtf32(acc[1][nt], ahi[1], alo[1], bh0, bh1, bl0, bl1);
 			}
-			{
+			if (first) {
 				const float c0 = gid < 4 ? row0[L::RGBD + gid] : 0.f;
 				const float c1 = gid < 4 ? row1[L::RGBD + gid] : 0.f;
 				uint32_t bh0, bl0, bh1, bl1;
@@ -264,16 +274,18 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	// ---- outputs ----
 	const size_t HW = (size_t)a.H * a.W;
 	if (inside) {
-		const size_t pix = (size_t)a.W * pyi + pxi;
 		T = T_out;
-		a.final_T[pix] = T;
-		a.n_contrib[pix] = last_contributor;
+		if (first) {
+			const size_t pix = (size_t)a.W * pyi + pxi;
+			a.final_T[pix] = T;
+			a.n_contrib[pix] = last_contributor;
+		}
 	}
 	s_w[lane] = T;
 	__syncwarp();
 	const int ox = bx0 + gid;  // fragment role: this thread holds pixels (x = gid, y = 0..3)
-	const bool heads = a.tgt_color != nullptr;              // fused loss heads (loss_heads.cuh)
-	const bool embed = heads && NFT > 0 && a.tgt_feature != nullptr;
+	const bool heads = first && a.tgt_color != nullptr;     // fused loss heads (loss_heads.cuh)
+	const bool embed = heads && NFT > 0 && a.tgt_feature != nullptr && !GRP;
 	const float invN = 1.0f / (float)HW;
 	float s_rgb = 0.f, s_cos = 0.f;                         // this thread's share of the two loss sums
 #pragma unroll
@@ -289,7 +301,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 #pragma unroll
 				for (int e = 0; e < 2; e++) {
 					const int f = 8 * nt + 2 * tig + e;
-					if (in && f < F) a.out_feature[(size_t)f * HW + pix] = acc[mt][nt][2 * h + e];
+					if (in && f < Fg) a.out_feature[(size_t)(c0 + f) * HW + pix] = acc[mt][nt][2 * h + e];
 				}
 			}
 			float col[2];
@@ -297,6 +309,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			for (int e = 0; e < 2; e++) {
 				const int c = 2 * tig + e;  // column of the {r,g,b,depth} tile
 				col[e] = acc[mt][NFT][2 * h + e] + (c < 3 ? Tp * a.bg[c] : 0.f);
+				if (!first) continue;
 				if (in && c < 3) a.out_color[(size_t)c * HW + pix] = col[e];
 				else if (in && c == 3 && a.out_depth) a.out_depth[pix] = col[e];
 			}
@@ -361,7 +374,9 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 #endif
 }
 
-int blend_supported(int F) { return F >= 0 && F <= 32; }
+// F > 32 runs in channel groups of 32 (BlendArgs::groups), each with the F = 32 instantiations
+int blend_supported(int F) { return F >= 0 && F <= MGS_MAX_FEATURE_CHANNELS; }
+int blend_groups(int F) { return F > 32 ? ceil_div(F, 32) : 1; }
 
 // 128-bit feature copies need 16-byte aligned rows of a 16-byte multiple
 bool feature_rows_vectorizable(const float* feature, int F)
@@ -369,24 +384,27 @@ bool feature_rows_vectorizable(const float* feature, int F)
 	return F > 0 && (F & 3) == 0 && (reinterpret_cast<uintptr_t>(feature) & 15) == 0;
 }
 
-template <int NFT>
+template <int NFT, bool GRP>
 static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 {
-	const int grid = a.grid_x * a.grid_y * 8;
-	// the cp.async row gather copies whole 8-wide feature tiles: exact fits only; other widths take the padded path
-	const bool vec = (NFT == 0) || (a.F == 8 * NFT && feature_rows_vectorizable(a.feature, a.F));
-	if (vec) blend_fwd_kernel<NFT, true><<<grid, 32, 0, s>>>(a);
-	else blend_fwd_kernel<NFT, false><<<grid, 32, 0, s>>>(a);
+	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
+	// the cp.async row gather copies whole 8-wide feature tiles: exact fits only; other widths take the padded path.  With
+	// groups, a row slice starts at channel 32 g: 16-byte aligned whenever F % 4 == 0, and a remainder group copies whole
+	// 4-channel pieces only.
+	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F));
+	if (vec) blend_fwd_kernel<NFT, true, GRP><<<grid, 32, 0, s>>>(a);
+	else blend_fwd_kernel<NFT, false, GRP><<<grid, 32, 0, s>>>(a);
 }
 
 
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s)
 {
+	if (a.groups > 1) { launch_fwd_t<4, true>(a, s); return; }
 	switch (nft_for(a.F)) {
-	case 0: launch_fwd_t<0>(a, s); break;
-	case 1: launch_fwd_t<1>(a, s); break;
-	case 2: launch_fwd_t<2>(a, s); break;
-	default: launch_fwd_t<4>(a, s); break;
+	case 0: launch_fwd_t<0, false>(a, s); break;
+	case 1: launch_fwd_t<1, false>(a, s); break;
+	case 2: launch_fwd_t<2, false>(a, s); break;
+	default: launch_fwd_t<4, false>(a, s); break;
 	}
 }
 

@@ -14,15 +14,18 @@ __global__ void __launch_bounds__(256) loss_heads_kernel(int V, int F, int N, co
 	const bool in = px < N;
 	const float invN = 1.0f / (float)N;
 	float s_rgb = 0.f, s_cos = 0.f;
+	const bool emb = F > 0 && feature && tgt_feature;
 	if (in) {
-		const size_t cb = (size_t)v * 3 * N + px;
+		if (color) {  // null: features only (the blend epilogue did the colour head; F > 32)
+			const size_t cb = (size_t)v * 3 * N + px;
 #pragma unroll
-		for (int c = 0; c < 3; c++) {
-			const float d = color[cb + (size_t)c * N] - tgt_color[cb + (size_t)c * N];
-			s_rgb += d * d;
-			cot_color[cb + (size_t)c * N] = (2.0f / 3.0f) * invN * d;
+			for (int c = 0; c < 3; c++) {
+				const float d = color[cb + (size_t)c * N] - tgt_color[cb + (size_t)c * N];
+				s_rgb += d * d;
+				cot_color[cb + (size_t)c * N] = (2.0f / 3.0f) * invN * d;
+			}
 		}
-		if (F > 0 && feature && tgt_feature) {
+		if (emb) {
 			const size_t fb = (size_t)v * F * N + px;
 			float xy = 0.f, xx = 0.f, yy = 0.f;
 			for (int f = 0; f < F; f++) {
@@ -41,8 +44,8 @@ __global__ void __launch_bounds__(256) loss_heads_kernel(int V, int F, int N, co
 		s_cos += __shfl_xor_sync(0xffffffffu, s_cos, o);
 	}
 	if ((threadIdx.x & 31) == 0) {
-		red_add(loss_acc + 2 * v, s_rgb);
-		if (F > 0 && feature && tgt_feature) red_add(loss_acc + 2 * v + 1, s_cos);
+		if (color) red_add(loss_acc + 2 * v, s_rgb);
+		if (emb) red_add(loss_acc + 2 * v + 1, s_cos);
 	}
 }
 

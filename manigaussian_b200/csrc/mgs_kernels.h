@@ -73,9 +73,12 @@ struct ProjectBwdViewsArgs {
 struct BlendArgs {
 	int W, H;
 	int grid_x, grid_y;
-	int F;                       // user feature channels (0 = none)
+	int F;                       // user feature channels (0 = none): also the row stride of feature / dL_dfeat
+	// Channel groups: G = ceil(F / 32) (1 when F <= 32); group g blends channels [32 g, min(F, 32 g + 32)).  Every group
+	// walks the same tile list; CTA index = (tile rank, group, 8x4 block), the group varying faster than the rank.
+	int groups;
 	const uint2* ranges;         // [T]
-	const uint32_t* tile_order;  // [T] launch order of the tiles (CTA group i works on tile tile_order[i]); null = identity
+	const uint32_t* tile_order;  // [T] launch order of the tiles (tile rank i works on tile tile_order[i]); null = identity
 	const uint32_t* point_list;  // [R] sorted Gaussian ids
 	const InstRec* recs;         // [R] sorted packed records
 	const float4* rgbd;          // [P] {r,g,b,depth}
@@ -98,6 +101,7 @@ struct BlendArgs {
 	float* dL_dfeat;             // [P,F] (zeroed by caller) nullable
 	// fused loss heads (loss_heads.cuh), all nullable.  Forward: with tgt_color the epilogue also writes the cotangent planes
 	// cot_color [3,H,W] (and, with tgt_feature, cot_feature [F,H,W]) and adds {sum (x-g)^2, sum_px cos} into loss_acc[0..1].
+	// tgt_feature only with groups == 1: the cosine needs a pixel's whole feature vector, which one CTA then holds.
 	// Backward: cot_scale[0..1] (device) multiply the colour / feature cotangent planes on load (the upstream gradients of
 	// the two scalar losses).
 	const float* tgt_color;
@@ -112,7 +116,8 @@ struct BlendArgs {
 	unsigned long long* cta_log; unsigned int* cta_log_n; unsigned int cta_log_cap;
 #endif
 };
-// loss_heads.cu: the same heads for images that already sit in memory (planar [3,H,W] / [F,H,W], V views in one launch)
+// loss_heads.cu: the same heads for images that already sit in memory (planar [3,H,W] / [F,H,W], V views in one launch).
+// color == null: features only -- the embedding head alone, into loss_acc[2 v + 1] (the colour head ran elsewhere).
 void launch_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* tgt_color, const float* tgt_feature,
 	float* cot_color, float* cot_feature, float* loss_acc, cudaStream_t s);
 
@@ -171,6 +176,7 @@ void launch_ranges_and_pack(const uint32_t* R_dev, int capacity, int num_tiles, 
 
 // blend_fwd.cu / blend_bwd.cu
 int blend_supported(int F);
+int blend_groups(int F);  // channel groups of 32 (BlendArgs::groups)
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s);
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
 

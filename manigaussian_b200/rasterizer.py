@@ -8,8 +8,9 @@ ManiGaussian's agents/manigaussian_bc/gaussian_renderer/__init__.py:14-94 runs u
 device memory, streams and autograd plumbing only; all computation happens in the sm_90a library behind
 include/mgs_rasterizer.h.
 
-Supersets of the reference: the feature width F is read from the tensor at run time (0..32) instead of being
-compiled in (config.h:16), and `return_depth=True` adds a view-space depth plane.
+Supersets of the reference: the feature width F is read from the tensor at run time (0..512) instead of being
+compiled in (config.h:16; widths above 32 blend in groups of 32 channels), and `return_depth=True` adds a view-space
+depth plane.
 """
 from typing import NamedTuple
 
