@@ -322,11 +322,16 @@ int mgs_activate_backward(int P, int F,
  *             "clamped" u8[P] (3 bits), "extent" f32[2P]
  *   binning : "point_list" u32[R] (== the reference's point_list), "tile_ids" u32[R] (== high word of the reference's
  *             sorted keys; the low word is the depth bits of point_list[i]), "point_list_unsorted" u32[R],
- *             "tile_ids_unsorted" u32[R], "records" 32-byte records [R], "pixel_masks" u32[8][S] with S = (R + 11) & ~3
- *             (row = 8x4 block of the tile, bit x * 4 + y = the instance contributed to pixel (x, y) of the block; written
- *             by the forward blend only where the backward reads it, other words are undefined)
+ *             "tile_ids_unsorted" u32[R], "records" 32-byte records [R], "block_bits" u8[R] (bit s = the instance can
+ *             reach 8x4 block s of its tile, s = 2 * (y / 4) + x / 8), "block_lists" u32[8][S] with S = (R + 11) & ~3
+ *             (row s, entries range.x .. range.x + block_count - 1 of a tile: the 0-based tile-list positions of the
+ *             instances with bit s set, in list order), "pixel_masks" u32[8][S] (same rows and slots, per block-list
+ *             entry: bit x * 4 + y = the instance contributed to pixel (x, y) of the block; written by the forward blend
+ *             only where the backward reads it, other words are undefined)
  *   image   : "final_T" f32[N], "n_contrib" u32[N], "ranges" u32[2T], "tile_order" u32[T] (tiles by descending list length,
- *             ties by tile id: the launch order of the blend CTAs; no reference counterpart)
+ *             ties by tile id: the launch order of the blend CTAs; no reference counterpart), "block_count" u32[8T]
+ *             (entries of block s's list of tile t at 8 t + s), "block_nwalk" u32[8T] (block-list entries up to and
+ *             including the block's last contributor, written by the forward blend for blocks with a pixel in the image)
  * Returns 0, or MGS_ERR_INVALID_ARG for an unknown name.
  */
 int mgs_state_array(const char* which_state, const char* name, char* state, int P_or_R_or_width, int height,

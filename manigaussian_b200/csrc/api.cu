@@ -48,7 +48,7 @@ static const bool g_trace = getenv("MGS_TRACE") != nullptr;  // diagnostic: name
 	} while (0)
 
 // ---- optional per-stage CUDA-event timing (bench.py's roofline leg); off by default, zero cost when off ----
-enum Stage { ST_PROJECT_FWD = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_SORT, ST_RANGES_PACK, ST_BLEND_FWD, ST_BLEND_BWD, ST_PROJECT_BWD, ST_ACTIVATE_FWD, ST_ACTIVATE_BWD, ST_COUNT };
+enum Stage { ST_PROJECT_FWD = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_SORT, ST_RANGES_PACK, ST_BLOCK_LISTS, ST_BLEND_FWD, ST_BLEND_BWD, ST_PROJECT_BWD, ST_ACTIVATE_FWD, ST_ACTIVATE_BWD, ST_COUNT };
 struct StageEvt { int stage; cudaEvent_t a, b; };
 static std::mutex g_prof_mu;
 static bool g_prof_on = false;
@@ -147,7 +147,7 @@ struct GeomState {
 	}
 };
 struct ImageState {
-	float* final_T; uint32_t* n_contrib; uint2* ranges; int* status; uint32_t* tile_order;
+	float* final_T; uint32_t* n_contrib; uint2* ranges; int* status; uint32_t* tile_order; uint32_t* block_count; uint32_t* block_nwalk;
 	static ImageState carve(char*& chunk, size_t N, size_t T)
 	{
 		ImageState s;
@@ -156,12 +156,14 @@ struct ImageState {
 		obtain(chunk, s.ranges, T);
 		obtain(chunk, s.status, 4);  // {instance count, overflow flag}, written by the instance emission
 		obtain(chunk, s.tile_order, T);
+		obtain(chunk, s.block_count, 8 * T);  // entries of each 8x4 block's work list, written by block_lists
+		obtain(chunk, s.block_nwalk, 8 * T);  // entries the backward replays, written by the forward blend
 		return s;
 	}
 };
 struct BinState {
 	uint32_t* point_list; uint32_t* point_list_unsorted; uint32_t* tile_keys; uint32_t* tile_keys_unsorted; InstRec* recs;
-	uint32_t* pix_mask; size_t mask_stride;
+	uint32_t* pix_mask; size_t mask_stride; uint32_t* block_list; uint8_t* block_bits;
 	char* sort_temp; size_t sort_bytes;
 	static BinState carve(char*& chunk, size_t R)
 	{
@@ -172,11 +174,13 @@ struct BinState {
 		obtain(chunk, b.tile_keys, Rp);            // tile id of every sorted instance (high word of the reference's keys)
 		obtain(chunk, b.tile_keys_unsorted, Rp);
 		obtain(chunk, b.recs, Rp);
-		// per-pixel contribution masks, [block of the tile][instance]: written by the forward blend, read by the backward.
-		// Never cleared: the forward writes the mask of every (block, instance) pair the backward reads (blend_fwd.cu).
-		// Rows are 16-byte aligned and padded, so the backward's aligned bulk copies stay inside the array.
+		// per-pixel contribution masks, [block of the tile][block-list entry]: written by the forward blend, read by the
+		// backward.  Never cleared: the forward writes the mask of every entry the backward reads (blend_fwd.cu).
 		b.mask_stride = (Rp + 3) & ~(size_t)3;
 		obtain(chunk, b.pix_mask, 8 * b.mask_stride);
+		// per-block work lists, same rows and slots as the masks: a block's list is a subset of its tile's
+		obtain(chunk, b.block_list, 8 * b.mask_stride);
+		obtain(chunk, b.block_bits, Rp + 8);       // the records' block masks, one byte per instance; block_lists reads whole 16-byte chunks
 		b.sort_bytes = cached_temp_bytes(1, (int)R);
 		obtain(chunk, b.sort_temp, b.sort_bytes);
 		return b;
@@ -391,9 +395,14 @@ static int enqueue_binning(const Cloud& c, const mgs_view& w, bool exact_capacit
 	{
 		StageTimer t_(ST_RANGES_PACK, st);
 		launch_ranges_and_pack(geom.point_offsets + P - 1, (int)cap, (int)s.T, s.gx, bin.tile_keys, bin.point_list, geom.means2D,
-			geom.conic_opacity, geom.extent, s.img.ranges, bin.recs, s.img.tile_order, st);
+			geom.conic_opacity, geom.extent, s.img.ranges, bin.recs, bin.block_bits, s.img.tile_order, st);
 	}
 	MGS_STAGE("ranges_pack");
+	{
+		StageTimer t_(ST_BLOCK_LISTS, st);
+		launch_block_lists(s.img.ranges, (int)s.T, bin.block_bits, bin.block_list, bin.mask_stride, s.img.block_count, st);
+	}
+	MGS_STAGE("block_lists");
 	if (w.status) MGS_CUDA(cudaMemcpyAsync(w.status, s.img.status, 2 * sizeof(int), cudaMemcpyDefault, st));
 	return 0;
 }
@@ -405,6 +414,7 @@ static BlendArgs blend_args(const ViewState& s, const mgs_view& w, int F, const 
 	ba.W = w.width; ba.H = w.height; ba.grid_x = s.gx; ba.grid_y = s.gy; ba.F = F; ba.groups = blend_groups(F);
 	ba.ranges = s.img.ranges; ba.tile_order = use_tile_order() ? s.img.tile_order : nullptr; ba.point_list = s.bin.point_list; ba.recs = s.bin.recs;
 	ba.rgbd = s.geom.rgbd; ba.feature = F > 0 ? feature : nullptr; ba.bg = w.background;
+	ba.block_list = s.bin.block_list; ba.block_count = s.img.block_count; ba.block_nwalk = s.img.block_nwalk;
 	ba.final_T = s.img.final_T; ba.n_contrib = s.img.n_contrib; ba.pix_mask = s.bin.pix_mask; ba.mask_stride = s.bin.mask_stride;
 	MGS_CTA_LOG_ARGS(ba);
 	return ba;
@@ -799,7 +809,7 @@ int mgs_profile_enable(int on)
 int mgs_profile_num_stages(void) { return ST_COUNT; }
 const char* mgs_profile_stage_name(int i)
 {
-	static const char* names[ST_COUNT] = { "project_fwd", "depth_sort", "scan", "emit_tiles", "tile_sort", "ranges_pack", "blend_fwd", "blend_bwd", "project_bwd", "activate_fwd", "activate_bwd" };
+	static const char* names[ST_COUNT] = { "project_fwd", "depth_sort", "scan", "emit_tiles", "tile_sort", "ranges_pack", "block_lists", "blend_fwd", "blend_bwd", "project_bwd", "activate_fwd", "activate_bwd" };
 	return (i >= 0 && i < ST_COUNT) ? names[i] : "";
 }
 int mgs_profile_read(float* total_ms, int* counts)
@@ -833,10 +843,12 @@ int mgs_state_array(const char* which_state, const char* name, char* state, int 
 		if (n == "point_list") p = b.point_list; else if (n == "tile_ids") p = b.tile_keys;
 		else if (n == "point_list_unsorted") p = b.point_list_unsorted; else if (n == "tile_ids_unsorted") p = b.tile_keys_unsorted;
 		else if (n == "records") p = b.recs; else if (n == "pixel_masks") p = b.pix_mask;
+		else if (n == "block_lists") p = b.block_list; else if (n == "block_bits") p = b.block_bits;
 	} else if (w == "image") {
 		ImageState s = ImageState::carve(state, (size_t)a0 * a1, num_tiles(a0, a1));
 		if (n == "final_T") p = s.final_T; else if (n == "n_contrib") p = s.n_contrib; else if (n == "ranges") p = s.ranges;
-		else if (n == "tile_order") p = s.tile_order;
+		else if (n == "tile_order") p = s.tile_order; else if (n == "block_count") p = s.block_count;
+		else if (n == "block_nwalk") p = s.block_nwalk;
 	}
 	if (!p) return fail(MGS_ERR_INVALID_ARG, "unknown state array " + w + "/" + n);
 	*out_ptr = p;

@@ -12,8 +12,9 @@
 //
 // The device-wide scan and radix passes are the CUDA toolkit's CUB primitives (a library call, as in the
 // reference; BASELINE.json's north_star asks for "cub-style radix sort").  The emit and ranges+pack kernels are
-// hand-written; the latter also gathers the per-instance 32-byte blend record into tile order, so the blend kernels
-// fetch a tile's work list with 1-D TMA bulk copies (the reference gathers by index inside the blend).
+// hand-written; the latter also gathers the per-instance 32-byte blend record into tile order and decides which 8x4
+// pixel blocks of its tile each instance can reach, and block_lists turns that into one work list per block, so a blend
+// warp gathers only the records that can reach its pixels.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
@@ -165,12 +166,13 @@ __device__ __forceinline__ uint32_t block_mask(float gx, float gy, float ca, flo
 	return mask;
 }
 
-// One thread per sorted instance: tile boundary detection + gather of the 32-byte blend record.
+// One thread per sorted instance: tile boundary detection + gather of the 32-byte blend record; the block mask also goes
+// to the compact block_bits array that block_lists_kernel reads.
 __global__ void __launch_bounds__(256) ranges_pack_kernel(const uint32_t* __restrict__ R_dev, int capacity, int grid_x,
 	const uint32_t* __restrict__ tile_keys,
 	const uint32_t* __restrict__ point_list, const float2* __restrict__ means2D,
 	const float4* __restrict__ conic_opacity, const float2* __restrict__ extent,
-	uint2* __restrict__ ranges, InstRec* __restrict__ recs)
+	uint2* __restrict__ ranges, InstRec* __restrict__ recs, uint8_t* __restrict__ block_bits)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const int R = (int)min(*R_dev, (uint32_t)capacity);
@@ -195,6 +197,50 @@ __global__ void __launch_bounds__(256) ranges_pack_kernel(const uint32_t* __rest
 	float4* dst = reinterpret_cast<float4*>(recs + idx);
 	dst[0] = make_float4(xy.x, xy.y, co.x, co.y);
 	dst[1] = make_float4(co.z, co.w, __uint_as_float(mask), __uint_as_float(g));
+	block_bits[idx] = (uint8_t)mask;
+}
+
+// Per-block work lists: one CTA per tile, warp s compacts, in list order, the 0-based tile-list positions of the
+// instances whose block bit s is set into row s of block_list (at range.x + k, so a row never outgrows the tile's slots)
+// and writes their number to block_count[8 tile + s].  The blend warp of block s then touches only the records that can
+// reach its pixels.  block_bits is read 16 bytes per lane from the 16-byte-aligned chunk at or below range.x (the array is
+// padded for the last one); the loop is a chain of dependent loads, so each lane takes as many instances as one load gives.
+__global__ void __launch_bounds__(256) block_lists_kernel(const uint2* __restrict__ ranges, const uint8_t* __restrict__ block_bits,
+	uint32_t* __restrict__ block_list, size_t stride, uint32_t* __restrict__ block_count)
+{
+	const int tile = blockIdx.x;
+	const int s = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const uint2 range = ranges[tile];
+	uint32_t* const row = block_list + s * stride + range.x;
+	const uint4* const chunks = reinterpret_cast<const uint4*>(block_bits);
+	uint32_t n = 0;
+	uint32_t c = (range.x >> 4) + lane;
+	uint4 v = 16 * c < range.y ? chunks[c] : make_uint4(0u, 0u, 0u, 0u);
+	for (uint32_t base = range.x & ~15u; base < range.y; base += 512) {
+		const uint4 cur = v;
+		const uint32_t p0 = 16 * c;
+		c += 32;
+		if (16 * c < range.y) v = chunks[c];  // the next step's bytes are in flight while this step is compacted
+		const uint32_t w[4] = { cur.x, cur.y, cur.z, cur.w };
+		uint32_t m = 0;  // bit b: instance p0 + b is in the tile and has block bit s
+#pragma unroll
+		for (int b = 0; b < 16; b++) {
+			const uint32_t p = p0 + b;
+			if (p >= range.x && p < range.y && ((w[b >> 2] >> (8 * (b & 3) + s)) & 1u)) m |= 1u << b;
+		}
+		// list order is lane-major: an inclusive scan of the per-lane counts places each lane's entries
+		const uint32_t cnt = __popc(m);
+		uint32_t incl = cnt;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+			if (lane >= o) incl += t;
+		}
+		uint32_t k = n + incl - cnt;
+		for (; m; m &= m - 1u) row[k++] = p0 + (uint32_t)(__ffs(m) - 1) - range.x;
+		n += __shfl_sync(0xffffffffu, incl, 31);
+	}
+	if (lane == 0) block_count[8 * tile + s] = n;
 }
 
 // Launch order of the blend CTAs: tiles by descending list length (rank by counting, ties by tile id).  The blend grids
@@ -230,11 +276,17 @@ void launch_tile_order(const uint2* ranges, int num_tiles, uint32_t* order, cuda
 
 void launch_ranges_and_pack(const uint32_t* R_dev, int capacity, int num_tiles, int grid_x, const uint32_t* tile_keys,
 	const uint32_t* point_list, const float2* means2D, const float4* conic_opacity, const float2* extent, uint2* ranges, InstRec* recs,
-	uint32_t* tile_order, cudaStream_t s)
+	uint8_t* block_bits, uint32_t* tile_order, cudaStream_t s)
 {
 	cudaMemsetAsync(ranges, 0, sizeof(uint2) * (size_t)num_tiles, s);
-	if (capacity > 0) ranges_pack_kernel<<<ceil_div(capacity, 256), 256, 0, s>>>(R_dev, capacity, grid_x, tile_keys, point_list, means2D, conic_opacity, extent, ranges, recs);
+	if (capacity > 0) ranges_pack_kernel<<<ceil_div(capacity, 256), 256, 0, s>>>(R_dev, capacity, grid_x, tile_keys, point_list, means2D, conic_opacity, extent, ranges, recs, block_bits);
 	if (tile_order) launch_tile_order(ranges, num_tiles, tile_order, s);
+}
+
+void launch_block_lists(const uint2* ranges, int num_tiles, const uint8_t* block_bits, uint32_t* block_list, size_t stride,
+	uint32_t* block_count, cudaStream_t s)
+{
+	if (num_tiles > 0) block_lists_kernel<<<num_tiles, 256, 0, s>>>(ranges, block_bits, block_list, stride, block_count);
 }
 
 }  // namespace mgs

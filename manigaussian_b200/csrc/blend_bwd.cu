@@ -10,10 +10,11 @@
 //
 // Design.  The reference has every pixel-thread issue 9+F global float atomics per contributing pair (41 at F=32).
 // Here the sums over the pixels of a warp's 8x4 block ARE matrix products, and they run on the tensor cores
-// (mma.sync m16n8k8 TF32, 3xTF32 split, blend_mma.cuh).  A single-warp CTA streams the first max(n_contrib) records of
-// its tile back to front through the TMA ring together with the pixel masks the forward wrote for its block (bit p: the
-// pair contributed to pixel p), queues the records whose mask is non-zero -- a survivor that reached no pixel of the block
-// has no gradient there -- and carries the mask with them; per chunk of BWD_CH queued survivors:
+// (mma.sync m16n8k8 TF32, 3xTF32 split, blend_mma.cuh).  A single-warp CTA replays its block's work list back to front
+// from the block's last contributor (block_nwalk), reading the list entries together with the pixel masks the forward
+// wrote for them (bit p: the pair contributed to pixel p); it queues the entries whose mask is non-zero -- an instance that
+// reached no pixel of the block has no gradient there -- gathers the records of each chunk of BWD_CH queued survivors by
+// list position (cp.async, the next chunk's while the current one runs) and carries the mask in the record; per chunk:
 //   1. gather    the chunk's channel rows C[g][ch] by Gaussian id (cp.async, 16-byte pieces)
 //   2. GEMM 1    Wd[g][p] = sum_ch C[g][ch] Gpx[p][ch]          (c_k . g for every survivor x pixel; Gpx = the block's
 //                                                                cotangent rows, staged once per CTA)
@@ -51,15 +52,10 @@ namespace mgs {
 #ifndef MGS_BWD_MIN_CTAS
 #define MGS_BWD_MIN_CTAS 12
 #endif
-#ifndef MGS_BWD_BATCH
-#define MGS_BWD_BATCH 64
-#endif
 constexpr int BWD_CH = MGS_BWD_CH;        // survivors per chunk: 16 or 32 (whole 16-row MMA tiles)
-constexpr int BWD_QCAP = BWD_CH + 32;
-constexpr int BWD_BATCH = MGS_BWD_BATCH;
+constexpr int BWD_QCAP = 64;              // survivor queue (a ring): a chunk plus the survivors of one more 32-entry step
 constexpr int BWD_MT = BWD_CH / 16;       // 16-row tiles of Gaussians
 static_assert(BWD_CH == 16 || BWD_CH == 32, "backward chunk size");
-static_assert(BWD_BATCH % 32 == 0, "backward record batch");
 
 // GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic
 template <int NFT, bool VEC, bool GRP>
@@ -72,14 +68,11 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	constexpr int GS = 2 * CHP;          // s_g stride per pixel pair
 	constexpr int XS = 2 * BWD_CH + 4;   // s_x / s_wgt stride per pixel pair (+4: spreads the pairs over the banks)
 	constexpr int ROWS_FLOATS = (BWD_CH * RS > 16 * XS) ? BWD_CH * RS : 16 * XS;  // the rows buffer is reused for the wgt tile
-	using Ring = WarpRecRingT<BWD_BATCH, true>;
-	__shared__ __align__(128) InstRec s_rec[RING * BWD_BATCH];
-	__shared__ __align__(16) uint32_t s_mrec[RING * Ring::MSTRIDE];  // pixel masks of the records in s_rec
-	__shared__ __align__(16) float4 s_q[BWD_QCAP * 2];     // survivor queue (linear, back to front): {x,y,ca,cb}, {cc,op,pixel mask,id}
+	__shared__ __align__(16) float4 s_rec[2][BWD_CH * 2];  // records of the current and the next chunk: {x,y,ca,cb}, {cc,op,pixel mask,id}
+	__shared__ uint2 s_qe[BWD_QCAP];                       // survivor queue, back to front: {list position, pixel mask}
 	__shared__ __align__(16) float s_rows[ROWS_FLOATS];    // C[j][RS]; after GEMM 1: wgt tile
 	__shared__ __align__(16) float s_x[16 * XS];           // Wd tile; the walk overwrites it with q in place; then per-Gaussian staging
 	__shared__ __align__(16) float s_g[16 * GS];           // cotangent rows of the block's pixels
-	__shared__ __align__(8) uint64_t s_bar[RING];
 
 #ifdef MGS_CTA_LOG
 	const unsigned long long t_start = cta_log_now();
@@ -97,6 +90,7 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	const int by0 = tile_y * TILE_Y + (sub >> 1) * WARP_BY;
 	const int pxi = bx0 + (lane >> 2), pyi = by0 + (lane & 3);  // walk role: lane = pixel (x = lane >> 2, y = lane & 3)
 	const bool inside = pxi < a.W && pyi < a.H;
+	if (__all_sync(0xffffffffu, !inside)) return;  // the forward skipped this block: it has no block_nwalk
 	const float fbx0 = (float)bx0, fby0 = (float)by0;
 	const size_t HW = (size_t)a.H * a.W;
 	const size_t pix = (size_t)a.W * pyi + pxi;
@@ -106,14 +100,12 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	const bool first = grp == 0;
 
 	// ---- per-pixel state and cotangent rows ----
-	uint32_t nc = 0;
 	float T = 0.f, bgterm = 0.f;
 	{
 		float g4[4] = { 0.f, 0.f, 0.f, 0.f };  // zero in groups >= 1: no colour / depth gradient, no background term
 		// upstream gradients of the fused loss heads (loss_heads.cuh): the cotangent planes were written for d loss = 1
 		const float sc_color = a.cot_scale ? a.cot_scale[0] : 1.f, sc_feat = a.cot_scale ? a.cot_scale[1] : 1.f;
 		if (inside) {
-			nc = a.n_contrib[pix];
 			T = a.final_T[pix];
 			if (first) {
 #pragma unroll
@@ -131,21 +123,16 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				grow[2 * i] = (inside && i < Fg && a.dL_dfeature) ? sc_feat * a.dL_dfeature[(size_t)(c0 + i) * HW + pix] : 0.f;
 		}
 	}
-	uint32_t maxc = nc;
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1) maxc = max(maxc, __shfl_xor_sync(0xffffffffu, maxc, o));
-	if (maxc == 0) return;  // nothing blended into this block
+	// only the entries up to the block's last contributor can have contributed to a pixel of the block
+	const int nwalk = (int)a.block_nwalk[8 * tile + sub];
+	if (nwalk == 0) return;  // nothing blended into this block
 	for (int i = lane; i < ROWS_FLOATS / 4; i += 32) reinterpret_cast<float4*>(s_rows)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 	__syncwarp();
 
 	const uint2 range = a.ranges[tile];
-	Ring ring;
-	// only the first maxc instances of the tile's list can have contributed to a pixel of this block
-	ring.init(s_rec, s_bar, a.recs + range.x, (int)maxc, true, s_mrec, a.pix_mask + sub * a.mask_stride + range.x);
-	const int nb = ring.num_batches();
-	int issued = 0;
-	for (; issued < min(nb, RING); issued++) ring.issue(issued);
-
+	const InstRec* const recs = a.recs + range.x;                                   // the tile's records, by 0-based list position
+	const uint32_t* const lrow = a.block_list + sub * a.mask_stride + range.x;     // this block's work list
+	const uint32_t* const mrow = a.pix_mask + sub * a.mask_stride + range.x;       // pixel masks, by block-list entry
 	const float pfx = (float)pxi, pfy = (float)pyi;
 	float S = 0.f;  // sum over the contributors behind the current one of a_j T_j (c_j . g)
 	const int xofs = (lane >> 1) * XS + (lane & 1) * 2;  // this pixel's slot in the [pi][j >> 1][e][j & 1] tiles
@@ -163,10 +150,41 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 		}
 	}
 	const float half_W = 0.5f * a.W, half_H = 0.5f * a.H;
-	int qcount = 0;
 
-	// consume the first cnt (<= BWD_CH) queued survivors
-	auto process_chunk = [&](int cnt) {
+	// Queue the survivors among the unread entries [0, hi), back to front, 32 entries per step (lane l takes entry
+	// hi - 1 - l; the step's list entries and masks were loaded a step ahead) until a chunk is queued, then start the
+	// gather of the chunk's records into s_rec[b]: lane j < cnt gathers survivor j and keeps its pixel mask in cpm.
+	int hi = nwalk, qhead = 0, qcount = 0;
+	uint32_t epos = 0, epm = 0, cpm = 0;
+	if (hi - 1 - lane >= 0) { epos = lrow[hi - 1 - lane]; epm = mrow[hi - 1 - lane]; }
+	auto next_chunk = [&](int b) -> int {
+		__syncwarp();  // the queue slots of the previous chunk have been read
+		while (qcount < BWD_CH && hi > 0) {
+			const bool hit = hi - 1 - lane >= 0 && epm != 0u;  // a survivor that reached no pixel of the block has no gradient
+			const uint32_t pos = epos, pm = epm;
+			hi -= 32;
+			if (hi - 1 - lane >= 0) { epos = lrow[hi - 1 - lane]; epm = mrow[hi - 1 - lane]; }
+			const uint32_t mask = __ballot_sync(0xffffffffu, hit);
+			if (hit) s_qe[(qhead + qcount + __popc(mask & ((1u << lane) - 1u))) & (BWD_QCAP - 1)] = make_uint2(pos, pm);
+			qcount += __popc(mask);
+		}
+		__syncwarp();
+		const int cnt = min(qcount, BWD_CH);
+		if (lane < cnt) {
+			const uint2 e = s_qe[(qhead + lane) & (BWD_QCAP - 1)];
+			cpm = e.y;
+			gather_rec(s_rec[b] + 2 * lane, recs + e.x);
+		}
+		cp_async_commit();
+		qhead += cnt;
+		qcount -= cnt;
+		return cnt;
+	};
+	int cnt_next = next_chunk(0);
+	const float4* s_q = nullptr;
+
+	// run the cnt (<= BWD_CH) survivors whose records sit in s_rec[buf]
+	auto process_chunk = [&](int cnt, int buf) {
 		// ---- 1. gather the channel rows ----
 		if (VEC) {
 			// lane r knows the Gaussian id of survivor r; 32 / (2 NFT) feature rows are copied per trip (lane = row x 16-byte
@@ -186,8 +204,6 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				}
 			}
 			if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
-			cp_async_commit();
-			cp_async_wait<0>();
 		} else if (lane < cnt) {
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
@@ -198,6 +214,9 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < Fg) ? __ldg(f + i) : 0.f;
 			}
 		}
+		cp_async_commit();
+		cnt_next = next_chunk(buf ^ 1);  // the next chunk's records travel while this chunk runs
+		cp_async_wait<1>();              // the channel rows
 		__syncwarp();
 		// ---- 2. GEMM 1: Wd[p][j] = Gpx[p][:] . C[j][:]   (M = pixels (2 tiles), N = survivors, K = channels) ----
 		{
@@ -393,63 +412,18 @@ __global__ void __launch_bounds__(32, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 			if (first) red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}: zero in the other groups
 		}
-		// the (< 32) survivors behind the chunk move to the head of the queue
-		const int left = qcount - cnt;
-		float4 k0, k1;
-		if (lane < left) { k0 = s_q[2 * (cnt + lane)]; k1 = s_q[2 * (cnt + lane) + 1]; }
-		__syncwarp();
-		if (lane < left) { s_q[2 * lane] = k0; s_q[2 * lane + 1] = k1; }
-		qcount = left;
-		__syncwarp();
 	};
 
-	// Fill the queue from the record stream (back to front), run a chunk whenever BWD_CH survivors are queued, and the
-	// remainder at the end.  One call site for the chunk: the kernel's code stays within the instruction cache.
-	int k = 0, c = 0, n = 0;
-	const float4* rec4 = nullptr;
-	bool open = false;  // batch k is landed and partly culled
-	for (;;) {
-		while (qcount < BWD_CH && k < nb) {
-			if (!open) {
-				rec4 = ring.wait(k);
-				n = ring.batch_n(k);
-				c = ((n - 1) >> 5) << 5;  // chunks of the batch, back to front
-				open = true;
-			}
-			const int j = c + lane;
-			float4 r0, r1;
-			uint32_t pm = 0;
-			bool hit = false;
-			if (j < n) {
-				r1 = rec4[2 * j + 1];
-				pm = ring.masks(k)[j];  // meaningful only where the block bit is set: the forward queued exactly those records
-				hit = rec_hits_block(r1, sub) && pm != 0u;  // a survivor that reached no pixel of the block has no gradient
-				if (hit) r0 = rec4[2 * j];
-			}
-			const uint32_t mask = __ballot_sync(0xffffffffu, hit);
-			if (hit) {
-				// survivors are appended in back-to-front order: the highest lane first
-				const uint32_t above = (lane == 31) ? 0u : (mask >> (lane + 1));
-				const int e = qcount + __popc(above);
-				r1.z = __uint_as_float(pm);  // the block bits are spent: the queue carries the pixel mask instead
-				s_q[2 * e] = r0;
-				s_q[2 * e + 1] = r1;
-			}
-			qcount += __popc(mask);
-			__syncwarp();
-			c -= 32;
-			if (c < 0) {
-				// every survivor of this batch sits in the queue: refill its buffer with the batch RING ahead
-				open = false;
-				if (issued < nb) { ring.issue(issued); issued++; }
-				k++;
-			}
-		}
-		if (qcount == 0) break;
-		process_chunk(min(qcount, BWD_CH));
+	for (int buf = 0; cnt_next > 0; buf ^= 1) {
+		const int cnt = cnt_next;
+		cp_async_wait<0>();  // this chunk's records
+		s_q = s_rec[buf];
+		if (lane < cnt) s_rec[buf][2 * lane + 1].z = __uint_as_float(cpm);  // the block mask is spent: carry the pixel mask
+		__syncwarp();
+		process_chunk(cnt, buf);
 	}
 #ifdef MGS_CTA_LOG
-	cta_log_put(a, t_start, 1u, (unsigned int)sub, maxc);
+	cta_log_put(a, t_start, 1u, (unsigned int)sub, (unsigned int)nwalk);
 #endif
 }
 

@@ -5,16 +5,16 @@
 // when T*(1-alpha) < 1e-4, colour gets + T*bg, features/depth do not; final_T and n_contrib saved).
 //
 // Design (not the reference's; see blend_common.cuh for the decomposition):
-//  * one single-warp CTA per 8x4 pixel block; the warp streams its tile's sorted records through a ring of 1-D TMA
-//    bulk copies, culls every 32-record chunk against the block with the per-Gaussian alpha >= 1/255 footprint
-//    (exact-conservative, one ballot) and QUEUES the survivors in shared memory;
-//  * whenever FWD_CH survivors are queued the warp runs one chunk in two phases:
+//  * one single-warp CTA per 8x4 pixel block; the warp walks its block's work list (the instances whose per-Gaussian
+//    alpha >= 1/255 footprint can reach the block, built by the binning stage) in chunks of FWD_CH, gathering each
+//    chunk's records by list position with cp.async while the previous chunk runs;
+//  * every chunk runs in two phases:
 //      walk       lane = pixel, sequential over the chunk's survivors: the exact transmittance recurrence of the
 //                 reference (same expf, same skip/stop tests, so final_T and n_contrib agree bit for bit); instead of
 //                 36 channel FMAs per survivor (7 of 32 lanes active on the benchmark cloud) the lane only stores its
 //                 blend weight w = alpha*T (0 when the pair does not contribute) into a [survivor][pixel] tile; one
-//                 ballot per survivor records which pixels of the block it contributed to (pix_mask, per block and
-//                 instance), so the backward replays these decisions instead of re-deriving them;
+//                 ballot per survivor records which pixels of the block it contributed to (pix_mask, per block-list
+//                 entry), so the backward replays these decisions instead of re-deriving them;
 //      contract   acc[pixel][channel] += W[pixel][survivor] * C[survivor][channel] on the tensor cores (mma.sync
 //                 m16n8k8 TF32, 3xTF32 split for fp32 accuracy, blend_mma.cuh), accumulators in the D fragments;
 //    the channel rows C of the chunk ({r,g,b,depth} quad + feature row, gathered by Gaussian id with 16-byte cp.async
@@ -38,13 +38,8 @@ namespace mgs {
 #ifndef MGS_FWD_MIN_CTAS
 #define MGS_FWD_MIN_CTAS 14
 #endif
-#ifndef MGS_FWD_BATCH
-#define MGS_FWD_BATCH 64
-#endif
-constexpr int FWD_CH = MGS_FWD_CH;        // survivors per tensor-core chunk (multiple of 8, <= 32)
-constexpr int FWD_QCAP = FWD_CH + 32;     // survivor queue: a chunk plus the survivors of one more 32-record cull
-constexpr int FWD_BATCH = MGS_FWD_BATCH;  // records per bulk copy (a multiple of the 32-record cull chunk)
-static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32 && FWD_BATCH % 32 == 0, "forward chunk size");
+constexpr int FWD_CH = MGS_FWD_CH;        // block-list entries per tensor-core chunk (multiple of 8, <= 32)
+static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32, "forward chunk size");
 
 // GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic
 template <int NFT, bool VEC, bool GRP>
@@ -53,12 +48,10 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	using L = RowLayout<NFT>;
 	constexpr int RS = L::RS;
 	constexpr int NT = NFT + 1;  // column tiles: NFT feature tiles + the {r,g,b,depth} tile
-	__shared__ __align__(128) InstRec s_rec[RING * FWD_BATCH];
-	__shared__ __align__(16) float4 s_q[FWD_QCAP * 2];    // survivor queue, linear: {x,y,ca,cb}, {cc,op,pos,id}; the chunk is its head
+	__shared__ __align__(16) float4 s_rec[2][FWD_CH * 2];  // records of the current and the next chunk: {x,y,ca,cb}, {cc,op,mask,id}
 	__shared__ __align__(16) float s_rows[FWD_CH * RS];   // channel rows of the current chunk
 	__shared__ __align__(16) float s_w[FWD_CH * 32];      // blend weights, per k-step [tig][gid][mt][e][h]: survivor 8 ks + tig + 4 e, pixel 4 gid + 2 mt + h
-	__shared__ uint32_t s_pm[FWD_CH];                     // pixel masks of the chunk's survivors, staged for the 8-lane store
-	__shared__ __align__(8) uint64_t s_bar[RING];
+	__shared__ uint32_t s_pm[FWD_CH];                     // pixel masks of the chunk's entries, staged for one coalesced store
 
 #ifdef MGS_CTA_LOG
 	const unsigned long long t_start = cta_log_now();
@@ -76,7 +69,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	// walk role: lane = pixel (x = lane >> 2, y = lane & 3)
 	const int pxi = bx0 + (lane >> 2), pyi = by0 + (lane & 3);
 	const bool inside = pxi < a.W && pyi < a.H;
-	if (__all_sync(0xffffffffu, !inside)) return;  // block entirely outside the image (ragged right/bottom tiles)
+	if (__all_sync(0xffffffffu, !inside)) return;  // block entirely outside the image (ragged right/bottom tiles); the backward skips it too
 	const float pfx = (float)pxi, pfy = (float)pyi;
 	const int F = a.F;                 // feature row stride
 	const int c0 = 32 * grp;           // first channel of the group
@@ -87,19 +80,16 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	for (int i = lane; i < FWD_CH * RS / 4; i += 32) reinterpret_cast<float4*>(s_rows)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 
 	const uint2 range = a.ranges[tile];
-	uint32_t* const mrow = a.pix_mask + sub * a.mask_stride + range.x;  // pixel masks of this block, by 0-based list position
-	WarpRecRingT<FWD_BATCH> ring;
-	ring.init(s_rec, s_bar, a.recs + range.x, (int)(range.y - range.x), false);
-	const int nb = ring.num_batches();
-	int issued = 0, waited = 0;
-	for (; issued < min(nb, RING); issued++) ring.issue(issued);
-
+	const InstRec* const recs = a.recs + range.x;                                  // the tile's records, by 0-based list position
+	const uint32_t* const lrow = a.block_list + sub * a.mask_stride + range.x;    // this block's work list
+	uint32_t* const mrow = a.pix_mask + sub * a.mask_stride + range.x;            // pixel masks, by block-list entry
+	const int count = (int)a.block_count[8 * tile + sub];
 	// T is the running product of (1 - alpha) over every evaluated pair, the stopping pair included: the product only
 	// shrinks, so once one test T (1 - alpha) < 1e-4 has failed every later one fails too and no "done" flag has to sit
 	// in the recurrence (the reference stops looking at that point; here the later pairs get zero weight).  T_out is the
 	// transmittance after the last accepted pair = the reference's final T.  Pixels outside the image start at 0.
 	float T = inside ? 1.0f : 0.0f, T_out = 1.0f;
-	uint32_t last_contributor = 0;
+	uint32_t last = 0;  // 1-based block-list entry of this pixel's last contributor
 	float acc[2][NT][4];
 #pragma unroll
 	for (int mt = 0; mt < 2; mt++)
@@ -108,14 +98,21 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 #pragma unroll
 			for (int i = 0; i < 4; i++) acc[mt][nt][i] = 0.f;
 
-	int qcount = 0;
 	const int wofs = (lane >> 2) * 8 + ((lane >> 1) & 1) * 4 + (lane & 1);  // this pixel's slot in a [tig][gid][mt][e][h] weight tile
 
-	// consume the first cnt (<= FWD_CH) queued survivors; returns true when every pixel of the block is finished
-	auto process_chunk = [&](int cnt) -> bool {
+	// lane j < FWD_CH gathers record j of a chunk; the list positions of the chunk after next are loaded a chunk ahead
+	uint32_t pos = lane < min(count, FWD_CH) ? lrow[lane] : 0u;
+	if (lane < min(count, FWD_CH)) gather_rec(s_rec[0] + 2 * lane, recs + pos);
+	cp_async_commit();
+	pos = lane < min(count - FWD_CH, FWD_CH) ? lrow[FWD_CH + lane] : 0u;
+	for (int k0 = 0, buf = 0; k0 < count; k0 += FWD_CH, buf ^= 1) {
+		const int cnt = min(count - k0, FWD_CH);
+		const float4* const s_q = s_rec[buf];
+		cp_async_wait<0>();  // this chunk's records
+		__syncwarp();
 		// ---- start the gather of the chunk's channel rows (lands while the walk runs) ----
 		if (VEC) {
-			// lane r knows the Gaussian id of survivor r; the feature rows are cut into 16-byte pieces and 32 / (2 NFT) rows
+			// lane r knows the Gaussian id of entry r; the feature rows are cut into 16-byte pieces and 32 / (2 NFT) rows
 			// are copied per trip (lane = row-in-trip x piece), the id travelling by shuffle: 4 instructions per LDGSTS
 			const uint32_t myid = lane < cnt ? __float_as_uint(s_q[2 * lane + 1].w) : 0u;
 			if (NFT > 0) {
@@ -131,7 +128,6 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				}
 			}
 			if (lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD, a.rgbd + myid);
-			cp_async_commit();
 		} else if (lane < cnt) {  // feature rows that are not whole 8-wide tiles (e.g. F = 3): plain loads, zero padded
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
@@ -142,7 +138,13 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				for (int i = 0; i < 8 * NFT; i++) row[i] = (i < Fg) ? __ldg(f + i) : 0.f;
 			}
 		}
-		// ---- walk: one k-step (8 survivors) per trip, in two passes so that the eight footprint evaluations (independent:
+		cp_async_commit();
+		// ---- the next chunk's records travel while this chunk runs ----
+		const int k1 = k0 + FWD_CH;
+		if (lane < min(count - k1, FWD_CH)) gather_rec(s_rec[buf ^ 1] + 2 * lane, recs + pos);
+		cp_async_commit();
+		pos = lane < min(count - k1 - FWD_CH, FWD_CH) ? lrow[k1 + FWD_CH + lane] : 0u;
+		// ---- walk: one k-step (8 entries) per trip, in two passes so that the eight footprint evaluations (independent:
 		// LDS, 8 FP ops, expf) overlap in the pipeline and only the short transmittance recurrence is sequential.
 		// Slots beyond cnt hold stale records and get zero weights. ----
 		const int nks = (cnt + 7) >> 3;
@@ -152,7 +154,6 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			const float4* q4 = s_q + 16 * ks;
 			float* wrow = s_w + 256 * ks;
 			float al[8];      // alpha of the pair, 0 where the pair is skipped (power > 0, alpha < 1/255, empty slot)
-			uint32_t ps[8];   // 1-based position of the survivor in the tile's list
 #pragma unroll
 			for (int u = 0; u < 8; u++) {
 				const float4 p = q4[2 * u], q = q4[2 * u + 1];
@@ -161,7 +162,6 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				const float alpha = min(ALPHA_MAX, q.y * expf(power));
 				const bool ok = (8 * ks + u < cnt) && !(power > 0.0f) && !(alpha < ALPHA_MIN);
 				al[u] = ok ? alpha : 0.f;
-				ps[u] = __float_as_uint(q.z);
 			}
 #pragma unroll
 			for (int u = 0; u < 8; u++) {
@@ -170,23 +170,22 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				const bool use = !(test_T < T_STOP);  // a skipped pair (alpha = 0) passes with zero weight and T unchanged
 				wrow[(u & 3) * 64 + (u >> 2) * 2 + wofs] = use ? alpha * T : 0.f;
 				T_out = use ? test_T : T_out;
-				last_contributor = (use && alpha != 0.f) ? ps[u] : last_contributor;
+				last = (use && alpha != 0.f) ? (uint32_t)(k0 + 8 * ks + u + 1) : last;
 				T = test_T;
 				s_pm[8 * ks + u] = __ballot_sync(0xffffffffu, use && alpha != 0.f);  // warp-uniform: every lane stores the same word
 			}
-			__syncwarp();
-			// The backward reads the masks of the queued survivors at positions <= max n_contrib of the block, and every one of
-			// them is walked here: a k-step is only skipped once every pixel has terminated, i.e. behind every pixel's last
-			// contributor.  So the array needs no clearing.
-			if (first && lane < 8 && 8 * ks + lane < cnt) mrow[__float_as_uint(q4[2 * lane + 1].z) - 1u] = s_pm[8 * ks + lane];
 		}
 		const int nk = ks;  // k-steps to contract
-		if (VEC) cp_async_wait<0>();
+		__syncwarp();
+		// The backward reads the masks of the entries up to the block's last contributor, and every one of them is walked
+		// here: a k-step is only skipped once every pixel has terminated.  So the array needs no clearing.
+		if (first && lane < min(cnt, 8 * nk)) mrow[k0 + lane] = s_pm[lane];
+		cp_async_wait<1>();  // the channel rows (the next chunk's records may still travel)
 		__syncwarp();
 		// ---- contract on the tensor cores ----
 		for (int ks = 0; ks < nk; ks++) {
 			const int g0 = 8 * ks + tig, g1 = g0 + 4;
-			// {a0..a3} of pixel tile mt: weights of survivors g0 (k = tig) and g1 (k = tig + 4) at pixels 4 gid + 2 mt + {0, 1}
+			// {a0..a3} of pixel tile mt: weights of entries g0 (k = tig) and g1 (k = tig + 4) at pixels 4 gid + 2 mt + {0, 1}
 			const float4 wa = *reinterpret_cast<const float4*>(s_w + ks * 256 + tig * 64 + gid * 8);
 			const float4 wb = *reinterpret_cast<const float4*>(s_w + ks * 256 + tig * 64 + gid * 8 + 4);
 			uint32_t ahi[2][4], alo[2][4];
@@ -196,7 +195,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			tf32_split(wb.z, ahi[1][2], alo[1][2]); tf32_split(wb.w, ahi[1][3], alo[1][3]);
 			const float* row0 = s_rows + g0 * RS;
 			const float* row1 = s_rows + g1 * RS;
-			// B fragments {b0, b1} = column gid of tile nt for survivors g0 and g1: scalar, conflict-free loads straight into
+			// B fragments {b0, b1} = column gid of tile nt for entries g0 and g1: scalar, conflict-free loads straight into
 			// the operand pair (a 128-bit row load would need a register move per operand)
 #pragma unroll
 			for (int nt = 0; nt < NFT; nt++) {
@@ -216,60 +215,10 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				mma_3xtf32(acc[1][NFT], ahi[1], alo[1], bh0, bh1, bl0, bl1);
 			}
 		}
-		// the (< 32) survivors behind the chunk move to the head of the queue
-		const int left = qcount - cnt;
-		float4 m0, m1;
-		if (lane < left) { m0 = s_q[2 * (cnt + lane)]; m1 = s_q[2 * (cnt + lane) + 1]; }
-		__syncwarp();  // also: s_w and s_rows are rewritten by the next chunk
-		if (lane < left) { s_q[2 * lane] = m0; s_q[2 * lane + 1] = m1; }
-		qcount = left;
-		__syncwarp();
-		return __all_sync(0xffffffffu, T < T_STOP);
-	};
-
-	// Fill the queue from the record stream, run a chunk whenever FWD_CH survivors are queued, and the remainder at the
-	// end.  One call site for the chunk: the kernel's code stays within the instruction cache.
-	int k = 0, c = 0, lo = 0, n = 0;
-	const float4* rec4 = nullptr;
-	bool open = false;  // batch k is landed and partly culled
-	for (;;) {
-		while (qcount < FWD_CH && k < nb) {
-			if (!open) {
-				rec4 = ring.wait(k);
-				waited = k + 1;
-				lo = ring.batch_lo(k); n = ring.batch_n(k);
-				c = 0;
-				open = true;
-			}
-			const int j = c + lane;
-			float4 r0, r1;
-			bool hit = false;
-			if (j < n) {
-				r1 = rec4[2 * j + 1];
-				hit = rec_hits_block(r1, sub);
-				if (hit) r0 = rec4[2 * j];
-			}
-			const uint32_t mask = __ballot_sync(0xffffffffu, hit);
-			if (hit) {
-				const int e = qcount + __popc(mask & ((1u << lane) - 1u));
-				r1.z = __uint_as_float((uint32_t)(lo + j) + 1u);  // the cull extent is spent: keep the 1-based list position instead
-				s_q[2 * e] = r0;
-				s_q[2 * e + 1] = r1;
-			}
-			qcount += __popc(mask);
-			__syncwarp();
-			c += 32;
-			if (c >= n) {
-				// every survivor of this batch sits in the queue: its buffer is free for the batch RING ahead
-				open = false;
-				if (issued < nb) { ring.issue(issued); issued++; }
-				k++;
-			}
-		}
-		if (qcount == 0) break;
-		if (process_chunk(min(qcount, FWD_CH))) break;  // every pixel of the block is finished
+		__syncwarp();  // s_w, s_rows and s_pm are rewritten by the next chunk
+		if (__all_sync(0xffffffffu, T < T_STOP)) break;  // every pixel of the block is finished
 	}
-	for (int k = waited; k < issued; k++) ring.wait(k);  // no bulk copy may be in flight when the CTA exits
+	cp_async_wait<0>();  // no record copy may be in flight when the CTA exits
 
 	// ---- outputs ----
 	const size_t HW = (size_t)a.H * a.W;
@@ -278,8 +227,14 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 		if (first) {
 			const size_t pix = (size_t)a.W * pyi + pxi;
 			a.final_T[pix] = T;
-			a.n_contrib[pix] = last_contributor;
+			a.n_contrib[pix] = last ? lrow[last - 1] + 1u : 0u;  // 1-based tile-list position, as the reference counts
 		}
+	}
+	if (first) {
+		uint32_t nwalk = last;
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) nwalk = max(nwalk, __shfl_xor_sync(0xffffffffu, nwalk, o));
+		if (lane == 0) a.block_nwalk[8 * tile + sub] = nwalk;
 	}
 	s_w[lane] = T;
 	__syncwarp();
@@ -370,7 +325,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 		}
 	}
 #ifdef MGS_CTA_LOG
-	cta_log_put(a, t_start, 0u, (unsigned int)sub, range.y - range.x);
+	cta_log_put(a, t_start, 0u, (unsigned int)sub, (unsigned int)count);
 #endif
 }
 

@@ -21,14 +21,14 @@ constexpr float ALPHA_MIN = 1.0f / 255.0f;  // forward.cu:354
 constexpr float ALPHA_MAX = 0.99f;          // forward.cu:353
 constexpr float T_STOP = 0.0001f;           // forward.cu:357
 
-// Per-instance record, written in (tile, depth) order by the binning stage so that one tile's work
-// list is one contiguous byte range (a single cp.async.bulk per batch).  32 bytes.
+// Per-instance record, written in (tile, depth) order by the binning stage; a blend warp gathers the records of its
+// block's work list by tile-list position (two 16-byte pieces each).  32 bytes.
 struct __align__(16) InstRec {
 	float x, y;        // pixel-space mean (geom means2D)
 	float ca, cb;      // conic.x, conic.y
 	float cc, op;      // conic.z, opacity
 	uint32_t blocks;   // bit s: the alpha >= 1/255 footprint can reach 8x4 pixel block s of the instance's tile
-	                   // (s = 2 * (y / 4) + x / 8).  Conservative; cull only, never changes a pixel.
+	                   // (s = 2 * (y / 4) + x / 8).  Conservative; selects the block lists, never changes a pixel.
 	uint32_t id;       // Gaussian index (== point_list entry)
 };
 static_assert(sizeof(InstRec) == 32, "InstRec must be 32 bytes");
@@ -103,35 +103,6 @@ __device__ __forceinline__ void tile_rect(float px, float py, int max_radius, ui
 // ------------------------------- PTX wrappers (sm_90+) -------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count)
-{
-	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes)
-{
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
-{
-	asm volatile(
-		"{\n\t"
-		".reg .pred p;\n\t"
-		"WAIT_LOOP:\n\t"
-		"mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-		"@p bra WAIT_DONE;\n\t"
-		"bra WAIT_LOOP;\n\t"
-		"WAIT_DONE:\n\t"
-		"}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// 1-D bulk (TMA) copy global -> shared, completion signalled on an mbarrier.  bytes % 16 == 0,
-// both addresses 16-byte aligned.  SASS: UBLKCP.
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar)
-{
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-		::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
 // 128-bit vector reduction to global memory (sm_90+): one L2 atomic transaction for 4 floats.
 // 16-byte asynchronous copy global -> shared with a PER-LANE address (SASS LDGSTS), tracked by per-thread commit groups
 __device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem)

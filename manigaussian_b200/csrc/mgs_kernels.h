@@ -81,6 +81,8 @@ struct BlendArgs {
 	const uint32_t* tile_order;  // [T] launch order of the tiles (tile rank i works on tile tile_order[i]); null = identity
 	const uint32_t* point_list;  // [R] sorted Gaussian ids
 	const InstRec* recs;         // [R] sorted packed records
+	const uint32_t* block_list;  // [8][mask_stride] per 8x4 block of the tile: 0-based list positions of the instances that can reach it
+	const uint32_t* block_count; // [8T] entries of each block's list
 	const float4* rgbd;          // [P] {r,g,b,depth}
 	const float* feature;        // [P,F] or null
 	const float* bg;             // [3]
@@ -88,8 +90,9 @@ struct BlendArgs {
 	// forward outputs / backward inputs
 	float* final_T;              // [N]
 	uint32_t* n_contrib;         // [N]
-	uint32_t* pix_mask;          // [8][mask_stride] per (8x4 block of the tile, instance): bit p = the pair contributed to pixel p
+	uint32_t* pix_mask;          // [8][mask_stride] per block-list entry: bit p = the pair contributed to pixel p of the block
 	size_t mask_stride;          // a multiple of 4: every row starts 16-byte aligned
+	uint32_t* block_nwalk;       // [8T] block-list entries up to and including the block's last contributor
 	float* out_color;            // [3,H,W]
 	float* out_feature;          // [F,H,W]
 	float* out_depth;            // [H,W] nullable
@@ -111,8 +114,8 @@ struct BlendArgs {
 	float* loss_acc;
 	const float* cot_scale;
 #ifdef MGS_CTA_LOG
-	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, list length,
-	// SM id, block id} -- the timeline of the single-warp CTAs across kernels and streams
+	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
+	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the single-warp CTAs across kernels and streams
 	unsigned long long* cta_log; unsigned int* cta_log_n; unsigned int cta_log_cap;
 #endif
 };
@@ -172,7 +175,12 @@ void launch_tile_sort(void* temp, size_t temp_bytes, const uint32_t* keys_in, ui
 void launch_tile_order(const uint2* ranges, int num_tiles, uint32_t* order, cudaStream_t s);
 // the instance count is read on the device from *R_dev (clamped to `capacity`), the grid covers `capacity`
 void launch_ranges_and_pack(const uint32_t* R_dev, int capacity, int num_tiles, int grid_x, const uint32_t* tile_keys, const uint32_t* point_list,
-	const float2* means2D, const float4* conic_opacity, const float2* extent, uint2* ranges, InstRec* recs, uint32_t* tile_order, cudaStream_t s);
+	const float2* means2D, const float4* conic_opacity, const float2* extent, uint2* ranges, InstRec* recs, uint8_t* block_bits,
+	uint32_t* tile_order, cudaStream_t s);
+// per (tile, 8x4 block): the 0-based tile-list positions of the instances whose block bit is set, in list order, into row s
+// of block_list ([8][stride], entries at range.x + k), and their number into block_count[8 tile + s]
+void launch_block_lists(const uint2* ranges, int num_tiles, const uint8_t* block_bits, uint32_t* block_list, size_t stride,
+	uint32_t* block_count, cudaStream_t s);
 
 // blend_fwd.cu / blend_bwd.cu
 int blend_supported(int F);
