@@ -662,7 +662,7 @@ int mgs_forward_views(
 	// view's long blend kernel, so no view's chain queues behind another view's blend
 	for (int phase = 0; phase < 3; phase++) {
 		// MGS_BLEND_BARRIER=1: all blends start together, after the binning chain of EVERY view.  A blend launch is one
-		// wave of single-warp CTAs that takes every shared-memory slot of the GPU, and the short binning kernels of the
+		// wave of small CTAs that takes every shared-memory slot of the GPU, and the short binning kernels of the
 		// other views crawl behind it (CTA timeline, tools/cta_timeline.py: blends 0 and 1 each run alone, 790 us for the
 		// four forward blends of the bench step; started together 590 us) -- but four binning chains side by side take
 		// 0.38 ms instead of 0.22 ms for the first alone, and the step time comes out the same (2.21 ms either way,

@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(256) block_lists_kernel(const uint2* __restric
 }
 
 // Launch order of the blend CTAs: tiles by descending list length (rank by counting, ties by tile id).  The blend grids
-// are about one wave of single-warp CTAs whose run time follows the list length; starting the long ones first leaves
+// are about one wave of small CTAs (one or two warps per 8x4 block) whose run time follows the list length; starting the long ones first leaves
 // the short ones for the tail of the wave (and of the last view's kernel in a multi-view step).
 __global__ void __launch_bounds__(256) tile_order_kernel(const uint2* __restrict__ ranges, int T, uint32_t* __restrict__ order)
 {

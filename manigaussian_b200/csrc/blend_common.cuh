@@ -1,11 +1,12 @@
 // Shared by the forward and backward blend kernels.
 //
-// Work decomposition: ONE WARP = ONE CTA = one 8x4 pixel block of a 16x16 tile (tile ids / work lists stay the
-// reference's 16x16 tiles; eight single-warp CTAs per tile, 8 G with G channel groups of 32 features when F > 32,
-// BlendArgs::groups).  The binning stage gives every block its own work list: the tile-list positions of the instances
-// whose footprint can reach the block (block_lists_kernel, binning.cu).  A warp reads its list coalesced and gathers the
-// chunk's 32-byte records by position with 16-byte cp.async (SASS LDGSTS), the next chunk's while the current one runs.
-// No CTA-wide barrier exists anywhere: warps of a heavy tile never wait for each other, finished warps free their SM
+// Work decomposition: ONE CTA = one 8x4 pixel block of a 16x16 tile (tile ids / work lists stay the reference's 16x16
+// tiles; eight CTAs per tile, 8 G with G channel groups of 32 features when F > 32, BlendArgs::groups).  The forward's CTA
+// is one warp; the backward's is two cooperating warps (a walker and a companion, blend_bwd.cu), one warp for channel groups.  The binning stage gives
+// every block its own work list: the tile-list positions of the instances whose footprint can reach the block
+// (block_lists_kernel, binning.cu).  A warp reads its list coalesced and gathers the chunk's 32-byte records by position
+// with 16-byte cp.async (SASS LDGSTS), the next chunk's while the current one runs.  The only barriers are the ones
+// between the two warps of a backward CTA; CTAs of a heavy tile never wait for each other, finished CTAs free their SM
 // slot immediately, and the hardware scheduler balances the 8*T*V small CTAs across the 132 SMs of an H100.
 #pragma once
 #include "mgs_common.cuh"
@@ -20,6 +21,21 @@ __device__ __forceinline__ void gather_rec(float4* dst, const InstRec* rec)
 {
 	cp_async16(dst, rec);
 	cp_async16(dst + 1, reinterpret_cast<const float4*>(rec) + 1);
+}
+
+// Named barrier BASE + s (s = 0 | 1, warp-uniform) over N threads: bar.sync waits for the barrier, bar.arrive signals it
+// without waiting.  The ids stay immediates: with an id held in a register ptxas reserves all 16 barriers of the CTA.
+template <int BASE, int N>
+__device__ __forceinline__ void named_bar_sync(int s)
+{
+	if (s == 0) asm volatile("bar.sync %0, %1;" ::"n"(BASE), "n"(N) : "memory");
+	else asm volatile("bar.sync %0, %1;" ::"n"(BASE + 1), "n"(N) : "memory");
+}
+template <int BASE, int N>
+__device__ __forceinline__ void named_bar_arrive(int s)
+{
+	if (s == 0) asm volatile("bar.arrive %0, %1;" ::"n"(BASE), "n"(N) : "memory");
+	else asm volatile("bar.arrive %0, %1;" ::"n"(BASE + 1), "n"(N) : "memory");
 }
 
 #ifdef MGS_CTA_LOG

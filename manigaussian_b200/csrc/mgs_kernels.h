@@ -115,7 +115,7 @@ struct BlendArgs {
 	const float* cot_scale;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
-	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the single-warp CTAs across kernels and streams
+	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams
 	unsigned long long* cta_log; unsigned int* cta_log_n; unsigned int cta_log_cap;
 #endif
 };

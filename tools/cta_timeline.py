@@ -1,5 +1,6 @@
 """Timeline of the blend CTAs of one c3 step (variant library built with -DMGS_CTA_LOG, MGS_VARIANT=ctalog):
-per kernel launch the start/end of the launch, the duration distribution of its single-warp CTAs, how long the longest
+per kernel launch the start/end of the launch, the duration distribution of its CTAs (one warp forward, two warps
+backward at F <= 32), how long the longest
 CTA alone runs (the kernel's critical path) and how much the launches of different views overlap.
 Run on a GPU box: MGS_VARIANT=ctalog MGS_NVCC_DEFINES=-DMGS_CTA_LOG MGS_NO_BUILD=1 python tools/cta_timeline.py [c3]"""
 import ctypes

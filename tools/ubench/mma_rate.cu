@@ -19,8 +19,9 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
 
 // ILP independent accumulator tiles per warp; mode 0 tf32, 1 bf16, 2 ffma (32 FMAs per "op" to compare per-instruction)
 template <int MODE, int ILP>
-__global__ void k(float* out, int iters, uint32_t seed)
+__global__ void k(float* out, long long* cyc, int iters, uint32_t seed)
 {
+	const long long c0 = clock64();
 	float d[ILP][4];
 	uint32_t a[4], b[2];
 	for (int i = 0; i < 4; i++) a[i] = seed * (threadIdx.x + i + 1);
@@ -41,20 +42,21 @@ __global__ void k(float* out, int iters, uint32_t seed)
 	float s = 0.f;
 	for (int j = 0; j < ILP; j++) for (int i = 0; i < 4; i++) s += d[j][i];
 	out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+	if (blockIdx.x == 0 && threadIdx.x == 0) *cyc = clock64() - c0;  // SM cycles of the timed loop, whatever the clock
 }
 
 template <int MODE, int ILP>
-void run(const char* name, int warps_per_sm, int nsm, float* out)
+void run(const char* name, int warps_per_sm, int nsm, float* out, long long* cyc)
 {
 	const int iters = 4096;
 	// one CTA per SM slot: warps_per_sm warps in ONE CTA per SM
 	dim3 grid(nsm), block(32 * warps_per_sm);
 	cudaEvent_t e0, e1;
 	cudaEventCreate(&e0); cudaEventCreate(&e1);
-	k<MODE, ILP><<<grid, block>>>(out, 16, 3u);
+	k<MODE, ILP><<<grid, block>>>(out, cyc, 16, 3u);
 	cudaDeviceSynchronize();
 	cudaEventRecord(e0);
-	k<MODE, ILP><<<grid, block>>>(out, iters, 3u);
+	k<MODE, ILP><<<grid, block>>>(out, cyc, iters, 3u);
 	cudaEventRecord(e1);
 	cudaDeviceSynchronize();
 	float ms = 0.f;
@@ -63,8 +65,13 @@ void run(const char* name, int warps_per_sm, int nsm, float* out)
 	const double per_sm_per_us = ops / nsm / (ms * 1e3);
 	// FMAs per instruction: tf32 m16n8k8 = 1024, bf16 m16n8k16 = 2048, ffma = 32
 	const double fma = MODE == 0 ? 1024 : (MODE == 1 ? 2048 : 32);
-	printf("%-6s ilp %d warps/SM %2d: %.3f ms  %.1f warp-instr/us/SM  %.1f FMA/ns/SM  chip %.1f TFMA/s\n", name, ILP, warps_per_sm, ms,
-	       per_sm_per_us, per_sm_per_us * fma / 1e3, per_sm_per_us * fma * nsm / 1e6);
+	long long c = 0;
+	cudaMemcpy(&c, cyc, sizeof(c), cudaMemcpyDeviceToHost);
+	// issue interval in SM cycles per warp instruction and scheduler (4 schedulers per SM), and the clock it implies
+	const double per_sched = (double)iters * ILP * (MODE == 2 ? 4 : 1) * (warps_per_sm < 4 ? 1 : warps_per_sm / 4);
+	printf("%-6s ilp %d warps/SM %2d: %.3f ms  %.1f warp-instr/us/SM  %.1f FMA/ns/SM  chip %.1f TFMA/s  %.2f cycles/instr/scheduler"
+	       "  (%.0f MHz)\n", name, ILP, warps_per_sm, ms, per_sm_per_us, per_sm_per_us * fma / 1e3, per_sm_per_us * fma * nsm / 1e6,
+	       c / per_sched, c / (ms * 1e3));
 }
 
 int main()
@@ -75,12 +82,14 @@ int main()
 	printf("%s, %d SMs, %d MHz\n", p.name, nsm, p.clockRate / 1000);
 	float* out;
 	cudaMalloc(&out, sizeof(float) * nsm * 1024);
+	long long* cyc;
+	cudaMalloc(&cyc, sizeof(long long));
 	for (int w : {1, 4, 8, 16}) {
-		if (w == 1) { run<0, 1>("tf32", w, nsm, out); run<1, 1>("bf16", w, nsm, out); run<2, 1>("ffma", w, nsm, out); }
-		run<0, 4>("tf32", w, nsm, out);
-		run<1, 4>("bf16", w, nsm, out);
-		run<2, 4>("ffma", w, nsm, out);
-		run<0, 8>("tf32", w, nsm, out);
+		if (w == 1) { run<0, 1>("tf32", w, nsm, out, cyc); run<1, 1>("bf16", w, nsm, out, cyc); run<2, 1>("ffma", w, nsm, out, cyc); }
+		run<0, 4>("tf32", w, nsm, out, cyc);
+		run<1, 4>("bf16", w, nsm, out, cyc);
+		run<2, 4>("ffma", w, nsm, out, cyc);
+		run<0, 8>("tf32", w, nsm, out, cyc);
 	}
 	printf("cuda status: %s\n", cudaGetErrorString(cudaGetLastError()));
 	return 0;
