@@ -91,6 +91,17 @@ extern "C" int mgs_debug_set_cta_log(void* log, void* counter, unsigned int cap)
 #else
 #define MGS_CTA_LOG_ARGS(ba) do { } while (0)
 #endif
+#ifdef MGS_BWD_PHASES
+static unsigned long long* g_bwd_phases = nullptr;
+extern "C" int mgs_debug_set_bwd_phases(void* acc)
+{
+	g_bwd_phases = static_cast<unsigned long long*>(acc);
+	return 0;
+}
+#define MGS_BWD_PHASES_ARGS(ba) do { (ba).bwd_phases = g_bwd_phases; } while (0)
+#else
+#define MGS_BWD_PHASES_ARGS(ba) do { } while (0)
+#endif
 
 template <typename T>
 static void obtain(char*& chunk, T*& ptr, size_t count, size_t alignment = 128)
@@ -417,6 +428,7 @@ static BlendArgs blend_args(const ViewState& s, const mgs_view& w, int F, const 
 	ba.block_list = s.bin.block_list; ba.block_count = s.img.block_count; ba.block_nwalk = s.img.block_nwalk;
 	ba.final_T = s.img.final_T; ba.n_contrib = s.img.n_contrib; ba.pix_mask = s.bin.pix_mask; ba.mask_stride = s.bin.mask_stride;
 	MGS_CTA_LOG_ARGS(ba);
+	MGS_BWD_PHASES_ARGS(ba);
 	return ba;
 }
 

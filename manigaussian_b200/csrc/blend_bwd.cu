@@ -27,7 +27,8 @@
 //                (sum_p q (u - x)^2 = u^2 M0 - 2 u Mx + Mxx with u = mean.x - block.x, ...; Y is exact in TF32)
 //   6. flush     per (block, Gaussian): 3 red.global.add.v4.f32 of the 10 small gradients + the feature row as
 //                red.v4 straight from the D fragments (column gid of feature tile nt is feature NFT*gid + nt, so a thread
-//                holds 8 consecutive features of its four Gaussians).
+//                holds 8 consecutive features of its four Gaussians; at F = 32 neighbouring lanes swap halves so that every
+//                pair of reductions fills whole 32-byte sectors).
 // Roles.  Only the walk is sequential (T and S carry from chunk to chunk), so it has a warp of its own: warp 0, the
 // walker W, owns T, S and the background term and runs step 3.  Warp 1, the companion C, runs everything else: the queue,
 // the gathers, GEMM 1, GEMM 2/3 and the flush.  They hand chunks to each other through a two-stage ring of {rows -> wgt,
@@ -59,6 +60,21 @@ namespace mgs {
 #endif
 #ifndef MGS_BWD_MIN_CTAS
 #define MGS_BWD_MIN_CTAS 8  // two-warp CTAs per SM: at most 128 registers per thread
+#endif
+// Timing-only switches of the two-warp kernel, never in the default build; their gradients are wrong by construction
+// (tools/bwd_phases.py, DESIGN §4):
+//   MGS_BWD_ABL_NO_FEATURE_RED  skip the feature-row reductions of the flush (dL/dfeature stays zero)
+//   MGS_BWD_ABL_FIXED_ROW       gather the channel rows of Gaussian id & 4095 instead of id: 576 KB of rows that stay in
+//                               L2, spread over its slices (one single row would make every CTA hammer one L2 line)
+#ifdef MGS_BWD_ABL_FIXED_ROW
+__device__ __forceinline__ uint32_t bwd_row_id(uint32_t id) { return id & 4095u; }
+#else
+__device__ __forceinline__ uint32_t bwd_row_id(uint32_t id) { return id; }
+#endif
+#ifdef MGS_BWD_ABL_NO_FEATURE_RED
+constexpr bool BWD_FEATURE_RED = false;
+#else
+constexpr bool BWD_FEATURE_RED = true;
 #endif
 constexpr int BWD_CH = MGS_BWD_CH;        // survivors per chunk: 16 or 32 (whole 16-row MMA tiles)
 constexpr int BWD_QCAP = 64;              // survivor queue (a ring): a chunk plus the survivors of one more 32-entry step
@@ -146,6 +162,10 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	// cnt = 0 through FULL, after which W stops and C finishes the last real chunk: both warps run the same sequence of
 	// barrier operations.
 	if (walker) {
+#ifdef MGS_BWD_PHASES
+		BwdPhaseClock ph;
+		ph.start();
+#endif
 		const float pfx = (float)pxi, pfy = (float)pyi;
 		float S = 0.f;  // sum over the contributors behind the current one of a_j T_j (c_j . g)
 		const int xofs = (lane >> 1) * XS + (lane & 1) * 2;  // this pixel's slot in the [pi][j >> 1][e][j & 1] tiles
@@ -154,6 +174,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 		for (int k = 0;; k++) {
 			const int s = k & 1;
 			named_bar_sync<BWD_BAR_FULL, 64>(s);
+			BWD_PH_LAP(ph, BWD_PH_FULL_WAIT);
 			const int cnt = s_cnt[s];
 			if (cnt == 0) break;
 			const float4* const s_q = s_rec[r];
@@ -195,8 +216,17 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			}
 			__syncwarp();
 			named_bar_arrive<BWD_BAR_DONE, 64>(s);
+			BWD_PH_LAP(ph, BWD_PH_WALK);
 		}
+#ifdef MGS_BWD_PHASES
+		ph.put(a.bwd_phases, BWD_PH_FULL_WAIT, BWD_PH_WALK, BWD_PH_W_TOTAL, false);
+#endif
 	} else {
+#ifdef MGS_BWD_PHASES
+		BwdPhaseClock ph;
+		ph.start();
+		ph.acc[BWD_PH_CTAS] = 1u;
+#endif
 		const float fbx0 = (float)bx0, fby0 = (float)by0;
 		const float half_W = 0.5f * a.W, half_H = 0.5f * a.H;
 		const InstRec* const recs = a.recs + a.ranges[tile].x;                                   // the tile's records, by 0-based list position
@@ -229,6 +259,12 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				const uint32_t pos = epos, pm = epm;
 				hi -= 32;
 				if (hi - 1 - lane >= 0) { epos = lrow[hi - 1 - lane]; epm = mrow[hi - 1 - lane]; }
+				// a chunk often takes two steps, and then the second step's loads above are waited on at once: bring the
+				// entries of the step after them into L1 now (the two lines' ends of the 32-entry window, lanes 0 and 31)
+				if (lane == 0 || lane == 31) {
+					const int j = hi - 33 - lane;
+					if (j >= 0) { prefetch_l1(lrow + j); prefetch_l1(mrow + j); }
+				}
 				const uint32_t mask = __ballot_sync(0xffffffffu, hit);
 				if (hit) s_qe[(qhead + qcount + __popc(mask & ((1u << lane) - 1u))) & (BWD_QCAP - 1)] = make_uint2(pos, pm);
 				qcount += __popc(mask);
@@ -243,6 +279,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			cp_async_commit();
 			qhead += cnt;
 			qcount -= cnt;
+			BWD_PH_LAP(ph, BWD_PH_QUEUE);
 			return cnt;
 		};
 
@@ -252,7 +289,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			if (VEC) {
 				// lane r knows the Gaussian id of survivor r; 32 / (2 NFT) feature rows are copied per trip (lane = row x 16-byte
 				// piece), the id travelling by shuffle
-				const uint32_t myid = lane < cnt ? __float_as_uint(s_q[2 * lane + 1].w) : 0u;
+				const uint32_t myid = lane < cnt ? bwd_row_id(__float_as_uint(s_q[2 * lane + 1].w)) : 0u;
 				if (NFT > 0) {
 					constexpr int NPF = NFT > 0 ? 2 * NFT : 1, RPI = 32 / NPF;
 					const int sub = lane / NPF, q = lane % NPF;
@@ -266,7 +303,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				}
 				if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
 			} else if (lane < cnt) {
-				const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
+				const uint32_t id = bwd_row_id(__float_as_uint(s_q[2 * lane + 1].w));
 				float* row = s_rows + lane * RS;
 				*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
 				if (NFT > 0) {
@@ -276,6 +313,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				}
 			}
 			cp_async_commit();
+			BWD_PH_LAP(ph, BWD_PH_ROW_ISSUE);
 		};
 
 		// GEMM 1 of the chunk whose channel rows sit in s_rows, into s_xs
@@ -385,6 +423,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				}
 			}
 			__syncwarp();  // every lane has read its q and wgt fragments: s_xs becomes the per-Gaussian staging area
+			BWD_PH_LAP(ph, BWD_PH_GEMM23);
 			between();
 			// ---- 6. flush ----
 			// feature gradients straight from the D fragments; moments and {r,g,b,depth} gradients to s_xs[g][0..9]
@@ -396,14 +435,30 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					const int g = 16 * mt + 2 * gid + h;  // D rows gid (h = 0) and gid + 8 (h = 1)
 					if (tig < 3) *reinterpret_cast<float2*>(s_m + g * 12 + 2 * tig) = make_float2(mom[mt][2 * h], mom[mt][2 * h + 1]);
 					if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
-					if (NFT > 0 && g < cnt && a.dL_dfeat) {
+					// F = 32: lane tig holds features 8 tig .. 8 tig + 7 of row g, one 32-byte sector (lo = the first four, hi
+					// = the last four).  Lanes tig and tig ^ 1 swap halves so that each red.v4 below pairs with its neighbour's
+					// into one whole sector: lane 2u + e adds into 16 u + 4 e (sector 2u: its own lo and the odd lane's lo), then
+					// 16 u + 8 + 4 e (sector 2u + 1: the even lane's hi and its own hi).  Same reductions, same values per
+					// address, but each one's L2 sector is written whole instead of as two half-sector updates.
+					float sa[4], sb[4];
+					if (VEC && NFT == 4) {
+#pragma unroll
+						for (int nt = 0; nt < 4; nt++) {
+							const float lo = dC[mt][nt % NT][2 * h], hi = dC[mt][nt % NT][2 * h + 1];
+							const float rv = __shfl_xor_sync(0xffffffffu, (tig & 1) ? lo : hi, 1);
+							sa[nt] = (tig & 1) ? rv : lo;
+							sb[nt] = (tig & 1) ? hi : rv;
+						}
+					}
+					if (BWD_FEATURE_RED && NFT > 0 && g < cnt && a.dL_dfeat) {
 						const uint32_t id = __float_as_uint(s_q[2 * g + 1].w);
 						float* df = a.dL_dfeat + (size_t)id * F;
 						// column 2 tig + e of feature tile nt is feature NFT (2 tig + e) + nt
 						if (VEC) {
 							if (NFT == 4) {
-								red_add_v4(df + 8 * tig, dC[mt][0][2 * h], dC[mt][1][2 * h], dC[mt][2][2 * h], dC[mt][3][2 * h]);
-								red_add_v4(df + 8 * tig + 4, dC[mt][0][2 * h + 1], dC[mt][1][2 * h + 1], dC[mt][2][2 * h + 1], dC[mt][3][2 * h + 1]);
+								const int p16 = 16 * (tig >> 1) + 4 * (tig & 1);
+								red_add_v4(df + p16, sa[0], sa[1], sa[2], sa[3]);
+								red_add_v4(df + p16 + 8, sb[0], sb[1], sb[2], sb[3]);
 							} else if (NFT == 2) {
 								red_add_v4(df + 4 * tig, dC[mt][0][2 * h], dC[mt][1 % NT][2 * h], dC[mt][0][2 * h + 1], dC[mt][1 % NT][2 * h + 1]);
 							} else {
@@ -442,6 +497,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 				red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}
 			}
+			BWD_PH_LAP(ph, BWD_PH_FLUSH);
 		};
 
 		// Chunk k: its records arrive in record slot r and its channel rows in stage k & 1, GEMM 1 runs as soon as the rows are
@@ -455,6 +511,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			cp_async_wait<0>();
 			if (lane < c) rec[2 * lane + 1].z = __uint_as_float(cpm);  // the block mask is spent: carry the pixel mask
 			__syncwarp();
+			BWD_PH_LAP(ph, BWD_PH_REC_WAIT);
 			gather_rows(c, rec, rows);
 		};
 		rows_of(cnt, s_rec[0], s_rows[0]);
@@ -465,16 +522,22 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			if (cnt > 0) {
 				cp_async_wait<0>();  // this chunk's channel rows
 				__syncwarp();
+				BWD_PH_LAP(ph, BWD_PH_ROW_WAIT);
 				gemm1(s_rows[s], s_x[s]);
+#ifdef MGS_BWD_PHASES
+				ph.acc[BWD_PH_CHUNKS]++;
+#endif
 			}
 			if (lane == 0) s_cnt[s] = cnt;
 			__syncwarp();
 			named_bar_arrive<BWD_BAR_FULL, 64>(s);
+			BWD_PH_LAP(ph, BWD_PH_GEMM1);
 			const int cnt_next = cnt > 0 ? next_chunk(s_rec[rn]) : 0;  // the next chunk's records travel while this one is finished
 			// the scalar-row path loads synchronously, nothing would travel during the flush: it gathers after it (registers)
 			auto next_rows = [&]() { rows_of(cnt_next, s_rec[rn], s_rows[s ^ 1]); };
 			if (k > 0) {
 				named_bar_sync<BWD_BAR_DONE, 64>(s ^ 1);
+				BWD_PH_LAP(ph, BWD_PH_DONE_WAIT);
 				finish(cnt_prev, s_rec[rp], s_rows[s ^ 1], s_x[s ^ 1], [&]() { if (VEC) next_rows(); });
 			}
 			if (!VEC || k == 0) next_rows();
@@ -484,6 +547,9 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			rp = r;
 			r = rn;
 		}
+#ifdef MGS_BWD_PHASES
+		ph.put(a.bwd_phases, BWD_PH_QUEUE, BWD_PH_FLUSH, BWD_PH_C_TOTAL, true);
+#endif
 	}
 #ifdef MGS_CTA_LOG
 	__syncthreads();  // the CTA ends with the companion's last flush, after the walker has left its loop

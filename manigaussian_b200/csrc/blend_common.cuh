@@ -60,4 +60,57 @@ __device__ __forceinline__ void cta_log_put(const BlendArgs& a, unsigned long lo
 }
 #endif
 
+#ifdef MGS_BWD_PHASES
+// Measurement build only (tools/bwd_phases.py): where a two-warp backward CTA spends its cycles.  Each warp keeps one
+// counter per phase (clock64() laps, lane 0's) and adds them into BlendArgs::bwd_phases when it leaves.
+enum BwdPhase {
+	// companion
+	BWD_PH_QUEUE,      // queue the next chunk's survivors, start its record gather
+	BWD_PH_REC_WAIT,   // wait for the next chunk's records
+	BWD_PH_ROW_ISSUE,  // issue the next chunk's channel-row copies
+	BWD_PH_ROW_WAIT,   // wait for this chunk's channel rows
+	BWD_PH_GEMM1,      // GEMM 1 and the FULL signal
+	BWD_PH_DONE_WAIT,  // wait for the walker to finish the previous chunk
+	BWD_PH_GEMM23,     // GEMM 2/3 of the previous chunk
+	BWD_PH_FLUSH,      // its reductions
+	BWD_PH_C_TOTAL,    // the companion's whole loop
+	// walker
+	BWD_PH_FULL_WAIT,  // wait for the next chunk
+	BWD_PH_WALK,       // walk it
+	BWD_PH_W_TOTAL,    // the walker's whole loop
+	BWD_PH_CHUNKS,     // chunks (non-empty) handed over
+	BWD_PH_CTAS,       // CTAs that reached the loop
+	BWD_PH_COUNT
+};
+struct BwdPhaseClock {
+	unsigned int acc[BWD_PH_COUNT];
+	long long t, t0;
+	__device__ __forceinline__ void start()
+	{
+#pragma unroll
+		for (int i = 0; i < BWD_PH_COUNT; i++) acc[i] = 0u;
+		t = t0 = clock64();
+	}
+	__device__ __forceinline__ void lap(int ph)
+	{
+		const long long n = clock64();
+		acc[ph] += (unsigned int)(n - t);
+		t = n;
+	}
+	// total: the phase that receives the whole loop; phases [first, last] are this warp's
+	__device__ __forceinline__ void put(unsigned long long* out, int first, int last, int total, bool lead)
+	{
+		acc[total] = (unsigned int)(clock64() - t0);
+		if (out == nullptr || (threadIdx.x & 31) != 0) return;
+#pragma unroll
+		for (int i = 0; i < BWD_PH_COUNT; i++)
+			if ((i >= first && i <= last) || i == total || (lead && (i == BWD_PH_CHUNKS || i == BWD_PH_CTAS)))
+				atomicAdd(out + i, (unsigned long long)acc[i]);
+	}
+};
+#define BWD_PH_LAP(ph, p) (ph).lap(p)
+#else
+#define BWD_PH_LAP(ph, p) do { } while (0)
+#endif
+
 }  // namespace mgs

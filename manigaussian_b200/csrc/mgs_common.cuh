@@ -121,6 +121,8 @@ __device__ __forceinline__ void red_add(float* addr, float a)
 {
 	asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(a) : "memory");
 }
+// bring the line holding p into L1 (no register, nothing to wait for)
+__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 __device__ __forceinline__ float4 ldg_nc_v4(const float4* p)
 {
 	float4 r;

@@ -118,6 +118,11 @@ struct BlendArgs {
 	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams
 	unsigned long long* cta_log; unsigned int* cta_log_n; unsigned int cta_log_cap;
 #endif
+#ifdef MGS_BWD_PHASES
+	// measurement build only (tools/bwd_phases.py): the two-warp backward adds its clock64() cycles per phase and its chunk
+	// count into bwd_phases[BWD_PH_COUNT] (blend_common.cuh)
+	unsigned long long* bwd_phases;
+#endif
 };
 // loss_heads.cu: the same heads for images that already sit in memory (planar [3,H,W] / [F,H,W], V views in one launch).
 // color == null: features only -- the embedding head alone, into loss_acc[2 v + 1] (the colour head ran elsewhere).
