@@ -275,6 +275,37 @@ int mgs_backward_views(
 	int debug,
 	void* join_stream);
 
+/*
+ * Several clouds in one step (no reference counterpart).  A ManiGaussian training step with the dynamic field renders two
+ * clouds -- the current frame and the deformed next frame (agents/manigaussian_bc/neural_rendering.py:283, :324) -- and
+ * 2 B clouds for B samples per GPU, which the reference cannot do at all (it asserts bs == 1, :386).  Cloud b renders
+ * views[view_offsets[b] .. view_offsets[b + 1]); view_offsets (host, B + 1 ints) starts at 0 and strictly increases.
+ * D, M, F and scale_modifier are shared by every cloud; a cloud with feature == NULL renders no features.  Every mgs_view
+ * field means what it means for mgs_forward_views / mgs_backward_views (capacity, status, overflow, loss heads, streams);
+ * dL_dmean2D is each view's own [P_b,3].
+ * mgs_forward_clouds enqueues stage by stage across ALL views of all clouds (every projection, then every binning chain,
+ * then every blend) between one fork from and one join into join_stream, so one cloud's short kernels never queue behind
+ * another cloud's blends.  No host synchronisation: a step built from these calls can be captured in a CUDA graph.
+ * mgs_backward_clouds runs the blend backward of every view on its stream, joins, then the per-Gaussian stage on
+ * join_stream in launches of up to 16 views that pack whole clouds.  Each cloud's outputs are the sums over its views
+ * (overwritten, or added to with accumulate = 1); NULL-ability as in mgs_backward, except:
+ *   - dL_dfeature NULL on a cloud with features: its feature gradient is not computed, but the feature cotangents still
+ *     reach its mean, conic and opacity gradients;
+ *   - shs without dL_dsh is MGS_ERR_INVALID_ARG: dL_dsh comes with the view-direction term of dL_dmean3D.
+ * Argument errors (B <= 0, bad view_offsets, P <= 0, missing pointers) return MGS_ERR_INVALID_ARG before anything is enqueued.
+ */
+typedef struct mgs_cloud {
+	int P;
+	const float *means3D, *shs, *colors_precomp, *feature, *opacities, *scales, *rotations, *cov3D_precomp;
+	/* backward outputs of this cloud: [P,3], [P] (or [P,1]), [P,3], [P,F], [P,6], [P,M,3], [P,3], [P,4] */
+	float *dL_dmean3D, *dL_dopacity, *dL_dcolor, *dL_dfeature, *dL_dcov3D, *dL_dsh, *dL_dscale, *dL_drot;
+} mgs_cloud;
+
+int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -27,6 +27,13 @@ class View(C.Structure):
                 ("cot_feature", C.c_void_p), ("loss_acc", C.c_void_p), ("cot_scale", C.c_void_p)]
 
 
+class Cloud(C.Structure):
+    """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
+    _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
+        "means3D", "shs", "colors_precomp", "feature", "opacities", "scales", "rotations", "cov3D_precomp",
+        "dL_dmean3D", "dL_dopacity", "dL_dcolor", "dL_dfeature", "dL_dcov3D", "dL_dsh", "dL_dscale", "dL_drot")]
+
+
 _lib = None
 
 
@@ -81,6 +88,11 @@ def lib():
                                      vp, f, vp, vp,                     # scales scale_modifier rotations cov3D_precomp
                                      vp, vp, vp, vp, vp, vp, vp, vp,    # dL: mean3D opacity color feature cov3D sh scale rot
                                      i, i, i, i, vp]                    # shared_mean2D accumulate stages debug join_stream
+    for name in ("mgs_forward_clouds", "mgs_backward_clouds"):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = [i, C.POINTER(Cloud), C.POINTER(C.c_int), C.POINTER(View),  # B clouds view_offsets views
+                                     i, i, i, f,                                                 # D M F scale_modifier
+                                     i, i, vp]  # prefiltered (forward) or accumulate (backward), debug, join_stream
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_mark_visible.restype = C.c_int
@@ -110,7 +122,7 @@ def lib():
 EXPORTED_SYMBOLS = (
     "mgs_abi_version", "mgs_last_error", "mgs_geometry_state_bytes", "mgs_image_state_bytes",
     "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_forward", "mgs_forward_begin",
-    "mgs_backward", "mgs_forward_views", "mgs_backward_views", "mgs_loss_heads",
+    "mgs_backward", "mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds", "mgs_loss_heads",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

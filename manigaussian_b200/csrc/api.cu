@@ -462,6 +462,39 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, int debug)
 	return 0;
 }
 
+// blend backward of one view on its stream: the view's blend-stage records, and the feature gradients summed with 128-bit
+// reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
+// and opacity gradients; only the feature rows are not reduced.
+static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, int debug)
+{
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+	const int F = c.F;
+	const ViewState s = carve_view(w, c.P);
+	MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)c.P * GB_STRIDE * sizeof(float), st));
+	BlendArgs ba = blend_args(s, w, F, c.feature);
+	ba.want_depth = w.dL_dpix_depth != nullptr;
+	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth;
+	ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
+	ba.cot_scale = w.cot_scale;
+	if (w.binning_capacity > 0) {
+		{ StageTimer t_(ST_BLEND_BWD, st); launch_blend_bwd(ba, st); }
+		MGS_STAGE("blend_bwd");
+	}
+	return 0;
+}
+
+// the per-Gaussian stage's view of one view: its blend-stage records, clamp bits and camera
+static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
+{
+	const ViewState s = carve_view(w, P);
+	ProjectBwdView pv;
+	pv.radii = w.radii; pv.gb = s.gb; pv.clamped = s.geom.clamped; pv.viewmatrix = w.viewmatrix; pv.projmatrix = w.projmatrix;
+	pv.cam_pos = w.cam_pos; pv.dL_dmean2D = dL_dmean2D;
+	pv.tan_fovx = w.tan_fovx; pv.tan_fovy = w.tan_fovy;
+	pv.focal_x = w.width / (2.0f * w.tan_fovx); pv.focal_y = w.height / (2.0f * w.tan_fovy);
+	return pv;
+}
+
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.
@@ -474,22 +507,9 @@ static int backward_views(int V, const mgs_view* views, const Cloud& c, float* d
 		if (F > 0 && !accumulate) MGS_CUDA(cudaMemsetAsync(dL_dfeature, 0, (size_t)P * F * sizeof(float), join));
 		int rc = fork_streams(V, views, join);
 		if (rc < 0) return rc;
-		// blend stage of every view on its own stream: per-view blend-stage records, feature gradients summed with 128-bit
-		// reductions straight into dL_dfeature
 		for (int v = 0; v < V; v++) {
-			const mgs_view& w = views[v];
-			cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
-			const ViewState s = carve_view(w, P);
-			MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)P * GB_STRIDE * sizeof(float), st));
-			BlendArgs ba = blend_args(s, w, F, c.feature);
-			ba.want_depth = w.dL_dpix_depth != nullptr;
-			ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth;
-			ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
-			ba.cot_scale = w.cot_scale;
-			if (w.binning_capacity > 0) {
-				{ StageTimer t_(ST_BLEND_BWD, st); launch_blend_bwd(ba, st); }
-				MGS_STAGE("blend_bwd");
-			}
+			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, debug);
+			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
 		if (rc < 0) return rc;
@@ -512,15 +532,8 @@ static int backward_views(int V, const mgs_view* views, const Cloud& c, float* d
 		pb.dL_dmean3D = dL_dmean3D; pb.dL_dopacity = dL_dopacity; pb.dL_dcolor = dL_dcolor; pb.dL_dcov3D = dL_dcov3D;
 		pb.dL_dsh = pb.shs ? dL_dsh : nullptr; pb.dL_dscale = have_sr ? dL_dscale : nullptr; pb.dL_drot = have_sr ? dL_drot : nullptr;
 		pb.dL_dconic = pb.accumulate ? nullptr : dL_dconic;
-		for (int u = 0; u < pb.V; u++) {
-			const mgs_view& w = views[v0 + u];
-			const ViewState s = carve_view(w, P);
-			ProjectBwdView& pv = pb.view[u];
-			pv.radii = w.radii; pv.gb = s.gb; pv.clamped = s.geom.clamped; pv.viewmatrix = w.viewmatrix; pv.projmatrix = w.projmatrix;
-			pv.cam_pos = w.cam_pos; pv.dL_dmean2D = shared_mean2D ? views[0].dL_dmean2D : w.dL_dmean2D;
-			pv.tan_fovx = w.tan_fovx; pv.tan_fovy = w.tan_fovy;
-			pv.focal_x = w.width / (2.0f * w.tan_fovx); pv.focal_y = w.height / (2.0f * w.tan_fovy);
-		}
+		for (int u = 0; u < pb.V; u++)
+			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); }
 		MGS_STAGE("project_bwd");
 	}
@@ -545,6 +558,43 @@ static int project_single_view(const Cloud& c, mgs_view& w, mgs_alloc_fn geometr
 	MGS_CUDA(cudaMemcpyAsync(host_count, carve_view(w, c.P).geom.point_offsets + c.P - 1, sizeof(int), cudaMemcpyDeviceToHost,
 		reinterpret_cast<cudaStream_t>(w.stream)));
 	return 0;
+}
+
+static int check_fwd_view(const mgs_view& w, bool need_cam_pos)
+{
+	if (!w.viewmatrix || !w.projmatrix || !w.background || !w.geometry_state || !w.binning_state || !w.image_state || !w.out_color || !w.radii)
+		return fail(MGS_ERR_INVALID_ARG, "view: matrices, background, the three state buffers, out_color and radii are required");
+	if (need_cam_pos && !w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: cam_pos is required with SHs");
+	if (w.width <= 0 || w.height <= 0 || w.binning_capacity < 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size or capacity");
+	return 0;
+}
+
+static int check_bwd_view(const mgs_view& w, bool need_dpix_F)
+{
+	if (!w.viewmatrix || !w.projmatrix || !w.background || !w.geometry_state || !w.binning_state || !w.image_state || !w.radii ||
+		!w.dL_dpix || !w.blend_scratch)
+		return fail(MGS_ERR_INVALID_ARG, "view: matrices, background, state buffers, radii, dL_dpix and blend_scratch are required");
+	if (need_dpix_F && !w.dL_dpix_F) return fail(MGS_ERR_INVALID_ARG, "view: dL_dpix_F is required with features");
+	return 0;
+}
+
+// the checks the multi-cloud forward and backward share: B, the view ranges and every cloud's size
+static int check_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views)
+{
+	if (B <= 0 || !clouds || !view_offsets || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one cloud, view_offsets and views");
+	if (view_offsets[0] != 0) return fail(MGS_ERR_INVALID_ARG, "view_offsets must start at 0");
+	for (int b = 0; b < B; b++) {
+		if (view_offsets[b + 1] <= view_offsets[b])
+			return fail(MGS_ERR_INVALID_ARG, "view_offsets must be strictly increasing: every cloud needs at least one view");
+		if (clouds[b].P <= 0) return fail(MGS_ERR_INVALID_ARG, "cloud: P must be > 0");
+	}
+	return 0;
+}
+
+static Cloud cloud_of(const mgs_cloud& k, int D, int M, int F, float scale_modifier)
+{
+	return Cloud{ k.P, D, M, k.feature ? F : 0, k.means3D, k.shs, k.colors_precomp, k.feature, k.opacities, k.scales, scale_modifier,
+		k.rotations, k.cov3D_precomp };
 }
 
 }  // namespace mgs
@@ -660,11 +710,8 @@ int mgs_forward_views(
 	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int v = 0; v < V; v++) {
-		const mgs_view& w = views[v];
-		if (!w.viewmatrix || !w.projmatrix || !w.background || !w.geometry_state || !w.binning_state || !w.image_state || !w.out_color || !w.radii)
-			return fail(MGS_ERR_INVALID_ARG, "view: matrices, background, the three state buffers, out_color and radii are required");
-		if (!colors_precomp && !w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: cam_pos is required with SHs");
-		if (w.width <= 0 || w.height <= 0 || w.binning_capacity < 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size or capacity");
+		int rc = check_fwd_view(views[v], !colors_precomp);
+		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp };
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
@@ -707,15 +754,121 @@ int mgs_backward_views(
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	if (F > 0 && (!feature_precomp || !dL_dfeature)) F = 0;
 	for (int v = 0; v < V; v++) {
-		const mgs_view& w = views[v];
-		if (!w.viewmatrix || !w.projmatrix || !w.background || !w.geometry_state || !w.binning_state || !w.image_state || !w.radii ||
-			!w.dL_dpix || !w.blend_scratch)
-			return fail(MGS_ERR_INVALID_ARG, "view: matrices, background, state buffers, radii, dL_dpix and blend_scratch are required");
-		if (F > 0 && !w.dL_dpix_F) return fail(MGS_ERR_INVALID_ARG, "view: dL_dpix_F is required with features");
+		int rc = check_bwd_view(views[v], F > 0);
+		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp };
 	return backward_views(V, views, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
+}
+
+int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
+	float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
+	(void)prefiltered;
+	int rc = check_clouds(B, clouds, view_offsets, views);
+	if (rc < 0) return rc;
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		if (!k.means3D || !k.opacities) return fail(MGS_ERR_INVALID_ARG, "cloud: means3D/opacities are required");
+		if (!k.colors_precomp && !k.shs) return fail(MGS_ERR_INVALID_ARG, "cloud: provide SHs or precomputed colours");
+		if (!k.cov3D_precomp && (!k.scales || !k.rotations))
+			return fail(MGS_ERR_INVALID_ARG, "cloud: provide scales+rotations or a precomputed 3D covariance");
+		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+			rc = check_fwd_view(views[v], !k.colors_precomp);
+			if (rc < 0) return rc;
+		}
+	}
+	const int V = view_offsets[B];
+	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
+	rc = fork_streams(V, views, join);
+	if (rc < 0) return rc;
+	// stage by stage across the views of every cloud, as in mgs_forward_views
+	for (int phase = 0; phase < 3; phase++) {
+		for (int b = 0; b < B; b++) {
+			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
+			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+				rc = phase == 0 ? enqueue_project(c, views[v], debug)
+					: phase == 1 ? enqueue_binning(c, views[v], false, debug) : enqueue_blend_fwd(c, views[v], debug);
+				if (rc < 0) return rc;
+			}
+		}
+	}
+	return join_streams(V, views, join);
+}
+
+int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream)
+{
+	int rc = check_clouds(B, clouds, view_offsets, views);
+	if (rc < 0) return rc;
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		if (!k.means3D || !k.dL_dmean3D || !k.dL_dopacity)
+			return fail(MGS_ERR_INVALID_ARG, "cloud: means3D, dL_dmean3D and dL_dopacity are required");
+		if (k.shs && !k.dL_dsh)
+			return fail(MGS_ERR_INVALID_ARG, "cloud: dL_dsh is required with SHs (it carries the view-direction term of dL_dmean3D)");
+		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+			rc = check_bwd_view(views[v], F > 0 && k.feature);
+			if (rc < 0) return rc;
+		}
+	}
+	const int V = view_offsets[B];
+	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		if (F > 0 && k.feature && k.dL_dfeature && !accumulate)
+			MGS_CUDA(cudaMemsetAsync(k.dL_dfeature, 0, (size_t)k.P * F * sizeof(float), join));
+	}
+	rc = fork_streams(V, views, join);
+	if (rc < 0) return rc;
+	for (int b = 0; b < B; b++) {
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
+		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, debug);
+			if (rc < 0) return rc;
+		}
+	}
+	rc = join_streams(V, views, join);
+	if (rc < 0) return rc;
+
+	// per-Gaussian stage on `join`: launches of at most MAX_BWD_VIEWS views that pack whole clouds; a cloud with more views
+	// spans launches, and its later launches add to what the earlier ones wrote
+	const cudaStream_t st = join;
+	ProjectBwdCloudsArgs pb{};
+	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier;
+	int nv = 0;  // views in pb
+	auto flush = [&]() -> int {
+		if (pb.B == 0) return 0;
+		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); }
+		MGS_STAGE("project_bwd");
+		pb.B = 0; nv = 0;
+		return 0;
+	};
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		const bool have_sr = k.scales && k.rotations && k.dL_dscale && k.dL_drot;
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			const int n = std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS);
+			if (nv + n > MAX_BWD_VIEWS) {
+				rc = flush();
+				if (rc < 0) return rc;
+			}
+			ProjectBwdCloud& pc = pb.cloud[pb.B++];
+			pc.P = k.P; pc.V = n; pc.view0 = nv;
+			pc.means3D = k.means3D; pc.shs = k.shs; pc.scales = have_sr ? k.scales : nullptr; pc.rotations = k.rotations;
+			// gradients w.r.t. scale/rotation not requested: the forward's own covariance (any view's copy) serves
+			pc.cov3D_precomp = (have_sr || k.cov3D_precomp) ? k.cov3D_precomp : carve_view(views[view_offsets[b]], k.P).geom.cov3D;
+			pc.accumulate = (accumulate || v0 > view_offsets[b]) ? 1 : 0;
+			pc.dL_dmean3D = k.dL_dmean3D; pc.dL_dopacity = k.dL_dopacity; pc.dL_dcolor = k.dL_dcolor; pc.dL_dcov3D = k.dL_dcov3D;
+			pc.dL_dsh = k.shs ? k.dL_dsh : nullptr; pc.dL_dscale = have_sr ? k.dL_dscale : nullptr; pc.dL_drot = have_sr ? k.dL_drot : nullptr;
+			for (int u = 0; u < n; u++) pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
+			nv += n;
+		}
+	}
+	return flush();
 }
 
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

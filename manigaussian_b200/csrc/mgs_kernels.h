@@ -69,6 +69,26 @@ struct ProjectBwdViewsArgs {
 	float* dL_dconic;   // [P,4] nullable; view 0 only (single-view callers)
 	ProjectBwdView view[MAX_BWD_VIEWS];
 };
+// the same chain rule for several clouds in one launch: cloud c sums views view[view0 .. view0 + V) of the launch
+// (every cloud has a view, so MAX_BWD_VIEWS clouds at most); dL_dmean2D per view only, no dL_dconic
+struct ProjectBwdCloud {
+	int P, V, view0;
+	int block0;                  // first CTA of the cloud, set by the launcher
+	const float* means3D;
+	const float* shs;            // nullable (precomputed colours)
+	const float* scales;         // nullable (precomputed covariance)
+	const float* rotations;
+	const float* cov3D_precomp;  // used when scales is null
+	int accumulate;
+	float* dL_dmean3D; float* dL_dopacity; float* dL_dcolor; float* dL_dcov3D; float* dL_dsh; float* dL_dscale; float* dL_drot;
+};
+struct ProjectBwdCloudsArgs {
+	int D, M, B;  // SH degree and coefficients of every cloud, B clouds
+	float scale_modifier;
+	ProjectBwdCloud cloud[MAX_BWD_VIEWS];
+	ProjectBwdView view[MAX_BWD_VIEWS];
+};
+static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 
 struct BlendArgs {
 	int W, H;
@@ -159,6 +179,7 @@ void launch_activate_bwd(ActivateArgs a, cudaStream_t s);
 
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s);
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s);
+void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s);
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s);
 
 // binning.cu

@@ -17,6 +17,7 @@
 // radius and clamp bits; the Gaussian's own inputs are read once, every output row is written once, and the sum over
 // views happens in registers -- no atomics, no zero-fill pass, no per-view gradient tensors.  The multi-view callers
 // (rasterize_views_backward_raw, render_views) write straight into the packed buffer that is the all-reduce message.
+// project_bwd_clouds_kernel runs the same body for several clouds in one launch (mgs_backward_clouds, DESIGN.md section 4).
 #include "mgs_common.cuh"
 #include "mgs_kernels.h"
 
@@ -43,11 +44,11 @@ __device__ __forceinline__ float dot3(const float* u, const float* v) { return u
 #ifndef MGS_PBWD_MINB
 #define MGS_PBWD_MINB 5
 #endif
-template <int NSH, int MIN_BLOCKS>
-__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
+// The chain rule of Gaussian idx over the views a.view[0 .. a.V).  Args: ProjectBwdViewsArgs, or CloudBwd (one cloud of a
+// multi-cloud launch) -- the same member names.
+template <int NSH, class Args>
+__device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx)
 {
-	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-	if (idx >= a.P) return;
 	const float p[3] = { a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2] };
 
 	// ---- the Gaussian's own covariance: S = L L^T, L = R(q) diag(mod * s), or the caller's ----
@@ -273,6 +274,43 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(Proj
 	}
 }
 
+template <int NSH, int MIN_BLOCKS>
+__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
+{
+	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= a.P) return;
+	project_bwd_gaussian<NSH>(a, idx);
+}
+
+namespace {
+// one cloud of a ProjectBwdCloudsArgs launch under the member names project_bwd_gaussian reads; per-view screen-space
+// gradients only, no dL_dconic
+struct CloudBwd {
+	int D, M, V;
+	const float* means3D; const float* shs; const float* scales; const float* rotations; float scale_modifier;
+	const float* cov3D_precomp;
+	int accumulate;
+	static constexpr int shared_mean2D = 0;
+	float* dL_dmean3D; float* dL_dopacity; float* dL_dcolor; float* dL_dcov3D; float* dL_dsh; float* dL_dscale; float* dL_drot;
+	static constexpr float* dL_dconic = nullptr;
+	const ProjectBwdView* view;
+};
+}  // namespace
+
+// several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
+template <int NSH, int MIN_BLOCKS>
+__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
+{
+	int c = 0;
+	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
+	const ProjectBwdCloud& cl = a.cloud[c];
+	const int idx = ((int)blockIdx.x - cl.block0) * blockDim.x + threadIdx.x;
+	if (idx >= cl.P) return;
+	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
+		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0 };
+	project_bwd_gaussian<NSH>(cb, idx);
+}
+
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0 || a.V <= 0) return;
@@ -281,6 +319,24 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	if (deg <= 1) project_bwd_views_kernel<12, MGS_PBWD_MINB><<<grid, 128, 0, s>>>(a);
 	else if (deg == 2) project_bwd_views_kernel<27, 4><<<grid, 128, 0, s>>>(a);
 	else project_bwd_views_kernel<48, 3><<<grid, 128, 0, s>>>(a);
+}
+
+void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
+{
+	if (a.B <= 0) return;
+	int grid = 0;
+	bool sh = false;
+	for (int c = 0; c < a.B; c++) {
+		a.cloud[c].block0 = grid;
+		grid += ceil_div(a.cloud[c].P, 128);
+		sh |= a.cloud[c].shs != nullptr;
+	}
+	const int deg = sh ? a.D : 0;
+	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
+	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
+	if (deg <= 1) project_bwd_clouds_kernel<12, 4><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_clouds_kernel<27, 4><<<grid, 128, 0, s>>>(a);
+	else project_bwd_clouds_kernel<48, 3><<<grid, 128, 0, s>>>(a);
 }
 
 }  // namespace mgs

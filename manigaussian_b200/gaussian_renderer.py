@@ -13,6 +13,9 @@ views are enqueued on per-view streams by one C call that never synchronises wit
 per-Gaussian gradients in registers into one packed buffer (`parallel.PackedGradients`), and -- for the view-parallel
 multi-GPU mode -- that buffer is all-reduced with ONE collective before the gradients are handed back to autograd.
 The reference has no counterpart (bs == 1 is asserted, neural_rendering.py:386; one view per call).
+
+`render_clouds` renders several clouds -- the current and the deformed next frame of the dynamic-field step, for every
+sample of the batch -- in one autograd node and one C call per direction, every view on its own stream.
 """
 import math
 
@@ -21,8 +24,8 @@ import torch
 from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, rasterize_views_backward_raw,
-                         rasterize_views_raw)
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, rasterize_clouds_backward_raw,
+                         rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
 MIN_DENOMINATOR = 1e-12  # gaussian_renderer/__init__.py:67; compiled into the kernel (activate.cu FEAT_EPS)
@@ -307,4 +310,173 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
            "radii": radii}
     if return_depth:
         ret["depth"] = depth
+    return ret
+
+
+_CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations
+
+
+class _RasterizeClouds(torch.autograd.Function):
+    """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None).  Outputs per cloud: (color,
+    feature image, radii, depth), or with targets (loss_rgb, loss_embed, color, feature image, radii) with gradients through
+    the two losses only."""
+
+    @staticmethod
+    def forward(ctx, meta, *flat):
+        cloud_views, return_depth, targets = meta
+        B, dev = len(cloud_views), flat[0].device
+        opts = dict(dtype=torch.float32, device=dev)
+        clouds, results, frozen, cots = [], [], [], []
+        for b, views in enumerate(cloud_views):
+            means3D, _, sh, colors, feature, opacities, scales, rotations = (_prep(t, dev) for t in flat[_CLOUD_INPUTS * b:_CLOUD_INPUTS * (b + 1)])
+            V, H, W = len(views), int(views[0].image_height), int(views[0].image_width)
+            F = int(feature.shape[1]) if feature is not None else 0
+            color = torch.empty((V, 3, H, W), **opts)
+            feat_img = torch.empty((V, F, H, W), **opts) if F else None
+            depth = torch.empty((V, H, W), **opts) if return_depth else None
+            c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, opacity=opacities, scales=scales,
+                     rotations=rotations, out_buffers=(color, feat_img, depth))
+            if targets is not None:
+                t_rgb = _prep(targets[b]["rgb"], dev)
+                t_emb = _prep(targets[b].get("embed"), dev) if F else None
+                if tuple(t_rgb.shape) != (V, 3, H, W) or (t_emb is not None and tuple(t_emb.shape) != (V, F, H, W)):
+                    raise ValueError(f"cloud {b}: targets must be [V,3,H,W] and [V,F,H,W]")
+                cot_rgb = torch.empty((V, 3, H, W), **opts)
+                cot_emb = torch.empty((V, F, H, W), **opts) if t_emb is not None else (torch.zeros((V, F, H, W), **opts) if F else None)
+                loss_acc = torch.empty((V, 2), **opts)
+                c["loss_heads"] = (t_rgb, t_emb, cot_rgb, cot_emb, loss_acc)
+                cots.append((cot_rgb, cot_emb))
+            clouds.append(c)
+        degree = cloud_views[0][0].sh_degree
+        include = clouds[0]["feature"] is not None
+        outs, streams = rasterize_clouds_raw(clouds, degree, include, cloud_views[0][0].scale_modifier, return_depth=return_depth,
+                                             debug=cloud_views[0][0].debug)
+        for b, c in enumerate(clouds):
+            color, feat_img, depth = c["out_buffers"]
+            radii = torch.stack([o[3] for o in outs[b]])
+            empty = lambda: torch.empty(0, device=dev)
+            if targets is not None:
+                N = float(color.shape[2] * color.shape[3])
+                loss_acc = c["loss_heads"][4]
+                loss_rgb = loss_acc[:, 0] / (3.0 * N)
+                loss_embed = 1.0 - loss_acc[:, 1] / N if c["loss_heads"][1] is not None else torch.zeros((len(c["views"]),), **opts)
+                results += [loss_rgb, loss_embed, color, feat_img if feat_img is not None else empty(), radii]
+                frozen += [radii, color] + ([feat_img] if feat_img is not None else [])
+            else:
+                results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty()]
+                frozen.append(radii)
+        ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots = meta, streams, degree, include, cots
+        # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
+        ctx.state = [[(o[0], o[3], o[4], o[5], o[6]) for o in co] for co in outs]
+        ctx.opac_shapes = [flat[_CLOUD_INPUTS * b + 5].shape for b in range(B)]
+        e = torch.empty(0, device=dev)
+        ctx.save_for_backward(*[x if x is not None else e for c in clouds for x in
+                                (c["means3D"], c["sh"], c["colors"], c["feature"], c["scales"], c["rotations"])])
+        ctx.mark_non_differentiable(*frozen)  # ONE call: a second one replaces the first
+        return tuple(results)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        cloud_views, return_depth, targets = ctx.meta
+        saved = ctx.saved_tensors
+        dev = saved[0].device
+        per = 5 if targets is not None else 4
+        clouds = []
+        for b, views in enumerate(cloud_views):
+            means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
+            V, H, W = len(views), int(views[0].image_height), int(views[0].image_width)
+            F = int(feature.shape[1]) if feature is not None else 0
+            g = grads[per * b:per * (b + 1)]
+            c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, scales=scales, rotations=rotations,
+                     want_feature=bool(ctx.needs_input_grad[1 + _CLOUD_INPUTS * b + 4]))
+            if targets is not None:
+                z = torch.zeros((V,), dtype=torch.float32, device=dev)
+                c["cot_scale"] = torch.stack([g[0] if g[0] is not None else z, g[1] if g[1] is not None else z], 1).contiguous()
+                c["grad_color"], c["grad_feature"] = ctx.cots[b]
+            else:
+                c["grad_color"] = g[0] if g[0] is not None else torch.zeros((V, 3, H, W), dtype=torch.float32, device=dev)
+                if F:
+                    c["grad_feature"] = g[1] if g[1] is not None else torch.zeros((V, F, H, W), dtype=torch.float32, device=dev)
+                if return_depth and g[3] is not None:
+                    c["grad_depth"] = g[3]
+            clouds.append(c)
+        # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
+        outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
+        res = rasterize_clouds_backward_raw(clouds, outs, ctx.streams, ctx.degree, ctx.include, cloud_views[0][0].scale_modifier,
+                                            debug=cloud_views[0][0].debug)
+        ret = [None]
+        for b, r in enumerate(res):
+            P = clouds[b]["means3D"].shape[0]
+            M = clouds[b]["sh"].shape[1] if clouds[b]["sh"] is not None else 0
+            ret += [r["dL_dmeans3D"], r["dL_dmeans2D"], r["dL_dsh"].view(P, M, 3) if M else None, r["dL_dcolors"], r["dL_dfeature"],
+                    r["dL_dopacity"].view(ctx.opac_shapes[b]), r["dL_dscales"], r["dL_drotations"]]
+        return tuple(ret)
+
+
+def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True):
+    """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
+    next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
+
+    clouds: sequence of dicts with the keyword names of render_views -- "cameras", optional "view_ids", "pts_xyz",
+    "rotations", "scales", "opacity", "features_color" or "pts_rgb", optional "features_language" and optional "targets".
+    The clouds share the SH degree, the feature width F and the colour mode (ValueError naming the field otherwise); within a
+    cloud all views share one image size, different clouds may differ.  Targets are given on all clouds or on none.
+    Returns one dict per cloud with the keys and shapes render_views returns for it ("loss_rgb" / "loss_embed" with targets).
+    A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
+    dyna step, which renders the detached current features); its feature cotangents still reach its other gradients."""
+    if not clouds:
+        raise ValueError("render_clouds needs at least one cloud")
+    with_targets = [c.get("targets") is not None for c in clouds]
+    if any(with_targets) and not all(with_targets):
+        raise ValueError("targets must be given on all clouds or on none")
+    if all(with_targets) and return_depth:
+        raise ValueError("targets and return_depth cannot be combined")
+    if len({c.get("features_color") is None for c in clouds}) > 1:
+        raise ValueError("clouds disagree on the colour mode (SHs or precomputed colors)")
+    device = clouds[0]["pts_xyz"].device
+    cloud_views = []
+    for b, c in enumerate(clouds):
+        include = c.get("features_language") is not None
+        sh_degree = 3 if c.get("features_color") is None else 1
+        cameras, view_ids = c["cameras"], c.get("view_ids")
+        if isinstance(cameras, CameraBatch):
+            ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
+            views = tuple(cameras.settings(i, _background(bg_color, device), sh_degree, include) for i in ids)
+        else:
+            views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+        if not views:
+            raise ValueError(f"cloud {b} has no views")
+        if c.get("features_color") is None and c.get("pts_rgb") is None:
+            raise ValueError("Please provide excatly one of either SHs or precomputed colors!")
+        if any((int(s.image_height), int(s.image_width)) != (int(views[0].image_height), int(views[0].image_width)) for s in views):
+            raise ValueError(f"cloud {b}: all views of a cloud need one image size")
+        cloud_views.append(views)
+    if len({int(s.sh_degree) for views in cloud_views for s in views}) > 1:
+        raise ValueError("clouds disagree on the SH degree")
+    _prep_clouds([dict(means3D=c["pts_xyz"], sh=c.get("features_color"), colors=c.get("pts_rgb") if c.get("features_color") is None else None,
+                       feature=c.get("features_language")) for c in clouds], device, True)
+    flat, vsps = [], []
+    for c, views in zip(clouds, cloud_views):
+        f = c.get("features_language")
+        if f is not None and normalize_feature:
+            f = normalize_features(f)
+        # its .grad receives each view's screen-space mean gradients, as in render_views
+        vsps.append(torch.zeros((len(views), c["pts_xyz"].shape[0], 3), dtype=torch.float32, device=device, requires_grad=True))
+        flat += [c["pts_xyz"], vsps[-1], c.get("features_color"), c.get("pts_rgb") if c.get("features_color") is None else None, f,
+                 c["opacity"], c["scales"], c["rotations"]]
+    targets = [c["targets"] for c in clouds] if all(with_targets) else None
+    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets), *flat)
+    ret = []
+    for b, c in enumerate(clouds):
+        include, vsp = c.get("features_language") is not None, vsps[b]
+        if targets is not None:
+            loss_rgb, loss_embed, color, feat_img, radii = out[5 * b:5 * b + 5]
+            ret.append({"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii,
+                        "loss_rgb": loss_rgb, "loss_embed": loss_embed})
+        else:
+            color, feat_img, radii, depth = out[4 * b:4 * b + 4]
+            r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii}
+            if return_depth:
+                r["depth"] = depth
+            ret.append(r)
     return ret

@@ -14,6 +14,7 @@ depth plane.
 """
 from typing import NamedTuple
 
+import ctypes
 import os
 
 import torch
@@ -560,48 +561,59 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
-            H, W = int(s.image_height), int(s.image_width)
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
-            gbytes, ibytes, _ = _state_sizes(L, P, W, H)
-            geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
-            img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
-            binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
-            radii = torch.empty((P,), dtype=torch.int32, device=dev)
-            bg, vm, pm, cp = (_prep(x, dev) for x in (s.bg, s.viewmatrix, s.projmatrix, s.campos))
-            if out_buffers is not None:
-                out_color = out_buffers[0][v]
-                out_feature = out_buffers[1][v] if (include_feature and F) else torch.zeros((1,), dtype=torch.float32, device=dev)
-                out_depth = out_buffers[2][v] if return_depth else None
-            else:
-                out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-                out_feature = torch.empty((F, H, W), dtype=torch.float32, device=dev) if include_feature else \
-                    torch.zeros((1,), dtype=torch.float32, device=dev)
-                out_depth = torch.empty((H, W), dtype=torch.float32, device=dev) if return_depth else None
-            w = arr[v]
-            w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
-            w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
-            w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
-            w.out_color, w.out_feature, w.out_depth, w.radii = _ptr(out_color), (_ptr(out_feature) if F else None), _ptr(out_depth), _ptr(radii)
-            w.status = status.data_ptr() + 8 * v
-            w.stream = streams[v].cuda_stream
-            if loss_heads is not None:
-                t_rgb, t_emb, c_rgb, c_emb, l_acc = loss_heads
-                w.target_color, w.cot_color, w.loss_acc = _ptr(t_rgb[v]), _ptr(c_rgb[v]), _ptr(l_acc[v])
-                if t_emb is not None and F:
-                    w.target_feature, w.cot_feature = _ptr(t_emb[v]), _ptr(c_emb[v])
-            keep.append((bg, vm, pm, cp))
-            ret = (cap, out_color, out_feature, radii, geom, binb, img) + ((out_depth,) if return_depth else ())
-            outs.append(ViewOut(ret))
+            o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads)
+            arr[v].status = status.data_ptr() + 8 * v
+            arr[v].stream = streams[v].cuda_stream
+            keep.append(k)
+            outs.append(o)
         _b.check(L.mgs_forward_views(V, arr, P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors),
                                      _ptr(language_feature) if F else None, _ptr(opacity), _ptr(scales), float(scale_modifier),
                                      _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream), "mgs_forward_views")
-        ev = torch.cuda.Event()
-        ev.record(main)
-        for v, o in enumerate(outs):
-            o.status, o.event = status[v], ev
-            if capacities is None and not capturing:
-                _PENDING_STATUS.append((keys[v], status[v], ev, o[0]))
+        _track_status(outs, keys, status, main, capacities is None and not capturing)
     return outs, streams
+
+
+def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads):
+    """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream).
+    Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
+    H, W = int(s.image_height), int(s.image_width)
+    gbytes, ibytes, _ = _state_sizes(L, P, W, H)
+    geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+    img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
+    binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
+    radii = torch.empty((P,), dtype=torch.int32, device=dev)
+    bg, vm, pm, cp = (_prep(x, dev) for x in (s.bg, s.viewmatrix, s.projmatrix, s.campos))
+    if out_buffers is not None:
+        out_color = out_buffers[0][v]
+        out_feature = out_buffers[1][v] if (include_feature and F) else torch.zeros((1,), dtype=torch.float32, device=dev)
+        out_depth = out_buffers[2][v] if return_depth else None
+    else:
+        out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        out_feature = torch.empty((F, H, W), dtype=torch.float32, device=dev) if include_feature else \
+            torch.zeros((1,), dtype=torch.float32, device=dev)
+        out_depth = torch.empty((H, W), dtype=torch.float32, device=dev) if return_depth else None
+    w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
+    w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
+    w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
+    w.out_color, w.out_feature, w.out_depth, w.radii = _ptr(out_color), (_ptr(out_feature) if F else None), _ptr(out_depth), _ptr(radii)
+    if loss_heads is not None:
+        t_rgb, t_emb, c_rgb, c_emb, l_acc = loss_heads
+        w.target_color, w.cot_color, w.loss_acc = _ptr(t_rgb[v]), _ptr(c_rgb[v]), _ptr(l_acc[v])
+        if t_emb is not None and F:
+            w.target_feature, w.cot_feature = _ptr(t_emb[v]), _ptr(c_emb[v])
+    ret = (cap, out_color, out_feature, radii, geom, binb, img) + ((out_depth,) if return_depth else ())
+    return ViewOut(ret), (bg, vm, pm, cp)
+
+
+def _track_status(outs, keys, status, main, pending):
+    """Hands each ViewOut its pinned status pair and, when `pending`, queues the pair for the capacity table."""
+    ev = torch.cuda.Event()
+    ev.record(main)
+    for v, o in enumerate(outs):
+        o.status, o.event = status[v], ev
+        if pending:
+            _PENDING_STATUS.append((keys[v], status[v], ev, o[0]))
 
 
 def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_feature, means3D, colors, language_feature, scales,
@@ -653,25 +665,14 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         arr = (_b.View * V)()
         keep = []
         for v, s in enumerate(views):
-            o = outs[v]
-            H, W = int(s.image_height), int(s.image_width)
-            bg, vm, pm, cp = (_prep(x, dev) for x in (s.bg, s.viewmatrix, s.projmatrix, s.campos))
-            gc = _prep(grads_color[v], dev)
-            gf = _prep(grads_feature[v], dev) if (F and grads_feature is not None) else None
-            gd = _prep(grads_depth[v], dev) if grads_depth is not None else None
-            scratch = torch.empty((_state_sizes(L, P, W, H)[2],), dtype=torch.uint8, device=dev)
             w = arr[v]
-            w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
-            w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
-            w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = o[4].data_ptr(), o[5].data_ptr(), o[6].data_ptr(), int(o[0])
-            w.radii = _ptr(o[3])
-            w.dL_dpix, w.dL_dpix_F, w.dL_dpix_depth = _ptr(gc), _ptr(gf), _ptr(gd)
-            w.blend_scratch = scratch.data_ptr()
+            keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
+                                       grads_feature[v] if (F and grads_feature is not None) else None,
+                                       grads_depth[v] if grads_depth is not None else None))
             w.dL_dmean2D = _ptr(m2d) if shared else _ptr(m2d[v])
             w.stream = streams[v].cuda_stream
             if cot_scale is not None:
                 w.cot_scale = cot_scale.data_ptr() + 8 * v
-            keep.append((bg, vm, pm, cp, gc, gf, gd, scratch))
         for stages in ((1, 2) if after_blend is not None else (3,)):
             _b.check(L.mgs_backward_views(V, arr, P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors),
                                           _ptr(language_feature) if F else None, _ptr(scales), float(scale_modifier), _ptr(rotations),
@@ -683,3 +684,172 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
             if stages == 1:
                 after_blend()
     return (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
+
+
+def _backward_view(L, w, s, o, dev, P, grad_color, grad_feature, grad_depth):
+    """Fills the backward fields of mgs_view `w` from the view's forward result `o` (a ViewOut) and its pixel gradients
+    (the caller sets dL_dmean2D, stream and cot_scale).  Returns the tensors that must stay alive until the call is enqueued."""
+    H, W = int(s.image_height), int(s.image_width)
+    bg, vm, pm, cp = (_prep(x, dev) for x in (s.bg, s.viewmatrix, s.projmatrix, s.campos))
+    gc, gf, gd = (_prep(x, dev) for x in (grad_color, grad_feature, grad_depth))
+    scratch = torch.empty((_state_sizes(L, P, W, H)[2],), dtype=torch.uint8, device=dev)
+    w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
+    w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
+    w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = o[4].data_ptr(), o[5].data_ptr(), o[6].data_ptr(), int(o[0])
+    w.radii = _ptr(o[3])
+    w.dL_dpix, w.dL_dpix_F, w.dL_dpix_depth = _ptr(gc), _ptr(gf), _ptr(gd)
+    w.blend_scratch = scratch.data_ptr()
+    return (bg, vm, pm, cp, gc, gf, gd, scratch)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Several clouds in one call (DESIGN.md section 1, row f5): both frames of ManiGaussian's dynamic-field step, for every sample of
+# the batch.  One C call (mgs_forward_clouds / mgs_backward_clouds) enqueues the views of ALL clouds stage by stage on their
+# own streams between one fork and one join, so the clouds' chains overlap instead of queueing behind each other's blends.
+_CLOUD_TENSORS = ("means3D", "sh", "colors", "feature", "opacity", "scales", "rotations", "cov3D_precomp")
+
+
+def _nonempty(t):
+    return t is not None and t.numel() != 0
+
+
+def _prep_clouds(clouds, dev, include_feature):
+    """Per cloud: its tensors as float32 contiguous on `dev`, and P, F, M.  Raises ValueError naming the field on which the
+    clouds disagree (the C call shares the colour mode, the covariance mode, M and F between all clouds)."""
+    out = []
+    for b, c in enumerate(clouds):
+        d = {k: _prep(c.get(k), dev) for k in _CLOUD_TENSORS}
+        d["P"] = int(d["means3D"].size(0))
+        if d["P"] == 0:
+            raise ValueError(f"cloud {b} has no Gaussians (P = 0)")
+        d["F"] = int(d["feature"].size(1)) if (include_feature and _nonempty(d["feature"])) else 0
+        d["M"] = int(d["sh"].size(1)) if _nonempty(d["sh"]) else 0
+        out.append(d)
+    for field, key in (("colour mode (SHs or precomputed colours)", lambda d: _nonempty(d["colors"])),
+                       ("covariance mode (scales/rotations or cov3D_precomp)", lambda d: _nonempty(d["cov3D_precomp"])),
+                       ("SH degree (SH coefficients per Gaussian)", lambda d: d["M"]),
+                       ("feature width F", lambda d: d["F"])):
+        if len({key(d) for d in out}) > 1:
+            raise ValueError(f"clouds disagree on the {field}")
+    return out
+
+
+def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False):
+    """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
+    of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
+    (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
+    "capacities" as rasterize_views_raw takes them.  degree, F, the colour and covariance modes are shared.  Returns
+    (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
+    Capacity history is kept per (device, P, W, H, cloud slot, view slot)."""
+    L = _b.lib()
+    dev = clouds[0]["means3D"].device
+    if not clouds[0]["means3D"].is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    pc = _prep_clouds(clouds, dev, include_feature)
+    F, M, B = pc[0]["F"], pc[0]["M"], len(clouds)
+    offsets = [0]
+    for c in clouds:
+        offsets.append(offsets[-1] + len(c["views"]))
+    V = offsets[-1]
+    main = torch.cuda.current_stream(dev)
+    streams = _view_streams(dev, V) if V > 1 else [main]
+    di = dev.index if dev.index is not None else torch.cuda.current_device()
+    keys = [[(di, d["P"], int(s.image_width), int(s.image_height), b, v) for v, s in enumerate(c["views"])]
+            for b, (c, d) in enumerate(zip(clouds, pc))]
+    capturing = torch.cuda.is_current_stream_capturing()
+    with torch.cuda.device(dev):
+        if not capturing:
+            _poll_status()
+        for b, (c, d) in enumerate(zip(clouds, pc)):
+            if c.get("capacities") is None and any(k not in _CAPACITY for k in keys[b]):
+                if capturing:
+                    raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is "
+                                       "learned from an eager call) or pass `capacities`")
+                _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
+                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug)
+        arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
+        status = _status_slots(V)
+        keep, outs = [], []
+        for b, (c, d) in enumerate(zip(clouds, pc)):
+            k = carr[b]
+            k.P = d["P"]
+            k.means3D, k.shs, k.colors_precomp, k.opacities = _ptr(d["means3D"]), _ptr(d["sh"]), _ptr(d["colors"]), _ptr(d["opacity"])
+            k.feature = _ptr(d["feature"]) if F else None
+            k.scales, k.rotations, k.cov3D_precomp = _ptr(d["scales"]), _ptr(d["rotations"]), _ptr(d["cov3D_precomp"])
+            caps = c.get("capacities")
+            cloud_outs = []
+            for v, s in enumerate(c["views"]):
+                g = offsets[b] + v
+                cap = int(caps[v]) if caps is not None else _CAPACITY[keys[b][v]]
+                o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
+                                      c.get("loss_heads"))
+                arr[g].status = status.data_ptr() + 8 * g
+                arr[g].stream = streams[g].cuda_stream
+                keep.append(kp)
+                cloud_outs.append(o)
+            outs.append(cloud_outs)
+        _b.check(L.mgs_forward_clouds(B, carr, offs, arr, int(degree), M, F, float(scale_modifier), 0, int(bool(debug)),
+                                      main.cuda_stream), "mgs_forward_clouds")
+        flat = [o for co in outs for o in co]
+        pending = not capturing and all(c.get("capacities") is None for c in clouds)
+        _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
+    return outs, streams
+
+
+def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False):
+    """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
+    per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
+    plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W],
+    "cot_scale" [V_b,2] (device; the loss heads' upstream gradients) and "want_feature" (default True; False: the cloud's
+    dL_dfeature is not computed, but its feature cotangents still reach the other gradients).  Returns one dict per cloud
+    holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
+    dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed)."""
+    L = _b.lib()
+    dev = clouds[0]["means3D"].device
+    pc = _prep_clouds(clouds, dev, include_feature)
+    F, M, B = pc[0]["F"], pc[0]["M"], len(clouds)
+    offsets = [0]
+    for c in clouds:
+        offsets.append(offsets[-1] + len(c["views"]))
+    V = offsets[-1]
+    main = torch.cuda.current_stream(dev)
+    opts = dict(dtype=torch.float32, device=dev)
+    grads = []
+    with torch.cuda.device(dev):
+        arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
+        keep = []
+        for b, (c, d) in enumerate(zip(clouds, pc)):
+            P, Vb = d["P"], len(c["views"])
+            has_sr = _nonempty(d["scales"])
+            gr = dict(dL_dmeans3D=torch.empty((P, 3), **opts), dL_dmeans2D=torch.empty((Vb, P, 3), **opts),
+                      dL_dopacity=torch.empty((P, 1), **opts),
+                      dL_dscales=torch.empty((P, 3), **opts) if has_sr else None,
+                      dL_drotations=torch.empty((P, 4), **opts) if has_sr else None,
+                      dL_dsh=torch.empty((P, M, 3), **opts) if M else None,
+                      dL_dcolors=torch.empty((P, 3), **opts) if _nonempty(d["colors"]) else None,
+                      dL_dcov3D=torch.empty((P, 6), **opts) if _nonempty(d["cov3D_precomp"]) else None,
+                      dL_dfeature=torch.empty((P, F), **opts) if (F and c.get("want_feature", True)) else None)
+            grads.append(gr)
+            k = carr[b]
+            k.P = P
+            k.means3D, k.shs, k.colors_precomp = _ptr(d["means3D"]), _ptr(d["sh"]), _ptr(d["colors"])
+            k.feature = _ptr(d["feature"]) if F else None
+            k.scales, k.rotations, k.cov3D_precomp = _ptr(d["scales"]), _ptr(d["rotations"]), _ptr(d["cov3D_precomp"])
+            k.dL_dmean3D, k.dL_dopacity, k.dL_dcolor = _ptr(gr["dL_dmeans3D"]), _ptr(gr["dL_dopacity"]), _ptr(gr["dL_dcolors"])
+            k.dL_dfeature, k.dL_dcov3D, k.dL_dsh = _ptr(gr["dL_dfeature"]), _ptr(gr["dL_dcov3D"]), _ptr(gr["dL_dsh"])
+            k.dL_dscale, k.dL_drot = _ptr(gr["dL_dscales"]), _ptr(gr["dL_drotations"])
+            cot = _prep(c.get("cot_scale"), dev)
+            for v, s in enumerate(c["views"]):
+                g = offsets[b] + v
+                w = arr[g]
+                keep.append(_backward_view(L, w, s, outs[b][v], dev, P, c["grad_color"][v],
+                                           c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
+                                           c["grad_depth"][v] if c.get("grad_depth") is not None else None))
+                w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
+                w.stream = streams[g].cuda_stream
+                if cot is not None:
+                    w.cot_scale = cot.data_ptr() + 8 * v
+            keep.append(cot)
+        _b.check(L.mgs_backward_clouds(B, carr, offs, arr, int(degree), M, F, float(scale_modifier), 0, int(bool(debug)),
+                                       main.cuda_stream), "mgs_backward_clouds")
+    return grads
