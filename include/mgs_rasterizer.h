@@ -21,6 +21,7 @@
  *    F > 32 is blended in groups of 32 channels (each group walks the tile lists again, so the blend costs grow with
  *    ceil(F / 32));
  *  - an optional depth plane (out_depth / dL_dpix_depth) renders view-space z as one more blended channel;
+ *  - an optional alpha plane (mgs_view_alpha, multi-view and multi-cloud calls) returns the accumulated opacity 1 - final_T;
  *  - work is enqueued on `stream` (the reference uses the legacy default stream);
  *  - outputs are fully overwritten: callers need not zero-initialise them.
  *
@@ -305,6 +306,64 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
 int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
 	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
+/*
+ * Alpha plane (no reference counterpart): the pixel's accumulated opacity alpha = 1 - final_T, e.g. for a mask loss or for
+ * the expected depth out_depth / alpha (out_depth has no background term and falls to 0 where nothing covers the pixel).
+ * The four calls below are the multi-view and multi-cloud calls above with one more argument, `alpha`: one mgs_view_alpha
+ * per view (V entries, or view_offsets[B] for clouds), or NULL for none; the calls above are these with alpha == NULL.
+ * Forward: out_alpha [H,W] is fully overwritten.  Backward: dL_dpix_alpha [H,W] adds T_final / (1 - a_k) * dL_dalpha to
+ * every contributor's dL/da_k (cot_scale does not scale it); a pixel nothing blended into has no alpha gradient.
+ * Either pointer may be NULL per view.  mgs_view and mgs_cloud keep their layouts: existing arrays of them stay valid.
+ */
+typedef struct mgs_view_alpha {
+	float* out_alpha;            /* forward output [H,W] = 1 - final_T, or NULL */
+	const float* dL_dpix_alpha;  /* backward input [H,W], or NULL */
+} mgs_view_alpha;
+
+int mgs_forward_views_alpha(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_alpha(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */

@@ -27,6 +27,11 @@ class View(C.Structure):
                 ("cot_feature", C.c_void_p), ("loss_acc", C.c_void_p), ("cot_scale", C.c_void_p)]
 
 
+class ViewAlpha(C.Structure):
+    """mirror of `mgs_view_alpha` (include/mgs_rasterizer.h): the optional alpha plane of one view"""
+    _fields_ = [("out_alpha", C.c_void_p), ("dL_dpix_alpha", C.c_void_p)]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -93,6 +98,12 @@ def lib():
         getattr(L, name).argtypes = [i, C.POINTER(Cloud), C.POINTER(C.c_int), C.POINTER(View),  # B clouds view_offsets views
                                      i, i, i, f,                                                 # D M F scale_modifier
                                      i, i, vp]  # prefiltered (forward) or accumulate (backward), debug, join_stream
+    # the same four calls with the alpha planes (one ViewAlpha per view, or NULL) after the views
+    for name in ("mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds"):
+        at = list(getattr(L, name).argtypes)
+        k = 4 if "clouds" in name else 2
+        getattr(L, name + "_alpha").restype = C.c_int
+        getattr(L, name + "_alpha").argtypes = at[:k] + [C.POINTER(ViewAlpha)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_mark_visible.restype = C.c_int
@@ -123,6 +134,7 @@ EXPORTED_SYMBOLS = (
     "mgs_abi_version", "mgs_last_error", "mgs_geometry_state_bytes", "mgs_image_state_bytes",
     "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_forward", "mgs_forward_begin",
     "mgs_backward", "mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds", "mgs_loss_heads",
+    "mgs_forward_views_alpha", "mgs_backward_views_alpha", "mgs_forward_clouds_alpha", "mgs_backward_clouds_alpha",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

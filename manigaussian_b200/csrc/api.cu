@@ -432,14 +432,14 @@ static BlendArgs blend_args(const ViewState& s, const mgs_view& w, int F, const 
 	return ba;
 }
 
-// forward blend, with the fused loss heads when the view has a target
-static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, int debug)
+// forward blend, with the fused loss heads when the view has a target; out_alpha (nullable) receives 1 - final_T
+static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = (c.F > 0 && c.feature && w.out_feature) ? c.F : 0;
 	BlendArgs ba = blend_args(carve_view(w, c.P), w, F, c.feature);
 	ba.want_depth = w.out_depth != nullptr;
-	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth;
+	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth; ba.out_alpha = out_alpha;
 	// the cosine embedding head needs a pixel's whole feature vector: in the blend epilogue when one CTA holds it (F <= 32),
 	// else in a features-only pass of the loss-heads kernel over the planes the blend just wrote
 	const bool embed = w.target_color && w.target_feature && F > 0;
@@ -464,8 +464,8 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, int debug)
 
 // blend backward of one view on its stream: the view's blend-stage records, and the feature gradients summed with 128-bit
 // reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
-// and opacity gradients; only the feature rows are not reduced.
-static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, int debug)
+// and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane.
+static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, const float* dL_dalpha, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = c.F;
@@ -473,7 +473,7 @@ static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeatu
 	MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)c.P * GB_STRIDE * sizeof(float), st));
 	BlendArgs ba = blend_args(s, w, F, c.feature);
 	ba.want_depth = w.dL_dpix_depth != nullptr;
-	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth;
+	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth; ba.dL_dalpha = dL_dalpha;
 	ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
 	ba.cot_scale = w.cot_scale;
 	if (w.binning_capacity > 0) {
@@ -497,9 +497,9 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
-// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.
-static int backward_views(int V, const mgs_view* views, const Cloud& c, float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor,
-	float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
+// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha: V entries or NULL.
+static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const Cloud& c, float* dL_dmean3D,
+	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
 	const int P = c.P, F = c.F;
@@ -508,7 +508,7 @@ static int backward_views(int V, const mgs_view* views, const Cloud& c, float* d
 		int rc = fork_streams(V, views, join);
 		if (rc < 0) return rc;
 		for (int v = 0; v < V; v++) {
-			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, debug);
+			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -643,7 +643,7 @@ int mgs_forward(
 	w.binning_capacity = num_rendered;
 	rc = enqueue_binning(c, w, true, debug);
 	if (rc < 0) return rc;
-	rc = enqueue_blend_fwd(c, w, debug);
+	rc = enqueue_blend_fwd(c, w, nullptr, debug);
 	return rc < 0 ? rc : num_rendered;
 }
 
@@ -691,12 +691,23 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgs_forward_views(
 	int V, const mgs_view* views,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
+	return mgs_forward_views_alpha(V, views, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales,
+		scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_alpha(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha,
 	int P, int D, int M, int F,
 	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
@@ -732,7 +743,8 @@ int mgs_forward_views(
 		}
 		for (int v = 0; v < V; v++) {
 			rc = phase == 0 ? enqueue_project(c, views[v], debug)
-				: phase == 1 ? enqueue_binning(c, views[v], false, debug) : enqueue_blend_fwd(c, views[v], debug);
+				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
+				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -741,6 +753,19 @@ int mgs_forward_views(
 
 int mgs_backward_views(
 	int V, const mgs_view* views,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
+	return mgs_backward_views_alpha(V, views, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier,
+		rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D,
+		accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_alpha(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha,
 	int P, int D, int M, int F,
 	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
 	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
@@ -758,12 +783,18 @@ int mgs_backward_views(
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp };
-	return backward_views(V, views, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
 int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
 	float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
+	return mgs_forward_clouds_alpha(B, clouds, view_offsets, views, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
+	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
 	(void)prefiltered;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -790,7 +821,8 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 				rc = phase == 0 ? enqueue_project(c, views[v], debug)
-					: phase == 1 ? enqueue_binning(c, views[v], false, debug) : enqueue_blend_fwd(c, views[v], debug);
+					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
+					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, debug);
 				if (rc < 0) return rc;
 			}
 		}
@@ -800,6 +832,12 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 
 int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
 	float scale_modifier, int accumulate, int debug, void* join_stream)
+{
+	return mgs_backward_clouds_alpha(B, clouds, view_offsets, views, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
+	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -827,7 +865,7 @@ int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets,
 	for (int b = 0; b < B; b++) {
 		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, debug);
+			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}

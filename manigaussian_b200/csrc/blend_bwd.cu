@@ -4,7 +4,9 @@
 // C-ABI.  Same mathematics (SURVEY.md A.4): walking a pixel's contributors back to front,
 //   T_k     = T_{k+1} / (1 - a_k)                      (T recovered by division from final_T, :521)
 //   dL/dc_k = a_k T_k g                                 (g = dL/dpixel, all channels)
-//   dL/da_k = T_k (c_k . g) - (S_k + T_final (bg . g_rgb)) / (1 - a_k),   S_k = sum_{j behind k} a_j T_j (c_j . g)
+//   dL/da_k = T_k (c_k . g) - (S_k + T_final (bg . g_rgb - h)) / (1 - a_k),   S_k = sum_{j behind k} a_j T_j (c_j . g)
+//           (h = dL/dalpha of the optional alpha plane 1 - T_final, whose derivative T_final / (1 - a_k) has the background
+//           term's form)
 //   dL/dG   = o_k dL/da_k  (the 0.99 clamp is gradient-transparent, :574), then mean2D / conic / opacity.
 // S_k is the scalar form of the reference's per-channel `accum_rec` recursion.
 //
@@ -132,6 +134,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	float T = 0.f, bgterm = 0.f;
 	if (walker) {
 		float g4[4] = { 0.f, 0.f, 0.f, 0.f };
+		float h = 0.f;  // alpha cotangent: d alpha / d a_k = T_final / (1 - a_k), the background term's form, with -h for bg . g
 		// upstream gradients of the fused loss heads (loss_heads.cuh): the cotangent planes were written for d loss = 1
 		const float sc_color = a.cot_scale ? a.cot_scale[0] : 1.f, sc_feat = a.cot_scale ? a.cot_scale[1] : 1.f;
 		if (inside) {
@@ -139,8 +142,9 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 #pragma unroll
 			for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
 			if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
+			if (a.dL_dalpha) h = a.dL_dalpha[pix];
 		}
-		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2]);
+		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
 #pragma unroll
 		for (int c = 0; c < 4; c++) { grow[2 * (RGBD + c)] = g4[c]; grow[2 * (RGBD + 4 + c)] = 0.f; }
@@ -606,6 +610,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 	float T = 0.f, bgterm = 0.f;
 	{
 		float g4[4] = { 0.f, 0.f, 0.f, 0.f };  // zero in groups >= 1: no colour / depth gradient, no background term
+		float h = 0.f;                         // alpha cotangent (group 0 only), enters the background term as in blend_bwd_kernel
 		// upstream gradients of the fused loss heads (loss_heads.cuh): the cotangent planes were written for d loss = 1
 		const float sc_color = a.cot_scale ? a.cot_scale[0] : 1.f, sc_feat = a.cot_scale ? a.cot_scale[1] : 1.f;
 		if (inside) {
@@ -614,9 +619,10 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 #pragma unroll
 				for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
 				if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
+				if (a.dL_dalpha) h = a.dL_dalpha[pix];
 			}
 		}
-		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2]);
+		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
 #pragma unroll
 		for (int c = 0; c < 4; c++) { grow[2 * (RGBD + c)] = g4[c]; grow[2 * (RGBD + 4 + c)] = 0.f; }

@@ -228,6 +228,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			const size_t pix = (size_t)a.W * pyi + pxi;
 			a.final_T[pix] = T;
 			a.n_contrib[pix] = last ? lrow[last - 1] + 1u : 0u;  // 1-based tile-list position, as the reference counts
+			if (a.out_alpha) a.out_alpha[pix] = 1.f - T;
 		}
 	}
 	if (first) {

@@ -116,10 +116,12 @@ struct BlendArgs {
 	float* out_color;            // [3,H,W]
 	float* out_feature;          // [F,H,W]
 	float* out_depth;            // [H,W] nullable
+	float* out_alpha;            // [H,W] nullable: accumulated opacity 1 - final_T
 	// backward only
 	const float* dL_dcolor;      // [3,H,W]
 	const float* dL_dfeature;    // [F,H,W] nullable
 	const float* dL_ddepth;      // [H,W] nullable
+	const float* dL_dalpha;      // [H,W] nullable: cotangent of out_alpha, enters the background term only
 	float* gb;                   // [P,GB_STRIDE] (zeroed by caller)
 	float* dL_dfeat;             // [P,F] (zeroed by caller) nullable
 	// fused loss heads (loss_heads.cuh), all nullable.  Forward: with tgt_color the epilogue also writes the cotangent planes

@@ -72,9 +72,10 @@ def _camera_scalars(nv, idx):
 
 
 def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=None, features_color=None,
-           features_language=None, return_depth=False):
+           features_language=None, return_depth=False, return_alpha=False):
     """Render view `idx` of data['novel_view'].  Same arguments and result as the reference's render(); with
-    return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended)."""
+    return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended, no background term), with
+    return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth)."""
     device = pts_xyz.device
     nv = data["novel_view"]
     bg = _background(bg_color, device)
@@ -90,7 +91,7 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
         viewmatrix=nv["world_view_transform"][idx], projmatrix=nv["full_proj_transform"][idx],
         sh_degree=3 if features_color is None else 1, campos=nv["camera_center"][idx], prefiltered=False, debug=False,
         include_feature=(features_language is not None))
-    rasterizer = GaussianRasterizer(raster_settings=raster_settings, return_depth=return_depth)
+    rasterizer = GaussianRasterizer(raster_settings=raster_settings, return_depth=return_depth, return_alpha=return_alpha)
     shs, colors_precomp = None, None
     if features_color is not None:
         shs = features_color
@@ -103,12 +104,15 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
     ret = {"render": out[0], "render_embed": out[1], "viewspace_points": screenspace_points, "radii": out[2]}
     if return_depth:
         ret["depth"] = out[3]
+    if return_alpha:
+        ret["alpha"] = out[-1]
     return ret
 
 
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, group):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
+                group):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -122,27 +126,30 @@ class _RasterizeViews(torch.autograd.Function):
         color = torch.empty((V, 3, H, W), **opts)
         feat_img = torch.empty((V, F, H, W), **opts) if include else None
         depth = torch.empty((V, H, W), **opts) if return_depth else None
+        alpha = torch.empty((V, H, W), **opts) if return_alpha else None
         degree = views[0].sh_degree
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
-                                            debug=views[0].debug, out_buffers=(color, feat_img, depth))
+                                            debug=views[0].debug, out_buffers=(color, feat_img, depth, alpha),
+                                            return_alpha=return_alpha)
         main = torch.cuda.current_stream(dev)
         for st in streams:
             main.wait_stream(st)
         radii = torch.stack([o[3] for o in outs])
         ctx.views, ctx.streams, ctx.group = views, streams, group
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
-        ctx.include, ctx.F, ctx.return_depth, ctx.degree = include, F, return_depth, degree
+        ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
         ctx.save_for_backward(means3D, sh if sh is not None else torch.empty(0, device=dev),
                               colors_precomp if colors_precomp is not None else torch.empty(0, device=dev),
                               feature if include else torch.empty(0, device=dev), scales, rotations)
         ctx.mark_non_differentiable(radii)
         empty = torch.empty(0, device=dev)
-        return color, (feat_img if include else empty), radii, (depth if return_depth else empty)
+        return (color, (feat_img if include else empty), radii, (depth if return_depth else empty),
+                (alpha if return_alpha else empty))
 
     @staticmethod
-    def backward(ctx, g_color, g_feat, _g_radii, g_depth):
+    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha):
         means3D, sh, colors_precomp, feature, scales, rotations = ctx.saved_tensors
         dev = means3D.device
         views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
@@ -156,6 +163,7 @@ class _RasterizeViews(torch.autograd.Function):
         g_color = _prep(g_color, dev)
         g_feat = _prep(g_feat, dev) if ctx.include else None
         g_depth = _prep(g_depth, dev) if (ctx.return_depth and g_depth is not None and g_depth.numel()) else None
+        g_alpha = _prep(g_alpha, dev) if (ctx.return_alpha and g_alpha is not None and g_alpha.numel()) else None
         pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)  # every row is written by the backward
         grp = None if ctx.group in (None, True) else ctx.group
         m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
@@ -163,7 +171,7 @@ class _RasterizeViews(torch.autograd.Function):
         rasterize_views_backward_raw(views, outs, ctx.streams, g_color, g_feat, means3D, colors_precomp if use_colors else None,
                                      feature if ctx.include else None, scales, rotations, views[0].scale_modifier, None,
                                      sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
-                                     accumulate_into=pk.views, means2D_per_view=m2d,
+                                     accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
                                      after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
@@ -172,7 +180,7 @@ class _RasterizeViews(torch.autograd.Function):
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None)
 
 
 class _RasterizeViewsLoss(torch.autograd.Function):
@@ -254,7 +262,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
-                 targets=None):
+                 targets=None, return_alpha=False):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -266,8 +274,10 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     epilogue: the result then also holds "loss_rgb" and "loss_embed" ([V] each: l2_loss and cosine_loss of
     agents/manigaussian_bc/loss.py per view; combine them as neural_rendering.py:300-318 does) through which -- and only
     through which -- gradients flow; "render"/"render_embed" are returned detached.
-    Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "viewspace_points" [V,P,3]
-    (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
+    return_alpha: also return "alpha" [V,H,W], the accumulated opacity 1 - final_T (differentiable; depth / alpha is the
+    expected depth).
+    Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
+    "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
     include = features_language is not None
     sh_degree = 3 if features_color is None else 1
@@ -289,6 +299,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
+        if return_alpha:
+            raise ValueError("targets and return_alpha cannot be combined")
         loss_rgb, loss_embed, color, feat_img, radii = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
             rotations, views, targets["rgb"], targets.get("embed"), sync_gradients)
@@ -296,20 +308,23 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
                 "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
     if V == 1 and sync_gradients is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
-        out = GaussianRasterizer(views[0], return_depth=return_depth)(
+        out = GaussianRasterizer(views[0], return_depth=return_depth, return_alpha=return_alpha)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
             colors_precomp=pts_rgb if features_color is None else None, language_feature_precomp=feat, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=None)
         color, feat_img, radii = out[0].unsqueeze(0), out[1].unsqueeze(0), out[2].unsqueeze(0)
         depth = out[3].unsqueeze(0) if return_depth else None
+        alpha = out[-1].unsqueeze(0) if return_alpha else None
     else:
-        color, feat_img, radii, depth = _RasterizeViews.apply(
+        color, feat_img, radii, depth, alpha = _RasterizeViews.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, bool(return_depth), sync_gradients)
+            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
         ret["depth"] = depth
+    if return_alpha:
+        ret["alpha"] = alpha
     return ret
 
 
@@ -317,13 +332,13 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 
 class _RasterizeClouds(torch.autograd.Function):
-    """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None).  Outputs per cloud: (color,
-    feature image, radii, depth), or with targets (loss_rgb, loss_embed, color, feature image, radii) with gradients through
+    """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha).  Outputs per
+    cloud: (color, feature image, radii, depth, alpha), or with targets (loss_rgb, loss_embed, color, feature image, radii) with gradients through
     the two losses only."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets = meta
+        cloud_views, return_depth, targets, return_alpha = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
         clouds, results, frozen, cots = [], [], [], []
@@ -334,8 +349,9 @@ class _RasterizeClouds(torch.autograd.Function):
             color = torch.empty((V, 3, H, W), **opts)
             feat_img = torch.empty((V, F, H, W), **opts) if F else None
             depth = torch.empty((V, H, W), **opts) if return_depth else None
+            alpha = torch.empty((V, H, W), **opts) if return_alpha else None
             c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, opacity=opacities, scales=scales,
-                     rotations=rotations, out_buffers=(color, feat_img, depth))
+                     rotations=rotations, out_buffers=(color, feat_img, depth, alpha))
             if targets is not None:
                 t_rgb = _prep(targets[b]["rgb"], dev)
                 t_emb = _prep(targets[b].get("embed"), dev) if F else None
@@ -350,9 +366,9 @@ class _RasterizeClouds(torch.autograd.Function):
         degree = cloud_views[0][0].sh_degree
         include = clouds[0]["feature"] is not None
         outs, streams = rasterize_clouds_raw(clouds, degree, include, cloud_views[0][0].scale_modifier, return_depth=return_depth,
-                                             debug=cloud_views[0][0].debug)
+                                             debug=cloud_views[0][0].debug, return_alpha=return_alpha)
         for b, c in enumerate(clouds):
-            color, feat_img, depth = c["out_buffers"]
+            color, feat_img, depth, alpha = c["out_buffers"]
             radii = torch.stack([o[3] for o in outs[b]])
             empty = lambda: torch.empty(0, device=dev)
             if targets is not None:
@@ -363,7 +379,8 @@ class _RasterizeClouds(torch.autograd.Function):
                 results += [loss_rgb, loss_embed, color, feat_img if feat_img is not None else empty(), radii]
                 frozen += [radii, color] + ([feat_img] if feat_img is not None else [])
             else:
-                results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty()]
+                results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty(),
+                            alpha if alpha is not None else empty()]
                 frozen.append(radii)
         ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots = meta, streams, degree, include, cots
         # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
@@ -377,10 +394,10 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets = ctx.meta
+        cloud_views, return_depth, targets, return_alpha = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
-        per = 5 if targets is not None else 4
+        per = 5
         clouds = []
         for b, views in enumerate(cloud_views):
             means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
@@ -399,6 +416,8 @@ class _RasterizeClouds(torch.autograd.Function):
                     c["grad_feature"] = g[1] if g[1] is not None else torch.zeros((V, F, H, W), dtype=torch.float32, device=dev)
                 if return_depth and g[3] is not None:
                     c["grad_depth"] = g[3]
+                if return_alpha and g[4] is not None:
+                    c["grad_alpha"] = g[4]
             clouds.append(c)
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
@@ -413,7 +432,7 @@ class _RasterizeClouds(torch.autograd.Function):
         return tuple(ret)
 
 
-def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True):
+def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False):
     """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
     next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
 
@@ -421,7 +440,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     "rotations", "scales", "opacity", "features_color" or "pts_rgb", optional "features_language" and optional "targets".
     The clouds share the SH degree, the feature width F and the colour mode (ValueError naming the field otherwise); within a
     cloud all views share one image size, different clouds may differ.  Targets are given on all clouds or on none.
-    Returns one dict per cloud with the keys and shapes render_views returns for it ("loss_rgb" / "loss_embed" with targets).
+    Returns one dict per cloud with the keys and shapes render_views returns for it ("loss_rgb" / "loss_embed" with targets,
+    "depth" / "alpha" [V,H,W] when asked for).
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
     dyna step, which renders the detached current features); its feature cotangents still reach its other gradients."""
     if not clouds:
@@ -431,6 +451,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         raise ValueError("targets must be given on all clouds or on none")
     if all(with_targets) and return_depth:
         raise ValueError("targets and return_depth cannot be combined")
+    if all(with_targets) and return_alpha:
+        raise ValueError("targets and return_alpha cannot be combined")
     if len({c.get("features_color") is None for c in clouds}) > 1:
         raise ValueError("clouds disagree on the colour mode (SHs or precomputed colors)")
     device = clouds[0]["pts_xyz"].device
@@ -465,7 +487,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         flat += [c["pts_xyz"], vsps[-1], c.get("features_color"), c.get("pts_rgb") if c.get("features_color") is None else None, f,
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
-    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets), *flat)
+    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha)), *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]
@@ -474,9 +496,11 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
             ret.append({"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii,
                         "loss_rgb": loss_rgb, "loss_embed": loss_embed})
         else:
-            color, feat_img, radii, depth = out[4 * b:4 * b + 4]
+            color, feat_img, radii, depth, alpha = out[5 * b:5 * b + 5]
             r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii}
             if return_depth:
                 r["depth"] = depth
+            if return_alpha:
+                r["alpha"] = alpha
             ret.append(r)
     return ret

@@ -9,8 +9,8 @@ device memory, streams and autograd plumbing only; all computation happens in th
 include/mgs_rasterizer.h.
 
 Supersets of the reference: the feature width F is read from the tensor at run time (0..512) instead of being
-compiled in (config.h:16; widths above 32 blend in groups of 32 channels), and `return_depth=True` adds a view-space
-depth plane.
+compiled in (config.h:16; widths above 32 blend in groups of 32 channels), `return_depth=True` adds a view-space
+depth plane, and `return_alpha=True` adds the accumulated-opacity plane 1 - final_T.
 """
 from typing import NamedTuple
 
@@ -257,21 +257,38 @@ def cpu_deep_copy_tuple(input_tuple):
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings, return_depth=False):
+                        cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp, raster_settings, return_depth)
+                                     rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, return_depth=False):
+                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
         s = raster_settings
         args = (s.bg, means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations, s.scale_modifier,
                 cov3Ds_precomp, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.image_height, s.image_width, sh,
                 s.sh_degree, s.campos, s.prefiltered, s.debug, s.include_feature)
         ctx.async_view = None
-        if s.debug:
+        views_path = means3D.is_cuda and means3D.size(0) > 0
+        alpha = None
+        if return_alpha and views_path:
+            # the alpha plane exists on the multi-view entry points only: debug renders take them too, with the snapshot dump
+            cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
+            try:
+                outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
+                                                    rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
+                                                    return_depth=return_depth, debug=s.debug, return_alpha=True)
+            except Exception as ex:
+                if s.debug:
+                    torch.save(cpu_args, "snapshot_fw.dump")
+                    print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
+                raise ex
+            out = outs[0]
+            alpha = out[-1]
+            ctx.async_view = (int(out[0]), streams)  # as below: never the outputs themselves
+        elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
             try:
                 out = rasterize_gaussians_raw(*args, return_depth=return_depth)
@@ -292,20 +309,24 @@ class _RasterizeGaussians(torch.autograd.Function):
             ctx.async_view = (int(out[0]), streams)
         else:
             out = rasterize_gaussians_raw(*args, return_depth=return_depth)
+            if return_alpha:  # no Gaussians: nothing covers any pixel
+                alpha = torch.zeros((int(s.image_height), int(s.image_width)), dtype=torch.float32, device=out[1].device)
         num_rendered, color, language_feature, radii, geomBuffer, binningBuffer, imgBuffer = out[:7]
         depth = out[7] if return_depth else None
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.return_depth = return_depth
+        ctx.return_alpha = return_alpha
         ctx.save_for_backward(colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii,
                               sh, geomBuffer, binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
-        if return_depth:
-            return color, language_feature, radii, depth
-        return color, language_feature, radii
+        return (color, language_feature, radii) + ((depth,) if return_depth else ()) + ((alpha,) if return_alpha else ())
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_out_language_feature, _radii=None, grad_out_depth=None):
+    def backward(ctx, grad_out_color, grad_out_language_feature, _radii=None, *grad_planes):
+        # grad_planes: the depth gradient when return_depth, then the alpha gradient when return_alpha
+        grad_out_depth = grad_planes[0] if ctx.return_depth else None
+        grad_out_alpha = grad_planes[-1] if ctx.return_alpha else None
         s = ctx.raster_settings
         (colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
          binningBuffer, imgBuffer) = ctx.saved_tensors
@@ -322,10 +343,18 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.async_view is not None:
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
-            grads = rasterize_views_backward_raw(
-                [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
-                colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
-                s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None)
+            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and ctx.return_alpha) else None
+            try:
+                grads = rasterize_views_backward_raw(
+                    [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
+                    colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
+                    s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None, debug=s.debug,
+                    grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None)
+            except Exception as ex:
+                if cpu_args is not None:
+                    torch.save(cpu_args, "snapshot_bw.dump")
+                    print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
+                raise ex
         elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)
             try:
@@ -345,7 +374,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, _or_none(grad_sh, sh), _or_none(grad_colors_precomp, colors_precomp),
                 _or_none(grad_language_feature_precomp, language_feature_precomp) if s.include_feature else None,
                 grad_opacities, _or_none(grad_scales, scales), _or_none(grad_rotations, rotations),
-                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None)
+                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None)
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -365,10 +394,13 @@ class GaussianRasterizationSettings(NamedTuple):
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, return_depth=False):
+    def __init__(self, raster_settings, return_depth=False, return_alpha=False):
+        """return_depth / return_alpha: forward() also returns the depth plane [H,W] and / or the alpha plane [H,W]
+        (accumulated opacity 1 - final_T), in that order after radii."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_depth = return_depth
+        self.return_alpha = return_alpha
 
     def markVisible(self, positions):
         # Mark visible points (based on frustum culling for camera) with a boolean
@@ -391,7 +423,7 @@ class GaussianRasterizer(nn.Module):
         rotations = empty if rotations is None else rotations
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, language_feature_precomp, opacities, scales,
-                                   rotations, cov3D_precomp, self.raster_settings, self.return_depth)
+                                   rotations, cov3D_precomp, self.raster_settings, self.return_depth, self.return_alpha)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -521,12 +553,13 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None):
+                        loss_heads=None, return_alpha=False):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
-    `out_buffers` = (color [V,3,H,W], feature [V,F,H,W] or None, depth [V,H,W] or None): render straight into slices of
-    caller-owned batch tensors instead of per-view allocations.  `capacities` (per-view instance capacities) overrides
+    `out_buffers` = (color [V,3,H,W], feature [V,F,H,W] or None, depth [V,H,W] or None[, alpha [V,H,W] or None]): render
+    straight into slices of caller-owned batch tensors instead of per-view allocations.  `return_alpha` appends the alpha
+    plane 1 - final_T [H,W] to every ViewOut (after depth, when that is asked for too).  `capacities` (per-view instance capacities) overrides
     the history-based sizing of the binning state.  `loss_heads` = (target_rgb [V,3,H,W], target_embed [V,F,H,W] or None,
     cot_rgb [V,3,H,W], cot_embed [V,F,H,W] or None, loss_acc [V,2]): the forward blend's epilogue also evaluates the L2 colour
     head and the cosine embedding head against the targets (C ABI mgs_view.target_*), leaving the loss sums in loss_acc and
@@ -558,25 +591,31 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                        debug)
         arr = (_b.View * V)()
+        aarr = (_b.ViewAlpha * V)() if return_alpha else None
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
-            o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads)
+            o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
+                                 aarr[v] if return_alpha else None)
             arr[v].status = status.data_ptr() + 8 * v
             arr[v].stream = streams[v].cuda_stream
             keep.append(k)
             outs.append(o)
-        _b.check(L.mgs_forward_views(V, arr, P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors),
-                                     _ptr(language_feature) if F else None, _ptr(opacity), _ptr(scales), float(scale_modifier),
-                                     _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream), "mgs_forward_views")
+        rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
+                _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
+        if return_alpha:
+            _b.check(L.mgs_forward_views_alpha(V, arr, aarr, *rest), "mgs_forward_views_alpha")
+        else:
+            _b.check(L.mgs_forward_views(V, arr, *rest), "mgs_forward_views")
         _track_status(outs, keys, status, main, capacities is None and not capturing)
     return outs, streams
 
 
-def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads):
-    """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream).
-    Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
+def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None):
+    """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream) and, when
+    `wa` (its mgs_view_alpha) is given, its alpha plane.  Returns the ViewOut and the tensors that must stay alive until the
+    call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
     gbytes, ibytes, _ = _state_sizes(L, P, W, H)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
@@ -593,6 +632,11 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
         out_feature = torch.empty((F, H, W), dtype=torch.float32, device=dev) if include_feature else \
             torch.zeros((1,), dtype=torch.float32, device=dev)
         out_depth = torch.empty((H, W), dtype=torch.float32, device=dev) if return_depth else None
+    out_alpha = None
+    if wa is not None:
+        ob = out_buffers[3] if (out_buffers is not None and len(out_buffers) > 3) else None
+        out_alpha = ob[v] if ob is not None else torch.empty((H, W), dtype=torch.float32, device=dev)
+        wa.out_alpha = _ptr(out_alpha)
     w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
     w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
     w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
@@ -603,6 +647,7 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
         if t_emb is not None and F:
             w.target_feature, w.cot_feature = _ptr(t_emb[v]), _ptr(c_emb[v])
     ret = (cap, out_color, out_feature, radii, geom, binb, img) + ((out_depth,) if return_depth else ())
+    ret += (out_alpha,) if wa is not None else ()
     return ViewOut(ret), (bg, vm, pm, cp)
 
 
@@ -619,7 +664,7 @@ def _track_status(outs, keys, status, main, pending):
 def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_feature, means3D, colors, language_feature, scales,
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
-                                 cot_scale=None):
+                                 cot_scale=None, grads_alpha=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -628,7 +673,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     accumulate=True.  `after_blend()` is called between the blend stage and the per-Gaussian stage, when dL_dfeature is final
     (multi-GPU: start its all-reduce there; it overlaps the per-Gaussian kernel).  `cot_scale` [V,2] (device): upstream
     gradients of the fused loss heads' two scalars per view, multiplied onto the colour / feature cotangent planes as they
-    are loaded.  The caller's current stream holds the result on return."""
+    are loaded.  `grads_alpha` (per view [H,W] or None): cotangents of the alpha planes of a `return_alpha` forward.  The
+    caller's current stream holds the result on return."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -663,9 +709,14 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     m2d = out("dL_dmeans2D", (P, 3)) if shared else means2D_per_view
     with torch.cuda.device(dev):
         arr = (_b.View * V)()
+        aarr = (_b.ViewAlpha * V)() if grads_alpha is not None else None
         keep = []
         for v, s in enumerate(views):
             w = arr[v]
+            if aarr is not None:
+                ga = _prep(grads_alpha[v], dev)
+                aarr[v].dL_dpix_alpha = _ptr(ga)
+                keep.append(ga)
             keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
                                        grads_feature[v] if (F and grads_feature is not None) else None,
                                        grads_depth[v] if grads_depth is not None else None))
@@ -674,13 +725,15 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
             if cot_scale is not None:
                 w.cot_scale = cot_scale.data_ptr() + 8 * v
         for stages in ((1, 2) if after_blend is not None else (3,)):
-            _b.check(L.mgs_backward_views(V, arr, P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors),
-                                          _ptr(language_feature) if F else None, _ptr(scales), float(scale_modifier), _ptr(rotations),
-                                          _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity), _ptr(dL_dcolors),
-                                          _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
-                                          _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
-                                          int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream),
-                     "mgs_backward_views")
+            rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
+                    _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
+                    _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
+                    _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
+                    int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
+            if aarr is not None:
+                _b.check(L.mgs_backward_views_alpha(V, arr, aarr, *rest), "mgs_backward_views_alpha")
+            else:
+                _b.check(L.mgs_backward_views(V, arr, *rest), "mgs_backward_views")
             if stages == 1:
                 after_blend()
     return (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
@@ -734,11 +787,12 @@ def _prep_clouds(clouds, dev, include_feature):
     return out
 
 
-def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False):
+def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
-    "capacities" as rasterize_views_raw takes them.  degree, F, the colour and covariance modes are shared.  Returns
+    "capacities" as rasterize_views_raw takes them.  degree, F, the colour and covariance modes are shared.  `return_alpha`
+    appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
     Capacity history is kept per (device, P, W, H, cloud slot, view slot)."""
     L = _b.lib()
@@ -768,6 +822,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
                            d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug)
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
+        aarr = (_b.ViewAlpha * V)() if return_alpha else None
         status = _status_slots(V)
         keep, outs = [], []
         for b, (c, d) in enumerate(zip(clouds, pc)):
@@ -782,14 +837,17 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 g = offsets[b] + v
                 cap = int(caps[v]) if caps is not None else _CAPACITY[keys[b][v]]
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
-                                      c.get("loss_heads"))
+                                      c.get("loss_heads"), aarr[g] if return_alpha else None)
                 arr[g].status = status.data_ptr() + 8 * g
                 arr[g].stream = streams[g].cuda_stream
                 keep.append(kp)
                 cloud_outs.append(o)
             outs.append(cloud_outs)
-        _b.check(L.mgs_forward_clouds(B, carr, offs, arr, int(degree), M, F, float(scale_modifier), 0, int(bool(debug)),
-                                      main.cuda_stream), "mgs_forward_clouds")
+        rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
+        if return_alpha:
+            _b.check(L.mgs_forward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_forward_clouds_alpha")
+        else:
+            _b.check(L.mgs_forward_clouds(B, carr, offs, arr, *rest), "mgs_forward_clouds")
         flat = [o for co in outs for o in co]
         pending = not capturing and all(c.get("capacities") is None for c in clouds)
         _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
@@ -799,7 +857,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
 def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
-    plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W],
+    plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
+    "grad_alpha" [V_b,H,W] (the cotangent of a `return_alpha` forward's alpha planes),
     "cot_scale" [V_b,2] (device; the loss heads' upstream gradients) and "want_feature" (default True; False: the cloud's
     dL_dfeature is not computed, but its feature cotangents still reach the other gradients).  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
@@ -817,6 +876,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     grads = []
     with torch.cuda.device(dev):
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
+        aarr = (_b.ViewAlpha * V)() if any(c.get("grad_alpha") is not None for c in clouds) else None
         keep = []
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
@@ -847,9 +907,16 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                                            c["grad_depth"][v] if c.get("grad_depth") is not None else None))
                 w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
                 w.stream = streams[g].cuda_stream
+                if c.get("grad_alpha") is not None:
+                    ga = _prep(c["grad_alpha"][v], dev)
+                    aarr[g].dL_dpix_alpha = _ptr(ga)
+                    keep.append(ga)
                 if cot is not None:
                     w.cot_scale = cot.data_ptr() + 8 * v
             keep.append(cot)
-        _b.check(L.mgs_backward_clouds(B, carr, offs, arr, int(degree), M, F, float(scale_modifier), 0, int(bool(debug)),
-                                       main.cuda_stream), "mgs_backward_clouds")
+        rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
+        if aarr is not None:
+            _b.check(L.mgs_backward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_backward_clouds_alpha")
+        else:
+            _b.check(L.mgs_backward_clouds(B, carr, offs, arr, *rest), "mgs_backward_clouds")
     return grads
