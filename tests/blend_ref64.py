@@ -1,0 +1,347 @@
+"""Float64 reference of the blend stage (forward and backward), with its contribution decisions as an input.
+
+The reference takes a view's projected and sorted state as given (tile `ranges`, `point_list`, `means2D`, `conic_opacity`,
+colours, depth, features) and re-does only the blend:
+
+* `decide` evaluates the reference's rule in float64 for every (tile-list entry, pixel of the tile): `power <= 0`,
+  `alpha = min(0.99, o G) >= 1/255`, stop when `T (1 - alpha) < 1e-4`.  A decision that lies inside the band the fp32
+  evaluation can move (a few ulp of the quadratic's terms, of `expf` and of the running product) is *borderline*; a pixel's
+  decisions after its first borderline one are unknown.  `decide_fp32` restates the C oracle's fp32 decisions instead.
+* `blend` computes, from a given set of contributor masks, the images (colour, features, depth, final_T, alpha, n_contrib)
+  and the blend-stage gradients in the reference's conventions (the 0.99 clamp is gradient-transparent; dL_dmeans2D carries
+  the 0.5 W / 0.5 H factors; dL_dconic.y is the reference's half-weight off-diagonal term), each with a per-element bound
+  from a first-order model of the reference's fp32 arithmetic.  The bounds are in units of u = 2^-24; a checked value is
+  within bound when |value - ref| <= KAPPA u B + tiny.
+
+Per tile everything is a (256 pixels x L entries) array: transmittances come from cumulative products, the suffix sums of
+the backward from reversed cumulative sums.
+"""
+import numpy as np
+
+ALPHA_MAX = np.float64(np.float32(0.99))
+ALPHA_MIN = np.float64(np.float32(1.0) / np.float32(255.0))
+T_STOP = np.float64(np.float32(0.0001))
+U = 2.0 ** -24
+# Bound scale per checked quantity: 4x the largest |x - ref| / (u B) measured for that quantity over the C oracle and the
+# stored outputs of the compiled reference on the four golden scenes (tests/test_blend_ref64_cpu.py) and both blend
+# kernels on every scene of tests/test_blend_pairs_gpu.py (H100 SXM).  The measured ratios are in those tests' docstrings.
+KAPPA = dict(color=14.5, feature=24.0, depth=11.1, final_T=7.1, alpha=2.0,
+             dL_dmeans2D=0.23, dL_dconic=0.012, dL_dopacity=0.7, dL_dcolors=1.6, dL_dfeature=5.3, dL_dcov3D=0.035)
+
+
+def tile_pixels(W, H, tile):
+    """Pixel coordinates of a 16x16 tile in (ly, lx) order, and which of them lie inside the image."""
+    gx = (W + 15) // 16
+    tx, ty = tile % gx, tile // gx
+    ly, lx = np.divmod(np.arange(256), 16)
+    px, py = tx * 16 + lx, ty * 16 + ly
+    return px, py, (px < W) & (py < H)
+
+
+def pixel_block_bit(lx, ly):
+    """(8x4 block of the tile, bit of the pixel in that block's 32-bit mask) for tile-local pixel coordinates."""
+    s = (ly // 4) * 2 + lx // 8
+    return s, (lx % 8) * 4 + ly % 4
+
+
+def _pairs(st, tile):
+    r0, r1 = (int(v) for v in st["ranges"][tile])
+    ids = st["point_list"][r0:r1].astype(np.int64)
+    px, py, inside = tile_pixels(st["W"], st["H"], tile)
+    m = st["means2D"][ids].astype(np.float64)
+    co = st["conic_opacity"][ids].astype(np.float64)
+    dx = m[None, :, 0] - px[:, None]
+    dy = m[None, :, 1] - py[:, None]
+    a, b, c, o = co[:, 0], co[:, 1], co[:, 2], co[:, 3]
+    power = -0.5 * (a * dx * dx + c * dy * dy) - b * dx * dy
+    mag = 0.5 * (np.abs(a) * dx * dx + np.abs(c) * dy * dy) + np.abs(b * dx * dy)
+    G = np.exp(power)
+    alpha = np.minimum(ALPHA_MAX, o * G)
+    # relative error of the fp32 alpha, in u: dx rounding + five operations on the quadratic's terms, expf, the product
+    ea = 8.0 * mag + np.where(power != 0, 2.0, 0.0) + np.where(o * G < ALPHA_MAX, 1.0, 0.0)
+    return dict(ids=ids, px=px, py=py, inside=inside, dx=dx, dy=dy, a=a, b=b, c=c, o=o, power=power, mag=mag, G=G,
+                alpha=alpha, ea=ea)
+
+
+def decide(st, tile, band=4.0):
+    """Float64 decisions of one tile.  Returns dict(mask [256,L] bool, first_border [256] (L where none),
+    foot_in [256,L] (surely inside the alpha >= 1/255 footprint, whatever T does), pairs)."""
+    p = _pairs(st, tile)
+    L = len(p["ids"])
+    alpha, power, ea = p["alpha"], p["power"], p["ea"]
+    pw_band = band * 8.0 * U * p["mag"]
+    al_band = band * U * ea * alpha
+    pos_in = power <= -pw_band
+    pos_out = power > pw_band
+    a_in = alpha >= ALPHA_MIN + al_band
+    a_out = alpha < ALPHA_MIN - al_band
+    foot_in = pos_in & a_in
+    foot_out = pos_out | a_out
+    foot_border = ~(foot_in | foot_out)
+    # transmittance: running product over the footprint contributors; the fp32 product drifts by (1 + ea alpha/(1-alpha)) u per step
+    om = np.where(foot_in, 1.0 - alpha, 1.0)
+    cp = np.cumprod(om, axis=1)
+    rel = np.cumsum(np.where(foot_in, 2.0 + ea * alpha / (1.0 - alpha), 0.0), axis=1) * U * band
+    stop = foot_in & (cp < T_STOP)
+    t_border = foot_in & (np.abs(cp - T_STOP) <= rel * cp)
+    idx = np.arange(L)[None, :]
+    first_stop = np.where(stop.any(1), np.argmax(stop, 1), L)
+    border = foot_border | t_border
+    first_border = np.where(border.any(1), np.argmax(border, 1), L)
+    # a border pair behind the stop does not matter
+    first_border = np.where(first_border > first_stop, L, first_border)
+    mask = foot_in & (idx < first_stop[:, None])
+    mask &= p["inside"][:, None]
+    first_border = np.where(p["inside"], first_border, L)
+    return dict(mask=mask, first_border=first_border, foot_in=foot_in & p["inside"][:, None], pairs=p)
+
+
+def decide_fp32(st, tile):
+    """The C oracle's own decisions (gs_oracle.c gso_render_forward, built with -ffp-contract=off), restated in numpy float32:
+    same operation order, expf correctly rounded."""
+    r0, r1 = (int(v) for v in st["ranges"][tile])
+    ids = st["point_list"][r0:r1].astype(np.int64)
+    px, py, inside = tile_pixels(st["W"], st["H"], tile)
+    f = np.float32
+    m = st["means2D"][ids].astype(f)
+    co = st["conic_opacity"][ids].astype(f)
+    dx = m[None, :, 0] - px[:, None].astype(f)
+    dy = m[None, :, 1] - py[:, None].astype(f)
+    power = f(-0.5) * (co[:, 0] * dx * dx + co[:, 2] * dy * dy) - co[:, 1] * dx * dy
+    G = np.exp(power.astype(np.float64)).astype(f)
+    alpha = np.minimum(f(0.99), co[:, 3] * G)
+    ok = ~(power > 0) & ~(alpha < f(1.0) / f(255.0))
+    om = np.where(ok, f(1) - alpha, f(1)).astype(f)
+    cp = np.cumprod(om, axis=1, dtype=f)
+    stop = ok & (cp < f(0.0001))
+    L = len(ids)
+    first_stop = np.where(stop.any(1), np.argmax(stop, 1), L)
+    return ok & (np.arange(L)[None, :] < first_stop[:, None]) & inside[:, None]
+
+
+def _channels(st, ids):
+    """[L, C] channel rows {r, g, b, depth?, features...} of the entries and the matching cotangent plane list."""
+    cols = [st["colors"][ids].astype(np.float64)]
+    if st.get("depth") is not None:
+        cols.append(st["depth"][ids].astype(np.float64)[:, None])
+    if st.get("feature") is not None and st["feature"].ndim == 2 and st["feature"].shape[1]:
+        cols.append(st["feature"][ids].astype(np.float64))
+    return np.concatenate(cols, 1)
+
+
+def _cot(st, px, py, inside):
+    """[256, C] cotangents of the tile's pixels in the order of _channels, and [256] alpha cotangents."""
+    x, y = np.where(inside, px, 0), np.where(inside, py, 0)
+    g = [st["g_color"][:, y, x].T.astype(np.float64)]
+    if st.get("depth") is not None:
+        gd = st.get("g_depth")
+        g.append((gd[y, x] if gd is not None else np.zeros(256))[:, None].astype(np.float64))
+    if st.get("feature") is not None and st["feature"].ndim == 2 and st["feature"].shape[1]:
+        g.append(st["g_feature"][:, y, x].T.astype(np.float64))
+    ga = st.get("g_alpha")
+    h = ga[y, x].astype(np.float64) if ga is not None else np.zeros(256)
+    g = np.concatenate(g, 1)
+    g[~inside] = 0
+    h[~inside] = 0
+    return g, h
+
+
+def blend(st, masks, backward=True):
+    """Images and blend-stage gradients in float64 from `masks` (per tile, [256, L] bool), with bounds.
+
+    Returns dict: per pixel `color` [3,H,W], `feature` [F,H,W], `depth` [H,W], `final_T`, `alpha` [H,W], `n_contrib` [H,W]
+    (1-based tile-list position of the last contributor) and `*_B` the matching bound magnitudes; per Gaussian
+    `dL_dmeans2D` [P,2], `dL_dconic` [P,3] (a, b, c slots), `dL_dopacity` [P], `dL_dcolors` [P,3], `dL_dfeature` [P,F],
+    and their `*_B`."""
+    out = new_out(st)
+    for tile in range(st["ranges"].shape[0]):
+        blend_tile(st, tile, masks[tile], out, backward)
+    return out
+
+
+def new_out(st):
+    """Zeroed result arrays of blend() for the state `st`."""
+    W, H, P = st["W"], st["H"], st["means2D"].shape[0]
+    F = st["feature"].shape[1] if (st.get("feature") is not None and st["feature"].ndim == 2) else 0
+    out = {k: np.zeros(s) for k, s in (("color", (3, H, W)), ("color_B", (3, H, W)), ("feature", (F, H, W)),
+                                       ("feature_B", (F, H, W)), ("depth", (H, W)), ("depth_B", (H, W)),
+                                       ("final_T", (H, W)), ("final_T_B", (H, W)), ("alpha", (H, W)), ("alpha_B", (H, W)))}
+    out["n_contrib"] = np.zeros((H, W), np.int64)
+    for k, s in (("dL_dmeans2D", (P, 2)), ("dL_dconic", (P, 3)), ("dL_dopacity", (P,)), ("dL_dcolors", (P, 3)),
+                 ("dL_dfeature", (P, F))):
+        out[k] = np.zeros(s)
+        out[k + "_B"] = np.zeros(s)
+    return out
+
+
+def blend_tile(st, tile, m, out, backward=True):
+    """Adds one tile's pixels and per-Gaussian gradient terms (contributor mask m [256, L]) into `out` (see blend)."""
+    W, H = st["W"], st["H"]
+    F = st["feature"].shape[1] if (st.get("feature") is not None and st["feature"].ndim == 2) else 0
+    has_d = st.get("depth") is not None
+    bg = np.asarray(st["bg"], np.float64)
+    nch = 3 + int(has_d)
+    if m.shape[1] == 0:
+        px, py, inside = tile_pixels(W, H, tile)
+        x, y = px[inside], py[inside]
+        out["final_T"][y, x] = 1.0
+        out["color"][:, y, x] = bg[:, None]
+        out["color_B"][:, y, x] = np.abs(bg)[:, None]
+        return
+    p = _pairs(st, tile)
+    inside, px, py = p["inside"], p["px"], p["py"]
+    x, y = px[inside], py[inside]
+    a = np.where(m, p["alpha"], 0.0)
+    ea = np.where(m, p["ea"], 0.0)
+    om = 1.0 - a
+    cp = np.cumprod(om, axis=1)
+    Tf = cp[:, -1]
+    Tb = np.concatenate([np.ones((256, 1)), cp[:, :-1]], 1)
+    w = a * Tb
+    step = np.where(m, 2.0 + ea * a / om, 0.0)
+    relT = np.cumsum(step, 1)                 # relative error of T after each entry (u)
+    relTb = relT - step
+    relTf = relT[:, -1]
+    C = _channels(st, p["ids"])
+    vals = w @ C
+    ew = ea + relTb + 2.0
+    vB = (np.abs(w) * ew) @ np.abs(C)
+    col = vals[:, :3] + Tf[:, None] * bg[None, :]
+    colB = vB[:, :3] + Tf[:, None] * np.abs(bg)[None, :] * (relTf[:, None] + 1.0)
+    out["color"][:, y, x] = col[inside].T
+    out["color_B"][:, y, x] = colB[inside].T
+    if has_d:
+        out["depth"][y, x] = vals[inside, 3]
+        out["depth_B"][y, x] = vB[inside, 3]
+    if F:
+        out["feature"][:, y, x] = vals[inside, nch:].T
+        out["feature_B"][:, y, x] = vB[inside, nch:].T
+    out["final_T"][y, x] = Tf[inside]
+    out["final_T_B"][y, x] = (Tf * (relTf + 1.0))[inside]
+    out["alpha"][y, x] = 1.0 - Tf[inside]
+    out["alpha_B"][y, x] = (Tf * (relTf + 1.0) + (1.0 - Tf))[inside]
+    L = m.shape[1]
+    last = np.where(m.any(1), L - np.argmax(m[:, ::-1], 1), 0)
+    out["n_contrib"][y, x] = last[inside]
+    if not backward:
+        return
+    g, h = _cot(st, px, py, inside)
+    dot = g @ C.T                                   # [256, L]  c_k . g
+    dabs = np.abs(g) @ np.abs(C).T
+    wd = w * dot
+    S = np.cumsum(wd[:, ::-1], 1)[:, ::-1] - wd     # sum over the contributors behind k
+    Sabs = np.cumsum((np.abs(w) * dabs)[:, ::-1], 1)[:, ::-1] - np.abs(w) * dabs
+    Bp = Tf * (g[:, :3] @ bg - h)
+    Babs = Tf * (np.abs(g[:, :3]) @ np.abs(bg) + np.abs(h))
+    dA = np.where(m, Tb * dot - (S + Bp[:, None]) / om, 0.0)
+    dAabs = np.where(m, Tb * dabs + (Sabs + Babs[:, None]) / om, 0.0)
+    # the backward rebuilds T_k from T_final: its relative error is the pixel's whole product drift; 1/(1-alpha)
+    # amplifies alpha's own error by 1/(1-alpha)
+    e = np.where(m, 4.0 + ea / om + relTf[:, None], 0.0)
+    G, o, dx, dy = p["G"], p["o"], p["dx"], p["dy"]
+    ids = p["ids"]
+    dG = o * dA
+    qabs = o * G * dAabs * e
+    gx_ = -G * (dx * p["a"] + dy * p["b"])
+    gy_ = -G * (dy * p["c"] + dx * p["b"])
+    mx = np.abs(dx) + 8.0
+    my = np.abs(dy) + 8.0
+    acc = [("dL_dmeans2D", 0, (dG * gx_ * (0.5 * W)).sum(0), (qabs * (np.abs(p["a"]) * mx + np.abs(p["b"]) * my) * (0.5 * W)).sum(0)),
+           ("dL_dmeans2D", 1, (dG * gy_ * (0.5 * H)).sum(0), (qabs * (np.abs(p["c"]) * my + np.abs(p["b"]) * mx) * (0.5 * H)).sum(0)),
+           ("dL_dconic", 0, (-0.5 * G * dx * dx * dG).sum(0), (0.5 * qabs * mx * mx).sum(0)),
+           ("dL_dconic", 1, (-0.5 * G * dx * dy * dG).sum(0), (0.5 * qabs * mx * my).sum(0)),
+           ("dL_dconic", 2, (-0.5 * G * dy * dy * dG).sum(0), (0.5 * qabs * my * my).sum(0)),
+           ("dL_dopacity", None, (G * dA).sum(0), (G * dAabs * e).sum(0))]
+    for k, c, v, vb in acc:
+        if c is None:
+            np.add.at(out[k], ids, v)
+            np.add.at(out[k + "_B"], ids, vb)
+        else:
+            np.add.at(out[k][:, c], ids, v)
+            np.add.at(out[k + "_B"][:, c], ids, vb)
+    ge = np.abs(w) * e
+    np.add.at(out["dL_dcolors"], ids, w.T @ g[:, :3])
+    np.add.at(out["dL_dcolors_B"], ids, ge.T @ np.abs(g[:, :3]))
+    if F:
+        np.add.at(out["dL_dfeature"], ids, w.T @ g[:, nch:])
+        np.add.at(out["dL_dfeature_B"], ids, ge.T @ np.abs(g[:, nch:]))
+
+
+def masks_from_blocks(st, block_lists, pixel_masks, block_nwalk):
+    """Contributor masks per tile from the kernels' per-block work lists and pixel masks (entries up to block_nwalk)."""
+    out = []
+    for tile in range(st["ranges"].shape[0]):
+        r0, r1 = (int(v) for v in st["ranges"][tile])
+        m = np.zeros((256, r1 - r0), bool)
+        px, py, inside = tile_pixels(st["W"], st["H"], tile)
+        for s in range(8):
+            k = int(block_nwalk[tile, s])
+            # a block with no pixel inside the image is never blended: its block_nwalk is not written
+            if k == 0 or not inside[pixel_block_bit(np.arange(256) % 16, np.arange(256) // 16)[0] == s].any():
+                continue
+            pos = block_lists[s, r0:r0 + k].astype(np.int64)
+            bits = pixel_masks[s, r0:r0 + k].astype(np.uint64)
+            for b in range(32):
+                xx, yy = b >> 2, b & 3
+                lx, ly = (s & 1) * 8 + xx, (s >> 1) * 4 + yy
+                m[ly * 16 + lx, pos] = ((bits >> np.uint64(b)) & np.uint64(1)).astype(bool)
+        out.append(m)
+    return out
+
+
+def ratio(got, ref, B, quantity, kappa=None):
+    """|got - ref| / (kappa u B + tiny), elementwise; kappa defaults to KAPPA[quantity] (kappa = 1: the raw ratio)."""
+    k = KAPPA[quantity] if kappa is None else kappa
+    return np.abs(np.asarray(got, np.float64) - ref) / (k * U * B + 1e-30)
+
+
+def cov3d_grad(ref, means3D, cov3D, viewmatrix, W, H, tanfovx, tanfovy):
+    """dL_dcov3D [P,6] and its bound from the blend-stage dL_dconic of `ref` (a blend() result), in float64: the
+    reference's computeCov2D backward (backward.cu:144-274, restated in oracle/gs_oracle.c gso_preprocess_backward) for
+    callers that pass cov3D_precomp.  The bound carries the conic gradient's own bound through the same linear map, plus
+    the chain's rounding: the 2D covariance's determinant cancels by (ac + b^2) / det for elongated splats."""
+    vm = np.asarray(viewmatrix, np.float64).reshape(-1)
+    p = np.asarray(means3D, np.float64)
+    V3 = np.asarray(cov3D, np.float64)
+    t = np.stack([vm[0] * p[:, 0] + vm[4] * p[:, 1] + vm[8] * p[:, 2] + vm[12],
+                  vm[1] * p[:, 0] + vm[5] * p[:, 1] + vm[9] * p[:, 2] + vm[13],
+                  vm[2] * p[:, 0] + vm[6] * p[:, 1] + vm[10] * p[:, 2] + vm[14]], 1)
+    fx, fy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
+    limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
+    tz = t[:, 2]
+    tx = np.clip(t[:, 0] / tz, -limx, limx) * tz
+    ty = np.clip(t[:, 1] / tz, -limy, limy) * tz
+    n = len(p)
+    J = np.zeros((n, 3, 3))
+    J[:, 0, 0], J[:, 0, 2] = fx / tz, -(fx * tx) / (tz * tz)
+    J[:, 1, 1], J[:, 1, 2] = fy / tz, -(fy * ty) / (tz * tz)
+    Wm = np.array([[vm[0], vm[4], vm[8]], [vm[1], vm[5], vm[9]], [vm[2], vm[6], vm[10]]])
+    T = J @ Wm                                  # gs_oracle.c m3mul(W, J) in row-major numpy terms
+    Vr = np.stack([V3[:, [0, 1, 2]], V3[:, [1, 3, 4]], V3[:, [2, 4, 5]]], 1)
+    cov = T @ Vr @ np.transpose(T, (0, 2, 1))
+    a, b, c = cov[:, 0, 0] + 0.3, cov[:, 0, 1], cov[:, 1, 1] + 0.3
+    det = a * c - b * b
+    w = 1.0 / (det * det + 1e-7)
+    g0, g1, g2 = (ref["dL_dconic"][:, i] for i in range(3))
+    B0, B1, B2 = (ref["dL_dconic_B"][:, i] for i in range(3))
+    dA = w * (-c * c * g0 + 2 * b * c * g1 - b * b * g2)
+    dC = w * (-a * a * g2 + 2 * a * b * g1 - b * b * g0)
+    dB = w * 2 * (b * c * g0 - (det + 2 * b * b) * g1 + a * b * g2)
+    e = 16.0 + 8.0 * (a * c + b * b) / np.abs(det)
+    ab, bb, cb = np.abs(a), np.abs(b), np.abs(c)
+    dA_B = w * (c * c * (B0 + e * abs(g0)) + 2 * bb * cb * (B1 + e * abs(g1)) + b * b * (B2 + e * abs(g2)))
+    dC_B = w * (a * a * (B2 + e * abs(g2)) + 2 * ab * bb * (B1 + e * abs(g1)) + b * b * (B0 + e * abs(g0)))
+    dB_B = w * 2 * (bb * cb * (B0 + e * abs(g0)) + (abs(det) + 2 * b * b) * (B1 + e * abs(g1)) + ab * bb * (B2 + e * abs(g2)))
+    out, outB = np.zeros((n, 6)), np.zeros((n, 6))
+    A = np.abs(T)
+    for k, (i, j) in enumerate(((0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2))):
+        f = 1.0 if i == j else 2.0   # off-diagonal entries appear twice in the symmetric cov3D
+        # dcov[ij] = f/2 (T0i T0j + T0j T0i) dA + (T0i T1j + T0j T1i)/ (2/f) dB + f/2 (T1i T1j + T1j T1i) dC
+        ca = 0.5 * f * (T[:, 0, i] * T[:, 0, j] + T[:, 0, j] * T[:, 0, i])
+        cb_ = (T[:, 0, i] * T[:, 1, j] + T[:, 0, j] * T[:, 1, i]) * (0.5 if i == j else 1.0)
+        cc = 0.5 * f * (T[:, 1, i] * T[:, 1, j] + T[:, 1, j] * T[:, 1, i])
+        out[:, k] = ca * dA + cb_ * dB + cc * dC
+        ca_, cbb, ccc = (0.5 * f * 2 * A[:, 0, i] * A[:, 0, j], (A[:, 0, i] * A[:, 1, j] + A[:, 0, j] * A[:, 1, i]) *
+                         (0.5 if i == j else 1.0), 0.5 * f * 2 * A[:, 1, i] * A[:, 1, j])
+        outB[:, k] = ca_ * (dA_B + 4 * abs(dA)) + cbb * (dB_B + 4 * abs(dB)) + ccc * (dC_B + 4 * abs(dC))
+    return out, outB
