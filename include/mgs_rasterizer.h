@@ -365,6 +365,82 @@ int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_off
 int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
 	const mgs_view_alpha* alpha, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
+/*
+ * Depth and mask heads (no reference counterpart; INTEGRATION.md §4): two more loss heads beside the fused colour and
+ * embedding heads of mgs_view, evaluated in the same forward-blend epilogue from the view's depth plane D and alpha plane
+ * A = 1 - final_T, so that a step with depth or mask supervision keeps the fused path (no image-sized kernel between the
+ * forward and the backward, no host synchronisation).  Per view, N = H*W:
+ *   depth  valid = (target_depth > 0) && (A > 0.5), d = D / A, n = sum valid:  loss_depth = sum_valid |d - target_depth| / n
+ *          (0 when n = 0);
+ *   mask   loss_mask = mean_px BCE(clamp(A, 1e-4, 1 - 1e-4), target_mask) as torch.nn.functional.binary_cross_entropy.
+ * The calls below are the _alpha calls with one more argument, `depth_mask`: one mgs_view_depth_mask per view (V entries,
+ * or view_offsets[B] for clouds), or NULL for none; the _alpha calls are these with depth_mask == NULL.  Pass the same
+ * array to the forward and the backward.  A view whose two targets are NULL has no depth or mask head.
+ * Forward: the heads need the colour head (the view's target_color).  loss_acc (device, 3 floats, zeroed by the call)
+ * receives {sum_valid |d - g|, n, sum_px BCE}: loss_depth = loss_acc[0] / max(loss_acc[1], 1), loss_mask = loss_acc[2] / N.
+ * With target_depth, cot_depth and cot_alpha_depth [H,W] receive the unscaled cotangents sign(d - g) / A and
+ * -sign(d - g) d / A on valid pixels, 0 elsewhere; with target_mask, cot_alpha_mask [H,W] receives d loss_mask / dA.
+ * Backward: the planes are read back with cot_scale (device, 2 floats {g_depth, g_mask}, or NULL for 1): the depth plane's
+ * cotangent is g_depth / max(n, 1) * cot_depth, and the alpha cotangent g_depth / max(n, 1) * cot_alpha_depth +
+ * g_mask * cot_alpha_mask, with n read from loss_acc on the device.  Argument errors (a target without its planes or
+ * loss_acc, a target without the view's colour head in the forward) return MGS_ERR_INVALID_ARG before anything is enqueued.
+ */
+typedef struct mgs_view_depth_mask {
+	const float* target_depth;     /* [H,W] or NULL */
+	const float* target_mask;      /* [H,W] in [0,1], or NULL */
+	float* cot_depth;              /* [H,W], with target_depth */
+	float* cot_alpha_depth;        /* [H,W], with target_depth */
+	float* cot_alpha_mask;         /* [H,W], with target_mask */
+	float* loss_acc;               /* device, 3 floats */
+	const float* cot_scale;        /* device, 2 floats, or NULL */
+} mgs_view_depth_mask;
+
+int mgs_forward_views_depth_mask(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_depth_mask(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int prefiltered,
+	int debug, void* join_stream);
+int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
+	int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -32,6 +32,12 @@ class ViewAlpha(C.Structure):
     _fields_ = [("out_alpha", C.c_void_p), ("dL_dpix_alpha", C.c_void_p)]
 
 
+class ViewDepthMask(C.Structure):
+    """mirror of `mgs_view_depth_mask` (include/mgs_rasterizer.h): the optional depth and mask heads of one view"""
+    _fields_ = [(n, C.c_void_p) for n in ("target_depth", "target_mask", "cot_depth", "cot_alpha_depth", "cot_alpha_mask",
+                                          "loss_acc", "cot_scale")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -104,6 +110,9 @@ def lib():
         k = 4 if "clouds" in name else 2
         getattr(L, name + "_alpha").restype = C.c_int
         getattr(L, name + "_alpha").argtypes = at[:k] + [C.POINTER(ViewAlpha)] + at[k:]
+        # ... and with the depth / mask heads (one ViewDepthMask per view, or NULL) after the alpha planes
+        getattr(L, name + "_depth_mask").restype = C.c_int
+        getattr(L, name + "_depth_mask").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_mark_visible.restype = C.c_int
@@ -135,6 +144,8 @@ EXPORTED_SYMBOLS = (
     "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_forward", "mgs_forward_begin",
     "mgs_backward", "mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds", "mgs_loss_heads",
     "mgs_forward_views_alpha", "mgs_backward_views_alpha", "mgs_forward_clouds_alpha", "mgs_backward_clouds_alpha",
+    "mgs_forward_views_depth_mask", "mgs_backward_views_depth_mask", "mgs_forward_clouds_depth_mask",
+    "mgs_backward_clouds_depth_mask",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -432,8 +432,30 @@ static BlendArgs blend_args(const ViewState& s, const mgs_view& w, int F, const 
 	return ba;
 }
 
-// forward blend, with the fused loss heads when the view has a target; out_alpha (nullable) receives 1 - final_T
-static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, int debug)
+// the depth / mask heads of one view: a target needs its planes and the accumulator, and (forward) the colour head
+static int check_depth_mask(const mgs_view& w, const mgs_view_depth_mask* dm, bool forward)
+{
+	if (!dm || (!dm->target_depth && !dm->target_mask)) return 0;
+	if (forward && !w.target_color) return fail(MGS_ERR_INVALID_ARG, "view: the depth / mask heads need the colour head (target_color)");
+	if (!dm->loss_acc) return fail(MGS_ERR_INVALID_ARG, "view: the depth / mask heads need loss_acc");
+	if (dm->target_depth && (!dm->cot_depth || !dm->cot_alpha_depth))
+		return fail(MGS_ERR_INVALID_ARG, "view: target_depth needs cot_depth and cot_alpha_depth");
+	if (dm->target_mask && !dm->cot_alpha_mask) return fail(MGS_ERR_INVALID_ARG, "view: target_mask needs cot_alpha_mask");
+	return 0;
+}
+
+// the BlendArgs fields of the depth / mask heads (dm nullable; checked by check_depth_mask)
+static void depth_mask_args(BlendArgs& ba, const mgs_view_depth_mask* dm)
+{
+	if (!dm || (!dm->target_depth && !dm->target_mask)) return;
+	ba.tgt_depth = dm->target_depth; ba.tgt_mask = dm->target_mask;
+	ba.cot_depth = dm->cot_depth; ba.cot_alpha_depth = dm->cot_alpha_depth; ba.cot_alpha_mask = dm->cot_alpha_mask;
+	ba.dm_acc = dm->loss_acc; ba.dm_scale = dm->cot_scale;
+}
+
+// forward blend, with the fused loss heads when the view has a target; out_alpha (nullable) receives 1 - final_T; dm
+// (nullable): the view's depth / mask heads
+static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, const mgs_view_depth_mask* dm, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = (c.F > 0 && c.feature && w.out_feature) ? c.F : 0;
@@ -450,6 +472,8 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha
 		ba.tgt_color = w.target_color; ba.tgt_feature = (embed && !embed_after) ? w.target_feature : nullptr;
 		ba.cot_color = w.cot_color; ba.cot_feature = w.cot_feature; ba.loss_acc = w.loss_acc;
 		MGS_CUDA(cudaMemsetAsync(w.loss_acc, 0, 2 * sizeof(float), st));
+		depth_mask_args(ba, dm);
+		if (ba.dm_acc) MGS_CUDA(cudaMemsetAsync(ba.dm_acc, 0, 3 * sizeof(float), st));
 	}
 	{
 		StageTimer t_(ST_BLEND_FWD, st);
@@ -464,18 +488,21 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha
 
 // blend backward of one view on its stream: the view's blend-stage records, and the feature gradients summed with 128-bit
 // reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
-// and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane.
-static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, const float* dL_dalpha, int debug)
+// and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane; dm
+// (nullable): the view's depth / mask heads, whose cotangent planes the walker's prologue folds in.
+static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, const float* dL_dalpha, const mgs_view_depth_mask* dm,
+	int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = c.F;
 	const ViewState s = carve_view(w, c.P);
 	MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)c.P * GB_STRIDE * sizeof(float), st));
 	BlendArgs ba = blend_args(s, w, F, c.feature);
-	ba.want_depth = w.dL_dpix_depth != nullptr;
 	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth; ba.dL_dalpha = dL_dalpha;
 	ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
 	ba.cot_scale = w.cot_scale;
+	depth_mask_args(ba, dm);
+	ba.want_depth = w.dL_dpix_depth != nullptr || ba.tgt_depth != nullptr;  // the depth head's cotangent reaches the view-space z
 	if (w.binning_capacity > 0) {
 		{ StageTimer t_(ST_BLEND_BWD, st); launch_blend_bwd(ba, st); }
 		MGS_STAGE("blend_bwd");
@@ -497,8 +524,8 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
-// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha: V entries or NULL.
-static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const Cloud& c, float* dL_dmean3D,
+// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm: V entries or NULL.
+static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -508,7 +535,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		int rc = fork_streams(V, views, join);
 		if (rc < 0) return rc;
 		for (int v = 0; v < V; v++) {
-			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, debug);
+			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -643,7 +670,7 @@ int mgs_forward(
 	w.binning_capacity = num_rendered;
 	rc = enqueue_binning(c, w, true, debug);
 	if (rc < 0) return rc;
-	rc = enqueue_blend_fwd(c, w, nullptr, debug);
+	rc = enqueue_blend_fwd(c, w, nullptr, nullptr, debug);
 	return rc < 0 ? rc : num_rendered;
 }
 
@@ -691,7 +718,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -713,6 +740,17 @@ int mgs_forward_views_alpha(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_depth_mask(V, views, alpha, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities,
+		scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_depth_mask(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
@@ -722,6 +760,7 @@ int mgs_forward_views_alpha(
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int v = 0; v < V; v++) {
 		int rc = check_fwd_view(views[v], !colors_precomp);
+		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp };
@@ -744,7 +783,7 @@ int mgs_forward_views_alpha(
 		for (int v = 0; v < V; v++) {
 			rc = phase == 0 ? enqueue_project(c, views[v], debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
-				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, debug);
+				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -772,6 +811,19 @@ int mgs_backward_views_alpha(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_depth_mask(V, views, alpha, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
+		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot,
+		shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_depth_mask(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
@@ -780,10 +832,11 @@ int mgs_backward_views_alpha(
 	if (F > 0 && (!feature_precomp || !dL_dfeature)) F = 0;
 	for (int v = 0; v < V; v++) {
 		int rc = check_bwd_view(views[v], F > 0);
+		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp };
-	return backward_views(V, views, alpha, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -795,6 +848,14 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 
 int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
 	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
+	return mgs_forward_clouds_depth_mask(B, clouds, view_offsets, views, alpha, nullptr, D, M, F, scale_modifier, prefiltered, debug,
+		join_stream);
+}
+
+int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int prefiltered,
+	int debug, void* join_stream)
 {
 	(void)prefiltered;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -808,6 +869,7 @@ int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_off
 			return fail(MGS_ERR_INVALID_ARG, "cloud: provide scales+rotations or a precomputed 3D covariance");
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			rc = check_fwd_view(views[v], !k.colors_precomp);
+			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 			if (rc < 0) return rc;
 		}
 	}
@@ -822,7 +884,7 @@ int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_off
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 				rc = phase == 0 ? enqueue_project(c, views[v], debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
-					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, debug);
+					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
 		}
@@ -839,6 +901,14 @@ int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets,
 int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
 	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_depth_mask(B, clouds, view_offsets, views, alpha, nullptr, D, M, F, scale_modifier, accumulate, debug,
+		join_stream);
+}
+
+int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
+	int debug, void* join_stream)
+{
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -850,6 +920,7 @@ int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_of
 			return fail(MGS_ERR_INVALID_ARG, "cloud: dL_dsh is required with SHs (it carries the view-direction term of dL_dmean3D)");
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			rc = check_bwd_view(views[v], F > 0 && k.feature);
+			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 			if (rc < 0) return rc;
 		}
 	}
@@ -865,7 +936,8 @@ int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_of
 	for (int b = 0; b < B; b++) {
 		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, debug);
+			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
+				depth_mask ? depth_mask + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}

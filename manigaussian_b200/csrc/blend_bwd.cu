@@ -88,8 +88,22 @@ static_assert(BWD_CH == 16 || BWD_CH == 32, "backward chunk size");
 // DONE + s  walker -> companion: wgt and q of the chunk are written            (bar.arrive by W, bar.sync by C)
 constexpr int BWD_BAR_FULL = 1, BWD_BAR_DONE = 3;
 
-// F <= 32 (one channel group); channel groups run blend_bwd_groups_kernel below
-template <int NFT, bool VEC>
+// Cotangents of the depth and mask heads (loss_heads.cuh) for one in-image pixel, folded into the depth cotangent g_depth and
+// the alpha cotangent h of the walker's prologue.  The forward wrote the planes for unit upstream gradients; the depth head's
+// scale g_depth / max(n, 1) needs the view's valid-pixel count n, which the forward's accumulator holds by now.
+__device__ __forceinline__ void depth_mask_cotangents(const BlendArgs& a, size_t pix, float& g_depth, float& h)
+{
+	if (a.tgt_depth) {
+		const float s_d = (a.dm_scale ? a.dm_scale[0] : 1.f) / fmaxf(a.dm_acc[1], 1.f);
+		g_depth += s_d * a.cot_depth[pix];
+		h += s_d * a.cot_alpha_depth[pix];
+	}
+	if (a.tgt_mask) h += (a.dm_scale ? a.dm_scale[1] : 1.f) * a.cot_alpha_mask[pix];
+}
+
+// F <= 32 (one channel group); channel groups run blend_bwd_groups_kernel below.  DM: the depth / mask heads
+// (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.
+template <int NFT, bool VEC, bool DM>
 __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendArgs a)
 {
 	constexpr int NT = NFT + 1;          // channel tiles of 8: NFT feature tiles + {r,g,b,depth, 4 x zero}
@@ -143,6 +157,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
 			if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
 			if (a.dL_dalpha) h = a.dL_dalpha[pix];
+			if (DM) depth_mask_cotangents(a, pix, g4[3], h);
 		}
 		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
@@ -563,7 +578,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 
 // Channel groups (F > 32, BlendArgs::groups): the same replay with one warp per block doing every step, 12 CTAs per SM.
 // At F = 64 and 128 the launch is several waves deep, and there the two-warp kernel measured slower on an H100.
-template <bool VEC>
+template <bool VEC, bool DM>
 __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 {
 	constexpr int NFT = 4;
@@ -620,6 +635,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				for (int ch = 0; ch < 3; ch++) g4[ch] = sc_color * a.dL_dcolor[ch * HW + pix];
 				if (a.dL_ddepth) g4[3] = a.dL_ddepth[pix];
 				if (a.dL_dalpha) h = a.dL_dalpha[pix];
+				if (DM) depth_mask_cotangents(a, pix, g4[3], h);
 			}
 		}
 		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
@@ -938,31 +954,38 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 
 bool feature_rows_vectorizable(const float* feature, int F);
 
-template <int NFT>
+template <int NFT, bool DM>
 static void launch_bwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8;
 	const bool vec = (NFT == 0) || (a.F == 8 * NFT && feature_rows_vectorizable(a.feature, a.F) &&
 		(reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0);
-	if (vec) blend_bwd_kernel<NFT, true><<<grid, 64, 0, s>>>(a);
-	else blend_bwd_kernel<NFT, false><<<grid, 64, 0, s>>>(a);
+	if (vec) blend_bwd_kernel<NFT, true, DM><<<grid, 64, 0, s>>>(a);
+	else blend_bwd_kernel<NFT, false, DM><<<grid, 64, 0, s>>>(a);
 }
 
-void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
+template <bool DM>
+static void launch_bwd_dm(const BlendArgs& a, cudaStream_t s)
 {
 	if (a.groups > 1) {
 		const int grid = a.grid_x * a.grid_y * 8 * a.groups;
 		const bool vec = feature_rows_vectorizable(a.feature, a.F) && (reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0;
-		if (vec) blend_bwd_groups_kernel<true><<<grid, 32, 0, s>>>(a);
-		else blend_bwd_groups_kernel<false><<<grid, 32, 0, s>>>(a);
+		if (vec) blend_bwd_groups_kernel<true, DM><<<grid, 32, 0, s>>>(a);
+		else blend_bwd_groups_kernel<false, DM><<<grid, 32, 0, s>>>(a);
 		return;
 	}
 	switch (nft_for(a.F)) {
-	case 0: launch_bwd_t<0>(a, s); break;
-	case 1: launch_bwd_t<1>(a, s); break;
-	case 2: launch_bwd_t<2>(a, s); break;
-	default: launch_bwd_t<4>(a, s); break;
+	case 0: launch_bwd_t<0, DM>(a, s); break;
+	case 1: launch_bwd_t<1, DM>(a, s); break;
+	case 2: launch_bwd_t<2, DM>(a, s); break;
+	default: launch_bwd_t<4, DM>(a, s); break;
 	}
+}
+
+void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
+{
+	if (a.tgt_depth || a.tgt_mask) launch_bwd_dm<true>(a, s);
+	else launch_bwd_dm<false>(a, s);
 }
 
 }  // namespace mgs

@@ -41,8 +41,9 @@ namespace mgs {
 constexpr int FWD_CH = MGS_FWD_CH;        // block-list entries per tensor-core chunk (multiple of 8, <= 32)
 static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32, "forward chunk size");
 
-// GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic
-template <int NFT, bool VEC, bool GRP>
+// GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic.
+// DM: the depth / mask heads (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.
+template <int NFT, bool VEC, bool GRP, bool DM>
 __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendArgs a)
 {
 	using L = RowLayout<NFT>;
@@ -242,8 +243,10 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	const int ox = bx0 + gid;  // fragment role: this thread holds pixels (x = gid, y = 0..3)
 	const bool heads = first && a.tgt_color != nullptr;     // fused loss heads (loss_heads.cuh)
 	const bool embed = heads && NFT > 0 && a.tgt_feature != nullptr && !GRP;
+	const bool dmh = DM && heads;                           // depth / mask heads
 	const float invN = 1.0f / (float)HW;
 	float s_rgb = 0.f, s_cos = 0.f;                         // this thread's share of the two loss sums
+	float s_dep = 0.f, s_n = 0.f, s_bce = 0.f;              // ... and of the depth / mask heads' sums
 #pragma unroll
 	for (int mt = 0; mt < 2; mt++) {
 #pragma unroll
@@ -277,6 +280,23 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 						const float d = col[e] - a.tgt_color[(size_t)c * HW + pix];
 						s_rgb += d * d;
 						a.cot_color[(size_t)c * HW + pix] = (2.0f / 3.0f) * invN * d;
+					}
+				}
+				// column 3 of the {r,g,b,depth} tile is col[1] of thread tig = 1: that thread evaluates both heads of the pixel,
+				// with the same D and A = 1 - T as the depth and alpha planes
+				if (dmh && tig == 1 && in) {
+					const float A = 1.f - Tp;
+					if (a.tgt_depth) {
+						const DepthTerms dt = depth_terms(col[1], A, a.tgt_depth[pix]);
+						s_dep += dt.err;
+						s_n += dt.n;
+						a.cot_depth[pix] = dt.cot_d;
+						a.cot_alpha_depth[pix] = dt.cot_a;
+					}
+					if (a.tgt_mask) {
+						const MaskTerms mk = mask_terms(A, a.tgt_mask[pix]);
+						s_bce += mk.bce;
+						a.cot_alpha_mask[pix] = mk.grad * invN;
 					}
 				}
 				if (embed) {
@@ -325,6 +345,18 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			if (embed) red_add(a.loss_acc + 1, s_cos);
 		}
 	}
+	if (dmh) {
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) {
+			s_dep += __shfl_xor_sync(0xffffffffu, s_dep, o);
+			s_n += __shfl_xor_sync(0xffffffffu, s_n, o);
+			s_bce += __shfl_xor_sync(0xffffffffu, s_bce, o);
+		}
+		if (lane == 0) {
+			if (a.tgt_depth) { red_add(a.dm_acc, s_dep); red_add(a.dm_acc + 1, s_n); }  // n: exact in fp32 up to 2^24 pixels
+			if (a.tgt_mask) red_add(a.dm_acc + 2, s_bce);
+		}
+	}
 #ifdef MGS_CTA_LOG
 	cta_log_put(a, t_start, 0u, (unsigned int)sub, (unsigned int)count);
 #endif
@@ -340,7 +372,7 @@ bool feature_rows_vectorizable(const float* feature, int F)
 	return F > 0 && (F & 3) == 0 && (reinterpret_cast<uintptr_t>(feature) & 15) == 0;
 }
 
-template <int NFT, bool GRP>
+template <int NFT, bool GRP, bool DM>
 static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
@@ -348,20 +380,27 @@ static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 	// groups, a row slice starts at channel 32 g: 16-byte aligned whenever F % 4 == 0, and a remainder group copies whole
 	// 4-channel pieces only.
 	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F));
-	if (vec) blend_fwd_kernel<NFT, true, GRP><<<grid, 32, 0, s>>>(a);
-	else blend_fwd_kernel<NFT, false, GRP><<<grid, 32, 0, s>>>(a);
+	if (vec) blend_fwd_kernel<NFT, true, GRP, DM><<<grid, 32, 0, s>>>(a);
+	else blend_fwd_kernel<NFT, false, GRP, DM><<<grid, 32, 0, s>>>(a);
+}
+
+template <bool DM>
+static void launch_fwd_dm(const BlendArgs& a, cudaStream_t s)
+{
+	if (a.groups > 1) { launch_fwd_t<4, true, DM>(a, s); return; }
+	switch (nft_for(a.F)) {
+	case 0: launch_fwd_t<0, false, DM>(a, s); break;
+	case 1: launch_fwd_t<1, false, DM>(a, s); break;
+	case 2: launch_fwd_t<2, false, DM>(a, s); break;
+	default: launch_fwd_t<4, false, DM>(a, s); break;
+	}
 }
 
 
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.groups > 1) { launch_fwd_t<4, true>(a, s); return; }
-	switch (nft_for(a.F)) {
-	case 0: launch_fwd_t<0, false>(a, s); break;
-	case 1: launch_fwd_t<1, false>(a, s); break;
-	case 2: launch_fwd_t<2, false>(a, s); break;
-	default: launch_fwd_t<4, false>(a, s); break;
-	}
+	if (a.tgt_color && (a.tgt_depth || a.tgt_mask)) launch_fwd_dm<true>(a, s);
+	else launch_fwd_dm<false>(a, s);
 }
 
 }  // namespace mgs

@@ -135,6 +135,17 @@ struct BlendArgs {
 	float* cot_feature;
 	float* loss_acc;
 	const float* cot_scale;
+	// depth and mask heads (loss_heads.cuh), with the colour head only, all nullable.  Forward: tgt_depth [H,W] writes cot_depth and
+	// cot_alpha_depth, tgt_mask [H,W] writes cot_alpha_mask (all [H,W], unscaled), and {sum |d - g|, n, sum BCE} are added into
+	// dm_acc[0..2].  Backward: with tgt_depth the depth cotangent is dm_scale[0] / max(dm_acc[1], 1) * cot_depth and the alpha
+	// cotangent gains the same scale times cot_alpha_depth; with tgt_mask it gains dm_scale[1] * cot_alpha_mask (dm_scale NULL: 1).
+	const float* tgt_depth;
+	const float* tgt_mask;
+	float* cot_depth;
+	float* cot_alpha_depth;
+	float* cot_alpha_mask;
+	float* dm_acc;
+	const float* dm_scale;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
 	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams

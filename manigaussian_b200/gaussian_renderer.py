@@ -183,13 +183,51 @@ class _RasterizeViews(torch.autograd.Function):
                 v["dL_dscales"], v["dL_drotations"], None, None, None, None)
 
 
+def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
+    """The depth / mask heads' `depth_mask` tuple for the raw calls (targets [V,H,W], their cotangent planes, the [V,3]
+    accumulator), or None when neither target is given."""
+    if t_depth is None and t_mask is None:
+        return None
+    t_depth, t_mask = _prep(t_depth, dev), _prep(t_mask, dev)
+    for name, t in (("depth", t_depth), ("mask", t_mask)):
+        if t is not None and tuple(t.shape) != (V, H, W):
+            raise ValueError(f"{where}: the {name} target must be [V,H,W] = [{V},{H},{W}]")
+    opts = dict(dtype=torch.float32, device=dev)
+    plane = lambda on: torch.empty((V, H, W), **opts) if on else None
+    return (t_depth, t_mask, plane(t_depth is not None), plane(t_depth is not None), plane(t_mask is not None),
+            torch.empty((V, 3), **opts))
+
+
+def _depth_mask_losses(dm, N, dev):
+    """(loss_depth, loss_mask, depth_pixels) [V] from the accumulator of a `depth_mask` tuple; empty for an absent head"""
+    empty = lambda: torch.empty(0, device=dev)
+    if dm is None:
+        return empty(), empty(), empty()
+    acc = dm[5]
+    if dm[0] is not None:
+        loss_depth, n = acc[:, 0] / acc[:, 1].clamp(min=1.0), acc[:, 1].clone()
+    else:
+        loss_depth, n = empty(), empty()
+    loss_mask = acc[:, 2] / N if dm[1] is not None else empty()
+    return loss_depth, loss_mask, n
+
+
+def _depth_mask_scale(dm, g_depth, g_mask, V, dev):
+    """[V,2] upstream gradients {g_depth, g_mask} of the depth / mask losses for the backward"""
+    z = torch.zeros((V,), dtype=torch.float32, device=dev)
+    return torch.stack([g_depth if (dm[0] is not None and g_depth is not None) else z,
+                        g_mask if (dm[1] is not None and g_mask is not None) else z], 1).contiguous()
+
+
 class _RasterizeViewsLoss(torch.autograd.Function):
     """render_views with the loss heads fused into the forward blend's epilogue (SURVEY.md 8(f) row f4): returns the per-view
-    L2 colour loss and cosine embedding loss of NeuralRenderer.forward (neural_rendering.py:300-318, loss.py:12-23); the
-    images come back too, but gradients flow through the two losses only."""
+    L2 colour loss and cosine embedding loss of NeuralRenderer.forward (neural_rendering.py:300-318, loss.py:12-23) and,
+    with depth / mask targets (row f7), the expected-depth L1 loss, the alpha mask BCE loss and the valid-pixel counts; the
+    images come back too, but gradients flow through the losses only."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
+                target_depth=None, target_mask=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -209,11 +247,12 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         cot_rgb = torch.empty((V, 3, H, W), **opts)
         cot_embed = torch.empty((V, F, H, W), **opts) if target_embed is not None else (torch.zeros((V, F, H, W), **opts) if include else None)
         loss_acc = torch.empty((V, 2), **opts)
+        dm = _depth_mask_heads(target_depth, target_mask, V, H, W, dev)
         degree = views[0].sh_degree
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, debug=views[0].debug,
                                             out_buffers=(color, feat_img, None),
-                                            loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc))
+                                            loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm)
         N = float(H * W)
         loss_rgb = loss_acc[:, 0] / (3.0 * N)
         loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
@@ -225,16 +264,18 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         ctx.include, ctx.F, ctx.degree = include, F, degree
         ctx.opac_shape = opacities.shape
         ctx.cots = (cot_rgb, cot_embed)
+        ctx.dm = dm  # the targets, cotangent planes and accumulator of the depth / mask heads: none of them is an output
         ctx.save_for_backward(means3D, sh if sh is not None else torch.empty(0, device=dev),
                               colors_precomp if colors_precomp is not None else torch.empty(0, device=dev),
                               feature if include else torch.empty(0, device=dev), scales, rotations)
-        # ONE call: a second mark_non_differentiable replaces the first
-        ctx.mark_non_differentiable(*([radii, color] + ([feat_img] if include else [])))
         empty = torch.empty(0, device=dev)
-        return loss_rgb, loss_embed, color, (feat_img if include else empty), radii
+        loss_depth, loss_mask, depth_pixels = _depth_mask_losses(dm, N, dev)
+        # ONE call: a second mark_non_differentiable replaces the first
+        ctx.mark_non_differentiable(radii, color, *([feat_img] if include else []), depth_pixels)
+        return loss_rgb, loss_embed, color, (feat_img if include else empty), radii, loss_depth, loss_mask, depth_pixels
 
     @staticmethod
-    def backward(ctx, g_rgb, g_embed, _gc, _gf, _gr):
+    def backward(ctx, g_rgb, g_embed, _gc, _gf, _gr, g_depth, g_mask, _gn):
         means3D, sh, colors_precomp, feature, scales, rotations = ctx.saved_tensors
         dev = means3D.device
         views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
@@ -251,13 +292,15 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                      colors_precomp if use_colors else None, feature if ctx.include else None, scales, rotations,
                                      views[0].scale_modifier, None, sh if M else None, ctx.degree, ctx.include, debug=views[0].debug,
                                      accumulate_into=pk.views, means2D_per_view=m2d, cot_scale=scale,
-                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None)
+                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
+                                     depth_mask=ctx.dm,
+                                     depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None)
         if ctx.group is not None:
             pk.all_reduce_finish(grp)
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None)
 
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
@@ -273,7 +316,12 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     targets: {"rgb": [V,3,H,W], "embed": [V,F,H,W] (optional)} fuses ManiGaussian's loss heads into the forward blend's
     epilogue: the result then also holds "loss_rgb" and "loss_embed" ([V] each: l2_loss and cosine_loss of
     agents/manigaussian_bc/loss.py per view; combine them as neural_rendering.py:300-318 does) through which -- and only
-    through which -- gradients flow; "render"/"render_embed" are returned detached.
+    through which -- gradients flow; "render"/"render_embed" are returned detached.  targets may also hold "depth" [V,H,W]
+    (ground-truth depth, 0 = unknown) and "mask" [V,H,W] (in [0,1]): the same epilogue then evaluates the expected-depth L1
+    head and the alpha mask head of INTEGRATION.md §4 per view and the result adds "loss_depth" [V] (mean |depth / alpha - gt|
+    over the pixels with gt > 0 and alpha > 0.5; 0 where there is none), "depth_pixels" [V] (their count, float, not
+    differentiable) and "loss_mask" [V] (binary cross-entropy of clamp(alpha, 1e-4, 1 - 1e-4) against the mask, mean over
+    the pixels).
     return_alpha: also return "alpha" [V,H,W], the accumulated opacity 1 - final_T (differentiable; depth / alpha is the
     expected depth).
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
@@ -301,11 +349,16 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
             raise ValueError("targets and return_depth cannot be combined")
         if return_alpha:
             raise ValueError("targets and return_alpha cannot be combined")
-        loss_rgb, loss_embed, color, feat_img, radii = _RasterizeViewsLoss.apply(
+        loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients)
-        return {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
-                "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
+            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"))
+        ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
+               "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
+        if targets.get("depth") is not None:
+            ret["loss_depth"], ret["depth_pixels"] = loss_depth, depth_pixels
+        if targets.get("mask") is not None:
+            ret["loss_mask"] = loss_mask
+        return ret
     if V == 1 and sync_gradients is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         out = GaussianRasterizer(views[0], return_depth=return_depth, return_alpha=return_alpha)(
@@ -333,15 +386,15 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 class _RasterizeClouds(torch.autograd.Function):
     """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha).  Outputs per
-    cloud: (color, feature image, radii, depth, alpha), or with targets (loss_rgb, loss_embed, color, feature image, radii) with gradients through
-    the two losses only."""
+    cloud: (color, feature image, radii, depth, alpha), or with targets (loss_rgb, loss_embed, color, feature image, radii,
+    loss_depth, loss_mask, depth_pixels) with gradients through the losses only."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
         cloud_views, return_depth, targets, return_alpha = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
-        clouds, results, frozen, cots = [], [], [], []
+        clouds, results, frozen, cots, dms = [], [], [], [], []
         for b, views in enumerate(cloud_views):
             means3D, _, sh, colors, feature, opacities, scales, rotations = (_prep(t, dev) for t in flat[_CLOUD_INPUTS * b:_CLOUD_INPUTS * (b + 1)])
             V, H, W = len(views), int(views[0].image_height), int(views[0].image_width)
@@ -361,7 +414,9 @@ class _RasterizeClouds(torch.autograd.Function):
                 cot_emb = torch.empty((V, F, H, W), **opts) if t_emb is not None else (torch.zeros((V, F, H, W), **opts) if F else None)
                 loss_acc = torch.empty((V, 2), **opts)
                 c["loss_heads"] = (t_rgb, t_emb, cot_rgb, cot_emb, loss_acc)
+                c["depth_mask"] = _depth_mask_heads(targets[b].get("depth"), targets[b].get("mask"), V, H, W, dev, f"cloud {b}")
                 cots.append((cot_rgb, cot_emb))
+                dms.append(c["depth_mask"])
             clouds.append(c)
         degree = cloud_views[0][0].sh_degree
         include = clouds[0]["feature"] is not None
@@ -376,13 +431,15 @@ class _RasterizeClouds(torch.autograd.Function):
                 loss_acc = c["loss_heads"][4]
                 loss_rgb = loss_acc[:, 0] / (3.0 * N)
                 loss_embed = 1.0 - loss_acc[:, 1] / N if c["loss_heads"][1] is not None else torch.zeros((len(c["views"]),), **opts)
-                results += [loss_rgb, loss_embed, color, feat_img if feat_img is not None else empty(), radii]
-                frozen += [radii, color] + ([feat_img] if feat_img is not None else [])
+                loss_depth, loss_mask, depth_pixels = _depth_mask_losses(c["depth_mask"], N, dev)
+                results += [loss_rgb, loss_embed, color, feat_img if feat_img is not None else empty(), radii, loss_depth, loss_mask,
+                            depth_pixels]
+                frozen += [radii, color, depth_pixels] + ([feat_img] if feat_img is not None else [])
             else:
                 results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty(),
                             alpha if alpha is not None else empty()]
                 frozen.append(radii)
-        ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots = meta, streams, degree, include, cots
+        ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots, ctx.dms = meta, streams, degree, include, cots, dms
         # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
         ctx.state = [[(o[0], o[3], o[4], o[5], o[6]) for o in co] for co in outs]
         ctx.opac_shapes = [flat[_CLOUD_INPUTS * b + 5].shape for b in range(B)]
@@ -397,7 +454,7 @@ class _RasterizeClouds(torch.autograd.Function):
         cloud_views, return_depth, targets, return_alpha = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
-        per = 5
+        per = 8 if targets is not None else 5
         clouds = []
         for b, views in enumerate(cloud_views):
             means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
@@ -410,6 +467,9 @@ class _RasterizeClouds(torch.autograd.Function):
                 z = torch.zeros((V,), dtype=torch.float32, device=dev)
                 c["cot_scale"] = torch.stack([g[0] if g[0] is not None else z, g[1] if g[1] is not None else z], 1).contiguous()
                 c["grad_color"], c["grad_feature"] = ctx.cots[b]
+                if ctx.dms[b] is not None:
+                    c["depth_mask"] = ctx.dms[b]
+                    c["depth_mask_scale"] = _depth_mask_scale(ctx.dms[b], g[5], g[6], V, dev)
             else:
                 c["grad_color"] = g[0] if g[0] is not None else torch.zeros((V, 3, H, W), dtype=torch.float32, device=dev)
                 if F:
@@ -441,7 +501,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     The clouds share the SH degree, the feature width F and the colour mode (ValueError naming the field otherwise); within a
     cloud all views share one image size, different clouds may differ.  Targets are given on all clouds or on none.
     Returns one dict per cloud with the keys and shapes render_views returns for it ("loss_rgb" / "loss_embed" with targets,
-    "depth" / "alpha" [V,H,W] when asked for).
+    and "loss_depth" / "depth_pixels" / "loss_mask" with "depth" / "mask" targets; "depth" / "alpha" [V,H,W] when asked for).
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
     dyna step, which renders the detached current features); its feature cotangents still reach its other gradients."""
     if not clouds:
@@ -492,9 +552,14 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]
         if targets is not None:
-            loss_rgb, loss_embed, color, feat_img, radii = out[5 * b:5 * b + 5]
-            ret.append({"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii,
-                        "loss_rgb": loss_rgb, "loss_embed": loss_embed})
+            loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels = out[8 * b:8 * b + 8]
+            r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii,
+                 "loss_rgb": loss_rgb, "loss_embed": loss_embed}
+            if targets[b].get("depth") is not None:
+                r["loss_depth"], r["depth_pixels"] = loss_depth, depth_pixels
+            if targets[b].get("mask") is not None:
+                r["loss_mask"] = loss_mask
+            ret.append(r)
         else:
             color, feat_img, radii, depth, alpha = out[5 * b:5 * b + 5]
             r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii}

@@ -553,7 +553,7 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None, return_alpha=False):
+                        loss_heads=None, return_alpha=False, depth_mask=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -563,7 +563,10 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     the history-based sizing of the binning state.  `loss_heads` = (target_rgb [V,3,H,W], target_embed [V,F,H,W] or None,
     cot_rgb [V,3,H,W], cot_embed [V,F,H,W] or None, loss_acc [V,2]): the forward blend's epilogue also evaluates the L2 colour
     head and the cosine embedding head against the targets (C ABI mgs_view.target_*), leaving the loss sums in loss_acc and
-    the cotangent planes ready for rasterize_views_backward_raw."""
+    the cotangent planes ready for rasterize_views_backward_raw.  `depth_mask` = (target_depth [V,H,W] or None, target_mask
+    [V,H,W] or None, cot_depth, cot_alpha_depth (both [V,H,W], with target_depth), cot_alpha_mask [V,H,W] (with target_mask),
+    loss_acc [V,3]), with `loss_heads` only: the same epilogue also evaluates the expected-depth L1 head and the alpha mask
+    head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -592,9 +595,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                        debug)
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
+        darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
+            if darr is not None:
+                _fill_depth_mask(darr[v], depth_mask, v)
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
                                  aarr[v] if return_alpha else None)
@@ -604,12 +610,27 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             outs.append(o)
         rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
-        if return_alpha:
+        if darr is not None:
+            _b.check(L.mgs_forward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_forward_views_depth_mask")
+        elif return_alpha:
             _b.check(L.mgs_forward_views_alpha(V, arr, aarr, *rest), "mgs_forward_views_alpha")
         else:
             _b.check(L.mgs_forward_views(V, arr, *rest), "mgs_forward_views")
         _track_status(outs, keys, status, main, capacities is None and not capturing)
     return outs, streams
+
+
+def _fill_depth_mask(wd, depth_mask, v, scale=None):
+    """Fills view v's mgs_view_depth_mask `wd` from a `depth_mask` tuple of rasterize_views_raw (and, for the backward, the
+    upstream gradients `scale` [V,2])."""
+    t_depth, t_mask, c_depth, c_alpha_depth, c_alpha_mask, acc = depth_mask
+    if t_depth is not None:
+        wd.target_depth, wd.cot_depth, wd.cot_alpha_depth = _ptr(t_depth[v]), _ptr(c_depth[v]), _ptr(c_alpha_depth[v])
+    if t_mask is not None:
+        wd.target_mask, wd.cot_alpha_mask = _ptr(t_mask[v]), _ptr(c_alpha_mask[v])
+    wd.loss_acc = _ptr(acc[v])
+    if scale is not None:
+        wd.cot_scale = scale.data_ptr() + 8 * v
 
 
 def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None):
@@ -664,7 +685,7 @@ def _track_status(outs, keys, status, main, pending):
 def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_feature, means3D, colors, language_feature, scales,
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
-                                 cot_scale=None, grads_alpha=None):
+                                 cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -674,7 +695,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     (multi-GPU: start its all-reduce there; it overlaps the per-Gaussian kernel).  `cot_scale` [V,2] (device): upstream
     gradients of the fused loss heads' two scalars per view, multiplied onto the colour / feature cotangent planes as they
     are loaded.  `grads_alpha` (per view [H,W] or None): cotangents of the alpha planes of a `return_alpha` forward.  The
-    caller's current stream holds the result on return."""
+    caller's current stream holds the result on return.  `depth_mask`: the tuple given to the forward, whose cotangent planes
+    are read back with `depth_mask_scale` [V,2] (device; the upstream gradients {g_depth, g_mask} of the depth and mask losses,
+    or None for 1)."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -710,9 +733,13 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     with torch.cuda.device(dev):
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if grads_alpha is not None else None
-        keep = []
+        darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
+        dscale = _prep(depth_mask_scale, dev)
+        keep = [dscale]
         for v, s in enumerate(views):
             w = arr[v]
+            if darr is not None:
+                _fill_depth_mask(darr[v], depth_mask, v, dscale)
             if aarr is not None:
                 ga = _prep(grads_alpha[v], dev)
                 aarr[v].dL_dpix_alpha = _ptr(ga)
@@ -730,7 +757,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if aarr is not None:
+            if darr is not None:
+                _b.check(L.mgs_backward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_backward_views_depth_mask")
+            elif aarr is not None:
                 _b.check(L.mgs_backward_views_alpha(V, arr, aarr, *rest), "mgs_backward_views_alpha")
             else:
                 _b.check(L.mgs_backward_views(V, arr, *rest), "mgs_backward_views")
@@ -791,7 +820,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
-    "capacities" as rasterize_views_raw takes them.  degree, F, the colour and covariance modes are shared.  `return_alpha`
+    "capacities" as rasterize_views_raw takes them, and "depth_mask" (with "loss_heads") as its `depth_mask`.  degree, F, the
+    colour and covariance modes are shared.  `return_alpha`
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
     Capacity history is kept per (device, P, W, H, cloud slot, view slot)."""
@@ -823,6 +853,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                            d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug)
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
+        darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
         status = _status_slots(V)
         keep, outs = [], []
         for b, (c, d) in enumerate(zip(clouds, pc)):
@@ -836,6 +867,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
             for v, s in enumerate(c["views"]):
                 g = offsets[b] + v
                 cap = int(caps[v]) if caps is not None else _CAPACITY[keys[b][v]]
+                if c.get("depth_mask") is not None:
+                    _fill_depth_mask(darr[g], c["depth_mask"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
                                       c.get("loss_heads"), aarr[g] if return_alpha else None)
                 arr[g].status = status.data_ptr() + 8 * g
@@ -844,7 +877,9 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 cloud_outs.append(o)
             outs.append(cloud_outs)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if return_alpha:
+        if darr is not None:
+            _b.check(L.mgs_forward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_forward_clouds_depth_mask")
+        elif return_alpha:
             _b.check(L.mgs_forward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_forward_clouds_alpha")
         else:
             _b.check(L.mgs_forward_clouds(B, carr, offs, arr, *rest), "mgs_forward_clouds")
@@ -859,7 +894,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
     plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
     "grad_alpha" [V_b,H,W] (the cotangent of a `return_alpha` forward's alpha planes),
-    "cot_scale" [V_b,2] (device; the loss heads' upstream gradients) and "want_feature" (default True; False: the cloud's
+    "cot_scale" [V_b,2] (device; the loss heads' upstream gradients), "depth_mask" and "depth_mask_scale" [V_b,2] (the
+    forward's depth / mask heads and their upstream gradients, as rasterize_views_backward_raw takes them) and "want_feature" (default True; False: the cloud's
     dL_dfeature is not computed, but its feature cotangents still reach the other gradients).  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
     dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed)."""
@@ -877,6 +913,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     with torch.cuda.device(dev):
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if any(c.get("grad_alpha") is not None for c in clouds) else None
+        darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
         keep = []
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
@@ -899,9 +936,13 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             k.dL_dfeature, k.dL_dcov3D, k.dL_dsh = _ptr(gr["dL_dfeature"]), _ptr(gr["dL_dcov3D"]), _ptr(gr["dL_dsh"])
             k.dL_dscale, k.dL_drot = _ptr(gr["dL_dscales"]), _ptr(gr["dL_drotations"])
             cot = _prep(c.get("cot_scale"), dev)
+            dscale = _prep(c.get("depth_mask_scale"), dev)
+            keep.append(dscale)
             for v, s in enumerate(c["views"]):
                 g = offsets[b] + v
                 w = arr[g]
+                if c.get("depth_mask") is not None:
+                    _fill_depth_mask(darr[g], c["depth_mask"], v, dscale)
                 keep.append(_backward_view(L, w, s, outs[b][v], dev, P, c["grad_color"][v],
                                            c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
                                            c["grad_depth"][v] if c.get("grad_depth") is not None else None))
@@ -915,7 +956,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     w.cot_scale = cot.data_ptr() + 8 * v
             keep.append(cot)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if aarr is not None:
+        if darr is not None:
+            _b.check(L.mgs_backward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_backward_clouds_depth_mask")
+        elif aarr is not None:
             _b.check(L.mgs_backward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_backward_clouds_alpha")
         else:
             _b.check(L.mgs_backward_clouds(B, carr, offs, arr, *rest), "mgs_backward_clouds")
