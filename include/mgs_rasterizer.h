@@ -441,6 +441,64 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
 	int debug, void* join_stream);
 
+/*
+ * Anti-aliased projection (Mip-Splatting's "2D filter"; the `antialiasing` setting of the 3DGS authors' current rasterizer,
+ * gsplat's rasterize_mode="antialiased"; INTEGRATION.md §5).  The projection dilates every screen-space covariance by
+ * 0.3 px^2 (Sigma' = Sigma + 0.3 I, as the reference does); with antialiasing = 1 it also scales the Gaussian's opacity by
+ *   s = sqrt(max(2.5e-5, det Sigma / det Sigma'))
+ * so that the dilated splat carries the energy of the undilated one: the blend sees o_eff = o s.  The conic, radius, screen
+ * mean, depth, tiles, instance count and sort keys are those of antialiasing = 0, bit for bit.  The backward chains dL/do_eff
+ * to dL/do and, through s, to the covariance (and so to means, scales, rotations or cov3D).
+ * The calls below are the _depth_mask calls with one more argument, `antialiasing` (0 or 1); the _depth_mask calls are these
+ * with 0.  Pass the same value to the forward and the backward: the backward reads o_eff back from the forward's geometry
+ * state.  Any other value returns MGS_ERR_INVALID_ARG before anything is enqueued.
+ */
+int mgs_forward_views_aa(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_aa(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
+	int accumulate, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

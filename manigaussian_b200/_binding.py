@@ -113,6 +113,9 @@ def lib():
         # ... and with the depth / mask heads (one ViewDepthMask per view, or NULL) after the alpha planes
         getattr(L, name + "_depth_mask").restype = C.c_int
         getattr(L, name + "_depth_mask").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask)] + at[k:]
+        # ... and with the anti-aliased projection switch (int antialiasing) after the depth / mask heads
+        getattr(L, name + "_aa").restype = C.c_int
+        getattr(L, name + "_aa").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_mark_visible.restype = C.c_int
@@ -146,6 +149,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_alpha", "mgs_backward_views_alpha", "mgs_forward_clouds_alpha", "mgs_backward_clouds_alpha",
     "mgs_forward_views_depth_mask", "mgs_backward_views_depth_mask", "mgs_forward_clouds_depth_mask",
     "mgs_backward_clouds_depth_mask",
+    "mgs_forward_views_aa", "mgs_backward_views_aa", "mgs_forward_clouds_aa", "mgs_backward_clouds_aa",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

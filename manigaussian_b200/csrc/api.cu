@@ -320,6 +320,7 @@ struct Cloud {
 	int P, D, M, F;
 	const float* means3D; const float* shs; const float* colors_precomp; const float* feature; const float* opacities;
 	const float* scales; float scale_modifier; const float* rotations; const float* cov3D_precomp;
+	int antialias;  // 1: the anti-aliased projection (opacity compensation); 0 where an initialiser leaves it out
 };
 
 // a view's tile grid and its state buffers, carved (pointers into a buffer the view does not provide are never used)
@@ -360,6 +361,7 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, int debug)
 	pa.radii = w.radii; pa.means2D = geom.means2D; pa.depths = geom.depths; pa.cov3D = geom.cov3D; pa.rgbd = geom.rgbd;
 	pa.conic_opacity = geom.conic_opacity; pa.extent = geom.extent; pa.clamped = geom.clamped; pa.tiles_touched = geom.tiles_touched;
 	pa.iota = geom.iota;
+	pa.antialias = c.antialias;
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
 
@@ -561,6 +563,8 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		pb.dL_dconic = pb.accumulate ? nullptr : dL_dconic;
 		for (int u = 0; u < pb.V; u++)
 			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
+		pb.antialias = c.antialias;
+		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); }
 		MGS_STAGE("project_bwd");
 	}
@@ -618,10 +622,16 @@ static int check_clouds(int B, const mgs_cloud* clouds, const int* view_offsets,
 	return 0;
 }
 
-static Cloud cloud_of(const mgs_cloud& k, int D, int M, int F, float scale_modifier)
+static Cloud cloud_of(const mgs_cloud& k, int D, int M, int F, float scale_modifier, int antialias)
 {
 	return Cloud{ k.P, D, M, k.feature ? F : 0, k.means3D, k.shs, k.colors_precomp, k.feature, k.opacities, k.scales, scale_modifier,
-		k.rotations, k.cov3D_precomp };
+		k.rotations, k.cov3D_precomp, antialias };
+}
+
+static int check_antialias(int antialiasing)
+{
+	if (antialiasing != 0 && antialiasing != 1) return fail(MGS_ERR_INVALID_ARG, "antialiasing must be 0 or 1");
+	return 0;
 }
 
 }  // namespace mgs
@@ -751,7 +761,19 @@ int mgs_forward_views_depth_mask(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_aa(V, views, alpha, depth_mask, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities,
+		scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_aa(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
@@ -763,7 +785,8 @@ int mgs_forward_views_depth_mask(
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 		if (rc < 0) return rc;
 	}
-	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp };
+	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+		antialiasing };
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	int rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
@@ -824,6 +847,20 @@ int mgs_backward_views_depth_mask(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_aa(V, views, alpha, depth_mask, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
+		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot,
+		shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_aa(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
@@ -835,7 +872,8 @@ int mgs_backward_views_depth_mask(
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 		if (rc < 0) return rc;
 	}
-	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp };
+	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
+		antialiasing };
 	return backward_views(V, views, alpha, depth_mask, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
@@ -857,7 +895,16 @@ int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vie
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int prefiltered,
 	int debug, void* join_stream)
 {
+	return mgs_forward_clouds_aa(B, clouds, view_offsets, views, alpha, depth_mask, 0, D, M, F, scale_modifier, prefiltered, debug,
+		join_stream);
+}
+
+int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -880,7 +927,7 @@ int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vie
 	// stage by stage across the views of every cloud, as in mgs_forward_views
 	for (int phase = 0; phase < 3; phase++) {
 		for (int b = 0; b < B; b++) {
-			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
+			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 				rc = phase == 0 ? enqueue_project(c, views[v], debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
@@ -909,6 +956,15 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
 	int debug, void* join_stream)
 {
+	return mgs_backward_clouds_aa(B, clouds, view_offsets, views, alpha, depth_mask, 0, D, M, F, scale_modifier, accumulate, debug,
+		join_stream);
+}
+
+int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
+	int accumulate, int debug, void* join_stream)
+{
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -934,7 +990,7 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
 	rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
 	for (int b = 0; b < B; b++) {
-		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier);
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
 				depth_mask ? depth_mask + v : nullptr, debug);
@@ -948,7 +1004,7 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
 	// spans launches, and its later launches add to what the earlier ones wrote
 	const cudaStream_t st = join;
 	ProjectBwdCloudsArgs pb{};
-	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier;
+	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
 	int nv = 0;  // views in pb
 	auto flush = [&]() -> int {
 		if (pb.B == 0) return 0;
@@ -974,7 +1030,10 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
 			pc.accumulate = (accumulate || v0 > view_offsets[b]) ? 1 : 0;
 			pc.dL_dmean3D = k.dL_dmean3D; pc.dL_dopacity = k.dL_dopacity; pc.dL_dcolor = k.dL_dcolor; pc.dL_dcov3D = k.dL_dcov3D;
 			pc.dL_dsh = k.shs ? k.dL_dsh : nullptr; pc.dL_dscale = have_sr ? k.dL_dscale : nullptr; pc.dL_drot = have_sr ? k.dL_drot : nullptr;
-			for (int u = 0; u < n; u++) pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
+			for (int u = 0; u < n; u++) {
+				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
+				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
+			}
 			nv += n;
 		}
 	}

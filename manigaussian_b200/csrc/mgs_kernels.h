@@ -35,6 +35,8 @@ struct ProjectFwdArgs {
 	uint8_t* clamped;  // 3 bits per Gaussian
 	uint32_t* tiles_touched;
 	uint32_t* iota;    // identity permutation (values of the depth sort)
+	int antialias;     // 1: opacity compensation for the 0.3 px^2 low-pass (launcher picks the instantiation; last, so the
+	                   // other members keep their parameter offsets)
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -68,6 +70,11 @@ struct ProjectBwdViewsArgs {
 	float* dL_drot;     // [P,4] nullable
 	float* dL_dconic;   // [P,4] nullable; view 0 only (single-view callers)
 	ProjectBwdView view[MAX_BWD_VIEWS];
+	// anti-aliased mode only (the launcher picks the instantiation): view u's conic_opacity [P] from its geometry state, whose
+	// .w is the compensated opacity o_eff the blend saw.  Kept out of ProjectBwdView and behind every other member so that the
+	// AA = false kernels read their parameters at the same offsets and strides as before the mode existed.
+	int antialias;
+	const float4* conic_opacity[MAX_BWD_VIEWS];
 };
 // the same chain rule for several clouds in one launch: cloud c sums views view[view0 .. view0 + V) of the launch
 // (every cloud has a view, so MAX_BWD_VIEWS clouds at most); dL_dmean2D per view only, no dL_dconic
@@ -87,6 +94,8 @@ struct ProjectBwdCloudsArgs {
 	float scale_modifier;
 	ProjectBwdCloud cloud[MAX_BWD_VIEWS];
 	ProjectBwdView view[MAX_BWD_VIEWS];
+	int antialias;                                 // as in ProjectBwdViewsArgs
+	const float4* conic_opacity[MAX_BWD_VIEWS];    // per view of the launch, AA only
 };
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 

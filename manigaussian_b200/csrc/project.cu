@@ -105,6 +105,10 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 	clamped_bits[idx] = bits;
 }
 
+// AA: the anti-aliased mode (Mip-Splatting's 2D filter, DESIGN.md section 4): the opacity is scaled by
+// s = sqrt(max(2.5e-5, det(Sigma) / det(Sigma + 0.3 I))), so that the dilated splat carries the energy of the undilated one.
+// Only conic_opacity.w and the extent's opacity change; the conic, radius, tiles and keys are those of AA = false.
+template <bool AA>
 __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -135,6 +139,8 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 
 	Cov2DTerms ct = cov2d_terms(p_orig, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, a.viewmatrix);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
+	float det0 = 0.f;  // det of the screen-space covariance before the low-pass (AA only)
+	if (AA) det0 = fmaf(-cov.m[0][1], cov.m[0][1], cov.m[0][0] * cov.m[1][1]);  // explicit fma: rounding independent of contraction
 	cov.m[0][0] += 0.3f;  // low-pass (forward.cu:111-112)
 	cov.m[1][1] += 0.3f;
 	const float cx = cov.m[0][0], cy = cov.m[0][1], cz = cov.m[1][1];
@@ -161,7 +167,8 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	}
 	a.rgbd[idx] = make_float4(c[0], c[1], c[2], p_view.z);  // blend channel quad 0 (depth rides as a channel)
 
-	const float opacity = a.opacities[idx];
+	float opacity = a.opacities[idx];
+	if (AA) opacity *= sqrtf(max(2.5e-5f, det0 / det));  // the blend sees o_eff = o s
 	out_radius = (int)my_radius;
 	out_tiles = (rmax.y - rmin.y) * (rmax.x - rmin.x);
 	a.depths[idx] = p_view.z;
@@ -198,7 +205,9 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* m
 
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
-	if (a.P > 0) project_fwd_kernel<<<ceil_div(a.P, 256), 256, 0, s>>>(a);
+	if (a.P <= 0) return;
+	if (a.antialias) project_fwd_kernel<true><<<ceil_div(a.P, 256), 256, 0, s>>>(a);
+	else project_fwd_kernel<false><<<ceil_div(a.P, 256), 256, 0, s>>>(a);
 }
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s)
 {

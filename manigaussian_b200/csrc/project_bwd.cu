@@ -46,7 +46,12 @@ __device__ __forceinline__ float dot3(const float* u, const float* v) { return u
 #endif
 // The chain rule of Gaussian idx over the views a.view[0 .. a.V).  Args: ProjectBwdViewsArgs, or CloudBwd (one cloud of a
 // multi-cloud launch) -- the same member names.
-template <int NSH, class Args>
+//
+// AA (anti-aliased mode): the blend saw o_eff = o s, s = sqrt(max(2.5e-5, r)), r = d0 / d1, d0 = det(S' - 0.3 I), d1 = det S'.
+// The record's opacity gradient g is dL/do_eff, so dL/do = sum_v s_v g_v, and where r > 2.5e-5 the view's dL/dS' gains
+// g o ds = g o_eff (grad d0 / d0 - grad d1 / d1) / 2 (s^2 = r there): no raw opacity and no square root beyond s itself.
+// o_eff is read back from the view's conic_opacity.w; s is recomputed from S'.
+template <int NSH, bool AA, class Args>
 __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx)
 {
 	const float p[3] = { a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2] };
@@ -97,6 +102,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		const float4* gb = reinterpret_cast<const float4*>(w.gb + (size_t)idx * GB_STRIDE);
 		const float4 g0 = gb[0], g1 = gb[1], g2 = gb[2];
 		const uint8_t cl = sh ? w.clamped[idx] : (uint8_t)0;
+		const float o_eff = AA ? a.conic_opacity[v][idx].w : 0.f;
 		const bool live = w.radii[idx] > 0;
 		float dm[2] = { 0.f, 0.f };
 		if (live) {
@@ -104,7 +110,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float gA = g0.z, gB = g0.w, gC = g1.x;        // dL/dconic (xx, xy halved, yy)
 			const float dcol[3] = { g1.z, g1.w, g2.x };
 			const float ddepth = g2.y;
-			gop += g1.y;
+			if (!AA) gop += g1.y;
 			gcol[0] += dcol[0]; gcol[1] += dcol[1]; gcol[2] += dcol[2];
 			if (a.dL_dconic && v == 0) {
 				float* o = a.dL_dconic + 4 * (size_t)idx;
@@ -137,7 +143,21 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float wgt = 1.0f / (det * det + 0.0000001f);
 			// H = -w adj(S') G adj(S')
 			const float e00 = cc * gA - cb * gB, e01 = cc * gB - cb * gC, e10 = ca * gB - cb * gA, e11 = ca * gC - cb * gB;
-			const float H00 = -wgt * (e00 * cc - e01 * cb), H01 = -wgt * (e01 * ca - e00 * cb), H11 = -wgt * (e11 * ca - e10 * cb);
+			float H00 = -wgt * (e00 * cc - e01 * cb), H01 = -wgt * (e01 * ca - e00 * cb), H11 = -wgt * (e11 * ca - e10 * cb);
+			if (AA) {
+				// opacity compensation: grad d0 = (c0, -2b, a0), grad d1 = (c, -2b, a) w.r.t. (a, b, c), b one variable;
+				// H01 is the gradient w.r.t. ONE off-diagonal entry, so it takes half of the b term
+				const float a0 = ca - 0.3f, c0 = cc - 0.3f;
+				const float d0 = fmaf(-cb, cb, a0 * c0);
+				const float r = d0 / det;
+				gop += sqrtf(fmaxf(2.5e-5f, r)) * g1.y;
+				if (r > 2.5e-5f) {
+					const float k = 0.5f * g1.y * o_eff, i0 = 1.0f / d0, i1 = 1.0f / det;
+					H00 += k * (c0 * i0 - cc * i1);
+					H11 += k * (a0 * i0 - ca * i1);
+					H01 += k * cb * (i1 - i0);
+				}
+			}
 			// dL/dS += M^T H M
 			float h0[3], h1[3];
 #pragma unroll
@@ -274,12 +294,12 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 	}
 }
 
-template <int NSH, int MIN_BLOCKS>
+template <int NSH, int MIN_BLOCKS, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= a.P) return;
-	project_bwd_gaussian<NSH>(a, idx);
+	project_bwd_gaussian<NSH, AA>(a, idx);
 }
 
 namespace {
@@ -294,11 +314,12 @@ struct CloudBwd {
 	float* dL_dmean3D; float* dL_dopacity; float* dL_dcolor; float* dL_dcov3D; float* dL_dsh; float* dL_dscale; float* dL_drot;
 	static constexpr float* dL_dconic = nullptr;
 	const ProjectBwdView* view;
+	const float4* const* conic_opacity;  // AA only
 };
 }  // namespace
 
 // several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
-template <int NSH, int MIN_BLOCKS>
+template <int NSH, int MIN_BLOCKS, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
 {
 	int c = 0;
@@ -307,8 +328,9 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	const int idx = ((int)blockIdx.x - cl.block0) * blockDim.x + threadIdx.x;
 	if (idx >= cl.P) return;
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
-		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0 };
-	project_bwd_gaussian<NSH>(cb, idx);
+		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
+		AA ? a.conic_opacity + cl.view0 : nullptr };
+	project_bwd_gaussian<NSH, AA>(cb, idx);
 }
 
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
@@ -316,9 +338,16 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	if (a.P <= 0 || a.V <= 0) return;
 	const int grid = ceil_div(a.P, 128);
 	const int deg = a.shs ? a.D : 0;
-	if (deg <= 1) project_bwd_views_kernel<12, MGS_PBWD_MINB><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_views_kernel<27, 4><<<grid, 128, 0, s>>>(a);
-	else project_bwd_views_kernel<48, 3><<<grid, 128, 0, s>>>(a);
+	if (a.antialias) {
+		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
+		if (deg <= 1) project_bwd_views_kernel<12, 4, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, 4, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_kernel<48, 3, true><<<grid, 128, 0, s>>>(a);
+		return;
+	}
+	if (deg <= 1) project_bwd_views_kernel<12, MGS_PBWD_MINB, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_views_kernel<27, 4, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_views_kernel<48, 3, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
@@ -334,9 +363,15 @@ void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 	const int deg = sh ? a.D : 0;
 	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
 	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
-	if (deg <= 1) project_bwd_clouds_kernel<12, 4><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_clouds_kernel<27, 4><<<grid, 128, 0, s>>>(a);
-	else project_bwd_clouds_kernel<48, 3><<<grid, 128, 0, s>>>(a);
+	if (a.antialias) {
+		if (deg <= 1) project_bwd_clouds_kernel<12, 4, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_kernel<27, 4, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_clouds_kernel<48, 3, true><<<grid, 128, 0, s>>>(a);
+		return;
+	}
+	if (deg <= 1) project_bwd_clouds_kernel<12, 4, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_clouds_kernel<27, 4, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_clouds_kernel<48, 3, false><<<grid, 128, 0, s>>>(a);
 }
 
 }  // namespace mgs

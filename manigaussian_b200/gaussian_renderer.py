@@ -72,10 +72,12 @@ def _camera_scalars(nv, idx):
 
 
 def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=None, features_color=None,
-           features_language=None, return_depth=False, return_alpha=False):
+           features_language=None, return_depth=False, return_alpha=False, antialiasing=False):
     """Render view `idx` of data['novel_view'].  Same arguments and result as the reference's render(); with
     return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended, no background term), with
-    return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth)."""
+    return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth).
+    antialiasing=True renders with the anti-aliased projection (opacity compensation for the 0.3 px^2 dilation,
+    INTEGRATION.md §5)."""
     device = pts_xyz.device
     nv = data["novel_view"]
     bg = _background(bg_color, device)
@@ -90,7 +92,7 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
         image_height=H, image_width=W, tanfovx=tanfovx, tanfovy=tanfovy, bg=bg, scale_modifier=1.0,
         viewmatrix=nv["world_view_transform"][idx], projmatrix=nv["full_proj_transform"][idx],
         sh_degree=3 if features_color is None else 1, campos=nv["camera_center"][idx], prefiltered=False, debug=False,
-        include_feature=(features_language is not None))
+        include_feature=(features_language is not None), antialiasing=bool(antialiasing))
     rasterizer = GaussianRasterizer(raster_settings=raster_settings, return_depth=return_depth, return_alpha=return_alpha)
     shs, colors_precomp = None, None
     if features_color is not None:
@@ -112,7 +114,7 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
-                group):
+                group, antialiasing=False):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -131,12 +133,12 @@ class _RasterizeViews(torch.autograd.Function):
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
                                             debug=views[0].debug, out_buffers=(color, feat_img, depth, alpha),
-                                            return_alpha=return_alpha)
+                                            return_alpha=return_alpha, antialiasing=antialiasing)
         main = torch.cuda.current_stream(dev)
         for st in streams:
             main.wait_stream(st)
         radii = torch.stack([o[3] for o in outs])
-        ctx.views, ctx.streams, ctx.group = views, streams, group
+        ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
         ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
@@ -172,7 +174,8 @@ class _RasterizeViews(torch.autograd.Function):
                                      feature if ctx.include else None, scales, rotations, views[0].scale_modifier, None,
                                      sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
                                      accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
-                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None)
+                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
+                                     antialiasing=ctx.antialiasing)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
             # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields
@@ -180,7 +183,7 @@ class _RasterizeViews(torch.autograd.Function):
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None)
 
 
 def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
@@ -227,7 +230,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
-                target_depth=None, target_mask=None):
+                target_depth=None, target_mask=None, antialiasing=False):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -252,12 +255,13 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, debug=views[0].debug,
                                             out_buffers=(color, feat_img, None),
-                                            loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm)
+                                            loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm,
+                                            antialiasing=antialiasing)
         N = float(H * W)
         loss_rgb = loss_acc[:, 0] / (3.0 * N)
         loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
         radii = torch.stack([o[3] for o in outs])
-        ctx.views, ctx.streams, ctx.group = views, streams, group
+        ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
         # capacity, radii and the three state buffers per view -- never the images: they are views of this node's outputs, and an
         # output kept on ctx is a reference cycle (output -> grad_fn -> ctx -> output) that leaks the whole step
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]
@@ -294,18 +298,19 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                      accumulate_into=pk.views, means2D_per_view=m2d, cot_scale=scale,
                                      after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
                                      depth_mask=ctx.dm,
-                                     depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None)
+                                     depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None,
+                                     antialiasing=ctx.antialiasing)
         if ctx.group is not None:
             pk.all_reduce_finish(grp)
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None)
 
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
-                 targets=None, return_alpha=False):
+                 targets=None, return_alpha=False, antialiasing=False):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -324,6 +329,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     the pixels).
     return_alpha: also return "alpha" [V,H,W], the accumulated opacity 1 - final_T (differentiable; depth / alpha is the
     expected depth).
+    antialiasing: render with the anti-aliased projection (opacity compensation for the 0.3 px^2 dilation, INTEGRATION.md
+    §5); also on when the given settings carry antialiasing=True.  Combines with every option above.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -337,6 +344,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
     if not views:
         raise ValueError("render_views needs at least one view")
+    aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for s in views)
     if features_color is None and pts_rgb is None:
         raise ValueError("Please provide excatly one of either SHs or precomputed colors!")
     feat = None
@@ -351,7 +359,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
             raise ValueError("targets and return_alpha cannot be combined")
         loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"))
+            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"), aa)
         ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
                "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
         if targets.get("depth") is not None:
@@ -361,7 +369,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         return ret
     if V == 1 and sync_gradients is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
-        out = GaussianRasterizer(views[0], return_depth=return_depth, return_alpha=return_alpha)(
+        st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True) if aa else views[0]
+        out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
             colors_precomp=pts_rgb if features_color is None else None, language_feature_precomp=feat, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=None)
@@ -371,7 +380,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     else:
         color, feat_img, radii, depth, alpha = _RasterizeViews.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients)
+            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
@@ -391,7 +400,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets, return_alpha = meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
         clouds, results, frozen, cots, dms = [], [], [], [], []
@@ -421,7 +430,7 @@ class _RasterizeClouds(torch.autograd.Function):
         degree = cloud_views[0][0].sh_degree
         include = clouds[0]["feature"] is not None
         outs, streams = rasterize_clouds_raw(clouds, degree, include, cloud_views[0][0].scale_modifier, return_depth=return_depth,
-                                             debug=cloud_views[0][0].debug, return_alpha=return_alpha)
+                                             debug=cloud_views[0][0].debug, return_alpha=return_alpha, antialiasing=antialiasing)
         for b, c in enumerate(clouds):
             color, feat_img, depth, alpha = c["out_buffers"]
             radii = torch.stack([o[3] for o in outs[b]])
@@ -451,7 +460,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets, return_alpha = ctx.meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
         per = 8 if targets is not None else 5
@@ -482,7 +491,7 @@ class _RasterizeClouds(torch.autograd.Function):
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
         res = rasterize_clouds_backward_raw(clouds, outs, ctx.streams, ctx.degree, ctx.include, cloud_views[0][0].scale_modifier,
-                                            debug=cloud_views[0][0].debug)
+                                            debug=cloud_views[0][0].debug, antialiasing=antialiasing)
         ret = [None]
         for b, r in enumerate(res):
             P = clouds[b]["means3D"].shape[0]
@@ -492,7 +501,8 @@ class _RasterizeClouds(torch.autograd.Function):
         return tuple(ret)
 
 
-def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False):
+def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False,
+                  antialiasing=False):
     """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
     next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
 
@@ -503,7 +513,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     Returns one dict per cloud with the keys and shapes render_views returns for it ("loss_rgb" / "loss_embed" with targets,
     and "loss_depth" / "depth_pixels" / "loss_mask" with "depth" / "mask" targets; "depth" / "alpha" [V,H,W] when asked for).
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
-    dyna step, which renders the detached current features); its feature cotangents still reach its other gradients."""
+    dyna step, which renders the detached current features); its feature cotangents still reach its other gradients.
+    antialiasing: every cloud renders with the anti-aliased projection, as in render_views."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
     with_targets = [c.get("targets") is not None for c in clouds]
@@ -547,7 +558,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         flat += [c["pts_xyz"], vsps[-1], c.get("features_color"), c.get("pts_rgb") if c.get("features_color") is None else None, f,
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
-    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha)), *flat)
+    aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for views in cloud_views for s in views)
+    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa), *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]

@@ -272,21 +272,25 @@ class _RasterizeGaussians(torch.autograd.Function):
                 s.sh_degree, s.campos, s.prefiltered, s.debug, s.include_feature)
         ctx.async_view = None
         views_path = means3D.is_cuda and means3D.size(0) > 0
+        aa = bool(getattr(s, "antialiasing", False))
+        ctx.antialiasing = aa
         alpha = None
-        if return_alpha and views_path:
-            # the alpha plane exists on the multi-view entry points only: debug renders take them too, with the snapshot dump
+        if (return_alpha or aa) and views_path:
+            # the alpha plane and the anti-aliased projection exist on the multi-view entry points only: debug renders take
+            # them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
                                                     rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
-                                                    return_depth=return_depth, debug=s.debug, return_alpha=True)
+                                                    return_depth=return_depth, debug=s.debug, return_alpha=return_alpha,
+                                                    antialiasing=aa)
             except Exception as ex:
                 if s.debug:
                     torch.save(cpu_args, "snapshot_fw.dump")
                     print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
                 raise ex
             out = outs[0]
-            alpha = out[-1]
+            alpha = out[-1] if return_alpha else None
             ctx.async_view = (int(out[0]), streams)  # as below: never the outputs themselves
         elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
@@ -343,13 +347,13 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.async_view is not None:
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
-            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and ctx.return_alpha) else None
+            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.antialiasing)) else None
             try:
                 grads = rasterize_views_backward_raw(
                     [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
                     colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
                     s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None, debug=s.debug,
-                    grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None)
+                    grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -377,7 +381,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                 _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None)
 
 
-class GaussianRasterizationSettings(NamedTuple):
+class _Settings(NamedTuple):
     image_height: int
     image_width: int
     tanfovx: float
@@ -391,6 +395,32 @@ class GaussianRasterizationSettings(NamedTuple):
     prefiltered: bool
     debug: bool
     include_feature: bool
+
+
+class GaussianRasterizationSettings(_Settings):
+    """The reference's 13 fields (DGR/diff_gaussian_rasterization/__init__.py:166-179) and a 14th argument, `antialiasing`
+    (default False; positional after include_feature, or by keyword): the anti-aliased projection of the 3DGS authors'
+    current rasterizer (Mip-Splatting's 2D filter; INTEGRATION.md §5).  `antialiasing` is an attribute, not a tuple field:
+    the settings still unpack into the reference's own 13-field NamedTuple, and `_fields` is the reference's."""
+    antialiasing = False
+
+    def __new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix, sh_degree, campos,
+                prefiltered, debug, include_feature, antialiasing=False):
+        self = super().__new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix,
+                               sh_degree, campos, prefiltered, debug, include_feature)
+        self.antialiasing = bool(antialiasing)
+        return self
+
+    @classmethod
+    def _make(cls, iterable):
+        return cls(*iterable)
+
+    def _replace(self, **kw):
+        aa = kw.pop("antialiasing", self.antialiasing)
+        return type(self)(*super()._replace(**kw), antialiasing=aa)
+
+    def __repr__(self):
+        return super().__repr__()[:-1] + f", antialiasing={self.antialiasing})"
 
 
 class GaussianRasterizer(nn.Module):
@@ -553,7 +583,7 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None, return_alpha=False, depth_mask=None):
+                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -566,7 +596,8 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     the cotangent planes ready for rasterize_views_backward_raw.  `depth_mask` = (target_depth [V,H,W] or None, target_mask
     [V,H,W] or None, cot_depth, cot_alpha_depth (both [V,H,W], with target_depth), cot_alpha_mask [V,H,W] (with target_mask),
     loss_acc [V,3]), with `loss_heads` only: the same epilogue also evaluates the expected-depth L1 head and the alpha mask
-    head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc."""
+    head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc.  `antialiasing`: the
+    anti-aliased projection (C ABI mgs_forward_views_aa); pass the same value to the backward."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -610,7 +641,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             outs.append(o)
         rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
-        if darr is not None:
+        if antialiasing:
+            _b.check(L.mgs_forward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_forward_views_aa")
+        elif darr is not None:
             _b.check(L.mgs_forward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_forward_views_depth_mask")
         elif return_alpha:
             _b.check(L.mgs_forward_views_alpha(V, arr, aarr, *rest), "mgs_forward_views_alpha")
@@ -685,7 +718,7 @@ def _track_status(outs, keys, status, main, pending):
 def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_feature, means3D, colors, language_feature, scales,
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
-                                 cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None):
+                                 cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -697,7 +730,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     are loaded.  `grads_alpha` (per view [H,W] or None): cotangents of the alpha planes of a `return_alpha` forward.  The
     caller's current stream holds the result on return.  `depth_mask`: the tuple given to the forward, whose cotangent planes
     are read back with `depth_mask_scale` [V,2] (device; the upstream gradients {g_depth, g_mask} of the depth and mask losses,
-    or None for 1)."""
+    or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_backward_views_aa)."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -757,7 +790,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if darr is not None:
+            if antialiasing:
+                _b.check(L.mgs_backward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_backward_views_aa")
+            elif darr is not None:
                 _b.check(L.mgs_backward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_backward_views_depth_mask")
             elif aarr is not None:
                 _b.check(L.mgs_backward_views_alpha(V, arr, aarr, *rest), "mgs_backward_views_alpha")
@@ -816,7 +851,8 @@ def _prep_clouds(clouds, dev, include_feature):
     return out
 
 
-def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False):
+def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False,
+                         antialiasing=False):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
@@ -824,7 +860,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     colour and covariance modes are shared.  `return_alpha`
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
-    Capacity history is kept per (device, P, W, H, cloud slot, view slot)."""
+    Capacity history is kept per (device, P, W, H, cloud slot, view slot).  `antialiasing`: the anti-aliased projection for
+    every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -877,7 +914,9 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 cloud_outs.append(o)
             outs.append(cloud_outs)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if darr is not None:
+        if antialiasing:
+            _b.check(L.mgs_forward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_forward_clouds_aa")
+        elif darr is not None:
             _b.check(L.mgs_forward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_forward_clouds_depth_mask")
         elif return_alpha:
             _b.check(L.mgs_forward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_forward_clouds_alpha")
@@ -889,7 +928,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     return outs, streams
 
 
-def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False):
+def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False,
+                                  antialiasing=False):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
     plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
@@ -898,7 +938,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     forward's depth / mask heads and their upstream gradients, as rasterize_views_backward_raw takes them) and "want_feature" (default True; False: the cloud's
     dL_dfeature is not computed, but its feature cotangents still reach the other gradients).  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
-    dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed)."""
+    dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed).  `antialiasing`: the value
+    the forward was given (C ABI mgs_backward_clouds_aa)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -956,7 +997,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     w.cot_scale = cot.data_ptr() + 8 * v
             keep.append(cot)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if darr is not None:
+        if antialiasing:
+            _b.check(L.mgs_backward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_backward_clouds_aa")
+        elif darr is not None:
             _b.check(L.mgs_backward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_backward_clouds_depth_mask")
         elif aarr is not None:
             _b.check(L.mgs_backward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_backward_clouds_alpha")
