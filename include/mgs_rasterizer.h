@@ -499,10 +499,103 @@ int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offse
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
 	int accumulate, int debug, void* join_stream);
 
+/*
+ * L1 + SSIM photometric loss (no reference counterpart in the rasterizer; the objective 3DGS trains with,
+ * (1 - lambda) L1 + lambda (1 - SSIM), lambda = 0.2, from gaussian-splatting utils/loss_utils.py, copied into ManiGaussian's
+ * agents/manigaussian_bc/loss.py).  For one view, x = out_color [3,H,W] (background included, not clamped), g = target_color
+ * [3,H,W], N = 3 H W:
+ *   loss_l1 = sum |x - g| / N;  its gradient is sign(x - g) / N with sign(0) = 0;
+ *   ssim    = mean over the 3 H W entries of S, exactly the reference's _ssim with window 11 and size_average: every plane is
+ *             convolved on its own, with zero padding 5, by the 11x11 Gaussian window of sigma 1.5 (1-D weights
+ *             exp(-(i - 5)^2 / 4.5) normalised to sum 1, outer product); with G(*) that convolution, mu_x = G(*)x,
+ *             mu_g = G(*)g, sxx = G(*)x^2 - mu_x^2, sgg = G(*)g^2 - mu_g^2, sxg = G(*)(xg) - mu_x mu_g, C1 = 0.01^2,
+ *             C2 = 0.03^2: S = (2 mu_x mu_g + C1)(2 sxg + C2) / ((mu_x^2 + mu_g^2 + C1)(sxx + sgg + C2)).
+ *             The result is SSIM itself, not 1 - SSIM.
+ * Gradient with respect to x only (the target is a constant).  With A, B, C, D the four factors of S above:
+ *   dS/dmu_x = 2 mu_g (B - A) / (C D) - 2 mu_x S (1/C - 1/D),  dS/dE[x^2] = -S / D,  dS/dE[xg] = 2 A / (C D),
+ *   d ssim / dx = (G(*)dS/dmu_x + 2 x G(*)dS/dE[x^2] + g G(*)dS/dE[xg]) / N.
+ * Images smaller than the window (down to 1x1) are valid.
+ * The calls below are the _aa calls with one more argument, `ssim`: one mgs_view_ssim per view (V entries, or view_offsets[B]
+ * for clouds), or NULL for none; the _aa calls are these with ssim == NULL.  Every entry of a non-NULL array is an SSIM head.
+ * Forward: behind the view's blend, on its stream, the head reads out_color and target_color, zeroes loss_acc and adds
+ * {sum |x - g|, sum S} into loss_acc[0..1] (loss_l1 = loss_acc[0] / N, ssim = loss_acc[1] / N), and writes the unscaled
+ * partials {dS/dmu_x, dS/dE[x^2], dS/dE[xg]} of every pixel into ssim_terms [3 partials x 3 channels, H, W].
+ * Backward: before the view's blend backward, on its stream, the head writes the view's complete colour cotangent
+ *   cot_color = s_rgb dL_dpix + g_l1 sign(x - g) / N + g_ssim d ssim / dx
+ * with s_rgb = the view's cot_scale[0] (or 1) and {g_l1, g_ssim} = cot_scale of this struct (or 1); the blend backward then
+ * reads cot_color with a colour scale of 1 and the view's feature scale unchanged (the head leaves both in loss_acc[2..3]).
+ * The view's out_color and target_color must again point at the forward's image and target.  Argument errors (an entry on
+ * a view without target_color, a missing ssim_terms, loss_acc or cot_color, or, in the backward, a missing out_color)
+ * return MGS_ERR_INVALID_ARG before anything is enqueued.
+ */
+typedef struct mgs_view_ssim {
+	float* ssim_terms;             /* [9,H,W]: written by the forward, read by the backward */
+	float* loss_acc;               /* device, 4 floats: {sum |x - g|, sum S}, then the blend backward's two scales */
+	const float* cot_scale;        /* device, 2 floats {g_l1, g_ssim}, or NULL for 1 */
+	float* cot_color;              /* [3,H,W]: receives the combined colour cotangent in the backward */
+} mgs_view_ssim;
+
+int mgs_forward_views_ssim(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_ssim(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
+	int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
+	int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,
 	const float* target_feature, float* cot_color, float* cot_feature, float* loss_acc, void* stream);
+
+/* L1 + SSIM (definitions above) for V images of C planes each that already sit in device memory, x and g [V,C,H,W]; any
+ * C >= 1 works (every plane is independent; N = C H W per image) with V C <= 65535.  mgs_ssim writes ssim_terms
+ * [V,3,C,H,W] and loss_acc [V,2] = {sum |x - g|, sum S} (zeroed by the call).  mgs_ssim_backward writes cot_out [V,C,H,W] =
+ * cot_in + scale[v,0] sign(x - g) / N + scale[v,1] d ssim / dx, with scale [V,2] (device; NULL for 1) and cot_in [V,C,H,W]
+ * (NULL for 0); x, g and ssim_terms must be those of the forward. */
+int mgs_ssim(int V, int C, int H, int W, const float* x, const float* g, float* ssim_terms, float* loss_acc, void* stream);
+int mgs_ssim_backward(int V, int C, int H, int W, const float* x, const float* g, const float* ssim_terms, const float* scale,
+	const float* cot_in, float* cot_out, void* stream);
 
 /* Frustum test.  Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:24-29, rasterizer_impl.cu:141-153).
  * present: uint8 [P], 1 where view-space z > 0.2. */

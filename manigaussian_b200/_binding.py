@@ -38,6 +38,11 @@ class ViewDepthMask(C.Structure):
                                           "loss_acc", "cot_scale")]
 
 
+class ViewSsim(C.Structure):
+    """mirror of `mgs_view_ssim` (include/mgs_rasterizer.h): the optional L1 + SSIM head of one view"""
+    _fields_ = [(n, C.c_void_p) for n in ("ssim_terms", "loss_acc", "cot_scale", "cot_color")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -116,8 +121,15 @@ def lib():
         # ... and with the anti-aliased projection switch (int antialiasing) after the depth / mask heads
         getattr(L, name + "_aa").restype = C.c_int
         getattr(L, name + "_aa").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i] + at[k:]
+        # ... and with the L1 + SSIM heads (one ViewSsim per view, or NULL) after the switch
+        getattr(L, name + "_ssim").restype = C.c_int
+        getattr(L, name + "_ssim").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mgs_ssim.restype = C.c_int
+    L.mgs_ssim.argtypes = [i, i, i, i, vp, vp, vp, vp, vp]                # V C H W x g ssim_terms loss_acc stream
+    L.mgs_ssim_backward.restype = C.c_int
+    L.mgs_ssim_backward.argtypes = [i, i, i, i, vp, vp, vp, vp, vp, vp, vp]  # V C H W x g ssim_terms scale cot_in cot_out stream
     L.mgs_mark_visible.restype = C.c_int
     L.mgs_mark_visible.argtypes = [i, vp, vp, vp, vp, vp]
     L.mgs_state_array.restype = C.c_int
@@ -150,6 +162,8 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_depth_mask", "mgs_backward_views_depth_mask", "mgs_forward_clouds_depth_mask",
     "mgs_backward_clouds_depth_mask",
     "mgs_forward_views_aa", "mgs_backward_views_aa", "mgs_forward_clouds_aa", "mgs_backward_clouds_aa",
+    "mgs_forward_views_ssim", "mgs_backward_views_ssim", "mgs_forward_clouds_ssim", "mgs_backward_clouds_ssim",
+    "mgs_ssim", "mgs_ssim_backward",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

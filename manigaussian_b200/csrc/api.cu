@@ -48,7 +48,7 @@ static const bool g_trace = getenv("MGS_TRACE") != nullptr;  // diagnostic: name
 	} while (0)
 
 // ---- optional per-stage CUDA-event timing (bench.py's roofline leg); off by default, zero cost when off ----
-enum Stage { ST_PROJECT_FWD = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_SORT, ST_RANGES_PACK, ST_BLOCK_LISTS, ST_BLEND_FWD, ST_BLEND_BWD, ST_PROJECT_BWD, ST_ACTIVATE_FWD, ST_ACTIVATE_BWD, ST_COUNT };
+enum Stage { ST_PROJECT_FWD = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_SORT, ST_RANGES_PACK, ST_BLOCK_LISTS, ST_BLEND_FWD, ST_BLEND_BWD, ST_PROJECT_BWD, ST_ACTIVATE_FWD, ST_ACTIVATE_BWD, ST_SSIM_FWD, ST_SSIM_BWD, ST_COUNT };
 struct StageEvt { int stage; cudaEvent_t a, b; };
 static std::mutex g_prof_mu;
 static bool g_prof_on = false;
@@ -488,6 +488,44 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha
 	return 0;
 }
 
+// the SSIM head of one view (s nullable): it reads the view's image and target, and needs its planes and accumulator
+static int check_ssim(const mgs_view& w, const mgs_view_ssim* s, bool forward)
+{
+	if (!s) return 0;
+	if (!w.target_color) return fail(MGS_ERR_INVALID_ARG, "view: the SSIM head needs the colour target (target_color)");
+	if (!s->ssim_terms || !s->loss_acc || !s->cot_color) return fail(MGS_ERR_INVALID_ARG, "view: the SSIM head needs ssim_terms, loss_acc and cot_color");
+	if (!forward && !w.out_color) return fail(MGS_ERR_INVALID_ARG, "view: the SSIM backward needs out_color (the forward's image)");
+	return 0;
+}
+
+// L1 + SSIM of one view's finished image, behind its blend on its stream (s nullable)
+static int enqueue_ssim_fwd(const mgs_view& w, const mgs_view_ssim* s, int debug)
+{
+	if (!s) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+	MGS_CUDA(cudaMemsetAsync(s->loss_acc, 0, 4 * sizeof(float), st));
+	{ StageTimer t_(ST_SSIM_FWD, st); launch_ssim_fwd(1, 3, w.height, w.width, w.out_color, w.target_color, s->ssim_terms, s->loss_acc, 2, st); }
+	MGS_STAGE("ssim_fwd");
+	return 0;
+}
+
+// the view's complete colour cotangent, before its blend backward on its stream (s nullable).  w becomes the view the
+// blend backward sees: that plane as dL_dpix, and the scales {1, the view's feature scale} the kernel leaves in loss_acc[2..3]
+static int enqueue_ssim_bwd(mgs_view& w, const mgs_view_ssim* s, int debug)
+{
+	if (!s) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+	{
+		StageTimer t_(ST_SSIM_BWD, st);
+		launch_ssim_bwd(1, 3, w.height, w.width, w.out_color, w.target_color, s->ssim_terms, s->cot_scale, w.dL_dpix, w.cot_scale,
+			s->cot_color, s->loss_acc + 2, st);
+	}
+	MGS_STAGE("ssim_bwd");
+	w.dL_dpix = s->cot_color;
+	w.cot_scale = s->loss_acc + 2;
+	return 0;
+}
+
 // blend backward of one view on its stream: the view's blend-stage records, and the feature gradients summed with 128-bit
 // reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
 // and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane; dm
@@ -526,8 +564,9 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
-// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm: V entries or NULL.
-static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm, const Cloud& c, float* dL_dmean3D,
+// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
+static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
+	const mgs_view_ssim* ssim, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -537,7 +576,9 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		int rc = fork_streams(V, views, join);
 		if (rc < 0) return rc;
 		for (int v = 0; v < V; v++) {
-			rc = enqueue_blend_bwd(c, views[v], dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr, debug);
+			mgs_view w = views[v];
+			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
+			if (rc == 0) rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -728,7 +769,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -772,6 +813,18 @@ int mgs_forward_views_aa(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_ssim(V, views, alpha, depth_mask, antialiasing, nullptr, P, D, M, F, means3D, shs, colors_precomp,
+		feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_ssim(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -783,6 +836,7 @@ int mgs_forward_views_aa(
 	for (int v = 0; v < V; v++) {
 		int rc = check_fwd_view(views[v], !colors_precomp);
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
+		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
@@ -807,6 +861,7 @@ int mgs_forward_views_aa(
 			rc = phase == 0 ? enqueue_project(c, views[v], debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
+			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -860,6 +915,20 @@ int mgs_backward_views_aa(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_ssim(V, views, alpha, depth_mask, antialiasing, nullptr, P, D, M, F, means3D, shs, colors_precomp,
+		feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D,
+		dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_ssim(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -870,11 +939,12 @@ int mgs_backward_views_aa(
 	for (int v = 0; v < V; v++) {
 		int rc = check_bwd_view(views[v], F > 0);
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
+		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -903,6 +973,14 @@ int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offset
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_ssim(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, nullptr, D, M, F, scale_modifier,
+		prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
+	int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -917,6 +995,7 @@ int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offset
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			rc = check_fwd_view(views[v], !k.colors_precomp);
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
+			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
 			if (rc < 0) return rc;
 		}
 	}
@@ -932,6 +1011,7 @@ int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offset
 				rc = phase == 0 ? enqueue_project(c, views[v], debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
+				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
 		}
@@ -964,6 +1044,14 @@ int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offse
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
 	int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_ssim(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, nullptr, D, M, F, scale_modifier,
+		accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
+	int F, float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -977,6 +1065,7 @@ int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offse
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			rc = check_bwd_view(views[v], F > 0 && k.feature);
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
+			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 			if (rc < 0) return rc;
 		}
 	}
@@ -992,8 +1081,11 @@ int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offse
 	for (int b = 0; b < B; b++) {
 		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-			rc = enqueue_blend_bwd(c, views[v], clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
-				depth_mask ? depth_mask + v : nullptr, debug);
+			mgs_view w = views[v];
+			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
+			if (rc == 0)
+				rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
+					depth_mask ? depth_mask + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1053,6 +1145,37 @@ int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature
 		loss_acc, st);
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess) return fail(MGS_ERR_CUDA, std::string("loss_heads: ") + cudaGetErrorString(e));
+	return 0;
+}
+
+static int check_ssim_planes(int V, int C, int H, int W)
+{
+	if (V <= 0 || C <= 0 || H <= 0 || W <= 0) return fail(MGS_ERR_INVALID_ARG, "bad V/C/H/W");
+	if ((long long)V * C > 65535) return fail(MGS_ERR_INVALID_ARG, "V * C must be at most 65535");
+	return 0;
+}
+
+int mgs_ssim(int V, int C, int H, int W, const float* x, const float* g, float* ssim_terms, float* loss_acc, void* stream)
+{
+	if (check_ssim_planes(V, C, H, W) < 0) return MGS_ERR_INVALID_ARG;
+	if (!x || !g || !ssim_terms || !loss_acc) return fail(MGS_ERR_INVALID_ARG, "x, g, ssim_terms and loss_acc are required");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(cudaMemsetAsync(loss_acc, 0, (size_t)V * 2 * sizeof(float), st));
+	{ StageTimer t_(ST_SSIM_FWD, st); launch_ssim_fwd(V, C, H, W, x, g, ssim_terms, loss_acc, 2, st); }
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) return fail(MGS_ERR_CUDA, std::string("ssim: ") + cudaGetErrorString(e));
+	return 0;
+}
+
+int mgs_ssim_backward(int V, int C, int H, int W, const float* x, const float* g, const float* ssim_terms, const float* scale,
+	const float* cot_in, float* cot_out, void* stream)
+{
+	if (check_ssim_planes(V, C, H, W) < 0) return MGS_ERR_INVALID_ARG;
+	if (!x || !g || !ssim_terms || !cot_out) return fail(MGS_ERR_INVALID_ARG, "x, g, ssim_terms and cot_out are required");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	{ StageTimer t_(ST_SSIM_BWD, st); launch_ssim_bwd(V, C, H, W, x, g, ssim_terms, scale, cot_in, nullptr, cot_out, nullptr, st); }
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) return fail(MGS_ERR_CUDA, std::string("ssim_backward: ") + cudaGetErrorString(e));
 	return 0;
 }
 
@@ -1143,7 +1266,7 @@ int mgs_profile_enable(int on)
 int mgs_profile_num_stages(void) { return ST_COUNT; }
 const char* mgs_profile_stage_name(int i)
 {
-	static const char* names[ST_COUNT] = { "project_fwd", "depth_sort", "scan", "emit_tiles", "tile_sort", "ranges_pack", "block_lists", "blend_fwd", "blend_bwd", "project_bwd", "activate_fwd", "activate_bwd" };
+	static const char* names[ST_COUNT] = { "project_fwd", "depth_sort", "scan", "emit_tiles", "tile_sort", "ranges_pack", "block_lists", "blend_fwd", "blend_bwd", "project_bwd", "activate_fwd", "activate_bwd", "ssim_fwd", "ssim_bwd" };
 	return (i >= 0 && i < ST_COUNT) ? names[i] : "";
 }
 int mgs_profile_read(float* total_ms, int* counts)

@@ -171,6 +171,14 @@ struct BlendArgs {
 void launch_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* tgt_color, const float* tgt_feature,
 	float* cot_color, float* cot_feature, float* loss_acc, cudaStream_t s);
 
+// ssim.cu: L1 + SSIM of V views of C planes each (x, g [V,C,H,W]).  Forward: terms [V,3,C,H,W] receives the unscaled
+// partials of S, acc + v * acc_stride the sums {|x - g|, S} (added).  Backward: cot_out [V,C,H,W] = cot_in_scale[0] * cot_in
+// + scale[2v] d l1 / dx + scale[2v+1] d ssim / dx (scale, cot_in, cot_in_scale nullable); blend_slot (nullable, V = 1)
+// receives {1, cot_in_scale[1]}.
+void launch_ssim_fwd(int V, int C, int H, int W, const float* x, const float* g, float* terms, float* acc, int acc_stride, cudaStream_t s);
+void launch_ssim_bwd(int V, int C, int H, int W, const float* x, const float* g, const float* terms, const float* scale,
+	const float* cot_in, const float* cot_in_scale, float* cot_out, float* blend_slot, cudaStream_t s);
+
 // activate.cu: view-independent per-Gaussian pre-ops (activations, deformation offsets, feature normalisation)
 struct ActivateArgs {
 	int P, F;

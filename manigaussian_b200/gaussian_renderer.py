@@ -215,6 +215,26 @@ def _depth_mask_losses(dm, N, dev):
     return loss_depth, loss_mask, n
 
 
+def _ssim_head(V, H, W, dev):
+    """The L1 + SSIM head's `ssim` tuple for the raw calls: the partials of S [V,9,H,W], the [V,4] accumulator and the
+    combined colour cotangent [V,3,H,W]"""
+    opts = dict(dtype=torch.float32, device=dev)
+    return torch.empty((V, 9, H, W), **opts), torch.empty((V, 4), **opts), torch.empty((V, 3, H, W), **opts)
+
+
+def _ssim_losses(head, N, dev):
+    """(loss_l1, ssim) [V] from the accumulator of an `ssim` tuple (N = 3 H W); empty without the head"""
+    if head is None:
+        return torch.empty(0, device=dev), torch.empty(0, device=dev)
+    return head[1][:, 0] / N, head[1][:, 1] / N
+
+
+def _pair_scale(g0, g1, V, dev):
+    """[V,2] upstream gradients of two per-view losses, 0 for one that received none (no host synchronisation)"""
+    z = torch.zeros((V,), dtype=torch.float32, device=dev)
+    return torch.stack([g0 if g0 is not None else z, g1 if g1 is not None else z], 1).contiguous()
+
+
 def _depth_mask_scale(dm, g_depth, g_mask, V, dev):
     """[V,2] upstream gradients {g_depth, g_mask} of the depth / mask losses for the backward"""
     z = torch.zeros((V,), dtype=torch.float32, device=dev)
@@ -225,12 +245,13 @@ def _depth_mask_scale(dm, g_depth, g_mask, V, dev):
 class _RasterizeViewsLoss(torch.autograd.Function):
     """render_views with the loss heads fused into the forward blend's epilogue (SURVEY.md 8(f) row f4): returns the per-view
     L2 colour loss and cosine embedding loss of NeuralRenderer.forward (neural_rendering.py:300-318, loss.py:12-23) and,
-    with depth / mask targets (row f7), the expected-depth L1 loss, the alpha mask BCE loss and the valid-pixel counts; the
-    images come back too, but gradients flow through the losses only."""
+    with depth / mask targets (row f7), the expected-depth L1 loss, the alpha mask BCE loss and the valid-pixel counts, and
+    with ssim (row f9) the L1 loss and the SSIM of the colour image; the images come back too, but gradients flow through the
+    losses only."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
-                target_depth=None, target_mask=None, antialiasing=False):
+                target_depth=None, target_mask=None, antialiasing=False, ssim=False):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -251,12 +272,13 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         cot_embed = torch.empty((V, F, H, W), **opts) if target_embed is not None else (torch.zeros((V, F, H, W), **opts) if include else None)
         loss_acc = torch.empty((V, 2), **opts)
         dm = _depth_mask_heads(target_depth, target_mask, V, H, W, dev)
+        ssim_head = _ssim_head(V, H, W, dev) if ssim else None
         degree = views[0].sh_degree
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, debug=views[0].debug,
                                             out_buffers=(color, feat_img, None),
                                             loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm,
-                                            antialiasing=antialiasing)
+                                            antialiasing=antialiasing, ssim=ssim_head)
         N = float(H * W)
         loss_rgb = loss_acc[:, 0] / (3.0 * N)
         loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
@@ -269,24 +291,29 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         ctx.opac_shape = opacities.shape
         ctx.cots = (cot_rgb, cot_embed)
         ctx.dm = dm  # the targets, cotangent planes and accumulator of the depth / mask heads: none of them is an output
+        # the SSIM head's planes and accumulator, and the colour target (an input); the backward also reads the image, an
+        # output, which therefore goes through save_for_backward
+        ctx.ssim, ctx.target_rgb = ssim_head, (target_rgb if ssim else None)
         ctx.save_for_backward(means3D, sh if sh is not None else torch.empty(0, device=dev),
                               colors_precomp if colors_precomp is not None else torch.empty(0, device=dev),
-                              feature if include else torch.empty(0, device=dev), scales, rotations)
+                              feature if include else torch.empty(0, device=dev), scales, rotations,
+                              color if ssim else torch.empty(0, device=dev))
         empty = torch.empty(0, device=dev)
         loss_depth, loss_mask, depth_pixels = _depth_mask_losses(dm, N, dev)
+        loss_l1, ssim_v = _ssim_losses(ssim_head, 3.0 * N, dev)
         # ONE call: a second mark_non_differentiable replaces the first
         ctx.mark_non_differentiable(radii, color, *([feat_img] if include else []), depth_pixels)
-        return loss_rgb, loss_embed, color, (feat_img if include else empty), radii, loss_depth, loss_mask, depth_pixels
+        return (loss_rgb, loss_embed, color, (feat_img if include else empty), radii, loss_depth, loss_mask, depth_pixels, loss_l1,
+                ssim_v)
 
     @staticmethod
-    def backward(ctx, g_rgb, g_embed, _gc, _gf, _gr, g_depth, g_mask, _gn):
-        means3D, sh, colors_precomp, feature, scales, rotations = ctx.saved_tensors
+    def backward(ctx, g_rgb, g_embed, _gc, _gf, _gr, g_depth, g_mask, _gn, g_l1, g_ssim):
+        means3D, sh, colors_precomp, feature, scales, rotations, color = ctx.saved_tensors
         dev = means3D.device
         views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
         M = sh.shape[1] if sh.numel() else 0
         use_colors = colors_precomp.numel() > 0
-        z = torch.zeros((V,), dtype=torch.float32, device=dev)
-        scale = torch.stack([g_rgb if g_rgb is not None else z, g_embed if g_embed is not None else z], 1).contiguous()
+        scale = _pair_scale(g_rgb, g_embed, V, dev)
         cot_rgb, cot_embed = ctx.cots
         pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)
         grp = None if ctx.group in (None, True) else ctx.group
@@ -299,18 +326,20 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                      after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
                                      depth_mask=ctx.dm,
                                      depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None,
-                                     antialiasing=ctx.antialiasing)
+                                     antialiasing=ctx.antialiasing,
+                                     ssim=ctx.ssim + (color, ctx.target_rgb) if ctx.ssim is not None else None,
+                                     ssim_scale=_pair_scale(g_l1, g_ssim, V, dev) if ctx.ssim is not None else None)
         if ctx.group is not None:
             pk.all_reduce_finish(grp)
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None, None)
 
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
-                 targets=None, return_alpha=False, antialiasing=False):
+                 targets=None, return_alpha=False, antialiasing=False, ssim=False):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -327,6 +356,10 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     over the pixels with gt > 0 and alpha > 0.5; 0 where there is none), "depth_pixels" [V] (their count, float, not
     differentiable) and "loss_mask" [V] (binary cross-entropy of clamp(alpha, 1e-4, 1 - 1e-4) against the mask, mean over
     the pixels).
+    ssim: with targets, also evaluate the photometric objective 3DGS trains with on the colour image (INTEGRATION.md §4,
+    fused tiled kernels behind each view's blend): the result adds "loss_l1" [V] (mean |render - rgb|) and "ssim" [V] (SSIM
+    with the 11x11 Gaussian window, sigma 1.5, as the reference's `ssim`; SSIM itself, not 1 - SSIM), both differentiable;
+    e.g. loss = 0.8 * out["loss_l1"] + 0.2 * (1 - out["ssim"]).
     return_alpha: also return "alpha" [V,H,W], the accumulated opacity 1 - final_T (differentiable; depth / alpha is the
     expected depth).
     antialiasing: render with the anti-aliased projection (opacity compensation for the 0.3 px^2 dilation, INTEGRATION.md
@@ -352,20 +385,26 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         feat = normalize_features(features_language) if normalize_feature else features_language
     V, P = len(views), pts_xyz.shape[0]
     screenspace_points = torch.zeros((V, P, 3), dtype=torch.float32, device=device, requires_grad=True)
+    if ssim and targets is None:
+        raise ValueError("ssim=True needs targets (the colour target \"rgb\")")
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
         if return_alpha:
             raise ValueError("targets and return_alpha cannot be combined")
-        loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels = _RasterizeViewsLoss.apply(
+        (loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels, loss_l1,
+         ssim_v) = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"), aa)
+            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"), aa,
+            bool(ssim))
         ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
                "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
         if targets.get("depth") is not None:
             ret["loss_depth"], ret["depth_pixels"] = loss_depth, depth_pixels
         if targets.get("mask") is not None:
             ret["loss_mask"] = loss_mask
+        if ssim:
+            ret["loss_l1"], ret["ssim"] = loss_l1, ssim_v
         return ret
     if V == 1 and sync_gradients is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
@@ -394,16 +433,16 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 
 class _RasterizeClouds(torch.autograd.Function):
-    """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha).  Outputs per
-    cloud: (color, feature image, radii, depth, alpha), or with targets (loss_rgb, loss_embed, color, feature image, radii,
-    loss_depth, loss_mask, depth_pixels) with gradients through the losses only."""
+    """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha, antialiasing,
+    ssim).  Outputs per cloud: (color, feature image, radii, depth, alpha), or with targets (loss_rgb, loss_embed, color,
+    feature image, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim) with gradients through the losses only."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets, return_alpha, antialiasing = meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
-        clouds, results, frozen, cots, dms = [], [], [], [], []
+        clouds, results, frozen, cots, dms, ssims, images = [], [], [], [], [], [], []
         for b, views in enumerate(cloud_views):
             means3D, _, sh, colors, feature, opacities, scales, rotations = (_prep(t, dev) for t in flat[_CLOUD_INPUTS * b:_CLOUD_INPUTS * (b + 1)])
             V, H, W = len(views), int(views[0].image_height), int(views[0].image_width)
@@ -424,8 +463,12 @@ class _RasterizeClouds(torch.autograd.Function):
                 loss_acc = torch.empty((V, 2), **opts)
                 c["loss_heads"] = (t_rgb, t_emb, cot_rgb, cot_emb, loss_acc)
                 c["depth_mask"] = _depth_mask_heads(targets[b].get("depth"), targets[b].get("mask"), V, H, W, dev, f"cloud {b}")
+                c["ssim"] = _ssim_head(V, H, W, dev) if ssim else None
                 cots.append((cot_rgb, cot_emb))
                 dms.append(c["depth_mask"])
+                # the SSIM head's planes and the colour target (an input); the image, an output, is saved for backward
+                ssims.append(c["ssim"] + (t_rgb,) if ssim else None)
+                images.append(color if ssim else torch.empty(0, device=dev))
             clouds.append(c)
         degree = cloud_views[0][0].sh_degree
         include = clouds[0]["feature"] is not None
@@ -441,29 +484,31 @@ class _RasterizeClouds(torch.autograd.Function):
                 loss_rgb = loss_acc[:, 0] / (3.0 * N)
                 loss_embed = 1.0 - loss_acc[:, 1] / N if c["loss_heads"][1] is not None else torch.zeros((len(c["views"]),), **opts)
                 loss_depth, loss_mask, depth_pixels = _depth_mask_losses(c["depth_mask"], N, dev)
+                loss_l1, ssim_v = _ssim_losses(c["ssim"], 3.0 * N, dev)
                 results += [loss_rgb, loss_embed, color, feat_img if feat_img is not None else empty(), radii, loss_depth, loss_mask,
-                            depth_pixels]
+                            depth_pixels, loss_l1, ssim_v]
                 frozen += [radii, color, depth_pixels] + ([feat_img] if feat_img is not None else [])
             else:
                 results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty(),
                             alpha if alpha is not None else empty()]
                 frozen.append(radii)
-        ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots, ctx.dms = meta, streams, degree, include, cots, dms
+        ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots, ctx.dms, ctx.ssims = meta, streams, degree, include, cots, dms, ssims
         # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
         ctx.state = [[(o[0], o[3], o[4], o[5], o[6]) for o in co] for co in outs]
         ctx.opac_shapes = [flat[_CLOUD_INPUTS * b + 5].shape for b in range(B)]
         e = torch.empty(0, device=dev)
         ctx.save_for_backward(*[x if x is not None else e for c in clouds for x in
-                                (c["means3D"], c["sh"], c["colors"], c["feature"], c["scales"], c["rotations"])])
+                                (c["means3D"], c["sh"], c["colors"], c["feature"], c["scales"], c["rotations"])], *images)
         ctx.mark_non_differentiable(*frozen)  # ONE call: a second one replaces the first
         return tuple(results)
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets, return_alpha, antialiasing = ctx.meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
-        per = 8 if targets is not None else 5
+        images = saved[6 * len(cloud_views):]
+        per = 10 if targets is not None else 5
         clouds = []
         for b, views in enumerate(cloud_views):
             means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
@@ -473,12 +518,14 @@ class _RasterizeClouds(torch.autograd.Function):
             c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, scales=scales, rotations=rotations,
                      want_feature=bool(ctx.needs_input_grad[1 + _CLOUD_INPUTS * b + 4]))
             if targets is not None:
-                z = torch.zeros((V,), dtype=torch.float32, device=dev)
-                c["cot_scale"] = torch.stack([g[0] if g[0] is not None else z, g[1] if g[1] is not None else z], 1).contiguous()
+                c["cot_scale"] = _pair_scale(g[0], g[1], V, dev)
                 c["grad_color"], c["grad_feature"] = ctx.cots[b]
                 if ctx.dms[b] is not None:
                     c["depth_mask"] = ctx.dms[b]
                     c["depth_mask_scale"] = _depth_mask_scale(ctx.dms[b], g[5], g[6], V, dev)
+                if ssim:
+                    c["ssim"] = ctx.ssims[b][:3] + (images[b], ctx.ssims[b][3])
+                    c["ssim_scale"] = _pair_scale(g[8], g[9], V, dev)
             else:
                 c["grad_color"] = g[0] if g[0] is not None else torch.zeros((V, 3, H, W), dtype=torch.float32, device=dev)
                 if F:
@@ -502,7 +549,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
 
 def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False,
-                  antialiasing=False):
+                  antialiasing=False, ssim=False):
     """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
     next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
 
@@ -514,12 +561,15 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     and "loss_depth" / "depth_pixels" / "loss_mask" with "depth" / "mask" targets; "depth" / "alpha" [V,H,W] when asked for).
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
     dyna step, which renders the detached current features); its feature cotangents still reach its other gradients.
-    antialiasing: every cloud renders with the anti-aliased projection, as in render_views."""
+    antialiasing: every cloud renders with the anti-aliased projection, as in render_views.
+    ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
     with_targets = [c.get("targets") is not None for c in clouds]
     if any(with_targets) and not all(with_targets):
         raise ValueError("targets must be given on all clouds or on none")
+    if ssim and not all(with_targets):
+        raise ValueError("ssim=True needs targets on every cloud (the colour target \"rgb\")")
     if all(with_targets) and return_depth:
         raise ValueError("targets and return_depth cannot be combined")
     if all(with_targets) and return_alpha:
@@ -559,18 +609,20 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for views in cloud_views for s in views)
-    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa), *flat)
+    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim)), *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]
         if targets is not None:
-            loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels = out[8 * b:8 * b + 8]
+            loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim_v = out[10 * b:10 * b + 10]
             r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii,
                  "loss_rgb": loss_rgb, "loss_embed": loss_embed}
             if targets[b].get("depth") is not None:
                 r["loss_depth"], r["depth_pixels"] = loss_depth, depth_pixels
             if targets[b].get("mask") is not None:
                 r["loss_mask"] = loss_mask
+            if ssim:
+                r["loss_l1"], r["ssim"] = loss_l1, ssim_v
             ret.append(r)
         else:
             color, feat_img, radii, depth, alpha = out[5 * b:5 * b + 5]

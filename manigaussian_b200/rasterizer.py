@@ -583,7 +583,7 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False):
+                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -597,7 +597,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     [V,H,W] or None, cot_depth, cot_alpha_depth (both [V,H,W], with target_depth), cot_alpha_mask [V,H,W] (with target_mask),
     loss_acc [V,3]), with `loss_heads` only: the same epilogue also evaluates the expected-depth L1 head and the alpha mask
     head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc.  `antialiasing`: the
-    anti-aliased projection (C ABI mgs_forward_views_aa); pass the same value to the backward."""
+    anti-aliased projection (C ABI mgs_forward_views_aa); pass the same value to the backward.  `ssim` = (ssim_terms
+    [V,9,H,W], loss_acc [V,4], cot_color [V,3,H,W]), with `loss_heads` only: behind each view's blend, the L1 + SSIM head
+    (C ABI mgs_view_ssim) leaves {sum |x - g|, sum S} in loss_acc[:, :2] and the partials of S in ssim_terms."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -627,11 +629,14 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
+        sarr = (_b.ViewSsim * V)() if ssim is not None else None
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
             if darr is not None:
                 _fill_depth_mask(darr[v], depth_mask, v)
+            if sarr is not None:
+                _fill_ssim(sarr[v], ssim, v)
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
                                  aarr[v] if return_alpha else None)
@@ -641,7 +646,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             outs.append(o)
         rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
-        if antialiasing:
+        if sarr is not None:
+            _b.check(L.mgs_forward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_forward_views_ssim")
+        elif antialiasing:
             _b.check(L.mgs_forward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_forward_views_aa")
         elif darr is not None:
             _b.check(L.mgs_forward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_forward_views_depth_mask")
@@ -664,6 +671,17 @@ def _fill_depth_mask(wd, depth_mask, v, scale=None):
     wd.loss_acc = _ptr(acc[v])
     if scale is not None:
         wd.cot_scale = scale.data_ptr() + 8 * v
+
+
+def _fill_ssim(ws, ssim, v, w=None, scale=None):
+    """Fills view v's mgs_view_ssim `ws` from an `ssim` tuple of rasterize_views_raw.  Backward: the tuple also holds the
+    forward's images and targets [V,3,H,W], which go into the view's mgs_view `w`, and `scale` [V,2] holds the upstream
+    gradients {g_l1, g_ssim}."""
+    ws.ssim_terms, ws.loss_acc, ws.cot_color = _ptr(ssim[0][v]), _ptr(ssim[1][v]), _ptr(ssim[2][v])
+    if w is not None:
+        w.out_color, w.target_color = _ptr(ssim[3][v]), _ptr(ssim[4][v])
+    if scale is not None:
+        ws.cot_scale = scale.data_ptr() + 8 * v
 
 
 def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None):
@@ -718,7 +736,8 @@ def _track_status(outs, keys, status, main, pending):
 def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_feature, means3D, colors, language_feature, scales,
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
-                                 cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False):
+                                 cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
+                                 ssim=None, ssim_scale=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -730,7 +749,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     are loaded.  `grads_alpha` (per view [H,W] or None): cotangents of the alpha planes of a `return_alpha` forward.  The
     caller's current stream holds the result on return.  `depth_mask`: the tuple given to the forward, whose cotangent planes
     are read back with `depth_mask_scale` [V,2] (device; the upstream gradients {g_depth, g_mask} of the depth and mask losses,
-    or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_backward_views_aa)."""
+    or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_backward_views_aa).  `ssim`: the tuple given to
+    the forward plus the forward's images and colour targets (both [V,3,H,W]); each view's L1 + SSIM head then writes its
+    complete colour cotangent, with `ssim_scale` [V,2] (device; the upstream gradients {g_l1, g_ssim}, or None for 1), before
+    its blend backward reads it."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -768,7 +790,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         aarr = (_b.ViewAlpha * V)() if grads_alpha is not None else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
         dscale = _prep(depth_mask_scale, dev)
-        keep = [dscale]
+        sarr = (_b.ViewSsim * V)() if ssim is not None else None
+        sscale = _prep(ssim_scale, dev)
+        keep = [dscale, sscale]
         for v, s in enumerate(views):
             w = arr[v]
             if darr is not None:
@@ -784,13 +808,17 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
             w.stream = streams[v].cuda_stream
             if cot_scale is not None:
                 w.cot_scale = cot_scale.data_ptr() + 8 * v
+            if sarr is not None:
+                _fill_ssim(sarr[v], ssim, v, w, sscale)
         for stages in ((1, 2) if after_blend is not None else (3,)):
             rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
                     _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if antialiasing:
+            if sarr is not None:
+                _b.check(L.mgs_backward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_backward_views_ssim")
+            elif antialiasing:
                 _b.check(L.mgs_backward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_backward_views_aa")
             elif darr is not None:
                 _b.check(L.mgs_backward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_backward_views_depth_mask")
@@ -856,7 +884,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
-    "capacities" as rasterize_views_raw takes them, and "depth_mask" (with "loss_heads") as its `depth_mask`.  degree, F, the
+    "capacities" as rasterize_views_raw takes them, and "depth_mask" and "ssim" (with "loss_heads") as its `depth_mask` and
+    `ssim`.  degree, F, the
     colour and covariance modes are shared.  `return_alpha`
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
@@ -891,6 +920,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
+        sarr = (_b.ViewSsim * V)() if any(c.get("ssim") is not None for c in clouds) else None
         status = _status_slots(V)
         keep, outs = [], []
         for b, (c, d) in enumerate(zip(clouds, pc)):
@@ -906,6 +936,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 cap = int(caps[v]) if caps is not None else _CAPACITY[keys[b][v]]
                 if c.get("depth_mask") is not None:
                     _fill_depth_mask(darr[g], c["depth_mask"], v)
+                if c.get("ssim") is not None:
+                    _fill_ssim(sarr[g], c["ssim"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
                                       c.get("loss_heads"), aarr[g] if return_alpha else None)
                 arr[g].status = status.data_ptr() + 8 * g
@@ -914,7 +946,10 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 cloud_outs.append(o)
             outs.append(cloud_outs)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if antialiasing:
+        if sarr is not None:
+            _b.check(L.mgs_forward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
+                     "mgs_forward_clouds_ssim")
+        elif antialiasing:
             _b.check(L.mgs_forward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_forward_clouds_aa")
         elif darr is not None:
             _b.check(L.mgs_forward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_forward_clouds_depth_mask")
@@ -936,7 +971,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     "grad_alpha" [V_b,H,W] (the cotangent of a `return_alpha` forward's alpha planes),
     "cot_scale" [V_b,2] (device; the loss heads' upstream gradients), "depth_mask" and "depth_mask_scale" [V_b,2] (the
     forward's depth / mask heads and their upstream gradients, as rasterize_views_backward_raw takes them) and "want_feature" (default True; False: the cloud's
-    dL_dfeature is not computed, but its feature cotangents still reach the other gradients).  Returns one dict per cloud
+    dL_dfeature is not computed, but its feature cotangents still reach the other gradients), and "ssim" and "ssim_scale" [V_b,2]
+    as rasterize_views_backward_raw takes them.  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
     dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed).  `antialiasing`: the value
     the forward was given (C ABI mgs_backward_clouds_aa)."""
@@ -955,6 +991,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if any(c.get("grad_alpha") is not None for c in clouds) else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
+        sarr = (_b.ViewSsim * V)() if any(c.get("ssim") is not None for c in clouds) else None
         keep = []
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
@@ -978,7 +1015,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             k.dL_dscale, k.dL_drot = _ptr(gr["dL_dscales"]), _ptr(gr["dL_drotations"])
             cot = _prep(c.get("cot_scale"), dev)
             dscale = _prep(c.get("depth_mask_scale"), dev)
-            keep.append(dscale)
+            sscale = _prep(c.get("ssim_scale"), dev)
+            keep += [dscale, sscale]
             for v, s in enumerate(c["views"]):
                 g = offsets[b] + v
                 w = arr[g]
@@ -995,9 +1033,14 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     keep.append(ga)
                 if cot is not None:
                     w.cot_scale = cot.data_ptr() + 8 * v
+                if c.get("ssim") is not None:
+                    _fill_ssim(sarr[g], c["ssim"], v, w, sscale)
             keep.append(cot)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if antialiasing:
+        if sarr is not None:
+            _b.check(L.mgs_backward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
+                     "mgs_backward_clouds_ssim")
+        elif antialiasing:
             _b.check(L.mgs_backward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_backward_clouds_aa")
         elif darr is not None:
             _b.check(L.mgs_backward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_backward_clouds_depth_mask")
