@@ -33,10 +33,13 @@
 //                pair of reductions fills whole 32-byte sectors).
 // Roles.  Only the walk is sequential (T and S carry from chunk to chunk), so it has a warp of its own: warp 0, the
 // walker W, owns T, S and the background term and runs step 3.  Warp 1, the companion C, runs everything else: the queue,
-// the gathers, GEMM 1, GEMM 2/3 and the flush.  They hand chunks to each other through a two-stage ring of {rows -> wgt,
-// Wd -> q} tiles (records: three slots) with named barriers (protocol at the loop below), so that while W walks chunk i,
-// C finishes chunk i - 1 and prepares chunk i + 1.  Splitting the roles also splits the registers: 128 per thread give
-// 8 CTAs (16 warps) per SM at F = 32, against 12 single-warp CTAs at 157 registers when one warp did all of it.
+// the gathers, GEMM 2/3 and the flush.  GEMM 1 goes to whichever warp would otherwise wait (W_GEMM1 in the kernel): with
+// feature tiles C carries the larger share of a chunk, and GEMM 1 moves to W, which reads the cotangent rows it staged
+// and writes Wd, which only its own walk reads; at small F the walk is the longer share, and C keeps GEMM 1.  The warps
+// hand chunks to each other through a two-stage ring of {rows -> wgt, Wd -> q} tiles (records: three slots) with named
+// barriers (protocol at the loop below), so that while W walks chunk i, C finishes chunk i - 1 and prepares chunk i + 1.
+// Splitting the roles also splits the registers: 128 per thread give 8 CTAs (16 warps) per SM at F = 32, against 12
+// single-warp CTAs at 157 registers when one warp did all of it.
 // Channel groups (F > 32) keep that single-warp CTA (blend_bwd_groups_kernel): their launches are several waves deep,
 // and there two-warp CTAs measured slower.
 // Index assignment.  An MMA A operand is four consecutive registers, a B operand two; a register move per operand would
@@ -84,7 +87,8 @@ constexpr int BWD_MT = BWD_CH / 16;       // 16-row tiles of Gaussians
 constexpr int BWD_NREC = 3;               // record slots: chunk i (walked), i - 1 (flushed), i + 1 (gathered)
 static_assert(BWD_CH == 16 || BWD_CH == 32, "backward chunk size");
 // named barriers of the hand-off (0 is __syncthreads'), one per signal and stage s = chunk & 1, 64 threads each:
-// FULL + s  companion -> walker: records, cnt and Wd of the chunk are in place (bar.arrive by C, bar.sync by W)
+// FULL + s  companion -> walker: records, cnt and channel rows (W_GEMM1) or Wd (otherwise) of the chunk are in place
+//           (bar.arrive by C, bar.sync by W)
 // DONE + s  walker -> companion: wgt and q of the chunk are written            (bar.arrive by W, bar.sync by C)
 constexpr int BWD_BAR_FULL = 1, BWD_BAR_DONE = 3;
 
@@ -113,6 +117,10 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	constexpr int GS = 2 * CHP;          // s_g stride per pixel pair
 	constexpr int XS = 2 * BWD_CH + 4;   // s_x / s_wgt stride per pixel pair (+4: spreads the pairs over the banks)
 	constexpr int ROWS_FLOATS = (BWD_CH * RS > 16 * XS) ? BWD_CH * RS : 16 * XS;  // the rows buffer is reused for the wgt tile
+	// GEMM 1 on the walker at F > 16 only: there the companion's GEMM 2 and feature flush make it the warp that bounds a
+	// chunk (c3, F = 32: blend_bwd 6 % shorter); at F <= 16 the walk does, and GEMM 1 on the walker made blend_bwd longer
+	// (c3 shape, F = 16 / 8 / 0: +4 / +2 / +9 %; DESIGN §4)
+	constexpr bool W_GEMM1 = NFT == 4;
 	__shared__ __align__(16) float4 s_rec[BWD_NREC][BWD_CH * 2];  // records by chunk mod 3: {x,y,ca,cb}, {cc,op,pixel mask,id}
 	__shared__ uint2 s_qe[BWD_QCAP];                              // survivor queue, back to front: {list position, pixel mask}
 	__shared__ __align__(16) float s_rows[2][ROWS_FLOATS];        // by stage: C[j][RS]; after GEMM 1: wgt tile
@@ -124,7 +132,11 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	const unsigned long long t_start = cta_log_now();
 #endif
 	const int lane = threadIdx.x & 31;
-	const bool walker = threadIdx.x < 32;  // warp 0 walks, warp 1 is the companion
+	// warp 0 walks, warp 1 is the companion.  The warp index comes through a shuffle so that the compiler knows it is
+	// warp-uniform: from threadIdx.x < 32 it assumes the roles may diverge inside a warp and wraps every shuffle, ballot
+	// and __syncwarp of the two branches in a divergence-safe WARPSYNC ... ENDCOLLECTIVE sequence (3,424 SASS instructions
+	// against 2,704 at F = 32)
+	const bool walker = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0) == 0;
 	const int gid = lane >> 2, tig = lane & 3;
 	const int sub = blockIdx.x & 7;
 	const int rank = (int)(blockIdx.x >> 3);
@@ -173,13 +185,53 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 	}
 	__syncthreads();  // s_g and the zeroed rows buffers are in place: the CTA's only barrier over both warps besides the hand-off
 
-	// Two-stage ring.  While W walks chunk i in stage i & 1, C finishes chunk i - 1 (GEMM 2/3, flush) and prepares chunk
-	// i + 1 (gathers, GEMM 1), both in stage (i + 1) & 1.  Each signal is raised once per use of its stage and consumed
-	// before it can be raised again: C raises FULL + s for chunk i + 2 only after it consumed DONE + s of chunk i, which W
-	// raises after it consumed FULL + s of chunk i; W raises DONE + s for chunk i + 2 only after it consumed FULL + s of
-	// chunk i + 2, which C raises after it consumed DONE + s of chunk i.  The end of the list travels as a chunk with
-	// cnt = 0 through FULL, after which W stops and C finishes the last real chunk: both warps run the same sequence of
-	// barrier operations.
+	// GEMM 1 of the chunk whose channel rows sit in s_rows, into s_xs
+	auto gemm1 = [&](const float* s_rows, float* s_xs) {
+		// ---- 2. GEMM 1: Wd[p][j] = Gpx[p][:] . C[j][:]   (M = pixels (2 tiles), N = survivors, K = channels) ----
+		float wd[2][BWD_CH / 8][4];
+#pragma unroll
+		for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+			for (int nt = 0; nt < BWD_CH / 8; nt++)
+#pragma unroll
+				for (int i = 0; i < 4; i++) wd[mt][nt][i] = 0.f;
+#pragma unroll
+		for (int ks = 0; ks < NT; ks++) {
+			uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+			for (int mt = 0; mt < 2; mt++) {
+				const float4 v = *reinterpret_cast<const float4*>(s_g + (8 * mt + gid) * GS + (8 * ks + 2 * tig) * 2);
+				tf32_split(v.x, ahi[mt][0], alo[mt][0]); tf32_split(v.y, ahi[mt][1], alo[mt][1]);
+				tf32_split(v.z, ahi[mt][2], alo[mt][2]); tf32_split(v.w, ahi[mt][3], alo[mt][3]);
+			}
+#pragma unroll
+			for (int nt = 0; nt < BWD_CH / 8; nt++) {
+				const float2 v = *reinterpret_cast<const float2*>(s_rows + (8 * nt + gid) * RS + 8 * ks + 2 * tig);
+				uint32_t bh0, bl0, bh1, bl1;
+				tf32_split(v.x, bh0, bl0);
+				tf32_split(v.y, bh1, bl1);
+				mma_3xtf32(wd[0][nt], ahi[0], alo[0], bh0, bh1, bl0, bl1);
+				mma_3xtf32(wd[1][nt], ahi[1], alo[1], bh0, bh1, bl0, bl1);
+			}
+		}
+		// D fragment (mt, nt): pixels (pi = 8 mt + gid, e = 0 | 1), survivors 8 nt + 2 tig (+1): one 16-byte store
+#pragma unroll
+		for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+			for (int nt = 0; nt < BWD_CH / 8; nt++)
+				*reinterpret_cast<float4*>(s_xs + (8 * mt + gid) * XS + (4 * nt + tig) * 4) =
+					make_float4(wd[mt][nt][0], wd[mt][nt][1], wd[mt][nt][2], wd[mt][nt][3]);
+	};
+
+	// Two-stage ring.  While W walks chunk i in stage i & 1 (with W_GEMM1 after its GEMM 1 turned the stage's rows into Wd;
+	// the walk turns Wd into q in place and overwrites the rows with wgt), C finishes chunk i - 1 (GEMM 2/3, flush) and
+	// prepares chunk i + 1 (records, rows, without W_GEMM1 its GEMM 1), both in stage (i + 1) & 1.  Each signal is raised
+	// once per use of its stage and consumed before it can be raised again: C raises FULL + s for chunk i + 2 only after it
+	// consumed DONE + s of chunk i, which W raises after it consumed FULL + s of chunk i; W raises DONE + s for chunk i + 2
+	// only after it consumed FULL + s of chunk i + 2, which C raises after it consumed DONE + s of chunk i.  Neither warp
+	// blocks on anything else but its own cp.async groups, so the waits cannot form a cycle (DESIGN §4).  The end of the
+	// list travels as a chunk with cnt = 0 through FULL, after which W stops and C finishes the last real chunk: both warps
+	// run the same sequence of barrier operations.
 	if (walker) {
 #ifdef MGS_BWD_PHASES
 		BwdPhaseClock ph;
@@ -200,6 +252,11 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			float* const s_wgt = s_rows[s];
 			float* const s_xs = s_x[s];
 			r = r == BWD_NREC - 1 ? 0 : r + 1;
+			if (W_GEMM1) {
+				gemm1(s_rows[s], s_xs);
+				__syncwarp();  // every lane's Wd is stored and every row read: the walk reads Wd and overwrites the rows with wgt
+				BWD_PH_LAP(ph, BWD_PH_GEMM1);
+			}
 			// ---- 3. walk, back to front (queue order): lane = pixel.  Per k-step of 8 survivors: first the eight footprint
 			// evaluations (independent, they overlap in the pipeline), then the short sequential recurrence on T and S. ----
 #pragma unroll 1
@@ -333,44 +390,6 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			}
 			cp_async_commit();
 			BWD_PH_LAP(ph, BWD_PH_ROW_ISSUE);
-		};
-
-		// GEMM 1 of the chunk whose channel rows sit in s_rows, into s_xs
-		auto gemm1 = [&](const float* s_rows, float* s_xs) {
-			// ---- 2. GEMM 1: Wd[p][j] = Gpx[p][:] . C[j][:]   (M = pixels (2 tiles), N = survivors, K = channels) ----
-			float wd[2][BWD_CH / 8][4];
-#pragma unroll
-			for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-				for (int nt = 0; nt < BWD_CH / 8; nt++)
-#pragma unroll
-					for (int i = 0; i < 4; i++) wd[mt][nt][i] = 0.f;
-#pragma unroll
-			for (int ks = 0; ks < NT; ks++) {
-				uint32_t ahi[2][4], alo[2][4];
-#pragma unroll
-				for (int mt = 0; mt < 2; mt++) {
-					const float4 v = *reinterpret_cast<const float4*>(s_g + (8 * mt + gid) * GS + (8 * ks + 2 * tig) * 2);
-					tf32_split(v.x, ahi[mt][0], alo[mt][0]); tf32_split(v.y, ahi[mt][1], alo[mt][1]);
-					tf32_split(v.z, ahi[mt][2], alo[mt][2]); tf32_split(v.w, ahi[mt][3], alo[mt][3]);
-				}
-#pragma unroll
-				for (int nt = 0; nt < BWD_CH / 8; nt++) {
-					const float2 v = *reinterpret_cast<const float2*>(s_rows + (8 * nt + gid) * RS + 8 * ks + 2 * tig);
-					uint32_t bh0, bl0, bh1, bl1;
-					tf32_split(v.x, bh0, bl0);
-					tf32_split(v.y, bh1, bl1);
-					mma_3xtf32(wd[0][nt], ahi[0], alo[0], bh0, bh1, bl0, bl1);
-					mma_3xtf32(wd[1][nt], ahi[1], alo[1], bh0, bh1, bl0, bl1);
-				}
-			}
-			// D fragment (mt, nt): pixels (pi = 8 mt + gid, e = 0 | 1), survivors 8 nt + 2 tig (+1): one 16-byte store
-#pragma unroll
-			for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-				for (int nt = 0; nt < BWD_CH / 8; nt++)
-					*reinterpret_cast<float4*>(s_xs + (8 * mt + gid) * XS + (4 * nt + tig) * 4) =
-						make_float4(wd[mt][nt][0], wd[mt][nt][1], wd[mt][nt][2], wd[mt][nt][3]);
 		};
 
 		// walked chunk of cnt survivors (records s_q, wgt tile s_wgt, q tile s_xs): GEMM 2/3, then between() (the wgt tile
@@ -519,10 +538,10 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			BWD_PH_LAP(ph, BWD_PH_FLUSH);
 		};
 
-		// Chunk k: its records arrive in record slot r and its channel rows in stage k & 1, GEMM 1 runs as soon as the rows are
-		// in, and the chunk is handed to W.  Then C finishes chunk k - 1 in stage (k - 1) & 1, and as soon as GEMM 2 has read
-		// that stage's wgt tile the rows of chunk k + 1 start travelling into it, during the flush.  Record slot r + 1 (mod 3)
-		// last held chunk k - 2, flushed in the previous trip.
+		// Chunk k: its records arrive in record slot r and its channel rows in stage k & 1, and the chunk is handed to W as
+		// soon as the rows are in.  Then C finishes chunk k - 1 in stage (k - 1) & 1, and as soon as GEMM 2 has read that
+		// stage's wgt tile the rows of chunk k + 1 start travelling into it, during the flush.  Record slot r + 1 (mod 3) last
+		// held chunk k - 2, flushed in the previous trip.
 		int cnt = next_chunk(s_rec[0]), cnt_prev = 0;
 		int r = 0, rp = BWD_NREC - 1;
 		auto rows_of = [&](int c, float4* rec, float* rows) {  // the chunk's records are in flight: carry the masks, gather its rows
@@ -540,9 +559,11 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			const int rn = r == BWD_NREC - 1 ? 0 : r + 1;
 			if (cnt > 0) {
 				cp_async_wait<0>();  // this chunk's channel rows
-				__syncwarp();
-				BWD_PH_LAP(ph, BWD_PH_ROW_WAIT);
-				gemm1(s_rows[s], s_x[s]);
+				if (!W_GEMM1) {
+					__syncwarp();
+					BWD_PH_LAP(ph, BWD_PH_ROW_WAIT);
+					gemm1(s_rows[s], s_x[s]);
+				}
 #ifdef MGS_BWD_PHASES
 				ph.acc[BWD_PH_CHUNKS]++;
 #endif
@@ -550,7 +571,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			if (lane == 0) s_cnt[s] = cnt;
 			__syncwarp();
 			named_bar_arrive<BWD_BAR_FULL, 64>(s);
-			BWD_PH_LAP(ph, BWD_PH_GEMM1);
+			BWD_PH_LAP(ph, W_GEMM1 ? BWD_PH_ROW_WAIT : BWD_PH_GEMM1);
 			const int cnt_next = cnt > 0 ? next_chunk(s_rec[rn]) : 0;  // the next chunk's records travel while this one is finished
 			// the scalar-row path loads synchronously, nothing would travel during the flush: it gathers after it (registers)
 			auto next_rows = [&]() { rows_of(cnt_next, s_rec[rn], s_rows[s ^ 1]); };

@@ -68,14 +68,14 @@ enum BwdPhase {
 	BWD_PH_QUEUE,      // queue the next chunk's survivors, start its record gather
 	BWD_PH_REC_WAIT,   // wait for the next chunk's records
 	BWD_PH_ROW_ISSUE,  // issue the next chunk's channel-row copies
-	BWD_PH_ROW_WAIT,   // wait for this chunk's channel rows
-	BWD_PH_GEMM1,      // GEMM 1 and the FULL signal
+	BWD_PH_ROW_WAIT,   // wait for this chunk's channel rows (and the FULL signal when the walker runs GEMM 1)
 	BWD_PH_DONE_WAIT,  // wait for the walker to finish the previous chunk
 	BWD_PH_GEMM23,     // GEMM 2/3 of the previous chunk
 	BWD_PH_FLUSH,      // its reductions
 	BWD_PH_C_TOTAL,    // the companion's whole loop
 	// walker
 	BWD_PH_FULL_WAIT,  // wait for the next chunk
+	BWD_PH_GEMM1,      // its GEMM 1 (at small F the companion's, with the FULL signal: W_GEMM1 in blend_bwd.cu)
 	BWD_PH_WALK,       // walk it
 	BWD_PH_W_TOTAL,    // the walker's whole loop
 	BWD_PH_CHUNKS,     // chunks (non-empty) handed over
@@ -97,14 +97,15 @@ struct BwdPhaseClock {
 		acc[ph] += (unsigned int)(n - t);
 		t = n;
 	}
-	// total: the phase that receives the whole loop; phases [first, last] are this warp's
+	// total: the phase that receives the whole loop; phases [first, last] are this warp's, and the lead (the companion)
+	// also adds GEMM 1, which stays zero on the warp that does not run it
 	__device__ __forceinline__ void put(unsigned long long* out, int first, int last, int total, bool lead)
 	{
 		acc[total] = (unsigned int)(clock64() - t0);
 		if (out == nullptr || (threadIdx.x & 31) != 0) return;
 #pragma unroll
 		for (int i = 0; i < BWD_PH_COUNT; i++)
-			if ((i >= first && i <= last) || i == total || (lead && (i == BWD_PH_CHUNKS || i == BWD_PH_CTAS)))
+			if ((i >= first && i <= last) || i == total || (lead && (i == BWD_PH_GEMM1 || i == BWD_PH_CHUNKS || i == BWD_PH_CTAS)))
 				atomicAdd(out + i, (unsigned long long)acc[i]);
 	}
 };

@@ -16,8 +16,8 @@ import torch
 import bench
 from manigaussian_b200 import _binding
 
-PHASES = ["queue", "record_wait", "row_issue", "row_wait", "gemm1", "done_wait", "gemm23", "flush", "companion_loop",
-          "full_wait", "walk", "walker_loop", "chunks", "ctas"]
+PHASES = ["queue", "record_wait", "row_issue", "row_wait", "done_wait", "gemm23", "flush", "companion_loop",
+          "full_wait", "gemm1", "walk", "walker_loop", "chunks", "ctas"]
 
 wl = dict(bench.WORKLOADS[sys.argv[1] if len(sys.argv) > 1 else "c3"])
 steps = int(sys.argv[2]) if len(sys.argv) > 2 else 20
