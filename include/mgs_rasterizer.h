@@ -128,7 +128,9 @@ int mgs_forward_begin(
 /*
  * Backward.  Replaces CudaRasterizer::Rasterizer::backward (rasterizer.h:62-91, rasterizer_impl.cu:359-463).
  *   dL_dpix [3,H,W], dL_dpix_F [F,H,W] or NULL, dL_dpix_depth [H,W] or NULL.
- *   Outputs (each fully written; NULL allowed for dL_dconic, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot):
+ *   Outputs (each fully written; NULL allowed for dL_dconic, dL_dcolor, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, each on
+ *   its own: dL_dmean3D keeps the SH view-direction term without dL_dsh; dL_dscale / dL_drot are zeros without scales and rotations;
+ *   dL_dconic, a single-view output, is written only with accumulate = 0, zeros for the Gaussians the view culled):
  *     dL_dmean2D [P,3], dL_dconic [P,4] (slots x,y,w like the reference's float4), dL_dopacity [P],
  *     dL_dcolor [P,3], dL_dfeature [P,F], dL_dmean3D [P,3], dL_dcov3D [P,6], dL_dsh [P,M,3],
  *     dL_dscale [P,3], dL_drot [P,4].
@@ -292,7 +294,8 @@ int mgs_backward_views(
  * (overwritten, or added to with accumulate = 1); NULL-ability as in mgs_backward, except:
  *   - dL_dfeature NULL on a cloud with features: its feature gradient is not computed, but the feature cotangents still
  *     reach its mean, conic and opacity gradients;
- *   - shs without dL_dsh is MGS_ERR_INVALID_ARG: dL_dsh comes with the view-direction term of dL_dmean3D.
+ *   - shs without dL_dsh is MGS_ERR_INVALID_ARG, checked before anything is enqueued (mgs_backward and mgs_backward_views
+ *     accept it and keep the view-direction term of dL_dmean3D; this entry point keeps its stricter check).
  * Argument errors (B <= 0, bad view_offsets, P <= 0, missing pointers) return MGS_ERR_INVALID_ARG before anything is enqueued.
  */
 typedef struct mgs_cloud {

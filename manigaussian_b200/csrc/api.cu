@@ -585,12 +585,15 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		if (rc < 0) return rc;
 	}  // blend stage: dL_dfeature is final here -- a caller may start exchanging it while the per-Gaussian stage runs
 	if (!(stages & 2)) return 0;
-	const bool have_sr = c.scales && c.rotations && dL_dscale && dL_drot;
+	// the chain to scale / rotation runs when either gradient is asked for; without scales (cov3D_precomp) the rows
+	// asked for are written as zeros.  shs are read whether or not dL_dsh is asked for: they carry the view-direction
+	// term of dL_dmean3D.
+	const bool have_sr = c.scales && c.rotations && (dL_dscale || dL_drot);
 	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
 		cudaStream_t st = join;
 		ProjectBwdViewsArgs pb{};
 		pb.P = P; pb.D = c.D; pb.M = c.M; pb.V = std::min(V - v0, (int)MAX_BWD_VIEWS);
-		pb.means3D = c.means3D; pb.shs = (c.shs && dL_dsh) ? c.shs : nullptr;
+		pb.means3D = c.means3D; pb.shs = c.shs;
 		pb.scales = have_sr ? c.scales : nullptr; pb.rotations = c.rotations; pb.scale_modifier = c.scale_modifier;
 		pb.cov3D_precomp = c.cov3D_precomp;
 		if (!have_sr && !c.cov3D_precomp) {
@@ -600,7 +603,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		pb.accumulate = (accumulate || v0 > 0) ? 1 : 0;
 		pb.shared_mean2D = shared_mean2D;
 		pb.dL_dmean3D = dL_dmean3D; pb.dL_dopacity = dL_dopacity; pb.dL_dcolor = dL_dcolor; pb.dL_dcov3D = dL_dcov3D;
-		pb.dL_dsh = pb.shs ? dL_dsh : nullptr; pb.dL_dscale = have_sr ? dL_dscale : nullptr; pb.dL_drot = have_sr ? dL_drot : nullptr;
+		pb.dL_dsh = dL_dsh; pb.dL_dscale = dL_dscale; pb.dL_drot = dL_drot;
 		pb.dL_dconic = pb.accumulate ? nullptr : dL_dconic;
 		for (int u = 0; u < pb.V; u++)
 			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
@@ -1107,7 +1110,7 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 	};
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
-		const bool have_sr = k.scales && k.rotations && k.dL_dscale && k.dL_drot;
+		const bool have_sr = k.scales && k.rotations && (k.dL_dscale || k.dL_drot);  // as in backward_views
 		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
 			const int n = std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS);
 			if (nv + n > MAX_BWD_VIEWS) {
@@ -1121,7 +1124,7 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 			pc.cov3D_precomp = (have_sr || k.cov3D_precomp) ? k.cov3D_precomp : carve_view(views[view_offsets[b]], k.P).geom.cov3D;
 			pc.accumulate = (accumulate || v0 > view_offsets[b]) ? 1 : 0;
 			pc.dL_dmean3D = k.dL_dmean3D; pc.dL_dopacity = k.dL_dopacity; pc.dL_dcolor = k.dL_dcolor; pc.dL_dcov3D = k.dL_dcov3D;
-			pc.dL_dsh = k.shs ? k.dL_dsh : nullptr; pc.dL_dscale = have_sr ? k.dL_dscale : nullptr; pc.dL_drot = have_sr ? k.dL_drot : nullptr;
+			pc.dL_dsh = k.dL_dsh; pc.dL_dscale = k.dL_dscale; pc.dL_drot = k.dL_drot;
 			for (int u = 0; u < n; u++) {
 				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
 				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;

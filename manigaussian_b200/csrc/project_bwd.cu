@@ -138,7 +138,10 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			}
 #pragma unroll
 			for (int c = 0; c < 3; c++) { u0[c] = dot3(S[c], m0); u1[c] = dot3(S[c], m1); }  // S M^T (S symmetric)
-			const float ca = dot3(m0, u0) + 0.3f, cb = dot3(m0, u1), cc = dot3(m1, u1) + 0.3f;
+			// a0, c0: the covariance before the low-pass, kept for AA (recovering them as ca - 0.3 would cancel to a relative
+			// error of u 0.3 / c0 on exactly the thin splats the compensation acts on)
+			const float a0 = dot3(m0, u0), c0 = dot3(m1, u1);
+			const float ca = a0 + 0.3f, cb = dot3(m0, u1), cc = c0 + 0.3f;
 			const float det = ca * cc - cb * cb;
 			const float wgt = 1.0f / (det * det + 0.0000001f);
 			// H = -w adj(S') G adj(S')
@@ -147,8 +150,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			if (AA) {
 				// opacity compensation: grad d0 = (c0, -2b, a0), grad d1 = (c, -2b, a) w.r.t. (a, b, c), b one variable;
 				// H01 is the gradient w.r.t. ONE off-diagonal entry, so it takes half of the b term
-				const float a0 = ca - 0.3f, c0 = cc - 0.3f;
-				const float d0 = fmaf(-cb, cb, a0 * c0);
+				const float d0 = fmaf(-cb, cb, a0 * c0);  // as the forward's det0
 				const float r = d0 / det;
 				gop += sqrtf(fmaxf(2.5e-5f, r)) * g1.y;
 				if (r > 2.5e-5f) {
@@ -226,6 +228,9 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				const float along = x * dd[0] + y * dd[1] + z * dd[2];
 				gp[0] += (dd[0] - x * along) * il; gp[1] += (dd[1] - y * along) * il; gp[2] += (dd[2] - z * along) * il;
 			}
+		} else if (a.dL_dconic && v == 0) {  // culled: the row is still written (the reference's zero-fill)
+			float* o = a.dL_dconic + 4 * (size_t)idx;
+			o[0] = 0.f; o[1] = 0.f; o[2] = 0.f; o[3] = 0.f;
 		}
 		// this view's screen-space gradient row (the reference's dL_dmeans2D, [P,3] with z = 0)
 		if (a.shared_mean2D) { gm2[0] += dm[0]; gm2[1] += dm[1]; }

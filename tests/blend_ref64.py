@@ -25,8 +25,10 @@ U = 2.0 ** -24
 # Bound scale per checked quantity: 4x the largest |x - ref| / (u B) measured for that quantity over the C oracle and the
 # stored outputs of the compiled reference on the four golden scenes (tests/test_blend_ref64_cpu.py) and both blend
 # kernels on every scene of tests/test_blend_pairs_gpu.py (H100 SXM).  The measured ratios are in those tests' docstrings.
+# dL_ddepth (w^T g_depth, the per-Gaussian depth cotangent), which the kernels keep in their blend-stage record only, is
+# measured against the C oracle's blend with the depth as a feature channel (test_depth_cotangent_matches_oracle_per_element).
 KAPPA = dict(color=14.5, feature=24.0, depth=11.1, final_T=7.1, alpha=2.0,
-             dL_dmeans2D=0.23, dL_dconic=0.012, dL_dopacity=0.7, dL_dcolors=1.6, dL_dfeature=5.3, dL_dcov3D=0.035)
+             dL_dmeans2D=0.23, dL_dconic=0.012, dL_dopacity=0.7, dL_dcolors=1.6, dL_ddepth=0.26, dL_dfeature=5.3)
 
 
 def tile_pixels(W, H, tile):
@@ -168,7 +170,7 @@ def new_out(st):
                                        ("final_T", (H, W)), ("final_T_B", (H, W)), ("alpha", (H, W)), ("alpha_B", (H, W)))}
     out["n_contrib"] = np.zeros((H, W), np.int64)
     for k, s in (("dL_dmeans2D", (P, 2)), ("dL_dconic", (P, 3)), ("dL_dopacity", (P,)), ("dL_dcolors", (P, 3)),
-                 ("dL_dfeature", (P, F))):
+                 ("dL_ddepth", (P,)), ("dL_dfeature", (P, F))):
         out[k] = np.zeros(s)
         out[k + "_B"] = np.zeros(s)
     return out
@@ -262,6 +264,9 @@ def blend_tile(st, tile, m, out, backward=True):
     ge = np.abs(w) * e
     np.add.at(out["dL_dcolors"], ids, w.T @ g[:, :3])
     np.add.at(out["dL_dcolors_B"], ids, ge.T @ np.abs(g[:, :3]))
+    if has_d:
+        np.add.at(out["dL_ddepth"], ids, w.T @ g[:, 3])
+        np.add.at(out["dL_ddepth_B"], ids, ge.T @ np.abs(g[:, 3]))
     if F:
         np.add.at(out["dL_dfeature"], ids, w.T @ g[:, nch:])
         np.add.at(out["dL_dfeature_B"], ids, ge.T @ np.abs(g[:, nch:]))
@@ -293,55 +298,3 @@ def ratio(got, ref, B, quantity, kappa=None):
     """|got - ref| / (kappa u B + tiny), elementwise; kappa defaults to KAPPA[quantity] (kappa = 1: the raw ratio)."""
     k = KAPPA[quantity] if kappa is None else kappa
     return np.abs(np.asarray(got, np.float64) - ref) / (k * U * B + 1e-30)
-
-
-def cov3d_grad(ref, means3D, cov3D, viewmatrix, W, H, tanfovx, tanfovy):
-    """dL_dcov3D [P,6] and its bound from the blend-stage dL_dconic of `ref` (a blend() result), in float64: the
-    reference's computeCov2D backward (backward.cu:144-274, restated in oracle/gs_oracle.c gso_preprocess_backward) for
-    callers that pass cov3D_precomp.  The bound carries the conic gradient's own bound through the same linear map, plus
-    the chain's rounding: the 2D covariance's determinant cancels by (ac + b^2) / det for elongated splats."""
-    vm = np.asarray(viewmatrix, np.float64).reshape(-1)
-    p = np.asarray(means3D, np.float64)
-    V3 = np.asarray(cov3D, np.float64)
-    t = np.stack([vm[0] * p[:, 0] + vm[4] * p[:, 1] + vm[8] * p[:, 2] + vm[12],
-                  vm[1] * p[:, 0] + vm[5] * p[:, 1] + vm[9] * p[:, 2] + vm[13],
-                  vm[2] * p[:, 0] + vm[6] * p[:, 1] + vm[10] * p[:, 2] + vm[14]], 1)
-    fx, fy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
-    limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
-    tz = t[:, 2]
-    tx = np.clip(t[:, 0] / tz, -limx, limx) * tz
-    ty = np.clip(t[:, 1] / tz, -limy, limy) * tz
-    n = len(p)
-    J = np.zeros((n, 3, 3))
-    J[:, 0, 0], J[:, 0, 2] = fx / tz, -(fx * tx) / (tz * tz)
-    J[:, 1, 1], J[:, 1, 2] = fy / tz, -(fy * ty) / (tz * tz)
-    Wm = np.array([[vm[0], vm[4], vm[8]], [vm[1], vm[5], vm[9]], [vm[2], vm[6], vm[10]]])
-    T = J @ Wm                                  # gs_oracle.c m3mul(W, J) in row-major numpy terms
-    Vr = np.stack([V3[:, [0, 1, 2]], V3[:, [1, 3, 4]], V3[:, [2, 4, 5]]], 1)
-    cov = T @ Vr @ np.transpose(T, (0, 2, 1))
-    a, b, c = cov[:, 0, 0] + 0.3, cov[:, 0, 1], cov[:, 1, 1] + 0.3
-    det = a * c - b * b
-    w = 1.0 / (det * det + 1e-7)
-    g0, g1, g2 = (ref["dL_dconic"][:, i] for i in range(3))
-    B0, B1, B2 = (ref["dL_dconic_B"][:, i] for i in range(3))
-    dA = w * (-c * c * g0 + 2 * b * c * g1 - b * b * g2)
-    dC = w * (-a * a * g2 + 2 * a * b * g1 - b * b * g0)
-    dB = w * 2 * (b * c * g0 - (det + 2 * b * b) * g1 + a * b * g2)
-    e = 16.0 + 8.0 * (a * c + b * b) / np.abs(det)
-    ab, bb, cb = np.abs(a), np.abs(b), np.abs(c)
-    dA_B = w * (c * c * (B0 + e * abs(g0)) + 2 * bb * cb * (B1 + e * abs(g1)) + b * b * (B2 + e * abs(g2)))
-    dC_B = w * (a * a * (B2 + e * abs(g2)) + 2 * ab * bb * (B1 + e * abs(g1)) + b * b * (B0 + e * abs(g0)))
-    dB_B = w * 2 * (bb * cb * (B0 + e * abs(g0)) + (abs(det) + 2 * b * b) * (B1 + e * abs(g1)) + ab * bb * (B2 + e * abs(g2)))
-    out, outB = np.zeros((n, 6)), np.zeros((n, 6))
-    A = np.abs(T)
-    for k, (i, j) in enumerate(((0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2))):
-        f = 1.0 if i == j else 2.0   # off-diagonal entries appear twice in the symmetric cov3D
-        # dcov[ij] = f/2 (T0i T0j + T0j T0i) dA + (T0i T1j + T0j T1i)/ (2/f) dB + f/2 (T1i T1j + T1j T1i) dC
-        ca = 0.5 * f * (T[:, 0, i] * T[:, 0, j] + T[:, 0, j] * T[:, 0, i])
-        cb_ = (T[:, 0, i] * T[:, 1, j] + T[:, 0, j] * T[:, 1, i]) * (0.5 if i == j else 1.0)
-        cc = 0.5 * f * (T[:, 1, i] * T[:, 1, j] + T[:, 1, j] * T[:, 1, i])
-        out[:, k] = ca * dA + cb_ * dB + cc * dC
-        ca_, cbb, ccc = (0.5 * f * 2 * A[:, 0, i] * A[:, 0, j], (A[:, 0, i] * A[:, 1, j] + A[:, 0, j] * A[:, 1, i]) *
-                         (0.5 if i == j else 1.0), 0.5 * f * 2 * A[:, 1, i] * A[:, 1, j])
-        outB[:, k] = ca_ * (dA_B + 4 * abs(dA)) + cbb * (dB_B + 4 * abs(dB)) + ccc * (dC_B + 4 * abs(dC))
-    return out, outB

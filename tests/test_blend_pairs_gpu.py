@@ -15,16 +15,17 @@ these and of the CPU-side ratios, per quantity):
 
 | scene | colour | depth | final_T | alpha | features | dmeans2D | dopacity | dcolors | dfeature | dcov3D |
 |---|---|---|---|---|---|---|---|---|---|---|
-| lists (F 3 / 40) | 2.42 | 1.98 | 0.16 | 0.28 | 1.57 / 3.45 | 0.0079 | 0.043 | 0.12 | 0.24 | 0.0025 |
-| term32 / term64 | 2.56 | 2.57 | 0.37 | 0.49 | 0.76 | 0.0029 | 0.0054 | 0.017 | 0.043 | 0.0018 |
-| empty_run (F 3 / 67) | 0.64 | 0.61 | 0.31 | 0.36 | 1.26 | 0.0033 | 0.0058 | 0.056 | 0.10 | 0.0027 |
-| needles | 1.58 | 2.20 | 0.37 | 0.33 | 3.81 | 0.0033 | 0.0078 | 0.037 | 0.033 | 0.0014 |
-| offscreen | 0.79 | 0.88 | 0.21 | 0.21 | 1.43 | 0.0029 | 0.0053 | 0.029 | 0.036 | 0.0029 |
-| opacity (F 32 / 67) | 1.55 | 0.91 | 0.31 | 0.49 | 2.52 | 0.0028 | 0.049 | 0.19 | 0.17 | 0.0015 |
-| ragged (F 0-67) | 2.89 | 1.78 | 0.10 | 0.48 | 2.49 | 0.011 | 0.030 | 0.065 | 0.14 | 0.0048 |
+| lists (F 3 / 40) | 2.42 | 1.98 | 0.16 | 0.28 | 1.57 / 3.45 | 0.0079 | 0.043 | 0.12 | 0.24 | 0 |
+| term32 / term64 | 2.56 | 2.57 | 0.37 | 0.49 | 0.76 | 0.0029 | 0.0054 | 0.017 | 0.043 | 0 |
+| empty_run (F 3 / 67) | 0.64 | 0.61 | 0.31 | 0.36 | 1.26 | 0.0033 | 0.0058 | 0.056 | 0.10 | 0 |
+| needles | 1.58 | 2.20 | 0.37 | 0.33 | 3.81 | 0.0033 | 0.0078 | 0.037 | 0.033 | 0 |
+| offscreen | 0.79 | 0.88 | 0.21 | 0.21 | 1.43 | 0.0029 | 0.0053 | 0.029 | 0.036 | 0 |
+| opacity (F 32 / 67) | 1.55 | 0.91 | 0.31 | 0.49 | 2.52 | 0.0028 | 0.049 | 0.19 | 0.17 | 0 |
+| ragged (F 0-67) | 2.89 | 1.78 | 0.10 | 0.48 | 2.49 | 0.011 | 0.030 | 0.065 | 0.14 | 0 |
 | ragged_f32 | 3.63 | 2.77 | 0.11 | 0.48 | 1.60 | 0.0054 | 0.010 | - | 0.072 | - |
 | sh3_big | 1.48 | 1.23 | 0.19 | 0.22 | 1.60 | 0.0100 | 0.017 | - | 0.12 | - |
 
+dcov3D: project_ref64.cov3d_grad, the raw ratio of the part the inherited conic bound does not cover, over u e.
 No cull violation in any scene; borderline pixels 0.12 % (needles), 0.10 % (opacity), 0.09 % (ragged_f32), 0 elsewhere.
 All 17 cases take about 10 s.
 """
@@ -32,6 +33,7 @@ import numpy as np
 import pytest
 
 import blend_ref64 as R64
+import project_ref64 as P64
 import util
 from manigaussian_b200 import scenes
 
@@ -394,10 +396,14 @@ def test_blend_pairs(scene, F):
     if k["dL_dcov3D"] is not None:
         # the conic gradients (GEMM 3's six moments) through the output the ABI returns for cov3D_precomp
         cam, g = inp["cam"], inp["g"]
-        c3, c3B = R64.cov3d_grad(ref, g["means3D"], g["cov3D_precomp"], cam["viewmatrix"], W, H, cam["tanfovx"], cam["tanfovy"])
-        live = k["radii"] > 0
-        problems.append(_check("(d) dL_dcov3D", k["dL_dcov3D"][live], c3[live], c3B[live],
-                               lambda u: _where_gaussian(k, np.nonzero(live)[0][u[0]]), report))
+        c3, bd = P64.cov3d_grad(ref, g, cam, live=k["radii"] > 0)
+        ok = (k["radii"] > 0) & ~bd
+        r = P64.raw_ratio(k["dL_dcov3D"][ok], tuple(np.broadcast_to(x, c3[0].shape)[ok] for x in c3))
+        report["(d) dL_dcov3D raw"] = float(r.max()) if r.size else 0.0
+        if r.size and r.max() > P64.KAPPA["dL_dcov3D"]:
+            i = np.argsort(r.max(1))[::-1][:5]
+            problems.append(f"(d) dL_dcov3D: {int((r > P64.KAPPA['dL_dcov3D']).any(1).sum())} Gaussians out of bound; worst "
+                            f"{[(_where_gaussian(k, np.nonzero(ok)[0][j]), float(r[j].max())) for j in i]}")
     print(f"[{scene} F={F}] " + " ".join(f"{a}={b:.3g}" for a, b in report.items()))
     _assert_edge(scene, k, st, ours)
     problems = [p for p in problems if p]

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 import blend_ref64 as R64
+import project_ref64 as P64
 import util
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "g[0-9]*.npz")))
@@ -50,7 +51,8 @@ def _golden(path):
 def test_reference_matches_oracle_and_golden_per_element(path):
     """Worst raw ratio |x - ref64| / (u B), C oracle / compiled reference: colour 0.34/1.62, final_T 0.22/1.77, features
     0.37/5.98, dL_dmeans2D 0.0048/0.057, dL_dopacity 0.019/0.17, dL_dcolors 0.069 (oracle) and 0.042/0.39 (g3),
-    dL_dfeature 0.072/1.32, dL_dconic 0.0029 (oracle), dL_dcov3D 0.0014/0.0087 (g3); the largest of each over g1-g4."""
+    dL_dfeature 0.072/1.32, dL_dconic 0.0029 (oracle), dL_dcov3D 0/0 (g3); the largest of each over g1-g4.  dL_dcov3D is chained by
+    project_ref64.cov3d_grad: the raw ratio of the part its inherited conic bound does not cover, over u e."""
     z, inp, fw, bw = _golden(path)
     st = oracle_state(inp, fw)
     T = st["ranges"].shape[0]
@@ -85,9 +87,12 @@ def test_reference_matches_oracle_and_golden_per_element(path):
         if src == "oracle":
             rows.append(worst(src + " dL_dconic", g["dL_dconic"][:, [0, 1, 3]], ref["dL_dconic"], ref["dL_dconic_B"]))
         if inp["g"]["cov3D_precomp"] is not None:
-            c3, c3B = R64.cov3d_grad(ref, inp["g"]["means3D"], inp["g"]["cov3D_precomp"], inp["cam"]["viewmatrix"], W, H,
-                                     inp["cam"]["tanfovx"], inp["cam"]["tanfovy"])
-            rows.append(worst(src + " dL_dcov3D", g["dL_dcov3D"][keep_g], c3[keep_g], c3B[keep_g]))
+            # the conic gradients chained to dL_dcov3D by the projection reference (tests/project_ref64.py)
+            c3, bd = P64.cov3d_grad(ref, inp["g"], inp["cam"], live=fw["radii"] > 0)
+            ok = keep_g & ~bd
+            r = P64.raw_ratio(g["dL_dcov3D"][ok], tuple(np.broadcast_to(x, c3[0].shape)[ok] for x in c3))
+            raw = float(r.max()) if r.size else 0.0
+            rows.append((src + " dL_dcov3D", raw / P64.KAPPA["dL_dcov3D"], raw))
         if inp["g"]["colors_precomp"] is not None:
             rows.append(worst(src + " dL_dcolors", g["dL_dcolors"][keep_g], ref["dL_dcolors"][keep_g], ref["dL_dcolors_B"][keep_g]))
         else:
@@ -97,6 +102,35 @@ def test_reference_matches_oracle_and_golden_per_element(path):
     print(os.path.basename(path), " ".join(f"{k}={v:.3g}(raw {r:.3g})" for k, v, r in rows))
     bad = [(k, v) for k, v, _ in rows if not v <= 1.0]
     assert not bad, bad
+
+
+@pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p)[:-4] for p in GOLDEN])
+def test_depth_cotangent_matches_oracle_per_element(path):
+    """The per-Gaussian depth cotangent dL_ddepth = w^T g_depth against the C oracle's blend backward with the view-space
+    depth as its one feature channel (the oracle renders no depth plane).  Worst raw ratio |x - ref64| / (u B) over g1-g4:
+    0.018 / 0.042 / 0.050 / 0.064."""
+    from oracle import gs_oracle as O
+    z = np.load(path)
+    kw = json.loads(bytes(z["recipe"]).decode())
+    if "bg" in kw:
+        kw["bg"] = tuple(kw["bg"])
+    kw["F"] = 0
+    inp = util.make_inputs(**kw, depth=True)
+    g, cam, ct = inp["g"], inp["cam"], inp["ct"]
+    vm = np.asarray(cam["viewmatrix"], np.float32).reshape(-1)
+    depth = (g["means3D"] @ np.array([vm[2], vm[6], vm[10]], np.float32) + vm[14]).astype(np.float32)
+    okw = dict(scales=g["scales"], rotations=g["rotations"], cov3D_precomp=g["cov3D_precomp"], shs=g["shs"],
+               sh_degree=g["sh_degree"], colors_precomp=g["colors_precomp"], feature=depth[:, None])
+    fw = O.forward(g["means3D"], g["opacities"], cam["viewmatrix"], cam["projmatrix"], cam["campos"], inp["W"], inp["H"],
+                   cam["tanfovx"], cam["tanfovy"], inp["bg"], **okw)
+    bw = O.backward(fw, ct["dL_dcolor"], ct["dL_ddepth"][None], g["means3D"], cam["viewmatrix"], cam["projmatrix"],
+                    cam["campos"], cam["tanfovx"], cam["tanfovy"], inp["bg"], **okw)
+    st = dict(oracle_state(dict(inp, F=0), fw), depth=depth, g_depth=ct["dL_ddepth"])
+    masks = [R64.decide_fp32(st, t) for t in range(st["ranges"].shape[0])]
+    ref = R64.blend(st, masks)
+    r = R64.ratio(bw["dL_dfeature"][:, 0], ref["dL_ddepth"], ref["dL_ddepth_B"], "dL_ddepth", kappa=1.0)
+    print(os.path.basename(path), f"dL_ddepth raw {r.max():.3g}")
+    assert r.max() <= R64.KAPPA["dL_ddepth"]
 
 
 def _loss(st, masks):
