@@ -586,6 +586,73 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
 	int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
+/*
+ * Camera gradients (no reference counterpart: the reference's backward returns None for the camera).  The calls below are
+ * the _ssim backward calls with one more argument, `cam`: one mgs_view_camera_grad per view (V entries, or view_offsets[B]
+ * for clouds), or NULL; the _ssim backward calls are these with cam == NULL.  An entry asks for the gradients of its view
+ * when any of its three outputs is non-NULL; each output is written (accumulate = 0) or added to (accumulate = 1) by the
+ * per-Gaussian stage (stage 2), a NULL output is skipped.  An entry with an output but no scratch returns
+ * MGS_ERR_INVALID_ARG before anything is enqueued.
+ *
+ * Definition.  With vm the view's viewmatrix (Rv[r][c] = vm[4c + r], tv[r] = vm[12 + r]), pm its projmatrix read the same
+ * way, and, per Gaussian p of the view with radius > 0, the chain rule of the per-Gaussian backward:
+ *   t = Rv p + tv; dt = dL/dt with the x/y frustum clamp masking d/dt.x, d/dt.y and the depth cotangent on t.z;
+ *   Q = [q0; q1] = dL/dM = 2 H M S (H including the anti-aliased compensation), cx, cy the clamped t.x, t.y;
+ *   dm = the screen-mean cotangent, (hx, hy, hw) = P (p, 1), iw = 1 / (hw + 1e-7), kx = hx iw^2, ky = hy iw^2;
+ * the gradients are the sums over those Gaussians of
+ *   dL/dvm[4c + r] = dt[r] p[c] + (J^T Q)[r][c]   (r, c < 3; J held at its value:
+ *                    (J^T Q)[0] = fx / tz q0, (J^T Q)[1] = fy / tz q1, (J^T Q)[2] = -fx cx / tz^2 q0 - fy cy / tz^2 q1)
+ *   dL/dvm[12 + r] = dt[r];  dL/dvm[3], [7], [11], [15] = 0 (the forward never reads them)
+ *   dL/dpm[4c] = dm0 iw ph[c],  dL/dpm[4c + 1] = dm1 iw ph[c],  dL/dpm[4c + 3] = -(dm0 kx + dm1 ky) ph[c],  ph = (p, 1);
+ *                    dL/dpm[4c + 2] = 0 (the forward does not use the clip-space z)
+ *   dL/dcampos = -(dd - dir along) / |v|  (v = p - campos, the SH branch's direction gradient dd and along = dir . dd: the
+ *                    view-direction term of dL/dmeans3D with the opposite sign; 0 without SHs).
+ * The gradient of a 16-float array is the gradient with respect to those 16 floats, so as a torch [4,4] it is directly the
+ * gradient of world_view_transform / full_proj_transform.  tan_fov, the focal lengths, the 1.3 tan_fov clamp limit, the
+ * near-plane cull, the radii and the tiles are constants: a projmatrix built from a learnable focal length receives only
+ * the screen-mean path.
+ * The sums are deterministic: every CTA of the per-Gaussian kernel writes one row of 27 partial sums per view into the
+ * entry's scratch in a fixed order, and a reduce kernel on join_stream sums each view's rows in a fixed tree.  A view's rows
+ * all come from one launch of at most 16 views.  These calls leave mgs_abi_version() at 300: they only add symbols, and a
+ * caller detects them by symbol, as the _ssim calls.
+ */
+typedef struct mgs_view_camera_grad {
+	float* dL_dviewmatrix;   /* device, 16 floats, or NULL */
+	float* dL_dprojmatrix;   /* device, 16 floats, or NULL */
+	float* dL_dcampos;       /* device, 3 floats, or NULL (zeros without SHs) */
+	float* scratch;          /* device, mgs_camera_grad_scratch_bytes(P) of the view's cloud */
+} mgs_view_camera_grad;
+
+size_t mgs_camera_grad_scratch_bytes(int P);
+int mgs_backward_views_cam(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -43,6 +43,11 @@ class ViewSsim(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("ssim_terms", "loss_acc", "cot_scale", "cot_color")]
 
 
+class ViewCameraGrad(C.Structure):
+    """mirror of `mgs_view_camera_grad` (include/mgs_rasterizer.h): the optional camera gradients of one view"""
+    _fields_ = [(n, C.c_void_p) for n in ("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "scratch")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -63,7 +68,7 @@ def lib():
     L = C.CDLL(path)
     L.mgs_abi_version.restype = C.c_int
     L.mgs_last_error.restype = C.c_char_p
-    for name in ("mgs_geometry_state_bytes", "mgs_binning_state_bytes", "mgs_backward_scratch_bytes"):
+    for name in ("mgs_geometry_state_bytes", "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_camera_grad_scratch_bytes"):
         getattr(L, name).restype = C.c_size_t
         getattr(L, name).argtypes = [C.c_int]
     L.mgs_image_state_bytes.restype = C.c_size_t
@@ -124,6 +129,12 @@ def lib():
         # ... and with the L1 + SSIM heads (one ViewSsim per view, or NULL) after the switch
         getattr(L, name + "_ssim").restype = C.c_int
         getattr(L, name + "_ssim").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + at[k:]
+        # ... and the backward with the camera gradients (one ViewCameraGrad per view, or NULL) after the L1 + SSIM heads
+        if "backward" in name:
+            cam = name.replace("_views", "_views_cam").replace("_clouds", "_clouds_cam")
+            getattr(L, cam).restype = C.c_int
+            getattr(L, cam).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim),
+                                                 C.POINTER(ViewCameraGrad)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -164,6 +175,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_aa", "mgs_backward_views_aa", "mgs_forward_clouds_aa", "mgs_backward_clouds_aa",
     "mgs_forward_views_ssim", "mgs_backward_views_ssim", "mgs_forward_clouds_ssim", "mgs_backward_clouds_ssim",
     "mgs_ssim", "mgs_ssim_backward",
+    "mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -231,6 +231,7 @@ size_t mgs_image_state_bytes(int width, int height)
 }
 size_t mgs_binning_state_bytes(int R) { return required([&](char*& p) { BinState::carve(p, (size_t)R); }); }
 size_t mgs_backward_scratch_bytes(int P) { return (size_t)P * GB_STRIDE * sizeof(float) + 128; }
+size_t mgs_camera_grad_scratch_bytes(int P) { return P > 0 ? camera_rows_bytes(P) : 0; }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -562,11 +563,32 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 	return pv;
 }
 
+// camera gradients of view v (cam: one entry per view, or NULL): an entry asks for them when it has an output
+static bool camera_on(const mgs_view_camera_grad* cam, int v)
+{
+	return cam && (cam[v].dL_dviewmatrix || cam[v].dL_dprojmatrix || cam[v].dL_dcampos);
+}
+static int check_camera(const mgs_view_camera_grad* cam, int V)
+{
+	for (int v = 0; v < V; v++)
+		if (camera_on(cam, v) && !cam[v].scratch)
+			return fail(MGS_ERR_INVALID_ARG, "camera gradients: an entry with an output needs scratch");
+	return 0;
+}
+// the view's rows pointer for its per-Gaussian launch, and its entry in that launch's reduce
+static void camera_view(const mgs_view_camera_grad* cam, int v, int P, float*& rows, CamReduceArgs& cr)
+{
+	if (!camera_on(cam, v)) return;
+	const mgs_view_camera_grad& e = cam[v];
+	rows = e.scratch;
+	cr.view[cr.V++] = CamReduceView{ e.scratch, (P + 127) / 128, e.dL_dviewmatrix, e.dL_dprojmatrix, e.dL_dcampos };
+}
+
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
-	const mgs_view_ssim* ssim, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -609,7 +631,11 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
 		pb.antialias = c.antialias;
 		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
-		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); }
+		CamReduceArgs cr{};
+		cr.accumulate = accumulate ? 1 : 0;
+		for (int u = 0; u < pb.V; u++) camera_view(cam, v0 + u, P, pb.cam_rows[u], cr);
+		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
+		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
 	}
 	return 0;
@@ -772,7 +798,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -932,6 +958,20 @@ int mgs_backward_views_ssim(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_cam(V, views, alpha, depth_mask, antialiasing, ssim, nullptr, P, D, M, F, means3D, shs, colors_precomp,
+		feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D,
+		dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_cam(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -945,9 +985,10 @@ int mgs_backward_views_ssim(
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 		if (rc < 0) return rc;
 	}
+	if (check_camera(cam, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1055,6 +1096,14 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
 	int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_cam(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, nullptr, D, M, F,
+		scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -1073,6 +1122,7 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 		}
 	}
 	const int V = view_offsets[B];
+	if (check_camera(cam, V) < 0) return MGS_ERR_INVALID_ARG;
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1098,14 +1148,18 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 	// per-Gaussian stage on `join`: launches of at most MAX_BWD_VIEWS views that pack whole clouds; a cloud with more views
 	// spans launches, and its later launches add to what the earlier ones wrote
 	const cudaStream_t st = join;
+	// a view's camera rows are summed by the reduce behind the one launch that holds the view
 	ProjectBwdCloudsArgs pb{};
 	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
+	CamReduceArgs cr{};
+	cr.accumulate = accumulate ? 1 : 0;
 	int nv = 0;  // views in pb
 	auto flush = [&]() -> int {
 		if (pb.B == 0) return 0;
-		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); }
+		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
-		pb.B = 0; nv = 0;
+		pb.B = 0; nv = 0; cr.V = 0;
+		for (float*& r : pb.cam_rows) r = nullptr;
 		return 0;
 	};
 	for (int b = 0; b < B; b++) {
@@ -1128,6 +1182,7 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
 			for (int u = 0; u < n; u++) {
 				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
 				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
+				camera_view(cam, v0 + u, k.P, pb.cam_rows[nv + u], cr);
 			}
 			nv += n;
 		}

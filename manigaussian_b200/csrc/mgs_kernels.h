@@ -75,7 +75,13 @@ struct ProjectBwdViewsArgs {
 	// AA = false kernels read their parameters at the same offsets and strides as before the mode existed.
 	int antialias;
 	const float4* conic_opacity[MAX_BWD_VIEWS];
+	// camera gradients (the launcher picks the CAM instantiation when any is set): view u's rows [CTAs of the launch][CAM_TERMS],
+	// one per CTA, or NULL.  Behind every other member for the same reason as conic_opacity.
+	float* cam_rows[MAX_BWD_VIEWS];
 };
+// the 27 camera terms one CTA writes per view: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1, 3}] at 12 + 3c + {0, 1,
+// 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.
+constexpr int CAM_TERMS = 27;
 // the same chain rule for several clouds in one launch: cloud c sums views view[view0 .. view0 + V) of the launch
 // (every cloud has a view, so MAX_BWD_VIEWS clouds at most); dL_dmean2D per view only, no dL_dconic
 struct ProjectBwdCloud {
@@ -96,8 +102,23 @@ struct ProjectBwdCloudsArgs {
 	ProjectBwdView view[MAX_BWD_VIEWS];
 	int antialias;                                 // as in ProjectBwdViewsArgs
 	const float4* conic_opacity[MAX_BWD_VIEWS];    // per view of the launch, AA only
+	float* cam_rows[MAX_BWD_VIEWS];                // per view of the launch: [CTAs of its cloud][CAM_TERMS], or NULL
 };
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
+// the second half of the camera gradients: view u's rows summed in row order into its 35 outputs (each nullable), written
+// (accumulate = 0) or added (1)
+struct CamReduceView {
+	const float* rows;
+	int nrows;
+	float* dL_dviewmatrix;  // 16
+	float* dL_dprojmatrix;  // 16
+	float* dL_dcampos;      // 3
+};
+struct CamReduceArgs {
+	int V, accumulate;
+	CamReduceView view[MAX_BWD_VIEWS];
+};
+inline size_t camera_rows_bytes(int P) { return (size_t)((P + 127) / 128) * CAM_TERMS * sizeof(float); }
 
 struct BlendArgs {
 	int W, H;
@@ -210,6 +231,7 @@ void launch_activate_bwd(ActivateArgs a, cudaStream_t s);
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s);
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s);
 void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s);
+void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s);
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s);
 
 // binning.cu

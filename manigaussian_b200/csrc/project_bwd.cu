@@ -36,6 +36,21 @@ __device__ const Sh16 kSh = { 0.28209479177387814f, 0.4886025119029199f,
 
 __device__ __forceinline__ float dot3(const float* u, const float* v) { return u[0] * v[0] + u[1] * v[1] + u[2] * v[2]; }
 
+// one step of a warp's recursive halving over 2H values: lane pairs (l, l ^ H) add their halves, the lane with bit H set keeps
+// the upper one in x[0 .. H).  Steps H = 16 .. 1 leave the warp's sum of x[l] on lane l.  The halves are picked with bit masks:
+// a select between array elements would put x in local memory.
+template <int H>
+__device__ __forceinline__ void warp_halve(float* x, const int lane)
+{
+	const int up = (lane & H) ? -1 : 0;
+#pragma unroll
+	for (int k = 0; k < H; k++) {
+		const int lo = __float_as_int(x[k]), hi = __float_as_int(x[k + H]);
+		const float got = __shfl_xor_sync(0xffffffffu, __int_as_float((lo & up) | (hi & ~up)), H);
+		x[k] = __int_as_float((hi & up) | (lo & ~up)) + got;
+	}
+}
+
 }  // namespace
 
 // NSH = floats of SH gradient kept in registers (3 (deg + 1)^2 for the largest degree the instantiation serves): the
@@ -51,9 +66,14 @@ __device__ __forceinline__ float dot3(const float* u, const float* v) { return u
 // The record's opacity gradient g is dL/do_eff, so dL/do = sum_v s_v g_v, and where r > 2.5e-5 the view's dL/dS' gains
 // g o ds = g o_eff (grad d0 / d0 - grad d1 / d1) / 2 (s^2 = r there): no raw opacity and no square root beyond s itself.
 // o_eff is read back from the view's conic_opacity.w; s is recomputed from S'.
-template <int NSH, bool AA, class Args>
-__device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx)
+//
+// CAM (camera gradients): per view, each thread forms the camera terms of its Gaussian (zeros where culled or past the end:
+// `in` false), the warp sums them into cam_sm[(warp, view)][CAM_TERMS], and the kernel sums its warps after the loop.  A CAM
+// thread therefore runs the whole view loop; it reads Gaussian 0 in place of a missing one and writes no per-Gaussian row.
+template <int NSH, bool AA, bool CAM, class Args>
+__device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx_in, const bool in, float* cam_sm)
 {
+	const int idx = CAM && !in ? 0 : idx_in;
 	const float p[3] = { a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2] };
 
 	// ---- the Gaussian's own covariance: S = L L^T, L = R(q) diag(mod * s), or the caller's ----
@@ -103,8 +123,11 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		const float4 g0 = gb[0], g1 = gb[1], g2 = gb[2];
 		const uint8_t cl = sh ? w.clamped[idx] : (uint8_t)0;
 		const float o_eff = AA ? a.conic_opacity[v][idx].w : 0.f;
-		const bool live = w.radii[idx] > 0;
+		const bool live = (!CAM || in) && w.radii[idx] > 0;
 		float dm[2] = { 0.f, 0.f };
+		float cg[32];  // CAM: this view's camera terms (CAM_TERMS used, padded to a warp)
+#pragma unroll
+		for (int k = 0; k < 32; k++) cg[k] = 0.f;
 		if (live) {
 			dm[0] = g0.x; dm[1] = g0.y;
 			const float gA = g0.z, gB = g0.w, gC = g1.x;        // dL/dconic (xx, xy halved, yy)
@@ -188,6 +211,22 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				gp[c] += Rv[0][c] * dt[0] + Rv[1][c] * dt[1] + Rv[2][c] * dt[2]
 					+ (pm[4 * c] * iw - pm[4 * c + 3] * kx) * dm[0] + (pm[4 * c + 1] * iw - pm[4 * c + 3] * ky) * dm[1];
 			}
+			if constexpr (CAM) {
+				// t = Rv p + tv and M = J Rv with J held: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt
+				const float j00 = fx * iz, j11 = fy * iz, j02 = -fx * cx * iz2, j12 = -fy * cy * iz2;
+#pragma unroll
+				for (int c = 0; c < 3; c++) {
+					cg[3 * c] = dt[0] * p[c] + j00 * q0[c];
+					cg[3 * c + 1] = dt[1] * p[c] + j11 * q1[c];
+					cg[3 * c + 2] = dt[2] * p[c] + j02 * q0[c] + j12 * q1[c];
+				}
+				cg[9] = dt[0]; cg[10] = dt[1]; cg[11] = dt[2];
+				// (hx, hy, hw) = P (p, 1): dL/dhx = dm0 iw, dL/dhy = dm1 iw, dL/dhw = -(dm0 kx + dm1 ky)
+				const float ax = dm[0] * iw, ay = dm[1] * iw, aw = -(dm[0] * kx + dm[1] * ky);
+				const float ph[4] = { p[0], p[1], p[2], 1.f };
+#pragma unroll
+				for (int c = 0; c < 4; c++) { cg[12 + 3 * c] = ax * ph[c]; cg[13 + 3 * c] = ay * ph[c]; cg[14 + 3 * c] = aw * ph[c]; }
+			}
 			// colour -> SH coefficients, and through the view direction into the mean
 			if (sh) {
 				const float dRGB[3] = { (cl & 1) ? 0.f : dcol[0], (cl & 2) ? 0.f : dcol[1], (cl & 4) ? 0.f : dcol[2] };
@@ -227,18 +266,29 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				// through the normalisation: d dir / d v = (I - dir dir^T) / |v|
 				const float along = x * dd[0] + y * dd[1] + z * dd[2];
 				gp[0] += (dd[0] - x * along) * il; gp[1] += (dd[1] - y * along) * il; gp[2] += (dd[2] - z * along) * il;
+				if constexpr (CAM) {  // v = p - campos: the same term with the opposite sign
+					cg[24] = -(dd[0] - x * along) * il; cg[25] = -(dd[1] - y * along) * il; cg[26] = -(dd[2] - z * along) * il;
+				}
 			}
-		} else if (a.dL_dconic && v == 0) {  // culled: the row is still written (the reference's zero-fill)
+		} else if (a.dL_dconic && v == 0 && in) {  // culled: the row is still written (the reference's zero-fill)
 			float* o = a.dL_dconic + 4 * (size_t)idx;
 			o[0] = 0.f; o[1] = 0.f; o[2] = 0.f; o[3] = 0.f;
 		}
 		// this view's screen-space gradient row (the reference's dL_dmeans2D, [P,3] with z = 0)
 		if (a.shared_mean2D) { gm2[0] += dm[0]; gm2[1] += dm[1]; }
-		else if (w.dL_dmean2D) {
+		else if (w.dL_dmean2D && in) {
 			float* o = w.dL_dmean2D + 3 * (size_t)idx;
 			o[0] = dm[0]; o[1] = dm[1]; o[2] = 0.f;
 		}
+		if constexpr (CAM) {
+			// recursive halving over the warp: 16 + 8 + 4 + 2 + 1 shuffles leave the sum of term `lane` on lane `lane`, in an
+			// order fixed by the lane numbers
+			const int lane = threadIdx.x & 31;
+			warp_halve<16>(cg, lane); warp_halve<8>(cg, lane); warp_halve<4>(cg, lane); warp_halve<2>(cg, lane); warp_halve<1>(cg, lane);
+			if (lane < CAM_TERMS) cam_sm[((threadIdx.x >> 5) * MAX_BWD_VIEWS + v) * CAM_TERMS + lane] = cg[0];
+		}
 	}
+	if (CAM && !in) return;
 
 	// ---- covariance -> scale and quaternion (once, on the sum over views) ----
 	float dscale[3] = { 0.f, 0.f, 0.f }, drot[4] = { 0.f, 0.f, 0.f, 0.f };
@@ -299,12 +349,32 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 	}
 }
 
-template <int NSH, int MIN_BLOCKS, bool AA>
+// CAM: after the view loop, one barrier and a sum over the CTA's 4 warps in warp order; row `blk` of each view's camera rows
+__device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* const* rows, int blk)
+{
+	__syncthreads();
+	for (int j = threadIdx.x; j < V * CAM_TERMS; j += blockDim.x) {
+		const int v = j / CAM_TERMS, k = j - v * CAM_TERMS;
+		float s = 0.f;
+#pragma unroll
+		for (int w = 0; w < 4; w++) s += cam_sm[(w * MAX_BWD_VIEWS + v) * CAM_TERMS + k];
+		if (rows[v]) rows[v][(size_t)blk * CAM_TERMS + k] = s;
+	}
+}
+
+// CAM before AA in the template list: the AA flag stays the last argument of every kernel name, as profiles read it
+template <int NSH, int MIN_BLOCKS, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-	if (idx >= a.P) return;
-	project_bwd_gaussian<NSH, AA>(a, idx);
+	if constexpr (CAM) {
+		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_TERMS];
+		project_bwd_gaussian<NSH, AA, true>(a, idx, idx < a.P, cam_sm);
+		cam_rows_out(cam_sm, a.V, a.cam_rows, blockIdx.x);
+	} else {
+		if (idx >= a.P) return;
+		project_bwd_gaussian<NSH, AA, false>(a, idx, true, nullptr);
+	}
 }
 
 namespace {
@@ -324,18 +394,92 @@ struct CloudBwd {
 }  // namespace
 
 // several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
-template <int NSH, int MIN_BLOCKS, bool AA>
+template <int NSH, int MIN_BLOCKS, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
 {
 	int c = 0;
 	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
 	const ProjectBwdCloud& cl = a.cloud[c];
 	const int idx = ((int)blockIdx.x - cl.block0) * blockDim.x + threadIdx.x;
-	if (idx >= cl.P) return;
+	if (!CAM && idx >= cl.P) return;
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
 		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
 		AA ? a.conic_opacity + cl.view0 : nullptr };
-	project_bwd_gaussian<NSH, AA>(cb, idx);
+	if constexpr (CAM) {
+		// the CTA serves one cloud: its rows belong to that cloud's views
+		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_TERMS];
+		project_bwd_gaussian<NSH, AA, true>(cb, idx, idx < cl.P, cam_sm);
+		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, (int)blockIdx.x - cl.block0);
+	} else {
+		project_bwd_gaussian<NSH, AA, false>(cb, idx, true, nullptr);
+	}
+}
+
+// one CTA of CAM_REDUCE_THREADS per view.  Thread t first sums rows t, t + 256, ... of every column in row order, then a
+// fixed tree over the 256 partials per column halves them 8 times: a fixed order, no serial chain over all rows.  Thread
+// j < 35 then owns output float j: view matrix 0..15, projection matrix 16..31, camera centre 32..34.
+constexpr int CAM_REDUCE_THREADS = 256;
+__global__ void __launch_bounds__(CAM_REDUCE_THREADS) camera_grad_reduce_kernel(CamReduceArgs a)
+{
+	__shared__ float part[CAM_TERMS][CAM_REDUCE_THREADS];
+	const CamReduceView& w = a.view[blockIdx.x];
+	const int t = threadIdx.x;
+	float acc[CAM_TERMS];
+#pragma unroll
+	for (int k = 0; k < CAM_TERMS; k++) acc[k] = 0.f;
+	for (int r = t; r < w.nrows; r += CAM_REDUCE_THREADS) {
+		const float* row = w.rows + (size_t)r * CAM_TERMS;
+#pragma unroll
+		for (int k = 0; k < CAM_TERMS; k++) acc[k] += row[k];
+	}
+#pragma unroll
+	for (int k = 0; k < CAM_TERMS; k++) part[k][t] = acc[k];
+	__syncthreads();
+	for (int h = CAM_REDUCE_THREADS / 2; h > 0; h >>= 1) {
+		for (int j = t; j < CAM_TERMS * h; j += CAM_REDUCE_THREADS) {
+			const int k = j / h, i = j - k * h;
+			part[k][i] += part[k][i + h];
+		}
+		__syncthreads();
+	}
+	const int j = t;
+	float* o = nullptr;
+	int k = -1;  // the row column, or -1 for an entry the forward never reads
+	if (j < 16) {
+		o = w.dL_dviewmatrix ? w.dL_dviewmatrix + j : nullptr;
+		if ((j & 3) != 3) k = 3 * (j >> 2) + (j & 3);
+	} else if (j < 32) {
+		const int i = j - 16, r = i & 3;
+		o = w.dL_dprojmatrix ? w.dL_dprojmatrix + i : nullptr;
+		if (r != 2) k = 12 + 3 * (i >> 2) + (r == 3 ? 2 : r);
+	} else if (j < 35) {
+		o = w.dL_dcampos ? w.dL_dcampos + (j - 32) : nullptr;
+		k = 24 + (j - 32);
+	}
+	if (!o) return;
+	const float s = k >= 0 ? part[k][0] : 0.f;
+	*o = a.accumulate ? *o + s : s;
+}
+
+void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s)
+{
+	if (a.V > 0) camera_grad_reduce_kernel<<<a.V, CAM_REDUCE_THREADS, 0, s>>>(a);
+}
+
+template <bool CAM>
+static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, cudaStream_t s)
+{
+	if (a.antialias) {
+		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
+		if (deg <= 1) project_bwd_views_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
+		return;
+	}
+	// CAM at degree <= 1: 4 blocks per SM, as for AA; the camera terms spill at the cap of 5 (96 registers)
+	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_views_kernel<27, 4, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_views_kernel<48, 3, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
@@ -343,40 +487,44 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	if (a.P <= 0 || a.V <= 0) return;
 	const int grid = ceil_div(a.P, 128);
 	const int deg = a.shs ? a.D : 0;
+	bool cam = false;
+	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr;
+	if (cam) project_bwd_views<true>(a, grid, deg, s);
+	else project_bwd_views<false>(a, grid, deg, s);
+}
+
+template <bool CAM>
+static void project_bwd_clouds(const ProjectBwdCloudsArgs& a, int grid, int deg, cudaStream_t s)
+{
+	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
+	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
 	if (a.antialias) {
-		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
-		if (deg <= 1) project_bwd_views_kernel<12, 4, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_views_kernel<27, 4, true><<<grid, 128, 0, s>>>(a);
-		else project_bwd_views_kernel<48, 3, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_clouds_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_kernel<27, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_clouds_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
-	if (deg <= 1) project_bwd_views_kernel<12, MGS_PBWD_MINB, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_views_kernel<27, 4, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_views_kernel<48, 3, false><<<grid, 128, 0, s>>>(a);
+	if (deg <= 1) project_bwd_clouds_kernel<12, 4, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_clouds_kernel<27, 4, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_clouds_kernel<48, 3, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 {
 	if (a.B <= 0) return;
-	int grid = 0;
+	int grid = 0, V = 0;
 	bool sh = false;
 	for (int c = 0; c < a.B; c++) {
 		a.cloud[c].block0 = grid;
 		grid += ceil_div(a.cloud[c].P, 128);
 		sh |= a.cloud[c].shs != nullptr;
+		V = a.cloud[c].view0 + a.cloud[c].V;
 	}
 	const int deg = sh ? a.D : 0;
-	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
-	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
-	if (a.antialias) {
-		if (deg <= 1) project_bwd_clouds_kernel<12, 4, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_clouds_kernel<27, 4, true><<<grid, 128, 0, s>>>(a);
-		else project_bwd_clouds_kernel<48, 3, true><<<grid, 128, 0, s>>>(a);
-		return;
-	}
-	if (deg <= 1) project_bwd_clouds_kernel<12, 4, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_clouds_kernel<27, 4, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_clouds_kernel<48, 3, false><<<grid, 128, 0, s>>>(a);
+	bool cam = false;
+	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr;
+	if (cam) project_bwd_clouds<true>(a, grid, deg, s);
+	else project_bwd_clouds<false>(a, grid, deg, s);
 }
 
 }  // namespace mgs

@@ -111,10 +111,29 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
     return ret
 
 
+def _camera_inputs(views, force=False):
+    """The views' stacked camera tensors (viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3]) as explicit inputs of a node
+    when any of them requires grad (or `force`), else (None, None, None): the node then returns their gradients."""
+    fields = [[getattr(s, n) for s in views] for n in ("viewmatrix", "projmatrix", "campos")]
+    if not force and not any(torch.is_tensor(t) and t.requires_grad for f in fields for t in f):
+        return None, None, None
+    return tuple(torch.stack([torch.as_tensor(t, dtype=torch.float32).reshape(shape) for t in f])
+                 for f, shape in zip(fields, ((4, 4), (4, 4), (3,))))
+
+
+def _camera_outputs(ctx, cam, first):
+    """Gradients for the camera inputs at positions first, first + 1, first + 2 of the node (None where not needed)"""
+    if cam is None:
+        return None, None, None
+    V = cam[0].shape[0]
+    shapes = ((V, 4, 4), (V, 4, 4), (V, 3))
+    return tuple(g.view(shape) if ctx.needs_input_grad[first + i] else None for i, (g, shape) in enumerate(zip(cam, shapes)))
+
+
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
-                group, antialiasing=False):
+                group, antialiasing=False, cam_vm=None, cam_pm=None, cam_cp=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -139,6 +158,7 @@ class _RasterizeViews(torch.autograd.Function):
             main.wait_stream(st)
         radii = torch.stack([o[3] for o in outs])
         ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
+        ctx.camera = cam_vm is not None
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
         ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
@@ -170,20 +190,22 @@ class _RasterizeViews(torch.autograd.Function):
         grp = None if ctx.group in (None, True) else ctx.group
         m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
         outs = [(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in ctx.state]
-        rasterize_views_backward_raw(views, outs, ctx.streams, g_color, g_feat, means3D, colors_precomp if use_colors else None,
-                                     feature if ctx.include else None, scales, rotations, views[0].scale_modifier, None,
-                                     sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
-                                     accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
-                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
-                                     antialiasing=ctx.antialiasing)
+        res = rasterize_views_backward_raw(views, outs, ctx.streams, g_color, g_feat, means3D, colors_precomp if use_colors else None,
+                                           feature if ctx.include else None, scales, rotations, views[0].scale_modifier, None,
+                                           sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
+                                           accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
+                                           after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
+                                           antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
-            # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields
+            # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields.
+            # A view's camera gradients are complete on the rank that rendered it.
             pk.all_reduce_finish(grp)
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None,
+                *_camera_outputs(ctx, res[9] if ctx.camera else None, 13))
 
 
 def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
@@ -251,7 +273,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
-                target_depth=None, target_mask=None, antialiasing=False, ssim=False):
+                target_depth=None, target_mask=None, antialiasing=False, ssim=False, cam_vm=None, cam_pm=None, cam_cp=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -284,6 +306,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
         radii = torch.stack([o[3] for o in outs])
         ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
+        ctx.camera = cam_vm is not None
         # capacity, radii and the three state buffers per view -- never the images: they are views of this node's outputs, and an
         # output kept on ctx is a reference cycle (output -> grad_fn -> ctx -> output) that leaks the whole step
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]
@@ -319,7 +342,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
         grp = None if ctx.group in (None, True) else ctx.group
         m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
         outs = [(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in ctx.state]
-        rasterize_views_backward_raw(views, outs, ctx.streams, cot_rgb, cot_embed if ctx.include else None, means3D,
+        res = rasterize_views_backward_raw(views, outs, ctx.streams, cot_rgb, cot_embed if ctx.include else None, means3D,
                                      colors_precomp if use_colors else None, feature if ctx.include else None, scales, rotations,
                                      views[0].scale_modifier, None, sh if M else None, ctx.degree, ctx.include, debug=views[0].debug,
                                      accumulate_into=pk.views, means2D_per_view=m2d, cot_scale=scale,
@@ -328,13 +351,15 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                      depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None,
                                      antialiasing=ctx.antialiasing,
                                      ssim=ctx.ssim + (color, ctx.target_rgb) if ctx.ssim is not None else None,
-                                     ssim_scale=_pair_scale(g_l1, g_ssim, V, dev) if ctx.ssim is not None else None)
+                                     ssim_scale=_pair_scale(g_l1, g_ssim, V, dev) if ctx.ssim is not None else None,
+                                     camera_grads=True if ctx.camera else None)
         if ctx.group is not None:
             pk.all_reduce_finish(grp)
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None, None)
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None, None,
+                *_camera_outputs(ctx, res[9] if ctx.camera else None, 16))
 
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
@@ -364,6 +389,9 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     expected depth).
     antialiasing: render with the anti-aliased projection (opacity compensation for the 0.3 px^2 dilation, INTEGRATION.md
     §5); also on when the given settings carry antialiasing=True.  Combines with every option above.
+    Camera gradients: when a view's viewmatrix, projmatrix or campos requires grad (e.g. cameras from
+    `cameras.camera_batch` of a learnable w2c), the backward also returns their gradients (INTEGRATION.md §6); this combines
+    with every option above.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -387,6 +415,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     screenspace_points = torch.zeros((V, P, 3), dtype=torch.float32, device=device, requires_grad=True)
     if ssim and targets is None:
         raise ValueError("ssim=True needs targets (the colour target \"rgb\")")
+    cams = _camera_inputs(views)
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
@@ -396,7 +425,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
          ssim_v) = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
             rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"), aa,
-            bool(ssim))
+            bool(ssim), *cams)
         ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
                "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
         if targets.get("depth") is not None:
@@ -406,7 +435,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         if ssim:
             ret["loss_l1"], ret["ssim"] = loss_l1, ssim_v
         return ret
-    if V == 1 and sync_gradients is None:
+    if V == 1 and sync_gradients is None and cams[0] is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True) if aa else views[0]
         out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha)(
@@ -419,7 +448,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     else:
         color, feat_img, radii, depth, alpha = _RasterizeViews.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa)
+            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa, *cams)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
@@ -439,7 +468,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim = meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
         clouds, results, frozen, cots, dms, ssims, images = [], [], [], [], [], [], []
@@ -504,7 +533,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim = ctx.meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
         images = saved[6 * len(cloud_views):]
@@ -538,13 +567,18 @@ class _RasterizeClouds(torch.autograd.Function):
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
         res = rasterize_clouds_backward_raw(clouds, outs, ctx.streams, ctx.degree, ctx.include, cloud_views[0][0].scale_modifier,
-                                            debug=cloud_views[0][0].debug, antialiasing=antialiasing)
+                                            debug=cloud_views[0][0].debug, antialiasing=antialiasing, camera_grads=camera)
         ret = [None]
         for b, r in enumerate(res):
             P = clouds[b]["means3D"].shape[0]
             M = clouds[b]["sh"].shape[1] if clouds[b]["sh"] is not None else 0
             ret += [r["dL_dmeans3D"], r["dL_dmeans2D"], r["dL_dsh"].view(P, M, 3) if M else None, r["dL_dcolors"], r["dL_dfeature"],
                     r["dL_dopacity"].view(ctx.opac_shapes[b]), r["dL_dscales"], r["dL_drotations"]]
+        if camera:  # the stacked camera tensors of every cloud behind its Gaussian inputs
+            first = 1 + _CLOUD_INPUTS * len(cloud_views)
+            for b, r in enumerate(res):
+                cam = (r["dL_dviewmatrix"], r["dL_dprojmatrix"], r["dL_dcampos"])
+                ret += _camera_outputs(ctx, cam, first + 3 * b)
         return tuple(ret)
 
 
@@ -562,6 +596,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
     dyna step, which renders the detached current features); its feature cotangents still reach its other gradients.
     antialiasing: every cloud renders with the anti-aliased projection, as in render_views.
+    Camera gradients: as in render_views, per cloud; clouds that share camera tensors (the dyna pair) receive the sum.
     ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
@@ -609,7 +644,13 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for views in cloud_views for s in views)
-    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim)), *flat)
+    cams = [_camera_inputs(views) for views in cloud_views]
+    camera = any(c[0] is not None for c in cams)
+    if camera:  # every cloud's stacked cameras, as explicit inputs (the dyna pair's shared tensors get both frames' sums)
+        cams = [c if c[0] is not None else _camera_inputs(views, force=True) for c, views in zip(cams, cloud_views)]
+        flat += [t for c in cams for t in c]
+    out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim), camera),
+                                 *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]

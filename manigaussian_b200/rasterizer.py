@@ -258,14 +258,19 @@ def cpu_deep_copy_tuple(input_tuple):
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
+    s = raster_settings
+    # camera tensors that require grad become explicit inputs of the node, which then returns their gradients
+    cam = (s.viewmatrix, s.projmatrix, s.campos)
+    if not any(torch.is_tensor(t) and t.requires_grad for t in cam):
+        cam = ()
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha)
+                                     rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha, *cam)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
+                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, *cam):
         s = raster_settings
         args = (s.bg, means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations, s.scale_modifier,
                 cov3Ds_precomp, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.image_height, s.image_width, sh,
@@ -274,10 +279,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         views_path = means3D.is_cuda and means3D.size(0) > 0
         aa = bool(getattr(s, "antialiasing", False))
         ctx.antialiasing = aa
+        ctx.camera = len(cam) > 0
         alpha = None
-        if (return_alpha or aa) and views_path:
-            # the alpha plane and the anti-aliased projection exist on the multi-view entry points only: debug renders take
-            # them too, with the snapshot dump
+        if (return_alpha or aa or ctx.camera) and views_path:
+            # the alpha plane, the anti-aliased projection and the camera gradients exist on the multi-view entry points only:
+            # debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
@@ -347,13 +353,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.async_view is not None:
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
-            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.antialiasing)) else None
+            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.antialiasing or ctx.camera)) else None
             try:
                 grads = rasterize_views_backward_raw(
                     [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
                     colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
                     s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None, debug=s.debug,
-                    grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing)
+                    grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing,
+                    camera_grads=True if ctx.camera else None)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -370,7 +377,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         else:
             grads = rasterize_gaussians_backward_raw(*args, dL_dout_depth=depth_grad)
         (grad_means2D, grad_colors_precomp, grad_language_feature_precomp, grad_opacities, grad_means3D,
-         grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations) = grads
+         grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations) = grads[:9]
+        grad_cam = ()
+        if ctx.camera:
+            # zero gradients when the views path did not run (no Gaussians: nothing depends on the camera)
+            dvm, dpm, dcp = grads[9] if len(grads) > 9 else (torch.zeros((1, 16), device=means3D.device),) * 2 + (
+                torch.zeros((1, 3), device=means3D.device),)
+            grad_cam = tuple(g.view(t.shape) if ctx.needs_input_grad[12 + i] else None
+                             for i, (g, t) in enumerate(zip((dvm, dpm, dcp), (s.viewmatrix, s.projmatrix, s.campos))))
 
         def _or_none(g, inp):
             return g if (inp is not None and inp.numel() != 0) else None
@@ -378,7 +392,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, _or_none(grad_sh, sh), _or_none(grad_colors_precomp, colors_precomp),
                 _or_none(grad_language_feature_precomp, language_feature_precomp) if s.include_feature else None,
                 grad_opacities, _or_none(grad_scales, scales), _or_none(grad_rotations, rotations),
-                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None)
+                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None) + grad_cam
 
 
 class _Settings(NamedTuple):
@@ -737,7 +751,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
-                                 ssim=None, ssim_scale=None):
+                                 ssim=None, ssim_scale=None, camera_grads=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -752,7 +766,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_backward_views_aa).  `ssim`: the tuple given to
     the forward plus the forward's images and colour targets (both [V,3,H,W]); each view's L1 + SSIM head then writes its
     complete colour cotangent, with `ssim_scale` [V,2] (device; the upstream gradients {g_l1, g_ssim}, or None for 1), before
-    its blend backward reads it."""
+    its blend backward reads it.  `camera_grads`: True, or a tuple (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16], dL_dcampos
+    [V,3]) of fp32 device tensors or None each, asks for the gradients with respect to each view's viewmatrix, projmatrix and
+    campos (C ABI mgs_backward_views_cam; written, or added to with accumulate=True); the return value then gains that tuple
+    (allocated for True) as a 10th element."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -810,13 +827,16 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 w.cot_scale = cot_scale.data_ptr() + 8 * v
             if sarr is not None:
                 _fill_ssim(sarr[v], ssim, v, w, sscale)
+        cam, carr = _camera_grads(L, camera_grads, [P] * V, dev, keep)
         for stages in ((1, 2) if after_blend is not None else (3,)):
             rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
                     _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if sarr is not None:
+            if carr is not None:
+                _b.check(L.mgs_backward_views_cam(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, *rest), "mgs_backward_views_cam")
+            elif sarr is not None:
                 _b.check(L.mgs_backward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_backward_views_ssim")
             elif antialiasing:
                 _b.check(L.mgs_backward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_backward_views_aa")
@@ -828,7 +848,35 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 _b.check(L.mgs_backward_views(V, arr, *rest), "mgs_backward_views")
             if stages == 1:
                 after_blend()
-    return (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
+    grads = (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
+    return grads + (cam,) if cam is not None else grads
+
+
+def _camera_grads(L, camera_grads, Ps, dev, keep):
+    """(outputs, ViewCameraGrad array) for the views of clouds of Ps[v] Gaussians, or (None, None) without camera_grads.
+    True allocates the three outputs [V,16], [V,16], [V,3]; a tuple names them (each a contiguous fp32 device tensor of that
+    shape, or None)."""
+    if camera_grads is None or camera_grads is False:
+        return None, None
+    V = len(Ps)
+    opts = dict(dtype=torch.float32, device=dev)
+    if camera_grads is True:
+        camera_grads = (torch.empty((V, 16), **opts), torch.empty((V, 16), **opts), torch.empty((V, 3), **opts))
+    shapes = ((V, 16), (V, 16), (V, 3))
+    for t, shape in zip(camera_grads, shapes):
+        if t is not None and (t.dtype != torch.float32 or t.device != dev or not t.is_contiguous() or t.numel() != shape[0] * shape[1]):
+            raise ValueError(f"camera_grads: expected contiguous fp32 tensors of {shape} on {dev}")
+    rows = [L.mgs_camera_grad_scratch_bytes(int(P)) // 4 for P in Ps]
+    scratch = torch.empty((max(sum(rows), 1),), **opts)
+    keep.append(scratch)
+    carr = (_b.ViewCameraGrad * V)()
+    off = 0
+    for v in range(V):
+        for name, t, n in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos"), camera_grads, (16, 16, 3)):
+            setattr(carr[v], name, t.data_ptr() + 4 * n * v if t is not None else None)
+        carr[v].scratch = scratch.data_ptr() + 4 * off
+        off += rows[v]
+    return tuple(camera_grads), carr
 
 
 def _backward_view(L, w, s, o, dev, P, grad_color, grad_feature, grad_depth):
@@ -964,7 +1012,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
 
 
 def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False,
-                                  antialiasing=False):
+                                  antialiasing=False, camera_grads=False):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
     plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
@@ -975,7 +1023,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     as rasterize_views_backward_raw takes them.  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
     dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed).  `antialiasing`: the value
-    the forward was given (C ABI mgs_backward_clouds_aa)."""
+    the forward was given (C ABI mgs_backward_clouds_aa).  `camera_grads=True`: every cloud's dict also holds the gradients
+    with respect to its views' viewmatrix, projmatrix and campos, "dL_dviewmatrix" [V_b,16], "dL_dprojmatrix" [V_b,16] and
+    "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1036,8 +1086,16 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 if c.get("ssim") is not None:
                     _fill_ssim(sarr[g], c["ssim"], v, w, sscale)
             keep.append(cot)
+        cam, camarr = _camera_grads(L, bool(camera_grads), [d["P"] for d, c in zip(pc, clouds) for _ in c["views"]], dev, keep)
+        if cam is not None:
+            for b, gr in enumerate(grads):
+                for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos"), cam):
+                    gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if sarr is not None:
+        if camarr is not None:
+            _b.check(L.mgs_backward_clouds_cam(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, *rest),
+                     "mgs_backward_clouds_cam")
+        elif sarr is not None:
             _b.check(L.mgs_backward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
                      "mgs_backward_clouds_ssim")
         elif antialiasing:
