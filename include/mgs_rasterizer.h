@@ -608,9 +608,9 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
  *   dL/dcampos = -(dd - dir along) / |v|  (v = p - campos, the SH branch's direction gradient dd and along = dir . dd: the
  *                    view-direction term of dL/dmeans3D with the opposite sign; 0 without SHs).
  * The gradient of a 16-float array is the gradient with respect to those 16 floats, so as a torch [4,4] it is directly the
- * gradient of world_view_transform / full_proj_transform.  tan_fov, the focal lengths, the 1.3 tan_fov clamp limit, the
- * near-plane cull, the radii and the tiles are constants: a projmatrix built from a learnable focal length receives only
- * the screen-mean path.
+ * gradient of world_view_transform / full_proj_transform.  In these calls tan_fov, the focal lengths, the 1.3 tan_fov clamp
+ * limit, the near-plane cull, the radii and the tiles are constants: a projmatrix built from a learnable focal length
+ * receives only the screen-mean path.  The _intr calls below add the focal-length path through J and the clamp limit.
  * The sums are deterministic: every CTA of the per-Gaussian kernel writes one row of 27 partial sums per view into the
  * entry's scratch in a fixed order, and a reduce kernel on join_stream sums each view's rows in a fixed tree.  A view's rows
  * all come from one launch of at most 16 views.  These calls leave mgs_abi_version() at 300: they only add symbols, and a
@@ -652,6 +652,84 @@ int mgs_backward_views_cam(
 int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
 	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
+/*
+ * Learnable intrinsics (no reference counterpart).  The _intr calls are the _ssim forward and the _cam backward calls with one
+ * more argument, `intr`: one mgs_view_intrinsics per view (V entries, or view_offsets[B] for clouds), or NULL; the older calls
+ * are these with intr == NULL, and the calls above keep the definition given there.
+ *
+ * Device field of view.  An entry's tan_fov, when set, points at the view's {tan_fovx, tan_fovy} in device memory, and the
+ * projection forward and backward read it there in place of mgs_view.tan_fovx / tan_fovy: a value an optimizer step has just
+ * written is used with no device->host read, and a captured CUDA graph reads the value at replay.  The kernels form
+ * fx = W / (2 tan_fovx) and fy = H / (2 tan_fovy) with the same float expression as the host path (the build has no fast
+ * math), so a device value equal to the host floats gives the host path's radii, sort keys, tiles and images bit for bit.
+ * The backward then runs the camera-gradient instantiation of the per-Gaussian stage (with or without outputs).
+ *
+ * Focal-length gradient.  dL_dtan_fov, when set, receives {dL/dtan_fovx, dL/dtan_fovy} under the rules of the camera outputs
+ * above: written (accumulate = 0) or added to (1) by stage 2, and it needs the view's mgs_view_camera_grad entry with scratch
+ * (MGS_ERR_INVALID_ARG before anything is enqueued otherwise); its per-CTA partial sums are kept in the view's geometry
+ * state, so mgs_camera_grad_scratch_bytes is unchanged and remains the only scratch size to provide.  Definition, with the quantities of the camera-gradient
+ * definition above (Q = [q0; q1] = dL/dM including the anti-aliased compensation, cx, cy the clamped t.x, t.y, tz = t.z) and
+ * dJ00 = q0 . Rv0, dJ02 = q0 . Rv2, dJ11 = q1 . Rv1, dJ12 = q1 . Rv2, the sum over the view's Gaussians with radius > 0 of
+ *   dL/dtan_fovx = -(fx / tan_fovx) (dJ00 / tz - dJ02 cx / tz^2)          (J through fx = W / (2 tan_fovx))
+ *                  - [|t.x / tz| > 1.3 tan_fovx] fx dJ02 (+-1.3) / tz      (the clamp cx = +-1.3 tan_fovx tz, sign of t.x / tz)
+ * and likewise dL/dtan_fovy with fy, dJ11, dJ12, cy.  The near-plane cull, the radii, the tiles and the sort stay constants.
+ * The projection-matrix path of the focal lengths and the principal point is dL/dprojmatrix above, to be chained by the
+ * caller (for a projmatrix built from K).  With intrinsics on, the 27 other camera terms are those the _cam calls write.
+ */
+typedef struct mgs_view_intrinsics {
+	const float* tan_fov;    /* device, 2 floats, or NULL: use mgs_view.tan_fovx / tan_fovy */
+	float* dL_dtan_fov;      /* device, 2 floats, or NULL */
+} mgs_view_intrinsics;
+
+int mgs_forward_views_intr(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_intr(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
+	int debug, void* join_stream);
 
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */

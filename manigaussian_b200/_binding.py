@@ -48,6 +48,12 @@ class ViewCameraGrad(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "scratch")]
 
 
+class ViewIntrinsics(C.Structure):
+    """mirror of `mgs_view_intrinsics` (include/mgs_rasterizer.h): the optional device field of view of one view and its
+    gradient"""
+    _fields_ = [(n, C.c_void_p) for n in ("tan_fov", "dL_dtan_fov")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -135,6 +141,12 @@ def lib():
             getattr(L, cam).restype = C.c_int
             getattr(L, cam).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim),
                                                  C.POINTER(ViewCameraGrad)] + at[k:]
+        # ... and the device field of view (one ViewIntrinsics per view, or NULL): after the L1 + SSIM heads in the forward,
+        # after the camera gradients in the backward
+        intr = name.replace("_views", "_views_intr").replace("_clouds", "_clouds_intr")
+        getattr(L, intr).restype = C.c_int
+        getattr(L, intr).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
+            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -176,6 +188,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_ssim", "mgs_backward_views_ssim", "mgs_forward_clouds_ssim", "mgs_backward_clouds_ssim",
     "mgs_ssim", "mgs_ssim_backward",
     "mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam",
+    "mgs_forward_views_intr", "mgs_backward_views_intr", "mgs_forward_clouds_intr", "mgs_backward_clouds_intr",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

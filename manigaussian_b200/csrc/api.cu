@@ -137,6 +137,7 @@ struct GeomState {
 	float* depths; uint8_t* clamped; float2* means2D; float* cov3D; float4* conic_opacity; float4* rgbd;
 	float2* extent; uint32_t* tiles_touched; uint32_t* point_offsets; uint32_t* iota; uint32_t* order; uint32_t* depth_sorted;
 	char* temp; size_t temp_bytes;
+	float* cam_intr;  // the backward's focal-length rows of this view (mgs_view_intrinsics.dL_dtan_fov), CAM_INTR_TERMS per CTA
 	static GeomState carve(char*& chunk, size_t P)
 	{
 		GeomState g;
@@ -154,6 +155,7 @@ struct GeomState {
 		obtain(chunk, g.depth_sorted, P);
 		g.temp_bytes = cached_temp_bytes(0, (int)P);
 		obtain(chunk, g.temp, g.temp_bytes);
+		obtain(chunk, g.cam_intr, camera_intr_rows((int)P));
 		return g;
 	}
 };
@@ -345,8 +347,12 @@ static ViewState carve_view(const mgs_view& w, int P)
 	return s;
 }
 
-// per-Gaussian projection, depth order and instance offsets; the instance count ends up in geom.point_offsets[P - 1]
-static int enqueue_project(const Cloud& c, const mgs_view& w, int debug)
+// the view's device {tan_fovx, tan_fovy} (intr: one entry per view, or NULL), or NULL for mgs_view.tan_fovx / tan_fovy
+static const float* device_fov(const mgs_view_intrinsics* intr, int v) { return intr ? intr[v].tan_fov : nullptr; }
+
+// per-Gaussian projection, depth order and instance offsets; the instance count ends up in geom.point_offsets[P - 1].
+// tan_fov: the view's device field of view, or NULL
+static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const ViewState s = carve_view(w, c.P);
@@ -363,6 +369,7 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, int debug)
 	pa.conic_opacity = geom.conic_opacity; pa.extent = geom.extent; pa.clamped = geom.clamped; pa.tiles_touched = geom.tiles_touched;
 	pa.iota = geom.iota;
 	pa.antialias = c.antialias;
+	pa.tan_fov = tan_fov;
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
 
@@ -563,32 +570,37 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 	return pv;
 }
 
-// camera gradients of view v (cam: one entry per view, or NULL): an entry asks for them when it has an output
-static bool camera_on(const mgs_view_camera_grad* cam, int v)
+// camera gradients of view v (cam, intr: one entry per view, or NULL): the view asks for them when its camera entry or its
+// intrinsics entry has an output; the rows live in the camera entry's scratch
+static float* tan_fov_grad(const mgs_view_intrinsics* intr, int v) { return intr ? intr[v].dL_dtan_fov : nullptr; }
+static bool camera_on(const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int v)
 {
-	return cam && (cam[v].dL_dviewmatrix || cam[v].dL_dprojmatrix || cam[v].dL_dcampos);
+	return (cam && (cam[v].dL_dviewmatrix || cam[v].dL_dprojmatrix || cam[v].dL_dcampos)) || tan_fov_grad(intr, v);
 }
-static int check_camera(const mgs_view_camera_grad* cam, int V)
+static int check_camera(const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int V)
 {
 	for (int v = 0; v < V; v++)
-		if (camera_on(cam, v) && !cam[v].scratch)
-			return fail(MGS_ERR_INVALID_ARG, "camera gradients: an entry with an output needs scratch");
+		if (camera_on(cam, intr, v) && !(cam && cam[v].scratch))
+			return fail(MGS_ERR_INVALID_ARG, "camera gradients: an entry with an output needs scratch (in its mgs_view_camera_grad)");
 	return 0;
 }
-// the view's rows pointer for its per-Gaussian launch, and its entry in that launch's reduce
-static void camera_view(const mgs_view_camera_grad* cam, int v, int P, float*& rows, CamReduceArgs& cr)
+// the view's rows pointer and device field of view for its per-Gaussian launch, and its entry in that launch's reduce
+static void camera_view(const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view& w, int v, int P, float*& rows,
+	ProjectBwdIntr& ki, CamReduceArgs& cr)
 {
-	if (!camera_on(cam, v)) return;
+	float* dtf = tan_fov_grad(intr, v);
+	ki = ProjectBwdIntr{ device_fov(intr, v), w.width, w.height, dtf ? carve_view(w, P).geom.cam_intr : nullptr };
+	if (!camera_on(cam, intr, v)) return;
 	const mgs_view_camera_grad& e = cam[v];
 	rows = e.scratch;
-	cr.view[cr.V++] = CamReduceView{ e.scratch, (P + 127) / 128, e.dL_dviewmatrix, e.dL_dprojmatrix, e.dL_dcampos };
+	cr.view[cr.V++] = CamReduceView{ e.scratch, (P + 127) / 128, e.dL_dviewmatrix, e.dL_dprojmatrix, e.dL_dcampos, ki.rows, dtf };
 }
 
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -633,7 +645,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
 		CamReduceArgs cr{};
 		cr.accumulate = accumulate ? 1 : 0;
-		for (int u = 0; u < pb.V; u++) camera_view(cam, v0 + u, P, pb.cam_rows[u], cr);
+		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
@@ -654,7 +666,7 @@ static int project_single_view(const Cloud& c, mgs_view& w, mgs_alloc_fn geometr
 	w.geometry_state = geometry_alloc(geometry_user, mgs_geometry_state_bytes(c.P));
 	w.image_state = image_alloc(image_user, mgs_image_state_bytes(w.width, w.height));
 	if (!w.geometry_state || !w.image_state) return fail(MGS_ERR_ALLOC, "state allocation failed");
-	int rc = enqueue_project(c, w, debug);
+	int rc = enqueue_project(c, w, nullptr, debug);
 	if (rc < 0) return rc;
 	MGS_CUDA(cudaMemcpyAsync(host_count, carve_view(w, c.P).geom.point_offsets + c.P - 1, sizeof(int), cudaMemcpyDeviceToHost,
 		reinterpret_cast<cudaStream_t>(w.stream)));
@@ -798,7 +810,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -854,6 +866,18 @@ int mgs_forward_views_ssim(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_intr(V, views, alpha, depth_mask, antialiasing, ssim, nullptr, P, D, M, F, means3D, shs, colors_precomp,
+		feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_intr(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -887,7 +911,7 @@ int mgs_forward_views_ssim(
 			if (rc < 0) return rc;
 		}
 		for (int v = 0; v < V; v++) {
-			rc = phase == 0 ? enqueue_project(c, views[v], debug)
+			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
 			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
@@ -972,6 +996,20 @@ int mgs_backward_views_cam(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_intr(V, views, alpha, depth_mask, antialiasing, ssim, cam, nullptr, P, D, M, F, means3D, shs,
+		colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
+		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_intr(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -985,10 +1023,10 @@ int mgs_backward_views_cam(
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 		if (rc < 0) return rc;
 	}
-	if (check_camera(cam, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1025,6 +1063,14 @@ int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offs
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
 	int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_intr(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, nullptr, D, M, F,
+		scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -1052,7 +1098,7 @@ int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offs
 		for (int b = 0; b < B; b++) {
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-				rc = phase == 0 ? enqueue_project(c, views[v], debug)
+				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
 				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
@@ -1104,6 +1150,15 @@ int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offs
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
 	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_intr(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, nullptr, D, M, F,
+		scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
+	int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -1122,7 +1177,7 @@ int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offs
 		}
 	}
 	const int V = view_offsets[B];
-	if (check_camera(cam, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1160,6 +1215,7 @@ int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offs
 		MGS_STAGE("project_bwd");
 		pb.B = 0; nv = 0; cr.V = 0;
 		for (float*& r : pb.cam_rows) r = nullptr;
+		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
 		return 0;
 	};
 	for (int b = 0; b < B; b++) {
@@ -1182,7 +1238,7 @@ int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offs
 			for (int u = 0; u < n; u++) {
 				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
 				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
-				camera_view(cam, v0 + u, k.P, pb.cam_rows[nv + u], cr);
+				camera_view(cam, intr, views[v0 + u], v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
 			}
 			nv += n;
 		}

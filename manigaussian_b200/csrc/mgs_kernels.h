@@ -37,6 +37,9 @@ struct ProjectFwdArgs {
 	uint32_t* iota;    // identity permutation (values of the depth sort)
 	int antialias;     // 1: opacity compensation for the 0.3 px^2 low-pass (launcher picks the instantiation; last, so the
 	                   // other members keep their parameter offsets)
+	// device {tan_fovx, tan_fovy}, or NULL: tan_fov* and focal_* above.  Non-NULL picks the instantiation that reads it and
+	// forms the focal lengths as the host does (W / (2 tan_fovx)); behind antialias for the same reason.
+	const float* tan_fov;
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -50,6 +53,14 @@ struct ProjectBwdView {
 	const float* cam_pos;
 	float* dL_dmean2D;         // [P,3] of this view (nullable); with shared_mean2D only view 0's is used and receives the sum
 	float tan_fovx, tan_fovy, focal_x, focal_y;
+};
+// a view's device field of view: {tan_fovx, tan_fovy} read in the kernel, or NULL for the ProjectBwdView's host values; W, H
+// the image size the focal lengths are formed from (fx = W / (2 tan_fovx), as on the host); rows: the view's focal-length
+// rows [CTAs of the launch][CAM_INTR_TERMS] (in its geometry state), or NULL
+struct ProjectBwdIntr {
+	const float* tan_fov;
+	int W, H;
+	float* rows;
 };
 struct ProjectBwdViewsArgs {
 	int P, D, M, V;
@@ -78,10 +89,16 @@ struct ProjectBwdViewsArgs {
 	// camera gradients (the launcher picks the CAM instantiation when any is set): view u's rows [CTAs of the launch][CAM_TERMS],
 	// one per CTA, or NULL.  Behind every other member for the same reason as conic_opacity.
 	float* cam_rows[MAX_BWD_VIEWS];
+	// device fields of view (the CAM instantiation reads them; the launcher picks it when any is set): behind cam_rows
+	ProjectBwdIntr intr[MAX_BWD_VIEWS];
 };
-// the 27 camera terms one CTA writes per view: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1, 3}] at 12 + 3c + {0, 1,
-// 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.
+// the 27 camera terms one CTA writes per view into its camera rows: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1,
+// 3}] at 12 + 3c + {0, 1, 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.  The kernel
+// forms CAM_ALL_TERMS: terms 27 + i, dL/dtan_fov, go to the view's focal-length rows (ProjectBwdIntr::rows), so the camera
+// rows keep their width and mgs_camera_grad_scratch_bytes its value.
 constexpr int CAM_TERMS = 27;
+constexpr int CAM_INTR_TERMS = 2;
+constexpr int CAM_ALL_TERMS = CAM_TERMS + CAM_INTR_TERMS;
 // the same chain rule for several clouds in one launch: cloud c sums views view[view0 .. view0 + V) of the launch
 // (every cloud has a view, so MAX_BWD_VIEWS clouds at most); dL_dmean2D per view only, no dL_dconic
 struct ProjectBwdCloud {
@@ -103,6 +120,7 @@ struct ProjectBwdCloudsArgs {
 	int antialias;                                 // as in ProjectBwdViewsArgs
 	const float4* conic_opacity[MAX_BWD_VIEWS];    // per view of the launch, AA only
 	float* cam_rows[MAX_BWD_VIEWS];                // per view of the launch: [CTAs of its cloud][CAM_TERMS], or NULL
+	ProjectBwdIntr intr[MAX_BWD_VIEWS];            // per view of the launch, as in ProjectBwdViewsArgs
 };
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 // the second half of the camera gradients: view u's rows summed in row order into its 35 outputs (each nullable), written
@@ -113,12 +131,15 @@ struct CamReduceView {
 	float* dL_dviewmatrix;  // 16
 	float* dL_dprojmatrix;  // 16
 	float* dL_dcampos;      // 3
+	const float* intr_rows; // [nrows][CAM_INTR_TERMS] focal-length rows, or NULL
+	float* dL_dtan_fov;     // 2
 };
 struct CamReduceArgs {
 	int V, accumulate;
 	CamReduceView view[MAX_BWD_VIEWS];
 };
 inline size_t camera_rows_bytes(int P) { return (size_t)((P + 127) / 128) * CAM_TERMS * sizeof(float); }
+inline size_t camera_intr_rows(int P) { return (size_t)((P + 127) / 128) * CAM_INTR_TERMS; }  // floats, in the geometry state
 
 struct BlendArgs {
 	int W, H;

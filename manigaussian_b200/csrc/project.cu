@@ -108,7 +108,9 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 // AA: the anti-aliased mode (Mip-Splatting's 2D filter, DESIGN.md section 4): the opacity is scaled by
 // s = sqrt(max(2.5e-5, det(Sigma) / det(Sigma + 0.3 I))), so that the dilated splat carries the energy of the undilated one.
 // Only conic_opacity.w and the extent's opacity change; the conic, radius, tiles and keys are those of AA = false.
-template <bool AA>
+// FOV: the field of view is read from the device ({tan_fovx, tan_fovy} at a.tan_fov) and the focal lengths are formed here
+// with the host's float expression, so equal values give the host path's results bit for bit.
+template <bool AA, bool FOV>
 __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -137,7 +139,12 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 		cov3D = a.cov3D + (size_t)idx * 6;
 	}
 
-	Cov2DTerms ct = cov2d_terms(p_orig, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, a.viewmatrix);
+	float tanx = a.tan_fovx, tany = a.tan_fovy, fx = a.focal_x, fy = a.focal_y;
+	if constexpr (FOV) {
+		tanx = a.tan_fov[0]; tany = a.tan_fov[1];
+		fx = a.W / (2.0f * tanx); fy = a.H / (2.0f * tany);  // as api.cu forms focal_x / focal_y
+	}
+	Cov2DTerms ct = cov2d_terms(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
 	float det0 = 0.f;  // det of the screen-space covariance before the low-pass (AA only)
 	if (AA) det0 = fmaf(-cov.m[0][1], cov.m[0][1], cov.m[0][0] * cov.m[1][1]);  // explicit fma: rounding independent of contraction
@@ -206,8 +213,14 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* m
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0) return;
-	if (a.antialias) project_fwd_kernel<true><<<ceil_div(a.P, 256), 256, 0, s>>>(a);
-	else project_fwd_kernel<false><<<ceil_div(a.P, 256), 256, 0, s>>>(a);
+	const int grid = ceil_div(a.P, 256);
+	if (a.tan_fov) {
+		if (a.antialias) project_fwd_kernel<true, true><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, true><<<grid, 256, 0, s>>>(a);
+	} else {
+		if (a.antialias) project_fwd_kernel<true, false><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, false><<<grid, 256, 0, s>>>(a);
+	}
 }
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s)
 {

@@ -67,7 +67,8 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // g o ds = g o_eff (grad d0 / d0 - grad d1 / d1) / 2 (s^2 = r there): no raw opacity and no square root beyond s itself.
 // o_eff is read back from the view's conic_opacity.w; s is recomputed from S'.
 //
-// CAM (camera gradients): per view, each thread forms the camera terms of its Gaussian (zeros where culled or past the end:
+// CAM (camera gradients, and the instantiation that reads a view's device field of view, a.intr[v].tan_fov, when set): per
+// view, each thread forms the camera terms of its Gaussian (zeros where culled or past the end:
 // `in` false), the warp sums them into cam_sm[(warp, view)][CAM_TERMS], and the kernel sums its warps after the loop.  A CAM
 // thread therefore runs the whole view loop; it reads Gaussian 0 in place of a missing one and writes no per-Gaussian row.
 template <int NSH, bool AA, bool CAM, class Args>
@@ -146,12 +147,16 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 #pragma unroll
 				for (int c = 0; c < 3; c++) Rv[r][c] = vm[4 * c + r];
 			const float tx = dot3(Rv[0], p) + vm[12], ty = dot3(Rv[1], p) + vm[13], tz = dot3(Rv[2], p) + vm[14];
-			const float limx = 1.3f * w.tan_fovx, limy = 1.3f * w.tan_fovy;
+			// CAM: the view's device field of view, when set; the focal lengths are then formed as the host forms focal_x / focal_y
+			const float* dfov = nullptr;
+			if constexpr (CAM) dfov = a.intr[v].tan_fov;
+			const float tanx = dfov ? dfov[0] : w.tan_fovx, tany = dfov ? dfov[1] : w.tan_fovy;
+			const float limx = 1.3f * tanx, limy = 1.3f * tany;
 			const float ux = tx / tz, uy = ty / tz;
 			const bool inx = !(ux < -limx || ux > limx), iny = !(uy < -limy || uy > limy);
 			const float cx = fminf(limx, fmaxf(-limx, ux)) * tz, cy = fminf(limy, fmaxf(-limy, uy)) * tz;
 			const float iz = 1.0f / tz, iz2 = iz * iz;
-			const float fx = w.focal_x, fy = w.focal_y;
+			const float fx = dfov ? a.intr[v].W / (2.0f * tanx) : w.focal_x, fy = dfov ? a.intr[v].H / (2.0f * tany) : w.focal_y;
 			// M = J Rv: row 0 = (fx / tz) Rv0 - (fx cx / tz^2) Rv2, row 1 likewise with y
 			float m0[3], m1[3], u0[3], u1[3];
 #pragma unroll
@@ -194,6 +199,13 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 #pragma unroll
 			for (int c = 0; c < 3; c++) { q0[c] = 2.f * (H00 * u0[c] + H01 * u1[c]); q1[c] = 2.f * (H01 * u0[c] + H11 * u1[c]); }
 			const float dJ00 = dot3(q0, Rv[0]), dJ02 = dot3(q0, Rv[2]), dJ11 = dot3(q1, Rv[1]), dJ12 = dot3(q1, Rv[2]);
+			if constexpr (CAM) {
+				// dL/dtan_fov: fx = W / (2 tan_fovx) moves J00 = fx / tz and J02 = -fx cx / tz^2 (dfx / dtan_fovx = -fx / tan_fovx),
+				// and where the x clamp holds, cx = +-1.3 tan_fovx tz moves J02.  Likewise for y.
+				const float sx = ux > 0.f ? 1.3f : -1.3f, sy = uy > 0.f ? 1.3f : -1.3f;
+				cg[27] = -(fx / tanx) * (dJ00 * iz - dJ02 * cx * iz2) - (inx ? 0.f : fx * dJ02 * sx * iz);
+				cg[28] = -(fy / tany) * (dJ11 * iz - dJ12 * cy * iz2) - (iny ? 0.f : fy * dJ12 * sy * iz);
+			}
 			const float iz3 = iz2 * iz;
 			float dt[3];
 			dt[0] = inx ? -fx * iz2 * dJ02 : 0.f;
@@ -285,7 +297,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			// order fixed by the lane numbers
 			const int lane = threadIdx.x & 31;
 			warp_halve<16>(cg, lane); warp_halve<8>(cg, lane); warp_halve<4>(cg, lane); warp_halve<2>(cg, lane); warp_halve<1>(cg, lane);
-			if (lane < CAM_TERMS) cam_sm[((threadIdx.x >> 5) * MAX_BWD_VIEWS + v) * CAM_TERMS + lane] = cg[0];
+			if (lane < CAM_ALL_TERMS) cam_sm[((threadIdx.x >> 5) * MAX_BWD_VIEWS + v) * CAM_ALL_TERMS + lane] = cg[0];
 		}
 	}
 	if (CAM && !in) return;
@@ -350,15 +362,20 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 }
 
 // CAM: after the view loop, one barrier and a sum over the CTA's 4 warps in warp order; row `blk` of each view's camera rows
-__device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* const* rows, int blk)
+// (terms < CAM_TERMS) and of its focal-length rows (the rest)
+__device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* const* rows, const ProjectBwdIntr* intr, int blk)
 {
 	__syncthreads();
-	for (int j = threadIdx.x; j < V * CAM_TERMS; j += blockDim.x) {
-		const int v = j / CAM_TERMS, k = j - v * CAM_TERMS;
+	for (int j = threadIdx.x; j < V * CAM_ALL_TERMS; j += blockDim.x) {
+		const int v = j / CAM_ALL_TERMS, k = j - v * CAM_ALL_TERMS;
 		float s = 0.f;
 #pragma unroll
-		for (int w = 0; w < 4; w++) s += cam_sm[(w * MAX_BWD_VIEWS + v) * CAM_TERMS + k];
-		if (rows[v]) rows[v][(size_t)blk * CAM_TERMS + k] = s;
+		for (int w = 0; w < 4; w++) s += cam_sm[(w * MAX_BWD_VIEWS + v) * CAM_ALL_TERMS + k];
+		if (k < CAM_TERMS) {
+			if (rows[v]) rows[v][(size_t)blk * CAM_TERMS + k] = s;
+		} else if (intr[v].rows) {
+			intr[v].rows[(size_t)blk * CAM_INTR_TERMS + k - CAM_TERMS] = s;
+		}
 	}
 }
 
@@ -368,9 +385,9 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(Proj
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if constexpr (CAM) {
-		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_TERMS];
+		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
 		project_bwd_gaussian<NSH, AA, true>(a, idx, idx < a.P, cam_sm);
-		cam_rows_out(cam_sm, a.V, a.cam_rows, blockIdx.x);
+		cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
 	} else {
 		if (idx >= a.P) return;
 		project_bwd_gaussian<NSH, AA, false>(a, idx, true, nullptr);
@@ -390,6 +407,7 @@ struct CloudBwd {
 	static constexpr float* dL_dconic = nullptr;
 	const ProjectBwdView* view;
 	const float4* const* conic_opacity;  // AA only
+	const ProjectBwdIntr* intr;          // CAM only
 };
 }  // namespace
 
@@ -404,12 +422,12 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	if (!CAM && idx >= cl.P) return;
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
 		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
-		AA ? a.conic_opacity + cl.view0 : nullptr };
+		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr };
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
-		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_TERMS];
+		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
 		project_bwd_gaussian<NSH, AA, true>(cb, idx, idx < cl.P, cam_sm);
-		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, (int)blockIdx.x - cl.block0);
+		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
 		project_bwd_gaussian<NSH, AA, false>(cb, idx, true, nullptr);
 	}
@@ -417,26 +435,30 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 
 // one CTA of CAM_REDUCE_THREADS per view.  Thread t first sums rows t, t + 256, ... of every column in row order, then a
 // fixed tree over the 256 partials per column halves them 8 times: a fixed order, no serial chain over all rows.  Thread
-// j < 35 then owns output float j: view matrix 0..15, projection matrix 16..31, camera centre 32..34.
+// j < 37 then owns output float j: view matrix 0..15, projection matrix 16..31, camera centre 32..34, tan_fov 35..36.
 constexpr int CAM_REDUCE_THREADS = 256;
 __global__ void __launch_bounds__(CAM_REDUCE_THREADS) camera_grad_reduce_kernel(CamReduceArgs a)
 {
-	__shared__ float part[CAM_TERMS][CAM_REDUCE_THREADS];
+	__shared__ float part[CAM_ALL_TERMS][CAM_REDUCE_THREADS];
 	const CamReduceView& w = a.view[blockIdx.x];
 	const int t = threadIdx.x;
-	float acc[CAM_TERMS];
+	float acc[CAM_ALL_TERMS];
 #pragma unroll
-	for (int k = 0; k < CAM_TERMS; k++) acc[k] = 0.f;
+	for (int k = 0; k < CAM_ALL_TERMS; k++) acc[k] = 0.f;
 	for (int r = t; r < w.nrows; r += CAM_REDUCE_THREADS) {
 		const float* row = w.rows + (size_t)r * CAM_TERMS;
 #pragma unroll
 		for (int k = 0; k < CAM_TERMS; k++) acc[k] += row[k];
+		if (w.intr_rows) {
+#pragma unroll
+			for (int k = 0; k < CAM_INTR_TERMS; k++) acc[CAM_TERMS + k] += w.intr_rows[(size_t)r * CAM_INTR_TERMS + k];
+		}
 	}
 #pragma unroll
-	for (int k = 0; k < CAM_TERMS; k++) part[k][t] = acc[k];
+	for (int k = 0; k < CAM_ALL_TERMS; k++) part[k][t] = acc[k];
 	__syncthreads();
 	for (int h = CAM_REDUCE_THREADS / 2; h > 0; h >>= 1) {
-		for (int j = t; j < CAM_TERMS * h; j += CAM_REDUCE_THREADS) {
+		for (int j = t; j < CAM_ALL_TERMS * h; j += CAM_REDUCE_THREADS) {
 			const int k = j / h, i = j - k * h;
 			part[k][i] += part[k][i + h];
 		}
@@ -455,6 +477,9 @@ __global__ void __launch_bounds__(CAM_REDUCE_THREADS) camera_grad_reduce_kernel(
 	} else if (j < 35) {
 		o = w.dL_dcampos ? w.dL_dcampos + (j - 32) : nullptr;
 		k = 24 + (j - 32);
+	} else if (j < 37) {
+		o = w.dL_dtan_fov ? w.dL_dtan_fov + (j - 35) : nullptr;
+		k = 27 + (j - 35);
 	}
 	if (!o) return;
 	const float s = k >= 0 ? part[k][0] : 0.f;
@@ -471,8 +496,9 @@ static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, c
 {
 	if (a.antialias) {
 		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
+		// CAM at degree 2: 3 blocks per SM, the camera and focal-length terms spill at the cap of 4 (128)
 		if (deg <= 1) project_bwd_views_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_views_kernel<27, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, CAM, true><<<grid, 128, 0, s>>>(a);
 		else project_bwd_views_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
@@ -487,8 +513,8 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	if (a.P <= 0 || a.V <= 0) return;
 	const int grid = ceil_div(a.P, 128);
 	const int deg = a.shs ? a.D : 0;
-	bool cam = false;
-	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr;
+	bool cam = false;  // camera rows, or a device field of view, which only the CAM instantiation reads
+	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
 	if (cam) project_bwd_views<true>(a, grid, deg, s);
 	else project_bwd_views<false>(a, grid, deg, s);
 }
@@ -500,7 +526,7 @@ static void project_bwd_clouds(const ProjectBwdCloudsArgs& a, int grid, int deg,
 	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
 	if (a.antialias) {
 		if (deg <= 1) project_bwd_clouds_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_clouds_kernel<27, 4, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
 		else project_bwd_clouds_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
@@ -522,7 +548,7 @@ void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 	}
 	const int deg = sh ? a.D : 0;
 	bool cam = false;
-	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr;
+	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
 	if (cam) project_bwd_clouds<true>(a, grid, deg, s);
 	else project_bwd_clouds<false>(a, grid, deg, s);
 }

@@ -111,29 +111,59 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
     return ret
 
 
-def _camera_inputs(views, force=False):
-    """The views' stacked camera tensors (viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3]) as explicit inputs of a node
-    when any of them requires grad (or `force`), else (None, None, None): the node then returns their gradients."""
+def _device_tan_fov(views):
+    """The views' field of view {tan_fovx, tan_fovy} [V,2] when any view carries it as CUDA tensors (e.g. cameras from
+    `cameras.camera_batch` of a learnable intr), stacked with its autograd history; None when every view has host floats."""
+    dev = next((t.device for s in views for t in (s.tanfovx, s.tanfovy) if torch.is_tensor(t) and t.is_cuda), None)
+    if dev is None:
+        return None
+    # host floats of other views are written by fill kernels: no host->device copy, so a CUDA graph can capture it
+    el = lambda t: t.reshape(()).to(torch.float32) if (torch.is_tensor(t) and t.is_cuda) else torch.full((), float(t), device=dev)  # noqa: E731
+    return torch.stack([torch.stack([el(s.tanfovx), el(s.tanfovy)]) for s in views])
+
+
+def _batch_cameras(cameras, ids):
+    """The stacked camera tensors of CameraBatch views `ids`, taken from the batch's own [B,...] tensors (no per-view
+    slicing and restacking): (viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3], tan_fov [V,2] or None)"""
+    every = list(ids) == list(range(len(cameras)))
+    pick = lambda t: (t if every else t[list(ids)]).to(torch.float32)  # noqa: E731
+    tf = pick(cameras.tan_fov) if cameras.tan_fov is not None else None
+    return pick(cameras.world_view_transform), pick(cameras.full_proj_transform), pick(cameras.camera_center), tf
+
+
+def _camera_inputs(views, force=False, batch=None):
+    """The views' stacked camera tensors (viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3], tan_fov [V,2] or None) as
+    explicit inputs of a node when any of them requires grad (or `force`): the node then returns their gradients.  Else
+    (None, None, None, tan_fov).  tan_fov is the device field of view of _device_tan_fov (None without one).  `batch`: the
+    same tensors from _batch_cameras, used as they are."""
+    if batch is not None:
+        if force or any(t is not None and t.requires_grad for t in batch):
+            return batch
+        return None, None, None, batch[3]
     fields = [[getattr(s, n) for s in views] for n in ("viewmatrix", "projmatrix", "campos")]
-    if not force and not any(torch.is_tensor(t) and t.requires_grad for f in fields for t in f):
-        return None, None, None
+    tf = _device_tan_fov(views)
+    if not force and not any(torch.is_tensor(t) and t.requires_grad for f in fields for t in f) and not (tf is not None and tf.requires_grad):
+        return None, None, None, tf
     return tuple(torch.stack([torch.as_tensor(t, dtype=torch.float32).reshape(shape) for t in f])
-                 for f, shape in zip(fields, ((4, 4), (4, 4), (3,))))
+                 for f, shape in zip(fields, ((4, 4), (4, 4), (3,)))) + (tf,)
 
 
 def _camera_outputs(ctx, cam, first):
-    """Gradients for the camera inputs at positions first, first + 1, first + 2 of the node (None where not needed)"""
+    """Gradients for the camera inputs at positions first .. first + 3 of the node (None where not needed; the 4th, tan_fov,
+    only with a device field of view)"""
     if cam is None:
-        return None, None, None
+        return None, None, None, None
     V = cam[0].shape[0]
-    shapes = ((V, 4, 4), (V, 4, 4), (V, 3))
-    return tuple(g.view(shape) if ctx.needs_input_grad[first + i] else None for i, (g, shape) in enumerate(zip(cam, shapes)))
+    shapes = ((V, 4, 4), (V, 4, 4), (V, 3), (V, 2))
+    cam = tuple(cam) + (None,) * (4 - len(cam))
+    return tuple(g.view(shape) if (g is not None and ctx.needs_input_grad[first + i]) else None
+                 for i, (g, shape) in enumerate(zip(cam, shapes)))
 
 
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
-                group, antialiasing=False, cam_vm=None, cam_pm=None, cam_cp=None):
+                group, antialiasing=False, cam_vm=None, cam_pm=None, cam_cp=None, cam_tf=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -152,13 +182,13 @@ class _RasterizeViews(torch.autograd.Function):
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
                                             debug=views[0].debug, out_buffers=(color, feat_img, depth, alpha),
-                                            return_alpha=return_alpha, antialiasing=antialiasing)
+                                            return_alpha=return_alpha, antialiasing=antialiasing, tan_fov=cam_tf)
         main = torch.cuda.current_stream(dev)
         for st in streams:
             main.wait_stream(st)
         radii = torch.stack([o[3] for o in outs])
         ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
-        ctx.camera = cam_vm is not None
+        ctx.camera, ctx.tan_fov = cam_vm is not None, (cam_tf.detach() if cam_tf is not None else None)
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
         ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
@@ -195,7 +225,8 @@ class _RasterizeViews(torch.autograd.Function):
                                            sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
                                            accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
                                            after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
-                                           antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None)
+                                           antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None,
+                                           tan_fov=ctx.tan_fov)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
             # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields.
@@ -273,7 +304,8 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
-                target_depth=None, target_mask=None, antialiasing=False, ssim=False, cam_vm=None, cam_pm=None, cam_cp=None):
+                target_depth=None, target_mask=None, antialiasing=False, ssim=False, cam_vm=None, cam_pm=None, cam_cp=None,
+                cam_tf=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -300,13 +332,13 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                             views[0].scale_modifier, None, sh, degree, include, debug=views[0].debug,
                                             out_buffers=(color, feat_img, None),
                                             loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm,
-                                            antialiasing=antialiasing, ssim=ssim_head)
+                                            antialiasing=antialiasing, ssim=ssim_head, tan_fov=cam_tf)
         N = float(H * W)
         loss_rgb = loss_acc[:, 0] / (3.0 * N)
         loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
         radii = torch.stack([o[3] for o in outs])
         ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
-        ctx.camera = cam_vm is not None
+        ctx.camera, ctx.tan_fov = cam_vm is not None, (cam_tf.detach() if cam_tf is not None else None)
         # capacity, radii and the three state buffers per view -- never the images: they are views of this node's outputs, and an
         # output kept on ctx is a reference cycle (output -> grad_fn -> ctx -> output) that leaks the whole step
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]
@@ -352,7 +384,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
                                      antialiasing=ctx.antialiasing,
                                      ssim=ctx.ssim + (color, ctx.target_rgb) if ctx.ssim is not None else None,
                                      ssim_scale=_pair_scale(g_l1, g_ssim, V, dev) if ctx.ssim is not None else None,
-                                     camera_grads=True if ctx.camera else None)
+                                     camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov)
         if ctx.group is not None:
             pk.all_reduce_finish(grp)
         v = pk.views
@@ -391,7 +423,10 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     §5); also on when the given settings carry antialiasing=True.  Combines with every option above.
     Camera gradients: when a view's viewmatrix, projmatrix or campos requires grad (e.g. cameras from
     `cameras.camera_batch` of a learnable w2c), the backward also returns their gradients (INTEGRATION.md §6); this combines
-    with every option above.
+    with every option above.  Learnable intrinsics: views whose tanfovx / tanfovy are CUDA tensors (cameras from
+    `cameras.camera_batch` of a learnable intr) are projected with that device value, with no device->host read and read
+    afresh at every CUDA-graph replay; when it requires grad, the backward returns its gradient through the Jacobian and the
+    frustum clamp, beside the projection-matrix path.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -401,8 +436,10 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
         bg = _background(bg_color, device)
         views = tuple(cameras.settings(i, bg, sh_degree, include) for i in ids)
+        batch = _batch_cameras(cameras, ids) if ids else None
     else:
         views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+        batch = None
     if not views:
         raise ValueError("render_views needs at least one view")
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for s in views)
@@ -415,7 +452,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     screenspace_points = torch.zeros((V, P, 3), dtype=torch.float32, device=device, requires_grad=True)
     if ssim and targets is None:
         raise ValueError("ssim=True needs targets (the colour target \"rgb\")")
-    cams = _camera_inputs(views)
+    cams = _camera_inputs(views, batch=batch)
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
@@ -435,7 +472,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         if ssim:
             ret["loss_l1"], ret["ssim"] = loss_l1, ssim_v
         return ret
-    if V == 1 and sync_gradients is None and cams[0] is None:
+    if V == 1 and sync_gradients is None and cams[0] is None and cams[3] is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True) if aa else views[0]
         out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha)(
@@ -574,11 +611,11 @@ class _RasterizeClouds(torch.autograd.Function):
             M = clouds[b]["sh"].shape[1] if clouds[b]["sh"] is not None else 0
             ret += [r["dL_dmeans3D"], r["dL_dmeans2D"], r["dL_dsh"].view(P, M, 3) if M else None, r["dL_dcolors"], r["dL_dfeature"],
                     r["dL_dopacity"].view(ctx.opac_shapes[b]), r["dL_dscales"], r["dL_drotations"]]
-        if camera:  # the stacked camera tensors of every cloud behind its Gaussian inputs
+        if camera:  # the stacked camera tensors of every cloud behind its Gaussian inputs, four per cloud
             first = 1 + _CLOUD_INPUTS * len(cloud_views)
             for b, r in enumerate(res):
-                cam = (r["dL_dviewmatrix"], r["dL_dprojmatrix"], r["dL_dcampos"])
-                ret += _camera_outputs(ctx, cam, first + 3 * b)
+                cam = (r["dL_dviewmatrix"], r["dL_dprojmatrix"], r["dL_dcampos"], r.get("dL_dtan_fov"))
+                ret += _camera_outputs(ctx, cam, first + 4 * b)
         return tuple(ret)
 
 
@@ -596,7 +633,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     A cloud whose "features_language" does not require grad gets no feature gradient computed (e.g. the next frame of the
     dyna step, which renders the detached current features); its feature cotangents still reach its other gradients.
     antialiasing: every cloud renders with the anti-aliased projection, as in render_views.
-    Camera gradients: as in render_views, per cloud; clouds that share camera tensors (the dyna pair) receive the sum.
+    Camera gradients: as in render_views, per cloud (with the field of view of cameras from a learnable intr); clouds that
+    share camera tensors (the dyna pair) receive the sum.
     ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
@@ -612,7 +650,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     if len({c.get("features_color") is None for c in clouds}) > 1:
         raise ValueError("clouds disagree on the colour mode (SHs or precomputed colors)")
     device = clouds[0]["pts_xyz"].device
-    cloud_views = []
+    cloud_views, batches = [], []
     for b, c in enumerate(clouds):
         include = c.get("features_language") is not None
         sh_degree = 3 if c.get("features_color") is None else 1
@@ -620,8 +658,10 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         if isinstance(cameras, CameraBatch):
             ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
             views = tuple(cameras.settings(i, _background(bg_color, device), sh_degree, include) for i in ids)
+            batches.append(_batch_cameras(cameras, ids) if ids else None)
         else:
             views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+            batches.append(None)
         if not views:
             raise ValueError(f"cloud {b} has no views")
         if c.get("features_color") is None and c.get("pts_rgb") is None:
@@ -644,10 +684,11 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for views in cloud_views for s in views)
-    cams = [_camera_inputs(views) for views in cloud_views]
+    cams = [_camera_inputs(views, batch=bt) for views, bt in zip(cloud_views, batches)]
     camera = any(c[0] is not None for c in cams)
     if camera:  # every cloud's stacked cameras, as explicit inputs (the dyna pair's shared tensors get both frames' sums)
-        cams = [c if c[0] is not None else _camera_inputs(views, force=True) for c, views in zip(cams, cloud_views)]
+        cams = [c if c[0] is not None else _camera_inputs(views, force=True, batch=bt)
+                for c, views, bt in zip(cams, cloud_views, batches)]
         flat += [t for c in cams for t in c]
     out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim), camera),
                                  *flat)

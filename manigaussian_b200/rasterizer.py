@@ -252,6 +252,10 @@ def state_array(which, name, state, a0, a1=0):
     return out.value
 
 
+def _is_device_fov(s):
+    return any(torch.is_tensor(t) and t.is_cuda for t in (s.tanfovx, s.tanfovy))
+
+
 def cpu_deep_copy_tuple(input_tuple):
     return tuple(item.cpu().clone() if isinstance(item, torch.Tensor) else item for item in input_tuple)
 
@@ -259,8 +263,11 @@ def cpu_deep_copy_tuple(input_tuple):
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
     s = raster_settings
-    # camera tensors that require grad become explicit inputs of the node, which then returns their gradients
+    # camera tensors that require grad become explicit inputs of the node, which then returns their gradients; a field of
+    # view held as CUDA tensors (learnable intrinsics) joins them as two more inputs, tanfovx and tanfovy
     cam = (s.viewmatrix, s.projmatrix, s.campos)
+    if _is_device_fov(s):
+        cam += (s.tanfovx, s.tanfovy)
     if not any(torch.is_tensor(t) and t.requires_grad for t in cam):
         cam = ()
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
@@ -280,6 +287,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         aa = bool(getattr(s, "antialiasing", False))
         ctx.antialiasing = aa
         ctx.camera = len(cam) > 0
+        # the device field of view, when the settings carry one (read by the kernels in place of host floats)
+        tf = _fov_column([s], means3D.device) if (views_path and _is_device_fov(s)) else None
+        ctx.tan_fov = tf
         alpha = None
         if (return_alpha or aa or ctx.camera) and views_path:
             # the alpha plane, the anti-aliased projection and the camera gradients exist on the multi-view entry points only:
@@ -289,7 +299,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
                                                     rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
                                                     return_depth=return_depth, debug=s.debug, return_alpha=return_alpha,
-                                                    antialiasing=aa)
+                                                    antialiasing=aa, tan_fov=tf)
             except Exception as ex:
                 if s.debug:
                     torch.save(cpu_args, "snapshot_fw.dump")
@@ -311,7 +321,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             # the count back on every call, rasterizer_impl.cu:284); the operator itself never exposes the count
             outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations,
                                                 s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
-                                                return_depth=return_depth)
+                                                return_depth=return_depth, tan_fov=tf)
             out = outs[0]
             # only the capacity and the streams: the images and radii in `outs` are OUTPUTS of this node, and an output kept on
             # ctx is a reference cycle (output -> grad_fn -> ctx -> output) that no collector frees -- the state buffers and the
@@ -360,7 +370,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                     colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
                     s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None, debug=s.debug,
                     grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing,
-                    camera_grads=True if ctx.camera else None)
+                    camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -381,10 +391,15 @@ class _RasterizeGaussians(torch.autograd.Function):
         grad_cam = ()
         if ctx.camera:
             # zero gradients when the views path did not run (no Gaussians: nothing depends on the camera)
-            dvm, dpm, dcp = grads[9] if len(grads) > 9 else (torch.zeros((1, 16), device=means3D.device),) * 2 + (
-                torch.zeros((1, 3), device=means3D.device),)
-            grad_cam = tuple(g.view(t.shape) if ctx.needs_input_grad[12 + i] else None
-                             for i, (g, t) in enumerate(zip((dvm, dpm, dcp), (s.viewmatrix, s.projmatrix, s.campos))))
+            z = lambda n: torch.zeros((1, n), device=means3D.device)  # noqa: E731
+            cg = grads[9] if len(grads) > 9 else (z(16), z(16), z(3), z(2))
+            dvm, dpm, dcp = cg[:3]
+            gs, ts = [dvm, dpm, dcp], [s.viewmatrix, s.projmatrix, s.campos]
+            if _is_device_fov(s):   # tanfovx, tanfovy: the two entries of the view's dL/dtan_fov
+                dtf = cg[3] if len(cg) > 3 else z(2)
+                gs += [dtf[0, 0], dtf[0, 1]]
+                ts += [s.tanfovx, s.tanfovy]
+            grad_cam = tuple(g.reshape(t.shape) if ctx.needs_input_grad[12 + i] else None for i, (g, t) in enumerate(zip(gs, ts)))
 
         def _or_none(g, inp):
             return g if (inp is not None and inp.numel() != 0) else None
@@ -597,7 +612,7 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None):
+                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -613,7 +628,10 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc.  `antialiasing`: the
     anti-aliased projection (C ABI mgs_forward_views_aa); pass the same value to the backward.  `ssim` = (ssim_terms
     [V,9,H,W], loss_acc [V,4], cot_color [V,3,H,W]), with `loss_heads` only: behind each view's blend, the L1 + SSIM head
-    (C ABI mgs_view_ssim) leaves {sum |x - g|, sum S} in loss_acc[:, :2] and the partials of S in ssim_terms."""
+    (C ABI mgs_view_ssim) leaves {sum |x - g|, sum S} in loss_acc[:, :2] and the partials of S in ssim_terms.  `tan_fov`
+    [V,2] (device): every view's {tan_fovx, tan_fovy}, read by the kernels in place of the settings' host floats (C ABI
+    mgs_forward_views_intr); views whose tanfovx / tanfovy are CUDA tensors use it without being asked.  Pass the same to
+    the backward."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -660,7 +678,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             outs.append(o)
         rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
-        if sarr is not None:
+        tf = _device_fov(views, tan_fov, dev)
+        if tf is not None:
+            keep.append(tf)
+            _b.check(L.mgs_forward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None), *rest),
+                     "mgs_forward_views_intr")
+        elif sarr is not None:
             _b.check(L.mgs_forward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_forward_views_ssim")
         elif antialiasing:
             _b.check(L.mgs_forward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_forward_views_aa")
@@ -724,7 +747,7 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
         out_alpha = ob[v] if ob is not None else torch.empty((H, W), dtype=torch.float32, device=dev)
         wa.out_alpha = _ptr(out_alpha)
     w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
-    w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
+    w.tan_fovx, w.tan_fovy, w.width, w.height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
     w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
     w.out_color, w.out_feature, w.out_depth, w.radii = _ptr(out_color), (_ptr(out_feature) if F else None), _ptr(out_depth), _ptr(radii)
     if loss_heads is not None:
@@ -735,6 +758,49 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
     ret = (cap, out_color, out_feature, radii, geom, binb, img) + ((out_depth,) if return_depth else ())
     ret += (out_alpha,) if wa is not None else ()
     return ViewOut(ret), (bg, vm, pm, cp)
+
+
+def _host_tan(x):
+    """mgs_view.tan_fov* of a view: its host float, or 0 for a CUDA tensor (the call then reads the device value through
+    mgs_view_intrinsics; no device->host read)"""
+    return 0.0 if (torch.is_tensor(x) and x.is_cuda) else float(x)
+
+
+def _device_fov(views, tan_fov, dev):
+    """The views' device field of view {tan_fovx, tan_fovy} [V,2] (fp32, contiguous, detached): `tan_fov` when given, else
+    stacked from views whose tanfovx / tanfovy are CUDA tensors; None when neither (the host floats serve)."""
+    if tan_fov is None:
+        if not any(torch.is_tensor(t) and t.is_cuda for s in views for t in (s.tanfovx, s.tanfovy)):
+            return None
+        return _fov_column(views, dev)
+    tan_fov = tan_fov.detach()
+    if tuple(tan_fov.shape) != (len(views), 2):
+        raise ValueError(f"tan_fov: expected [{len(views)},2], got {tuple(tan_fov.shape)}")
+    return _prep(tan_fov, dev)
+
+
+def _fov_column(views, dev):
+    """[V,2] fp32 device tensor of the views' {tanfovx, tanfovy}: device values are copied on the device, host floats are
+    written by fill kernels -- no host->device copy from pageable memory, so it can be captured in a CUDA graph."""
+    out = torch.empty((len(views), 2), dtype=torch.float32, device=dev)
+    with torch.no_grad():
+        for v, s in enumerate(views):
+            for i, t in enumerate((s.tanfovx, s.tanfovy)):
+                if torch.is_tensor(t) and t.is_cuda:
+                    out[v, i].copy_(t.reshape(()))
+                else:
+                    out[v, i].fill_(float(t))
+    return out
+
+
+def _intrinsics_array(tf, dtf):
+    """ViewIntrinsics array of the views' device field of view tf [V,2] and its gradient output dtf [V,2] (or None)."""
+    V = tf.shape[0]
+    iarr = (_b.ViewIntrinsics * V)()
+    for v in range(V):
+        iarr[v].tan_fov = tf.data_ptr() + 8 * v
+        iarr[v].dL_dtan_fov = dtf.data_ptr() + 8 * v if dtf is not None else None
+    return iarr
 
 
 def _track_status(outs, keys, status, main, pending):
@@ -751,7 +817,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
-                                 ssim=None, ssim_scale=None, camera_grads=None):
+                                 ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -769,7 +835,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     its blend backward reads it.  `camera_grads`: True, or a tuple (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16], dL_dcampos
     [V,3]) of fp32 device tensors or None each, asks for the gradients with respect to each view's viewmatrix, projmatrix and
     campos (C ABI mgs_backward_views_cam; written, or added to with accumulate=True); the return value then gains that tuple
-    (allocated for True) as a 10th element."""
+    (allocated for True) as a 10th element.  `tan_fov`: as given to the forward (views with CUDA-tensor tanfov* imply it);
+    with it the call is mgs_backward_views_intr, and `camera_grads` gains a 4th entry, dL_dtan_fov [V,2] (the gradient with
+    respect to each view's {tan_fovx, tan_fovy}; allocated for True, or named in a 4-tuple)."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -827,14 +895,20 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 w.cot_scale = cot_scale.data_ptr() + 8 * v
             if sarr is not None:
                 _fill_ssim(sarr[v], ssim, v, w, sscale)
-        cam, carr = _camera_grads(L, camera_grads, [P] * V, dev, keep)
+        tf = _device_fov(views, tan_fov, dev)
+        cam, carr = _camera_grads(L, camera_grads, [P] * V, dev, keep, tf is not None)
+        iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+        keep.append(tf)
         for stages in ((1, 2) if after_blend is not None else (3,)):
             rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
                     _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if carr is not None:
+            if iarr is not None:
+                _b.check(L.mgs_backward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, *rest),
+                         "mgs_backward_views_intr")
+            elif carr is not None:
                 _b.check(L.mgs_backward_views_cam(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, *rest), "mgs_backward_views_cam")
             elif sarr is not None:
                 _b.check(L.mgs_backward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_backward_views_ssim")
@@ -852,17 +926,20 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     return grads + (cam,) if cam is not None else grads
 
 
-def _camera_grads(L, camera_grads, Ps, dev, keep):
+def _camera_grads(L, camera_grads, Ps, dev, keep, intr=False):
     """(outputs, ViewCameraGrad array) for the views of clouds of Ps[v] Gaussians, or (None, None) without camera_grads.
-    True allocates the three outputs [V,16], [V,16], [V,3]; a tuple names them (each a contiguous fp32 device tensor of that
-    shape, or None)."""
+    True allocates the three outputs [V,16], [V,16], [V,3] (and with `intr` a 4th, dL_dtan_fov [V,2]); a tuple names them
+    (each a contiguous fp32 device tensor of that shape, or None)."""
     if camera_grads is None or camera_grads is False:
         return None, None
     V = len(Ps)
     opts = dict(dtype=torch.float32, device=dev)
     if camera_grads is True:
-        camera_grads = (torch.empty((V, 16), **opts), torch.empty((V, 16), **opts), torch.empty((V, 3), **opts))
-    shapes = ((V, 16), (V, 16), (V, 3))
+        camera_grads = (torch.empty((V, 16), **opts), torch.empty((V, 16), **opts), torch.empty((V, 3), **opts)) + \
+            ((torch.empty((V, 2), **opts),) if intr else ())
+    if intr and len(camera_grads) == 3:
+        camera_grads = tuple(camera_grads) + (None,)
+    shapes = ((V, 16), (V, 16), (V, 3), (V, 2))
     for t, shape in zip(camera_grads, shapes):
         if t is not None and (t.dtype != torch.float32 or t.device != dev or not t.is_contiguous() or t.numel() != shape[0] * shape[1]):
             raise ValueError(f"camera_grads: expected contiguous fp32 tensors of {shape} on {dev}")
@@ -887,7 +964,7 @@ def _backward_view(L, w, s, o, dev, P, grad_color, grad_feature, grad_depth):
     gc, gf, gd = (_prep(x, dev) for x in (grad_color, grad_feature, grad_depth))
     scratch = torch.empty((_state_sizes(L, P, W, H)[2],), dtype=torch.uint8, device=dev)
     w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
-    w.tan_fovx, w.tan_fovy, w.width, w.height = float(s.tanfovx), float(s.tanfovy), W, H
+    w.tan_fovx, w.tan_fovy, w.width, w.height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
     w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = o[4].data_ptr(), o[5].data_ptr(), o[6].data_ptr(), int(o[0])
     w.radii = _ptr(o[3])
     w.dL_dpix, w.dL_dpix_F, w.dL_dpix_depth = _ptr(gc), _ptr(gf), _ptr(gd)
@@ -938,7 +1015,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
     Capacity history is kept per (device, P, W, H, cloud slot, view slot).  `antialiasing`: the anti-aliased projection for
-    every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward."""
+    every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
+    (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -994,7 +1072,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 cloud_outs.append(o)
             outs.append(cloud_outs)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if sarr is not None:
+        tf = _clouds_fov(clouds, dev)
+        if tf is not None:
+            keep.append(tf)
+            _b.check(L.mgs_forward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None),
+                                               *rest), "mgs_forward_clouds_intr")
+        elif sarr is not None:
             _b.check(L.mgs_forward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
                      "mgs_forward_clouds_ssim")
         elif antialiasing:
@@ -1011,6 +1094,15 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     return outs, streams
 
 
+def _clouds_fov(clouds, dev):
+    """[V,2] device field of view of every view of the clouds in order, or None when no cloud has one (the clouds without
+    one contribute their host floats)"""
+    tfs = [_device_fov(c["views"], c.get("tan_fov"), dev) for c in clouds]
+    if all(t is None for t in tfs):
+        return None
+    return torch.cat([t if t is not None else _fov_column(c["views"], dev) for t, c in zip(tfs, clouds)])
+
+
 def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False,
                                   antialiasing=False, camera_grads=False):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
@@ -1025,7 +1117,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed).  `antialiasing`: the value
     the forward was given (C ABI mgs_backward_clouds_aa).  `camera_grads=True`: every cloud's dict also holds the gradients
     with respect to its views' viewmatrix, projmatrix and campos, "dL_dviewmatrix" [V_b,16], "dL_dprojmatrix" [V_b,16] and
-    "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam)."""
+    "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam).  Clouds with a device field of view (see rasterize_clouds_raw)
+    make the call mgs_backward_clouds_intr, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1086,13 +1179,20 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 if c.get("ssim") is not None:
                     _fill_ssim(sarr[g], c["ssim"], v, w, sscale)
             keep.append(cot)
-        cam, camarr = _camera_grads(L, bool(camera_grads), [d["P"] for d, c in zip(pc, clouds) for _ in c["views"]], dev, keep)
+        tf = _clouds_fov(clouds, dev)
+        keep.append(tf)
+        cam, camarr = _camera_grads(L, bool(camera_grads), [d["P"] for d, c in zip(pc, clouds) for _ in c["views"]], dev, keep,
+                                    tf is not None)
         if cam is not None:
             for b, gr in enumerate(grads):
-                for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos"), cam):
+                for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if camarr is not None:
+        if tf is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None)
+            _b.check(L.mgs_backward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, *rest),
+                     "mgs_backward_clouds_intr")
+        elif camarr is not None:
             _b.check(L.mgs_backward_clouds_cam(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, *rest),
                      "mgs_backward_clouds_cam")
         elif sarr is not None:
