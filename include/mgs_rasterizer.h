@@ -22,6 +22,7 @@
  *    ceil(F / 32));
  *  - an optional depth plane (out_depth / dL_dpix_depth) renders view-space z as one more blended channel;
  *  - an optional alpha plane (mgs_view_alpha, multi-view and multi-cloud calls) returns the accumulated opacity 1 - final_T;
+ *  - an optional median-depth plane and per-pixel surface Gaussian id (mgs_view_median, the same calls);
  *  - work is enqueued on `stream` (the reference uses the legacy default stream);
  *  - outputs are fully overwritten: callers need not zero-initialise them.
  *
@@ -730,6 +731,82 @@ int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_off
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
 	int debug, void* join_stream);
+
+/*
+ * Median depth and surface Gaussian (no reference counterpart; 2DGS's median_contributor).  The _median calls are the _intr
+ * calls with one more argument, `median`: one mgs_view_median per view (V entries, or view_offsets[B] for clouds), or NULL;
+ * the _intr calls are these with median == NULL.
+ *
+ * Definition.  For pixel p, walk its contributors front to back with the forward blend's own decisions (the pairs whose
+ * pixel-mask bit is set, "pixel_masks" of mgs_state_array) and its fp32 transmittance T before each pair:
+ *   - the median contributor is the last contributor whose incoming T > 0.5.  T only decreases, so this is the contributor
+ *     at which T first falls to 0.5 or below; where T never gets there it is the pixel's last contributor (mask such pixels
+ *     with the alpha plane, e.g. alpha > 0.5);
+ *   - median_id[p] = that Gaussian's index in its cloud, or -1 where the pixel has no contributor;
+ *   - out_median_depth[p] = that Gaussian's view-space depth, bit for bit the value the depth channel blends for it, or 0
+ *     where the pixel has no contributor.
+ * Backward: dL/dz_i += sum over the pixels p with median_id[p] = i of dL_dpix_median_depth[p], z_i the view-space depth of
+ * Gaussian i, which reaches means3D and the camera gradients through the projection's depth path.  The choice of the
+ * contributor is piecewise constant: no gradient goes to opacity, conic, colour, features or means2D.  The sums use float
+ * atomics, like the blend backward's.
+ * Per view each pointer may be NULL; median_id must be set wherever out_median_depth (forward) or dL_dpix_median_depth
+ * (backward) is, else MGS_ERR_INVALID_ARG before anything is enqueued.  The backward reads the median_id its forward wrote.
+ */
+typedef struct mgs_view_median {
+	float* out_median_depth;              /* forward output [H,W], or NULL */
+	int* median_id;                       /* forward output [H,W] int32; backward input */
+	const float* dL_dpix_median_depth;    /* backward input [H,W], or NULL */
+} mgs_view_median;
+
+int mgs_forward_views_median(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_median(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F, float scale_modifier, int prefiltered,
+	int debug, void* join_stream);
+int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */

@@ -54,6 +54,12 @@ class ViewIntrinsics(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("tan_fov", "dL_dtan_fov")]
 
 
+class ViewMedian(C.Structure):
+    """mirror of `mgs_view_median` (include/mgs_rasterizer.h): the optional median-depth plane and surface-Gaussian ids of
+    one view"""
+    _fields_ = [(n, C.c_void_p) for n in ("out_median_depth", "median_id", "dL_dpix_median_depth")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -147,6 +153,11 @@ def lib():
         getattr(L, intr).restype = C.c_int
         getattr(L, intr).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
             ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics)] + at[k:]
+        # ... and the median planes (one ViewMedian per view, or NULL) after the field of view
+        med = name.replace("_views", "_views_median").replace("_clouds", "_clouds_median")
+        getattr(L, med).restype = C.c_int
+        getattr(L, med).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
+            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -189,6 +200,7 @@ EXPORTED_SYMBOLS = (
     "mgs_ssim", "mgs_ssim_backward",
     "mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam",
     "mgs_forward_views_intr", "mgs_backward_views_intr", "mgs_forward_clouds_intr", "mgs_backward_clouds_intr",
+    "mgs_forward_views_median", "mgs_backward_views_median", "mgs_forward_clouds_median", "mgs_backward_clouds_median",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

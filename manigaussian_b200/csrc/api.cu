@@ -463,15 +463,25 @@ static void depth_mask_args(BlendArgs& ba, const mgs_view_depth_mask* dm)
 	ba.dm_acc = dm->loss_acc; ba.dm_scale = dm->cot_scale;
 }
 
+// the median plane of one view (m nullable): a median-depth output or cotangent needs the id plane
+static int check_median(const mgs_view_median* m)
+{
+	if (m && !m->median_id && (m->out_median_depth || m->dL_dpix_median_depth))
+		return fail(MGS_ERR_INVALID_ARG, "view: out_median_depth and dL_dpix_median_depth need median_id (in its mgs_view_median)");
+	return 0;
+}
+
 // forward blend, with the fused loss heads when the view has a target; out_alpha (nullable) receives 1 - final_T; dm
-// (nullable): the view's depth / mask heads
-static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, const mgs_view_depth_mask* dm, int debug)
+// (nullable): the view's depth / mask heads; med (nullable): its median plane (checked by check_median)
+static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, const mgs_view_depth_mask* dm,
+	const mgs_view_median* med, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = (c.F > 0 && c.feature && w.out_feature) ? c.F : 0;
 	BlendArgs ba = blend_args(carve_view(w, c.P), w, F, c.feature);
 	ba.want_depth = w.out_depth != nullptr;
 	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth; ba.out_alpha = out_alpha;
+	if (med && med->median_id) { ba.median_id = med->median_id; ba.out_median_depth = med->out_median_depth; }
 	// the cosine embedding head needs a pixel's whole feature vector: in the blend epilogue when one CTA holds it (F <= 32),
 	// else in a features-only pass of the loss-heads kernel over the planes the blend just wrote
 	const bool embed = w.target_color && w.target_feature && F > 0;
@@ -537,14 +547,19 @@ static int enqueue_ssim_bwd(mgs_view& w, const mgs_view_ssim* s, int debug)
 // blend backward of one view on its stream: the view's blend-stage records, and the feature gradients summed with 128-bit
 // reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
 // and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane; dm
-// (nullable): the view's depth / mask heads, whose cotangent planes the walker's prologue folds in.
+// (nullable): the view's depth / mask heads, whose cotangent planes the walker's prologue folds in; med (nullable): its
+// median plane, whose cotangent goes to the median contributors' depth slots.
 static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, const float* dL_dalpha, const mgs_view_depth_mask* dm,
-	int debug)
+	const mgs_view_median* med, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = c.F;
 	const ViewState s = carve_view(w, c.P);
 	MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)c.P * GB_STRIDE * sizeof(float), st));
+	if (med && med->dL_dpix_median_depth) {
+		launch_median_depth_bwd(w.width * w.height, med->median_id, med->dL_dpix_median_depth, s.gb, st);
+		MGS_STAGE("median_depth_bwd");
+	}
 	BlendArgs ba = blend_args(s, w, F, c.feature);
 	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth; ba.dL_dalpha = dL_dalpha;
 	ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
@@ -600,7 +615,8 @@ static void camera_view(const mgs_view_camera_grad* cam, const mgs_view_intrinsi
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
+	const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -612,7 +628,9 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		for (int v = 0; v < V; v++) {
 			mgs_view w = views[v];
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
-			if (rc == 0) rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr, debug);
+			if (rc == 0)
+				rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr,
+					med ? med + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -762,7 +780,7 @@ int mgs_forward(
 	w.binning_capacity = num_rendered;
 	rc = enqueue_binning(c, w, true, debug);
 	if (rc < 0) return rc;
-	rc = enqueue_blend_fwd(c, w, nullptr, nullptr, debug);
+	rc = enqueue_blend_fwd(c, w, nullptr, nullptr, nullptr, debug);
 	return rc < 0 ? rc : num_rendered;
 }
 
@@ -810,7 +828,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -878,6 +896,18 @@ int mgs_forward_views_intr(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_median(V, views, alpha, depth_mask, antialiasing, ssim, intr, nullptr, P, D, M, F, means3D, shs,
+		colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_median(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -890,6 +920,7 @@ int mgs_forward_views_intr(
 		int rc = check_fwd_view(views[v], !colors_precomp);
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
+		if (rc == 0) rc = check_median(median ? median + v : nullptr);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
@@ -913,7 +944,8 @@ int mgs_forward_views_intr(
 		for (int v = 0; v < V; v++) {
 			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
-				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
+				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
+					median ? median + v : nullptr, debug);
 			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
@@ -1010,6 +1042,20 @@ int mgs_backward_views_intr(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_median(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, nullptr, P, D, M, F, means3D, shs,
+		colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
+		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_median(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -1021,12 +1067,13 @@ int mgs_backward_views_intr(
 		int rc = check_bwd_view(views[v], F > 0);
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
+		if (rc == 0) rc = check_median(median ? median + v : nullptr);
 		if (rc < 0) return rc;
 	}
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1071,6 +1118,15 @@ int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offs
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
 	const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_median(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, nullptr, D, M, F,
+		scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F, float scale_modifier, int prefiltered,
+	int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -1086,6 +1142,7 @@ int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offs
 			rc = check_fwd_view(views[v], !k.colors_precomp);
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
+			if (rc == 0) rc = check_median(median ? median + v : nullptr);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1100,7 +1157,8 @@ int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offs
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
-					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr, debug);
+					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
+						median ? median + v : nullptr, debug);
 				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
@@ -1159,6 +1217,15 @@ int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_off
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
 	int debug, void* join_stream)
 {
+	return mgs_backward_clouds_median(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, nullptr, D, M,
+		F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -1173,6 +1240,7 @@ int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_off
 			rc = check_bwd_view(views[v], F > 0 && k.feature);
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
+			if (rc == 0) rc = check_median(median ? median + v : nullptr);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1193,7 +1261,7 @@ int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_off
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
 			if (rc == 0)
 				rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
-					depth_mask ? depth_mask + v : nullptr, debug);
+					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}

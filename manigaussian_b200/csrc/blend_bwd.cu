@@ -1009,4 +1009,20 @@ void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
 	else launch_bwd_dm<false>(a, s);
 }
 
+// The median depth is the view-space z of one Gaussian per pixel, chosen by a piecewise-constant rule: its cotangent goes to
+// that Gaussian's depth slot of the blend-stage records and nowhere else.  One thread per pixel.
+__global__ void median_depth_bwd_kernel(int N, const int* __restrict__ median_id, const float* __restrict__ dL_dmedian, float* gb)
+{
+	const int p = blockIdx.x * blockDim.x + threadIdx.x;
+	if (p >= N) return;
+	const int id = median_id[p];
+	const float g = dL_dmedian[p];
+	if (id >= 0 && g != 0.f) red_add(gb + (size_t)id * GB_STRIDE + 9, g);
+}
+
+void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s)
+{
+	if (N > 0) median_depth_bwd_kernel<<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb);
+}
+
 }  // namespace mgs

@@ -43,7 +43,8 @@ static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32, "forward chunk size");
 
 // GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic.
 // DM: the depth / mask heads (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.
-template <int NFT, bool VEC, bool GRP, bool DM>
+// MED: the median contributor (BlendArgs::median_id / out_median_depth); likewise.
+template <int NFT, bool VEC, bool GRP, bool DM, bool MED>
 __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendArgs a)
 {
 	using L = RowLayout<NFT>;
@@ -91,6 +92,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 	// transmittance after the last accepted pair = the reference's final T.  Pixels outside the image start at 0.
 	float T = inside ? 1.0f : 0.0f, T_out = 1.0f;
 	uint32_t last = 0;  // 1-based block-list entry of this pixel's last contributor
+	uint32_t med = 0;   // MED: 1-based block-list entry of its last contributor with incoming T > 0.5
 	float acc[2][NT][4];
 #pragma unroll
 	for (int mt = 0; mt < 2; mt++)
@@ -172,6 +174,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				wrow[(u & 3) * 64 + (u >> 2) * 2 + wofs] = use ? alpha * T : 0.f;
 				T_out = use ? test_T : T_out;
 				last = (use && alpha != 0.f) ? (uint32_t)(k0 + 8 * ks + u + 1) : last;
+				if (MED) med = (use && alpha != 0.f && T > 0.5f) ? (uint32_t)(k0 + 8 * ks + u + 1) : med;
 				T = test_T;
 				s_pm[8 * ks + u] = __ballot_sync(0xffffffffu, use && alpha != 0.f);  // warp-uniform: every lane stores the same word
 			}
@@ -230,6 +233,12 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			a.final_T[pix] = T;
 			a.n_contrib[pix] = last ? lrow[last - 1] + 1u : 0u;  // 1-based tile-list position, as the reference counts
 			if (a.out_alpha) a.out_alpha[pix] = 1.f - T;
+			if (MED) {
+				// the entry's tile-list position names the Gaussian; its depth is the value the depth channel blends
+				const int id = med ? (int)a.point_list[range.x + lrow[med - 1]] : -1;
+				a.median_id[pix] = id;
+				if (a.out_median_depth) a.out_median_depth[pix] = med ? a.rgbd[id].w : 0.f;
+			}
 		}
 	}
 	if (first) {
@@ -372,7 +381,7 @@ bool feature_rows_vectorizable(const float* feature, int F)
 	return F > 0 && (F & 3) == 0 && (reinterpret_cast<uintptr_t>(feature) & 15) == 0;
 }
 
-template <int NFT, bool GRP, bool DM>
+template <int NFT, bool GRP, bool DM, bool MED>
 static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
@@ -380,27 +389,31 @@ static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 	// groups, a row slice starts at channel 32 g: 16-byte aligned whenever F % 4 == 0, and a remainder group copies whole
 	// 4-channel pieces only.
 	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F));
-	if (vec) blend_fwd_kernel<NFT, true, GRP, DM><<<grid, 32, 0, s>>>(a);
-	else blend_fwd_kernel<NFT, false, GRP, DM><<<grid, 32, 0, s>>>(a);
+	if (vec) blend_fwd_kernel<NFT, true, GRP, DM, MED><<<grid, 32, 0, s>>>(a);
+	else blend_fwd_kernel<NFT, false, GRP, DM, MED><<<grid, 32, 0, s>>>(a);
 }
 
-template <bool DM>
+template <bool DM, bool MED>
 static void launch_fwd_dm(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.groups > 1) { launch_fwd_t<4, true, DM>(a, s); return; }
+	if (a.groups > 1) { launch_fwd_t<4, true, DM, MED>(a, s); return; }
 	switch (nft_for(a.F)) {
-	case 0: launch_fwd_t<0, false, DM>(a, s); break;
-	case 1: launch_fwd_t<1, false, DM>(a, s); break;
-	case 2: launch_fwd_t<2, false, DM>(a, s); break;
-	default: launch_fwd_t<4, false, DM>(a, s); break;
+	case 0: launch_fwd_t<0, false, DM, MED>(a, s); break;
+	case 1: launch_fwd_t<1, false, DM, MED>(a, s); break;
+	case 2: launch_fwd_t<2, false, DM, MED>(a, s); break;
+	default: launch_fwd_t<4, false, DM, MED>(a, s); break;
 	}
 }
 
 
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.tgt_color && (a.tgt_depth || a.tgt_mask)) launch_fwd_dm<true>(a, s);
-	else launch_fwd_dm<false>(a, s);
+	const bool dm = a.tgt_color && (a.tgt_depth || a.tgt_mask);
+	if (a.median_id) {
+		if (dm) launch_fwd_dm<true, true>(a, s);
+		else launch_fwd_dm<false, true>(a, s);
+	} else if (dm) launch_fwd_dm<true, false>(a, s);
+	else launch_fwd_dm<false, false>(a, s);
 }
 
 }  // namespace mgs

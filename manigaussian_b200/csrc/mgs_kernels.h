@@ -197,6 +197,12 @@ struct BlendArgs {
 	float* cot_alpha_mask;
 	float* dm_acc;
 	const float* dm_scale;
+	// median depth (forward, nullable; the launcher picks the MED instantiation when median_id is set): median_id [H,W]
+	// receives the id of the pixel's median contributor, the last one whose incoming T > 0.5 (-1 without a contributor), and
+	// out_median_depth [H,W] (nullable) its view-space depth rgbd[id].w (0 without).  Behind every other member, so that the
+	// blend kernels without it read their parameters at the same offsets as before.
+	int* median_id;
+	float* out_median_depth;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
 	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams
@@ -286,5 +292,7 @@ int blend_supported(int F);
 int blend_groups(int F);  // channel groups of 32 (BlendArgs::groups)
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s);
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
+// the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0
+void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s);
 
 }  // namespace mgs

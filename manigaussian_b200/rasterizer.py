@@ -10,7 +10,8 @@ include/mgs_rasterizer.h.
 
 Supersets of the reference: the feature width F is read from the tensor at run time (0..512) instead of being
 compiled in (config.h:16; widths above 32 blend in groups of 32 channels), `return_depth=True` adds a view-space
-depth plane, and `return_alpha=True` adds the accumulated-opacity plane 1 - final_T.
+depth plane, and `return_alpha=True` adds the accumulated-opacity plane 1 - final_T.  `return_median_depth=True` adds the
+median-depth plane and each pixel's surface Gaussian.
 """
 from typing import NamedTuple
 
@@ -261,7 +262,7 @@ def cpu_deep_copy_tuple(input_tuple):
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False):
+                        cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False):
     s = raster_settings
     # camera tensors that require grad become explicit inputs of the node, which then returns their gradients; a field of
     # view held as CUDA tensors (learnable intrinsics) joins them as two more inputs, tanfovx and tanfovy
@@ -271,13 +272,17 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_p
     if not any(torch.is_tensor(t) and t.requires_grad for t in cam):
         cam = ()
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha, *cam)
+                                     rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha,
+                                     bool(return_median_depth), *cam)
+
+
+_CAM_FIRST = 13  # position of the first camera input of _RasterizeGaussians
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, *cam):
+                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median=False, *cam):
         s = raster_settings
         args = (s.bg, means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations, s.scale_modifier,
                 cov3Ds_precomp, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.image_height, s.image_width, sh,
@@ -290,23 +295,26 @@ class _RasterizeGaussians(torch.autograd.Function):
         # the device field of view, when the settings carry one (read by the kernels in place of host floats)
         tf = _fov_column([s], means3D.device) if (views_path and _is_device_fov(s)) else None
         ctx.tan_fov = tf
-        alpha = None
-        if (return_alpha or aa or ctx.camera) and views_path:
-            # the alpha plane, the anti-aliased projection and the camera gradients exist on the multi-view entry points only:
-            # debug renders take them too, with the snapshot dump
+        alpha = med_depth = med_id = None
+        if (return_alpha or return_median or aa or ctx.camera) and views_path:
+            # the alpha plane, the median planes, the anti-aliased projection and the camera gradients exist on the multi-view
+            # entry points only: debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
                                                     rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
                                                     return_depth=return_depth, debug=s.debug, return_alpha=return_alpha,
-                                                    antialiasing=aa, tan_fov=tf)
+                                                    antialiasing=aa, tan_fov=tf, return_median=return_median)
             except Exception as ex:
                 if s.debug:
                     torch.save(cpu_args, "snapshot_fw.dump")
                     print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
                 raise ex
             out = outs[0]
-            alpha = out[-1] if return_alpha else None
+            planes = 7 + bool(return_depth)
+            alpha = out[planes] if return_alpha else None
+            if return_median:
+                med_depth, med_id = out[-2], out[-1]
             ctx.async_view = (int(out[0]), streams)  # as below: never the outputs themselves
         elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
@@ -329,27 +337,39 @@ class _RasterizeGaussians(torch.autograd.Function):
             ctx.async_view = (int(out[0]), streams)
         else:
             out = rasterize_gaussians_raw(*args, return_depth=return_depth)
-            if return_alpha:  # no Gaussians: nothing covers any pixel
-                alpha = torch.zeros((int(s.image_height), int(s.image_width)), dtype=torch.float32, device=out[1].device)
+            # no Gaussians: nothing covers any pixel
+            hw, odev = (int(s.image_height), int(s.image_width)), out[1].device
+            if return_alpha:
+                alpha = torch.zeros(hw, dtype=torch.float32, device=odev)
+            if return_median:
+                med_depth, med_id = torch.zeros(hw, dtype=torch.float32, device=odev), torch.full(hw, -1, dtype=torch.int32, device=odev)
         num_rendered, color, language_feature, radii, geomBuffer, binningBuffer, imgBuffer = out[:7]
         depth = out[7] if return_depth else None
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.return_depth = return_depth
         ctx.return_alpha = return_alpha
+        ctx.return_median = return_median
+        # the id plane is an output: it reaches the backward through save_for_backward, never through ctx (reference cycle)
         ctx.save_for_backward(colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii,
-                              sh, geomBuffer, binningBuffer, imgBuffer)
-        ctx.mark_non_differentiable(radii)
-        return (color, language_feature, radii) + ((depth,) if return_depth else ()) + ((alpha,) if return_alpha else ())
+                              sh, geomBuffer, binningBuffer, imgBuffer, med_id if return_median else None)
+        if return_median:
+            ctx.mark_non_differentiable(radii, med_id)
+        else:
+            ctx.mark_non_differentiable(radii)
+        return (color, language_feature, radii) + ((depth,) if return_depth else ()) + ((alpha,) if return_alpha else ()) + \
+            ((med_depth, med_id) if return_median else ())
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_language_feature, _radii=None, *grad_planes):
-        # grad_planes: the depth gradient when return_depth, then the alpha gradient when return_alpha
+        # grad_planes: the depth gradient when return_depth, then the alpha gradient when return_alpha, then the median-depth
+        # gradient and the (absent) id gradient when return_median
         grad_out_depth = grad_planes[0] if ctx.return_depth else None
-        grad_out_alpha = grad_planes[-1] if ctx.return_alpha else None
+        grad_out_alpha = grad_planes[int(ctx.return_depth)] if ctx.return_alpha else None
+        grad_out_median = grad_planes[-2] if ctx.return_median else None
         s = ctx.raster_settings
         (colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-         binningBuffer, imgBuffer) = ctx.saved_tensors
+         binningBuffer, imgBuffer, med_id) = ctx.saved_tensors
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, s.image_height, s.image_width), dtype=torch.float32, device=means3D.device)
         if s.include_feature and grad_out_language_feature is None:
@@ -363,14 +383,17 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.async_view is not None:
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
-            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.antialiasing or ctx.camera)) else None
+            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.return_median or ctx.antialiasing or
+                                                                  ctx.camera)) else None
             try:
                 grads = rasterize_views_backward_raw(
                     [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
                     colors_precomp, language_feature_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree,
                     s.include_feature, grads_depth=[depth_grad] if depth_grad is not None else None, debug=s.debug,
                     grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing,
-                    camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov)
+                    camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov,
+                    grads_median=[grad_out_median] if grad_out_median is not None else None,
+                    median_ids=[med_id] if grad_out_median is not None else None)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -399,7 +422,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                 dtf = cg[3] if len(cg) > 3 else z(2)
                 gs += [dtf[0, 0], dtf[0, 1]]
                 ts += [s.tanfovx, s.tanfovy]
-            grad_cam = tuple(g.reshape(t.shape) if ctx.needs_input_grad[12 + i] else None for i, (g, t) in enumerate(zip(gs, ts)))
+            grad_cam = tuple(g.reshape(t.shape) if ctx.needs_input_grad[_CAM_FIRST + i] else None for i, (g, t) in enumerate(zip(gs, ts)))
 
         def _or_none(g, inp):
             return g if (inp is not None and inp.numel() != 0) else None
@@ -407,7 +430,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, _or_none(grad_sh, sh), _or_none(grad_colors_precomp, colors_precomp),
                 _or_none(grad_language_feature_precomp, language_feature_precomp) if s.include_feature else None,
                 grad_opacities, _or_none(grad_scales, scales), _or_none(grad_rotations, rotations),
-                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None) + grad_cam
+                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None, None) + grad_cam
 
 
 class _Settings(NamedTuple):
@@ -453,13 +476,16 @@ class GaussianRasterizationSettings(_Settings):
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, return_depth=False, return_alpha=False):
+    def __init__(self, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False):
         """return_depth / return_alpha: forward() also returns the depth plane [H,W] and / or the alpha plane [H,W]
-        (accumulated opacity 1 - final_T), in that order after radii."""
+        (accumulated opacity 1 - final_T), in that order after radii.  return_median_depth: it then also returns the
+        median-depth plane [H,W] (differentiable) and the median contributor's Gaussian id [H,W] int32 (-1 where nothing
+        covers the pixel; include/mgs_rasterizer.h, mgs_view_median), behind the other planes."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_depth = return_depth
         self.return_alpha = return_alpha
+        self.return_median_depth = return_median_depth
 
     def markVisible(self, positions):
         # Mark visible points (based on frustum culling for camera) with a boolean
@@ -482,7 +508,8 @@ class GaussianRasterizer(nn.Module):
         rotations = empty if rotations is None else rotations
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, language_feature_precomp, opacities, scales,
-                                   rotations, cov3D_precomp, self.raster_settings, self.return_depth, self.return_alpha)
+                                   rotations, cov3D_precomp, self.raster_settings, self.return_depth, self.return_alpha,
+                                   self.return_median_depth)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -612,7 +639,8 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
-                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None):
+                        loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
+                        return_median=False):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -631,7 +659,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     (C ABI mgs_view_ssim) leaves {sum |x - g|, sum S} in loss_acc[:, :2] and the partials of S in ssim_terms.  `tan_fov`
     [V,2] (device): every view's {tan_fovx, tan_fovy}, read by the kernels in place of the settings' host floats (C ABI
     mgs_forward_views_intr); views whose tanfovx / tanfovy are CUDA tensors use it without being asked.  Pass the same to
-    the backward."""
+    the backward.  `return_median` appends the median-depth plane [H,W] and the median contributor's Gaussian id [H,W] int32
+    (-1 where nothing covers the pixel) to every ViewOut, behind the other planes (C ABI mgs_view_median); with `out_buffers`
+    they go to out_buffers[4] and out_buffers[5] ([V,H,W] each) when those are given."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -662,6 +692,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
         sarr = (_b.ViewSsim * V)() if ssim is not None else None
+        marr = (_b.ViewMedian * V)() if return_median else None
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
@@ -671,7 +702,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _fill_ssim(sarr[v], ssim, v)
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
-                                 aarr[v] if return_alpha else None)
+                                 aarr[v] if return_alpha else None, marr[v] if return_median else None)
             arr[v].status = status.data_ptr() + 8 * v
             arr[v].stream = streams[v].cuda_stream
             keep.append(k)
@@ -679,8 +710,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
-        if tf is not None:
-            keep.append(tf)
+        keep.append(tf)
+        if marr is not None:
+            _b.check(L.mgs_forward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
+                     "mgs_forward_views_median")
+        elif tf is not None:
             _b.check(L.mgs_forward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None), *rest),
                      "mgs_forward_views_intr")
         elif sarr is not None:
@@ -721,10 +756,10 @@ def _fill_ssim(ws, ssim, v, w=None, scale=None):
         ws.cot_scale = scale.data_ptr() + 8 * v
 
 
-def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None):
+def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None):
     """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream) and, when
-    `wa` (its mgs_view_alpha) is given, its alpha plane.  Returns the ViewOut and the tensors that must stay alive until the
-    call is enqueued."""
+    `wa` (its mgs_view_alpha) is given, its alpha plane, and when `wm` (its mgs_view_median) is given, its median planes.
+    Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
     gbytes, ibytes, _ = _state_sizes(L, P, W, H)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
@@ -757,6 +792,12 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
             w.target_feature, w.cot_feature = _ptr(t_emb[v]), _ptr(c_emb[v])
     ret = (cap, out_color, out_feature, radii, geom, binb, img) + ((out_depth,) if return_depth else ())
     ret += (out_alpha,) if wa is not None else ()
+    if wm is not None:
+        ob = out_buffers if (out_buffers is not None and len(out_buffers) > 5) else (None,) * 6
+        med_depth = ob[4][v] if ob[4] is not None else torch.empty((H, W), dtype=torch.float32, device=dev)
+        med_id = ob[5][v] if ob[5] is not None else torch.empty((H, W), dtype=torch.int32, device=dev)
+        wm.out_median_depth, wm.median_id = _ptr(med_depth), _ptr(med_id)
+        ret += (med_depth, med_id)
     return ViewOut(ret), (bg, vm, pm, cp)
 
 
@@ -817,7 +858,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
-                                 ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None):
+                                 ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -837,7 +878,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     campos (C ABI mgs_backward_views_cam; written, or added to with accumulate=True); the return value then gains that tuple
     (allocated for True) as a 10th element.  `tan_fov`: as given to the forward (views with CUDA-tensor tanfov* imply it);
     with it the call is mgs_backward_views_intr, and `camera_grads` gains a 4th entry, dL_dtan_fov [V,2] (the gradient with
-    respect to each view's {tan_fovx, tan_fovy}; allocated for True, or named in a 4-tuple)."""
+    respect to each view's {tan_fovx, tan_fovy}; allocated for True, or named in a 4-tuple).  `grads_median` (per view [H,W]
+    or None): cotangents of the median-depth planes of a `return_median` forward, with `median_ids` (per view [H,W] int32)
+    the id planes that forward returned (C ABI mgs_backward_views_median)."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -878,6 +921,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         sarr = (_b.ViewSsim * V)() if ssim is not None else None
         sscale = _prep(ssim_scale, dev)
         keep = [dscale, sscale]
+        marr = _median_array(grads_median, median_ids, V, dev, keep)
         for v, s in enumerate(views):
             w = arr[v]
             if darr is not None:
@@ -905,7 +949,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if iarr is not None:
+            if marr is not None:
+                _b.check(L.mgs_backward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, *rest),
+                         "mgs_backward_views_median")
+            elif iarr is not None:
                 _b.check(L.mgs_backward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, *rest),
                          "mgs_backward_views_intr")
             elif carr is not None:
@@ -924,6 +971,24 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 after_blend()
     grads = (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
     return grads + (cam,) if cam is not None else grads
+
+
+def _median_array(grads, ids, V, dev, keep):
+    """ViewMedian array of V views' median-depth cotangents and id planes (per view [H,W] each, or None), or None without
+    cotangents.  The tensors that must stay alive until the call is enqueued go to `keep`."""
+    if grads is None:
+        return None
+    if ids is None:
+        raise ValueError("median-depth cotangents need the forward's median ids")
+    marr = (_b.ViewMedian * V)()
+    for v in range(V):
+        if grads[v] is None:
+            continue
+        g = _prep(grads[v], dev)
+        i = ids[v].to(device=dev, dtype=torch.int32).contiguous()
+        marr[v].median_id, marr[v].dL_dpix_median_depth = _ptr(i), _ptr(g)
+        keep += [g, i]
+    return marr
 
 
 def _camera_grads(L, camera_grads, Ps, dev, keep, intr=False):
@@ -1005,7 +1070,7 @@ def _prep_clouds(clouds, dev, include_feature):
 
 
 def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False,
-                         antialiasing=False):
+                         antialiasing=False, return_median=False):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
@@ -1016,7 +1081,9 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
     Capacity history is kept per (device, P, W, H, cloud slot, view slot).  `antialiasing`: the anti-aliased projection for
     every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
-    (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr)."""
+    (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr).
+    `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
+    mgs_forward_clouds_median)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -1047,6 +1114,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
         sarr = (_b.ViewSsim * V)() if any(c.get("ssim") is not None for c in clouds) else None
+        marr = (_b.ViewMedian * V)() if return_median else None
         status = _status_slots(V)
         keep, outs = [], []
         for b, (c, d) in enumerate(zip(clouds, pc)):
@@ -1065,7 +1133,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 if c.get("ssim") is not None:
                     _fill_ssim(sarr[g], c["ssim"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
-                                      c.get("loss_heads"), aarr[g] if return_alpha else None)
+                                      c.get("loss_heads"), aarr[g] if return_alpha else None, marr[g] if return_median else None)
                 arr[g].status = status.data_ptr() + 8 * g
                 arr[g].stream = streams[g].cuda_stream
                 keep.append(kp)
@@ -1073,8 +1141,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
             outs.append(cloud_outs)
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
-        if tf is not None:
-            keep.append(tf)
+        keep.append(tf)
+        if marr is not None:
+            _b.check(L.mgs_forward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
+                     "mgs_forward_clouds_median")
+        elif tf is not None:
             _b.check(L.mgs_forward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None),
                                                *rest), "mgs_forward_clouds_intr")
         elif sarr is not None:
@@ -1118,7 +1190,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     the forward was given (C ABI mgs_backward_clouds_aa).  `camera_grads=True`: every cloud's dict also holds the gradients
     with respect to its views' viewmatrix, projmatrix and campos, "dL_dviewmatrix" [V_b,16], "dL_dprojmatrix" [V_b,16] and
     "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam).  Clouds with a device field of view (see rasterize_clouds_raw)
-    make the call mgs_backward_clouds_intr, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict."""
+    make the call mgs_backward_clouds_intr, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict.  A cloud's
+    "grad_median" [V_b,H,W] is the cotangent of a `return_median` forward's median-depth planes, with "median_id" [V_b,H,W]
+    int32 the id planes that forward returned (C ABI mgs_backward_clouds_median)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1136,6 +1210,11 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
         sarr = (_b.ViewSsim * V)() if any(c.get("ssim") is not None for c in clouds) else None
         keep = []
+        marr = None
+        if any(c.get("grad_median") is not None for c in clouds):
+            gm = [c["grad_median"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
+            ids = [c["median_id"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
+            marr = _median_array(gm, ids, V, dev, keep)
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
             has_sr = _nonempty(d["scales"])
@@ -1188,7 +1267,11 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if tf is not None:
+        if marr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
+                                                  *rest), "mgs_backward_clouds_median")
+        elif tf is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None)
             _b.check(L.mgs_backward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, *rest),
                      "mgs_backward_clouds_intr")
