@@ -23,6 +23,7 @@
  *  - an optional depth plane (out_depth / dL_dpix_depth) renders view-space z as one more blended channel;
  *  - an optional alpha plane (mgs_view_alpha, multi-view and multi-cloud calls) returns the accumulated opacity 1 - final_T;
  *  - an optional median-depth plane and per-pixel surface Gaussian id (mgs_view_median, the same calls);
+ *  - an optional surface-normal plane (mgs_view_normal, the same calls);
  *  - work is enqueued on `stream` (the reference uses the legacy default stream);
  *  - outputs are fully overwritten: callers need not zero-initialise them.
  *
@@ -807,6 +808,92 @@ int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_o
 	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
 	float scale_modifier, int accumulate, int debug, void* join_stream);
+
+/*
+ * Surface normals (no reference counterpart; the rend_normal plane of 2DGS / RaDe-GS / GaussianShader).  The _normal calls are
+ * the _median calls with one more argument, `normal`: one mgs_view_normal per view (V entries, or view_offsets[B] for clouds),
+ * or NULL; the _median calls are these with normal == NULL.
+ *
+ * Definition.  Per Gaussian i and view v, from scales [P,3] and rotations [P,4] (r, x, y, z):
+ *   - k = argmin_j scales[i][j], the lowest index on ties (scale_modifier does not change it);
+ *   - q^ = q / |q| (normalised here: a normal is a unit vector even when the caller's quaternion is not), and
+ *     a = R(q^) e_k, the WORLD-space direction of the axis that scale k stretches (Sigma a = s_k^2 a for the covariance the
+ *     projection builds), R(q^) the rotation matrix of q^:
+ *       e_0 -> (1 - 2(y^2 + z^2), 2(xy + rz), 2(xz - ry)),  e_1 -> (2(xy - rz), 1 - 2(x^2 + z^2), 2(yz + rx)),
+ *       e_2 -> (2(xz + ry), 2(yz - rx), 1 - 2(x^2 + y^2));
+ *   - s = +1 if a . (cam_pos_v - mean_i) >= 0, else -1, and n_{i,v} = s a: the normal faces the camera.
+ * Plane: out_normal[c][p] = sum_k w_{p,k} n_{k,v}[c], c < 3, with the blend weights w = alpha T and the contributors of the
+ * colour image.  No background term and no clamp, like depth and features.  The plane is NOT normalised: its length is about
+ * alpha where one surface dominates; divide by the alpha plane or normalise.
+ * Backward, given dL_dpix_normal [3,H,W]: the normal channels enter dL/dalpha (and through it opacity, conic, means2D) like
+ * any other channel; dL/dn_{i,v} = sum_p w_{p,i} dL_dpix_normal[:, p]; dL/da_i = sum_v s_{i,v} dL/dn_{i,v} is chained through
+ * R(q^) e_k and the normalisation ((I - q^ q^T) / |q|) and ADDED to dL_drot.  k and s are piecewise constant: scales, means3D
+ * and the camera receive nothing from them, and as the plane is in world space the view matrix does not enter it.
+ * State: a view with a normal plane needs a geometry_state of mgs_geometry_state_bytes_normal(P) bytes, and in the backward
+ * a blend_scratch of mgs_backward_scratch_bytes_normal(P) bytes (the per-Gaussian quads and their gradients live behind the
+ * other arrays; "geometry" / "nrm" of mgs_state_array).  Per view each pointer may be NULL.  MGS_ERR_INVALID_ARG, before
+ * anything is enqueued: a plane or cotangent with cov3D_precomp (there is no rotation to take a normal from), without cam_pos,
+ * or beside the depth / mask heads (mgs_view_depth_mask targets); a dL_dpix_normal without out_normal, the plane that view's
+ * forward wrote (the backward reads the quads that forward stored).
+ */
+typedef struct mgs_view_normal {
+	float* out_normal;              /* forward output [3,H,W], or NULL; names the forward's plane in the backward */
+	const float* dL_dpix_normal;    /* backward input [3,H,W], or NULL */
+} mgs_view_normal;
+
+size_t mgs_geometry_state_bytes_normal(int P);
+size_t mgs_backward_scratch_bytes_normal(int P);
+
+int mgs_forward_views_normal(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views_normal(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, int D, int M, int F,
+	float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */

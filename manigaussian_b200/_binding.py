@@ -60,6 +60,11 @@ class ViewMedian(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("out_median_depth", "median_id", "dL_dpix_median_depth")]
 
 
+class ViewNormal(C.Structure):
+    """mirror of `mgs_view_normal` (include/mgs_rasterizer.h): the optional surface-normal plane of one view"""
+    _fields_ = [(n, C.c_void_p) for n in ("out_normal", "dL_dpix_normal")]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -80,7 +85,8 @@ def lib():
     L = C.CDLL(path)
     L.mgs_abi_version.restype = C.c_int
     L.mgs_last_error.restype = C.c_char_p
-    for name in ("mgs_geometry_state_bytes", "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_camera_grad_scratch_bytes"):
+    for name in ("mgs_geometry_state_bytes", "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_camera_grad_scratch_bytes",
+                 "mgs_geometry_state_bytes_normal", "mgs_backward_scratch_bytes_normal"):
         getattr(L, name).restype = C.c_size_t
         getattr(L, name).argtypes = [C.c_int]
     L.mgs_image_state_bytes.restype = C.c_size_t
@@ -158,6 +164,12 @@ def lib():
         getattr(L, med).restype = C.c_int
         getattr(L, med).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
             ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian)] + at[k:]
+        # ... and the normal plane (one ViewNormal per view, or NULL) after the median planes
+        nrm = name.replace("_views", "_views_normal").replace("_clouds", "_clouds_normal")
+        getattr(L, nrm).restype = C.c_int
+        getattr(L, nrm).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
+            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
+            [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal)] + at[k:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -201,6 +213,8 @@ EXPORTED_SYMBOLS = (
     "mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam",
     "mgs_forward_views_intr", "mgs_backward_views_intr", "mgs_forward_clouds_intr", "mgs_backward_clouds_intr",
     "mgs_forward_views_median", "mgs_backward_views_median", "mgs_forward_clouds_median", "mgs_backward_clouds_median",
+    "mgs_forward_views_normal", "mgs_backward_views_normal", "mgs_forward_clouds_normal", "mgs_backward_clouds_normal",
+    "mgs_geometry_state_bytes_normal", "mgs_backward_scratch_bytes_normal",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

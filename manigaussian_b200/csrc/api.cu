@@ -234,6 +234,12 @@ size_t mgs_image_state_bytes(int width, int height)
 size_t mgs_binning_state_bytes(int R) { return required([&](char*& p) { BinState::carve(p, (size_t)R); }); }
 size_t mgs_backward_scratch_bytes(int P) { return (size_t)P * GB_STRIDE * sizeof(float) + 128; }
 size_t mgs_camera_grad_scratch_bytes(int P) { return P > 0 ? camera_rows_bytes(P) : 0; }
+// with the normal plane: the per-Gaussian quads nrm [P] behind the geometry state, the gradients gn [P,4] behind the scratch
+size_t mgs_geometry_state_bytes_normal(int P)
+{
+	return required([&](char*& p) { GeomState::carve(p, (size_t)P); float4* nrm; obtain(p, nrm, (size_t)P); });
+}
+size_t mgs_backward_scratch_bytes_normal(int P) { return mgs_backward_scratch_bytes(P) + (size_t)P * 4 * sizeof(float) + 128; }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -332,6 +338,10 @@ struct ViewState {
 	size_t T;
 	GeomState geom; ImageState img; BinState bin;
 	float* gb;  // blend-stage gradients of the backward, [P, GB_STRIDE] in blend_scratch
+	// normal plane only (buffers sized by the _normal queries): the per-Gaussian quads behind the geometry state, and the
+	// blend-stage normal gradients [P,4] behind gb
+	float4* nrm;
+	float* gn;
 };
 static ViewState carve_view(const mgs_view& w, int P)
 {
@@ -344,6 +354,8 @@ static ViewState carve_view(const mgs_view& w, int P)
 	s.img = ImageState::carve(i, (size_t)w.width * w.height, s.T);
 	s.bin = BinState::carve(b, (size_t)w.binning_capacity);
 	obtain(sc, s.gb, (size_t)P * GB_STRIDE);
+	obtain(g, s.nrm, (size_t)P);
+	obtain(sc, s.gn, (size_t)P * 4);
 	return s;
 }
 
@@ -471,14 +483,42 @@ static int check_median(const mgs_view_median* m)
 	return 0;
 }
 
+// the normal plane of one view (n nullable): it needs scales and rotations to take the axis from, the camera centre to face,
+// and has no instantiation beside the depth / mask heads; a cotangent needs the plane its forward wrote
+static int check_normal(const mgs_view& w, const mgs_view_normal* n, const float* scales, const float* rotations,
+	const float* cov3D_precomp, const mgs_view_depth_mask* dm)
+{
+	if (!n || (!n->out_normal && !n->dL_dpix_normal)) return 0;
+	if (cov3D_precomp || !scales || !rotations)
+		return fail(MGS_ERR_INVALID_ARG, "view: the normal plane needs scales and rotations (a precomputed covariance has no axis to take)");
+	if (!n->out_normal) return fail(MGS_ERR_INVALID_ARG, "view: dL_dpix_normal needs out_normal, the plane its forward wrote");
+	if (!w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: the normal plane needs cam_pos");
+	if (dm && (dm->target_depth || dm->target_mask))
+		return fail(MGS_ERR_INVALID_ARG, "view: the normal plane cannot be combined with the depth / mask heads");
+	return 0;
+}
+
+// the view's per-Gaussian normal quads, behind its projection on its stream (nm nullable)
+static int enqueue_normals_fwd(const Cloud& c, const mgs_view& w, const mgs_view_normal* nm, int debug)
+{
+	if (!nm || !nm->out_normal) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+	launch_normals_fwd(c.P, c.means3D, c.scales, c.rotations, w.cam_pos, carve_view(w, c.P).nrm, st);
+	MGS_STAGE("normals_fwd");
+	return 0;
+}
+
 // forward blend, with the fused loss heads when the view has a target; out_alpha (nullable) receives 1 - final_T; dm
-// (nullable): the view's depth / mask heads; med (nullable): its median plane (checked by check_median)
+// (nullable): the view's depth / mask heads; med (nullable): its median plane (checked by check_median); nm (nullable): its
+// normal plane (checked by check_normal)
 static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha, const mgs_view_depth_mask* dm,
-	const mgs_view_median* med, int debug)
+	const mgs_view_median* med, const mgs_view_normal* nm, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = (c.F > 0 && c.feature && w.out_feature) ? c.F : 0;
-	BlendArgs ba = blend_args(carve_view(w, c.P), w, F, c.feature);
+	const ViewState vs = carve_view(w, c.P);
+	BlendArgs ba = blend_args(vs, w, F, c.feature);
+	if (nm && nm->out_normal) { ba.nrm = vs.nrm; ba.out_normal = nm->out_normal; }
 	ba.want_depth = w.out_depth != nullptr;
 	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth; ba.out_alpha = out_alpha;
 	if (med && med->median_id) { ba.median_id = med->median_id; ba.out_median_depth = med->out_median_depth; }
@@ -548,9 +588,10 @@ static int enqueue_ssim_bwd(mgs_view& w, const mgs_view_ssim* s, int debug)
 // reductions straight into dL_dfeature.  dL_dfeature NULL with c.F > 0: the feature cotangents still reach the mean, conic
 // and opacity gradients; only the feature rows are not reduced.  dL_dalpha (nullable): cotangent of the alpha plane; dm
 // (nullable): the view's depth / mask heads, whose cotangent planes the walker's prologue folds in; med (nullable): its
-// median plane, whose cotangent goes to the median contributors' depth slots.
+// median plane, whose cotangent goes to the median contributors' depth slots; nm (nullable): its normal plane, whose
+// cotangent is blended back into the view's gn.
 static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeature, const float* dL_dalpha, const mgs_view_depth_mask* dm,
-	const mgs_view_median* med, int debug)
+	const mgs_view_median* med, const mgs_view_normal* nm, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const int F = c.F;
@@ -564,6 +605,10 @@ static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeatu
 	ba.dL_dcolor = w.dL_dpix; ba.dL_dfeature = F > 0 ? w.dL_dpix_F : nullptr; ba.dL_ddepth = w.dL_dpix_depth; ba.dL_dalpha = dL_dalpha;
 	ba.gb = s.gb; ba.dL_dfeat = F > 0 ? dL_dfeature : nullptr;
 	ba.cot_scale = w.cot_scale;
+	if (nm && nm->dL_dpix_normal) {
+		MGS_CUDA(cudaMemsetAsync(s.gn, 0, (size_t)c.P * 4 * sizeof(float), st));
+		ba.nrm = s.nrm; ba.dL_dnormal = nm->dL_dpix_normal; ba.gn = s.gn;
+	}
 	depth_mask_args(ba, dm);
 	ba.want_depth = w.dL_dpix_depth != nullptr || ba.tgt_depth != nullptr;  // the depth head's cotangent reaches the view-space z
 	if (w.binning_capacity > 0) {
@@ -611,12 +656,31 @@ static void camera_view(const mgs_view_camera_grad* cam, const mgs_view_intrinsi
 	cr.view[cr.V++] = CamReduceView{ e.scratch, (P + 127) / 128, e.dL_dviewmatrix, e.dL_dprojmatrix, e.dL_dcampos, ki.rows, dtf };
 }
 
+// the normal planes' share of dL_drot for views [v0, v0 + n) of one cloud (n <= MAX_BWD_VIEWS), behind the per-Gaussian
+// launch that wrote dL_drot, on the same stream: the views with a normal cotangent, in view order
+static int enqueue_normals_bwd(const Cloud& c, const mgs_view* views, const mgs_view_normal* nm, int v0, int n, float* dL_drot, int debug,
+	cudaStream_t st)
+{
+	if (!nm || !dL_drot) return 0;
+	NormalsBwdArgs na{};
+	na.P = c.P; na.means3D = c.means3D; na.scales = c.scales; na.rotations = c.rotations; na.dL_drot = dL_drot;
+	for (int v = v0; v < v0 + n; v++) {
+		if (!nm[v].dL_dpix_normal) continue;
+		na.gn[na.V] = carve_view(views[v], c.P).gn;
+		na.cam_pos[na.V++] = views[v].cam_pos;
+	}
+	if (na.V == 0) return 0;
+	launch_normals_bwd(na, st);
+	MGS_STAGE("normals_bwd");
+	return 0;
+}
+
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
 	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
-	const Cloud& c, float* dL_dmean3D,
+	const mgs_view_normal* nm, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -630,7 +694,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
 			if (rc == 0)
 				rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr,
-					med ? med + v : nullptr, debug);
+					med ? med + v : nullptr, nm ? nm + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -667,6 +731,8 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
+		const int rc = enqueue_normals_bwd(c, views, nm, v0, pb.V, dL_drot, debug, st);
+		if (rc < 0) return rc;
 	}
 	return 0;
 }
@@ -780,7 +846,7 @@ int mgs_forward(
 	w.binning_capacity = num_rendered;
 	rc = enqueue_binning(c, w, true, debug);
 	if (rc < 0) return rc;
-	rc = enqueue_blend_fwd(c, w, nullptr, nullptr, nullptr, debug);
+	rc = enqueue_blend_fwd(c, w, nullptr, nullptr, nullptr, nullptr, debug);
 	return rc < 0 ? rc : num_rendered;
 }
 
@@ -828,7 +894,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -908,6 +974,18 @@ int mgs_forward_views_median(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_normal(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, nullptr, P, D, M, F, means3D, shs,
+		colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_normal(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -921,6 +999,7 @@ int mgs_forward_views_median(
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
 		if (rc == 0) rc = check_median(median ? median + v : nullptr);
+		if (rc == 0) rc = check_normal(views[v], normal ? normal + v : nullptr, scales, rotations, cov3D_precomp, depth_mask ? depth_mask + v : nullptr);
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
@@ -945,7 +1024,8 @@ int mgs_forward_views_median(
 			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
-					median ? median + v : nullptr, debug);
+					median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
+			if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
 			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
@@ -1056,6 +1136,21 @@ int mgs_backward_views_median(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_normal(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, nullptr, P, D, M, F, means3D,
+		shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
+		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_normal(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -1068,12 +1163,13 @@ int mgs_backward_views_median(
 		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 		if (rc == 0) rc = check_median(median ? median + v : nullptr);
+		if (rc == 0) rc = check_normal(views[v], normal ? normal + v : nullptr, scales, rotations, cov3D_precomp, depth_mask ? depth_mask + v : nullptr);
 		if (rc < 0) return rc;
 	}
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1127,6 +1223,15 @@ int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_of
 	const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F, float scale_modifier, int prefiltered,
 	int debug, void* join_stream)
 {
+	return mgs_forward_clouds_normal(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, nullptr, D, M,
+		F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, int D, int M, int F,
+	float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -1143,6 +1248,9 @@ int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_of
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
 			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
 			if (rc == 0) rc = check_median(median ? median + v : nullptr);
+			if (rc == 0)
+				rc = check_normal(views[v], normal ? normal + v : nullptr, k.scales, k.rotations, k.cov3D_precomp,
+					depth_mask ? depth_mask + v : nullptr);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1158,7 +1266,8 @@ int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_of
 				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
-						median ? median + v : nullptr, debug);
+						median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
+				if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
 				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
@@ -1226,6 +1335,15 @@ int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_o
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
 	float scale_modifier, int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_normal(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, nullptr,
+		D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -1241,6 +1359,9 @@ int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_o
 			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
 			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
 			if (rc == 0) rc = check_median(median ? median + v : nullptr);
+			if (rc == 0)
+				rc = check_normal(views[v], normal ? normal + v : nullptr, k.scales, k.rotations, k.cov3D_precomp,
+					depth_mask ? depth_mask + v : nullptr);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1261,7 +1382,7 @@ int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_o
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
 			if (rc == 0)
 				rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
-					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, debug);
+					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1311,7 +1432,19 @@ int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_o
 			nv += n;
 		}
 	}
-	return flush();
+	rc = flush();
+	if (rc < 0) return rc;
+	// the normal planes' share of every cloud's dL_drot, behind the launches that wrote it: one launch per cloud and
+	// MAX_BWD_VIEWS of its views
+	for (int b = 0; b < B && normal; b++) {
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			rc = enqueue_normals_bwd(c, views, normal, v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS), clouds[b].dL_drot,
+				debug, st);
+			if (rc < 0) return rc;
+		}
+	}
+	return 0;
 }
 
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,
@@ -1477,6 +1610,7 @@ int mgs_state_array(const char* which_state, const char* name, char* state, int 
 		else if (n == "tiles_touched") p = g.tiles_touched; else if (n == "point_offsets") p = g.point_offsets;
 		else if (n == "depth_order") p = g.order;
 		else if (n == "clamped") p = g.clamped; else if (n == "extent") p = g.extent;
+		else if (n == "nrm") { float4* q; obtain(state, q, (size_t)a0); p = q; }  // a state sized by mgs_geometry_state_bytes_normal
 	} else if (w == "binning") {
 		BinState b = BinState::carve(state, (size_t)a0);
 		if (n == "point_list") p = b.point_list; else if (n == "tile_ids") p = b.tile_keys;

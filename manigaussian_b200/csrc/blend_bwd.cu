@@ -106,8 +106,10 @@ __device__ __forceinline__ void depth_mask_cotangents(const BlendArgs& a, size_t
 }
 
 // F <= 32 (one channel group); channel groups run blend_bwd_groups_kernel below.  DM: the depth / mask heads
-// (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.
-template <int NFT, bool VEC, bool DM>
+// (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.  NRM: the normal plane
+// (BlendArgs::nrm / dL_dnormal / gn): the quad {nx, ny, nz, 0} and its cotangent fill columns 4..7 of the {r,g,b,depth} tile,
+// so GEMM 1 and GEMM 2 carry them as issued, and the flush adds dL/dn into gn; likewise.
+template <int NFT, bool VEC, bool DM, bool NRM>
 __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendArgs a)
 {
 	constexpr int NT = NFT + 1;          // channel tiles of 8: NFT feature tiles + {r,g,b,depth, 4 x zero}
@@ -174,7 +176,11 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
 #pragma unroll
-		for (int c = 0; c < 4; c++) { grow[2 * (RGBD + c)] = g4[c]; grow[2 * (RGBD + 4 + c)] = 0.f; }
+		for (int c = 0; c < 4; c++) {
+			grow[2 * (RGBD + c)] = g4[c];
+			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
+			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside) ? a.dL_dnormal[c * HW + pix] : 0.f;
+		}
 		if (NFT > 0) {
 #pragma unroll
 			for (int i = 0; i < 8 * NFT; i++)
@@ -378,10 +384,12 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					}
 				}
 				if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
+				if (NRM && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
 			} else if (lane < cnt) {
 				const uint32_t id = bwd_row_id(__float_as_uint(s_q[2 * lane + 1].w));
 				float* row = s_rows + lane * RS;
 				*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
+				if (NRM) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
 				if (NFT > 0) {
 					const float* f = a.feature + (size_t)id * F;
 #pragma unroll
@@ -473,6 +481,8 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					const int g = 16 * mt + 2 * gid + h;  // D rows gid (h = 0) and gid + 8 (h = 1)
 					if (tig < 3) *reinterpret_cast<float2*>(s_m + g * 12 + 2 * tig) = make_float2(mom[mt][2 * h], mom[mt][2 * h + 1]);
 					if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
+					// columns 4..7 of the tile, {dnx, dny, dnz, 0}, behind the [BWD_CH][12] rows
+					if (NRM && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 					// F = 32: lane tig holds features 8 tig .. 8 tig + 7 of row g, one 32-byte sector (lo = the first four, hi
 					// = the last four).  Lanes tig and tig ^ 1 swap halves so that each red.v4 below pairs with its neighbour's
 					// into one whole sector: lane 2u + e adds into 16 u + 4 e (sector 2u: its own lo and the odd lane's lo), then
@@ -534,6 +544,10 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				red_add_v4(gb, dmx, dmy, -0.5f * q_dxx, -0.5f * q_dxy);
 				red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 				red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}
+				if (NRM) {
+					const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
+					red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
+				}
 			}
 			BWD_PH_LAP(ph, BWD_PH_FLUSH);
 		};
@@ -599,7 +613,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 
 // Channel groups (F > 32, BlendArgs::groups): the same replay with one warp per block doing every step, 12 CTAs per SM.
 // At F = 64 and 128 the launch is several waves deep, and there the two-warp kernel measured slower on an H100.
-template <bool VEC, bool DM>
+template <bool VEC, bool DM, bool NRM>
 __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 {
 	constexpr int NFT = 4;
@@ -662,7 +676,11 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 		bgterm = T * (a.bg[0] * g4[0] + a.bg[1] * g4[1] + a.bg[2] * g4[2] - h);
 		float* grow = s_g + (lane >> 1) * GS + (lane & 1);  // element (pixel, ch) at [pi][ch][e]
 #pragma unroll
-		for (int c = 0; c < 4; c++) { grow[2 * (RGBD + c)] = g4[c]; grow[2 * (RGBD + 4 + c)] = 0.f; }
+		for (int c = 0; c < 4; c++) {
+			grow[2 * (RGBD + c)] = g4[c];
+			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
+			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside && first) ? a.dL_dnormal[c * HW + pix] : 0.f;
+		}
 		if (NFT > 0) {
 #pragma unroll
 			for (int i = 0; i < 8 * NFT; i++)
@@ -750,10 +768,12 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				}
 			}
 			if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
+			if (NRM && first && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
 		} else if (lane < cnt) {
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
 			*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
+			if (NRM && first) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
 			if (NFT > 0) {
 				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
@@ -910,6 +930,8 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				const int g = 16 * mt + 2 * gid + h;  // D rows gid (h = 0) and gid + 8 (h = 1)
 				if (tig < 3) *reinterpret_cast<float2*>(s_m + g * 12 + 2 * tig) = make_float2(mom[mt][2 * h], mom[mt][2 * h + 1]);
 				if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
+				// columns 4..7 of the tile, {dnx, dny, dnz, 0}, behind the [BWD_CH][12] rows
+				if (NRM && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 				if (NFT > 0 && g < cnt && a.dL_dfeat) {
 					const uint32_t id = __float_as_uint(s_q[2 * g + 1].w);
 					float* df = a.dL_dfeat + (size_t)id * F + c0;
@@ -957,6 +979,10 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 			red_add_v4(gb, dmx, dmy, -0.5f * q_dxx, -0.5f * q_dxy);
 			red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 			if (first) red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}: zero in the other groups
+			if (NRM && first) {
+				const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
+				red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
+			}
 		}
 	};
 
@@ -975,38 +1001,39 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 
 bool feature_rows_vectorizable(const float* feature, int F);
 
-template <int NFT, bool DM>
+template <int NFT, bool DM, bool NRM>
 static void launch_bwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8;
 	const bool vec = (NFT == 0) || (a.F == 8 * NFT && feature_rows_vectorizable(a.feature, a.F) &&
 		(reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0);
-	if (vec) blend_bwd_kernel<NFT, true, DM><<<grid, 64, 0, s>>>(a);
-	else blend_bwd_kernel<NFT, false, DM><<<grid, 64, 0, s>>>(a);
+	if (vec) blend_bwd_kernel<NFT, true, DM, NRM><<<grid, 64, 0, s>>>(a);
+	else blend_bwd_kernel<NFT, false, DM, NRM><<<grid, 64, 0, s>>>(a);
 }
 
-template <bool DM>
+template <bool DM, bool NRM>
 static void launch_bwd_dm(const BlendArgs& a, cudaStream_t s)
 {
 	if (a.groups > 1) {
 		const int grid = a.grid_x * a.grid_y * 8 * a.groups;
 		const bool vec = feature_rows_vectorizable(a.feature, a.F) && (reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0;
-		if (vec) blend_bwd_groups_kernel<true, DM><<<grid, 32, 0, s>>>(a);
-		else blend_bwd_groups_kernel<false, DM><<<grid, 32, 0, s>>>(a);
+		if (vec) blend_bwd_groups_kernel<true, DM, NRM><<<grid, 32, 0, s>>>(a);
+		else blend_bwd_groups_kernel<false, DM, NRM><<<grid, 32, 0, s>>>(a);
 		return;
 	}
 	switch (nft_for(a.F)) {
-	case 0: launch_bwd_t<0, DM>(a, s); break;
-	case 1: launch_bwd_t<1, DM>(a, s); break;
-	case 2: launch_bwd_t<2, DM>(a, s); break;
-	default: launch_bwd_t<4, DM>(a, s); break;
+	case 0: launch_bwd_t<0, DM, NRM>(a, s); break;
+	case 1: launch_bwd_t<1, DM, NRM>(a, s); break;
+	case 2: launch_bwd_t<2, DM, NRM>(a, s); break;
+	default: launch_bwd_t<4, DM, NRM>(a, s); break;
 	}
 }
 
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.tgt_depth || a.tgt_mask) launch_bwd_dm<true>(a, s);
-	else launch_bwd_dm<false>(a, s);
+	if (a.nrm) launch_bwd_dm<false, true>(a, s);  // never with the depth / mask heads (launch_blend_fwd)
+	else if (a.tgt_depth || a.tgt_mask) launch_bwd_dm<true, false>(a, s);
+	else launch_bwd_dm<false, false>(a, s);
 }
 
 // The median depth is the view-space z of one Gaussian per pixel, chosen by a piecewise-constant rule: its cotangent goes to

@@ -44,7 +44,9 @@ static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32, "forward chunk size");
 // GRP: F > 32, channel groups (BlendArgs::groups); the F <= 32 instantiations carry none of the group arithmetic.
 // DM: the depth / mask heads (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.
 // MED: the median contributor (BlendArgs::median_id / out_median_depth); likewise.
-template <int NFT, bool VEC, bool GRP, bool DM, bool MED>
+// NRM: the normal plane (BlendArgs::nrm / out_normal): the per-Gaussian quad {nx, ny, nz, 0} fills columns 4..7 of the
+// {r,g,b,depth} tile, zero padding otherwise, so the MMAs the kernel issues anyway blend it; likewise.
+template <int NFT, bool VEC, bool GRP, bool DM, bool MED, bool NRM>
 __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendArgs a)
 {
 	using L = RowLayout<NFT>;
@@ -131,10 +133,12 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				}
 			}
 			if (lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD, a.rgbd + myid);
+			if (NRM && lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD + 4, a.nrm + myid);
 		} else if (lane < cnt) {  // feature rows that are not whole 8-wide tiles (e.g. F = 3): plain loads, zero padded
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
 			if (first) *reinterpret_cast<float4*>(row + L::RGBD) = a.rgbd[id];
+			if (NRM && first) *reinterpret_cast<float4*>(row + L::RGBD + 4) = a.nrm[id];
 			if (NFT > 0) {
 				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
@@ -210,8 +214,8 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				mma_3xtf32(acc[1][nt], ahi[1], alo[1], bh0, bh1, bl0, bl1);
 			}
 			if (first) {
-				const float c0 = gid < 4 ? row0[L::RGBD + gid] : 0.f;
-				const float c1 = gid < 4 ? row1[L::RGBD + gid] : 0.f;
+				const float c0 = (NRM || gid < 4) ? row0[L::RGBD + gid] : 0.f;
+				const float c1 = (NRM || gid < 4) ? row1[L::RGBD + gid] : 0.f;
 				uint32_t bh0, bl0, bh1, bl1;
 				tf32_split(c0, bh0, bl0);
 				tf32_split(c1, bh1, bl1);
@@ -280,6 +284,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				if (!first) continue;
 				if (in && c < 3) a.out_color[(size_t)c * HW + pix] = col[e];
 				else if (in && c == 3 && a.out_depth) a.out_depth[pix] = col[e];
+				else if (NRM && in && c > 3 && c < 7) a.out_normal[(size_t)(c - 4) * HW + pix] = col[e];  // no background term
 			}
 			if (heads) {  // warp-uniform
 #pragma unroll
@@ -381,7 +386,7 @@ bool feature_rows_vectorizable(const float* feature, int F)
 	return F > 0 && (F & 3) == 0 && (reinterpret_cast<uintptr_t>(feature) & 15) == 0;
 }
 
-template <int NFT, bool GRP, bool DM, bool MED>
+template <int NFT, bool GRP, bool DM, bool MED, bool NRM>
 static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
@@ -389,31 +394,33 @@ static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 	// groups, a row slice starts at channel 32 g: 16-byte aligned whenever F % 4 == 0, and a remainder group copies whole
 	// 4-channel pieces only.
 	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F));
-	if (vec) blend_fwd_kernel<NFT, true, GRP, DM, MED><<<grid, 32, 0, s>>>(a);
-	else blend_fwd_kernel<NFT, false, GRP, DM, MED><<<grid, 32, 0, s>>>(a);
+	if (vec) blend_fwd_kernel<NFT, true, GRP, DM, MED, NRM><<<grid, 32, 0, s>>>(a);
+	else blend_fwd_kernel<NFT, false, GRP, DM, MED, NRM><<<grid, 32, 0, s>>>(a);
 }
 
-template <bool DM, bool MED>
+template <bool DM, bool MED, bool NRM>
 static void launch_fwd_dm(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.groups > 1) { launch_fwd_t<4, true, DM, MED>(a, s); return; }
+	if (a.groups > 1) { launch_fwd_t<4, true, DM, MED, NRM>(a, s); return; }
 	switch (nft_for(a.F)) {
-	case 0: launch_fwd_t<0, false, DM, MED>(a, s); break;
-	case 1: launch_fwd_t<1, false, DM, MED>(a, s); break;
-	case 2: launch_fwd_t<2, false, DM, MED>(a, s); break;
-	default: launch_fwd_t<4, false, DM, MED>(a, s); break;
+	case 0: launch_fwd_t<0, false, DM, MED, NRM>(a, s); break;
+	case 1: launch_fwd_t<1, false, DM, MED, NRM>(a, s); break;
+	case 2: launch_fwd_t<2, false, DM, MED, NRM>(a, s); break;
+	default: launch_fwd_t<4, false, DM, MED, NRM>(a, s); break;
 	}
 }
-
 
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s)
 {
 	const bool dm = a.tgt_color && (a.tgt_depth || a.tgt_mask);
-	if (a.median_id) {
-		if (dm) launch_fwd_dm<true, true>(a, s);
-		else launch_fwd_dm<false, true>(a, s);
-	} else if (dm) launch_fwd_dm<true, false>(a, s);
-	else launch_fwd_dm<false, false>(a, s);
+	if (a.nrm) {  // never with the depth / mask heads: the entry points refuse that pair, so it has no instantiation
+		if (a.median_id) launch_fwd_dm<false, true, true>(a, s);
+		else launch_fwd_dm<false, false, true>(a, s);
+	} else if (a.median_id) {
+		if (dm) launch_fwd_dm<true, true, false>(a, s);
+		else launch_fwd_dm<false, true, false>(a, s);
+	} else if (dm) launch_fwd_dm<true, false, false>(a, s);
+	else launch_fwd_dm<false, false, false>(a, s);
 }
 
 }  // namespace mgs

@@ -203,6 +203,14 @@ struct BlendArgs {
 	// blend kernels without it read their parameters at the same offsets as before.
 	int* median_id;
 	float* out_median_depth;
+	// normal plane (nullable; the launchers pick the NRM instantiations when nrm is set): nrm [P] is the view's per-Gaussian
+	// quad {nx, ny, nz, 0} (normals.cu), blended in columns 4..6 of the {r,g,b,depth} tile.  Forward: out_normal [3,H,W].
+	// Backward: dL_dnormal [3,H,W] is its cotangent, and gn [P,4] (zeroed by the caller) receives dL/dn.  Behind
+	// out_median_depth for the same reason.
+	const float4* nrm;
+	float* out_normal;
+	const float* dL_dnormal;
+	float* gn;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
 	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams
@@ -294,5 +302,22 @@ void launch_blend_fwd(const BlendArgs& a, cudaStream_t s);
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
 // the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0
 void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s);
+
+// normals.cu: nrm[i] = {s a, 0}, a the world-space direction of Gaussian i's shortest axis (unit, from the normalised
+// quaternion), s = +-1 so that it faces cam_pos
+void launch_normals_fwd(int P, const float* means3D, const float* scales, const float* rotations, const float* cam_pos, float4* nrm,
+	cudaStream_t s);
+// dL_drot[i] += the chain of sum_v s_{i,v} gn[v][i] through the axis and the quaternion's normalisation, for the V views of
+// one launch (gn[v]: view v's [P,4] blend-stage normal gradients, cam_pos[v] its camera centre)
+struct NormalsBwdArgs {
+	int P, V;
+	const float* means3D;
+	const float* scales;
+	const float* rotations;
+	float* dL_drot;  // [P,4]
+	const float* gn[MAX_BWD_VIEWS];
+	const float* cam_pos[MAX_BWD_VIEWS];
+};
+void launch_normals_bwd(const NormalsBwdArgs& a, cudaStream_t s);
 
 }  // namespace mgs

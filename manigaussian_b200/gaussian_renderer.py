@@ -72,13 +72,16 @@ def _camera_scalars(nv, idx):
 
 
 def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=None, features_color=None,
-           features_language=None, return_depth=False, return_alpha=False, antialiasing=False, return_median_depth=False):
+           features_language=None, return_depth=False, return_alpha=False, antialiasing=False, return_median_depth=False,
+           return_normal=False):
     """Render view `idx` of data['novel_view'].  Same arguments and result as the reference's render(); with
     return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended, no background term), with
     return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth), with
     return_median_depth=True "median_depth" [H,W] (the depth of the contributor at which the pixel's opacity crosses one
     half, differentiable) and "median_id" [H,W] int32 (that Gaussian's index, -1 where nothing covers the pixel;
-    INTEGRATION.md §7).  antialiasing=True renders with the anti-aliased projection (opacity compensation for the 0.3 px^2
+    INTEGRATION.md §7), with return_normal=True "normal" [3,H,W] (each Gaussian's shortest axis in world space, turned to
+    face the camera, alpha-blended and not normalised: normal / alpha is the expected normal; differentiable, INTEGRATION.md
+    §8).  antialiasing=True renders with the anti-aliased projection (opacity compensation for the 0.3 px^2
     dilation, INTEGRATION.md §5)."""
     device = pts_xyz.device
     nv = data["novel_view"]
@@ -96,7 +99,7 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
         sh_degree=3 if features_color is None else 1, campos=nv["camera_center"][idx], prefiltered=False, debug=False,
         include_feature=(features_language is not None), antialiasing=bool(antialiasing))
     rasterizer = GaussianRasterizer(raster_settings=raster_settings, return_depth=return_depth, return_alpha=return_alpha,
-                                    return_median_depth=return_median_depth)
+                                    return_median_depth=return_median_depth, return_normal=return_normal)
     shs, colors_precomp = None, None
     if features_color is not None:
         shs = features_color
@@ -112,7 +115,9 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
     if return_alpha:
         ret["alpha"] = out[3 + bool(return_depth)]
     if return_median_depth:
-        ret["median_depth"], ret["median_id"] = out[-2], out[-1]
+        ret["median_depth"], ret["median_id"] = out[-2 - bool(return_normal)], out[-1 - bool(return_normal)]
+    if return_normal:
+        ret["normal"] = out[-1]
     return ret
 
 
@@ -168,7 +173,8 @@ def _camera_outputs(ctx, cam, first):
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
-                group, antialiasing=False, return_median=False, cam_vm=None, cam_pm=None, cam_cp=None, cam_tf=None):
+                group, antialiasing=False, return_median=False, return_normal=False, cam_vm=None, cam_pm=None, cam_cp=None,
+                cam_tf=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -185,12 +191,14 @@ class _RasterizeViews(torch.autograd.Function):
         alpha = torch.empty((V, H, W), **opts) if return_alpha else None
         med_depth = torch.empty((V, H, W), **opts) if return_median else None
         med_id = torch.empty((V, H, W), dtype=torch.int32, device=dev) if return_median else None
+        normal = torch.empty((V, 3, H, W), **opts) if return_normal else None
         degree = views[0].sh_degree
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
-                                            debug=views[0].debug, out_buffers=(color, feat_img, depth, alpha, med_depth, med_id),
+                                            debug=views[0].debug,
+                                            out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal),
                                             return_alpha=return_alpha, antialiasing=antialiasing, tan_fov=cam_tf,
-                                            return_median=return_median)
+                                            return_median=return_median, return_normal=return_normal)
         main = torch.cuda.current_stream(dev)
         for st in streams:
             main.wait_stream(st)
@@ -201,17 +209,19 @@ class _RasterizeViews(torch.autograd.Function):
         ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
         empty = torch.empty(0, device=dev)
-        # the id planes are an output: they reach the backward through save_for_backward (an output on ctx is a reference cycle)
+        # the id and normal planes are outputs: they reach the backward through save_for_backward (an output on ctx is a
+        # reference cycle)
         ctx.save_for_backward(means3D, sh if sh is not None else empty, colors_precomp if colors_precomp is not None else empty,
-                              feature if include else empty, scales, rotations, med_id if return_median else empty)
+                              feature if include else empty, scales, rotations, med_id if return_median else empty,
+                              normal if return_normal else empty)
         ctx.mark_non_differentiable(radii, *([med_id] if return_median else []))
         return (color, (feat_img if include else empty), radii, (depth if return_depth else empty),
                 (alpha if return_alpha else empty), (med_depth if return_median else empty),
-                (med_id if return_median else empty))
+                (med_id if return_median else empty), (normal if return_normal else empty))
 
     @staticmethod
-    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha, g_median, _g_median_id):
-        means3D, sh, colors_precomp, feature, scales, rotations, med_id = ctx.saved_tensors
+    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha, g_median, _g_median_id, g_normal):
+        means3D, sh, colors_precomp, feature, scales, rotations, med_id, normal = ctx.saved_tensors
         dev = means3D.device
         views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -226,6 +236,7 @@ class _RasterizeViews(torch.autograd.Function):
         g_depth = _prep(g_depth, dev) if (ctx.return_depth and g_depth is not None and g_depth.numel()) else None
         g_alpha = _prep(g_alpha, dev) if (ctx.return_alpha and g_alpha is not None and g_alpha.numel()) else None
         g_median = _prep(g_median, dev) if (med_id.numel() and g_median is not None and g_median.numel()) else None
+        g_normal = _prep(g_normal, dev) if (normal.numel() and g_normal is not None and g_normal.numel()) else None
         pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)  # every row is written by the backward
         grp = None if ctx.group in (None, True) else ctx.group
         m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
@@ -236,7 +247,8 @@ class _RasterizeViews(torch.autograd.Function):
                                            accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
                                            after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
                                            antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None,
-                                           tan_fov=ctx.tan_fov, grads_median=g_median, median_ids=med_id if g_median is not None else None)
+                                           tan_fov=ctx.tan_fov, grads_median=g_median, median_ids=med_id if g_median is not None else None,
+                                           grads_normal=g_normal, normals=normal if g_normal is not None else None)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
             # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields.
@@ -245,8 +257,8 @@ class _RasterizeViews(torch.autograd.Function):
         v = pk.views
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None,
-                *_camera_outputs(ctx, res[9] if ctx.camera else None, 14))
+                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None,
+                *_camera_outputs(ctx, res[9] if ctx.camera else None, 15))
 
 
 def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
@@ -406,7 +418,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
-                 targets=None, return_alpha=False, antialiasing=False, ssim=False, return_median_depth=False):
+                 targets=None, return_alpha=False, antialiasing=False, ssim=False, return_median_depth=False, return_normal=False):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -440,6 +452,10 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     return_median_depth: also return "median_depth" [V,H,W], the view-space depth of the contributor at which each pixel's
     accumulated opacity crosses one half (differentiable; its gradient reaches only that Gaussian's depth), and "median_id"
     [V,H,W] int32, that Gaussian's index (-1 where nothing covers the pixel; INTEGRATION.md §7).  Not with targets.
+    return_normal: also return "normal" [V,3,H,W], each Gaussian's shortest axis in world space, turned to face the view's
+    camera, blended with the colour's weights (differentiable: its gradient reaches the rotations, and opacities and means
+    through the blend weights; not normalised, normal / alpha is the expected normal; INTEGRATION.md §8).  Not with targets:
+    the depth / mask heads have no kernel beside it.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -473,6 +489,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
             raise ValueError("targets and return_alpha cannot be combined")
         if return_median_depth:
             raise ValueError("targets and return_median_depth cannot be combined")
+        if return_normal:
+            raise ValueError("targets and return_normal cannot be combined")
         (loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels, loss_l1,
          ssim_v) = _RasterizeViewsLoss.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
@@ -490,18 +508,22 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     if V == 1 and sync_gradients is None and cams[0] is None and cams[3] is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True) if aa else views[0]
-        out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha, return_median_depth=return_median_depth)(
+        out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha, return_median_depth=return_median_depth,
+                                 return_normal=return_normal)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
             colors_precomp=pts_rgb if features_color is None else None, language_feature_precomp=feat, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=None)
         color, feat_img, radii = out[0].unsqueeze(0), out[1].unsqueeze(0), out[2].unsqueeze(0)
         depth = out[3].unsqueeze(0) if return_depth else None
         alpha = out[3 + bool(return_depth)].unsqueeze(0) if return_alpha else None
-        med_depth, med_id = (out[-2].unsqueeze(0), out[-1].unsqueeze(0)) if return_median_depth else (None, None)
+        nn = bool(return_normal)
+        med_depth, med_id = (out[-2 - nn].unsqueeze(0), out[-1 - nn].unsqueeze(0)) if return_median_depth else (None, None)
+        normal = out[-1].unsqueeze(0) if return_normal else None
     else:
-        color, feat_img, radii, depth, alpha, med_depth, med_id = _RasterizeViews.apply(
+        color, feat_img, radii, depth, alpha, med_depth, med_id, normal = _RasterizeViews.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa, bool(return_median_depth), *cams)
+            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa, bool(return_median_depth),
+            bool(return_normal), *cams)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
@@ -510,6 +532,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         ret["alpha"] = alpha
     if return_median_depth:
         ret["median_depth"], ret["median_id"] = med_depth, med_id
+    if return_normal:
+        ret["normal"] = normal
     return ret
 
 
@@ -518,13 +542,14 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 class _RasterizeClouds(torch.autograd.Function):
     """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha, antialiasing,
-    ssim, camera, return_median).  Outputs per cloud: (color, feature image, radii, depth, alpha, median depth, median id), or
+    ssim, camera, return_median, return_normal).  Outputs per cloud: (color, feature image, radii, depth, alpha, median depth,
+    median id, normal), or
     with targets (loss_rgb, loss_embed, color, feature image, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim) with
     gradients through the losses only."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median = meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = meta
         B, dev = len(cloud_views), flat[0].device
         opts = dict(dtype=torch.float32, device=dev)
         clouds, results, frozen, cots, dms, ssims, images = [], [], [], [], [], [], []
@@ -538,10 +563,13 @@ class _RasterizeClouds(torch.autograd.Function):
             alpha = torch.empty((V, H, W), **opts) if return_alpha else None
             med_depth = torch.empty((V, H, W), **opts) if return_median else None
             med_id = torch.empty((V, H, W), dtype=torch.int32, device=dev) if return_median else None
+            normal = torch.empty((V, 3, H, W), **opts) if return_normal else None
             c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, opacity=opacities, scales=scales,
-                     rotations=rotations, out_buffers=(color, feat_img, depth, alpha, med_depth, med_id))
-            if return_median:
-                images.append(med_id)  # the id planes are outputs: saved for backward, never kept on ctx
+                     rotations=rotations, out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal))
+            if targets is None:
+                # the id and normal planes are outputs: saved for backward, never kept on ctx
+                images += [med_id if return_median else torch.empty(0, device=dev),
+                           normal if return_normal else torch.empty(0, device=dev)]
             if targets is not None:
                 t_rgb = _prep(targets[b]["rgb"], dev)
                 t_emb = _prep(targets[b].get("embed"), dev) if F else None
@@ -563,9 +591,9 @@ class _RasterizeClouds(torch.autograd.Function):
         include = clouds[0]["feature"] is not None
         outs, streams = rasterize_clouds_raw(clouds, degree, include, cloud_views[0][0].scale_modifier, return_depth=return_depth,
                                              debug=cloud_views[0][0].debug, return_alpha=return_alpha, antialiasing=antialiasing,
-                                             return_median=return_median)
+                                             return_median=return_median, return_normal=return_normal)
         for b, c in enumerate(clouds):
-            color, feat_img, depth, alpha, med_depth, med_id = c["out_buffers"]
+            color, feat_img, depth, alpha, med_depth, med_id, normal = c["out_buffers"]
             radii = torch.stack([o[3] for o in outs[b]])
             empty = lambda: torch.empty(0, device=dev)
             if targets is not None:
@@ -581,7 +609,7 @@ class _RasterizeClouds(torch.autograd.Function):
             else:
                 results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty(),
                             alpha if alpha is not None else empty(), med_depth if med_depth is not None else empty(),
-                            med_id if med_id is not None else empty()]
+                            med_id if med_id is not None else empty(), normal if normal is not None else empty()]
                 frozen += [radii] + ([med_id] if med_id is not None else [])
         ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots, ctx.dms, ctx.ssims = meta, streams, degree, include, cots, dms, ssims
         # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
@@ -595,11 +623,11 @@ class _RasterizeClouds(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median = ctx.meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = ctx.meta
         saved = ctx.saved_tensors
         dev = saved[0].device
-        images = saved[6 * len(cloud_views):]  # per cloud: the image (targets with ssim) or the median ids (return_median)
-        per = 10 if targets is not None else 7
+        images = saved[6 * len(cloud_views):]  # per cloud: the image (targets with ssim), or the median ids and the normal plane
+        per = 10 if targets is not None else 8
         clouds = []
         for b, views in enumerate(cloud_views):
             means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
@@ -626,7 +654,9 @@ class _RasterizeClouds(torch.autograd.Function):
                 if return_alpha and g[4] is not None:
                     c["grad_alpha"] = g[4]
                 if return_median and g[5] is not None:
-                    c["grad_median"], c["median_id"] = g[5], images[b]
+                    c["grad_median"], c["median_id"] = g[5], images[2 * b]
+                if return_normal and g[7] is not None:
+                    c["grad_normal"], c["normal"] = g[7], images[2 * b + 1]
             clouds.append(c)
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
@@ -647,7 +677,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
 
 def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False,
-                  antialiasing=False, ssim=False, return_median_depth=False):
+                  antialiasing=False, ssim=False, return_median_depth=False, return_normal=False):
     """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
     next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
 
@@ -663,7 +693,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     Camera gradients: as in render_views, per cloud (with the field of view of cameras from a learnable intr); clouds that
     share camera tensors (the dyna pair) receive the sum.
     ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets.
-    return_median_depth: every cloud also returns "median_depth" and "median_id" [V,H,W], as in render_views; not with targets."""
+    return_median_depth: every cloud also returns "median_depth" and "median_id" [V,H,W], as in render_views; not with targets.
+    return_normal: every cloud also returns "normal" [V,3,H,W], as in render_views; not with targets."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
     with_targets = [c.get("targets") is not None for c in clouds]
@@ -677,6 +708,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         raise ValueError("targets and return_alpha cannot be combined")
     if all(with_targets) and return_median_depth:
         raise ValueError("targets and return_median_depth cannot be combined")
+    if all(with_targets) and return_normal:
+        raise ValueError("targets and return_normal cannot be combined")
     if len({c.get("features_color") is None for c in clouds}) > 1:
         raise ValueError("clouds disagree on the colour mode (SHs or precomputed colors)")
     device = clouds[0]["pts_xyz"].device
@@ -721,7 +754,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                 for c, views, bt in zip(cams, cloud_views, batches)]
         flat += [t for c in cams for t in c]
     out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim), camera,
-                                  bool(return_median_depth)), *flat)
+                                  bool(return_median_depth), bool(return_normal)), *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]
@@ -737,7 +770,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                 r["loss_l1"], r["ssim"] = loss_l1, ssim_v
             ret.append(r)
         else:
-            color, feat_img, radii, depth, alpha, med_depth, med_id = out[7 * b:7 * b + 7]
+            color, feat_img, radii, depth, alpha, med_depth, med_id, normal = out[8 * b:8 * b + 8]
             r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii}
             if return_depth:
                 r["depth"] = depth
@@ -745,5 +778,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                 r["alpha"] = alpha
             if return_median_depth:
                 r["median_depth"], r["median_id"] = med_depth, med_id
+            if return_normal:
+                r["normal"] = normal
             ret.append(r)
     return ret

@@ -11,7 +11,7 @@ include/mgs_rasterizer.h.
 Supersets of the reference: the feature width F is read from the tensor at run time (0..512) instead of being
 compiled in (config.h:16; widths above 32 blend in groups of 32 channels), `return_depth=True` adds a view-space
 depth plane, and `return_alpha=True` adds the accumulated-opacity plane 1 - final_T.  `return_median_depth=True` adds the
-median-depth plane and each pixel's surface Gaussian.
+median-depth plane and each pixel's surface Gaussian, and `return_normal=True` the surface-normal plane.
 """
 from typing import NamedTuple
 
@@ -262,7 +262,8 @@ def cpu_deep_copy_tuple(input_tuple):
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                        cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False):
+                        cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False,
+                        return_normal=False):
     s = raster_settings
     # camera tensors that require grad become explicit inputs of the node, which then returns their gradients; a field of
     # view held as CUDA tensors (learnable intrinsics) joins them as two more inputs, tanfovx and tanfovy
@@ -273,16 +274,17 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_p
         cam = ()
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
                                      rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha,
-                                     bool(return_median_depth), *cam)
+                                     bool(return_median_depth), bool(return_normal), *cam)
 
 
-_CAM_FIRST = 13  # position of the first camera input of _RasterizeGaussians
+_CAM_FIRST = 14  # position of the first camera input of _RasterizeGaussians
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median=False, *cam):
+                cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median=False,
+                return_normal=False, *cam):
         s = raster_settings
         args = (s.bg, means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations, s.scale_modifier,
                 cov3Ds_precomp, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.image_height, s.image_width, sh,
@@ -295,8 +297,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         # the device field of view, when the settings carry one (read by the kernels in place of host floats)
         tf = _fov_column([s], means3D.device) if (views_path and _is_device_fov(s)) else None
         ctx.tan_fov = tf
-        alpha = med_depth = med_id = None
-        if (return_alpha or return_median or aa or ctx.camera) and views_path:
+        alpha = med_depth = med_id = normal = None
+        if return_normal and (cov3Ds_precomp is not None and cov3Ds_precomp.numel() != 0):
+            raise ValueError("return_normal needs scales and rotations: a precomputed covariance has no axis to take a normal from")
+        if (return_alpha or return_median or return_normal or aa or ctx.camera) and views_path:
             # the alpha plane, the median planes, the anti-aliased projection and the camera gradients exist on the multi-view
             # entry points only: debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
@@ -304,7 +308,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
                                                     rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
                                                     return_depth=return_depth, debug=s.debug, return_alpha=return_alpha,
-                                                    antialiasing=aa, tan_fov=tf, return_median=return_median)
+                                                    antialiasing=aa, tan_fov=tf, return_median=return_median,
+                                                    return_normal=return_normal)
             except Exception as ex:
                 if s.debug:
                     torch.save(cpu_args, "snapshot_fw.dump")
@@ -313,8 +318,10 @@ class _RasterizeGaussians(torch.autograd.Function):
             out = outs[0]
             planes = 7 + bool(return_depth)
             alpha = out[planes] if return_alpha else None
+            if return_normal:
+                normal = out[-1]
             if return_median:
-                med_depth, med_id = out[-2], out[-1]
+                med_depth, med_id = out[-2 - bool(return_normal)], out[-1 - bool(return_normal)]
             ctx.async_view = (int(out[0]), streams)  # as below: never the outputs themselves
         elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
@@ -343,6 +350,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 alpha = torch.zeros(hw, dtype=torch.float32, device=odev)
             if return_median:
                 med_depth, med_id = torch.zeros(hw, dtype=torch.float32, device=odev), torch.full(hw, -1, dtype=torch.int32, device=odev)
+            if return_normal:
+                normal = torch.zeros((3,) + hw, dtype=torch.float32, device=odev)
         num_rendered, color, language_feature, radii, geomBuffer, binningBuffer, imgBuffer = out[:7]
         depth = out[7] if return_depth else None
         ctx.raster_settings = s
@@ -350,26 +359,30 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.return_depth = return_depth
         ctx.return_alpha = return_alpha
         ctx.return_median = return_median
-        # the id plane is an output: it reaches the backward through save_for_backward, never through ctx (reference cycle)
+        ctx.return_normal = return_normal
+        # the id and normal planes are outputs: they reach the backward through save_for_backward, never through ctx (reference
+        # cycle)
         ctx.save_for_backward(colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii,
-                              sh, geomBuffer, binningBuffer, imgBuffer, med_id if return_median else None)
+                              sh, geomBuffer, binningBuffer, imgBuffer, med_id if return_median else None,
+                              normal if return_normal else None)
         if return_median:
             ctx.mark_non_differentiable(radii, med_id)
         else:
             ctx.mark_non_differentiable(radii)
         return (color, language_feature, radii) + ((depth,) if return_depth else ()) + ((alpha,) if return_alpha else ()) + \
-            ((med_depth, med_id) if return_median else ())
+            ((med_depth, med_id) if return_median else ()) + ((normal,) if return_normal else ())
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_language_feature, _radii=None, *grad_planes):
         # grad_planes: the depth gradient when return_depth, then the alpha gradient when return_alpha, then the median-depth
-        # gradient and the (absent) id gradient when return_median
+        # gradient and the (absent) id gradient when return_median, then the normal gradient when return_normal
         grad_out_depth = grad_planes[0] if ctx.return_depth else None
         grad_out_alpha = grad_planes[int(ctx.return_depth)] if ctx.return_alpha else None
-        grad_out_median = grad_planes[-2] if ctx.return_median else None
+        grad_out_median = grad_planes[-2 - int(ctx.return_normal)] if ctx.return_median else None
+        grad_out_normal = grad_planes[-1] if ctx.return_normal else None
         s = ctx.raster_settings
         (colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-         binningBuffer, imgBuffer, med_id) = ctx.saved_tensors
+         binningBuffer, imgBuffer, med_id, normal) = ctx.saved_tensors
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, s.image_height, s.image_width), dtype=torch.float32, device=means3D.device)
         if s.include_feature and grad_out_language_feature is None:
@@ -383,8 +396,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.async_view is not None:
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
-            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.return_median or ctx.antialiasing or
-                                                                  ctx.camera)) else None
+            cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.return_median or ctx.return_normal or
+                                                                  ctx.antialiasing or ctx.camera)) else None
             try:
                 grads = rasterize_views_backward_raw(
                     [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
@@ -393,7 +406,9 @@ class _RasterizeGaussians(torch.autograd.Function):
                     grads_alpha=[grad_out_alpha] if grad_out_alpha is not None else None, antialiasing=ctx.antialiasing,
                     camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov,
                     grads_median=[grad_out_median] if grad_out_median is not None else None,
-                    median_ids=[med_id] if grad_out_median is not None else None)
+                    median_ids=[med_id] if grad_out_median is not None else None,
+                    grads_normal=[grad_out_normal] if (grad_out_normal is not None and normal is not None) else None,
+                    normals=[normal] if (grad_out_normal is not None and normal is not None) else None)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -430,7 +445,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, _or_none(grad_sh, sh), _or_none(grad_colors_precomp, colors_precomp),
                 _or_none(grad_language_feature_precomp, language_feature_precomp) if s.include_feature else None,
                 grad_opacities, _or_none(grad_scales, scales), _or_none(grad_rotations, rotations),
-                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None, None) + grad_cam
+                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None, None, None) + grad_cam
 
 
 class _Settings(NamedTuple):
@@ -476,16 +491,19 @@ class GaussianRasterizationSettings(_Settings):
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False):
+    def __init__(self, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False, return_normal=False):
         """return_depth / return_alpha: forward() also returns the depth plane [H,W] and / or the alpha plane [H,W]
         (accumulated opacity 1 - final_T), in that order after radii.  return_median_depth: it then also returns the
         median-depth plane [H,W] (differentiable) and the median contributor's Gaussian id [H,W] int32 (-1 where nothing
-        covers the pixel; include/mgs_rasterizer.h, mgs_view_median), behind the other planes."""
+        covers the pixel; include/mgs_rasterizer.h, mgs_view_median), behind the other planes.  return_normal: it then also
+        returns, last, the surface-normal plane [3,H,W] (world space, camera facing, not normalised, differentiable;
+        mgs_view_normal); needs scales and rotations."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_depth = return_depth
         self.return_alpha = return_alpha
         self.return_median_depth = return_median_depth
+        self.return_normal = return_normal
 
     def markVisible(self, positions):
         # Mark visible points (based on frustum culling for camera) with a boolean
@@ -509,7 +527,7 @@ class GaussianRasterizer(nn.Module):
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, language_feature_precomp, opacities, scales,
                                    rotations, cov3D_precomp, self.raster_settings, self.return_depth, self.return_alpha,
-                                   self.return_median_depth)
+                                   self.return_median_depth, self.return_normal)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -604,11 +622,16 @@ class ViewOut(tuple):
         return bool(self.status[1])
 
 
-def _state_sizes(L, P, W, H):
-    key = (P, W, H)
+def _state_sizes(L, P, W, H, normal=False):
+    """(geometry state, image state, backward scratch) bytes; `normal`: with the normal plane's per-Gaussian arrays"""
+    key = (P, W, H, bool(normal))
     s = _SIZES.get(key)
     if s is None:
-        s = (int(L.mgs_geometry_state_bytes(P)), int(L.mgs_image_state_bytes(W, H)), int(L.mgs_backward_scratch_bytes(P)))
+        if normal:
+            s = (int(L.mgs_geometry_state_bytes_normal(P)), int(L.mgs_image_state_bytes(W, H)),
+                 int(L.mgs_backward_scratch_bytes_normal(P)))
+        else:
+            s = (int(L.mgs_geometry_state_bytes(P)), int(L.mgs_image_state_bytes(W, H)), int(L.mgs_backward_scratch_bytes(P)))
         _SIZES[key] = s
     return s
 
@@ -640,7 +663,7 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False):
+                        return_median=False, return_normal=False):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -661,7 +684,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     mgs_forward_views_intr); views whose tanfovx / tanfovy are CUDA tensors use it without being asked.  Pass the same to
     the backward.  `return_median` appends the median-depth plane [H,W] and the median contributor's Gaussian id [H,W] int32
     (-1 where nothing covers the pixel) to every ViewOut, behind the other planes (C ABI mgs_view_median); with `out_buffers`
-    they go to out_buffers[4] and out_buffers[5] ([V,H,W] each) when those are given."""
+    they go to out_buffers[4] and out_buffers[5] ([V,H,W] each) when those are given.  `return_normal` appends, last, the
+    surface-normal plane [3,H,W] to every ViewOut (C ABI mgs_view_normal; out_buffers[6] [V,3,H,W] when given); it needs scales
+    and rotations, and cannot be combined with `depth_mask`."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -693,6 +718,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
         sarr = (_b.ViewSsim * V)() if ssim is not None else None
         marr = (_b.ViewMedian * V)() if return_median else None
+        narr = (_b.ViewNormal * V)() if return_normal else None
         status = _status_slots(V)
         keep, outs = [], []
         for v, s in enumerate(views):
@@ -702,7 +728,8 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _fill_ssim(sarr[v], ssim, v)
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
-                                 aarr[v] if return_alpha else None, marr[v] if return_median else None)
+                                 aarr[v] if return_alpha else None, marr[v] if return_median else None,
+                                 narr[v] if return_normal else None)
             arr[v].status = status.data_ptr() + 8 * v
             arr[v].stream = streams[v].cuda_stream
             keep.append(k)
@@ -711,7 +738,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if marr is not None:
+        if narr is not None:
+            _b.check(L.mgs_forward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
+                     "mgs_forward_views_normal")
+        elif marr is not None:
             _b.check(L.mgs_forward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
                      "mgs_forward_views_median")
@@ -756,12 +787,13 @@ def _fill_ssim(ws, ssim, v, w=None, scale=None):
         ws.cot_scale = scale.data_ptr() + 8 * v
 
 
-def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None):
+def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None, wn=None):
     """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream) and, when
-    `wa` (its mgs_view_alpha) is given, its alpha plane, and when `wm` (its mgs_view_median) is given, its median planes.
+    `wa` (its mgs_view_alpha) is given, its alpha plane, when `wm` (its mgs_view_median) is given, its median planes, and when
+    `wn` (its mgs_view_normal) is given, its normal plane.
     Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
-    gbytes, ibytes, _ = _state_sizes(L, P, W, H)
+    gbytes, ibytes, _ = _state_sizes(L, P, W, H, wn is not None)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
     img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
     binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
@@ -798,6 +830,11 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
         med_id = ob[5][v] if ob[5] is not None else torch.empty((H, W), dtype=torch.int32, device=dev)
         wm.out_median_depth, wm.median_id = _ptr(med_depth), _ptr(med_id)
         ret += (med_depth, med_id)
+    if wn is not None:
+        ob = out_buffers[6] if (out_buffers is not None and len(out_buffers) > 6) else None
+        normal = ob[v] if ob is not None else torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        wn.out_normal = _ptr(normal)
+        ret += (normal,)
     return ViewOut(ret), (bg, vm, pm, cp)
 
 
@@ -858,7 +895,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  rotations, scale_modifier, cov3D_precomp, sh, degree, include_feature, grads_depth=None,
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
-                                 ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None):
+                                 ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
+                                 grads_normal=None, normals=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -880,7 +918,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     with it the call is mgs_backward_views_intr, and `camera_grads` gains a 4th entry, dL_dtan_fov [V,2] (the gradient with
     respect to each view's {tan_fovx, tan_fovy}; allocated for True, or named in a 4-tuple).  `grads_median` (per view [H,W]
     or None): cotangents of the median-depth planes of a `return_median` forward, with `median_ids` (per view [H,W] int32)
-    the id planes that forward returned (C ABI mgs_backward_views_median)."""
+    the id planes that forward returned (C ABI mgs_backward_views_median).  `grads_normal` (per view [3,H,W] or None):
+    cotangents of the normal planes of a `return_normal` forward, with `normals` (per view [3,H,W]) the planes that forward
+    returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -922,6 +962,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         sscale = _prep(ssim_scale, dev)
         keep = [dscale, sscale]
         marr = _median_array(grads_median, median_ids, V, dev, keep)
+        narr = _normal_array(grads_normal, normals, V, dev, keep)
         for v, s in enumerate(views):
             w = arr[v]
             if darr is not None:
@@ -932,7 +973,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 keep.append(ga)
             keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
                                        grads_feature[v] if (F and grads_feature is not None) else None,
-                                       grads_depth[v] if grads_depth is not None else None))
+                                       grads_depth[v] if grads_depth is not None else None, narr is not None))
             w.dL_dmean2D = _ptr(m2d) if shared else _ptr(m2d[v])
             w.stream = streams[v].cuda_stream
             if cot_scale is not None:
@@ -949,7 +990,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if marr is not None:
+            if narr is not None:
+                _b.check(L.mgs_backward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, *rest),
+                         "mgs_backward_views_normal")
+            elif marr is not None:
                 _b.check(L.mgs_backward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, *rest),
                          "mgs_backward_views_median")
             elif iarr is not None:
@@ -991,6 +1035,23 @@ def _median_array(grads, ids, V, dev, keep):
     return marr
 
 
+def _normal_array(grads, planes, V, dev, keep):
+    """ViewNormal array of V views' normal cotangents and forward planes (per view [3,H,W] each, or None), or None without
+    cotangents.  The tensors that must stay alive until the call is enqueued go to `keep`."""
+    if grads is None:
+        return None
+    if planes is None:
+        raise ValueError("normal cotangents need the forward's normal planes")
+    narr = (_b.ViewNormal * V)()
+    for v in range(V):
+        if grads[v] is None:
+            continue
+        g = _prep(grads[v], dev)
+        narr[v].out_normal, narr[v].dL_dpix_normal = _ptr(planes[v]), _ptr(g)
+        keep += [g, planes[v]]
+    return narr
+
+
 def _camera_grads(L, camera_grads, Ps, dev, keep, intr=False):
     """(outputs, ViewCameraGrad array) for the views of clouds of Ps[v] Gaussians, or (None, None) without camera_grads.
     True allocates the three outputs [V,16], [V,16], [V,3] (and with `intr` a 4th, dL_dtan_fov [V,2]); a tuple names them
@@ -1021,13 +1082,13 @@ def _camera_grads(L, camera_grads, Ps, dev, keep, intr=False):
     return tuple(camera_grads), carr
 
 
-def _backward_view(L, w, s, o, dev, P, grad_color, grad_feature, grad_depth):
+def _backward_view(L, w, s, o, dev, P, grad_color, grad_feature, grad_depth, normal=False):
     """Fills the backward fields of mgs_view `w` from the view's forward result `o` (a ViewOut) and its pixel gradients
-    (the caller sets dL_dmean2D, stream and cot_scale).  Returns the tensors that must stay alive until the call is enqueued."""
+    (the caller sets dL_dmean2D, stream and cot_scale); `normal`: the scratch also holds the normal gradients.  Returns the tensors that must stay alive until the call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
     bg, vm, pm, cp = (_prep(x, dev) for x in (s.bg, s.viewmatrix, s.projmatrix, s.campos))
     gc, gf, gd = (_prep(x, dev) for x in (grad_color, grad_feature, grad_depth))
-    scratch = torch.empty((_state_sizes(L, P, W, H)[2],), dtype=torch.uint8, device=dev)
+    scratch = torch.empty((_state_sizes(L, P, W, H, normal)[2],), dtype=torch.uint8, device=dev)
     w.viewmatrix, w.projmatrix, w.cam_pos, w.background = _ptr(vm), _ptr(pm), _ptr(cp), _ptr(bg)
     w.tan_fovx, w.tan_fovy, w.width, w.height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
     w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = o[4].data_ptr(), o[5].data_ptr(), o[6].data_ptr(), int(o[0])
@@ -1070,7 +1131,7 @@ def _prep_clouds(clouds, dev, include_feature):
 
 
 def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False,
-                         antialiasing=False, return_median=False):
+                         antialiasing=False, return_median=False, return_normal=False):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
@@ -1083,7 +1144,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
     (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr).
     `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
-    mgs_forward_clouds_median)."""
+    mgs_forward_clouds_median).  `return_normal` appends, last, every view's normal plane [3,H,W], as in rasterize_views_raw
+    (C ABI mgs_forward_clouds_normal)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -1115,6 +1177,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
         sarr = (_b.ViewSsim * V)() if any(c.get("ssim") is not None for c in clouds) else None
         marr = (_b.ViewMedian * V)() if return_median else None
+        narr = (_b.ViewNormal * V)() if return_normal else None
         status = _status_slots(V)
         keep, outs = [], []
         for b, (c, d) in enumerate(zip(clouds, pc)):
@@ -1133,7 +1196,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                 if c.get("ssim") is not None:
                     _fill_ssim(sarr[g], c["ssim"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
-                                      c.get("loss_heads"), aarr[g] if return_alpha else None, marr[g] if return_median else None)
+                                      c.get("loss_heads"), aarr[g] if return_alpha else None, marr[g] if return_median else None,
+                                      narr[g] if return_normal else None)
                 arr[g].status = status.data_ptr() + 8 * g
                 arr[g].stream = streams[g].cuda_stream
                 keep.append(kp)
@@ -1142,7 +1206,11 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        if marr is not None:
+        if narr is not None:
+            _b.check(L.mgs_forward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
+                     "mgs_forward_clouds_normal")
+        elif marr is not None:
             _b.check(L.mgs_forward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
                      "mgs_forward_clouds_median")
@@ -1192,7 +1260,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam).  Clouds with a device field of view (see rasterize_clouds_raw)
     make the call mgs_backward_clouds_intr, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict.  A cloud's
     "grad_median" [V_b,H,W] is the cotangent of a `return_median` forward's median-depth planes, with "median_id" [V_b,H,W]
-    int32 the id planes that forward returned (C ABI mgs_backward_clouds_median)."""
+    int32 the id planes that forward returned (C ABI mgs_backward_clouds_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
+    cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
+    mgs_backward_clouds_normal)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1215,6 +1285,11 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             gm = [c["grad_median"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
             ids = [c["median_id"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
             marr = _median_array(gm, ids, V, dev, keep)
+        narr = None
+        if any(c.get("grad_normal") is not None for c in clouds):
+            gn = [c["grad_normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
+            pl = [c["normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
+            narr = _normal_array(gn, pl, V, dev, keep)
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
             has_sr = _nonempty(d["scales"])
@@ -1246,7 +1321,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     _fill_depth_mask(darr[g], c["depth_mask"], v, dscale)
                 keep.append(_backward_view(L, w, s, outs[b][v], dev, P, c["grad_color"][v],
                                            c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
-                                           c["grad_depth"][v] if c.get("grad_depth") is not None else None))
+                                           c["grad_depth"][v] if c.get("grad_depth") is not None else None,
+                                           c.get("grad_normal") is not None))
                 w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
                 w.stream = streams[g].cuda_stream
                 if c.get("grad_alpha") is not None:
@@ -1267,7 +1343,11 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if marr is not None:
+        if narr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
+                                                  narr, *rest), "mgs_backward_clouds_normal")
+        elif marr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
                                                   *rest), "mgs_backward_clouds_median")
