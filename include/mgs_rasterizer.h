@@ -895,6 +895,51 @@ int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_o
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
 	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
+/*
+ * Lifting 2D maps onto the Gaussians (no reference counterpart; the lift of Gaussian Grouping, SAGA, Feature Splatting and
+ * LUDVIG).  Given one map per view, mgs_lift_views computes per Gaussian g
+ *   lifted[g][c] = sum_v sum_p w_vpg map_v[c][p],     weight[g] = sum_v sum_p w_vpg,
+ * so lifted / weight is the Gaussian's blend-weighted average of the maps and weight alone its visibility over the views.
+ * Definition.  For each view the contributors and weights are the forward blend's own: the same expf, the same skip tests
+ * (power > 0, alpha < 1/255), the same 0.99 clamp, the same T (1 - alpha) < 1e-4 stop, and T the running product, so
+ * w_vpg is bit for bit the weight with which the colour image of that view blends Gaussian g into pixel p (alpha with the
+ * compensated opacity o_eff when antialiasing = 1).  There is no background term; pixels outside the image do not count.
+ * lifted is dL/dfeature of a feature render (normalize_feature off) with cotangent map_v, without the backward's geometry.
+ *   - map_v (mgs_view_lift.map) is [C,H,W] fp32, planar like the feature images; C in [0, MGS_MAX_FEATURE_CHANNELS] is the
+ *     same for every view; with C = 0 only weight is computed and lift may be NULL.
+ *   - out_lifted [P,C] (NULL allowed with C = 0) and out_weight [P] are zero-filled by the call on join_stream, then every
+ *     view of the call is summed into them (float atomics: the order of the sums is not fixed).
+ *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
+ *     (sized as for mgs_forward_views) and binning_capacity, status and stream are used; background and every image,
+ *     backward and loss-head field are ignored.  The view's state afterwards holds its projection and binning; the blend
+ *     state (final_T, n_contrib, pixel masks, block_nwalk) is not written, so it cannot serve a backward.
+ *   - shs or colors_precomp must be given as in mgs_forward_views, and are never read for the lift: the projection stage
+ *     is the forward's own.  intr (NULL, or one mgs_view_intrinsics per view) gives device fields of view; its dL_dtan_fov
+ *     is not used.  The outputs are not differentiable.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for C outside
+ * [0, MGS_MAX_FEATURE_CHANNELS]; MGS_ERR_INVALID_ARG for V <= 0, P <= 0, a NULL map while C > 0, a NULL output, a view
+ * without its state buffers, matrices or radii, and the Gaussian-argument errors of mgs_forward_views.
+ */
+typedef struct mgs_view_lift {
+	const float* map;               /* [C,H,W] fp32, or NULL with C = 0 */
+} mgs_view_lift;
+
+int mgs_lift_views(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int C,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* out_lifted,
+	float* out_weight,
+	int debug,
+	void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

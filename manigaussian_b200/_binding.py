@@ -65,6 +65,11 @@ class ViewNormal(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("out_normal", "dL_dpix_normal")]
 
 
+class ViewLift(C.Structure):
+    """mirror of `mgs_view_lift` (include/mgs_rasterizer.h): the 2D map [C,H,W] one view lifts onto the Gaussians"""
+    _fields_ = [("map", C.c_void_p)]
+
+
 class Cloud(C.Structure):
     """mirror of `mgs_cloud` (include/mgs_rasterizer.h)"""
     _fields_ = [("P", C.c_int)] + [(n, C.c_void_p) for n in (
@@ -170,6 +175,12 @@ def lib():
         getattr(L, nrm).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
             ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
             [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal)] + at[k:]
+    L.mgs_lift_views.restype = C.c_int
+    L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
+                                 i, i, i, i,                        # P D M C
+                                 vp, vp, vp,                        # means3D shs colors
+                                 vp, vp, f, vp, vp,                 # opacities scales scale_modifier rotations cov3D_precomp
+                                 vp, vp, i, vp]                     # out_lifted out_weight debug join_stream
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -215,6 +226,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_median", "mgs_backward_views_median", "mgs_forward_clouds_median", "mgs_backward_clouds_median",
     "mgs_forward_views_normal", "mgs_backward_views_normal", "mgs_forward_clouds_normal", "mgs_backward_clouds_normal",
     "mgs_geometry_state_bytes_normal", "mgs_backward_scratch_bytes_normal",
+    "mgs_lift_views",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

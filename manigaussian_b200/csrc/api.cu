@@ -1033,6 +1033,62 @@ int mgs_forward_views_normal(
 	return join_streams(V, views, join);
 }
 
+int mgs_lift_views(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream)
+{
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
+	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "map channel count must be in [0, " MGS_STR(MGS_MAX_FEATURE_CHANNELS) "]");
+	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
+	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
+	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours (never read: they keep the projection the forward's)");
+	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
+	if (!out_weight || (C > 0 && !out_lifted)) return fail(MGS_ERR_INVALID_ARG, "out_weight (and out_lifted with C > 0) are required");
+	if (C > 0 && !lift) return fail(MGS_ERR_INVALID_ARG, "C > 0 needs one mgs_view_lift per view");
+	for (int v = 0; v < V; v++) {
+		const mgs_view& w = views[v];
+		if (!w.geometry_state || !w.binning_state || !w.image_state)
+			return fail(MGS_ERR_INVALID_ARG, "view: the three state buffers are required");
+		if (!w.viewmatrix || !w.projmatrix || !w.radii) return fail(MGS_ERR_INVALID_ARG, "view: matrices and radii are required");
+		if (shs && !colors_precomp && !w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: cam_pos is required with SHs");
+		if (w.width <= 0 || w.height <= 0 || w.binning_capacity < 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size or capacity");
+		if (C > 0 && !lift[v].map) return fail(MGS_ERR_INVALID_ARG, "view: map is required with C > 0");
+	}
+	const Cloud c{ P, D, M, 0, means3D, shs, colors_precomp, nullptr, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+		antialiasing };
+	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
+	// every view adds into the same outputs: zero them before any view stream starts
+	MGS_CUDA(cudaMemsetAsync(out_weight, 0, (size_t)P * sizeof(float), join));
+	if (C > 0) MGS_CUDA(cudaMemsetAsync(out_lifted, 0, (size_t)P * C * sizeof(float), join));
+	int rc = fork_streams(V, views, join);
+	if (rc < 0) return rc;
+	// stage by stage across the views, as mgs_forward_views_normal: the lift takes the forward blend's place
+	for (int phase = 0; phase < 3; phase++) {
+		for (int v = 0; v < V; v++) {
+			const mgs_view& w = views[v];
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), debug);
+			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
+			else {
+				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+				const ViewState s = carve_view(w, P);
+				LiftArgs la{};
+				la.W = w.width; la.H = w.height; la.grid_x = s.gx; la.grid_y = s.gy; la.C = C; la.groups = blend_groups(C);
+				la.ranges = s.img.ranges; la.tile_order = use_tile_order() ? s.img.tile_order : nullptr; la.recs = s.bin.recs;
+				la.block_list = s.bin.block_list; la.block_count = s.img.block_count; la.mask_stride = s.bin.mask_stride;
+				la.map = C > 0 ? lift[v].map : nullptr; la.lifted = C > 0 ? out_lifted : nullptr; la.weight = out_weight;
+				{ StageTimer t_(ST_BLEND_FWD, st); launch_lift(la, st); }
+				MGS_STAGE("lift");
+			}
+			if (rc < 0) return rc;
+		}
+	}
+	return join_streams(V, views, join);
+}
+
 int mgs_backward_views(
 	int V, const mgs_view* views,
 	int P, int D, int M, int F,

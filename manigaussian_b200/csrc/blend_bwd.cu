@@ -435,7 +435,9 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					tf32_split(w4.x, ahi[mt][0], alo[mt][0]); tf32_split(w4.y, ahi[mt][1], alo[mt][1]);
 					tf32_split(w4.z, ahi[mt][2], alo[mt][2]); tf32_split(w4.w, ahi[mt][3], alo[mt][3]);
 				}
-				// B pairs of GEMM 2: cotangents of the pair's two pixels, channels NFT gid .. NFT gid + NFT - 1, then {r,g,b,depth}[gid]
+				// B pairs of GEMM 2: cotangents of the pair's two pixels, channels NFT gid .. NFT gid + NFT - 1, then {r,g,b,depth}[gid].
+				// This is gemm2_step (blend_mma.cuh) spelled out: through the helper ptxas schedules the NFT = 4 normal-plane
+				// instantiation differently (same instruction count, other order), and this kernel's SASS stays as measured.
 				const float* gp = s_g + (4 * ks + tig) * GS;
 				if (NFT > 0) {
 					float f[2 * (NFT > 0 ? NFT : 1)];
@@ -881,37 +883,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				tf32_split(q4.z, qhi[mt][2], qlo[mt][2]); tf32_split(q4.w, qhi[mt][3], qlo[mt][3]);
 			}
 			// B pairs of GEMM 2: cotangents of the pair's two pixels, channels NFT gid .. NFT gid + NFT - 1, then {r,g,b,depth}[gid]
-			const float* gp = s_g + (4 * ks + tig) * GS;
-			if (NFT > 0) {
-				float f[2 * (NFT > 0 ? NFT : 1)];
-				if (NFT == 4) {
-					const float4 u0 = *reinterpret_cast<const float4*>(gp + 8 * gid), u1 = *reinterpret_cast<const float4*>(gp + 8 * gid + 4);
-					f[0] = u0.x; f[1] = u0.y; f[2 % (2 * NFT)] = u0.z; f[3 % (2 * NFT)] = u0.w;
-					f[4 % (2 * NFT)] = u1.x; f[5 % (2 * NFT)] = u1.y; f[6 % (2 * NFT)] = u1.z; f[7 % (2 * NFT)] = u1.w;
-				} else if (NFT == 2) {
-					const float4 u0 = *reinterpret_cast<const float4*>(gp + 4 * gid);
-					f[0] = u0.x; f[1] = u0.y; f[2 % (2 * NFT)] = u0.z; f[3 % (2 * NFT)] = u0.w;
-				} else {
-					const float2 u0 = *reinterpret_cast<const float2*>(gp + 2 * gid);
-					f[0] = u0.x; f[1] = u0.y;
-				}
-#pragma unroll
-				for (int nt = 0; nt < NFT; nt++) {
-					uint32_t bh0, bl0, bh1, bl1;
-					tf32_split(f[2 * nt], bh0, bl0);
-					tf32_split(f[2 * nt + 1], bh1, bl1);
-#pragma unroll
-					for (int mt = 0; mt < BWD_MT; mt++) mma_3xtf32(dC[mt][nt], ahi[mt], alo[mt], bh0, bh1, bl0, bl1);
-				}
-			}
-			{
-				const float2 c = *reinterpret_cast<const float2*>(gp + 2 * (RGBD + gid));  // columns 4..7 are the zero padding
-				uint32_t bh0, bl0, bh1, bl1;
-				tf32_split(c.x, bh0, bl0);
-				tf32_split(c.y, bh1, bl1);
-#pragma unroll
-				for (int mt = 0; mt < BWD_MT; mt++) mma_3xtf32(dC[mt][NFT], ahi[mt], alo[mt], bh0, bh1, bl0, bl1);
-			}
+			gemm2_step<NFT, BWD_MT>(dC, ahi, alo, s_g + (4 * ks + tig) * GS, gid);
 			// GEMM 3: the basis is exact in TF32, only q is split
 #pragma unroll
 			for (int mt = 0; mt < BWD_MT; mt++) {
@@ -934,30 +906,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				if (NRM && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 				if (NFT > 0 && g < cnt && a.dL_dfeat) {
 					const uint32_t id = __float_as_uint(s_q[2 * g + 1].w);
-					float* df = a.dL_dfeat + (size_t)id * F + c0;
-					// column 2 tig + e of feature tile nt is feature NFT (2 tig + e) + nt
-					if (VEC) {
-						if (NFT == 4) {  // Fg % 4 == 0 here
-							if (!GRP || 8 * tig < Fg)
-								red_add_v4(df + 8 * tig, dC[mt][0][2 * h], dC[mt][1][2 * h], dC[mt][2][2 * h], dC[mt][3][2 * h]);
-							if (!GRP || 8 * tig + 4 < Fg)
-								red_add_v4(df + 8 * tig + 4, dC[mt][0][2 * h + 1], dC[mt][1][2 * h + 1], dC[mt][2][2 * h + 1], dC[mt][3][2 * h + 1]);
-						} else if (NFT == 2) {
-							red_add_v4(df + 4 * tig, dC[mt][0][2 * h], dC[mt][1 % NT][2 * h], dC[mt][0][2 * h + 1], dC[mt][1 % NT][2 * h + 1]);
-						} else {
-							red_add(df + 2 * tig, dC[mt][0][2 * h]);
-							red_add(df + 2 * tig + 1, dC[mt][0][2 * h + 1]);
-						}
-					} else {
-#pragma unroll
-						for (int nt = 0; nt < NFT; nt++) {
-#pragma unroll
-							for (int e = 0; e < 2; e++) {
-								const int f = NFT * (2 * tig + e) + nt;
-								if (f < Fg) red_add(df + f, dC[mt][nt][2 * h + e]);
-							}
-						}
-					}
+					red_feature_row<NFT, VEC, GRP>(a.dL_dfeat + (size_t)id * F + c0, dC[mt], h, tig, Fg);
 				}
 			}
 		}

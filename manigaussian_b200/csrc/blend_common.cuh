@@ -23,6 +23,22 @@ __device__ __forceinline__ void gather_rec(float4* dst, const InstRec* rec)
 	cp_async16(dst + 1, reinterpret_cast<const float4*>(rec) + 1);
 }
 
+// The footprint evaluations of one k-step of the forward walk (lane = pixel at (pfx, pfy)): alpha of the pairs with the
+// eight records q4[2 u], q4[2 u + 1] of k-step ks, 0 where the pair is skipped (power > 0, alpha < 1/255, or slot 8 ks + u
+// at or past cnt).  Shared by blend_fwd_kernel and lift_kernel, so that the lift's weights are the forward's bit for bit.
+__device__ __forceinline__ void walk_alphas(const float4* q4, float pfx, float pfy, int ks, int cnt, float (&al)[8])
+{
+#pragma unroll
+	for (int u = 0; u < 8; u++) {
+		const float4 p = q4[2 * u], q = q4[2 * u + 1];
+		const float dx = p.x - pfx, dy = p.y - pfy;
+		const float power = -0.5f * (p.z * dx * dx + q.x * dy * dy) - p.w * dx * dy;
+		const float alpha = min(ALPHA_MAX, q.y * expf(power));
+		const bool ok = (8 * ks + u < cnt) && !(power > 0.0f) && !(alpha < ALPHA_MIN);
+		al[u] = ok ? alpha : 0.f;
+	}
+}
+
 // Named barrier BASE + s (s = 0 | 1, warp-uniform) over N threads: bar.sync waits for the barrier, bar.arrive signals it
 // without waiting.  The ids stay immediates: with an id held in a register ptxas reserves all 16 barriers of the CTA.
 template <int BASE, int N>

@@ -161,15 +161,7 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			const float4* q4 = s_q + 16 * ks;
 			float* wrow = s_w + 256 * ks;
 			float al[8];      // alpha of the pair, 0 where the pair is skipped (power > 0, alpha < 1/255, empty slot)
-#pragma unroll
-			for (int u = 0; u < 8; u++) {
-				const float4 p = q4[2 * u], q = q4[2 * u + 1];
-				const float dx = p.x - pfx, dy = p.y - pfy;
-				const float power = -0.5f * (p.z * dx * dx + q.x * dy * dy) - p.w * dx * dy;
-				const float alpha = min(ALPHA_MAX, q.y * expf(power));
-				const bool ok = (8 * ks + u < cnt) && !(power > 0.0f) && !(alpha < ALPHA_MIN);
-				al[u] = ok ? alpha : 0.f;
-			}
+			walk_alphas(q4, pfx, pfy, ks, cnt, al);
 #pragma unroll
 			for (int u = 0; u < 8; u++) {
 				const float alpha = al[u];

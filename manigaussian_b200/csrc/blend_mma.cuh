@@ -74,4 +74,79 @@ __device__ __forceinline__ void load_feat(const float* row, int gid, float (&f)[
 	}
 }
 
+// GEMM 2 of the backward blend for one k-step of pixels (blend_bwd.cu), dC[g][ch] += wgt[g][p] C[p][ch]: the A quads of MT
+// 16-row Gaussian tiles, split, times the B pairs of the channel rows gp of pixel pair 4 ks + tig in the [pi][ch][e] layout
+// (row stride 2 (8 NFT + 8): channels NFT gid .. NFT gid + NFT - 1 for feature tiles 0 .. NFT - 1, then {r,g,b,depth}[gid] for
+// tile NFT, whose columns 4..7 are the zero padding or the normal quad).  rgbd = false skips tile NFT.  Shared by blend_bwd and
+// lift_kernel (lift.cu), which runs the same contraction with the blend weights against a 2D map.
+template <int NFT, int MT>
+__device__ __forceinline__ void gemm2_step(float (&dC)[MT][NFT + 1][4], const uint32_t (&ahi)[MT][4], const uint32_t (&alo)[MT][4],
+	const float* gp, int gid, bool rgbd = true)
+{
+	constexpr int RGBD = 8 * NFT;
+	if (NFT > 0) {
+		float f[2 * (NFT > 0 ? NFT : 1)];
+		if (NFT == 4) {
+			const float4 u0 = *reinterpret_cast<const float4*>(gp + 8 * gid), u1 = *reinterpret_cast<const float4*>(gp + 8 * gid + 4);
+			f[0] = u0.x; f[1] = u0.y; f[2 % (2 * NFT)] = u0.z; f[3 % (2 * NFT)] = u0.w;
+			f[4 % (2 * NFT)] = u1.x; f[5 % (2 * NFT)] = u1.y; f[6 % (2 * NFT)] = u1.z; f[7 % (2 * NFT)] = u1.w;
+		} else if (NFT == 2) {
+			const float4 u0 = *reinterpret_cast<const float4*>(gp + 4 * gid);
+			f[0] = u0.x; f[1] = u0.y; f[2 % (2 * NFT)] = u0.z; f[3 % (2 * NFT)] = u0.w;
+		} else {
+			const float2 u0 = *reinterpret_cast<const float2*>(gp + 2 * gid);
+			f[0] = u0.x; f[1] = u0.y;
+		}
+#pragma unroll
+		for (int nt = 0; nt < NFT; nt++) {
+			uint32_t bh0, bl0, bh1, bl1;
+			tf32_split(f[2 * nt], bh0, bl0);
+			tf32_split(f[2 * nt + 1], bh1, bl1);
+#pragma unroll
+			for (int mt = 0; mt < MT; mt++) mma_3xtf32(dC[mt][nt], ahi[mt], alo[mt], bh0, bh1, bl0, bl1);
+		}
+	}
+	if (rgbd) {
+		const float2 c = *reinterpret_cast<const float2*>(gp + 2 * (RGBD + gid));  // columns 4..7 are the zero padding
+		uint32_t bh0, bl0, bh1, bl1;
+		tf32_split(c.x, bh0, bl0);
+		tf32_split(c.y, bh1, bl1);
+#pragma unroll
+		for (int mt = 0; mt < MT; mt++) mma_3xtf32(dC[mt][NFT], ahi[mt], alo[mt], bh0, bh1, bl0, bl1);
+	}
+}
+
+// The feature row of GEMM 2's D row (h = 0: gid, 1: gid + 8) of one Gaussian tile d into df (the row's first channel of the
+// group) with float reductions: column 2 tig + e of feature tile nt is feature NFT (2 tig + e) + nt, so with VEC (16-byte
+// aligned rows, Fg % 4 == 0, and Fg = 8 NFT without GRP) a thread holds whole 4-channel pieces and adds them as
+// red.global.add.v4.f32 (at NFT = 4 two per 32-byte sector); else scalar reductions of the channels below Fg.  Shared by
+// blend_bwd_groups_kernel and lift_kernel.
+template <int NFT, bool VEC, bool GRP>
+__device__ __forceinline__ void red_feature_row(float* df, const float (&d)[NFT + 1][4], int h, int tig, int Fg)
+{
+	constexpr int NT = NFT + 1;
+	if (VEC) {
+		if (NFT == 4) {  // Fg % 4 == 0 here
+			if (!GRP || 8 * tig < Fg)
+				red_add_v4(df + 8 * tig, d[0][2 * h], d[1 % NT][2 * h], d[2 % NT][2 * h], d[3 % NT][2 * h]);
+			if (!GRP || 8 * tig + 4 < Fg)
+				red_add_v4(df + 8 * tig + 4, d[0][2 * h + 1], d[1 % NT][2 * h + 1], d[2 % NT][2 * h + 1], d[3 % NT][2 * h + 1]);
+		} else if (NFT == 2) {
+			red_add_v4(df + 4 * tig, d[0][2 * h], d[1 % NT][2 * h], d[0][2 * h + 1], d[1 % NT][2 * h + 1]);
+		} else {
+			red_add(df + 2 * tig, d[0][2 * h]);
+			red_add(df + 2 * tig + 1, d[0][2 * h + 1]);
+		}
+	} else {
+#pragma unroll
+		for (int nt = 0; nt < NFT; nt++) {
+#pragma unroll
+			for (int e = 0; e < 2; e++) {
+				const int f = NFT * (2 * tig + e) + nt;
+				if (f < Fg) red_add(df + f, d[nt][2 * h + e]);
+			}
+		}
+	}
+}
+
 }  // namespace mgs

@@ -303,6 +303,26 @@ void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
 // the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0
 void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s);
 
+// lift.cu: lifted[id][c] += sum_p w_p,id map[c][p] and weight[id] += sum_p w_p,id over one view's pixels, w = alpha T the
+// forward blend's weights (include/mgs_rasterizer.h, mgs_lift_views).  The tile grid, lists and records are the view's, as
+// in BlendArgs; nothing of the view's state is written.
+struct LiftArgs {
+	int W, H;
+	int grid_x, grid_y;
+	int C;                       // map channels (0 = weights only): also the row stride of lifted
+	int groups;                  // channel groups of 32 (blend_groups(C)), indexed as in BlendArgs
+	const uint2* ranges;         // [T]
+	const uint32_t* tile_order;  // [T] or null
+	const InstRec* recs;         // [R]
+	const uint32_t* block_list;  // [8][mask_stride]
+	const uint32_t* block_count; // [8T]
+	size_t mask_stride;
+	const float* map;            // [C,H,W] or null (C = 0)
+	float* lifted;               // [P,C] (zeroed by the caller) or null (C = 0)
+	float* weight;               // [P] (zeroed by the caller)
+};
+void launch_lift(const LiftArgs& a, cudaStream_t s);
+
 // normals.cu: nrm[i] = {s a, 0}, a the world-space direction of Gaussian i's shortest axis (unit, from the normalised
 // quaternion), s = +-1 so that it faces cam_pos
 void launch_normals_fwd(int P, const float* means3D, const float* scales, const float* rotations, const float* cam_pos, float4* nrm,

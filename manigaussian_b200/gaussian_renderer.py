@@ -24,8 +24,8 @@ import torch
 from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, rasterize_clouds_backward_raw,
-                         rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, lift_views_raw,
+                         rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
 MIN_DENOMINATOR = 1e-12  # gaussian_renderer/__init__.py:67; compiled into the kernel (activate.cu FEAT_EPS)
@@ -535,6 +535,66 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     if return_normal:
         ret["normal"] = normal
     return ret
+
+
+def lift_views(cameras, pts_xyz, rotations, scales, opacity, maps, view_ids=None, antialiasing=False):
+    """Lift one 2D map per camera onto the Gaussians with the blend's own weights (INTEGRATION.md §9).
+
+    cameras / view_ids as `render_views` (a `cameras.CameraBatch`, including device field-of-view cameras of a learnable
+    intr, or a sequence of GaussianRasterizationSettings).  maps: [V,C,H,W], a list of V [C,H,W] (fp32, on the cloud's
+    device), or None for the weights only; C may be 0 .. 512.  For every Gaussian g, with w_vpg = alpha T the weight with
+    which view v's render blends g into pixel p (no background term):
+        lifted[g][c] = sum_v sum_p w_vpg maps[v][c][p]        weight[g] = sum_v sum_p w_vpg
+    lifted / weight is the Gaussian's weighted average of the maps (where weight > 0), weight alone a visibility score over
+    the views.  The same cloud rendered with these cameras and `antialiasing` gives the weights used here.  Inputs that
+    require grad are detached; the outputs are not differentiable.  Returns {"lifted": [P,C], "weight": [P]}; raises
+    ValueError on a shape, dtype or device mismatch."""
+    device = pts_xyz.device
+    if isinstance(cameras, CameraBatch):
+        ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
+        bg = _background((0.0, 0.0, 0.0), device)
+        views = tuple(cameras.settings(i, bg, 0, False) for i in ids)
+    else:
+        views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+    if not views:
+        raise ValueError("lift_views needs at least one view")
+    aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for s in views)
+    P = pts_xyz.shape[0] if (torch.is_tensor(pts_xyz) and pts_xyz.dim() == 2) else -1
+    inputs = (("pts_xyz", pts_xyz, (3,)), ("rotations", rotations, (4,)), ("scales", scales, (3,)), ("opacity", opacity, None))
+    for name, t, tail in inputs:
+        if not torch.is_tensor(t):
+            raise ValueError(f"{name}: expected a tensor")
+        shape_ok = tuple(t.shape) in ((P, 1), (P,)) if tail is None else tuple(t.shape) == (P,) + tail
+        if P <= 0 or not shape_ok:
+            raise ValueError(f"{name}: expected [{P},{'1' if tail is None else tail[0]}], got {tuple(t.shape)}")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name}: expected float32, got {t.dtype}")
+    V = len(views)
+    if maps is not None:
+        if torch.is_tensor(maps):
+            if maps.dim() != 4:
+                raise ValueError(f"maps: expected [V,C,H,W] or a list of [C,H,W], got {tuple(maps.shape)}")
+            maps = list(maps.unbind(0))
+        maps = list(maps)
+        if len(maps) != V:
+            raise ValueError(f"maps: expected {V} maps (one per view), got {len(maps)}")
+        C = maps[0].shape[0] if torch.is_tensor(maps[0]) and maps[0].dim() == 3 else -1
+        for v, (m, s) in enumerate(zip(maps, views)):
+            want = (C, int(s.image_height), int(s.image_width))
+            if not torch.is_tensor(m) or tuple(m.shape) != want:
+                raise ValueError(f"maps[{v}]: expected {list(want)} [C,H,W], got {tuple(m.shape) if torch.is_tensor(m) else type(m)}")
+            if m.dtype != torch.float32:
+                raise ValueError(f"maps[{v}]: expected float32, got {m.dtype}")
+        if C > 512:
+            raise ValueError(f"maps: at most 512 channels, got {C}")
+    for name, t in [(n, x) for n, x, _ in inputs] + [(f"maps[{v}]", m) for v, m in enumerate(maps or ())]:
+        if t.device != device or not t.is_cuda:
+            raise ValueError(f"{name}: expected a CUDA tensor on {device}, got {t.device}")
+    if maps is not None:
+        maps = [m.detach() for m in maps]
+    lifted, weight = lift_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0, None, maps,
+                                    antialiasing=aa)
+    return {"lifted": lifted, "weight": weight}
 
 
 _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations

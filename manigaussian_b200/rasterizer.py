@@ -763,6 +763,77 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     return outs, streams
 
 
+def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, maps, antialiasing=False,
+                   tan_fov=None, debug=False):
+    """Lift one 2D map per view onto the Gaussians (C ABI mgs_lift_views): lifted [P,C] = sum over the views and pixels of
+    the forward blend's weights w = alpha T times the map, weight [P] = the sum of the weights.  `maps`: [V,C,H,W] or a
+    sequence of V [C,H,W] fp32 tensors on the cloud's device (each view's own H, W), or None for weight only.  `views`,
+    `antialiasing` and `tan_fov` as in rasterize_views_raw; the binning state is sized from the same capacity table (a
+    steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
+    needs colours, which the lift never reads: a zero [P,3] buffer stands in for them."""
+    L = _b.lib()
+    dev = means3D.device
+    if not means3D.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    P = means3D.size(0)
+    if P == 0:
+        raise RuntimeError("lift_views_raw needs at least one Gaussian")
+    means3D, opacity, scales, rotations, cov3D_precomp = (_prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp))
+    V = len(views)
+    C = int(maps[0].shape[0]) if maps is not None else 0
+    colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
+    main = torch.cuda.current_stream(dev)
+    streams = _view_streams(dev, V) if V > 1 else [main]
+    di = dev.index if dev.index is not None else torch.cuda.current_device()
+    keys = [(di, P, int(s.image_width), int(s.image_height), v) for v, s in enumerate(views)]
+    capturing = torch.cuda.is_current_stream_capturing()
+    with torch.cuda.device(dev):
+        if not capturing:
+            _poll_status()
+        if any(k not in _CAPACITY for k in keys):
+            if capturing:
+                raise RuntimeError("lift the views once before capturing them in a CUDA graph (the binning capacity is learned "
+                                   "from an eager call)")
+            _calibrate(L, views, keys, dev, P, 0, 0, means3D, None, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                       debug)
+        arr = (_b.View * V)()
+        larr = (_b.ViewLift * V)()
+        status = _status_slots(V)
+        keep, outs = [colors], []
+        for v, s in enumerate(views):
+            H, W = int(s.image_height), int(s.image_width)
+            gbytes, ibytes, _ = _state_sizes(L, P, W, H)
+            cap = _CAPACITY[keys[v]]
+            geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+            img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
+            binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
+            radii = torch.empty((P,), dtype=torch.int32, device=dev)
+            vm, pm = _prep(s.viewmatrix, dev), _prep(s.projmatrix, dev)
+            w = arr[v]
+            w.viewmatrix, w.projmatrix = _ptr(vm), _ptr(pm)
+            w.tan_fovx, w.tan_fovy, w.width, w.height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
+            w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
+            w.radii = radii.data_ptr()
+            w.status = status.data_ptr() + 8 * v
+            w.stream = streams[v].cuda_stream
+            if C:
+                m = _prep(maps[v], dev)
+                larr[v].map = m.data_ptr()
+                keep.append(m)
+            keep += [geom, img, binb, radii, vm, pm]
+            outs.append(ViewOut((cap,)))
+        lifted = torch.empty((P, C), dtype=torch.float32, device=dev)
+        weight = torch.empty((P,), dtype=torch.float32, device=dev)
+        tf = _device_fov(views, tan_fov, dev)
+        keep.append(tf)
+        _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), _intrinsics_array(tf, None) if tf is not None else None,
+                                  P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier),
+                                  _ptr(rotations), _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight),
+                                  int(bool(debug)), main.cuda_stream), "mgs_lift_views")
+        _track_status(outs, keys, status, main, not capturing)
+    return lifted, weight
+
+
 def _fill_depth_mask(wd, depth_mask, v, scale=None):
     """Fills view v's mgs_view_depth_mask `wd` from a `depth_mask` tuple of rasterize_views_raw (and, for the backward, the
     upstream gradients `scale` [V,2])."""
