@@ -8,8 +8,9 @@
 // so that no image-sized PyTorch kernel runs between the forward and the backward of a training step.
 //   S_rgb = sum (x - g)^2        ->  loss_rgb   = S_rgb / (3 N),     d loss_rgb / dx_c   = 2 (x_c - g_c) / (3 N)
 //   S_cos = sum_px cos_px        ->  loss_embed = 1 - S_cos / N,     d loss_embed / dx_f = -(1/N) d cos / dx_f
-//   cos = x.y / (max(|x|, eps) max(|y|, eps));  d cos / dx = y / (nx ny) - (x.y) x / (|x|^2 nx ny)   (second term only
-//   where |x| > eps: below it the clamped norm is a constant, as in ATen's backward of clamp_min)
+//   cos = x.y / (nx ny), nx = max(|x|, eps), ny = max(|y|, eps);  d cos / dx = y / (nx ny) - cos x / (|x| nx)   for |x| > 0
+//   (ATen's cosine_similarity backward: continuous at |x| = eps, where |x| nx = |x|^2 above eps and |x| eps below; 0 at x = 0).
+//   Norms whose square overflows fp32 (|x| >~ 1e19) are outside what these heads evaluate.
 #pragma once
 #include "mgs_common.cuh"
 
@@ -19,7 +20,7 @@ constexpr float COS_EPS = 1e-8f;  // F.cosine_similarity's default eps
 
 struct CosTerms {
 	float inv_nn;   // 1 / (max(|x|, eps) max(|y|, eps))
-	float k;        // (x.y) / |x|^2 * inv_nn where |x| > eps, else 0
+	float k;        // cos / (|x| max(|x|, eps)) where |x| > 0, else 0
 	float cos;
 };
 __device__ __forceinline__ CosTerms cos_terms(float xy, float xx, float yy)
@@ -28,7 +29,8 @@ __device__ __forceinline__ CosTerms cos_terms(float xy, float xx, float yy)
 	CosTerms t;
 	t.inv_nn = 1.0f / (fmaxf(nx, COS_EPS) * fmaxf(ny, COS_EPS));
 	t.cos = xy * t.inv_nn;
-	t.k = nx > COS_EPS ? t.cos / xx : 0.f;
+	// above eps |x| max(|x|, eps) = |x|^2 = xx; below it the clamped norm is a constant, but |x| still carries x's direction
+	t.k = nx > COS_EPS ? t.cos / xx : (nx > 0.f ? t.cos / (nx * COS_EPS) : 0.f);
 	return t;
 }
 // d cos / dx_f

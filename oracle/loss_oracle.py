@@ -27,7 +27,8 @@ def cosine_head(embed, gt):
     nx, ny = np.sqrt((x * x).sum(0)), np.sqrt((y * y).sum(0))
     cx, cy = np.maximum(nx, EPS), np.maximum(ny, EPS)
     cos = (x * y).sum(0) / (cx * cy)
-    # d cos / dx = y / (cx cy) - (x.y) x / (nx^2 cx cy) where nx > eps (the clamp is constant below it)
-    k = np.where(nx > EPS, cos / np.where(nx > EPS, nx * nx, 1.0), 0.0)
+    # d cos / dx = y / (cx cy) - cos x / (nx cx) for nx > 0, as ATen's cosine_similarity backward (continuous at nx = eps:
+    # below it the clamped norm is a constant, but nx still depends on x); 0 at x = 0
+    k = np.where(nx > 0, cos / np.where(nx > 0, nx * cx, 1.0), 0.0)
     dcos = y / (cx * cy) - k * x
     return float(1.0 - cos.mean()), (-dcos / N)
