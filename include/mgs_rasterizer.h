@@ -940,6 +940,59 @@ int mgs_lift_views(
 	int debug,
 	void* join_stream);
 
+/*
+ * Orthographic views (no reference counterpart; gsplat's camera_model="ortho", the virtual views of RVT / RVT-2 and the
+ * top-down colour and height maps of Transporter / CLIPort).  The _ortho calls are the _normal calls (and mgs_lift_views)
+ * with one more argument, `ortho`: a host array of one int per view (V entries, or view_offsets[B] for clouds), 0 for a
+ * perspective view and 1 for an orthographic one, or NULL for all perspective.  The older calls are the _ortho calls with
+ * ortho = NULL.  One call may mix both kinds, also among the views of one cloud; the backward sums them in one pass.
+ * Definition, for an orthographic view, with t = Rv p + tv as for a pinhole view:
+ *   - tan_fovx / tan_fovy (mgs_view, or mgs_view_intrinsics.tan_fov on the device) hold the half-width and half-height of
+ *     the view volume in view-space units.  fx = W / (2 tan_fovx) and fy = H / (2 tan_fovy), the same float expressions as
+ *     for a pinhole view, are then pixels per unit.
+ *   - The Jacobian is J = [[fx, 0, 0], [0, fy, 0]], independent of t, with no frustum clamp.
+ *   - Unchanged from the pinhole path: the near cull t.z > 0.2; the screen mean through the caller's projmatrix,
+ *     ndc = (P p).xy / ((P p).w + 1e-7) (an orthographic matrix has w = 1); the depth t.z; the 0.3 px^2 dilation, the
+ *     anti-aliased compensation, conic, radius, tiles, sort keys and everything after the projection.
+ *   - The SH view direction and the normal plane's facing test use p - cam_pos as for a pinhole view (as gsplat does for
+ *     every camera model), not the view's constant ray direction.
+ *   - Backward: M = J Rv has rows fx Rv0 and fy Rv1; dL/dt is the depth cotangent on t.z alone.  Camera gradients take
+ *     J^T dL/dM with rows (fx q0, fy q1, 0); dL/dtan_fovx = -(fx / tan_fovx) dL/dJ00 and dL/dtan_fovy = -(fy / tan_fovy) dL/dJ11,
+ *     the gradient of a learnable half extent.
+ * Argument errors: an ortho entry other than 0 or 1 returns MGS_ERR_INVALID_ARG before anything is enqueued.
+ */
+int mgs_forward_views_ortho(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_views_ortho(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
+int mgs_forward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho, int D, int M,
+	int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+int mgs_lift_views_ortho(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

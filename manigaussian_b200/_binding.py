@@ -175,12 +175,20 @@ def lib():
         getattr(L, nrm).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
             ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
             [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal)] + at[k:]
+        # ... and the camera models (int ortho[] per view, or NULL) after the normal planes
+        orth = name.replace("_views", "_views_ortho").replace("_clouds", "_clouds_ortho")
+        getattr(L, orth).restype = C.c_int
+        getattr(L, orth).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
+            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
+            [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal), C.POINTER(C.c_int)] + at[k:]
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
                                  i, i, i, i,                        # P D M C
                                  vp, vp, vp,                        # means3D shs colors
                                  vp, vp, f, vp, vp,                 # opacities scales scale_modifier rotations cov3D_precomp
                                  vp, vp, i, vp]                     # out_lifted out_weight debug join_stream
+    L.mgs_lift_views_ortho.restype = C.c_int
+    L.mgs_lift_views_ortho.argtypes = L.mgs_lift_views.argtypes[:5] + [C.POINTER(C.c_int)] + L.mgs_lift_views.argtypes[5:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -227,6 +235,8 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_normal", "mgs_backward_views_normal", "mgs_forward_clouds_normal", "mgs_backward_clouds_normal",
     "mgs_geometry_state_bytes_normal", "mgs_backward_scratch_bytes_normal",
     "mgs_lift_views",
+    "mgs_forward_views_ortho", "mgs_backward_views_ortho", "mgs_forward_clouds_ortho", "mgs_backward_clouds_ortho",
+    "mgs_lift_views_ortho",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

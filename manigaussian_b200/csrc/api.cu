@@ -362,9 +362,18 @@ static ViewState carve_view(const mgs_view& w, int P)
 // the view's device {tan_fovx, tan_fovy} (intr: one entry per view, or NULL), or NULL for mgs_view.tan_fovx / tan_fovy
 static const float* device_fov(const mgs_view_intrinsics* intr, int v) { return intr ? intr[v].tan_fov : nullptr; }
 
+// view v's camera model (ortho: one flag per view, or NULL): 1 orthographic, 0 perspective
+static int ortho_of(const int* ortho, int v) { return ortho ? ortho[v] : 0; }
+static int check_ortho(const int* ortho, int V)
+{
+	for (int v = 0; ortho && v < V; v++)
+		if (ortho[v] != 0 && ortho[v] != 1) return fail(MGS_ERR_INVALID_ARG, "ortho: every entry must be 0 (perspective) or 1 (orthographic)");
+	return 0;
+}
+
 // per-Gaussian projection, depth order and instance offsets; the instance count ends up in geom.point_offsets[P - 1].
-// tan_fov: the view's device field of view, or NULL
-static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, int debug)
+// tan_fov: the view's device field of view, or NULL; ortho: 1 for an orthographic view
+static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, int ortho, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const ViewState s = carve_view(w, c.P);
@@ -382,6 +391,7 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_f
 	pa.iota = geom.iota;
 	pa.antialias = c.antialias;
 	pa.tan_fov = tan_fov;
+	pa.ortho = ortho;
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
 
@@ -680,7 +690,7 @@ static int enqueue_normals_bwd(const Cloud& c, const mgs_view* views, const mgs_
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
 	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
-	const mgs_view_normal* nm, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_normal* nm, const int* ortho, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -728,6 +738,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		CamReduceArgs cr{};
 		cr.accumulate = accumulate ? 1 : 0;
 		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
+		for (int u = 0; u < pb.V; u++) pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << u);
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
@@ -750,7 +761,7 @@ static int project_single_view(const Cloud& c, mgs_view& w, mgs_alloc_fn geometr
 	w.geometry_state = geometry_alloc(geometry_user, mgs_geometry_state_bytes(c.P));
 	w.image_state = image_alloc(image_user, mgs_image_state_bytes(w.width, w.height));
 	if (!w.geometry_state || !w.image_state) return fail(MGS_ERR_ALLOC, "state allocation failed");
-	int rc = enqueue_project(c, w, nullptr, debug);
+	int rc = enqueue_project(c, w, nullptr, 0, debug);
 	if (rc < 0) return rc;
 	MGS_CUDA(cudaMemcpyAsync(host_count, carve_view(w, c.P).geom.point_offsets + c.P - 1, sizeof(int), cudaMemcpyDeviceToHost,
 		reinterpret_cast<cudaStream_t>(w.stream)));
@@ -894,7 +905,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -986,9 +997,23 @@ int mgs_forward_views_normal(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_ortho(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, nullptr, P, D, M, F, means3D,
+		shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_ortho(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
 	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours");
@@ -1021,7 +1046,7 @@ int mgs_forward_views_normal(
 			if (rc < 0) return rc;
 		}
 		for (int v = 0; v < V; v++) {
-			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
+			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 					median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
@@ -1040,8 +1065,20 @@ int mgs_lift_views(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_lifted, float* out_weight, int debug, void* join_stream)
 {
+	return mgs_lift_views_ortho(V, views, lift, antialiasing, intr, nullptr, P, D, M, C, means3D, shs, colors_precomp, opacities, scales,
+		scale_modifier, rotations, cov3D_precomp, out_lifted, out_weight, debug, join_stream);
+}
+
+int mgs_lift_views_ortho(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "map channel count must be in [0, " MGS_STR(MGS_MAX_FEATURE_CHANNELS) "]");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
@@ -1070,7 +1107,7 @@ int mgs_lift_views(
 	for (int phase = 0; phase < 3; phase++) {
 		for (int v = 0; v < V; v++) {
 			const mgs_view& w = views[v];
-			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), debug);
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug);
 			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
 			else {
 				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
@@ -1207,9 +1244,25 @@ int mgs_backward_views_normal(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_ortho(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, nullptr, P, D, M, F,
+		means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity,
+		dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_ortho(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !dL_dmean3D || !dL_dopacity) return fail(MGS_ERR_INVALID_ARG, "means3D, dL_dmean3D and dL_dopacity are required");
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -1225,7 +1278,7 @@ int mgs_backward_views_normal(
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1288,10 +1341,20 @@ int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_of
 	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, int D, int M, int F,
 	float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_ortho(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, nullptr,
+		D, M, F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho, int D, int M,
+	int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
+	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1319,7 +1382,7 @@ int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_of
 		for (int b = 0; b < B; b++) {
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), debug)
+				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 						median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
@@ -1400,9 +1463,19 @@ int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_o
 	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
 	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
+	return mgs_backward_clouds_ortho(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
+		nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
+	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1458,7 +1531,7 @@ int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_o
 		if (pb.B == 0) return 0;
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
-		pb.B = 0; nv = 0; cr.V = 0;
+		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0;
 		for (float*& r : pb.cam_rows) r = nullptr;
 		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
 		return 0;
@@ -1484,6 +1557,7 @@ int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_o
 				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
 				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
 				camera_view(cam, intr, views[v0 + u], v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
+				pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << (nv + u));
 			}
 			nv += n;
 		}

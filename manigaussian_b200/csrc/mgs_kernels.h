@@ -40,6 +40,8 @@ struct ProjectFwdArgs {
 	// device {tan_fovx, tan_fovy}, or NULL: tan_fov* and focal_* above.  Non-NULL picks the instantiation that reads it and
 	// forms the focal lengths as the host does (W / (2 tan_fovx)); behind antialias for the same reason.
 	const float* tan_fov;
+	// 1: an orthographic view (tan_fov* hold its half extents; picks the ORTHO instantiation); behind tan_fov for the same reason
+	int ortho;
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -91,6 +93,9 @@ struct ProjectBwdViewsArgs {
 	float* cam_rows[MAX_BWD_VIEWS];
 	// device fields of view (the CAM instantiation reads them; the launcher picks it when any is set): behind cam_rows
 	ProjectBwdIntr intr[MAX_BWD_VIEWS];
+	// bit u: view u is orthographic.  Only the ORTHO instantiations (of CAM) read it; the launcher picks them when any bit is
+	// set.  Behind intr for the same reason as conic_opacity.
+	uint16_t ortho;
 };
 // the 27 camera terms one CTA writes per view into its camera rows: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1,
 // 3}] at 12 + 3c + {0, 1, 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.  The kernel
@@ -121,7 +126,10 @@ struct ProjectBwdCloudsArgs {
 	const float4* conic_opacity[MAX_BWD_VIEWS];    // per view of the launch, AA only
 	float* cam_rows[MAX_BWD_VIEWS];                // per view of the launch: [CTAs of its cloud][CAM_TERMS], or NULL
 	ProjectBwdIntr intr[MAX_BWD_VIEWS];            // per view of the launch, as in ProjectBwdViewsArgs
+	uint16_t ortho;                                // bit u: view u of the launch is orthographic, as in ProjectBwdViewsArgs
 };
+static_assert(MAX_BWD_VIEWS <= 16, "the orthographic view mask has 16 bits");
+static_assert(sizeof(ProjectBwdViewsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 // the second half of the camera gradients: view u's rows summed in row order into its 35 outputs (each nullable), written
 // (accumulate = 0) or added (1)

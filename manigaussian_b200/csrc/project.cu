@@ -38,22 +38,30 @@ struct Cov2DTerms {
 	float txtz, tytz;
 	M3 T, Vrk, W;
 };
-// Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196)
+// Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196).
+// ORTHO: the orthographic Jacobian J = [[fx, 0, 0], [0, fy, 0]] (fx, fy in pixels per view-space unit), with no frustum clamp
+template <bool ORTHO = false>
 __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, float fy, float tanx, float tany,
 	const float* cov3D, const float* vm)
 {
 	Cov2DTerms o;
 	V3 t = xform4x3(mean, vm);
-	const float limx = 1.3f * tanx;
-	const float limy = 1.3f * tany;
-	const float txtz = t.x / t.z;
-	const float tytz = t.y / t.z;
-	t.x = min(limx, max(-limx, txtz)) * t.z;
-	t.y = min(limy, max(-limy, tytz)) * t.z;
-	M3 J = m3(
-		fx / t.z, 0.0f, -(fx * t.x) / (t.z * t.z),
-		0.0f, fy / t.z, -(fy * t.y) / (t.z * t.z),
-		0.f, 0.f, 0.f);
+	M3 J;
+	float txtz = 0.f, tytz = 0.f;
+	if constexpr (ORTHO) {
+		J = m3(fx, 0.0f, 0.0f, 0.0f, fy, 0.0f, 0.f, 0.f, 0.f);
+	} else {
+		const float limx = 1.3f * tanx;
+		const float limy = 1.3f * tany;
+		txtz = t.x / t.z;
+		tytz = t.y / t.z;
+		t.x = min(limx, max(-limx, txtz)) * t.z;
+		t.y = min(limy, max(-limy, tytz)) * t.z;
+		J = m3(
+			fx / t.z, 0.0f, -(fx * t.x) / (t.z * t.z),
+			0.0f, fy / t.z, -(fy * t.y) / (t.z * t.z),
+			0.f, 0.f, 0.f);
+	}
 	o.W = m3(vm[0], vm[4], vm[8], vm[1], vm[5], vm[9], vm[2], vm[6], vm[10]);
 	o.T = mul(o.W, J);
 	o.Vrk = m3(cov3D[0], cov3D[1], cov3D[2], cov3D[1], cov3D[3], cov3D[4], cov3D[2], cov3D[4], cov3D[5]);
@@ -110,7 +118,10 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 // Only conic_opacity.w and the extent's opacity change; the conic, radius, tiles and keys are those of AA = false.
 // FOV: the field of view is read from the device ({tan_fovx, tan_fovy} at a.tan_fov) and the focal lengths are formed here
 // with the host's float expression, so equal values give the host path's results bit for bit.
-template <bool AA, bool FOV>
+// ORTHO: an orthographic view (include/mgs_rasterizer.h, mgs_forward_views_ortho): tan_fov holds the view volume's half
+// extents, fx = W / (2 tan_fovx) is in pixels per unit, and J does not depend on t.  The screen mean still goes through the
+// caller's projmatrix (w = 1 for an orthographic matrix), and everything after the covariance is the perspective path's.
+template <bool AA, bool FOV, bool ORTHO>
 __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -144,7 +155,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 		tanx = a.tan_fov[0]; tany = a.tan_fov[1];
 		fx = a.W / (2.0f * tanx); fy = a.H / (2.0f * tany);  // as api.cu forms focal_x / focal_y
 	}
-	Cov2DTerms ct = cov2d_terms(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix);
+	Cov2DTerms ct = cov2d_terms<ORTHO>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
 	float det0 = 0.f;  // det of the screen-space covariance before the low-pass (AA only)
 	if (AA) det0 = fmaf(-cov.m[0][1], cov.m[0][1], cov.m[0][0] * cov.m[1][1]);  // explicit fma: rounding independent of contraction
@@ -210,16 +221,26 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* m
 	present[idx] = xform4x3(p, viewmatrix).z > NEAR_Z;
 }
 
+template <bool ORTHO>
+static void launch_project_fwd_model(const ProjectFwdArgs& a, int grid, cudaStream_t s)
+{
+	if (a.tan_fov) {
+		if (a.antialias) project_fwd_kernel<true, true, ORTHO><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, true, ORTHO><<<grid, 256, 0, s>>>(a);
+	} else {
+		if (a.antialias) project_fwd_kernel<true, false, ORTHO><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, false, ORTHO><<<grid, 256, 0, s>>>(a);
+	}
+}
+
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0) return;
 	const int grid = ceil_div(a.P, 256);
-	if (a.tan_fov) {
-		if (a.antialias) project_fwd_kernel<true, true><<<grid, 256, 0, s>>>(a);
-		else project_fwd_kernel<false, true><<<grid, 256, 0, s>>>(a);
+	if (a.ortho) {
+		launch_project_fwd_model<true>(a, grid, s);
 	} else {
-		if (a.antialias) project_fwd_kernel<true, false><<<grid, 256, 0, s>>>(a);
-		else project_fwd_kernel<false, false><<<grid, 256, 0, s>>>(a);
+		launch_project_fwd_model<false>(a, grid, s);
 	}
 }
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s)

@@ -71,7 +71,11 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // view, each thread forms the camera terms of its Gaussian (zeros where culled or past the end:
 // `in` false), the warp sums them into cam_sm[(warp, view)][CAM_TERMS], and the kernel sums its warps after the loop.  A CAM
 // thread therefore runs the whole view loop; it reads Gaussian 0 in place of a missing one and writes no per-Gaussian row.
-template <int NSH, bool AA, bool CAM, class Args>
+//
+// ORTHO (CAM only): bit v of a.ortho marks view v orthographic.  There J = [[fx, 0, 0], [0, fy, 0]] does not move with t, so
+// M = J Rv has rows fx Rv0 and fy Rv1, dL/dt is the depth cotangent on t.z alone, the camera terms take J^T Q = (fx q0, fy q1, 0)
+// and dL/dtan_fov = -(f / tan_fov) dJ00 (dJ11).  The bit is the same for every thread of the launch.
+template <int NSH, bool AA, bool CAM, bool ORTHO, class Args>
 __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx_in, const bool in, float* cam_sm)
 {
 	const int idx = CAM && !in ? 0 : idx_in;
@@ -120,6 +124,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		const ProjectBwdView& w = a.view[v];
 		// the view's record is loaded before the radius is known (the scratch row of an invisible Gaussian is zero-filled
 		// memory, never unmapped): the four loads of a view overlap instead of queueing behind the radius
+		const bool orv = ORTHO && ((a.ortho >> v) & 1u);  // view v is orthographic
 		const float4* gb = reinterpret_cast<const float4*>(w.gb + (size_t)idx * GB_STRIDE);
 		const float4 g0 = gb[0], g1 = gb[1], g2 = gb[2];
 		const uint8_t cl = sh ? w.clamped[idx] : (uint8_t)0;
@@ -159,10 +164,15 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float fx = dfov ? a.intr[v].W / (2.0f * tanx) : w.focal_x, fy = dfov ? a.intr[v].H / (2.0f * tany) : w.focal_y;
 			// M = J Rv: row 0 = (fx / tz) Rv0 - (fx cx / tz^2) Rv2, row 1 likewise with y
 			float m0[3], m1[3], u0[3], u1[3];
+			if (orv) {
 #pragma unroll
-			for (int c = 0; c < 3; c++) {
-				m0[c] = fx * iz * Rv[0][c] - fx * cx * iz2 * Rv[2][c];
-				m1[c] = fy * iz * Rv[1][c] - fy * cy * iz2 * Rv[2][c];
+				for (int c = 0; c < 3; c++) { m0[c] = fx * Rv[0][c]; m1[c] = fy * Rv[1][c]; }
+			} else {
+#pragma unroll
+				for (int c = 0; c < 3; c++) {
+					m0[c] = fx * iz * Rv[0][c] - fx * cx * iz2 * Rv[2][c];
+					m1[c] = fy * iz * Rv[1][c] - fy * cy * iz2 * Rv[2][c];
+				}
 			}
 #pragma unroll
 			for (int c = 0; c < 3; c++) { u0[c] = dot3(S[c], m0); u1[c] = dot3(S[c], m1); }  // S M^T (S symmetric)
@@ -202,15 +212,24 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			if constexpr (CAM) {
 				// dL/dtan_fov: fx = W / (2 tan_fovx) moves J00 = fx / tz and J02 = -fx cx / tz^2 (dfx / dtan_fovx = -fx / tan_fovx),
 				// and where the x clamp holds, cx = +-1.3 tan_fovx tz moves J02.  Likewise for y.
-				const float sx = ux > 0.f ? 1.3f : -1.3f, sy = uy > 0.f ? 1.3f : -1.3f;
-				cg[27] = -(fx / tanx) * (dJ00 * iz - dJ02 * cx * iz2) - (inx ? 0.f : fx * dJ02 * sx * iz);
-				cg[28] = -(fy / tany) * (dJ11 * iz - dJ12 * cy * iz2) - (iny ? 0.f : fy * dJ12 * sy * iz);
+				if (orv) {
+					cg[27] = -(fx / tanx) * dJ00;
+					cg[28] = -(fy / tany) * dJ11;
+				} else {
+					const float sx = ux > 0.f ? 1.3f : -1.3f, sy = uy > 0.f ? 1.3f : -1.3f;
+					cg[27] = -(fx / tanx) * (dJ00 * iz - dJ02 * cx * iz2) - (inx ? 0.f : fx * dJ02 * sx * iz);
+					cg[28] = -(fy / tany) * (dJ11 * iz - dJ12 * cy * iz2) - (iny ? 0.f : fy * dJ12 * sy * iz);
+				}
 			}
 			const float iz3 = iz2 * iz;
 			float dt[3];
-			dt[0] = inx ? -fx * iz2 * dJ02 : 0.f;
-			dt[1] = iny ? -fy * iz2 * dJ12 : 0.f;
-			dt[2] = -fx * iz2 * dJ00 - fy * iz2 * dJ11 + 2.f * fx * cx * iz3 * dJ02 + 2.f * fy * cy * iz3 * dJ12 + ddepth;  // depth = t.z
+			if (orv) {
+				dt[0] = 0.f; dt[1] = 0.f; dt[2] = ddepth;
+			} else {
+				dt[0] = inx ? -fx * iz2 * dJ02 : 0.f;
+				dt[1] = iny ? -fy * iz2 * dJ12 : 0.f;
+				dt[2] = -fx * iz2 * dJ00 - fy * iz2 * dJ11 + 2.f * fx * cx * iz3 * dJ02 + 2.f * fy * cy * iz3 * dJ12 + ddepth;  // depth = t.z
+			}
 			// screen-space mean through the full projection: ndc = (P p).xy / ((P p).w + 1e-7)
 			const float* pm = w.projmatrix;  // P[r][c] = pm[4 c + r]
 			const float hx = pm[0] * p[0] + pm[4] * p[1] + pm[8] * p[2] + pm[12];
@@ -225,7 +244,8 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			}
 			if constexpr (CAM) {
 				// t = Rv p + tv and M = J Rv with J held: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt
-				const float j00 = fx * iz, j11 = fy * iz, j02 = -fx * cx * iz2, j12 = -fy * cy * iz2;
+				const float j00 = orv ? fx : fx * iz, j11 = orv ? fy : fy * iz;
+				const float j02 = orv ? 0.f : -fx * cx * iz2, j12 = orv ? 0.f : -fy * cy * iz2;
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
 					cg[3 * c] = dt[0] * p[c] + j00 * q0[c];
@@ -379,18 +399,20 @@ __device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* 
 	}
 }
 
-// CAM before AA in the template list: the AA flag stays the last argument of every kernel name, as profiles read it
-template <int NSH, int MIN_BLOCKS, bool CAM, bool AA>
+// ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before it, as
+// profiles and the coverage tests read them.  ORTHO is instantiated with CAM only.
+template <int NSH, int MIN_BLOCKS, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
+	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if constexpr (CAM) {
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true>(a, idx, idx < a.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO>(a, idx, idx < a.P, cam_sm);
 		cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
 	} else {
 		if (idx >= a.P) return;
-		project_bwd_gaussian<NSH, AA, false>(a, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false>(a, idx, true, nullptr);
 	}
 }
 
@@ -408,13 +430,15 @@ struct CloudBwd {
 	const ProjectBwdView* view;
 	const float4* const* conic_opacity;  // AA only
 	const ProjectBwdIntr* intr;          // CAM only
+	unsigned ortho;                      // ORTHO only: bit v, view v of the cloud is orthographic
 };
 }  // namespace
 
 // several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
-template <int NSH, int MIN_BLOCKS, bool CAM, bool AA>
+template <int NSH, int MIN_BLOCKS, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
 {
+	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
 	int c = 0;
 	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
 	const ProjectBwdCloud& cl = a.cloud[c];
@@ -422,14 +446,14 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	if (!CAM && idx >= cl.P) return;
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
 		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
-		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr };
+		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr, ORTHO ? (unsigned)a.ortho >> cl.view0 : 0u };
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true>(cb, idx, idx < cl.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO>(cb, idx, idx < cl.P, cam_sm);
 		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
-		project_bwd_gaussian<NSH, AA, false>(cb, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false>(cb, idx, true, nullptr);
 	}
 }
 
@@ -491,21 +515,22 @@ void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s)
 	if (a.V > 0) camera_grad_reduce_kernel<<<a.V, CAM_REDUCE_THREADS, 0, s>>>(a);
 }
 
-template <bool CAM>
+// ORTHO runs at the blocks per SM of its CAM sibling
+template <bool CAM, bool ORTHO>
 static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, cudaStream_t s)
 {
 	if (a.antialias) {
 		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
 		// CAM at degree 2: 3 blocks per SM, the camera and focal-length terms spill at the cap of 4 (128)
-		if (deg <= 1) project_bwd_views_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, CAM, true><<<grid, 128, 0, s>>>(a);
-		else project_bwd_views_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_views_kernel<12, 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_kernel<48, 3, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
 	// CAM at degree <= 1: 4 blocks per SM, as for AA; the camera terms spill at the cap of 5 (96 registers)
-	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_views_kernel<27, 4, CAM, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_views_kernel<48, 3, CAM, false><<<grid, 128, 0, s>>>(a);
+	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_views_kernel<27, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_views_kernel<48, 3, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
@@ -515,24 +540,25 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	const int deg = a.shs ? a.D : 0;
 	bool cam = false;  // camera rows, or a device field of view, which only the CAM instantiation reads
 	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (cam) project_bwd_views<true>(a, grid, deg, s);
-	else project_bwd_views<false>(a, grid, deg, s);
+	if (a.ortho) project_bwd_views<true, true>(a, grid, deg, s);  // an orthographic view: the ORTHO instantiation of CAM
+	else if (cam) project_bwd_views<true, false>(a, grid, deg, s);
+	else project_bwd_views<false, false>(a, grid, deg, s);
 }
 
-template <bool CAM>
+template <bool CAM, bool ORTHO>
 static void project_bwd_clouds(const ProjectBwdCloudsArgs& a, int grid, int deg, cudaStream_t s)
 {
 	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
 	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
 	if (a.antialias) {
-		if (deg <= 1) project_bwd_clouds_kernel<12, 4, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
-		else project_bwd_clouds_kernel<48, 3, CAM, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_clouds_kernel<12, 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+		else project_bwd_clouds_kernel<48, 3, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
-	if (deg <= 1) project_bwd_clouds_kernel<12, 4, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_clouds_kernel<27, 4, CAM, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_clouds_kernel<48, 3, CAM, false><<<grid, 128, 0, s>>>(a);
+	if (deg <= 1) project_bwd_clouds_kernel<12, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_clouds_kernel<27, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_clouds_kernel<48, 3, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
@@ -549,8 +575,9 @@ void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 	const int deg = sh ? a.D : 0;
 	bool cam = false;
 	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (cam) project_bwd_clouds<true>(a, grid, deg, s);
-	else project_bwd_clouds<false>(a, grid, deg, s);
+	if (a.ortho) project_bwd_clouds<true, true>(a, grid, deg, s);
+	else if (cam) project_bwd_clouds<true, false>(a, grid, deg, s);
+	else project_bwd_clouds<false, false>(a, grid, deg, s);
 }
 
 }  // namespace mgs

@@ -300,9 +300,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         alpha = med_depth = med_id = normal = None
         if return_normal and (cov3Ds_precomp is not None and cov3Ds_precomp.numel() != 0):
             raise ValueError("return_normal needs scales and rotations: a precomputed covariance has no axis to take a normal from")
-        if (return_alpha or return_median or return_normal or aa or ctx.camera) and views_path:
-            # the alpha plane, the median planes, the anti-aliased projection and the camera gradients exist on the multi-view
-            # entry points only: debug renders take them too, with the snapshot dump
+        orth = bool(getattr(s, "orthographic", False))
+        ctx.orthographic = orth
+        if (return_alpha or return_median or return_normal or aa or orth or ctx.camera) and views_path:
+            # the alpha plane, the median planes, the anti-aliased and orthographic projections and the camera gradients exist on
+            # the multi-view entry points only: debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
                 outs, streams = rasterize_views_raw([s], means3D, colors_precomp, language_feature_precomp, opacities, scales,
@@ -397,7 +399,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             cap, streams = ctx.async_view
             outs = [ViewOut((cap, None, None, radii, geomBuffer, binningBuffer, imgBuffer))]
             cpu_args = cpu_deep_copy_tuple(args) if (s.debug and (ctx.return_alpha or ctx.return_median or ctx.return_normal or
-                                                                  ctx.antialiasing or ctx.camera)) else None
+                                                                  ctx.antialiasing or ctx.orthographic or ctx.camera)) else None
             try:
                 grads = rasterize_views_backward_raw(
                     [s], outs, streams, [grad_out_color], [grad_out_language_feature] if s.include_feature else None, means3D,
@@ -468,14 +470,19 @@ class GaussianRasterizationSettings(_Settings):
     """The reference's 13 fields (DGR/diff_gaussian_rasterization/__init__.py:166-179) and a 14th argument, `antialiasing`
     (default False; positional after include_feature, or by keyword): the anti-aliased projection of the 3DGS authors'
     current rasterizer (Mip-Splatting's 2D filter; INTEGRATION.md §5).  `antialiasing` is an attribute, not a tuple field:
-    the settings still unpack into the reference's own 13-field NamedTuple, and `_fields` is the reference's."""
+    the settings still unpack into the reference's own 13-field NamedTuple, and `_fields` is the reference's.
+    `orthographic` (default False; keyword, or positional after antialiasing) is an attribute in the same way: True makes the
+    view orthographic, with tanfovx / tanfovy its half-width and half-height in view-space units and projmatrix an
+    orthographic matrix (cameras.projection_orthographic; include/mgs_rasterizer.h, mgs_forward_views_ortho)."""
     antialiasing = False
+    orthographic = False
 
     def __new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix, sh_degree, campos,
-                prefiltered, debug, include_feature, antialiasing=False):
+                prefiltered, debug, include_feature, antialiasing=False, orthographic=False):
         self = super().__new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix,
                                sh_degree, campos, prefiltered, debug, include_feature)
         self.antialiasing = bool(antialiasing)
+        self.orthographic = bool(orthographic)
         return self
 
     @classmethod
@@ -484,10 +491,11 @@ class GaussianRasterizationSettings(_Settings):
 
     def _replace(self, **kw):
         aa = kw.pop("antialiasing", self.antialiasing)
-        return type(self)(*super()._replace(**kw), antialiasing=aa)
+        orth = kw.pop("orthographic", self.orthographic)
+        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth)
 
     def __repr__(self):
-        return super().__repr__()[:-1] + f", antialiasing={self.antialiasing})"
+        return super().__repr__()[:-1] + f", antialiasing={self.antialiasing}, orthographic={self.orthographic})"
 
 
 class GaussianRasterizer(nn.Module):
@@ -636,14 +644,32 @@ def _state_sizes(L, P, W, H, normal=False):
     return s
 
 
-def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug):
+def _ortho_flags(views, ortho=None):
+    """Per-view camera models: `ortho` (V truthy values) when given, else each view's `orthographic` attribute; a ctypes int
+    array for the _ortho calls, or None when every view is perspective (the calls without the argument then serve)."""
+    flags = [bool(o) for o in ortho] if ortho is not None else [bool(getattr(s, "orthographic", False)) for s in views]
+    if len(flags) != len(views):
+        raise ValueError(f"ortho: expected {len(views)} flags, got {len(flags)}")
+    return (ctypes.c_int * len(flags))(*flags) if any(flags) else None
+
+
+def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug,
+               ortho=None):
     """First call for a (cloud size, image size): one projection + scan per view with a host read of the instance count
-    (the reference does this on EVERY call), only to seed the capacity table."""
+    (the reference does this on EVERY call), only to seed the capacity table.  An orthographic view (`ortho`: the views'
+    flags, or None) is counted by a weight-only lift with one binning slot, whose status holds the full count: the
+    single-view mgs_forward_begin has no camera model, and the lift is the cheapest call that takes one.  Its weights are
+    discarded."""
     counts = torch.zeros(len(views), dtype=torch.int32).pin_memory()
     st = torch.cuda.current_stream(dev)
-    keep = []
+    keep, ortho_status = [], {}
     for v, s in enumerate(views):
         if keys[v] in _CAPACITY:
+            continue
+        if ortho is not None and ortho[v]:
+            ortho_status[v], k = _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier,
+                                              cov3D_precomp, debug, st)
+            keep.append(k)
             continue
         H, W = int(s.image_height), int(s.image_width)
         ga, ia = _Alloc(dev), _Alloc(dev)
@@ -657,13 +683,40 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
     st.synchronize()
     for v in range(len(views)):
         if keys[v] not in _CAPACITY:
-            _CAPACITY[keys[v]] = _round_capacity(int(counts[v]) * 1.25 + 4096)
+            n = int(ortho_status[v][0]) if v in ortho_status else int(counts[v])
+            _CAPACITY[keys[v]] = _round_capacity(n * 1.25 + 4096)
+
+
+def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug, st):
+    """Enqueues orthographic view `s`'s projection and binning on `st` with one binning slot.  Returns its pinned status
+    {instance count, overflow}, valid once `st` is synchronised, and what must stay alive until then."""
+    H, W = int(s.image_height), int(s.image_width)
+    gbytes, ibytes, _ = _state_sizes(L, P, W, H)
+    geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+    img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
+    binb = torch.empty(int(L.mgs_binning_state_bytes(1)), dtype=torch.uint8, device=dev)
+    radii = torch.empty((P,), dtype=torch.int32, device=dev)
+    weight = torch.empty((P,), dtype=torch.float32, device=dev)
+    status = torch.zeros((2,), dtype=torch.int32).pin_memory()
+    vm, pm = _prep(s.viewmatrix, dev), _prep(s.projmatrix, dev)
+    tf = _device_fov([s], None, dev)
+    colors = colors if _nonempty(colors) else torch.zeros((P, 3), dtype=torch.float32, device=dev)
+    w = (_b.View * 1)()
+    w[0].viewmatrix, w[0].projmatrix = _ptr(vm), _ptr(pm)
+    w[0].tan_fovx, w[0].tan_fovy, w[0].width, w[0].height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
+    w[0].geometry_state, w[0].binning_state, w[0].image_state, w[0].binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), 1
+    w[0].radii, w[0].status, w[0].stream = radii.data_ptr(), status.data_ptr(), st.cuda_stream
+    _b.check(L.mgs_lift_views_ortho(1, w, None, 0, _intrinsics_array(tf, None) if tf is not None else None, (ctypes.c_int * 1)(1),
+                                    P, 0, 0, 0, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier),
+                                    _ptr(rotations), _ptr(cov3D_precomp), None, _ptr(weight), int(bool(debug)), st.cuda_stream),
+             "mgs_lift_views_ortho")
+    return status, (geom, img, binb, radii, weight, vm, pm, tf, colors)
 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False, return_normal=False):
+                        return_median=False, return_normal=False, ortho=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -686,7 +739,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     (-1 where nothing covers the pixel) to every ViewOut, behind the other planes (C ABI mgs_view_median); with `out_buffers`
     they go to out_buffers[4] and out_buffers[5] ([V,H,W] each) when those are given.  `return_normal` appends, last, the
     surface-normal plane [3,H,W] to every ViewOut (C ABI mgs_view_normal; out_buffers[6] [V,3,H,W] when given); it needs scales
-    and rotations, and cannot be combined with `depth_mask`."""
+    and rotations, and cannot be combined with `depth_mask`.  `ortho` (V flags) marks the orthographic views; by default each
+    view's `orthographic` attribute does.  With any orthographic view the call is mgs_forward_views_ortho; pass the same
+    flags (or views) to the backward."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -699,6 +754,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
+    oarr = _ortho_flags(views, ortho)
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]  # a single view needs no side stream
     di = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -712,7 +768,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call) or pass `capacities`")
             _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug)
+                       debug, oarr)
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
@@ -738,7 +794,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if narr is not None:
+        if oarr is not None:
+            _b.check(L.mgs_forward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                               _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
+                     "mgs_forward_views_ortho")
+        elif narr is not None:
             _b.check(L.mgs_forward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
                      "mgs_forward_views_normal")
@@ -764,11 +824,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
 
 
 def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, maps, antialiasing=False,
-                   tan_fov=None, debug=False):
+                   tan_fov=None, debug=False, ortho=None):
     """Lift one 2D map per view onto the Gaussians (C ABI mgs_lift_views): lifted [P,C] = sum over the views and pixels of
     the forward blend's weights w = alpha T times the map, weight [P] = the sum of the weights.  `maps`: [V,C,H,W] or a
     sequence of V [C,H,W] fp32 tensors on the cloud's device (each view's own H, W), or None for weight only.  `views`,
-    `antialiasing` and `tan_fov` as in rasterize_views_raw; the binning state is sized from the same capacity table (a
+    `antialiasing`, `tan_fov` and `ortho` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with an orthographic view); the binning state is sized from the same capacity table (a
     steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
     needs colours, which the lift never reads: a zero [P,3] buffer stands in for them."""
     L = _b.lib()
@@ -780,6 +840,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         raise RuntimeError("lift_views_raw needs at least one Gaussian")
     means3D, opacity, scales, rotations, cov3D_precomp = (_prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp))
     V = len(views)
+    oarr = _ortho_flags(views, ortho)
     C = int(maps[0].shape[0]) if maps is not None else 0
     colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
     main = torch.cuda.current_stream(dev)
@@ -795,7 +856,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
                 raise RuntimeError("lift the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call)")
             _calibrate(L, views, keys, dev, P, 0, 0, means3D, None, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug)
+                       debug, oarr)
         arr = (_b.View * V)()
         larr = (_b.ViewLift * V)()
         status = _status_slots(V)
@@ -826,10 +887,13 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         weight = torch.empty((P,), dtype=torch.float32, device=dev)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), _intrinsics_array(tf, None) if tf is not None else None,
-                                  P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier),
-                                  _ptr(rotations), _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight),
-                                  int(bool(debug)), main.cuda_stream), "mgs_lift_views")
+        iarr = _intrinsics_array(tf, None) if tf is not None else None
+        rest = (P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
+                _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight), int(bool(debug)), main.cuda_stream)
+        if oarr is not None:
+            _b.check(L.mgs_lift_views_ortho(V, arr, larr, int(bool(antialiasing)), iarr, oarr, *rest), "mgs_lift_views_ortho")
+        else:
+            _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), iarr, *rest), "mgs_lift_views")
         _track_status(outs, keys, status, main, not capturing)
     return lifted, weight
 
@@ -967,7 +1031,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
                                  ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
-                                 grads_normal=None, normals=None):
+                                 grads_normal=None, normals=None, ortho=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -991,7 +1055,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     or None): cotangents of the median-depth planes of a `return_median` forward, with `median_ids` (per view [H,W] int32)
     the id planes that forward returned (C ABI mgs_backward_views_median).  `grads_normal` (per view [3,H,W] or None):
     cotangents of the normal planes of a `return_normal` forward, with `normals` (per view [3,H,W]) the planes that forward
-    returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations."""
+    returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
+    forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1000,6 +1065,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
+    oarr = _ortho_flags(views, ortho)
     main = torch.cuda.current_stream(dev)
     opts = dict(dtype=torch.float32, device=dev)
     acc = accumulate_into or {}
@@ -1061,7 +1127,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if narr is not None:
+            if oarr is not None:
+                _b.check(L.mgs_backward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
+                                                    *rest), "mgs_backward_views_ortho")
+            elif narr is not None:
                 _b.check(L.mgs_backward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, *rest),
                          "mgs_backward_views_normal")
             elif marr is not None:
@@ -1216,7 +1285,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr).
     `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
     mgs_forward_clouds_median).  `return_normal` appends, last, every view's normal plane [3,H,W], as in rasterize_views_raw
-    (C ABI mgs_forward_clouds_normal)."""
+    (C ABI mgs_forward_clouds_normal).  A cloud's optional "ortho" (V_b flags; by default its views' `orthographic`
+    attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -1242,7 +1312,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                     raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is "
                                        "learned from an eager call) or pass `capacities`")
                 _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
-                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug)
+                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug, _ortho_flags(c["views"], c.get("ortho")))
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
@@ -1277,7 +1347,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        if narr is not None:
+        oarr = _clouds_ortho(clouds)
+        if oarr is not None:
+            _b.check(L.mgs_forward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
+                     "mgs_forward_clouds_ortho")
+        elif narr is not None:
             _b.check(L.mgs_forward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
                      "mgs_forward_clouds_normal")
@@ -1303,6 +1378,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         pending = not capturing and all(c.get("capacities") is None for c in clouds)
         _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
     return outs, streams
+
+
+def _clouds_ortho(clouds):
+    """The _ortho calls' int array over every view of the clouds in order, or None when every view is perspective"""
+    flags = [f for c in clouds for f in (_ortho_flags(c["views"], c.get("ortho")) or [0] * len(c["views"]))]
+    return (ctypes.c_int * len(flags))(*flags) if any(flags) else None
 
 
 def _clouds_fov(clouds, dev):
@@ -1333,7 +1414,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     "grad_median" [V_b,H,W] is the cotangent of a `return_median` forward's median-depth planes, with "median_id" [V_b,H,W]
     int32 the id planes that forward returned (C ABI mgs_backward_clouds_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
     cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
-    mgs_backward_clouds_normal)."""
+    mgs_backward_clouds_normal).  Clouds with an orthographic view (see rasterize_clouds_raw) make the call
+    mgs_backward_clouds_ortho."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1414,7 +1496,12 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        if narr is not None:
+        oarr = _clouds_ortho(clouds)
+        if oarr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
+                                                 narr, oarr, *rest), "mgs_backward_clouds_ortho")
+        elif narr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
                                                   narr, *rest), "mgs_backward_clouds_normal")
