@@ -993,6 +993,79 @@ int mgs_lift_views_ortho(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
+/*
+ * Fisheye views (gsplat's camera_model="fisheye"; OpenCV's cv::fisheye model, Kannala-Brandt with four coefficients, all
+ * k = 0 being the equidistant fisheye).  The _fisheye calls are the _ortho calls with one more argument, `fisheye`: a host
+ * array of one mgs_view_fisheye per view (V entries, or view_offsets[B] for clouds), or NULL for none.  An entry with
+ * fisheye = 0 is ignored (the view is perspective or, by its ortho flag, orthographic).  The _ortho calls are the _fisheye
+ * calls with fisheye = NULL.  One call may mix all three models, also among the views of one cloud.
+ * Definition, for a fisheye view, with t = Rv p + tv as for a pinhole view:
+ *   - r = sqrt(t.x^2 + t.y^2), theta = atan2(r, t.z), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8).
+ *   - Screen mean: u = fx theta_d t.x / r + cx, v = fy theta_d t.y / r + cy ((cx, cy) at r = 0).  (cx, cy) are in the blend's
+ *     pixel coordinates, where pixel (i, j) has its centre at (i, j), as in OpenCV: calibrated values are used as they are,
+ *     and a centred camera has cx = (W - 1) / 2.  projmatrix is not read (its gradient is zero); the argument checks are
+ *     unchanged, so callers pass the pinhole matrix of the same K.
+ *   - fx = W / (2 tan_fovx), fy = H / (2 tan_fovy), the same float expressions as for a pinhole view: tan_fovx holds
+ *     W / (2 fx) with fx in pixels per radian.  mgs_view_intrinsics.tan_fov and dL_dtan_fov work unchanged; dL_dtan_fov is then
+ *     the gradient of a learnable fisheye focal length.
+ *   - Jacobian of (u, v) w.r.t. t, with a = theta_d / r, rho' = d theta_d / d theta = 1 + 3 k1 theta^2 + 5 k2 theta^4 +
+ *     7 k3 theta^6 + 9 k4 theta^8, s = r^2 + t.z^2, b = rho' t.z / s and c = (b - a) / r^2:
+ *         J = [[fx (a + c x^2), fx c x y, -fx x rho' / s], [fy c x y, fy (a + c y^2), -fy y rho' / s]]   (x, y = t.x, t.y)
+ *     As r -> 0, a -> 1 / t.z and c -> (2 k1 - 2/3) / t.z^3.  Below r / t.z = 1/8 the kernels take a and c (and c's
+ *     derivatives) from their series in (r / t.z)^2, where the expression above cancels in fp32.  No frustum clamp.
+ *   - Cull: the near cull t.z > 0.2, and a Gaussian whose mean has theta > theta_max is culled the same way (radius 0).
+ *   - Depth is t.z (sort key and depth plane); the SH view direction and the normal plane's facing test use p - cam_pos.
+ *     Every stage after the projection is unchanged.  The covariance is the EWA linearisation J Sigma J^T at the mean, as in
+ *     gsplat: large splats near the rim of a wide view are approximated by it, a property of the model.
+ *   - Backward: the blend's dL/dmean2D (dm) is, for every view, the gradient w.r.t. ndc = (2 u + 1) / W - 1 (the reference's
+ *     convention), so the pixel-space mean (u, v) has the cotangent (du, dv) = (dm0 / (W / 2), dm1 / (H / 2)).  M = J Rv;
+ *     dL/dt = J^T (du, dv) + (dL/dJ = dL/dM Rv^T contracted with dJ/dt, all six entries) + the depth cotangent on t.z.
+ *     Camera gradients: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt, dL/dprojmatrix = 0, dL/dcampos as for a pinhole view (SH),
+ *     dL/dtan_fovx = -(du (u - cx) + sum_j dJ0j J0j) / tan_fovx and likewise for y.  The principal point,
+ *     the coefficients and theta_max receive no gradient.
+ * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: a fisheye flag other than 0 or 1; a view that is both
+ * orthographic and fisheye; a non-finite cx, cy, k1..k4 or theta_max; theta_max outside (0, pi/2].
+ */
+typedef struct mgs_view_fisheye {
+	int fisheye;                    /* 1: a fisheye view; 0: the entry is ignored */
+	float cx, cy;                   /* principal point in pixels (pixel centres at integers) */
+	float k1, k2, k3, k4;           /* Kannala-Brandt coefficients */
+	float theta_max;                /* cull: theta of the mean above it, in (0, pi/2] */
+} mgs_view_fisheye;
+int mgs_forward_views_fisheye(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_views_fisheye(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
+int mgs_forward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int accumulate, int debug,
+	void* join_stream);
+int mgs_lift_views_fisheye(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

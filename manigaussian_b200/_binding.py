@@ -65,6 +65,11 @@ class ViewNormal(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("out_normal", "dL_dpix_normal")]
 
 
+class ViewFisheye(C.Structure):
+    """mirror of `mgs_view_fisheye` (include/mgs_rasterizer.h): one view's Kannala-Brandt fisheye parameters"""
+    _fields_ = [("fisheye", C.c_int)] + [(n, C.c_float) for n in ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")]
+
+
 class ViewLift(C.Structure):
     """mirror of `mgs_view_lift` (include/mgs_rasterizer.h): the 2D map [C,H,W] one view lifts onto the Gaussians"""
     _fields_ = [("map", C.c_void_p)]
@@ -181,6 +186,11 @@ def lib():
         getattr(L, orth).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
             ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
             [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal), C.POINTER(C.c_int)] + at[k:]
+        # ... and the fisheye parameters (one ViewFisheye per view, or NULL) after the camera models
+        fish = name.replace("_views", "_views_fisheye").replace("_clouds", "_clouds_fisheye")
+        getattr(L, fish).restype = C.c_int
+        getattr(L, fish).argtypes = getattr(L, orth).argtypes[:len(getattr(L, orth).argtypes) - len(at) + k] + \
+            [C.POINTER(ViewFisheye)] + at[k:]
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
                                  i, i, i, i,                        # P D M C
@@ -189,6 +199,9 @@ def lib():
                                  vp, vp, i, vp]                     # out_lifted out_weight debug join_stream
     L.mgs_lift_views_ortho.restype = C.c_int
     L.mgs_lift_views_ortho.argtypes = L.mgs_lift_views.argtypes[:5] + [C.POINTER(C.c_int)] + L.mgs_lift_views.argtypes[5:]
+    L.mgs_lift_views_fisheye.restype = C.c_int
+    L.mgs_lift_views_fisheye.argtypes = L.mgs_lift_views_ortho.argtypes[:6] + [C.POINTER(ViewFisheye)] + \
+        L.mgs_lift_views_ortho.argtypes[6:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -237,6 +250,8 @@ EXPORTED_SYMBOLS = (
     "mgs_lift_views",
     "mgs_forward_views_ortho", "mgs_backward_views_ortho", "mgs_forward_clouds_ortho", "mgs_backward_clouds_ortho",
     "mgs_lift_views_ortho",
+    "mgs_forward_views_fisheye", "mgs_backward_views_fisheye", "mgs_forward_clouds_fisheye", "mgs_backward_clouds_fisheye",
+    "mgs_lift_views_fisheye",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

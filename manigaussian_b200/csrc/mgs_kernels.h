@@ -4,6 +4,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "fisheye.cuh"
+
 namespace mgs {
 
 struct InstRec;
@@ -42,6 +44,12 @@ struct ProjectFwdArgs {
 	const float* tan_fov;
 	// 1: an orthographic view (tan_fov* hold its half extents; picks the ORTHO instantiation); behind tan_fov for the same reason
 	int ortho;
+	// 1: a Kannala-Brandt fisheye view (picks the FISHEYE instantiation; projmatrix is not read): principal point, coefficients
+	// and the theta cull of include/mgs_rasterizer.h's mgs_view_fisheye.  Behind ortho for the same reason.
+	int fisheye;
+	float fe_cx, fe_cy;
+	FisheyeK fe_k;
+	float fe_theta_max;
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -96,6 +104,10 @@ struct ProjectBwdViewsArgs {
 	// bit u: view u is orthographic.  Only the ORTHO instantiations (of CAM) read it; the launcher picks them when any bit is
 	// set.  Behind intr for the same reason as conic_opacity.
 	uint16_t ortho;
+	// bit u: view u is a fisheye view with coefficients fe_k[u].  Only the FISHEYE instantiations (of ORTHO and CAM: they serve
+	// all three models) read them; the launcher picks them when any bit is set.  Behind ortho for the same reason.
+	uint16_t fisheye;
+	FisheyeK fe_k[MAX_BWD_VIEWS];
 };
 // the 27 camera terms one CTA writes per view into its camera rows: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1,
 // 3}] at 12 + 3c + {0, 1, 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.  The kernel
@@ -127,8 +139,10 @@ struct ProjectBwdCloudsArgs {
 	float* cam_rows[MAX_BWD_VIEWS];                // per view of the launch: [CTAs of its cloud][CAM_TERMS], or NULL
 	ProjectBwdIntr intr[MAX_BWD_VIEWS];            // per view of the launch, as in ProjectBwdViewsArgs
 	uint16_t ortho;                                // bit u: view u of the launch is orthographic, as in ProjectBwdViewsArgs
+	uint16_t fisheye;                              // bit u: view u of the launch is a fisheye view, as in ProjectBwdViewsArgs
+	FisheyeK fe_k[MAX_BWD_VIEWS];                  // per view of the launch, as in ProjectBwdViewsArgs
 };
-static_assert(MAX_BWD_VIEWS <= 16, "the orthographic view mask has 16 bits");
+static_assert(MAX_BWD_VIEWS <= 16, "the orthographic and fisheye view masks have 16 bits");
 static_assert(sizeof(ProjectBwdViewsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 // the second half of the camera gradients: view u's rows summed in row order into its 35 outputs (each nullable), written

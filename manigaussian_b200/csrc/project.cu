@@ -39,17 +39,25 @@ struct Cov2DTerms {
 	M3 T, Vrk, W;
 };
 // Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196).
-// ORTHO: the orthographic Jacobian J = [[fx, 0, 0], [0, fy, 0]] (fx, fy in pixels per view-space unit), with no frustum clamp
-template <bool ORTHO = false>
+// MODEL_ORTHO: the orthographic Jacobian J = [[fx, 0, 0], [0, fy, 0]] (fx, fy in pixels per view-space unit), with no frustum
+// clamp.  MODEL_FISHEYE: the Kannala-Brandt Jacobian from the radial terms fr of the unclamped t (fisheye.cuh), no clamp.
+constexpr int MODEL_PINHOLE = 0, MODEL_ORTHO = 1, MODEL_FISHEYE = 2;
+template <int MODEL = MODEL_PINHOLE>
 __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, float fy, float tanx, float tany,
-	const float* cov3D, const float* vm)
+	const float* cov3D, const float* vm, const FisheyeRadial* fr = nullptr)
 {
 	Cov2DTerms o;
 	V3 t = xform4x3(mean, vm);
 	M3 J;
 	float txtz = 0.f, tytz = 0.f;
-	if constexpr (ORTHO) {
+	if constexpr (MODEL == MODEL_ORTHO) {
 		J = m3(fx, 0.0f, 0.0f, 0.0f, fy, 0.0f, 0.f, 0.f, 0.f);
+	} else if constexpr (MODEL == MODEL_FISHEYE) {
+		const float cxy = fr->c * t.x * t.y;
+		J = m3(
+			fx * (fr->a + fr->c * t.x * t.x), fx * cxy, -fx * t.x * fr->g,
+			fy * cxy, fy * (fr->a + fr->c * t.y * t.y), -fy * t.y * fr->g,
+			0.f, 0.f, 0.f);
 	} else {
 		const float limx = 1.3f * tanx;
 		const float limy = 1.3f * tany;
@@ -118,10 +126,13 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 // Only conic_opacity.w and the extent's opacity change; the conic, radius, tiles and keys are those of AA = false.
 // FOV: the field of view is read from the device ({tan_fovx, tan_fovy} at a.tan_fov) and the focal lengths are formed here
 // with the host's float expression, so equal values give the host path's results bit for bit.
-// ORTHO: an orthographic view (include/mgs_rasterizer.h, mgs_forward_views_ortho): tan_fov holds the view volume's half
+// MODEL_ORTHO: an orthographic view (include/mgs_rasterizer.h, mgs_forward_views_ortho): tan_fov holds the view volume's half
 // extents, fx = W / (2 tan_fovx) is in pixels per unit, and J does not depend on t.  The screen mean still goes through the
 // caller's projmatrix (w = 1 for an orthographic matrix), and everything after the covariance is the perspective path's.
-template <bool AA, bool FOV, bool ORTHO>
+// MODEL_FISHEYE: a Kannala-Brandt view (mgs_forward_views_fisheye): projmatrix is not read; the screen mean is
+// (fx a t.x + cx, fy a t.y + cy), J the map's Jacobian (fisheye.cuh), and a mean with theta > theta_max is culled like one
+// behind the near plane.  Everything after the covariance is the perspective path's.
+template <bool AA, bool FOV, int MODEL>
 __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -136,11 +147,19 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	a.depths[idx] = __uint_as_float(0x7f800000u);  // +inf: culled Gaussians sort behind every visible one
 
 	V3 p_orig = { a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2] };
-	float4 p_hom = xform4x4(p_orig, a.projmatrix);
-	float p_w = 1.0f / (p_hom.w + 0.0000001f);
-	float p_proj_x = p_hom.x * p_w, p_proj_y = p_hom.y * p_w;
+	float p_proj_x = 0.f, p_proj_y = 0.f;
+	if constexpr (MODEL != MODEL_FISHEYE) {
+		float4 p_hom = xform4x4(p_orig, a.projmatrix);
+		float p_w = 1.0f / (p_hom.w + 0.0000001f);
+		p_proj_x = p_hom.x * p_w; p_proj_y = p_hom.y * p_w;
+	}
 	V3 p_view = xform4x3(p_orig, a.viewmatrix);
 	if (p_view.z <= NEAR_Z) return;  // near cull only (auxiliary.h:154)
+	FisheyeRadial fr{};
+	if constexpr (MODEL == MODEL_FISHEYE) {
+		fr = fisheye_radial<false>(p_view.x, p_view.y, p_view.z, a.fe_k);
+		if (fr.theta > a.fe_theta_max) return;
+	}
 
 	const float* cov3D;
 	if (a.cov3D_precomp != nullptr) {
@@ -155,7 +174,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 		tanx = a.tan_fov[0]; tany = a.tan_fov[1];
 		fx = a.W / (2.0f * tanx); fy = a.H / (2.0f * tany);  // as api.cu forms focal_x / focal_y
 	}
-	Cov2DTerms ct = cov2d_terms<ORTHO>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix);
+	Cov2DTerms ct = cov2d_terms<MODEL>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix, &fr);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
 	float det0 = 0.f;  // det of the screen-space covariance before the low-pass (AA only)
 	if (AA) det0 = fmaf(-cov.m[0][1], cov.m[0][1], cov.m[0][0] * cov.m[1][1]);  // explicit fma: rounding independent of contraction
@@ -172,7 +191,12 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	float lambda1 = mid + sqrtf(max(0.1f, mid * mid - det));
 	float lambda2 = mid - sqrtf(max(0.1f, mid * mid - det));
 	float my_radius = ceilf(3.f * sqrtf(max(lambda1, lambda2)));
-	float px = ndc2pix(p_proj_x, a.W), py = ndc2pix(p_proj_y, a.H);
+	float px, py;
+	if constexpr (MODEL == MODEL_FISHEYE) {
+		px = fx * fr.a * p_view.x + a.fe_cx; py = fy * fr.a * p_view.y + a.fe_cy;
+	} else {
+		px = ndc2pix(p_proj_x, a.W); py = ndc2pix(p_proj_y, a.H);
+	}
 	uint2 rmin, rmax;
 	tile_rect(px, py, (int)my_radius, rmin, rmax, a.grid_x, a.grid_y);
 	if ((rmax.x - rmin.x) * (rmax.y - rmin.y) == 0) return;
@@ -221,15 +245,15 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* m
 	present[idx] = xform4x3(p, viewmatrix).z > NEAR_Z;
 }
 
-template <bool ORTHO>
+template <int MODEL>
 static void launch_project_fwd_model(const ProjectFwdArgs& a, int grid, cudaStream_t s)
 {
 	if (a.tan_fov) {
-		if (a.antialias) project_fwd_kernel<true, true, ORTHO><<<grid, 256, 0, s>>>(a);
-		else project_fwd_kernel<false, true, ORTHO><<<grid, 256, 0, s>>>(a);
+		if (a.antialias) project_fwd_kernel<true, true, MODEL><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, true, MODEL><<<grid, 256, 0, s>>>(a);
 	} else {
-		if (a.antialias) project_fwd_kernel<true, false, ORTHO><<<grid, 256, 0, s>>>(a);
-		else project_fwd_kernel<false, false, ORTHO><<<grid, 256, 0, s>>>(a);
+		if (a.antialias) project_fwd_kernel<true, false, MODEL><<<grid, 256, 0, s>>>(a);
+		else project_fwd_kernel<false, false, MODEL><<<grid, 256, 0, s>>>(a);
 	}
 }
 
@@ -237,10 +261,12 @@ void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0) return;
 	const int grid = ceil_div(a.P, 256);
-	if (a.ortho) {
-		launch_project_fwd_model<true>(a, grid, s);
+	if (a.fisheye) {
+		launch_project_fwd_model<MODEL_FISHEYE>(a, grid, s);
+	} else if (a.ortho) {
+		launch_project_fwd_model<MODEL_ORTHO>(a, grid, s);
 	} else {
-		launch_project_fwd_model<false>(a, grid, s);
+		launch_project_fwd_model<MODEL_PINHOLE>(a, grid, s);
 	}
 }
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s)

@@ -75,7 +75,13 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // ORTHO (CAM only): bit v of a.ortho marks view v orthographic.  There J = [[fx, 0, 0], [0, fy, 0]] does not move with t, so
 // M = J Rv has rows fx Rv0 and fy Rv1, dL/dt is the depth cotangent on t.z alone, the camera terms take J^T Q = (fx q0, fy q1, 0)
 // and dL/dtan_fov = -(f / tan_fov) dJ00 (dJ11).  The bit is the same for every thread of the launch.
-template <int NSH, bool AA, bool CAM, bool ORTHO, class Args>
+//
+// FISH (ORTHO and CAM only): bit v of a.fisheye marks view v a Kannala-Brandt fisheye view with coefficients a.fe_k[v]
+// (fisheye.cuh).  There the screen mean is the fisheye map of t in pixels, not of projmatrix: with (du, dv) = (dm0 / (W / 2),
+// dm1 / (H / 2)) its cotangent (dm, the blend's dL/dmean2D, is w.r.t. ndc), dL/dt gains J^T (du, dv) and the
+// projection-matrix terms are zero; all six entries of J move with t, dL/dt takes the contraction of dL/dJ with dJ/dt,
+// the camera terms take the full J^T Q, and dL/dtan_fovx = -(du (u - cx) + sum_j dJ0j J0j) / tan_fovx (y likewise).
+template <int NSH, bool AA, bool CAM, bool ORTHO, bool FISH, class Args>
 __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx_in, const bool in, float* cam_sm)
 {
 	const int idx = CAM && !in ? 0 : idx_in;
@@ -125,6 +131,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		// the view's record is loaded before the radius is known (the scratch row of an invisible Gaussian is zero-filled
 		// memory, never unmapped): the four loads of a view overlap instead of queueing behind the radius
 		const bool orv = ORTHO && ((a.ortho >> v) & 1u);  // view v is orthographic
+		const bool fev = FISH && ((a.fisheye >> v) & 1u);  // view v is a fisheye view
 		const float4* gb = reinterpret_cast<const float4*>(w.gb + (size_t)idx * GB_STRIDE);
 		const float4 g0 = gb[0], g1 = gb[1], g2 = gb[2];
 		const uint8_t cl = sh ? w.clamped[idx] : (uint8_t)0;
@@ -164,7 +171,23 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float fx = dfov ? a.intr[v].W / (2.0f * tanx) : w.focal_x, fy = dfov ? a.intr[v].H / (2.0f * tany) : w.focal_y;
 			// M = J Rv: row 0 = (fx / tz) Rv0 - (fx cx / tz^2) Rv2, row 1 likewise with y
 			float m0[3], m1[3], u0[3], u1[3];
-			if (orv) {
+			FisheyeRadial fr{};
+			float j01 = 0.f, j10 = 0.f, fj00 = 0.f, fj11 = 0.f, fj02 = 0.f, fj12 = 0.f;  // FISH: J
+			float du = 0.f, dv = 0.f;  // FISH: the cotangent of the pixel-space mean (u, v)
+			if (fev) {
+				// dm is the blend's dL/dmean2D, the gradient w.r.t. ndc = (2 u + 1) / W - 1 (the reference's convention: the
+				// blend scales its pixel-space gradient by W / 2, H / 2); the fisheye mean is in pixels
+				du = dm[0] / (0.5f * a.intr[v].W); dv = dm[1] / (0.5f * a.intr[v].H);
+				fr = fisheye_radial<true>(tx, ty, tz, a.fe_k[v]);
+				const float cxy = fr.c * tx * ty;
+				fj00 = fx * (fr.a + fr.c * tx * tx); j01 = fx * cxy; fj02 = -fx * tx * fr.g;
+				j10 = fy * cxy; fj11 = fy * (fr.a + fr.c * ty * ty); fj12 = -fy * ty * fr.g;
+#pragma unroll
+				for (int c = 0; c < 3; c++) {
+					m0[c] = fj00 * Rv[0][c] + j01 * Rv[1][c] + fj02 * Rv[2][c];
+					m1[c] = j10 * Rv[0][c] + fj11 * Rv[1][c] + fj12 * Rv[2][c];
+				}
+			} else if (orv) {
 #pragma unroll
 				for (int c = 0; c < 3; c++) { m0[c] = fx * Rv[0][c]; m1[c] = fy * Rv[1][c]; }
 			} else {
@@ -212,7 +235,12 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			if constexpr (CAM) {
 				// dL/dtan_fov: fx = W / (2 tan_fovx) moves J00 = fx / tz and J02 = -fx cx / tz^2 (dfx / dtan_fovx = -fx / tan_fovx),
 				// and where the x clamp holds, cx = +-1.3 tan_fovx tz moves J02.  Likewise for y.
-				if (orv) {
+				if (fev) {
+					// u - cx = fx a t.x and every entry of J's first row scale with fx
+					const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
+					cg[27] = -(du * fx * fr.a * tx + dJ00 * fj00 + dJ01 * j01 + dJ02 * fj02) / tanx;
+					cg[28] = -(dv * fy * fr.a * ty + dJ10 * j10 + dJ11 * fj11 + dJ12 * fj12) / tany;
+				} else if (orv) {
 					cg[27] = -(fx / tanx) * dJ00;
 					cg[28] = -(fy / tany) * dJ11;
 				} else {
@@ -223,7 +251,19 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			}
 			const float iz3 = iz2 * iz;
 			float dt[3];
-			if (orv) {
+			if (fev) {
+				// dL/dJ contracted with dJ/dt (fisheye.cuh: da/dx = c x, da/dz = -g, (dg/dr) / r = -cz), then J^T (du, dv)
+				const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
+				const float A = fx * dJ00, Bs = fx * dJ01 + fy * dJ10, Cc = fx * dJ02, Ee = fy * dJ11, Ff = fy * dJ12;
+				const float cx2 = fr.c + fr.C1 * tx * tx, cy2 = fr.c + fr.C1 * ty * ty;
+				dt[0] = A * tx * (2.f * fr.c + cx2) + Bs * ty * cx2 + Ee * tx * cy2 - Cc * (fr.g - fr.cz * tx * tx) + Ff * fr.cz * tx * ty;
+				dt[1] = A * ty * cx2 + Bs * tx * cy2 + Ee * ty * (2.f * fr.c + cy2) + Cc * fr.cz * tx * ty - Ff * (fr.g - fr.cz * ty * ty);
+				dt[2] = A * (fr.cz * tx * tx - fr.g) + Bs * fr.cz * tx * ty + Ee * (fr.cz * ty * ty - fr.g) - (Cc * tx + Ff * ty) * fr.gz
+					+ ddepth;
+				dt[0] += fj00 * du + j10 * dv;
+				dt[1] += j01 * du + fj11 * dv;
+				dt[2] += fj02 * du + fj12 * dv;
+			} else if (orv) {
 				dt[0] = 0.f; dt[1] = 0.f; dt[2] = ddepth;
 			} else {
 				dt[0] = inx ? -fx * iz2 * dJ02 : 0.f;
@@ -237,24 +277,26 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float hw = pm[3] * p[0] + pm[7] * p[1] + pm[11] * p[2] + pm[15];
 			const float iw = 1.0f / (hw + 0.0000001f);
 			const float kx = hx * iw * iw, ky = hy * iw * iw;
+			const float dmp[2] = { fev ? 0.f : dm[0], fev ? 0.f : dm[1] };  // the mean's path through projmatrix
 #pragma unroll
 			for (int c = 0; c < 3; c++) {
 				gp[c] += Rv[0][c] * dt[0] + Rv[1][c] * dt[1] + Rv[2][c] * dt[2]
-					+ (pm[4 * c] * iw - pm[4 * c + 3] * kx) * dm[0] + (pm[4 * c + 1] * iw - pm[4 * c + 3] * ky) * dm[1];
+					+ (pm[4 * c] * iw - pm[4 * c + 3] * kx) * dmp[0] + (pm[4 * c + 1] * iw - pm[4 * c + 3] * ky) * dmp[1];
 			}
 			if constexpr (CAM) {
 				// t = Rv p + tv and M = J Rv with J held: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt
-				const float j00 = orv ? fx : fx * iz, j11 = orv ? fy : fy * iz;
-				const float j02 = orv ? 0.f : -fx * cx * iz2, j12 = orv ? 0.f : -fy * cy * iz2;
+				const float j00 = fev ? fj00 : orv ? fx : fx * iz, j11 = fev ? fj11 : orv ? fy : fy * iz;
+				const float j02 = fev ? fj02 : orv ? 0.f : -fx * cx * iz2, j12 = fev ? fj12 : orv ? 0.f : -fy * cy * iz2;
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
 					cg[3 * c] = dt[0] * p[c] + j00 * q0[c];
 					cg[3 * c + 1] = dt[1] * p[c] + j11 * q1[c];
 					cg[3 * c + 2] = dt[2] * p[c] + j02 * q0[c] + j12 * q1[c];
+					if (fev) { cg[3 * c] += j10 * q1[c]; cg[3 * c + 1] += j01 * q0[c]; }
 				}
 				cg[9] = dt[0]; cg[10] = dt[1]; cg[11] = dt[2];
 				// (hx, hy, hw) = P (p, 1): dL/dhx = dm0 iw, dL/dhy = dm1 iw, dL/dhw = -(dm0 kx + dm1 ky)
-				const float ax = dm[0] * iw, ay = dm[1] * iw, aw = -(dm[0] * kx + dm[1] * ky);
+				const float ax = dmp[0] * iw, ay = dmp[1] * iw, aw = -(dmp[0] * kx + dmp[1] * ky);
 				const float ph[4] = { p[0], p[1], p[2], 1.f };
 #pragma unroll
 				for (int c = 0; c < 4; c++) { cg[12 + 3 * c] = ax * ph[c]; cg[13 + 3 * c] = ay * ph[c]; cg[14 + 3 * c] = aw * ph[c]; }
@@ -399,20 +441,21 @@ __device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* 
 	}
 }
 
-// ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before it, as
-// profiles and the coverage tests read them.  ORTHO is instantiated with CAM only.
-template <int NSH, int MIN_BLOCKS, bool ORTHO, bool CAM, bool AA>
+// FISH, ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before it, as
+// profiles and the coverage tests read them.  ORTHO is instantiated with CAM only, FISH with ORTHO and CAM only.
+template <int NSH, int MIN_BLOCKS, bool FISH, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
 	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
+	static_assert(ORTHO || !FISH, "the fisheye backward is an ORTHO instantiation");
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if constexpr (CAM) {
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO>(a, idx, idx < a.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH>(a, idx, idx < a.P, cam_sm);
 		cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
 	} else {
 		if (idx >= a.P) return;
-		project_bwd_gaussian<NSH, AA, false, false>(a, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false>(a, idx, true, nullptr);
 	}
 }
 
@@ -431,14 +474,17 @@ struct CloudBwd {
 	const float4* const* conic_opacity;  // AA only
 	const ProjectBwdIntr* intr;          // CAM only
 	unsigned ortho;                      // ORTHO only: bit v, view v of the cloud is orthographic
+	unsigned fisheye;                    // FISH only: bit v, view v of the cloud is a fisheye view
+	const FisheyeK* fe_k;                // FISH only: per view of the cloud
 };
 }  // namespace
 
 // several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
-template <int NSH, int MIN_BLOCKS, bool ORTHO, bool CAM, bool AA>
+template <int NSH, int MIN_BLOCKS, bool FISH, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
 {
 	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
+	static_assert(ORTHO || !FISH, "the fisheye backward is an ORTHO instantiation");
 	int c = 0;
 	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
 	const ProjectBwdCloud& cl = a.cloud[c];
@@ -446,14 +492,15 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	if (!CAM && idx >= cl.P) return;
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
 		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
-		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr, ORTHO ? (unsigned)a.ortho >> cl.view0 : 0u };
+		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr, ORTHO ? (unsigned)a.ortho >> cl.view0 : 0u,
+		FISH ? (unsigned)a.fisheye >> cl.view0 : 0u, FISH ? a.fe_k + cl.view0 : nullptr };
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO>(cb, idx, idx < cl.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH>(cb, idx, idx < cl.P, cam_sm);
 		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
-		project_bwd_gaussian<NSH, AA, false, false>(cb, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false>(cb, idx, true, nullptr);
 	}
 }
 
@@ -515,22 +562,23 @@ void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s)
 	if (a.V > 0) camera_grad_reduce_kernel<<<a.V, CAM_REDUCE_THREADS, 0, s>>>(a);
 }
 
-// ORTHO runs at the blocks per SM of its CAM sibling
-template <bool CAM, bool ORTHO>
+// ORTHO and FISH run at the blocks per SM of their CAM sibling
+template <bool CAM, bool ORTHO, bool FISH = false>
 static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, cudaStream_t s)
 {
 	if (a.antialias) {
 		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
 		// CAM at degree 2: 3 blocks per SM, the camera and focal-length terms spill at the cap of 4 (128)
-		if (deg <= 1) project_bwd_views_kernel<12, 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else project_bwd_views_kernel<48, 3, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_views_kernel<12, 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_kernel<48, 3, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
 	// CAM at degree <= 1: 4 blocks per SM, as for AA; the camera terms spill at the cap of 5 (96 registers)
-	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_views_kernel<27, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_views_kernel<48, 3, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	// FISH at degree 2: 3 blocks per SM, the fisheye second derivatives spill at the cap of 4 (128 registers)
+	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_views_kernel<27, FISH ? 3 : 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_views_kernel<48, 3, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
@@ -540,25 +588,26 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	const int deg = a.shs ? a.D : 0;
 	bool cam = false;  // camera rows, or a device field of view, which only the CAM instantiation reads
 	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (a.ortho) project_bwd_views<true, true>(a, grid, deg, s);  // an orthographic view: the ORTHO instantiation of CAM
+	if (a.fisheye) project_bwd_views<true, true, true>(a, grid, deg, s);  // a fisheye view: the FISH instantiation, all models
+	else if (a.ortho) project_bwd_views<true, true>(a, grid, deg, s);  // an orthographic view: the ORTHO instantiation of CAM
 	else if (cam) project_bwd_views<true, false>(a, grid, deg, s);
 	else project_bwd_views<false, false>(a, grid, deg, s);
 }
 
-template <bool CAM, bool ORTHO>
+template <bool CAM, bool ORTHO, bool FISH = false>
 static void project_bwd_clouds(const ProjectBwdCloudsArgs& a, int grid, int deg, cudaStream_t s)
 {
 	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
 	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
 	if (a.antialias) {
-		if (deg <= 1) project_bwd_clouds_kernel<12, 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
-		else project_bwd_clouds_kernel<48, 3, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_clouds_kernel<12, 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+		else project_bwd_clouds_kernel<48, 3, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
-	if (deg <= 1) project_bwd_clouds_kernel<12, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_clouds_kernel<27, 4, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_clouds_kernel<48, 3, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	if (deg <= 1) project_bwd_clouds_kernel<12, 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_clouds_kernel<27, FISH ? 3 : 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+	else project_bwd_clouds_kernel<48, 3, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
@@ -575,7 +624,8 @@ void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 	const int deg = sh ? a.D : 0;
 	bool cam = false;
 	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (a.ortho) project_bwd_clouds<true, true>(a, grid, deg, s);
+	if (a.fisheye) project_bwd_clouds<true, true, true>(a, grid, deg, s);
+	else if (a.ortho) project_bwd_clouds<true, true>(a, grid, deg, s);
 	else if (cam) project_bwd_clouds<true, false>(a, grid, deg, s);
 	else project_bwd_clouds<false, false>(a, grid, deg, s);
 }

@@ -300,10 +300,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         alpha = med_depth = med_id = normal = None
         if return_normal and (cov3Ds_precomp is not None and cov3Ds_precomp.numel() != 0):
             raise ValueError("return_normal needs scales and rotations: a precomputed covariance has no axis to take a normal from")
-        orth = bool(getattr(s, "orthographic", False))
+        orth = bool(getattr(s, "orthographic", False)) or getattr(s, "fisheye", None) is not None
         ctx.orthographic = orth
         if (return_alpha or return_median or return_normal or aa or orth or ctx.camera) and views_path:
-            # the alpha plane, the median planes, the anti-aliased and orthographic projections and the camera gradients exist on
+            # the alpha plane, the median planes, the anti-aliased, orthographic and fisheye projections and the camera gradients exist on
             # the multi-view entry points only: debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
@@ -473,16 +473,24 @@ class GaussianRasterizationSettings(_Settings):
     the settings still unpack into the reference's own 13-field NamedTuple, and `_fields` is the reference's.
     `orthographic` (default False; keyword, or positional after antialiasing) is an attribute in the same way: True makes the
     view orthographic, with tanfovx / tanfovy its half-width and half-height in view-space units and projmatrix an
-    orthographic matrix (cameras.projection_orthographic; include/mgs_rasterizer.h, mgs_forward_views_ortho)."""
+    orthographic matrix (cameras.projection_orthographic; include/mgs_rasterizer.h, mgs_forward_views_ortho).
+    `fisheye` (default None; keyword, or positional after orthographic) is an attribute in the same way: the view's
+    Kannala-Brandt parameters (cx, cy, k1, k2, k3, k4, theta_max), or a dict with those keys, make it a fisheye view, with
+    tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (fx, fy in pixels per radian; include/mgs_rasterizer.h,
+    mgs_forward_views_fisheye; cameras.build_fisheye_cameras).  It cannot be combined with orthographic=True."""
     antialiasing = False
     orthographic = False
+    fisheye = None
 
     def __new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix, sh_degree, campos,
-                prefiltered, debug, include_feature, antialiasing=False, orthographic=False):
+                prefiltered, debug, include_feature, antialiasing=False, orthographic=False, fisheye=None):
         self = super().__new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix,
                                sh_degree, campos, prefiltered, debug, include_feature)
         self.antialiasing = bool(antialiasing)
         self.orthographic = bool(orthographic)
+        self.fisheye = _fisheye_params(fisheye)
+        if self.orthographic and self.fisheye is not None:
+            raise ValueError("a view cannot be both orthographic and fisheye")
         return self
 
     @classmethod
@@ -492,10 +500,25 @@ class GaussianRasterizationSettings(_Settings):
     def _replace(self, **kw):
         aa = kw.pop("antialiasing", self.antialiasing)
         orth = kw.pop("orthographic", self.orthographic)
-        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth)
+        fe = kw.pop("fisheye", self.fisheye)
+        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth, fisheye=fe)
 
     def __repr__(self):
-        return super().__repr__()[:-1] + f", antialiasing={self.antialiasing}, orthographic={self.orthographic})"
+        return super().__repr__()[:-1] + (f", antialiasing={self.antialiasing}, orthographic={self.orthographic}, "
+                                          f"fisheye={self.fisheye})")
+
+
+FISHEYE_KEYS = ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")
+
+
+def _fisheye_params(x):
+    """A view's fisheye parameters as a tuple of 7 floats (FISHEYE_KEYS order) from such a sequence or a dict, or None"""
+    if x is None:
+        return None
+    vals = [x[k] for k in FISHEYE_KEYS] if isinstance(x, dict) else list(x)
+    if len(vals) != len(FISHEYE_KEYS):
+        raise ValueError(f"fisheye: expected {FISHEYE_KEYS}, got {x!r}")
+    return tuple(float(v) for v in vals)
 
 
 class GaussianRasterizer(nn.Module):
@@ -653,22 +676,40 @@ def _ortho_flags(views, ortho=None):
     return (ctypes.c_int * len(flags))(*flags) if any(flags) else None
 
 
+def _fisheye_array(views, fisheye=None):
+    """Per-view fisheye parameters: `fisheye` (V entries, each None or parameters) when given, else each view's `fisheye`
+    attribute; a ctypes ViewFisheye array for the _fisheye calls, or None when no view is fisheye."""
+    fe = [_fisheye_params(f) for f in fisheye] if fisheye is not None else [getattr(s, "fisheye", None) for s in views]
+    if len(fe) != len(views):
+        raise ValueError(f"fisheye: expected {len(views)} entries, got {len(fe)}")
+    if all(f is None for f in fe):
+        return None
+    arr = (_b.ViewFisheye * len(fe))()
+    for v, f in enumerate(fe):
+        if f is not None:
+            arr[v].fisheye = 1
+            for k, x in zip(FISHEYE_KEYS, f):
+                setattr(arr[v], k, x)
+    return arr
+
+
 def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug,
-               ortho=None):
+               ortho=None, fisheye=None):
     """First call for a (cloud size, image size): one projection + scan per view with a host read of the instance count
     (the reference does this on EVERY call), only to seed the capacity table.  An orthographic view (`ortho`: the views'
     flags, or None) is counted by a weight-only lift with one binning slot, whose status holds the full count: the
     single-view mgs_forward_begin has no camera model, and the lift is the cheapest call that takes one.  Its weights are
-    discarded."""
+    discarded.  A fisheye view (`fisheye`: the views' ViewFisheye array, or None) is counted the same way."""
     counts = torch.zeros(len(views), dtype=torch.int32).pin_memory()
     st = torch.cuda.current_stream(dev)
     keep, ortho_status = [], {}
     for v, s in enumerate(views):
         if keys[v] in _CAPACITY:
             continue
-        if ortho is not None and ortho[v]:
+        fe = fisheye[v] if fisheye is not None and fisheye[v].fisheye else None
+        if (ortho is not None and ortho[v]) or fe is not None:
             ortho_status[v], k = _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier,
-                                              cov3D_precomp, debug, st)
+                                              cov3D_precomp, debug, st, fe)
             keep.append(k)
             continue
         H, W = int(s.image_height), int(s.image_width)
@@ -687,9 +728,10 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
             _CAPACITY[keys[v]] = _round_capacity(n * 1.25 + 4096)
 
 
-def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug, st):
-    """Enqueues orthographic view `s`'s projection and binning on `st` with one binning slot.  Returns its pinned status
-    {instance count, overflow}, valid once `st` is synchronised, and what must stay alive until then."""
+def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug, st, fisheye=None):
+    """Enqueues orthographic view `s`'s projection and binning on `st` with one binning slot, or fisheye view `s`'s with
+    `fisheye` its ViewFisheye entry.  Returns its pinned status {instance count, overflow}, valid once `st` is synchronised,
+    and what must stay alive until then."""
     H, W = int(s.image_height), int(s.image_width)
     gbytes, ibytes, _ = _state_sizes(L, P, W, H)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
@@ -706,17 +748,20 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
     w[0].tan_fovx, w[0].tan_fovy, w[0].width, w[0].height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
     w[0].geometry_state, w[0].binning_state, w[0].image_state, w[0].binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), 1
     w[0].radii, w[0].status, w[0].stream = radii.data_ptr(), status.data_ptr(), st.cuda_stream
-    _b.check(L.mgs_lift_views_ortho(1, w, None, 0, _intrinsics_array(tf, None) if tf is not None else None, (ctypes.c_int * 1)(1),
-                                    P, 0, 0, 0, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier),
-                                    _ptr(rotations), _ptr(cov3D_precomp), None, _ptr(weight), int(bool(debug)), st.cuda_stream),
-             "mgs_lift_views_ortho")
+    iarr = _intrinsics_array(tf, None) if tf is not None else None
+    rest = (P, 0, 0, 0, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
+            _ptr(cov3D_precomp), None, _ptr(weight), int(bool(debug)), st.cuda_stream)
+    if fisheye is not None:
+        _b.check(L.mgs_lift_views_fisheye(1, w, None, 0, iarr, None, (_b.ViewFisheye * 1)(fisheye), *rest), "mgs_lift_views_fisheye")
+    else:
+        _b.check(L.mgs_lift_views_ortho(1, w, None, 0, iarr, (ctypes.c_int * 1)(1), *rest), "mgs_lift_views_ortho")
     return status, (geom, img, binb, radii, weight, vm, pm, tf, colors)
 
 
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False, return_normal=False, ortho=None):
+                        return_median=False, return_normal=False, ortho=None, fisheye=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -741,7 +786,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     surface-normal plane [3,H,W] to every ViewOut (C ABI mgs_view_normal; out_buffers[6] [V,3,H,W] when given); it needs scales
     and rotations, and cannot be combined with `depth_mask`.  `ortho` (V flags) marks the orthographic views; by default each
     view's `orthographic` attribute does.  With any orthographic view the call is mgs_forward_views_ortho; pass the same
-    flags (or views) to the backward."""
+    flags (or views) to the backward.  `fisheye` (V entries, each None or a view's fisheye parameters, as the settings'
+    `fisheye` attribute) marks the fisheye views, by default each view's `fisheye` attribute; with any fisheye view the call
+    is mgs_forward_views_fisheye."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -755,6 +802,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
     oarr = _ortho_flags(views, ortho)
+    farr = _fisheye_array(views, fisheye)
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]  # a single view needs no side stream
     di = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -768,7 +816,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call) or pass `capacities`")
             _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug, oarr)
+                       debug, oarr, farr)
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
@@ -794,7 +842,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if oarr is not None:
+        if farr is not None:
+            _b.check(L.mgs_forward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                 *rest), "mgs_forward_views_fisheye")
+        elif oarr is not None:
             _b.check(L.mgs_forward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
                      "mgs_forward_views_ortho")
@@ -824,11 +876,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
 
 
 def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, maps, antialiasing=False,
-                   tan_fov=None, debug=False, ortho=None):
+                   tan_fov=None, debug=False, ortho=None, fisheye=None):
     """Lift one 2D map per view onto the Gaussians (C ABI mgs_lift_views): lifted [P,C] = sum over the views and pixels of
     the forward blend's weights w = alpha T times the map, weight [P] = the sum of the weights.  `maps`: [V,C,H,W] or a
     sequence of V [C,H,W] fp32 tensors on the cloud's device (each view's own H, W), or None for weight only.  `views`,
-    `antialiasing`, `tan_fov` and `ortho` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with an orthographic view); the binning state is sized from the same capacity table (a
+    `antialiasing`, `tan_fov`, `ortho` and `fisheye` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with an orthographic
+    view, mgs_lift_views_fisheye with a fisheye one); the binning state is sized from the same capacity table (a
     steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
     needs colours, which the lift never reads: a zero [P,3] buffer stands in for them."""
     L = _b.lib()
@@ -841,6 +894,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
     means3D, opacity, scales, rotations, cov3D_precomp = (_prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp))
     V = len(views)
     oarr = _ortho_flags(views, ortho)
+    farr = _fisheye_array(views, fisheye)
     C = int(maps[0].shape[0]) if maps is not None else 0
     colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
     main = torch.cuda.current_stream(dev)
@@ -856,7 +910,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
                 raise RuntimeError("lift the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call)")
             _calibrate(L, views, keys, dev, P, 0, 0, means3D, None, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug, oarr)
+                       debug, oarr, farr)
         arr = (_b.View * V)()
         larr = (_b.ViewLift * V)()
         status = _status_slots(V)
@@ -890,7 +944,9 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         iarr = _intrinsics_array(tf, None) if tf is not None else None
         rest = (P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
                 _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight), int(bool(debug)), main.cuda_stream)
-        if oarr is not None:
+        if farr is not None:
+            _b.check(L.mgs_lift_views_fisheye(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, *rest), "mgs_lift_views_fisheye")
+        elif oarr is not None:
             _b.check(L.mgs_lift_views_ortho(V, arr, larr, int(bool(antialiasing)), iarr, oarr, *rest), "mgs_lift_views_ortho")
         else:
             _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), iarr, *rest), "mgs_lift_views")
@@ -1031,7 +1087,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
                                  ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
-                                 grads_normal=None, normals=None, ortho=None):
+                                 grads_normal=None, normals=None, ortho=None, fisheye=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -1056,7 +1112,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     the id planes that forward returned (C ABI mgs_backward_views_median).  `grads_normal` (per view [3,H,W] or None):
     cotangents of the normal planes of a `return_normal` forward, with `normals` (per view [3,H,W]) the planes that forward
     returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
-    forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho."""
+    forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho.
+    `fisheye`: as given to the forward (by default the views' `fisheye` attributes); with a fisheye view the call is
+    mgs_backward_views_fisheye."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1066,6 +1124,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
     oarr = _ortho_flags(views, ortho)
+    farr = _fisheye_array(views, fisheye)
     main = torch.cuda.current_stream(dev)
     opts = dict(dtype=torch.float32, device=dev)
     acc = accumulate_into or {}
@@ -1127,7 +1186,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if oarr is not None:
+            if farr is not None:
+                _b.check(L.mgs_backward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
+                                                      farr, *rest), "mgs_backward_views_fisheye")
+            elif oarr is not None:
                 _b.check(L.mgs_backward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
                                                     *rest), "mgs_backward_views_ortho")
             elif narr is not None:
@@ -1286,7 +1348,9 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
     mgs_forward_clouds_median).  `return_normal` appends, last, every view's normal plane [3,H,W], as in rasterize_views_raw
     (C ABI mgs_forward_clouds_normal).  A cloud's optional "ortho" (V_b flags; by default its views' `orthographic`
-    attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry."""
+    attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry.  A cloud's
+    optional "fisheye" (V_b entries, each None or parameters; by default its views' `fisheye` attributes) marks its fisheye
+    views (C ABI mgs_forward_clouds_fisheye), likewise."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -1312,7 +1376,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                     raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is "
                                        "learned from an eager call) or pass `capacities`")
                 _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
-                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug, _ortho_flags(c["views"], c.get("ortho")))
+                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug, _ortho_flags(c["views"], c.get("ortho")),
+                           _fisheye_array(c["views"], c.get("fisheye")))
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
@@ -1347,8 +1412,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        oarr = _clouds_ortho(clouds)
-        if oarr is not None:
+        oarr, farr = _clouds_ortho(clouds), _clouds_fisheye(clouds)
+        if farr is not None:
+            _b.check(L.mgs_forward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                  *rest), "mgs_forward_clouds_fisheye")
+        elif oarr is not None:
             _b.check(L.mgs_forward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
                      "mgs_forward_clouds_ortho")
@@ -1386,6 +1455,13 @@ def _clouds_ortho(clouds):
     return (ctypes.c_int * len(flags))(*flags) if any(flags) else None
 
 
+def _clouds_fisheye(clouds):
+    """The _fisheye calls' ViewFisheye array over every view of the clouds in order, or None when no view is fisheye"""
+    fe = [f for c in clouds for f in ([_fisheye_params(x) for x in c["fisheye"]] if c.get("fisheye") is not None
+                                      else [getattr(s, "fisheye", None) for s in c["views"]])]
+    return _fisheye_array([None] * len(fe), fe)
+
+
 def _clouds_fov(clouds, dev):
     """[V,2] device field of view of every view of the clouds in order, or None when no cloud has one (the clouds without
     one contribute their host floats)"""
@@ -1415,7 +1491,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     int32 the id planes that forward returned (C ABI mgs_backward_clouds_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
     cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
     mgs_backward_clouds_normal).  Clouds with an orthographic view (see rasterize_clouds_raw) make the call
-    mgs_backward_clouds_ortho."""
+    mgs_backward_clouds_ortho, and clouds with a fisheye view mgs_backward_clouds_fisheye."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1496,8 +1572,12 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        oarr = _clouds_ortho(clouds)
-        if oarr is not None:
+        oarr, farr = _clouds_ortho(clouds), _clouds_fisheye(clouds)
+        if farr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
+                                                   narr, oarr, farr, *rest), "mgs_backward_clouds_fisheye")
+        elif oarr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
                                                  narr, oarr, *rest), "mgs_backward_clouds_ortho")
