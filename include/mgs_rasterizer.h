@@ -1066,6 +1066,77 @@ int mgs_lift_views_fisheye(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
+/*
+ * Distorted-pinhole views (OpenCV's cv::projectPoints with the 8-coefficient D = (k1, k2, p1, p2, k3, k4, k5, k6);
+ * COLMAP's OPENCV / FULL_OPENCV).  The _distorted calls are the _fisheye calls with one more argument, `distortion`: a host
+ * array of one mgs_view_distortion per view (V entries, or view_offsets[B] for clouds), or NULL for none.  An entry with
+ * distorted = 0 is ignored (the view's model is then given by its ortho flag and fisheye entry).  The _fisheye calls are the
+ * _distorted calls with distortion = NULL.  One call may mix all four models, also among the views of one cloud.
+ * Definition, for a distorted view, with t = Rv p + tv as for every view:
+ *   - x = t.x / t.z, y = t.y / t.z, r2 = x^2 + y^2,
+ *     R = (1 + k1 r2 + k2 r2^2 + k3 r2^3) / (1 + k4 r2 + k5 r2^2 + k6 r2^3),
+ *     xd = x R + 2 p1 x y + p2 (r2 + 2 x^2),   yd = y R + p1 (r2 + 2 y^2) + 2 p2 x y.
+ *   - Screen mean: u = fx xd + cx, v = fy yd + cy.  (cx, cy) are in the blend's pixel coordinates, where pixel (i, j) has its
+ *     centre at (i, j), as in OpenCV and as for fisheye views.  projmatrix is not read (its gradient is zero).
+ *   - fx = W / (2 tan_fovx), fy = H / (2 tan_fovy), as for every view: tan_fovx holds W / (2 fx).  mgs_view_intrinsics.tan_fov
+ *     and dL_dtan_fov work unchanged; dL_dtan_fov is then the gradient of a learnable focal length.
+ *   - Jacobian of (u, v) w.r.t. t, exact at the mean: J = diag(fx, fy) Dd [[1/t.z, 0, -x/t.z], [0, 1/t.z, -y/t.z]], with
+ *     Dd = d(xd, yd) / d(x, y) = [[R + 2 x^2 R' + 2 p1 y + 6 p2 x, 2 x y R' + 2 p1 x + 2 p2 y],
+ *                                 [2 x y R' + 2 p1 x + 2 p2 y, R + 2 y^2 R' + 6 p1 y + 2 p2 x]],  R' = dR / dr2.  No frustum clamp.
+ *   - Cull, like a mean behind the near plane (radius 0): r2 > r_max^2 (past the first fold of the radial map, where far-off
+ *     points fold back into the image), or det Dd <= 0 (a local fold, which the tangential terms can add).  Every kept
+ *     Gaussian then has a finite EWA conic.
+ *   - Depth is t.z (sort key and depth plane); the SH view direction and the normal plane's facing test use p - cam_pos.
+ *     Every stage after the projection is unchanged.
+ *   - Backward: (du, dv) = (dm0 / (W / 2), dm1 / (H / 2)) is the pixel-space mean's cotangent (dm, the blend's dL/dmean2D,
+ *     is w.r.t. ndc, as for fisheye views).  M = J Rv; dL/dt = J^T (du, dv) + (dL/dJ = dL/dM Rv^T contracted with dJ/dt, which
+ *     takes Dd's derivatives) + the depth cotangent on t.z.  Camera gradients: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt,
+ *     dL/dprojmatrix = 0, dL/dcampos as for a pinhole view (SH), dL/dtan_fovx = -(du (u - cx) + sum_j dJ0j J0j) / tan_fovx and
+ *     likewise for y.  The principal point, the coefficients and r_max receive no gradient.
+ * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: a flag other than 0 or 1; a distorted view that is also
+ * orthographic or fisheye; a non-finite cx, cy or coefficient; r_max <= 0 or NaN (r_max = +inf is allowed).
+ */
+typedef struct mgs_view_distortion {
+	int distorted;                  /* 1: a distorted-pinhole view; 0: the entry is ignored */
+	float cx, cy;                   /* principal point in pixels (pixel centres at integers) */
+	float k1, k2, p1, p2, k3, k4, k5, k6;  /* OpenCV's D, in its order; 4 or 5 coefficients: the rest 0 */
+	float r_max;                    /* cull: sqrt(x^2 + y^2) of the mean above it, > 0 or +inf */
+} mgs_view_distortion;
+int mgs_forward_views_distorted(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_views_distorted(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
+int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream);
+int mgs_lift_views_distorted(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -70,6 +70,12 @@ class ViewFisheye(C.Structure):
     _fields_ = [("fisheye", C.c_int)] + [(n, C.c_float) for n in ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")]
 
 
+class ViewDistortion(C.Structure):
+    """mirror of `mgs_view_distortion` (include/mgs_rasterizer.h): one view's OpenCV distortion parameters"""
+    _fields_ = [("distorted", C.c_int)] + \
+        [(n, C.c_float) for n in ("cx", "cy", "k1", "k2", "p1", "p2", "k3", "k4", "k5", "k6", "r_max")]
+
+
 class ViewLift(C.Structure):
     """mirror of `mgs_view_lift` (include/mgs_rasterizer.h): the 2D map [C,H,W] one view lifts onto the Gaussians"""
     _fields_ = [("map", C.c_void_p)]
@@ -191,6 +197,11 @@ def lib():
         getattr(L, fish).restype = C.c_int
         getattr(L, fish).argtypes = getattr(L, orth).argtypes[:len(getattr(L, orth).argtypes) - len(at) + k] + \
             [C.POINTER(ViewFisheye)] + at[k:]
+        # ... and the distortion parameters (one ViewDistortion per view, or NULL) after the fisheye parameters
+        dist = name.replace("_views", "_views_distorted").replace("_clouds", "_clouds_distorted")
+        getattr(L, dist).restype = C.c_int
+        getattr(L, dist).argtypes = getattr(L, fish).argtypes[:len(getattr(L, fish).argtypes) - len(at) + k] + \
+            [C.POINTER(ViewDistortion)] + at[k:]
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
                                  i, i, i, i,                        # P D M C
@@ -202,6 +213,9 @@ def lib():
     L.mgs_lift_views_fisheye.restype = C.c_int
     L.mgs_lift_views_fisheye.argtypes = L.mgs_lift_views_ortho.argtypes[:6] + [C.POINTER(ViewFisheye)] + \
         L.mgs_lift_views_ortho.argtypes[6:]
+    L.mgs_lift_views_distorted.restype = C.c_int
+    L.mgs_lift_views_distorted.argtypes = L.mgs_lift_views_fisheye.argtypes[:7] + [C.POINTER(ViewDistortion)] + \
+        L.mgs_lift_views_fisheye.argtypes[7:]
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -252,6 +266,8 @@ EXPORTED_SYMBOLS = (
     "mgs_lift_views_ortho",
     "mgs_forward_views_fisheye", "mgs_backward_views_fisheye", "mgs_forward_clouds_fisheye", "mgs_backward_clouds_fisheye",
     "mgs_lift_views_fisheye",
+    "mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
+    "mgs_backward_clouds_distorted", "mgs_lift_views_distorted",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -390,11 +390,29 @@ static int check_fisheye(const mgs_view_fisheye* fe, const int* ortho, int V)
 	return 0;
 }
 
+// view v's distortion parameters (dc: one entry per view, or NULL), or NULL for a view without lens distortion
+static const mgs_view_distortion* distortion_of(const mgs_view_distortion* dc, int v) { return dc && dc[v].distorted ? dc + v : nullptr; }
+static int check_distortion(const mgs_view_distortion* dc, const int* ortho, const mgs_view_fisheye* fe, int V)
+{
+	for (int v = 0; dc && v < V; v++) {
+		const mgs_view_distortion& d = dc[v];
+		if (d.distorted != 0 && d.distorted != 1) return fail(MGS_ERR_INVALID_ARG, "distortion: every flag must be 0 or 1");
+		if (!d.distorted) continue;
+		if (ortho_of(ortho, v) || fisheye_of(fe, v))
+			return fail(MGS_ERR_INVALID_ARG, "distortion: a distorted view cannot also be orthographic or fisheye");
+		const float x[10] = { d.cx, d.cy, d.k1, d.k2, d.p1, d.p2, d.k3, d.k4, d.k5, d.k6 };
+		for (float xi : x)
+			if (!std::isfinite(xi)) return fail(MGS_ERR_INVALID_ARG, "distortion: cx, cy and the coefficients must be finite");
+		if (!(d.r_max > 0.f)) return fail(MGS_ERR_INVALID_ARG, "distortion: r_max must be > 0 (+inf for no fold)");
+	}
+	return 0;
+}
+
 // per-Gaussian projection, depth order and instance offsets; the instance count ends up in geom.point_offsets[P - 1].
 // tan_fov: the view's device field of view, or NULL; ortho: 1 for an orthographic view; fe: a fisheye view's parameters,
-// or NULL
+// or NULL; dc: a distorted view's parameters, or NULL
 static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, int ortho, int debug,
-	const mgs_view_fisheye* fe = nullptr)
+	const mgs_view_fisheye* fe = nullptr, const mgs_view_distortion* dc = nullptr)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const ViewState s = carve_view(w, c.P);
@@ -416,6 +434,12 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_f
 	if (fe) {
 		pa.fisheye = 1;
 		pa.fe_cx = fe->cx; pa.fe_cy = fe->cy; pa.fe_k = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 }; pa.fe_theta_max = fe->theta_max;
+	}
+	if (dc) {
+		pa.distorted = 1;
+		pa.dc_cx = dc->cx; pa.dc_cy = dc->cy;
+		pa.dc_k = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
+		pa.dc_r2_max = dc->r_max * dc->r_max;  // +inf stays +inf
 	}
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
@@ -717,13 +741,20 @@ static void set_fisheye(const mgs_view_fisheye* fe, int u, uint16_t& mask, Fishe
 	mask |= (uint16_t)(1u << u);
 	k[u] = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 };
 }
+// launch view u of a backward: a distorted view sets bit u of the mask and its coefficients
+static void set_distortion(const mgs_view_distortion* dc, int u, uint16_t& mask, DistK* k)
+{
+	if (!dc) return;
+	mask |= (uint16_t)(1u << u);
+	k[u] = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
+}
 
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
 // does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
 	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
-	const mgs_view_normal* nm, const int* ortho, const mgs_view_fisheye* fe, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_normal* nm, const int* ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join)
 {
@@ -773,6 +804,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
 		for (int u = 0; u < pb.V; u++) pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << u);
 		for (int u = 0; u < pb.V; u++) set_fisheye(fisheye_of(fe, v0 + u), u, pb.fisheye, pb.fe_k);
+		for (int u = 0; u < pb.V; u++) set_distortion(distortion_of(dc, v0 + u), u, pb.distorted, pb.dc_k);
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
@@ -939,7 +971,7 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -1058,11 +1090,26 @@ int mgs_forward_views_fisheye(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_distorted(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye,
+		nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations,
+		cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_distorted(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
 	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours");
@@ -1095,7 +1142,8 @@ int mgs_forward_views_fisheye(
 			if (rc < 0) return rc;
 		}
 		for (int v = 0; v < V; v++) {
-			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v))
+			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
+					distortion_of(distortion, v))
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 					median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
@@ -1137,10 +1185,23 @@ int mgs_lift_views_fisheye(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_lifted, float* out_weight, int debug, void* join_stream)
 {
+	return mgs_lift_views_distorted(V, views, lift, antialiasing, intr, ortho, fisheye, nullptr, P, D, M, C, means3D, shs,
+		colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, out_lifted, out_weight, debug, join_stream);
+}
+
+int mgs_lift_views_distorted(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_lifted, float* out_weight, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "map channel count must be in [0, " MGS_STR(MGS_MAX_FEATURE_CHANNELS) "]");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
@@ -1169,7 +1230,8 @@ int mgs_lift_views_fisheye(
 	for (int phase = 0; phase < 3; phase++) {
 		for (int v = 0; v < V; v++) {
 			const mgs_view& w = views[v];
-			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v));
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
+					distortion_of(distortion, v));
 			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
 			else {
 				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
@@ -1336,11 +1398,28 @@ int mgs_backward_views_fisheye(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_distorted(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho,
+		fisheye, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp,
+		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages,
+		debug, join_stream);
+}
+
+int mgs_backward_views_distorted(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !dL_dmean3D || !dL_dopacity) return fail(MGS_ERR_INVALID_ARG, "means3D, dL_dmean3D and dL_dopacity are required");
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -1356,7 +1435,7 @@ int mgs_backward_views_fisheye(
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, fisheye, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, fisheye, distortion, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
 
@@ -1437,12 +1516,22 @@ int mgs_forward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_o
 	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
 	const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_distorted(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median,
+		normal, ortho, fisheye, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1470,7 +1559,8 @@ int mgs_forward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_o
 		for (int b = 0; b < B; b++) {
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v))
+				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
+					distortion_of(distortion, v))
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 						median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
@@ -1570,11 +1660,22 @@ int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_
 	const int* ortho, const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int accumulate, int debug,
 	void* join_stream)
 {
+	return mgs_backward_clouds_distorted(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median,
+		normal, ortho, fisheye, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int accumulate, int debug,
+	void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1621,7 +1722,7 @@ int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_
 	// spans launches, and its later launches add to what the earlier ones wrote
 	const cudaStream_t st = join;
 	// a view's camera rows are summed by the reduce behind the one launch that holds the view
-	ProjectBwdCloudsArgs pb{};
+	ProjectBwdCloudsDistArgs pb{};
 	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
 	CamReduceArgs cr{};
 	cr.accumulate = accumulate ? 1 : 0;
@@ -1630,7 +1731,7 @@ int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_
 		if (pb.B == 0) return 0;
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
-		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0; pb.fisheye = 0;
+		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0; pb.fisheye = 0; pb.distorted = 0;
 		for (float*& r : pb.cam_rows) r = nullptr;
 		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
 		return 0;
@@ -1658,6 +1759,7 @@ int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_
 				camera_view(cam, intr, views[v0 + u], v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
 				pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << (nv + u));
 				set_fisheye(fisheye_of(fisheye, v0 + u), nv + u, pb.fisheye, pb.fe_k);
+				set_distortion(distortion_of(distortion, v0 + u), nv + u, pb.distorted, pb.dc_k);
 			}
 			nv += n;
 		}

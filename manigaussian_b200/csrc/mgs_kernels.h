@@ -4,6 +4,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "distortion.cuh"
 #include "fisheye.cuh"
 
 namespace mgs {
@@ -50,6 +51,13 @@ struct ProjectFwdArgs {
 	float fe_cx, fe_cy;
 	FisheyeK fe_k;
 	float fe_theta_max;
+	// 1: an OpenCV distorted-pinhole view (picks the DISTORTED instantiation; projmatrix is not read): principal point,
+	// coefficients and the squared radius cull of include/mgs_rasterizer.h's mgs_view_distortion.  Behind the fisheye members
+	// for the same reason.
+	int distorted;
+	float dc_cx, dc_cy;
+	DistK dc_k;
+	float dc_r2_max;
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -108,6 +116,10 @@ struct ProjectBwdViewsArgs {
 	// all three models) read them; the launcher picks them when any bit is set.  Behind ortho for the same reason.
 	uint16_t fisheye;
 	FisheyeK fe_k[MAX_BWD_VIEWS];
+	// bit u: view u is a distorted-pinhole view with coefficients dc_k[u].  Only the DIST instantiations (of FISH, ORTHO and
+	// CAM: they serve all four models) read them; the launcher picks them when any bit is set.  Behind fe_k for the same reason.
+	uint16_t distorted;
+	DistK dc_k[MAX_BWD_VIEWS];
 };
 // the 27 camera terms one CTA writes per view into its camera rows: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1,
 // 3}] at 12 + 3c + {0, 1, 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.  The kernel
@@ -142,9 +154,16 @@ struct ProjectBwdCloudsArgs {
 	uint16_t fisheye;                              // bit u: view u of the launch is a fisheye view, as in ProjectBwdViewsArgs
 	FisheyeK fe_k[MAX_BWD_VIEWS];                  // per view of the launch, as in ProjectBwdViewsArgs
 };
-static_assert(MAX_BWD_VIEWS <= 16, "the orthographic and fisheye view masks have 16 bits");
+// the clouds launch with distorted-pinhole views: the DIST instantiations take this larger block (CUDA 12.1+ on Volta and
+// later accept kernel parameters up to 32,764 bytes), so every other clouds kernel keeps its parameter block under 4 KB
+struct ProjectBwdCloudsDistArgs : ProjectBwdCloudsArgs {
+	uint16_t distorted;                            // bit u: view u of the launch is a distorted-pinhole view
+	DistK dc_k[MAX_BWD_VIEWS];                     // per view of the launch, as in ProjectBwdViewsArgs
+};
+static_assert(MAX_BWD_VIEWS <= 16, "the orthographic, fisheye and distorted view masks have 16 bits");
 static_assert(sizeof(ProjectBwdViewsArgs) <= 4096, "kernel parameters are limited to 4 KB");
 static_assert(sizeof(ProjectBwdCloudsArgs) <= 4096, "kernel parameters are limited to 4 KB");
+static_assert(sizeof(ProjectBwdCloudsDistArgs) <= 32764, "large kernel parameters are limited to 32,764 bytes");
 // the second half of the camera gradients: view u's rows summed in row order into its 35 outputs (each nullable), written
 // (accumulate = 0) or added (1)
 struct CamReduceView {
@@ -287,7 +306,7 @@ void launch_activate_bwd(ActivateArgs a, cudaStream_t s);
 
 void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s);
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s);
-void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s);
+void launch_project_bwd_clouds(ProjectBwdCloudsDistArgs a, cudaStream_t s);
 void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s);
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s);
 

@@ -41,10 +41,12 @@ struct Cov2DTerms {
 // Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196).
 // MODEL_ORTHO: the orthographic Jacobian J = [[fx, 0, 0], [0, fy, 0]] (fx, fy in pixels per view-space unit), with no frustum
 // clamp.  MODEL_FISHEYE: the Kannala-Brandt Jacobian from the radial terms fr of the unclamped t (fisheye.cuh), no clamp.
-constexpr int MODEL_PINHOLE = 0, MODEL_ORTHO = 1, MODEL_FISHEYE = 2;
+// MODEL_DISTORTED: J = diag(fx, fy) Dd [[1/z, 0, -x/z], [0, 1/z, -y/z]] from the distortion terms ds of the unclamped
+// (x, y) = t.xy / t.z (distortion.cuh), no clamp.
+constexpr int MODEL_PINHOLE = 0, MODEL_ORTHO = 1, MODEL_FISHEYE = 2, MODEL_DISTORTED = 3;
 template <int MODEL = MODEL_PINHOLE>
 __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, float fy, float tanx, float tany,
-	const float* cov3D, const float* vm, const FisheyeRadial* fr = nullptr)
+	const float* cov3D, const float* vm, const FisheyeRadial* fr = nullptr, const DistTerms* ds = nullptr)
 {
 	Cov2DTerms o;
 	V3 t = xform4x3(mean, vm);
@@ -57,6 +59,12 @@ __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, floa
 		J = m3(
 			fx * (fr->a + fr->c * t.x * t.x), fx * cxy, -fx * t.x * fr->g,
 			fy * cxy, fy * (fr->a + fr->c * t.y * t.y), -fy * t.y * fr->g,
+			0.f, 0.f, 0.f);
+	} else if constexpr (MODEL == MODEL_DISTORTED) {
+		const float iz = 1.0f / t.z, x = t.x * iz, y = t.y * iz;
+		J = m3(
+			fx * ds->d00 * iz, fx * ds->d01 * iz, -fx * (ds->d00 * x + ds->d01 * y) * iz,
+			fy * ds->d01 * iz, fy * ds->d11 * iz, -fy * (ds->d01 * x + ds->d11 * y) * iz,
 			0.f, 0.f, 0.f);
 	} else {
 		const float limx = 1.3f * tanx;
@@ -132,6 +140,9 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 // MODEL_FISHEYE: a Kannala-Brandt view (mgs_forward_views_fisheye): projmatrix is not read; the screen mean is
 // (fx a t.x + cx, fy a t.y + cy), J the map's Jacobian (fisheye.cuh), and a mean with theta > theta_max is culled like one
 // behind the near plane.  Everything after the covariance is the perspective path's.
+// MODEL_DISTORTED: an OpenCV distorted-pinhole view (mgs_forward_views_distorted): projmatrix is not read; the screen mean
+// is (fx xd + cx, fy yd + cy), J = diag(fx, fy) Dd (d(x, y) / dt) (distortion.cuh), and a mean past the first fold
+// (r2 > r2_max) or on a local fold (det Dd <= 0) is culled like one behind the near plane.
 template <bool AA, bool FOV, int MODEL>
 __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 {
@@ -148,7 +159,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 
 	V3 p_orig = { a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2] };
 	float p_proj_x = 0.f, p_proj_y = 0.f;
-	if constexpr (MODEL != MODEL_FISHEYE) {
+	if constexpr (MODEL != MODEL_FISHEYE && MODEL != MODEL_DISTORTED) {
 		float4 p_hom = xform4x4(p_orig, a.projmatrix);
 		float p_w = 1.0f / (p_hom.w + 0.0000001f);
 		p_proj_x = p_hom.x * p_w; p_proj_y = p_hom.y * p_w;
@@ -159,6 +170,12 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	if constexpr (MODEL == MODEL_FISHEYE) {
 		fr = fisheye_radial<false>(p_view.x, p_view.y, p_view.z, a.fe_k);
 		if (fr.theta > a.fe_theta_max) return;
+	}
+	DistTerms ds{};
+	if constexpr (MODEL == MODEL_DISTORTED) {
+		const float iz = 1.0f / p_view.z;
+		ds = distortion_terms<false>(p_view.x * iz, p_view.y * iz, a.dc_k);
+		if (ds.r2 > a.dc_r2_max || fmaf(-ds.d01, ds.d01, ds.d00 * ds.d11) <= 0.f) return;
 	}
 
 	const float* cov3D;
@@ -174,7 +191,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 		tanx = a.tan_fov[0]; tany = a.tan_fov[1];
 		fx = a.W / (2.0f * tanx); fy = a.H / (2.0f * tany);  // as api.cu forms focal_x / focal_y
 	}
-	Cov2DTerms ct = cov2d_terms<MODEL>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix, &fr);
+	Cov2DTerms ct = cov2d_terms<MODEL>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix, &fr, &ds);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
 	float det0 = 0.f;  // det of the screen-space covariance before the low-pass (AA only)
 	if (AA) det0 = fmaf(-cov.m[0][1], cov.m[0][1], cov.m[0][0] * cov.m[1][1]);  // explicit fma: rounding independent of contraction
@@ -194,6 +211,8 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	float px, py;
 	if constexpr (MODEL == MODEL_FISHEYE) {
 		px = fx * fr.a * p_view.x + a.fe_cx; py = fy * fr.a * p_view.y + a.fe_cy;
+	} else if constexpr (MODEL == MODEL_DISTORTED) {
+		px = fx * ds.xd + a.dc_cx; py = fy * ds.yd + a.dc_cy;
 	} else {
 		px = ndc2pix(p_proj_x, a.W); py = ndc2pix(p_proj_y, a.H);
 	}
@@ -261,7 +280,9 @@ void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0) return;
 	const int grid = ceil_div(a.P, 256);
-	if (a.fisheye) {
+	if (a.distorted) {
+		launch_project_fwd_model<MODEL_DISTORTED>(a, grid, s);
+	} else if (a.fisheye) {
 		launch_project_fwd_model<MODEL_FISHEYE>(a, grid, s);
 	} else if (a.ortho) {
 		launch_project_fwd_model<MODEL_ORTHO>(a, grid, s);

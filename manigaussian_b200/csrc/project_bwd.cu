@@ -21,6 +21,8 @@
 #include "mgs_common.cuh"
 #include "mgs_kernels.h"
 
+#include <type_traits>
+
 namespace mgs {
 
 namespace {
@@ -81,7 +83,13 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // dm1 / (H / 2)) its cotangent (dm, the blend's dL/dmean2D, is w.r.t. ndc), dL/dt gains J^T (du, dv) and the
 // projection-matrix terms are zero; all six entries of J move with t, dL/dt takes the contraction of dL/dJ with dJ/dt,
 // the camera terms take the full J^T Q, and dL/dtan_fovx = -(du (u - cx) + sum_j dJ0j J0j) / tan_fovx (y likewise).
-template <int NSH, bool AA, bool CAM, bool ORTHO, bool FISH, class Args>
+//
+// DIST (FISH, ORTHO and CAM only): bit v of a.distorted marks view v an OpenCV distorted-pinhole view with coefficients
+// a.dc_k[v] (distortion.cuh).  As for FISH, the screen mean (u, v) = (fx xd + cx, fy yd + cy) is in pixels and its cotangent is
+// (du, dv); J = F Dd P with F = diag(fx, fy), P = d(x, y) / dt = [[1/z, 0, -x/z], [0, 1/z, -y/z]].  With G = F dL/dJ,
+// dL/dJ : dJ/dt = (G P^T) : dDd/d(x, y) chained through P, plus (Dd G) : dP/dt (Dd is symmetric); J^T (du, dv) enters through
+// the same chain.  The camera terms and dL/dtan_fov are the fisheye ones with u - cx = fx xd.
+template <int NSH, bool AA, bool CAM, bool ORTHO, bool FISH, bool DIST, class Args>
 __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx_in, const bool in, float* cam_sm)
 {
 	const int idx = CAM && !in ? 0 : idx_in;
@@ -132,6 +140,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		// memory, never unmapped): the four loads of a view overlap instead of queueing behind the radius
 		const bool orv = ORTHO && ((a.ortho >> v) & 1u);  // view v is orthographic
 		const bool fev = FISH && ((a.fisheye >> v) & 1u);  // view v is a fisheye view
+		const bool dsv = DIST && ((a.distorted >> v) & 1u);  // view v is a distorted-pinhole view
 		const float4* gb = reinterpret_cast<const float4*>(w.gb + (size_t)idx * GB_STRIDE);
 		const float4 g0 = gb[0], g1 = gb[1], g2 = gb[2];
 		const uint8_t cl = sh ? w.clamped[idx] : (uint8_t)0;
@@ -173,8 +182,21 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			float m0[3], m1[3], u0[3], u1[3];
 			FisheyeRadial fr{};
 			float j01 = 0.f, j10 = 0.f, fj00 = 0.f, fj11 = 0.f, fj02 = 0.f, fj12 = 0.f;  // FISH: J
-			float du = 0.f, dv = 0.f;  // FISH: the cotangent of the pixel-space mean (u, v)
-			if (fev) {
+			float du = 0.f, dv = 0.f;  // FISH, DIST: the cotangent of the pixel-space mean (u, v)
+			DistTerms ds{};
+			float nx = 0.f, ny = 0.f;  // DIST: the normalised coordinates t.xy / t.z
+			if (dsv) {
+				du = dm[0] / (0.5f * a.intr[v].W); dv = dm[1] / (0.5f * a.intr[v].H);
+				nx = tx * iz; ny = ty * iz;
+				ds = distortion_terms<true>(nx, ny, a.dc_k[v]);
+				fj00 = fx * ds.d00 * iz; j01 = fx * ds.d01 * iz; fj02 = -fx * (ds.d00 * nx + ds.d01 * ny) * iz;
+				j10 = fy * ds.d01 * iz; fj11 = fy * ds.d11 * iz; fj12 = -fy * (ds.d01 * nx + ds.d11 * ny) * iz;
+#pragma unroll
+				for (int c = 0; c < 3; c++) {
+					m0[c] = fj00 * Rv[0][c] + j01 * Rv[1][c] + fj02 * Rv[2][c];
+					m1[c] = j10 * Rv[0][c] + fj11 * Rv[1][c] + fj12 * Rv[2][c];
+				}
+			} else if (fev) {
 				// dm is the blend's dL/dmean2D, the gradient w.r.t. ndc = (2 u + 1) / W - 1 (the reference's convention: the
 				// blend scales its pixel-space gradient by W / 2, H / 2); the fisheye mean is in pixels
 				du = dm[0] / (0.5f * a.intr[v].W); dv = dm[1] / (0.5f * a.intr[v].H);
@@ -235,7 +257,12 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			if constexpr (CAM) {
 				// dL/dtan_fov: fx = W / (2 tan_fovx) moves J00 = fx / tz and J02 = -fx cx / tz^2 (dfx / dtan_fovx = -fx / tan_fovx),
 				// and where the x clamp holds, cx = +-1.3 tan_fovx tz moves J02.  Likewise for y.
-				if (fev) {
+				if (dsv) {
+					// u - cx = fx xd and every entry of J's first row scale with fx
+					const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
+					cg[27] = -(du * fx * ds.xd + dJ00 * fj00 + dJ01 * j01 + dJ02 * fj02) / tanx;
+					cg[28] = -(dv * fy * ds.yd + dJ10 * j10 + dJ11 * fj11 + dJ12 * fj12) / tany;
+				} else if (fev) {
 					// u - cx = fx a t.x and every entry of J's first row scale with fx
 					const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
 					cg[27] = -(du * fx * fr.a * tx + dJ00 * fj00 + dJ01 * j01 + dJ02 * fj02) / tanx;
@@ -251,7 +278,21 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			}
 			const float iz3 = iz2 * iz;
 			float dt[3];
-			if (fev) {
+			if (dsv) {
+				// G = F dL/dJ; K = G P^T contracts with dDd/d(x, y), N = Dd G with dP/dt; (gx, gy) = dL/d(x, y), J^T (du, dv)
+				// included through F Dd
+				const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
+				const float G00 = fx * dJ00, G01 = fx * dJ01, G02 = fx * dJ02, G10 = fy * dJ10, G11 = fy * dJ11, G12 = fy * dJ12;
+				const float K00 = (G00 - nx * G02) * iz, Kx = (G01 - ny * G02 + G10 - nx * G12) * iz, K11 = (G11 - ny * G12) * iz;
+				const float eu = fx * du, ev = fy * dv;
+				const float gx = K00 * ds.hxxx + Kx * ds.hxxy + K11 * ds.hxyy + ds.d00 * eu + ds.d01 * ev;
+				const float gy = K00 * ds.hxxy + Kx * ds.hxyy + K11 * ds.hyyy + ds.d01 * eu + ds.d11 * ev;
+				const float N00 = ds.d00 * G00 + ds.d01 * G10, N02 = ds.d00 * G02 + ds.d01 * G12;
+				const float N11 = ds.d01 * G01 + ds.d11 * G11, N12 = ds.d01 * G02 + ds.d11 * G12;
+				dt[0] = (gx - N02 * iz) * iz;
+				dt[1] = (gy - N12 * iz) * iz;
+				dt[2] = (2.f * (N02 * nx + N12 * ny) - N00 - N11) * iz2 - (gx * nx + gy * ny) * iz + ddepth;
+			} else if (fev) {
 				// dL/dJ contracted with dJ/dt (fisheye.cuh: da/dx = c x, da/dz = -g, (dg/dr) / r = -cz), then J^T (du, dv)
 				const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
 				const float A = fx * dJ00, Bs = fx * dJ01 + fy * dJ10, Cc = fx * dJ02, Ee = fy * dJ11, Ff = fy * dJ12;
@@ -277,7 +318,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float hw = pm[3] * p[0] + pm[7] * p[1] + pm[11] * p[2] + pm[15];
 			const float iw = 1.0f / (hw + 0.0000001f);
 			const float kx = hx * iw * iw, ky = hy * iw * iw;
-			const float dmp[2] = { fev ? 0.f : dm[0], fev ? 0.f : dm[1] };  // the mean's path through projmatrix
+			const float dmp[2] = { fev || dsv ? 0.f : dm[0], fev || dsv ? 0.f : dm[1] };  // the mean's path through projmatrix
 #pragma unroll
 			for (int c = 0; c < 3; c++) {
 				gp[c] += Rv[0][c] * dt[0] + Rv[1][c] * dt[1] + Rv[2][c] * dt[2]
@@ -285,14 +326,15 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			}
 			if constexpr (CAM) {
 				// t = Rv p + tv and M = J Rv with J held: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt
-				const float j00 = fev ? fj00 : orv ? fx : fx * iz, j11 = fev ? fj11 : orv ? fy : fy * iz;
-				const float j02 = fev ? fj02 : orv ? 0.f : -fx * cx * iz2, j12 = fev ? fj12 : orv ? 0.f : -fy * cy * iz2;
+				const bool full = fev || dsv;  // J has all six entries
+				const float j00 = full ? fj00 : orv ? fx : fx * iz, j11 = full ? fj11 : orv ? fy : fy * iz;
+				const float j02 = full ? fj02 : orv ? 0.f : -fx * cx * iz2, j12 = full ? fj12 : orv ? 0.f : -fy * cy * iz2;
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
 					cg[3 * c] = dt[0] * p[c] + j00 * q0[c];
 					cg[3 * c + 1] = dt[1] * p[c] + j11 * q1[c];
 					cg[3 * c + 2] = dt[2] * p[c] + j02 * q0[c] + j12 * q1[c];
-					if (fev) { cg[3 * c] += j10 * q1[c]; cg[3 * c + 1] += j01 * q0[c]; }
+					if (full) { cg[3 * c] += j10 * q1[c]; cg[3 * c + 1] += j01 * q0[c]; }
 				}
 				cg[9] = dt[0]; cg[10] = dt[1]; cg[11] = dt[2];
 				// (hx, hy, hw) = P (p, 1): dL/dhx = dm0 iw, dL/dhy = dm1 iw, dL/dhw = -(dm0 kx + dm1 ky)
@@ -441,21 +483,23 @@ __device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* 
 	}
 }
 
-// FISH, ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before it, as
-// profiles and the coverage tests read them.  ORTHO is instantiated with CAM only, FISH with ORTHO and CAM only.
-template <int NSH, int MIN_BLOCKS, bool FISH, bool ORTHO, bool CAM, bool AA>
+// DIST, FISH, ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before
+// it, as profiles and the coverage tests read them.  ORTHO is instantiated with CAM only, FISH with ORTHO and CAM only, DIST
+// with FISH, ORTHO and CAM only.
+template <int NSH, int MIN_BLOCKS, bool DIST, bool FISH, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
 	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
 	static_assert(ORTHO || !FISH, "the fisheye backward is an ORTHO instantiation");
+	static_assert(FISH || !DIST, "the distorted backward is a FISH instantiation");
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if constexpr (CAM) {
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH>(a, idx, idx < a.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(a, idx, idx < a.P, cam_sm);
 		cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
 	} else {
 		if (idx >= a.P) return;
-		project_bwd_gaussian<NSH, AA, false, false, false>(a, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false, false>(a, idx, true, nullptr);
 	}
 }
 
@@ -476,15 +520,46 @@ struct CloudBwd {
 	unsigned ortho;                      // ORTHO only: bit v, view v of the cloud is orthographic
 	unsigned fisheye;                    // FISH only: bit v, view v of the cloud is a fisheye view
 	const FisheyeK* fe_k;                // FISH only: per view of the cloud
+	unsigned distorted;                  // DIST only: bit v, view v of the cloud is a distorted-pinhole view
+	const DistK* dc_k;                   // DIST only: per view of the cloud
 };
+// the parameter block a clouds launch passes: the larger one for the DIST kernels (mgs_kernels.h), the parent's otherwise
+template <bool DIST>
+using CloudsArgs = typename std::conditional<DIST, ProjectBwdCloudsDistArgs, ProjectBwdCloudsArgs>::type;
 }  // namespace
 
-// several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c
-template <int NSH, int MIN_BLOCKS, bool FISH, bool ORTHO, bool CAM, bool AA>
+// several clouds in one launch: CTAs [cloud[c].block0, cloud[c + 1].block0) serve cloud c.  Two overloads of one name: the
+// parent's parameter block, and the DIST instantiations' larger one (mgs_kernels.h), which adds each view's coefficients.
+template <int NSH, int MIN_BLOCKS, bool DIST, bool FISH, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsArgs a)
 {
 	static_assert(CAM || !ORTHO, "the orthographic backward is a CAM instantiation");
 	static_assert(ORTHO || !FISH, "the fisheye backward is an ORTHO instantiation");
+	static_assert(!DIST, "the distorted backward takes ProjectBwdCloudsDistArgs");
+	int c = 0;
+	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
+	const ProjectBwdCloud& cl = a.cloud[c];
+	const int idx = ((int)blockIdx.x - cl.block0) * blockDim.x + threadIdx.x;
+	if (!CAM && idx >= cl.P) return;
+	unsigned dmask = 0u;  // no distorted view
+	const DistK* dk = nullptr;
+	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
+		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
+		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr, ORTHO ? (unsigned)a.ortho >> cl.view0 : 0u,
+		FISH ? (unsigned)a.fisheye >> cl.view0 : 0u, FISH ? a.fe_k + cl.view0 : nullptr, dmask, dk };
+	if constexpr (CAM) {
+		// the CTA serves one cloud: its rows belong to that cloud's views
+		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(cb, idx, idx < cl.P, cam_sm);
+		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
+	} else {
+		project_bwd_gaussian<NSH, AA, false, false, false, false>(cb, idx, true, nullptr);
+	}
+}
+template <int NSH, int MIN_BLOCKS, bool DIST, bool FISH, bool ORTHO, bool CAM, bool AA>
+__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(ProjectBwdCloudsDistArgs a)
+{
+	static_assert(DIST && FISH && ORTHO && CAM, "the distorted backward is a FISH, ORTHO and CAM instantiation");
 	int c = 0;
 	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
 	const ProjectBwdCloud& cl = a.cloud[c];
@@ -493,14 +568,14 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	const CloudBwd cb{ a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp, cl.accumulate,
 		cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
 		AA ? a.conic_opacity + cl.view0 : nullptr, CAM ? a.intr + cl.view0 : nullptr, ORTHO ? (unsigned)a.ortho >> cl.view0 : 0u,
-		FISH ? (unsigned)a.fisheye >> cl.view0 : 0u, FISH ? a.fe_k + cl.view0 : nullptr };
+		FISH ? (unsigned)a.fisheye >> cl.view0 : 0u, FISH ? a.fe_k + cl.view0 : nullptr, (unsigned)a.distorted >> cl.view0, a.dc_k + cl.view0 };
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH>(cb, idx, idx < cl.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(cb, idx, idx < cl.P, cam_sm);
 		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
-		project_bwd_gaussian<NSH, AA, false, false, false>(cb, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false, false>(cb, idx, true, nullptr);
 	}
 }
 
@@ -562,23 +637,25 @@ void launch_camera_grad_reduce(const CamReduceArgs& a, cudaStream_t s)
 	if (a.V > 0) camera_grad_reduce_kernel<<<a.V, CAM_REDUCE_THREADS, 0, s>>>(a);
 }
 
-// ORTHO and FISH run at the blocks per SM of their CAM sibling
-template <bool CAM, bool ORTHO, bool FISH = false>
+// ORTHO, FISH and DIST run at the blocks per SM of their CAM sibling, except where a bound below says otherwise
+template <bool CAM, bool ORTHO, bool FISH = false, bool DIST = false>
 static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, cudaStream_t s)
 {
 	if (a.antialias) {
 		// 4 blocks per SM at degree <= 1: the compensation's registers do not fit the cap of 5 (96) without spilling
 		// CAM at degree 2: 3 blocks per SM, the camera and focal-length terms spill at the cap of 4 (128)
-		if (deg <= 1) project_bwd_views_kernel<12, 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else project_bwd_views_kernel<48, 3, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		// DIST: 3 blocks per SM at degree <= 1 and 2 at degree 3, where the distortion's second derivatives spill at the caps
+		if (deg <= 1) project_bwd_views_kernel<12, DIST ? 3 : 4, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_kernel<27, CAM ? 3 : 4, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_kernel<48, DIST ? 2 : 3, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
 	// CAM at degree <= 1: 4 blocks per SM, as for AA; the camera terms spill at the cap of 5 (96 registers)
 	// FISH at degree 2: 3 blocks per SM, the fisheye second derivatives spill at the cap of 4 (128 registers)
-	if (deg <= 1) project_bwd_views_kernel<12, CAM ? 4 : MGS_PBWD_MINB, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_views_kernel<27, FISH ? 3 : 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else project_bwd_views_kernel<48, 3, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	// DIST at degree <= 1: 3 blocks per SM, the distortion's second derivatives spill at the cap of 4 (128 registers)
+	if (deg <= 1) project_bwd_views_kernel<12, DIST ? 3 : CAM ? 4 : MGS_PBWD_MINB, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else if (deg == 2) project_bwd_views_kernel<27, FISH ? 3 : 4, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	else project_bwd_views_kernel<48, 3, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
@@ -588,29 +665,30 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	const int deg = a.shs ? a.D : 0;
 	bool cam = false;  // camera rows, or a device field of view, which only the CAM instantiation reads
 	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (a.fisheye) project_bwd_views<true, true, true>(a, grid, deg, s);  // a fisheye view: the FISH instantiation, all models
+	if (a.distorted) project_bwd_views<true, true, true, true>(a, grid, deg, s);  // a distorted view: DIST, all four models
+	else if (a.fisheye) project_bwd_views<true, true, true>(a, grid, deg, s);  // a fisheye view: the FISH instantiation, all models
 	else if (a.ortho) project_bwd_views<true, true>(a, grid, deg, s);  // an orthographic view: the ORTHO instantiation of CAM
 	else if (cam) project_bwd_views<true, false>(a, grid, deg, s);
 	else project_bwd_views<false, false>(a, grid, deg, s);
 }
 
-template <bool CAM, bool ORTHO, bool FISH = false>
-static void project_bwd_clouds(const ProjectBwdCloudsArgs& a, int grid, int deg, cudaStream_t s)
+template <bool CAM, bool ORTHO, bool FISH = false, bool DIST = false>
+static void launch_clouds(const CloudsArgs<DIST>& a, int grid, int deg, cudaStream_t s)
 {
 	// 4 blocks per SM at degree <= 1: the register cap of 5 (96) spills here, and the launch is small where it matters most
 	// (one CTA per 128 Gaussians of each cloud: 16k Gaussians fill one wave)
 	if (a.antialias) {
-		if (deg <= 1) project_bwd_clouds_kernel<12, 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
-		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
-		else project_bwd_clouds_kernel<48, 3, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
+		if (deg <= 1) project_bwd_clouds_kernel<12, DIST ? 3 : 4, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+		else if (deg == 2) project_bwd_clouds_kernel<27, CAM ? 3 : 4, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+		else project_bwd_clouds_kernel<48, DIST ? 2 : 3, DIST, FISH, ORTHO, CAM, true><<<grid, 128, 0, s>>>(a);
 		return;
 	}
-	if (deg <= 1) project_bwd_clouds_kernel<12, 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
-	else if (deg == 2) project_bwd_clouds_kernel<27, FISH ? 3 : 4, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);  // as in the views launcher
-	else project_bwd_clouds_kernel<48, 3, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
+	if (deg <= 1) project_bwd_clouds_kernel<12, DIST ? 3 : 4, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+	else if (deg == 2) project_bwd_clouds_kernel<27, FISH ? 3 : 4, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);  // as in the views launcher
+	else project_bwd_clouds_kernel<48, 3, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
-void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
+void launch_project_bwd_clouds(ProjectBwdCloudsDistArgs a, cudaStream_t s)
 {
 	if (a.B <= 0) return;
 	int grid = 0, V = 0;
@@ -624,10 +702,15 @@ void launch_project_bwd_clouds(ProjectBwdCloudsArgs a, cudaStream_t s)
 	const int deg = sh ? a.D : 0;
 	bool cam = false;
 	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (a.fisheye) project_bwd_clouds<true, true, true>(a, grid, deg, s);
-	else if (a.ortho) project_bwd_clouds<true, true>(a, grid, deg, s);
-	else if (cam) project_bwd_clouds<true, false>(a, grid, deg, s);
-	else project_bwd_clouds<false, false>(a, grid, deg, s);
+	if (a.distorted) {
+		launch_clouds<true, true, true, true>(a, grid, deg, s);
+		return;
+	}
+	const ProjectBwdCloudsArgs& b = a;  // the parent's parameter block
+	if (b.fisheye) launch_clouds<true, true, true>(b, grid, deg, s);
+	else if (b.ortho) launch_clouds<true, true>(b, grid, deg, s);
+	else if (cam) launch_clouds<true, false>(b, grid, deg, s);
+	else launch_clouds<false, false>(b, grid, deg, s);
 }
 
 }  // namespace mgs

@@ -454,6 +454,9 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     them with pinhole views, and they combine with every option here.  Fisheye views: cameras from
     `cameras.build_fisheye_cameras` or `cameras.fisheye_camera_batch` (or settings with a `fisheye` attribute) are rendered
     with the Kannala-Brandt projection (INTEGRATION.md §11), mixed with pinhole and orthographic views as above.
+    Distorted-pinhole views: cameras from `cameras.build_distorted_cameras` or `cameras.distorted_camera_batch` (or settings
+    with a `distortion` attribute) are rendered with OpenCV's radial, tangential and rational lens distortion
+    (INTEGRATION.md §12), mixed with the other three models as above.
     return_median_depth: also return "median_depth" [V,H,W], the view-space depth of the contributor at which each pixel's
     accumulated opacity crosses one half (differentiable; its gradient reaches only that Gaussian's depth), and "median_id"
     [V,H,W] int32, that Gaussian's index (-1 where nothing covers the pixel; INTEGRATION.md §7).  Not with targets.
@@ -514,7 +517,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True,
                                            orthographic=getattr(views[0], "orthographic", False),
-                                           fisheye=getattr(views[0], "fisheye", None)) if aa else views[0]
+                                           fisheye=getattr(views[0], "fisheye", None),
+                                           distortion=getattr(views[0], "distortion", None)) if aa else views[0]
         out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha, return_median_depth=return_median_depth,
                                  return_normal=return_normal)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
@@ -553,7 +557,7 @@ def lift_views(cameras, pts_xyz, rotations, scales, opacity, maps, view_ids=None
     which view v's render blends g into pixel p (no background term):
         lifted[g][c] = sum_v sum_p w_vpg maps[v][c][p]        weight[g] = sum_v sum_p w_vpg
     lifted / weight is the Gaussian's weighted average of the maps (where weight > 0), weight alone a visibility score over
-    the views.  The same cloud rendered with these cameras (orthographic and fisheye ones included) and `antialiasing` gives the weights
+    the views.  The same cloud rendered with these cameras (orthographic, fisheye and distorted ones included) and `antialiasing` gives the weights
     used here.  Inputs that
     require grad are detached; the outputs are not differentiable.  Returns {"lifted": [P,C], "weight": [P]}; raises
     ValueError on a shape, dtype or device mismatch."""

@@ -300,10 +300,12 @@ class _RasterizeGaussians(torch.autograd.Function):
         alpha = med_depth = med_id = normal = None
         if return_normal and (cov3Ds_precomp is not None and cov3Ds_precomp.numel() != 0):
             raise ValueError("return_normal needs scales and rotations: a precomputed covariance has no axis to take a normal from")
-        orth = bool(getattr(s, "orthographic", False)) or getattr(s, "fisheye", None) is not None
+        orth = bool(getattr(s, "orthographic", False)) or getattr(s, "fisheye", None) is not None \
+            or getattr(s, "distortion", None) is not None
         ctx.orthographic = orth
         if (return_alpha or return_median or return_normal or aa or orth or ctx.camera) and views_path:
-            # the alpha plane, the median planes, the anti-aliased, orthographic and fisheye projections and the camera gradients exist on
+            # the alpha plane, the median planes, the anti-aliased, orthographic, fisheye and distorted projections and the camera
+            # gradients exist on
             # the multi-view entry points only: debug renders take them too, with the snapshot dump
             cpu_args = cpu_deep_copy_tuple(args) if s.debug else None
             try:
@@ -477,13 +479,18 @@ class GaussianRasterizationSettings(_Settings):
     `fisheye` (default None; keyword, or positional after orthographic) is an attribute in the same way: the view's
     Kannala-Brandt parameters (cx, cy, k1, k2, k3, k4, theta_max), or a dict with those keys, make it a fisheye view, with
     tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (fx, fy in pixels per radian; include/mgs_rasterizer.h,
-    mgs_forward_views_fisheye; cameras.build_fisheye_cameras).  It cannot be combined with orthographic=True."""
+    mgs_forward_views_fisheye; cameras.build_fisheye_cameras).  It cannot be combined with orthographic=True.
+    `distortion` (default None; keyword, or positional after fisheye) is an attribute in the same way: the view's OpenCV
+    parameters (cx, cy, k1, k2, p1, p2, k3, k4, k5, k6, r_max), or a dict with those keys, make it a distorted-pinhole view,
+    with tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (include/mgs_rasterizer.h, mgs_forward_views_distorted;
+    cameras.build_distorted_cameras).  It cannot be combined with orthographic=True or fisheye."""
     antialiasing = False
     orthographic = False
     fisheye = None
+    distortion = None
 
     def __new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix, sh_degree, campos,
-                prefiltered, debug, include_feature, antialiasing=False, orthographic=False, fisheye=None):
+                prefiltered, debug, include_feature, antialiasing=False, orthographic=False, fisheye=None, distortion=None):
         self = super().__new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix,
                                sh_degree, campos, prefiltered, debug, include_feature)
         self.antialiasing = bool(antialiasing)
@@ -491,6 +498,9 @@ class GaussianRasterizationSettings(_Settings):
         self.fisheye = _fisheye_params(fisheye)
         if self.orthographic and self.fisheye is not None:
             raise ValueError("a view cannot be both orthographic and fisheye")
+        self.distortion = _distortion_params(distortion)
+        if self.distortion is not None and (self.orthographic or self.fisheye is not None):
+            raise ValueError("a distorted view cannot also be orthographic or fisheye")
         return self
 
     @classmethod
@@ -501,11 +511,12 @@ class GaussianRasterizationSettings(_Settings):
         aa = kw.pop("antialiasing", self.antialiasing)
         orth = kw.pop("orthographic", self.orthographic)
         fe = kw.pop("fisheye", self.fisheye)
-        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth, fisheye=fe)
+        dc = kw.pop("distortion", self.distortion)
+        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth, fisheye=fe, distortion=dc)
 
     def __repr__(self):
         return super().__repr__()[:-1] + (f", antialiasing={self.antialiasing}, orthographic={self.orthographic}, "
-                                          f"fisheye={self.fisheye})")
+                                          f"fisheye={self.fisheye}, distortion={self.distortion})")
 
 
 FISHEYE_KEYS = ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")
@@ -518,6 +529,19 @@ def _fisheye_params(x):
     vals = [x[k] for k in FISHEYE_KEYS] if isinstance(x, dict) else list(x)
     if len(vals) != len(FISHEYE_KEYS):
         raise ValueError(f"fisheye: expected {FISHEYE_KEYS}, got {x!r}")
+    return tuple(float(v) for v in vals)
+
+
+DISTORTION_KEYS = ("cx", "cy", "k1", "k2", "p1", "p2", "k3", "k4", "k5", "k6", "r_max")
+
+
+def _distortion_params(x):
+    """A view's distortion parameters as a tuple of 11 floats (DISTORTION_KEYS order) from such a sequence or a dict, or None"""
+    if x is None:
+        return None
+    vals = [x[k] for k in DISTORTION_KEYS] if isinstance(x, dict) else list(x)
+    if len(vals) != len(DISTORTION_KEYS):
+        raise ValueError(f"distortion: expected {DISTORTION_KEYS}, got {x!r}")
     return tuple(float(v) for v in vals)
 
 
@@ -693,13 +717,32 @@ def _fisheye_array(views, fisheye=None):
     return arr
 
 
+def _distortion_array(views, distortion=None):
+    """Per-view distortion parameters: `distortion` (V entries, each None or parameters) when given, else each view's
+    `distortion` attribute; a ctypes ViewDistortion array for the _distorted calls, or None when no view is distorted."""
+    dc = [_distortion_params(d) for d in distortion] if distortion is not None else \
+        [getattr(s, "distortion", None) for s in views]
+    if len(dc) != len(views):
+        raise ValueError(f"distortion: expected {len(views)} entries, got {len(dc)}")
+    if all(d is None for d in dc):
+        return None
+    arr = (_b.ViewDistortion * len(dc))()
+    for v, d in enumerate(dc):
+        if d is not None:
+            arr[v].distorted = 1
+            for k, x in zip(DISTORTION_KEYS, d):
+                setattr(arr[v], k, x)
+    return arr
+
+
 def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug,
-               ortho=None, fisheye=None):
+               ortho=None, fisheye=None, distortion=None):
     """First call for a (cloud size, image size): one projection + scan per view with a host read of the instance count
     (the reference does this on EVERY call), only to seed the capacity table.  An orthographic view (`ortho`: the views'
     flags, or None) is counted by a weight-only lift with one binning slot, whose status holds the full count: the
     single-view mgs_forward_begin has no camera model, and the lift is the cheapest call that takes one.  Its weights are
-    discarded.  A fisheye view (`fisheye`: the views' ViewFisheye array, or None) is counted the same way."""
+    discarded.  A fisheye view (`fisheye`: the views' ViewFisheye array, or None) and a distorted view (`distortion`: the
+    views' ViewDistortion array, or None) are counted the same way."""
     counts = torch.zeros(len(views), dtype=torch.int32).pin_memory()
     st = torch.cuda.current_stream(dev)
     keep, ortho_status = [], {}
@@ -707,9 +750,10 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
         if keys[v] in _CAPACITY:
             continue
         fe = fisheye[v] if fisheye is not None and fisheye[v].fisheye else None
-        if (ortho is not None and ortho[v]) or fe is not None:
+        dc = distortion[v] if distortion is not None and distortion[v].distorted else None
+        if (ortho is not None and ortho[v]) or fe is not None or dc is not None:
             ortho_status[v], k = _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier,
-                                              cov3D_precomp, debug, st, fe)
+                                              cov3D_precomp, debug, st, fe, dc)
             keep.append(k)
             continue
         H, W = int(s.image_height), int(s.image_width)
@@ -728,9 +772,10 @@ def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, 
             _CAPACITY[keys[v]] = _round_capacity(n * 1.25 + 4096)
 
 
-def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug, st, fisheye=None):
-    """Enqueues orthographic view `s`'s projection and binning on `st` with one binning slot, or fisheye view `s`'s with
-    `fisheye` its ViewFisheye entry.  Returns its pinned status {instance count, overflow}, valid once `st` is synchronised,
+def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug, st, fisheye=None,
+                 distortion=None):
+    """Enqueues orthographic view `s`'s projection and binning on `st` with one binning slot, fisheye view `s`'s with
+    `fisheye` its ViewFisheye entry, or distorted view `s`'s with `distortion` its ViewDistortion entry.  Returns its pinned status {instance count, overflow}, valid once `st` is synchronised,
     and what must stay alive until then."""
     H, W = int(s.image_height), int(s.image_width)
     gbytes, ibytes, _ = _state_sizes(L, P, W, H)
@@ -751,7 +796,10 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
     iarr = _intrinsics_array(tf, None) if tf is not None else None
     rest = (P, 0, 0, 0, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
             _ptr(cov3D_precomp), None, _ptr(weight), int(bool(debug)), st.cuda_stream)
-    if fisheye is not None:
+    if distortion is not None:
+        _b.check(L.mgs_lift_views_distorted(1, w, None, 0, iarr, None, None, (_b.ViewDistortion * 1)(distortion), *rest),
+                 "mgs_lift_views_distorted")
+    elif fisheye is not None:
         _b.check(L.mgs_lift_views_fisheye(1, w, None, 0, iarr, None, (_b.ViewFisheye * 1)(fisheye), *rest), "mgs_lift_views_fisheye")
     else:
         _b.check(L.mgs_lift_views_ortho(1, w, None, 0, iarr, (ctypes.c_int * 1)(1), *rest), "mgs_lift_views_ortho")
@@ -761,7 +809,7 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False, return_normal=False, ortho=None, fisheye=None):
+                        return_median=False, return_normal=False, ortho=None, fisheye=None, distortion=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -788,7 +836,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     view's `orthographic` attribute does.  With any orthographic view the call is mgs_forward_views_ortho; pass the same
     flags (or views) to the backward.  `fisheye` (V entries, each None or a view's fisheye parameters, as the settings'
     `fisheye` attribute) marks the fisheye views, by default each view's `fisheye` attribute; with any fisheye view the call
-    is mgs_forward_views_fisheye."""
+    is mgs_forward_views_fisheye.  `distortion` (V entries, each None or a view's distortion parameters, as the settings'
+    `distortion` attribute) marks the distorted-pinhole views, by default each view's `distortion` attribute; with any
+    distorted view the call is mgs_forward_views_distorted."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -803,6 +853,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     V = len(views)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
+    dcarr = _distortion_array(views, distortion)
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]  # a single view needs no side stream
     di = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -816,7 +867,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call) or pass `capacities`")
             _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug, oarr, farr)
+                       debug, oarr, farr, dcarr)
         arr = (_b.View * V)()
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
@@ -842,7 +893,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if farr is not None:
+        if dcarr is not None:
+            _b.check(L.mgs_forward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                   _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                   dcarr, *rest), "mgs_forward_views_distorted")
+        elif farr is not None:
             _b.check(L.mgs_forward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                  *rest), "mgs_forward_views_fisheye")
@@ -876,12 +931,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
 
 
 def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, maps, antialiasing=False,
-                   tan_fov=None, debug=False, ortho=None, fisheye=None):
+                   tan_fov=None, debug=False, ortho=None, fisheye=None, distortion=None):
     """Lift one 2D map per view onto the Gaussians (C ABI mgs_lift_views): lifted [P,C] = sum over the views and pixels of
     the forward blend's weights w = alpha T times the map, weight [P] = the sum of the weights.  `maps`: [V,C,H,W] or a
     sequence of V [C,H,W] fp32 tensors on the cloud's device (each view's own H, W), or None for weight only.  `views`,
-    `antialiasing`, `tan_fov`, `ortho` and `fisheye` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with an orthographic
-    view, mgs_lift_views_fisheye with a fisheye one); the binning state is sized from the same capacity table (a
+    `antialiasing`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with
+    an orthographic view, mgs_lift_views_fisheye with a fisheye one, mgs_lift_views_distorted with a distorted one); the binning state is sized from the same capacity table (a
     steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
     needs colours, which the lift never reads: a zero [P,3] buffer stands in for them."""
     L = _b.lib()
@@ -895,6 +950,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
     V = len(views)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
+    dcarr = _distortion_array(views, distortion)
     C = int(maps[0].shape[0]) if maps is not None else 0
     colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
     main = torch.cuda.current_stream(dev)
@@ -910,7 +966,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
                 raise RuntimeError("lift the views once before capturing them in a CUDA graph (the binning capacity is learned "
                                    "from an eager call)")
             _calibrate(L, views, keys, dev, P, 0, 0, means3D, None, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug, oarr, farr)
+                       debug, oarr, farr, dcarr)
         arr = (_b.View * V)()
         larr = (_b.ViewLift * V)()
         status = _status_slots(V)
@@ -944,7 +1000,10 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         iarr = _intrinsics_array(tf, None) if tf is not None else None
         rest = (P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
                 _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight), int(bool(debug)), main.cuda_stream)
-        if farr is not None:
+        if dcarr is not None:
+            _b.check(L.mgs_lift_views_distorted(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, dcarr, *rest),
+                     "mgs_lift_views_distorted")
+        elif farr is not None:
             _b.check(L.mgs_lift_views_fisheye(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, *rest), "mgs_lift_views_fisheye")
         elif oarr is not None:
             _b.check(L.mgs_lift_views_ortho(V, arr, larr, int(bool(antialiasing)), iarr, oarr, *rest), "mgs_lift_views_ortho")
@@ -1087,7 +1146,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
                                  ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
-                                 grads_normal=None, normals=None, ortho=None, fisheye=None):
+                                 grads_normal=None, normals=None, ortho=None, fisheye=None, distortion=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -1114,7 +1173,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
     forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho.
     `fisheye`: as given to the forward (by default the views' `fisheye` attributes); with a fisheye view the call is
-    mgs_backward_views_fisheye."""
+    mgs_backward_views_fisheye.  `distortion`: likewise, mgs_backward_views_distorted with a distorted view."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1125,6 +1184,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     V = len(views)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
+    dcarr = _distortion_array(views, distortion)
     main = torch.cuda.current_stream(dev)
     opts = dict(dtype=torch.float32, device=dev)
     acc = accumulate_into or {}
@@ -1186,7 +1246,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if farr is not None:
+            if dcarr is not None:
+                _b.check(L.mgs_backward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
+                                                        oarr, farr, dcarr, *rest), "mgs_backward_views_distorted")
+            elif farr is not None:
                 _b.check(L.mgs_backward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
                                                       farr, *rest), "mgs_backward_views_fisheye")
             elif oarr is not None:
@@ -1350,7 +1413,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     (C ABI mgs_forward_clouds_normal).  A cloud's optional "ortho" (V_b flags; by default its views' `orthographic`
     attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry.  A cloud's
     optional "fisheye" (V_b entries, each None or parameters; by default its views' `fisheye` attributes) marks its fisheye
-    views (C ABI mgs_forward_clouds_fisheye), likewise."""
+    views (C ABI mgs_forward_clouds_fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
+    mgs_forward_clouds_distorted)."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
@@ -1377,7 +1441,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                                        "learned from an eager call) or pass `capacities`")
                 _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
                            d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug, _ortho_flags(c["views"], c.get("ortho")),
-                           _fisheye_array(c["views"], c.get("fisheye")))
+                           _fisheye_array(c["views"], c.get("fisheye")), _distortion_array(c["views"], c.get("distortion")))
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
@@ -1412,8 +1476,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        oarr, farr = _clouds_ortho(clouds), _clouds_fisheye(clouds)
-        if farr is not None:
+        oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
+        if dcarr is not None:
+            _b.check(L.mgs_forward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                    _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                    dcarr, *rest), "mgs_forward_clouds_distorted")
+        elif farr is not None:
             _b.check(L.mgs_forward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                   _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                   *rest), "mgs_forward_clouds_fisheye")
@@ -1462,6 +1530,13 @@ def _clouds_fisheye(clouds):
     return _fisheye_array([None] * len(fe), fe)
 
 
+def _clouds_distortion(clouds):
+    """The _distorted calls' ViewDistortion array over every view of the clouds in order, or None when no view is distorted"""
+    dc = [d for c in clouds for d in ([_distortion_params(x) for x in c["distortion"]] if c.get("distortion") is not None
+                                      else [getattr(s, "distortion", None) for s in c["views"]])]
+    return _distortion_array([None] * len(dc), dc)
+
+
 def _clouds_fov(clouds, dev):
     """[V,2] device field of view of every view of the clouds in order, or None when no cloud has one (the clouds without
     one contribute their host floats)"""
@@ -1491,7 +1566,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     int32 the id planes that forward returned (C ABI mgs_backward_clouds_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
     cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
     mgs_backward_clouds_normal).  Clouds with an orthographic view (see rasterize_clouds_raw) make the call
-    mgs_backward_clouds_ortho, and clouds with a fisheye view mgs_backward_clouds_fisheye."""
+    mgs_backward_clouds_ortho, clouds with a fisheye view mgs_backward_clouds_fisheye, and clouds with a distorted view
+    mgs_backward_clouds_distorted."""
     L = _b.lib()
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
@@ -1572,8 +1648,12 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        oarr, farr = _clouds_ortho(clouds), _clouds_fisheye(clouds)
-        if farr is not None:
+        oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
+        if dcarr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
+                                                     marr, narr, oarr, farr, dcarr, *rest), "mgs_backward_clouds_distorted")
+        elif farr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
                                                    narr, oarr, farr, *rest), "mgs_backward_clouds_fisheye")
