@@ -1137,6 +1137,61 @@ int mgs_lift_views_distorted(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
+/*
+ * Planar depth.  The _planar calls are the _distorted calls with one more argument, `planar_depth` (0 or 1, for every view of
+ * the call, like antialiasing); the _distorted calls are the _planar calls with planar_depth = 0.  Without it each Gaussian
+ * paints its centre depth z = t.z over its whole footprint; with it, Gaussian i's depth at pixel p is its depth along the
+ * pixel's ray, affine in the pixel offset (RaDe-GS, PGSR).  Definition, for Gaussian i in view v, with t = Rv p + tv:
+ *   - Sigma_c = Rv S Rv^T, S the world-space covariance (from scales and rotations, or cov3D_precomp);
+ *   - J the 2x3 screen Jacobian the projection uses for the view's model, in pixels (pinhole with its 1.3 tan_fov clamp,
+ *     orthographic, fisheye or distorted), Q the blend's conic, the inverse of J Sigma_c J^T + 0.3 I (also in AA mode);
+ *   - k = e3^T Sigma_c J^T, the covariance of depth with screen position, and (a, b) = k Q, the regression of t.z on the
+ *     dilated screen position;
+ *   - d_i(p) = z + a (px - mu_x) + b (py - mu_y), mu the blend's screen mean in pixels, pixel (i, j) centred at (i, j).
+ * The depth plane is sum_i w_i d_i(p) (w the blend weights), and so are what is derived from it: the expected-depth L1 head
+ * (mgs_view_depth_mask.target_depth), depth / alpha, and the median depth, which becomes d_i(p) of the pixel's median
+ * contributor.  Colour, features, alpha, radii, tiles, sort keys and median_id do not change.  The blend carries the
+ * per-Gaussian quad {a, b, e = -(a mu_x + b mu_y), 0} in columns 4..7 of its {r,g,b,depth} tile, so the depth is
+ * col3 + px col4 + py col5 + col6; the quads live where the normal plane's do, so the geometry state must be sized by
+ * mgs_geometry_state_bytes_normal and the backward scratch by mgs_backward_scratch_bytes_normal.
+ * Backward: the depth cotangent g (including the depth head's) enters the blend as the column cotangents (g, g px, g py, g),
+ * which makes dL/dalpha that of the planar depth; the blend returns dL/d(a, b, e) per Gaussian and view, and the per-Gaussian
+ * stage chains them through e to mu (added to dL/dmean2D in its convention), through Q (added to the conic's gradient) and
+ * through k to Sigma_c, J and the third row of Rv, and from there to means3D, scales, rotations (or cov3D), the camera
+ * gradients and dL_dtan_fov for all four models.  The median depth's cotangent reaches z, a, b and mu of its contributor.
+ * dL_dconic (single-view calls) stays the blend's conic gradient.
+ * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: planar_depth other than 0 or 1; planar_depth together
+ * with a normal plane in the same call (both need columns 4..6 of the tile; a fourth column tile for both is left for later).
+ */
+int mgs_forward_views_planar(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_views_planar(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int planar_depth,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
+int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F,
+	float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -202,6 +202,10 @@ def lib():
         getattr(L, dist).restype = C.c_int
         getattr(L, dist).argtypes = getattr(L, fish).argtypes[:len(getattr(L, fish).argtypes) - len(at) + k] + \
             [C.POINTER(ViewDistortion)] + at[k:]
+        # ... and the planar_depth flag after the distortion parameters
+        pln = name.replace("_views", "_views_planar").replace("_clouds", "_clouds_planar")
+        getattr(L, pln).restype = C.c_int
+        getattr(L, pln).argtypes = getattr(L, dist).argtypes[:len(getattr(L, dist).argtypes) - len(at) + k] + [i] + at[k:]
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
                                  i, i, i, i,                        # P D M C
@@ -268,6 +272,7 @@ EXPORTED_SYMBOLS = (
     "mgs_lift_views_fisheye",
     "mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
     "mgs_backward_clouds_distorted", "mgs_lift_views_distorted",
+    "mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -331,6 +331,7 @@ struct Cloud {
 	const float* means3D; const float* shs; const float* colors_precomp; const float* feature; const float* opacities;
 	const float* scales; float scale_modifier; const float* rotations; const float* cov3D_precomp;
 	int antialias;  // 1: the anti-aliased projection (opacity compensation); 0 where an initialiser leaves it out
+	int planar;     // 1: planar depth (include/mgs_rasterizer.h, mgs_forward_views_planar); 0 where an initialiser leaves it out
 };
 
 // a view's tile grid and its state buffers, carved (pointers into a buffer the view does not provide are never used)
@@ -443,6 +444,18 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_f
 	}
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
+	if (c.planar) {
+		// the view's planar-depth quads, where the normal plane keeps its quads (the _normal size queries)
+		PlanarFwdArgs la{};
+		la.P = c.P; la.means3D = c.means3D; la.cov3D = c.cov3D_precomp ? c.cov3D_precomp : geom.cov3D; la.viewmatrix = w.viewmatrix;
+		la.W = w.width; la.H = w.height; la.tan_fovx = w.tan_fovx; la.tan_fovy = w.tan_fovy; la.tan_fov = tan_fov;
+		la.model = dc ? 3 : fe ? 2 : ortho ? 1 : 0;
+		if (fe) la.fe_k = pa.fe_k;
+		if (dc) la.dc_k = pa.dc_k;
+		la.radii = w.radii; la.means2D = geom.means2D; la.conic_opacity = geom.conic_opacity; la.quad = s.nrm;
+		launch_planar_fwd(la, st);
+		MGS_STAGE("planar_fwd");
+	}
 
 	// Gaussians in depth order (stable: ascending id among equal depth bits; culled ones carry +inf and emit nothing)
 	{
@@ -578,6 +591,7 @@ static int enqueue_blend_fwd(const Cloud& c, const mgs_view& w, float* out_alpha
 	const ViewState vs = carve_view(w, c.P);
 	BlendArgs ba = blend_args(vs, w, F, c.feature);
 	if (nm && nm->out_normal) { ba.nrm = vs.nrm; ba.out_normal = nm->out_normal; }
+	if (c.planar) { ba.nrm = vs.nrm; ba.planar = 1; }
 	ba.want_depth = w.out_depth != nullptr;
 	ba.out_color = w.out_color; ba.out_feature = w.out_feature; ba.out_depth = w.out_depth; ba.out_alpha = out_alpha;
 	if (med && med->median_id) { ba.median_id = med->median_id; ba.out_median_depth = med->out_median_depth; }
@@ -656,8 +670,10 @@ static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeatu
 	const int F = c.F;
 	const ViewState s = carve_view(w, c.P);
 	MGS_CUDA(cudaMemsetAsync(s.gb, 0, (size_t)c.P * GB_STRIDE * sizeof(float), st));
+	if (c.planar) MGS_CUDA(cudaMemsetAsync(s.gn, 0, (size_t)c.P * 4 * sizeof(float), st));
 	if (med && med->dL_dpix_median_depth) {
-		launch_median_depth_bwd(w.width * w.height, med->median_id, med->dL_dpix_median_depth, s.gb, st);
+		launch_median_depth_bwd(w.width * w.height, med->median_id, med->dL_dpix_median_depth, s.gb, st, w.width,
+			c.planar ? s.gn : nullptr);
 		MGS_STAGE("median_depth_bwd");
 	}
 	BlendArgs ba = blend_args(s, w, F, c.feature);
@@ -668,6 +684,7 @@ static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeatu
 		MGS_CUDA(cudaMemsetAsync(s.gn, 0, (size_t)c.P * 4 * sizeof(float), st));
 		ba.nrm = s.nrm; ba.dL_dnormal = nm->dL_dpix_normal; ba.gn = s.gn;
 	}
+	if (c.planar) { ba.nrm = s.nrm; ba.gn = s.gn; ba.planar = 1; }
 	depth_mask_args(ba, dm);
 	ba.want_depth = w.dL_dpix_depth != nullptr || ba.tgt_depth != nullptr;  // the depth head's cotangent reaches the view-space z
 	if (w.binning_capacity > 0) {
@@ -687,6 +704,13 @@ static ProjectBwdView bwd_view(const mgs_view& w, int P, float* dL_dmean2D)
 	pv.tan_fovx = w.tan_fovx; pv.tan_fovy = w.tan_fovy;
 	pv.focal_x = w.width / (2.0f * w.tan_fovx); pv.focal_y = w.height / (2.0f * w.tan_fovy);
 	return pv;
+}
+// the per-Gaussian stage's planar-depth arrays of one view: its quad gradients, quads and screen means
+static void planar_view(const Cloud& c, const mgs_view& w, const float4*& g, const float4*& q, const float2*& mean)
+{
+	if (!c.planar) return;
+	const ViewState s = carve_view(w, c.P);
+	g = reinterpret_cast<const float4*>(s.gn); q = s.nrm; mean = s.geom.means2D;
 }
 
 // camera gradients of view v (cam, intr: one entry per view, or NULL): the view asks for them when its camera entry or its
@@ -805,6 +829,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		for (int u = 0; u < pb.V; u++) pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << u);
 		for (int u = 0; u < pb.V; u++) set_fisheye(fisheye_of(fe, v0 + u), u, pb.fisheye, pb.fe_k);
 		for (int u = 0; u < pb.V; u++) set_distortion(distortion_of(dc, v0 + u), u, pb.distorted, pb.dc_k);
+		for (int u = 0; u < pb.V; u++) planar_view(c, views[v0 + u], pb.pl_g[u], pb.pl_q[u], pb.pl_mean[u]);
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
 		MGS_STAGE("project_bwd");
@@ -865,15 +890,26 @@ static int check_clouds(int B, const mgs_cloud* clouds, const int* view_offsets,
 	return 0;
 }
 
-static Cloud cloud_of(const mgs_cloud& k, int D, int M, int F, float scale_modifier, int antialias)
+static Cloud cloud_of(const mgs_cloud& k, int D, int M, int F, float scale_modifier, int antialias, int planar = 0)
 {
 	return Cloud{ k.P, D, M, k.feature ? F : 0, k.means3D, k.shs, k.colors_precomp, k.feature, k.opacities, k.scales, scale_modifier,
-		k.rotations, k.cov3D_precomp, antialias };
+		k.rotations, k.cov3D_precomp, antialias, planar };
 }
 
 static int check_antialias(int antialiasing)
 {
 	if (antialiasing != 0 && antialiasing != 1) return fail(MGS_ERR_INVALID_ARG, "antialiasing must be 0 or 1");
+	return 0;
+}
+
+// planar depth: a flag, and never beside a normal plane (both take columns 4..6 of the blend's {r,g,b,depth} tile); normal: V
+// entries or NULL
+static int check_planar(int planar_depth, const mgs_view_normal* normal, int V)
+{
+	if (planar_depth != 0 && planar_depth != 1) return fail(MGS_ERR_INVALID_ARG, "planar_depth must be 0 or 1");
+	for (int v = 0; planar_depth && normal && v < V; v++)
+		if (normal[v].out_normal || normal[v].dL_dpix_normal)
+			return fail(MGS_ERR_INVALID_ARG, "planar_depth cannot be combined with a normal plane in the same call");
 	return 0;
 }
 
@@ -1104,9 +1140,24 @@ int mgs_forward_views_distorted(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_planar(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye,
+		distortion, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations,
+		cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_planar(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
@@ -1124,7 +1175,7 @@ int mgs_forward_views_distorted(
 		if (rc < 0) return rc;
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-		antialiasing };
+		antialiasing, planar_depth };
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	int rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
@@ -1414,7 +1465,25 @@ int mgs_backward_views_distorted(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_planar(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho, fisheye,
+		distortion, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp,
+		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages,
+		debug, join_stream);
+}
+
+int mgs_backward_views_planar(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int planar_depth,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
+	if (V > 0 && views && check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
@@ -1434,7 +1503,7 @@ int mgs_backward_views_distorted(
 	}
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
-		antialiasing };
+		antialiasing, planar_depth };
 	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, fisheye, distortion, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
 }
@@ -1525,6 +1594,15 @@ int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view
 	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
 	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_planar(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho,
+		fisheye, distortion, 0, D, M, F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -1532,6 +1610,7 @@ int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view
 	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1557,7 +1636,7 @@ int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view
 	// stage by stage across the views of every cloud, as in mgs_forward_views
 	for (int phase = 0; phase < 3; phase++) {
 		for (int b = 0; b < B; b++) {
-			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
 					distortion_of(distortion, v))
@@ -1670,12 +1749,23 @@ int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* vie
 	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int accumulate, int debug,
 	void* join_stream)
 {
+	return mgs_backward_clouds_planar(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
+		ortho, fisheye, distortion, 0, D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int accumulate, int debug,
+	void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
 	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1705,7 +1795,7 @@ int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* vie
 	rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
 	for (int b = 0; b < B; b++) {
-		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
 		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
 			mgs_view w = views[v];
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
@@ -1734,6 +1824,7 @@ int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* vie
 		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0; pb.fisheye = 0; pb.distorted = 0;
 		for (float*& r : pb.cam_rows) r = nullptr;
 		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
+		for (int u = 0; u < MAX_BWD_VIEWS; u++) { pb.pl_g[u] = nullptr; pb.pl_q[u] = nullptr; pb.pl_mean[u] = nullptr; }
 		return 0;
 	};
 	for (int b = 0; b < B; b++) {
@@ -1760,6 +1851,8 @@ int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* vie
 				pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << (nv + u));
 				set_fisheye(fisheye_of(fisheye, v0 + u), nv + u, pb.fisheye, pb.fe_k);
 				set_distortion(distortion_of(distortion, v0 + u), nv + u, pb.distorted, pb.dc_k);
+				planar_view(cloud_of(k, D, M, F, scale_modifier, antialiasing, planar_depth), views[v0 + u], pb.pl_g[nv + u], pb.pl_q[nv + u],
+					pb.pl_mean[nv + u]);
 			}
 			nv += n;
 		}

@@ -108,8 +108,10 @@ __device__ __forceinline__ void depth_mask_cotangents(const BlendArgs& a, size_t
 // F <= 32 (one channel group); channel groups run blend_bwd_groups_kernel below.  DM: the depth / mask heads
 // (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.  NRM: the normal plane
 // (BlendArgs::nrm / dL_dnormal / gn): the quad {nx, ny, nz, 0} and its cotangent fill columns 4..7 of the {r,g,b,depth} tile,
-// so GEMM 1 and GEMM 2 carry them as issued, and the flush adds dL/dn into gn; likewise.
-template <int NFT, bool VEC, bool DM, bool NRM>
+// so GEMM 1 and GEMM 2 carry them as issued, and the flush adds dL/dn into gn; likewise.  PLN: planar depth
+// (BlendArgs::planar): the quad {a, b, e, 0} fills the same columns and the depth cotangent g enters them as {g px, g py, g, 0},
+// so dL/dalpha is that of the planar depth, and the flush adds {dL/da, dL/db, dL/de, 0} into gn; likewise.
+template <int NFT, bool VEC, bool DM, bool NRM, bool PLN>
 __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendArgs a)
 {
 	constexpr int NT = NFT + 1;          // channel tiles of 8: NFT feature tiles + {r,g,b,depth, 4 x zero}
@@ -180,6 +182,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			grow[2 * (RGBD + c)] = g4[c];
 			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
 			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside) ? a.dL_dnormal[c * HW + pix] : 0.f;
+			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)pxi : c == 1 ? g4[3] * (float)pyi : c == 2 ? g4[3] : 0.f;
 		}
 		if (NFT > 0) {
 #pragma unroll
@@ -384,12 +387,12 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					}
 				}
 				if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
-				if (NRM && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
+				if ((NRM || PLN) && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
 			} else if (lane < cnt) {
 				const uint32_t id = bwd_row_id(__float_as_uint(s_q[2 * lane + 1].w));
 				float* row = s_rows + lane * RS;
 				*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
-				if (NRM) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
+				if (NRM || PLN) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
 				if (NFT > 0) {
 					const float* f = a.feature + (size_t)id * F;
 #pragma unroll
@@ -484,7 +487,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 					if (tig < 3) *reinterpret_cast<float2*>(s_m + g * 12 + 2 * tig) = make_float2(mom[mt][2 * h], mom[mt][2 * h + 1]);
 					if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 					// columns 4..7 of the tile, {dnx, dny, dnz, 0}, behind the [BWD_CH][12] rows
-					if (NRM && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
+					if ((NRM || PLN) && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 					// F = 32: lane tig holds features 8 tig .. 8 tig + 7 of row g, one 32-byte sector (lo = the first four, hi
 					// = the last four).  Lanes tig and tig ^ 1 swap halves so that each red.v4 below pairs with its neighbour's
 					// into one whole sector: lane 2u + e adds into 16 u + 4 e (sector 2u: its own lo and the odd lane's lo), then
@@ -546,7 +549,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				red_add_v4(gb, dmx, dmy, -0.5f * q_dxx, -0.5f * q_dxy);
 				red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 				red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}
-				if (NRM) {
+				if (NRM || PLN) {
 					const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
 					red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
 				}
@@ -615,7 +618,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 
 // Channel groups (F > 32, BlendArgs::groups): the same replay with one warp per block doing every step, 12 CTAs per SM.
 // At F = 64 and 128 the launch is several waves deep, and there the two-warp kernel measured slower on an H100.
-template <bool VEC, bool DM, bool NRM>
+template <bool VEC, bool DM, bool NRM, bool PLN>
 __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 {
 	constexpr int NFT = 4;
@@ -682,6 +685,8 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 			grow[2 * (RGBD + c)] = g4[c];
 			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
 			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside && first) ? a.dL_dnormal[c * HW + pix] : 0.f;
+			// PLN: g4 is zero outside the image and in groups >= 1
+			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)pxi : c == 1 ? g4[3] * (float)pyi : c == 2 ? g4[3] : 0.f;
 		}
 		if (NFT > 0) {
 #pragma unroll
@@ -770,12 +775,12 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				}
 			}
 			if (lane < cnt) cp_async16(s_rows + lane * RS + RGBD, a.rgbd + myid);
-			if (NRM && first && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
+			if ((NRM || PLN) && first && lane < cnt) cp_async16(s_rows + lane * RS + RGBD + 4, a.nrm + myid);
 		} else if (lane < cnt) {
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
 			*reinterpret_cast<float4*>(row + RGBD) = a.rgbd[id];
-			if (NRM && first) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
+			if ((NRM || PLN) && first) *reinterpret_cast<float4*>(row + RGBD + 4) = a.nrm[id];
 			if (NFT > 0) {
 				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
@@ -903,7 +908,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 				if (tig < 3) *reinterpret_cast<float2*>(s_m + g * 12 + 2 * tig) = make_float2(mom[mt][2 * h], mom[mt][2 * h + 1]);
 				if (tig < 2) *reinterpret_cast<float2*>(s_m + g * 12 + 6 + 2 * tig) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 				// columns 4..7 of the tile, {dnx, dny, dnz, 0}, behind the [BWD_CH][12] rows
-				if (NRM && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
+				if ((NRM || PLN) && tig >= 2) *reinterpret_cast<float2*>(s_m + BWD_CH * 12 + g * 4 + 2 * (tig - 2)) = make_float2(dC[mt][NFT][2 * h], dC[mt][NFT][2 * h + 1]);
 				if (NFT > 0 && g < cnt && a.dL_dfeat) {
 					const uint32_t id = __float_as_uint(s_q[2 * g + 1].w);
 					red_feature_row<NFT, VEC, GRP>(a.dL_dfeat + (size_t)id * F + c0, dC[mt], h, tig, Fg);
@@ -928,7 +933,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 			red_add_v4(gb, dmx, dmy, -0.5f * q_dxx, -0.5f * q_dxy);
 			red_add_v4(gb + 4, -0.5f * q_dyy, __fdividef(m0.x, op), m1.z, m1.w);
 			if (first) red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}: zero in the other groups
-			if (NRM && first) {
+			if ((NRM || PLN) && first) {
 				const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
 				red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
 			}
@@ -950,55 +955,67 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 
 bool feature_rows_vectorizable(const float* feature, int F);
 
-template <int NFT, bool DM, bool NRM>
+template <int NFT, bool DM, bool NRM, bool PLN>
 static void launch_bwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8;
 	const bool vec = (NFT == 0) || (a.F == 8 * NFT && feature_rows_vectorizable(a.feature, a.F) &&
 		(reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0);
-	if (vec) blend_bwd_kernel<NFT, true, DM, NRM><<<grid, 64, 0, s>>>(a);
-	else blend_bwd_kernel<NFT, false, DM, NRM><<<grid, 64, 0, s>>>(a);
+	if (vec) blend_bwd_kernel<NFT, true, DM, NRM, PLN><<<grid, 64, 0, s>>>(a);
+	else blend_bwd_kernel<NFT, false, DM, NRM, PLN><<<grid, 64, 0, s>>>(a);
 }
 
-template <bool DM, bool NRM>
+template <bool DM, bool NRM, bool PLN = false>
 static void launch_bwd_dm(const BlendArgs& a, cudaStream_t s)
 {
 	if (a.groups > 1) {
 		const int grid = a.grid_x * a.grid_y * 8 * a.groups;
 		const bool vec = feature_rows_vectorizable(a.feature, a.F) && (reinterpret_cast<uintptr_t>(a.dL_dfeat) & 15) == 0;
-		if (vec) blend_bwd_groups_kernel<true, DM, NRM><<<grid, 32, 0, s>>>(a);
-		else blend_bwd_groups_kernel<false, DM, NRM><<<grid, 32, 0, s>>>(a);
+		if (vec) blend_bwd_groups_kernel<true, DM, NRM, PLN><<<grid, 32, 0, s>>>(a);
+		else blend_bwd_groups_kernel<false, DM, NRM, PLN><<<grid, 32, 0, s>>>(a);
 		return;
 	}
 	switch (nft_for(a.F)) {
-	case 0: launch_bwd_t<0, DM, NRM>(a, s); break;
-	case 1: launch_bwd_t<1, DM, NRM>(a, s); break;
-	case 2: launch_bwd_t<2, DM, NRM>(a, s); break;
-	default: launch_bwd_t<4, DM, NRM>(a, s); break;
+	case 0: launch_bwd_t<0, DM, NRM, PLN>(a, s); break;
+	case 1: launch_bwd_t<1, DM, NRM, PLN>(a, s); break;
+	case 2: launch_bwd_t<2, DM, NRM, PLN>(a, s); break;
+	default: launch_bwd_t<4, DM, NRM, PLN>(a, s); break;
 	}
 }
 
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.nrm) launch_bwd_dm<false, true>(a, s);  // never with the depth / mask heads (launch_blend_fwd)
+	if (a.planar) {  // never with the normal plane (launch_blend_fwd)
+		if (a.tgt_depth || a.tgt_mask) launch_bwd_dm<true, false, true>(a, s);
+		else launch_bwd_dm<false, false, true>(a, s);
+	} else if (a.nrm) launch_bwd_dm<false, true>(a, s);  // never with the depth / mask heads (launch_blend_fwd)
 	else if (a.tgt_depth || a.tgt_mask) launch_bwd_dm<true, false>(a, s);
 	else launch_bwd_dm<false, false>(a, s);
 }
 
 // The median depth is the view-space z of one Gaussian per pixel, chosen by a piecewise-constant rule: its cotangent goes to
-// that Gaussian's depth slot of the blend-stage records and nowhere else.  One thread per pixel.
-__global__ void median_depth_bwd_kernel(int N, const int* __restrict__ median_id, const float* __restrict__ dL_dmedian, float* gb)
+// that Gaussian's depth slot of the blend-stage records and nowhere else.  One thread per pixel.  PLN (planar depth): the
+// median depth is z + a px + b py + e, so the cotangent also goes to the contributor's quad gradients gn.
+template <bool PLN>
+__global__ void median_depth_bwd_kernel(int N, const int* __restrict__ median_id, const float* __restrict__ dL_dmedian, float* gb, int W,
+	float* gn)
 {
 	const int p = blockIdx.x * blockDim.x + threadIdx.x;
 	if (p >= N) return;
 	const int id = median_id[p];
 	const float g = dL_dmedian[p];
 	if (id >= 0 && g != 0.f) red_add(gb + (size_t)id * GB_STRIDE + 9, g);
+	if (PLN && id >= 0 && g != 0.f) {
+		const int py = p / W, px = p - py * W;
+		red_add_v4(gn + (size_t)id * 4, g * (float)px, g * (float)py, g, 0.f);
+	}
 }
 
-void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s)
+void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s, int W, float* gn)
 {
-	if (N > 0) median_depth_bwd_kernel<<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb);
+	if (N <= 0) return;
+	if (gn) median_depth_bwd_kernel<true><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn);
+	else median_depth_bwd_kernel<false><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn);
 }
 
 }  // namespace mgs

@@ -46,7 +46,9 @@ static_assert(FWD_CH % 8 == 0 && FWD_CH <= 32, "forward chunk size");
 // MED: the median contributor (BlendArgs::median_id / out_median_depth); likewise.
 // NRM: the normal plane (BlendArgs::nrm / out_normal): the per-Gaussian quad {nx, ny, nz, 0} fills columns 4..7 of the
 // {r,g,b,depth} tile, zero padding otherwise, so the MMAs the kernel issues anyway blend it; likewise.
-template <int NFT, bool VEC, bool GRP, bool DM, bool MED, bool NRM>
+// PLN: planar depth (BlendArgs::planar): the quad {a, b, e, 0} fills the same columns, and the depth is col3 + px col4 +
+// py col5 + col6 (also for the depth / mask heads); the median depth is its contributor's z + a px + b py + e; likewise.
+template <int NFT, bool VEC, bool GRP, bool DM, bool MED, bool NRM, bool PLN>
 __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendArgs a)
 {
 	using L = RowLayout<NFT>;
@@ -133,12 +135,12 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				}
 			}
 			if (lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD, a.rgbd + myid);
-			if (NRM && lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD + 4, a.nrm + myid);
+			if ((NRM || PLN) && lane < cnt && first) cp_async16(s_rows + lane * RS + L::RGBD + 4, a.nrm + myid);
 		} else if (lane < cnt) {  // feature rows that are not whole 8-wide tiles (e.g. F = 3): plain loads, zero padded
 			const uint32_t id = __float_as_uint(s_q[2 * lane + 1].w);
 			float* row = s_rows + lane * RS;
 			if (first) *reinterpret_cast<float4*>(row + L::RGBD) = a.rgbd[id];
-			if (NRM && first) *reinterpret_cast<float4*>(row + L::RGBD + 4) = a.nrm[id];
+			if ((NRM || PLN) && first) *reinterpret_cast<float4*>(row + L::RGBD + 4) = a.nrm[id];
 			if (NFT > 0) {
 				const float* f = a.feature + (size_t)id * F + c0;
 #pragma unroll
@@ -206,8 +208,8 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				mma_3xtf32(acc[1][nt], ahi[1], alo[1], bh0, bh1, bl0, bl1);
 			}
 			if (first) {
-				const float c0 = (NRM || gid < 4) ? row0[L::RGBD + gid] : 0.f;
-				const float c1 = (NRM || gid < 4) ? row1[L::RGBD + gid] : 0.f;
+				const float c0 = (NRM || PLN || gid < 4) ? row0[L::RGBD + gid] : 0.f;
+				const float c1 = (NRM || PLN || gid < 4) ? row1[L::RGBD + gid] : 0.f;
 				uint32_t bh0, bl0, bh1, bl1;
 				tf32_split(c0, bh0, bl0);
 				tf32_split(c1, bh1, bl1);
@@ -233,7 +235,14 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 				// the entry's tile-list position names the Gaussian; its depth is the value the depth channel blends
 				const int id = med ? (int)a.point_list[range.x + lrow[med - 1]] : -1;
 				a.median_id[pix] = id;
-				if (a.out_median_depth) a.out_median_depth[pix] = med ? a.rgbd[id].w : 0.f;
+				if constexpr (PLN) {
+					// the contributor's planar depth z + a px + b py + e at this pixel
+					if (a.out_median_depth) {
+						float md = 0.f;
+						if (med) { const float4 q = a.nrm[id]; md = a.rgbd[id].w + q.x * pfx + q.y * pfy + q.z; }
+						a.out_median_depth[pix] = md;
+					}
+				} else if (a.out_median_depth) a.out_median_depth[pix] = med ? a.rgbd[id].w : 0.f;
 			}
 		}
 	}
@@ -260,6 +269,14 @@ __global__ void __launch_bounds__(32, MGS_FWD_MIN_CTAS) blend_fwd_kernel(BlendAr
 			const bool in = ox < a.W && oy < a.H;
 			const size_t pix = in ? (size_t)a.W * oy + ox : 0;
 			const float Tp = s_w[4 * gid + y];
+			if constexpr (PLN) {
+				// the depth, column 3 on thread tig = 1, gains px col4 + py col5 + col6 from threads tig = 2 and 3 of the quad
+				const int q0 = lane & ~3;
+				const float c4 = __shfl_sync(0xffffffffu, acc[mt][NFT][2 * h], q0 | 2);
+				const float c5 = __shfl_sync(0xffffffffu, acc[mt][NFT][2 * h + 1], q0 | 2);
+				const float c6 = __shfl_sync(0xffffffffu, acc[mt][NFT][2 * h], q0 | 3);
+				if (tig == 1) acc[mt][NFT][2 * h + 1] += (float)ox * c4 + (float)oy * c5 + c6;
+			}
 #pragma unroll
 			for (int nt = 0; nt < NFT; nt++) {
 #pragma unroll
@@ -378,7 +395,7 @@ bool feature_rows_vectorizable(const float* feature, int F)
 	return F > 0 && (F & 3) == 0 && (reinterpret_cast<uintptr_t>(feature) & 15) == 0;
 }
 
-template <int NFT, bool GRP, bool DM, bool MED, bool NRM>
+template <int NFT, bool GRP, bool DM, bool MED, bool NRM, bool PLN>
 static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 {
 	const int grid = a.grid_x * a.grid_y * 8 * a.groups;
@@ -386,26 +403,32 @@ static void launch_fwd_t(const BlendArgs& a, cudaStream_t s)
 	// groups, a row slice starts at channel 32 g: 16-byte aligned whenever F % 4 == 0, and a remainder group copies whole
 	// 4-channel pieces only.
 	const bool vec = (NFT == 0) || ((a.F == 8 * NFT || GRP) && feature_rows_vectorizable(a.feature, a.F));
-	if (vec) blend_fwd_kernel<NFT, true, GRP, DM, MED, NRM><<<grid, 32, 0, s>>>(a);
-	else blend_fwd_kernel<NFT, false, GRP, DM, MED, NRM><<<grid, 32, 0, s>>>(a);
+	if (vec) blend_fwd_kernel<NFT, true, GRP, DM, MED, NRM, PLN><<<grid, 32, 0, s>>>(a);
+	else blend_fwd_kernel<NFT, false, GRP, DM, MED, NRM, PLN><<<grid, 32, 0, s>>>(a);
 }
 
-template <bool DM, bool MED, bool NRM>
+template <bool DM, bool MED, bool NRM, bool PLN = false>
 static void launch_fwd_dm(const BlendArgs& a, cudaStream_t s)
 {
-	if (a.groups > 1) { launch_fwd_t<4, true, DM, MED, NRM>(a, s); return; }
+	if (a.groups > 1) { launch_fwd_t<4, true, DM, MED, NRM, PLN>(a, s); return; }
 	switch (nft_for(a.F)) {
-	case 0: launch_fwd_t<0, false, DM, MED, NRM>(a, s); break;
-	case 1: launch_fwd_t<1, false, DM, MED, NRM>(a, s); break;
-	case 2: launch_fwd_t<2, false, DM, MED, NRM>(a, s); break;
-	default: launch_fwd_t<4, false, DM, MED, NRM>(a, s); break;
+	case 0: launch_fwd_t<0, false, DM, MED, NRM, PLN>(a, s); break;
+	case 1: launch_fwd_t<1, false, DM, MED, NRM, PLN>(a, s); break;
+	case 2: launch_fwd_t<2, false, DM, MED, NRM, PLN>(a, s); break;
+	default: launch_fwd_t<4, false, DM, MED, NRM, PLN>(a, s); break;
 	}
 }
 
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s)
 {
 	const bool dm = a.tgt_color && (a.tgt_depth || a.tgt_mask);
-	if (a.nrm) {  // never with the depth / mask heads: the entry points refuse that pair, so it has no instantiation
+	if (a.planar) {  // never with the normal plane: both take columns 4..6 (the entry points refuse the pair)
+		if (a.median_id) {
+			if (dm) launch_fwd_dm<true, true, false, true>(a, s);
+			else launch_fwd_dm<false, true, false, true>(a, s);
+		} else if (dm) launch_fwd_dm<true, false, false, true>(a, s);
+		else launch_fwd_dm<false, false, false, true>(a, s);
+	} else if (a.nrm) {  // never with the depth / mask heads: the entry points refuse that pair, so it has no instantiation
 		if (a.median_id) launch_fwd_dm<false, true, true>(a, s);
 		else launch_fwd_dm<false, false, true>(a, s);
 	} else if (a.median_id) {

@@ -120,6 +120,13 @@ struct ProjectBwdViewsArgs {
 	// CAM: they serve all four models) read them; the launcher picks them when any bit is set.  Behind fe_k for the same reason.
 	uint16_t distorted;
 	DistK dc_k[MAX_BWD_VIEWS];
+	// planar depth: view u's blend-stage quad gradients pl_g [P] ({dL/da, dL/db, dL/de, 0}), its forward quads pl_q [P]
+	// ({a, b, e, 0}, planar.cu) and its screen means pl_mean [P] (pixels), or NULL where the view has none.  Only the planar
+	// kernels (project_bwd_{views,clouds}_planar_kernel: the DIST body, all four models) read them; the launcher picks them when
+	// any is set.  Behind dc_k for the same reason as conic_opacity.
+	const float4* pl_g[MAX_BWD_VIEWS];
+	const float4* pl_q[MAX_BWD_VIEWS];
+	const float2* pl_mean[MAX_BWD_VIEWS];
 };
 // the 27 camera terms one CTA writes per view into its camera rows: dL/dvm[4c + r] at 3c + r (c < 4, r < 3), dL/dpm[4c + {0, 1,
 // 3}] at 12 + 3c + {0, 1, 2}, dL/dcampos at 24 + i.  The other 8 of the 35 outputs are constants of the forward.  The kernel
@@ -159,6 +166,9 @@ struct ProjectBwdCloudsArgs {
 struct ProjectBwdCloudsDistArgs : ProjectBwdCloudsArgs {
 	uint16_t distorted;                            // bit u: view u of the launch is a distorted-pinhole view
 	DistK dc_k[MAX_BWD_VIEWS];                     // per view of the launch, as in ProjectBwdViewsArgs
+	const float4* pl_g[MAX_BWD_VIEWS];             // per view of the launch, as in ProjectBwdViewsArgs (PLN only)
+	const float4* pl_q[MAX_BWD_VIEWS];
+	const float2* pl_mean[MAX_BWD_VIEWS];
 };
 static_assert(MAX_BWD_VIEWS <= 16, "the orthographic, fisheye and distorted view masks have 16 bits");
 static_assert(sizeof(ProjectBwdViewsArgs) <= 4096, "kernel parameters are limited to 4 KB");
@@ -252,6 +262,10 @@ struct BlendArgs {
 	float* out_normal;
 	const float* dL_dnormal;
 	float* gn;
+	// planar depth (the launchers pick the PLN instantiations when set): nrm holds the view's planar quads {a, b, e, 0}
+	// (planar.cu) instead, and the depth plane, the depth / mask heads and the median depth take each Gaussian's depth
+	// z + a px + b py + e at pixel (px, py).  Backward: gn receives {dL/da, dL/db, dL/de, 0}.  Behind gn for the same reason.
+	int planar;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
 	// the block's list (forward) or replayed (backward), SM id, block id} -- the timeline of the blend CTAs across kernels and streams
@@ -341,8 +355,10 @@ int blend_supported(int F);
 int blend_groups(int F);  // channel groups of 32 (BlendArgs::groups)
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s);
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
-// the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0
-void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s);
+// the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0;
+// with gn (planar depth, W the image width) also gn[median_id[p]] += dL_dmedian[p] {px, py, 1, 0}
+void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s, int W = 0,
+	float* gn = nullptr);
 
 // lift.cu: lifted[id][c] += sum_p w_p,id map[c][p] and weight[id] += sum_p w_p,id over one view's pixels, w = alpha T the
 // forward blend's weights (include/mgs_rasterizer.h, mgs_lift_views).  The tile grid, lists and records are the view's, as
@@ -380,5 +396,25 @@ struct NormalsBwdArgs {
 	const float* cam_pos[MAX_BWD_VIEWS];
 };
 void launch_normals_bwd(const NormalsBwdArgs& a, cudaStream_t s);
+
+// planar.cu: quad[i] = {a, b, e, 0} of Gaussian i in one view (include/mgs_rasterizer.h, planar depth): (a, b) = k Q with
+// k = e3^T Sigma_c J^T and Q the conic of the projection's record, e = -(a mu_x + b mu_y); zeros where radii[i] == 0
+struct PlanarFwdArgs {
+	int P;
+	const float* means3D;
+	const float* cov3D;          // [P,6] world-space covariance: the caller's, or the projection's own
+	const float* viewmatrix;
+	int W, H;
+	float tan_fovx, tan_fovy;    // host field of view (tan_fov NULL)
+	const float* tan_fov;        // device {tan_fovx, tan_fovy}, or NULL
+	int model;                   // 0 pinhole, 1 orthographic, 2 fisheye, 3 distorted pinhole
+	FisheyeK fe_k;
+	DistK dc_k;
+	const int* radii;
+	const float2* means2D;
+	const float4* conic_opacity;
+	float4* quad;
+};
+void launch_planar_fwd(const PlanarFwdArgs& a, cudaStream_t s);
 
 }  // namespace mgs

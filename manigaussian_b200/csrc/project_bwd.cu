@@ -89,7 +89,14 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // (du, dv); J = F Dd P with F = diag(fx, fy), P = d(x, y) / dt = [[1/z, 0, -x/z], [0, 1/z, -y/z]].  With G = F dL/dJ,
 // dL/dJ : dJ/dt = (G P^T) : dDd/d(x, y) chained through P, plus (Dd G) : dP/dt (Dd is symmetric); J^T (du, dv) enters through
 // the same chain.  The camera terms and dL/dtan_fov are the fisheye ones with u - cx = fx xd.
-template <int NSH, bool AA, bool CAM, bool ORTHO, bool FISH, bool DIST, class Args>
+//
+// PLN (DIST, FISH, ORTHO and CAM only): planar depth on the views with a.pl_g[v] set.  The blend's quad gradients {ga, gb, ge}
+// of (a, b, e = -(a mu_x + b mu_y)) give dL/d(a, b) = (ga - mu_x ge, gb - mu_y ge) and, through e, the screen mean's cotangent
+// -(a, b) ge in pixels, added to dm in its convention.  With (a, b) = k Q, k_j = Rv2^T S m_j (m_j row j of M = J Rv):
+// dL/dQ = k^T dL/d(a, b) joins G, dk = dL/d(a, b) Q, and dk reaches S (sym(Rv2 n^T), n = dk_0 m_0 + dk_1 m_1), M (dL/dm_j +=
+// dk_j S Rv2, so the existing chain carries it through J to t, the camera and the field of view) and the third row of Rv
+// (dk_0 S m_0 + dk_1 S m_1).
+template <int NSH, bool AA, bool CAM, bool ORTHO, bool FISH, bool DIST, bool PLN, class Args>
 __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int idx_in, const bool in, float* cam_sm)
 {
 	const int idx = CAM && !in ? 0 : idx_in;
@@ -152,7 +159,18 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 		for (int k = 0; k < 32; k++) cg[k] = 0.f;
 		if (live) {
 			dm[0] = g0.x; dm[1] = g0.y;
-			const float gA = g0.z, gB = g0.w, gC = g1.x;        // dL/dconic (xx, xy halved, yy)
+			float gA = g0.z, gB = g0.w, gC = g1.x;              // dL/dconic (xx, xy halved, yy)
+			bool plv = false;                                   // PLN: the view has planar depth
+			float pga = 0.f, pgb = 0.f;                         // PLN: dL/d(a, b), e's share included
+			if constexpr (PLN) {
+				plv = a.pl_g[v] != nullptr;
+				if (plv) {
+					const float4 g = a.pl_g[v][idx], q = a.pl_q[v][idx];
+					const float2 mu = a.pl_mean[v][idx];
+					pga = g.x - mu.x * g.z; pgb = g.y - mu.y * g.z;
+					dm[0] -= q.x * g.z * (0.5f * a.intr[v].W); dm[1] -= q.y * g.z * (0.5f * a.intr[v].H);
+				}
+			}
 			const float dcol[3] = { g1.z, g1.w, g2.x };
 			const float ddepth = g2.y;
 			if (!AA) gop += g1.y;
@@ -226,6 +244,21 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const float a0 = dot3(m0, u0), c0 = dot3(m1, u1);
 			const float ca = a0 + 0.3f, cb = dot3(m0, u1), cc = c0 + 0.3f;
 			const float det = ca * cc - cb * cb;
+			float dk0 = 0.f, dk1 = 0.f;  // PLN: dL/dk
+			if constexpr (PLN) {
+				if (plv) {
+					const float k0 = dot3(Rv[2], u0), k1 = dot3(Rv[2], u1);
+					const float idet = 1.0f / det, QA = cc * idet, QB = -cb * idet, QC = ca * idet;
+					gA += k0 * pga; gC += k1 * pgb; gB += 0.5f * (k0 * pgb + k1 * pga);
+					dk0 = pga * QA + pgb * QB; dk1 = pga * QB + pgb * QC;
+					float n[3];
+#pragma unroll
+					for (int c = 0; c < 3; c++) n[c] = dk0 * m0[c] + dk1 * m1[c];
+					const float* r2 = Rv[2];
+					D[0] += r2[0] * n[0]; D[1] += 0.5f * (r2[0] * n[1] + n[0] * r2[1]); D[2] += 0.5f * (r2[0] * n[2] + n[0] * r2[2]);
+					D[3] += r2[1] * n[1]; D[4] += 0.5f * (r2[1] * n[2] + n[1] * r2[2]); D[5] += r2[2] * n[2];
+				}
+			}
 			const float wgt = 1.0f / (det * det + 0.0000001f);
 			// H = -w adj(S') G adj(S')
 			const float e00 = cc * gA - cb * gB, e01 = cc * gB - cb * gC, e10 = ca * gB - cb * gA, e11 = ca * gC - cb * gB;
@@ -253,6 +286,15 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			float q0[3], q1[3];
 #pragma unroll
 			for (int c = 0; c < 3; c++) { q0[c] = 2.f * (H00 * u0[c] + H01 * u1[c]); q1[c] = 2.f * (H01 * u0[c] + H11 * u1[c]); }
+			if constexpr (PLN) {
+				if (plv) {
+#pragma unroll
+					for (int c = 0; c < 3; c++) {
+						const float sr = dot3(S[c], Rv[2]);
+						q0[c] += dk0 * sr; q1[c] += dk1 * sr;
+					}
+				}
+			}
 			const float dJ00 = dot3(q0, Rv[0]), dJ02 = dot3(q0, Rv[2]), dJ11 = dot3(q1, Rv[1]), dJ12 = dot3(q1, Rv[2]);
 			if constexpr (CAM) {
 				// dL/dtan_fov: fx = W / (2 tan_fovx) moves J00 = fx / tz and J02 = -fx cx / tz^2 (dfx / dtan_fovx = -fx / tan_fovx),
@@ -335,6 +377,10 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 					cg[3 * c + 1] = dt[1] * p[c] + j11 * q1[c];
 					cg[3 * c + 2] = dt[2] * p[c] + j02 * q0[c] + j12 * q1[c];
 					if (full) { cg[3 * c] += j10 * q1[c]; cg[3 * c + 1] += j01 * q0[c]; }
+				}
+				if constexpr (PLN) {
+#pragma unroll
+					for (int c = 0; c < 3; c++) cg[3 * c + 2] += dk0 * u0[c] + dk1 * u1[c];  // k through the third row of Rv
 				}
 				cg[9] = dt[0]; cg[10] = dt[1]; cg[11] = dt[2];
 				// (hx, hy, hw) = P (p, 1): dL/dhx = dm0 iw, dL/dhy = dm1 iw, dL/dhw = -(dm0 kx + dm1 ky)
@@ -485,7 +531,7 @@ __device__ __forceinline__ void cam_rows_out(const float* cam_sm, int V, float* 
 
 // DIST, FISH, ORTHO, CAM, AA last in the template list: AA stays the last argument of every kernel name and CAM the one before
 // it, as profiles and the coverage tests read them.  ORTHO is instantiated with CAM only, FISH with ORTHO and CAM only, DIST
-// with FISH, ORTHO and CAM only.
+// with FISH, ORTHO and CAM only.  The planar-depth backward (PLN) has kernels of its own names below.
 template <int NSH, int MIN_BLOCKS, bool DIST, bool FISH, bool ORTHO, bool CAM, bool AA>
 __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(ProjectBwdViewsArgs a)
 {
@@ -495,11 +541,11 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_kernel(Proj
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if constexpr (CAM) {
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(a, idx, idx < a.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST, false>(a, idx, idx < a.P, cam_sm);
 		cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
 	} else {
 		if (idx >= a.P) return;
-		project_bwd_gaussian<NSH, AA, false, false, false, false>(a, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false, false, false>(a, idx, true, nullptr);
 	}
 }
 
@@ -522,6 +568,12 @@ struct CloudBwd {
 	const FisheyeK* fe_k;                // FISH only: per view of the cloud
 	unsigned distorted;                  // DIST only: bit v, view v of the cloud is a distorted-pinhole view
 	const DistK* dc_k;                   // DIST only: per view of the cloud
+};
+// PLN only: with each view's planar-depth arrays (a type of its own, so the other instantiations keep their code)
+struct CloudBwdPln : CloudBwd {
+	const float4* const* pl_g;
+	const float4* const* pl_q;
+	const float2* const* pl_mean;
 };
 // the parameter block a clouds launch passes: the larger one for the DIST kernels (mgs_kernels.h), the parent's otherwise
 template <bool DIST>
@@ -550,10 +602,10 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(cb, idx, idx < cl.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST, false>(cb, idx, idx < cl.P, cam_sm);
 		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
-		project_bwd_gaussian<NSH, AA, false, false, false, false>(cb, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false, false, false>(cb, idx, true, nullptr);
 	}
 }
 template <int NSH, int MIN_BLOCKS, bool DIST, bool FISH, bool ORTHO, bool CAM, bool AA>
@@ -572,11 +624,38 @@ __global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_kernel(Pro
 	if constexpr (CAM) {
 		// the CTA serves one cloud: its rows belong to that cloud's views
 		__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
-		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST>(cb, idx, idx < cl.P, cam_sm);
+		project_bwd_gaussian<NSH, AA, true, ORTHO, FISH, DIST, false>(cb, idx, idx < cl.P, cam_sm);
 		cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 	} else {
-		project_bwd_gaussian<NSH, AA, false, false, false, false>(cb, idx, true, nullptr);
+		project_bwd_gaussian<NSH, AA, false, false, false, false, false>(cb, idx, true, nullptr);
 	}
+}
+
+// planar depth (PLN): the DIST, FISH, ORTHO and CAM body with the planar terms, for every model; kernels of their own names, so
+// that the names of the kernels above stay as profiles and the coverage tests read them
+template <int NSH, int MIN_BLOCKS, bool AA>
+__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_views_planar_kernel(ProjectBwdViewsArgs a)
+{
+	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+	__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
+	project_bwd_gaussian<NSH, AA, true, true, true, true, true>(a, idx, idx < a.P, cam_sm);
+	cam_rows_out(cam_sm, a.V, a.cam_rows, a.intr, blockIdx.x);
+}
+template <int NSH, int MIN_BLOCKS, bool AA>
+__global__ void __launch_bounds__(128, MIN_BLOCKS) project_bwd_clouds_planar_kernel(ProjectBwdCloudsDistArgs a)
+{
+	int c = 0;
+	while (c + 1 < a.B && (int)blockIdx.x >= a.cloud[c + 1].block0) c++;
+	const ProjectBwdCloud& cl = a.cloud[c];
+	const int idx = ((int)blockIdx.x - cl.block0) * blockDim.x + threadIdx.x;
+	const CloudBwdPln cp{ { a.D, a.M, cl.V, cl.means3D, cl.shs, cl.scales, cl.rotations, a.scale_modifier, cl.cov3D_precomp,
+		cl.accumulate, cl.dL_dmean3D, cl.dL_dopacity, cl.dL_dcolor, cl.dL_dcov3D, cl.dL_dsh, cl.dL_dscale, cl.dL_drot, a.view + cl.view0,
+		AA ? a.conic_opacity + cl.view0 : nullptr, a.intr + cl.view0, (unsigned)a.ortho >> cl.view0, (unsigned)a.fisheye >> cl.view0,
+		a.fe_k + cl.view0, (unsigned)a.distorted >> cl.view0, a.dc_k + cl.view0 },
+		a.pl_g + cl.view0, a.pl_q + cl.view0, a.pl_mean + cl.view0 };
+	__shared__ float cam_sm[4 * MAX_BWD_VIEWS * CAM_ALL_TERMS];
+	project_bwd_gaussian<NSH, AA, true, true, true, true, true>(cp, idx, idx < cl.P, cam_sm);
+	cam_rows_out(cam_sm, cl.V, a.cam_rows + cl.view0, a.intr + cl.view0, (int)blockIdx.x - cl.block0);
 }
 
 // one CTA of CAM_REDUCE_THREADS per view.  Thread t first sums rows t, t + 256, ... of every column in row order, then a
@@ -658,6 +737,40 @@ static void project_bwd_views(const ProjectBwdViewsArgs& a, int grid, int deg, c
 	else project_bwd_views_kernel<48, 3, DIST, FISH, ORTHO, CAM, false><<<grid, 128, 0, s>>>(a);
 }
 
+// the PLN kernels at the blocks per SM of the DIST ones, except at degree 3 without AA: 2, the planar terms spill at the cap of
+// 3 (168 registers)
+static void launch_planar_views(const ProjectBwdViewsArgs& a, int grid, int deg, cudaStream_t s)
+{
+	if (a.antialias) {
+		if (deg <= 1) project_bwd_views_planar_kernel<12, 3, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_planar_kernel<27, 3, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_planar_kernel<48, 2, true><<<grid, 128, 0, s>>>(a);
+	} else {
+		if (deg <= 1) project_bwd_views_planar_kernel<12, 3, false><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_views_planar_kernel<27, 3, false><<<grid, 128, 0, s>>>(a);
+		else project_bwd_views_planar_kernel<48, 2, false><<<grid, 128, 0, s>>>(a);
+	}
+}
+static void launch_planar_clouds(const ProjectBwdCloudsDistArgs& a, int grid, int deg, cudaStream_t s)
+{
+	if (a.antialias) {
+		if (deg <= 1) project_bwd_clouds_planar_kernel<12, 3, true><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_planar_kernel<27, 3, true><<<grid, 128, 0, s>>>(a);
+		else project_bwd_clouds_planar_kernel<48, 2, true><<<grid, 128, 0, s>>>(a);
+	} else {
+		if (deg <= 1) project_bwd_clouds_planar_kernel<12, 3, false><<<grid, 128, 0, s>>>(a);
+		else if (deg == 2) project_bwd_clouds_planar_kernel<27, 3, false><<<grid, 128, 0, s>>>(a);
+		else project_bwd_clouds_planar_kernel<48, 2, false><<<grid, 128, 0, s>>>(a);
+	}
+}
+
+static bool planar_any(const float4* const* pl_g, int V)
+{
+	for (int u = 0; u < V; u++)
+		if (pl_g[u]) return true;
+	return false;
+}
+
 void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0 || a.V <= 0) return;
@@ -665,7 +778,8 @@ void launch_project_bwd_views(const ProjectBwdViewsArgs& a, cudaStream_t s)
 	const int deg = a.shs ? a.D : 0;
 	bool cam = false;  // camera rows, or a device field of view, which only the CAM instantiation reads
 	for (int u = 0; u < a.V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
-	if (a.distorted) project_bwd_views<true, true, true, true>(a, grid, deg, s);  // a distorted view: DIST, all four models
+	if (planar_any(a.pl_g, a.V)) launch_planar_views(a, grid, deg, s);  // planar depth: the PLN kernels, all four models
+	else if (a.distorted) project_bwd_views<true, true, true, true>(a, grid, deg, s);  // a distorted view: DIST, all four models
 	else if (a.fisheye) project_bwd_views<true, true, true>(a, grid, deg, s);  // a fisheye view: the FISH instantiation, all models
 	else if (a.ortho) project_bwd_views<true, true>(a, grid, deg, s);  // an orthographic view: the ORTHO instantiation of CAM
 	else if (cam) project_bwd_views<true, false>(a, grid, deg, s);
@@ -702,6 +816,10 @@ void launch_project_bwd_clouds(ProjectBwdCloudsDistArgs a, cudaStream_t s)
 	const int deg = sh ? a.D : 0;
 	bool cam = false;
 	for (int u = 0; u < V; u++) cam |= a.cam_rows[u] != nullptr || a.intr[u].tan_fov != nullptr;
+	if (planar_any(a.pl_g, V)) {
+		launch_planar_clouds(a, grid, deg, s);
+		return;
+	}
 	if (a.distorted) {
 		launch_clouds<true, true, true, true>(a, grid, deg, s);
 		return;

@@ -71,9 +71,16 @@ def _camera_scalars(nv, idx):
             int(nv["height"][idx]), int(nv["width"][idx]))
 
 
+def _with_planar_depth(s):
+    """The settings `s` with planar_depth=True (include/mgs_rasterizer.h, mgs_forward_views_planar), its other attributes kept."""
+    return GaussianRasterizationSettings(*tuple(s)[:13], antialiasing=getattr(s, "antialiasing", False),
+                                         orthographic=getattr(s, "orthographic", False), fisheye=getattr(s, "fisheye", None),
+                                         distortion=getattr(s, "distortion", None), planar_depth=True)
+
+
 def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=None, features_color=None,
            features_language=None, return_depth=False, return_alpha=False, antialiasing=False, return_median_depth=False,
-           return_normal=False):
+           return_normal=False, planar_depth=False):
     """Render view `idx` of data['novel_view'].  Same arguments and result as the reference's render(); with
     return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended, no background term), with
     return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth), with
@@ -97,7 +104,7 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
         image_height=H, image_width=W, tanfovx=tanfovx, tanfovy=tanfovy, bg=bg, scale_modifier=1.0,
         viewmatrix=nv["world_view_transform"][idx], projmatrix=nv["full_proj_transform"][idx],
         sh_degree=3 if features_color is None else 1, campos=nv["camera_center"][idx], prefiltered=False, debug=False,
-        include_feature=(features_language is not None), antialiasing=bool(antialiasing))
+        include_feature=(features_language is not None), antialiasing=bool(antialiasing), planar_depth=bool(planar_depth))
     rasterizer = GaussianRasterizer(raster_settings=raster_settings, return_depth=return_depth, return_alpha=return_alpha,
                                     return_median_depth=return_median_depth, return_normal=return_normal)
     shs, colors_precomp = None, None
@@ -418,7 +425,8 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
-                 targets=None, return_alpha=False, antialiasing=False, ssim=False, return_median_depth=False, return_normal=False):
+                 targets=None, return_alpha=False, antialiasing=False, ssim=False, return_median_depth=False, return_normal=False,
+                 planar_depth=False):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -464,6 +472,9 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     camera, blended with the colour's weights (differentiable: its gradient reaches the rotations, and opacities and means
     through the blend weights; not normalised, normal / alpha is the expected normal; INTEGRATION.md §8).  Not with targets:
     the depth / mask heads have no kernel beside it.
+    planar_depth: the depth plane, the depth head (targets["depth"]) and the median depth take each Gaussian's depth along
+    the pixel's ray, affine in the pixel offset, instead of its centre depth (include/mgs_rasterizer.h,
+    mgs_forward_views_planar); also on when the given settings carry planar_depth=True.  Not with return_normal.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -479,6 +490,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         batch = None
     if not views:
         raise ValueError("render_views needs at least one view")
+    if planar_depth:
+        views = tuple(_with_planar_depth(s) for s in views)
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for s in views)
     if features_color is None and pts_rgb is None:
         raise ValueError("Please provide excatly one of either SHs or precomputed colors!")
@@ -518,7 +531,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True,
                                            orthographic=getattr(views[0], "orthographic", False),
                                            fisheye=getattr(views[0], "fisheye", None),
-                                           distortion=getattr(views[0], "distortion", None)) if aa else views[0]
+                                           distortion=getattr(views[0], "distortion", None),
+                                           planar_depth=getattr(views[0], "planar_depth", False)) if aa else views[0]
         out = GaussianRasterizer(st, return_depth=return_depth, return_alpha=return_alpha, return_median_depth=return_median_depth,
                                  return_normal=return_normal)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
@@ -749,7 +763,7 @@ class _RasterizeClouds(torch.autograd.Function):
 
 
 def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normalize_feature=True, return_alpha=False,
-                  antialiasing=False, ssim=False, return_median_depth=False, return_normal=False):
+                  antialiasing=False, ssim=False, return_median_depth=False, return_normal=False, planar_depth=False):
     """Render several Gaussian clouds, each with its own cameras, in one autograd node: e.g. the current and the deformed
     next frame of ManiGaussian's dynamic-field step (neural_rendering.py:283, :324) for every sample of the batch.
 
@@ -766,7 +780,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     share camera tensors (the dyna pair) receive the sum.
     ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets.
     return_median_depth: every cloud also returns "median_depth" and "median_id" [V,H,W], as in render_views; not with targets.
-    return_normal: every cloud also returns "normal" [V,3,H,W], as in render_views; not with targets."""
+    return_normal: every cloud also returns "normal" [V,3,H,W], as in render_views; not with targets.
+    planar_depth: every cloud's depth follows each Gaussian's tilt, as in render_views."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
     with_targets = [c.get("targets") is not None for c in clouds]
@@ -808,6 +823,8 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         raise ValueError("clouds disagree on the SH degree")
     _prep_clouds([dict(means3D=c["pts_xyz"], sh=c.get("features_color"), colors=c.get("pts_rgb") if c.get("features_color") is None else None,
                        feature=c.get("features_language")) for c in clouds], device, True)
+    if planar_depth:
+        cloud_views = [tuple(_with_planar_depth(s) for s in views) for views in cloud_views]
     flat, vsps = [], []
     for c, views in zip(clouds, cloud_views):
         f = c.get("features_language")

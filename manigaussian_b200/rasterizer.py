@@ -300,8 +300,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         alpha = med_depth = med_id = normal = None
         if return_normal and (cov3Ds_precomp is not None and cov3Ds_precomp.numel() != 0):
             raise ValueError("return_normal needs scales and rotations: a precomputed covariance has no axis to take a normal from")
+        # planar depth, like the camera models, exists on the multi-view entry points only
         orth = bool(getattr(s, "orthographic", False)) or getattr(s, "fisheye", None) is not None \
-            or getattr(s, "distortion", None) is not None
+            or getattr(s, "distortion", None) is not None or bool(getattr(s, "planar_depth", False))
         ctx.orthographic = orth
         if (return_alpha or return_median or return_normal or aa or orth or ctx.camera) and views_path:
             # the alpha plane, the median planes, the anti-aliased, orthographic, fisheye and distorted projections and the camera
@@ -483,14 +484,20 @@ class GaussianRasterizationSettings(_Settings):
     `distortion` (default None; keyword, or positional after fisheye) is an attribute in the same way: the view's OpenCV
     parameters (cx, cy, k1, k2, p1, p2, k3, k4, k5, k6, r_max), or a dict with those keys, make it a distorted-pinhole view,
     with tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (include/mgs_rasterizer.h, mgs_forward_views_distorted;
-    cameras.build_distorted_cameras).  It cannot be combined with orthographic=True or fisheye."""
+    cameras.build_distorted_cameras).  It cannot be combined with orthographic=True or fisheye.
+    `planar_depth` (default False; keyword, or positional after distortion) is an attribute in the same way: True makes the
+    depth plane, the depth head and the median depth take each Gaussian's depth along the pixel's ray, affine in the pixel
+    offset, instead of its centre depth (include/mgs_rasterizer.h, mgs_forward_views_planar).  It is a per-call setting: the
+    views of one call must agree."""
     antialiasing = False
     orthographic = False
     fisheye = None
     distortion = None
+    planar_depth = False
 
     def __new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix, sh_degree, campos,
-                prefiltered, debug, include_feature, antialiasing=False, orthographic=False, fisheye=None, distortion=None):
+                prefiltered, debug, include_feature, antialiasing=False, orthographic=False, fisheye=None, distortion=None,
+                planar_depth=False):
         self = super().__new__(cls, image_height, image_width, tanfovx, tanfovy, bg, scale_modifier, viewmatrix, projmatrix,
                                sh_degree, campos, prefiltered, debug, include_feature)
         self.antialiasing = bool(antialiasing)
@@ -501,6 +508,7 @@ class GaussianRasterizationSettings(_Settings):
         self.distortion = _distortion_params(distortion)
         if self.distortion is not None and (self.orthographic or self.fisheye is not None):
             raise ValueError("a distorted view cannot also be orthographic or fisheye")
+        self.planar_depth = bool(planar_depth)
         return self
 
     @classmethod
@@ -512,11 +520,13 @@ class GaussianRasterizationSettings(_Settings):
         orth = kw.pop("orthographic", self.orthographic)
         fe = kw.pop("fisheye", self.fisheye)
         dc = kw.pop("distortion", self.distortion)
-        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth, fisheye=fe, distortion=dc)
+        pd = kw.pop("planar_depth", self.planar_depth)
+        return type(self)(*super()._replace(**kw), antialiasing=aa, orthographic=orth, fisheye=fe, distortion=dc, planar_depth=pd)
 
     def __repr__(self):
         return super().__repr__()[:-1] + (f", antialiasing={self.antialiasing}, orthographic={self.orthographic}, "
-                                          f"fisheye={self.fisheye}, distortion={self.distortion})")
+                                          f"fisheye={self.fisheye}, distortion={self.distortion}, "
+                                          f"planar_depth={self.planar_depth})")
 
 
 FISHEYE_KEYS = ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")
@@ -691,6 +701,20 @@ def _state_sizes(L, P, W, H, normal=False):
     return s
 
 
+def _planar_flag(views, planar_depth=None, normal=False):
+    """The call's planar-depth flag: `planar_depth` when given, else the views' `planar_depth` attribute (every view of one
+    call must agree).  Raises ValueError beside a normal plane (both take the same columns of the blend's channel tile)."""
+    if planar_depth is None:
+        flags = {bool(getattr(s, "planar_depth", False)) for s in views}
+        if len(flags) > 1:
+            raise ValueError("planar_depth is a per-call setting: every view of one call must have the same value")
+        planar_depth = flags.pop() if flags else False
+    planar_depth = bool(planar_depth)
+    if planar_depth and normal:
+        raise ValueError("planar_depth cannot be combined with a normal plane (return_normal) in the same call")
+    return planar_depth
+
+
 def _ortho_flags(views, ortho=None):
     """Per-view camera models: `ortho` (V truthy values) when given, else each view's `orthographic` attribute; a ctypes int
     array for the _ortho calls, or None when every view is perspective (the calls without the argument then serve)."""
@@ -809,7 +833,7 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False, return_normal=False, ortho=None, fisheye=None, distortion=None):
+                        return_median=False, return_normal=False, ortho=None, fisheye=None, distortion=None, planar_depth=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -838,7 +862,9 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     `fisheye` attribute) marks the fisheye views, by default each view's `fisheye` attribute; with any fisheye view the call
     is mgs_forward_views_fisheye.  `distortion` (V entries, each None or a view's distortion parameters, as the settings'
     `distortion` attribute) marks the distorted-pinhole views, by default each view's `distortion` attribute; with any
-    distorted view the call is mgs_forward_views_distorted."""
+    distorted view the call is mgs_forward_views_distorted.  `planar_depth` (default: the views' `planar_depth` attribute):
+    each Gaussian's depth follows its tilt across its footprint, in the depth plane, the depth head and the median depth
+    (C ABI mgs_forward_views_planar); it cannot be combined with `return_normal`."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -851,6 +877,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
+    pln = _planar_flag(views, planar_depth, return_normal)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
     dcarr = _distortion_array(views, distortion)
@@ -884,7 +911,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
                                  aarr[v] if return_alpha else None, marr[v] if return_median else None,
-                                 narr[v] if return_normal else None)
+                                 narr[v] if return_normal else None, quads=pln)
             arr[v].status = status.data_ptr() + 8 * v
             arr[v].stream = streams[v].cuda_stream
             keep.append(k)
@@ -893,7 +920,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if dcarr is not None:
+        if pln:
+            _b.check(L.mgs_forward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                dcarr, 1, *rest), "mgs_forward_views_planar")
+        elif dcarr is not None:
             _b.check(L.mgs_forward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                    _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                    dcarr, *rest), "mgs_forward_views_distorted")
@@ -1037,13 +1068,15 @@ def _fill_ssim(ws, ssim, v, w=None, scale=None):
         ws.cot_scale = scale.data_ptr() + 8 * v
 
 
-def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None, wn=None):
+def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None, wn=None,
+                  quads=False):
     """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream) and, when
     `wa` (its mgs_view_alpha) is given, its alpha plane, when `wm` (its mgs_view_median) is given, its median planes, and when
-    `wn` (its mgs_view_normal) is given, its normal plane.
+    `wn` (its mgs_view_normal) is given, its normal plane.  `quads`: the geometry state also holds per-Gaussian quads (the
+    planar-depth call), as with `wn`.
     Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
-    gbytes, ibytes, _ = _state_sizes(L, P, W, H, wn is not None)
+    gbytes, ibytes, _ = _state_sizes(L, P, W, H, wn is not None or quads)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
     img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
     binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
@@ -1146,7 +1179,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
                                  ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
-                                 grads_normal=None, normals=None, ortho=None, fisheye=None, distortion=None):
+                                 grads_normal=None, normals=None, ortho=None, fisheye=None, distortion=None, planar_depth=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -1173,7 +1206,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
     forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho.
     `fisheye`: as given to the forward (by default the views' `fisheye` attributes); with a fisheye view the call is
-    mgs_backward_views_fisheye.  `distortion`: likewise, mgs_backward_views_distorted with a distorted view."""
+    mgs_backward_views_fisheye.  `distortion`: likewise, mgs_backward_views_distorted with a distorted view.  `planar_depth`:
+    as given to the forward (mgs_backward_views_planar)."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1182,6 +1216,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
+    pln = _planar_flag(views, planar_depth, grads_normal is not None)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
     dcarr = _distortion_array(views, distortion)
@@ -1229,7 +1264,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 keep.append(ga)
             keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
                                        grads_feature[v] if (F and grads_feature is not None) else None,
-                                       grads_depth[v] if grads_depth is not None else None, narr is not None))
+                                       grads_depth[v] if grads_depth is not None else None, narr is not None or pln))
             w.dL_dmean2D = _ptr(m2d) if shared else _ptr(m2d[v])
             w.stream = streams[v].cuda_stream
             if cot_scale is not None:
@@ -1246,7 +1281,10 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if dcarr is not None:
+            if pln:
+                _b.check(L.mgs_backward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
+                                                     oarr, farr, dcarr, 1, *rest), "mgs_backward_views_planar")
+            elif dcarr is not None:
                 _b.check(L.mgs_backward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
                                                         oarr, farr, dcarr, *rest), "mgs_backward_views_distorted")
             elif farr is not None:
@@ -1396,7 +1434,7 @@ def _prep_clouds(clouds, dev, include_feature):
 
 
 def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False,
-                         antialiasing=False, return_median=False, return_normal=False):
+                         antialiasing=False, return_median=False, return_normal=False, planar_depth=None):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
@@ -1416,6 +1454,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     views (C ABI mgs_forward_clouds_fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
     mgs_forward_clouds_distorted)."""
     L = _b.lib()
+    pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, return_normal)
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
         raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
@@ -1467,7 +1506,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                     _fill_ssim(sarr[g], c["ssim"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
                                       c.get("loss_heads"), aarr[g] if return_alpha else None, marr[g] if return_median else None,
-                                      narr[g] if return_normal else None)
+                                      narr[g] if return_normal else None, quads=pln)
                 arr[g].status = status.data_ptr() + 8 * g
                 arr[g].stream = streams[g].cuda_stream
                 keep.append(kp)
@@ -1477,7 +1516,11 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
         oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
-        if dcarr is not None:
+        if pln:
+            _b.check(L.mgs_forward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                                 dcarr, 1, *rest), "mgs_forward_clouds_planar")
+        elif dcarr is not None:
             _b.check(L.mgs_forward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                     _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                     dcarr, *rest), "mgs_forward_clouds_distorted")
@@ -1547,7 +1590,7 @@ def _clouds_fov(clouds, dev):
 
 
 def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False,
-                                  antialiasing=False, camera_grads=False):
+                                  antialiasing=False, camera_grads=False, planar_depth=None):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
     plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
@@ -1569,6 +1612,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     mgs_backward_clouds_ortho, clouds with a fisheye view mgs_backward_clouds_fisheye, and clouds with a distorted view
     mgs_backward_clouds_distorted."""
     L = _b.lib()
+    pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, any(c.get("grad_normal") is not None for c in clouds))
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
     F, M, B = pc[0]["F"], pc[0]["M"], len(clouds)
@@ -1627,7 +1671,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 keep.append(_backward_view(L, w, s, outs[b][v], dev, P, c["grad_color"][v],
                                            c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
                                            c["grad_depth"][v] if c.get("grad_depth") is not None else None,
-                                           c.get("grad_normal") is not None))
+                                           c.get("grad_normal") is not None or pln))
                 w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
                 w.stream = streams[g].cuda_stream
                 if c.get("grad_alpha") is not None:
@@ -1649,7 +1693,11 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
-        if dcarr is not None:
+        if pln:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
+                                                  marr, narr, oarr, farr, dcarr, 1, *rest), "mgs_backward_clouds_planar")
+        elif dcarr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
                                                      marr, narr, oarr, farr, dcarr, *rest), "mgs_backward_clouds_distorted")
