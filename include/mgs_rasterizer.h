@@ -1192,6 +1192,68 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F,
 	float scale_modifier, int accumulate, int debug, void* join_stream);
 
+/*
+ * Field queries (no reference counterpart): the cloud's density and features at Q arbitrary 3D points, with no camera.
+ * Definition, for Gaussian i (mean mu, scales s, quaternion q, opacity o, feature row f) and a point x, with q^ = q / |q| and
+ * R(q^) the rasterizer's rotation (Sigma = R^T S^2 R for a unit quaternion):
+ *   m_i(x) = | S^-1 R(q^) (x - mu) |^2   (evaluated in the Gaussian's own frame, never through an inverted Sigma),
+ *   g_i(x) = o exp(-m_i(x) / 2) if that is >= 1/255, else 0   (the blend's alpha threshold, without its 0.99 clamp),
+ *   density(x) = sum_i g_i(x),     features(x)[c] = sum_i g_i(x) f[c],   C = 0 .. MGS_MAX_FEATURE_CHANNELS.
+ * The support of Gaussian i is the ellipsoid m <= 2 ln(255 o); a Gaussian with o <= 1/255, a scale <= 0 or a non-finite mean,
+ * scale, quaternion or opacity contributes nothing and gets zero gradients.  A non-finite point gets density 0.  Features
+ * are used as given (they must be finite: they enter tensor-core sums with zero weights).
+ *   - points [Q,3], means3D [P,3], scales [P,3], rotations [P,4], opacities [P], features [P,C] (NULL with C = 0).
+ *   - out_density [Q]; out_features [Q,C], or [C,Q] with channel_first = 1 (a channel-first voxel grid without a copy);
+ *     both fully written.
+ * Method: a uniform grid of bins over the points' bounding box (its size is internal and picked from Q and the box; it
+ * changes nothing but the order of fp32 sums), per-bin lists of the Gaussians whose support box reaches the bin in
+ * ascending id, and one warp per 32 points of a bin with the feature contraction on the tensor cores (3xTF32).  The state
+ * is requested through the two allocators: the query state (sized by Q and P) first, then, after the one stream
+ * synchronisation of the call (the pair count is read back to size the bin lists exactly, so no pair is dropped), the
+ * pair state.  Returns the (bin, Gaussian) pair count (MGS_ERR_UNSUPPORTED above 2^31 - 1).  Not capturable in a CUDA graph.
+ * Backward: mgs_field_query_backward takes both state buffers as the forward left them (it allocates and reads back
+ * nothing), the same points, scales, rotations, features and channel_first, and the cotangents dL_ddensity [Q] and
+ * dL_dout_features (laid out as out_features), each NULL for zero.  It writes, each output optional (NULL skips it and the
+ * work only it needs): dL_dpoints [Q,3], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drotations [P,4] (through the
+ * normalisation of q), dL_dopacities [P] and dL_dfeature [P,C].  The cutoff is held fixed, as the blend holds its thresholds.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for C outside
+ * [0, MGS_MAX_FEATURE_CHANNELS]; MGS_ERR_INVALID_ARG for Q <= 0, P <= 0, a NULL allocator, input or required output, and
+ * channel_first other than 0 or 1.
+ */
+int mgs_field_query(
+	mgs_alloc_fn state_alloc, void* state_user,
+	mgs_alloc_fn pair_alloc, void* pair_user,
+	int Q, int P, int C,
+	const float* points,
+	const float* means3D,
+	const float* scales,
+	const float* rotations,
+	const float* opacities,
+	const float* features,
+	int channel_first,
+	float* out_density,
+	float* out_features,
+	int debug,
+	void* stream);
+int mgs_field_query_backward(
+	const char* state, const char* pair_state,
+	int Q, int P, int C,
+	const float* points,
+	const float* scales,
+	const float* rotations,
+	const float* features,
+	int channel_first,
+	const float* dL_ddensity,
+	const float* dL_dout_features,
+	float* dL_dpoints,
+	float* dL_dmeans3D,
+	float* dL_dscales,
+	float* dL_drotations,
+	float* dL_dopacities,
+	float* dL_dfeature,
+	int debug,
+	void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -220,6 +220,15 @@ def lib():
     L.mgs_lift_views_distorted.restype = C.c_int
     L.mgs_lift_views_distorted.argtypes = L.mgs_lift_views_fisheye.argtypes[:7] + [C.POINTER(ViewDistortion)] + \
         L.mgs_lift_views_fisheye.argtypes[7:]
+    L.mgs_field_query.restype = C.c_int
+    L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
+                                  vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
+                                  vp, vp, i, vp]                        # out_density out_features debug stream
+    L.mgs_field_query_backward.restype = C.c_int
+    L.mgs_field_query_backward.argtypes = [vp, vp, i, i, i,             # state pair_state Q P C
+                                           vp, vp, vp, vp, i, vp, vp,   # points scales rotations features channel_first dL_ddensity dL_dout_features
+                                           vp, vp, vp, vp, vp, vp,      # dL: points means3D scales rotations opacities feature
+                                           i, vp]                       # debug stream
     L.mgs_loss_heads.restype = C.c_int
     L.mgs_loss_heads.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mgs_ssim.restype = C.c_int
@@ -273,6 +282,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
     "mgs_backward_clouds_distorted", "mgs_lift_views_distorted",
     "mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar",
+    "mgs_field_query", "mgs_field_query_backward",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

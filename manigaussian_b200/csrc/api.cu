@@ -2054,3 +2054,55 @@ int mgs_state_array(const char* which_state, const char* name, char* state, int 
 }
 
 }  // extern "C"
+
+int mgs_field_query(
+	mgs_alloc_fn state_alloc, void* state_user, mgs_alloc_fn pair_alloc, void* pair_user,
+	int Q, int P, int C,
+	const float* points, const float* means3D, const float* scales, const float* rotations, const float* opacities,
+	const float* features, int channel_first, float* out_density, float* out_features, int debug, void* stream)
+{
+	using namespace mgs;
+	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
+	if (Q <= 0 || P <= 0) return fail(MGS_ERR_INVALID_ARG, "Q and P must be > 0");
+	if (!state_alloc || !pair_alloc) return fail(MGS_ERR_INVALID_ARG, "allocator callbacks are required");
+	if (!points || !means3D || !scales || !rotations || !opacities || !out_density)
+		return fail(MGS_ERR_INVALID_ARG, "points, means3D, scales, rotations, opacities and out_density are required");
+	if (C > 0 && (!features || !out_features)) return fail(MGS_ERR_INVALID_ARG, "features and out_features are required with C > 0");
+	if (channel_first != 0 && channel_first != 1) return fail(MGS_ERR_INVALID_ARG, "channel_first must be 0 or 1");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	char* state = state_alloc(state_user, field_state_bytes(Q, P));
+	if (!state) return fail(MGS_ERR_ALLOC, "query state allocation failed");
+	unsigned long long npairs = 0;
+	MGS_CUDA(field_front(state, Q, P, points, means3D, scales, rotations, opacities, &npairs, st));
+	MGS_STAGE("field_front");
+	MGS_CUDA(cudaStreamSynchronize(st));  // the one host read of the query: the pair count sizes the bin lists
+	if (npairs > 0x7fffffffull) return fail(MGS_ERR_UNSUPPORTED, "more than 2^31-1 (bin, Gaussian) pairs");
+	char* pairs = pair_alloc(pair_user, field_pair_state_bytes((long long)npairs, Q));
+	if (!pairs) return fail(MGS_ERR_ALLOC, "pair state allocation failed");
+	MGS_CUDA(field_pairs(state, pairs, Q, P, (long long)npairs, st));
+	MGS_STAGE("field_pairs");
+	MGS_CUDA(field_forward(state, pairs, Q, P, C, points, features, channel_first, out_density, out_features, st));
+	MGS_STAGE("field_forward");
+	return (int)npairs;
+}
+
+int mgs_field_query_backward(
+	const char* state, const char* pair_state, int Q, int P, int C,
+	const float* points, const float* scales, const float* rotations, const float* features, int channel_first,
+	const float* dL_ddensity, const float* dL_dout_features,
+	float* dL_dpoints, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations, float* dL_dopacities, float* dL_dfeature,
+	int debug, void* stream)
+{
+	using namespace mgs;
+	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
+	if (Q <= 0 || P <= 0) return fail(MGS_ERR_INVALID_ARG, "Q and P must be > 0");
+	if (!state || !pair_state || !points || !scales || !rotations)
+		return fail(MGS_ERR_INVALID_ARG, "state, pair_state, points, scales and rotations are required");
+	if (C > 0 && dL_dout_features && !features) return fail(MGS_ERR_INVALID_ARG, "features are required with dL_dout_features");
+	if (channel_first != 0 && channel_first != 1) return fail(MGS_ERR_INVALID_ARG, "channel_first must be 0 or 1");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(field_backward(const_cast<char*>(state), const_cast<char*>(pair_state), Q, P, C, points, features, scales, rotations,
+		channel_first, dL_ddensity, dL_dout_features, dL_dpoints, dL_dmeans3D, dL_dscales, dL_drotations, dL_dopacities, dL_dfeature, st));
+	MGS_STAGE("field_backward");
+	return 0;
+}

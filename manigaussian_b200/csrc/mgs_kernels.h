@@ -417,4 +417,49 @@ struct PlanarFwdArgs {
 };
 void launch_planar_fwd(const PlanarFwdArgs& a, cudaStream_t s);
 
+// field.cu: density and features of the Gaussian field at 3D points (include/mgs_rasterizer.h, mgs_field_query).  The query
+// state (field_state_bytes) holds the grid, the records, the grouped queries and the warp items; the pair state
+// (field_pair_state_bytes of the pair count field_front returns) the bin lists.  The backward reads both as the forward left
+// them.
+struct FieldGrid {
+	float lo[3];   // corner of the queries' bounding box
+	float inv[3];  // bins per unit length along each axis (0 on an axis of zero extent)
+	int n[3];      // bins along each axis
+};
+struct FieldArgs {
+	int Q, P, C, groups, channel_first;
+	const float* points;          // [Q,3]
+	const float* features;        // [P,C] or null
+	const float* scales;          // [P,3] (backward)
+	const float* rotations;       // [P,4] (backward)
+	const float4* recs;           // [P][4] records {A_k, mu_k}_k, {o, 0, 0, 0}
+	const float4* ext;            // [P] support half-extent, w = 1 for a Gaussian with support
+	const uint32_t* pairs;        // Gaussian ids sorted by bin, ascending within a bin
+	const uint2* gbin;            // [bins] range of each bin's Gaussians in pairs
+	const uint32_t* qorder;       // query ids sorted by bin
+	const uint4* items;           // warp items {first, end (in qorder), bin, 0}
+	const int* nitems;            // item count
+	float* density;               // [Q]
+	float* out_features;          // [Q,C] or [C,Q] (channel_first)
+	const float* dL_ddensity;     // [Q] or null
+	const float* dL_dfeatures;    // as out_features, or null
+	float* dL_dpoints;            // [Q,3] or null
+	float4* ggeo;                 // [P][4] per-Gaussian record gradients (zeroed), or null
+	float* dL_dfeat;              // [P,C] (zeroed) or null
+	float* dL_dmeans; float* dL_dscales; float* dL_drot; float* dL_dopac;  // each [P,k] or null
+};
+int field_bins(int Q);
+size_t field_state_bytes(int Q, int P);
+size_t field_pair_state_bytes(long long npairs, int Q);
+// enqueues the grid, the records, the query grouping and the scan of the per-Gaussian bin counts, and copies the pair count
+// to *host_pairs (the caller synchronises before reading it)
+cudaError_t field_front(char* state, int Q, int P, const float* points, const float* means, const float* scales, const float* rot,
+	const float* opac, unsigned long long* host_pairs, cudaStream_t st);
+cudaError_t field_pairs(char* state, char* pair_state, int Q, int P, long long npairs, cudaStream_t st);
+cudaError_t field_forward(char* state, char* pair_state, int Q, int P, int C, const float* points, const float* features,
+	int channel_first, float* density, float* out_features, cudaStream_t st);
+cudaError_t field_backward(char* state, char* pair_state, int Q, int P, int C, const float* points, const float* features,
+	const float* scales, const float* rotations, int channel_first, const float* dL_ddensity, const float* dL_dfeatures,
+	float* dL_dpoints, float* dL_dmeans, float* dL_dscales, float* dL_drot, float* dL_dopac, float* dL_dfeat, cudaStream_t st);
+
 }  // namespace mgs

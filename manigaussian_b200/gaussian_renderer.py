@@ -24,7 +24,8 @@ import torch
 from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, lift_views_raw,
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
+                         field_query_raw, lift_views_raw,
                          rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
@@ -621,6 +622,111 @@ def lift_views(cameras, pts_xyz, rotations, scales, opacity, maps, view_ids=None
     lifted, weight = lift_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0, None, maps,
                                     antialiasing=aa)
     return {"lifted": lifted, "weight": weight}
+
+
+class _QueryField(torch.autograd.Function):
+    """density and features of the field at points: one node, differentiable in the points and every Gaussian tensor"""
+
+    @staticmethod
+    def forward(ctx, channel_first, points, pts_xyz, rotations, scales, opacity, features):
+        density, out, state, pairs, _ = field_query_raw(points.detach(), pts_xyz.detach(), scales.detach(), rotations.detach(),
+                                                        opacity.detach(), None if features is None else features.detach(),
+                                                        channel_first=channel_first)
+        ctx.channel_first = channel_first
+        ctx.opacity_shape = opacity.shape
+        ctx.has_features = features is not None
+        ctx.save_for_backward(points, rotations, scales, features, state, pairs)
+        if out is None:
+            out = torch.empty(0, dtype=torch.float32, device=points.device)
+            ctx.mark_non_differentiable(out)
+        return density, out
+
+    @staticmethod
+    def backward(ctx, grad_density, grad_features):
+        points, rotations, scales, features, state, pairs = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        needs = (need[1], need[2], need[4], need[3], need[5], ctx.has_features and need[6])
+        if not any(needs):
+            return (None,) * 7
+        g = field_query_backward_raw(state, pairs, points.detach(), scales.detach(), rotations.detach(),
+                                     features.detach() if ctx.has_features else None, grad_density,
+                                     grad_features if ctx.has_features else None, channel_first=ctx.channel_first, needs=needs)
+        dop = g[4].view(ctx.opacity_shape) if g[4] is not None else None
+        return None, g[0], g[1], g[3], g[2], dop, g[5]
+
+
+def _field_inputs(where, pts_xyz, rotations, scales, opacity, features, points=None):
+    """ValueError on a shape, dtype or device mismatch of query_field / voxelize's tensors"""
+    P = pts_xyz.shape[0] if (torch.is_tensor(pts_xyz) and pts_xyz.dim() == 2) else -1
+    inputs = [("pts_xyz", pts_xyz, (3,)), ("rotations", rotations, (4,)), ("scales", scales, (3,)), ("opacity", opacity, None)]
+    for name, t, tail in inputs:
+        if not torch.is_tensor(t):
+            raise ValueError(f"{where}: {name}: expected a tensor")
+        shape_ok = tuple(t.shape) in ((P, 1), (P,)) if tail is None else tuple(t.shape) == (P,) + tail
+        if P <= 0 or not shape_ok:
+            raise ValueError(f"{where}: {name}: expected [{P},{'1' if tail is None else tail[0]}], got {tuple(t.shape)}")
+    if features is not None:
+        if not torch.is_tensor(features) or features.dim() != 2 or features.shape[0] != P:
+            raise ValueError(f"{where}: features: expected [{P},C], got {tuple(features.shape) if torch.is_tensor(features) else type(features)}")
+        if features.shape[1] > 512:
+            raise ValueError(f"{where}: features: at most 512 channels, got {features.shape[1]}")
+        inputs.append(("features", features, None))
+    if points is not None:
+        if not torch.is_tensor(points) or points.dim() != 2 or points.shape[1] != 3 or points.shape[0] == 0:
+            raise ValueError(f"{where}: points: expected [Q,3] with Q > 0, got {tuple(points.shape) if torch.is_tensor(points) else type(points)}")
+        inputs.insert(0, ("points", points, None))
+    device = pts_xyz.device
+    for name, t, _ in inputs:
+        if t.dtype != torch.float32:
+            raise ValueError(f"{where}: {name}: expected float32, got {t.dtype}")
+    for name, t, _ in inputs:
+        if t.device != device or not t.is_cuda:
+            raise ValueError(f"{where}: {name}: expected a CUDA tensor on {device}, got {t.device}")
+
+
+def query_field(points, pts_xyz, rotations, scales, opacity, features=None):
+    """The Gaussian field at 3D points (INTEGRATION.md §14): for every point x,
+        density(x) = sum_i g_i(x),   features(x)[c] = sum_i g_i(x) features[i][c],
+        g_i(x) = o_i exp(-|S_i^-1 R(q_i / |q_i|) (x - mu_i)|^2 / 2) where that is >= 1/255, else 0.
+    points [Q,3]; pts_xyz [P,3], rotations [P,4] (normalised here), scales [P,3] (activated), opacity [P] or [P,1]
+    (activated), features [P,C] (C <= 512, used as given) or None; float32 on one CUDA device.  One autograd node,
+    differentiable in every tensor argument (the 1/255 cutoff held fixed); one host synchronisation per call.  Returns
+    {"density": [Q], "features": [Q,C] or None}; raises ValueError on a shape, dtype or device mismatch."""
+    _field_inputs("query_field", pts_xyz, rotations, scales, opacity, features, points)
+    density, out = _QueryField.apply(False, points, pts_xyz, rotations, scales, opacity, features)
+    return {"density": density, "features": out if features is not None else None}
+
+
+def _grid(bounds, resolution):
+    b = [float(v) for v in bounds]
+    if len(b) != 6 or not all(b[k + 3] > b[k] for k in range(3)):
+        raise ValueError(f"voxelize: bounds must be (x0, y0, z0, x1, y1, z1) with x1 > x0, y1 > y0, z1 > z0, got {bounds}")
+    n = [int(resolution)] * 3 if isinstance(resolution, int) else [int(r) for r in resolution]
+    if len(n) != 3 or min(n) <= 0:
+        raise ValueError(f"voxelize: resolution must be a positive int or three of them, got {resolution}")
+    return b, n
+
+
+def voxel_centres(bounds, resolution, device):
+    """Centres lo + (i + 1/2) (hi - lo) / n of an [X,Y,Z] grid over bounds (x0, y0, z0, x1, y1, z1), as [X*Y*Z,3] points in
+    x-major order (point (i, j, k) at (i Y + j) Z + k)."""
+    b, n = _grid(bounds, resolution)
+    axes = [torch.tensor(b[k], dtype=torch.float64) + (torch.arange(n[k], dtype=torch.float64) + 0.5) * ((b[k + 3] - b[k]) / n[k])
+            for k in range(3)]
+    grid = torch.stack(torch.meshgrid(*axes, indexing="ij"), dim=-1).reshape(-1, 3)
+    return grid.to(device=device, dtype=torch.float32), n
+
+
+def voxelize(bounds, resolution, pts_xyz, rotations, scales, opacity, features=None):
+    """query_field at the centres of an [X,Y,Z] voxel grid over bounds (x0, y0, z0, x1, y1, z1), e.g. SCENE_BOUNDS, with
+    resolution n or (X, Y, Z): voxel (i, j, k) is sampled at lo + (i + 1/2, j + 1/2, k + 1/2) (hi - lo) / n.  The same node,
+    differentiable in the Gaussian tensors; the features come out channel first as PerAct's voxel input takes them, written
+    in that layout by the kernel.  Returns {"density": [X,Y,Z], "features": [C,X,Y,Z] or None}."""
+    _grid(bounds, resolution)
+    _field_inputs("voxelize", pts_xyz, rotations, scales, opacity, features)
+    points, n = voxel_centres(bounds, resolution, pts_xyz.device)
+    density, out = _QueryField.apply(True, points, pts_xyz, rotations, scales, opacity, features)
+    return {"density": density.view(*n), "features": out.view(-1, *n) if features is not None else None}
 
 
 _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations

@@ -1736,3 +1736,48 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
         else:
             _b.check(L.mgs_backward_clouds(B, carr, offs, arr, *rest), "mgs_backward_clouds")
     return grads
+
+
+def field_query_raw(points, means3D, scales, rotations, opacity, features=None, channel_first=False, debug=False):
+    """Density and features of the Gaussian field at points [Q,3] (C ABI mgs_field_query; definition in
+    include/mgs_rasterizer.h).  features [P,C] or None.  Returns (density [Q], features [Q,C] ([C,Q] with channel_first) or
+    None, query state, pair state, pair count); the two states serve field_query_backward_raw.  One host synchronisation."""
+    if not points.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = points.device
+    Q, P = points.size(0), means3D.size(0)
+    points, means3D, scales, rotations, opacity = (_prep(x, dev) for x in (points, means3D, scales, rotations, opacity))
+    C = features.size(1) if features is not None else 0
+    features = _prep(features, dev) if C else None
+    density = torch.empty((Q,), dtype=torch.float32, device=dev)
+    out = torch.empty((C, Q) if channel_first else (Q, C), dtype=torch.float32, device=dev) if C else None
+    sa, pa = _Alloc(dev), _Alloc(dev)
+    with torch.cuda.device(dev):
+        n = _checked((sa, pa), L.mgs_field_query(_ALLOC_CB, sa.key, _ALLOC_CB, pa.key, Q, P, C, _ptr(points), _ptr(means3D),
+                                                 _ptr(scales), _ptr(rotations), _ptr(opacity), _ptr(features), int(bool(channel_first)),
+                                                 _ptr(density), _ptr(out), int(bool(debug)), _stream(dev)), "mgs_field_query")
+    return density, out, sa.release(), pa.release(), n
+
+
+def field_query_backward_raw(state, pair_state, points, scales, rotations, features, grad_density, grad_features,
+                             channel_first=False, needs=(True,) * 6, debug=False):
+    """Gradients of a field_query_raw call (C ABI mgs_field_query_backward) from the cotangents grad_density [Q] and
+    grad_features (laid out as the forward's features), each None for zero.  `needs` selects, in this order, dL/dpoints,
+    dL/dmeans3D, dL/dscales, dL/drotations, dL/dopacity [P] and dL/dfeatures; each unselected one is None and not computed."""
+    L = _b.lib()
+    dev = points.device
+    Q, P = points.size(0), scales.size(0)
+    points, scales, rotations = (_prep(x, dev) for x in (points, scales, rotations))
+    C = features.size(1) if features is not None else 0
+    features = _prep(features, dev) if C else None
+    grad_density = _prep(grad_density, dev)
+    grad_features = _prep(grad_features, dev) if C else None
+    shapes = ((Q, 3), (P, 3), (P, 3), (P, 4), (P,), (P, C))
+    outs = [torch.empty(s, dtype=torch.float32, device=dev) if n and (k < 5 or C) else None
+            for k, (s, n) in enumerate(zip(shapes, needs))]
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_field_query_backward(_ptr(state), _ptr(pair_state), Q, P, C, _ptr(points), _ptr(scales), _ptr(rotations),
+                                            _ptr(features), int(bool(channel_first)), _ptr(grad_density), _ptr(grad_features),
+                                            *[_ptr(o) for o in outs], int(bool(debug)), _stream(dev)), "mgs_field_query_backward")
+    return tuple(outs)
