@@ -1193,6 +1193,77 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 	float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
+ * Optical flow.  The _flow calls are the _planar calls with the flow arguments after planar_depth; the _planar calls are the
+ * _flow calls with NULL for them.  The flow plane relates a cloud to its deformed next frame: for one view v of a cloud with
+ * means mu_i and paired next-frame means mu'_i (flow_means3D [P,3], the same P, paired by index):
+ *   - m_i is Gaussian i's screen mean in pixels, as the projection forms it: through projmatrix and ndc2pix for pinhole and
+ *     orthographic views, the lens map for fisheye and distorted views;
+ *   - m'_i is the same map applied to mu'_i, with the view's own camera, or with the view's next-frame pose when one is given
+ *     (next_viewmatrix / next_projmatrix, e.g. a wrist camera that moved with the gripper).  The model, intrinsics (a device
+ *     tan_fov included), principal point, coefficients and image size are always the view's own;
+ *   - valid_i holds when mu'_i passes the cull the projection applies to a mean of that model: view-space z > NEAR_Z, and for
+ *     fisheye views theta <= theta_max, for distorted views r2 <= r2_max and det Dd > 0;
+ *   - delta_i = valid_i ? m'_i - m_i : 0, in pixels (m' has no frustum clamp: it is a mean, not the Jacobian);
+ *   - flow[c][p] = sum_i w_{p,i} delta_i[c], c = 0 (x, to the right) and 1 (y, down), w = alpha T the weights the colour
+ *     image blends with.  There is no background term and no normalisation: flow / alpha is the expected flow.
+ * Both ends come from one device function, so delta_i is 0 bit for bit when mu'_i == mu_i and no next pose is given.  The
+ * per-Gaussian quads {dx, dy, 0, 0} live where the normal plane's do (columns 4..7 of the blend's {r,g,b,depth} tile): the
+ * geometry state must be sized by mgs_geometry_state_bytes_normal and the backward scratch by mgs_backward_scratch_bytes_normal.
+ * Backward, for a cotangent g [2,H,W] (channel 2 of dL_dpix_flow is ignored): the channels enter dL/dalpha like any other
+ * channel (opacity, conic and means2D of the current frame, with the anti-aliased compensation where it is on); with
+ * gd_i = sum_p w_{p,i} g[:, p], -gd_i joins view v's dL/dmean2D in the blend's convention (pixels times W / 2, H / 2), from
+ * where the per-Gaussian stage carries it to means3D, the camera gradients and dL_dtan_fov; (dm'/dmu')^T gd_i, summed over
+ * the views, is dL_dflow_means3D (written, or added with accumulate = 1; NULL skips it), and where the view has no next pose
+ * (dm'/dcamera)^T gd_i joins its dL_dviewmatrix, dL_dprojmatrix and dL_dtan_fov.  Invalid pairs receive nothing through delta.
+ * Flow needs no rotations (cov3D_precomp works), and adds no host synchronisation.
+ * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: flow beside a normal plane or planar_depth (they share the
+ * tile's columns 4..7), or beside the depth / mask heads of the same view; out_flow without next means (flow_means3D, or the
+ * cloud's mgs_cloud_flow.means3D); dL_dpix_flow without out_flow, the plane that view's forward wrote; only one of
+ * next_viewmatrix and next_projmatrix.
+ */
+typedef struct mgs_view_flow {
+	const float* next_viewmatrix;   /* [16] the next frame's pose, or NULL for the view's own */
+	const float* next_projmatrix;   /* [16], NULL exactly when next_viewmatrix is */
+	float* out_flow;                /* forward output [3,H,W] (channel 2 written as 0), or NULL; names the forward's plane in the backward */
+	const float* dL_dpix_flow;      /* backward input [3,H,W] (channel 2 ignored), or NULL */
+} mgs_view_flow;
+/* one per cloud of a clouds call: the cloud's next-frame means [P,3] (or NULL) and their gradient [P,3] (or NULL) */
+typedef struct mgs_cloud_flow {
+	const float* means3D;
+	float* dL_dmeans3D;
+} mgs_cloud_flow;
+int mgs_forward_views_flow(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	const mgs_view_flow* flow, const float* flow_means3D,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream);
+int mgs_backward_views_flow(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int planar_depth, const mgs_view_flow* flow, const float* flow_means3D, float* dL_dflow_means3D,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
+int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, const mgs_view_flow* flow,
+	const mgs_cloud_flow* flow_clouds, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	const mgs_view_flow* flow, const mgs_cloud_flow* flow_clouds, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream);
+
+/*
  * Field queries (no reference counterpart): the cloud's density and features at Q arbitrary 3D points, with no camera.
  * Definition, for Gaussian i (mean mu, scales s, quaternion q, opacity o, feature row f) and a point x, with q^ = q / |q| and
  * R(q^) the rasterizer's rotation (Sigma = R^T S^2 R for a unit quaternion):

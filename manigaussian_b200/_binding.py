@@ -65,6 +65,16 @@ class ViewNormal(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("out_normal", "dL_dpix_normal")]
 
 
+class ViewFlow(C.Structure):
+    """mirror of `mgs_view_flow` (include/mgs_rasterizer.h): the optional flow plane of one view and its next-frame pose"""
+    _fields_ = [(n, C.c_void_p) for n in ("next_viewmatrix", "next_projmatrix", "out_flow", "dL_dpix_flow")]
+
+
+class CloudFlow(C.Structure):
+    """mirror of `mgs_cloud_flow` (include/mgs_rasterizer.h): one cloud's next-frame means and their gradient"""
+    _fields_ = [(n, C.c_void_p) for n in ("means3D", "dL_dmeans3D")]
+
+
 class ViewFisheye(C.Structure):
     """mirror of `mgs_view_fisheye` (include/mgs_rasterizer.h): one view's Kannala-Brandt fisheye parameters"""
     _fields_ = [("fisheye", C.c_int)] + [(n, C.c_float) for n in ("cx", "cy", "k1", "k2", "k3", "k4", "theta_max")]
@@ -206,6 +216,13 @@ def lib():
         pln = name.replace("_views", "_views_planar").replace("_clouds", "_clouds_planar")
         getattr(L, pln).restype = C.c_int
         getattr(L, pln).argtypes = getattr(L, dist).argtypes[:len(getattr(L, dist).argtypes) - len(at) + k] + [i] + at[k:]
+        # ... and the flow planes after the planar_depth flag: views calls take the next-frame means (and the backward their
+        # gradient), clouds calls one CloudFlow per cloud
+        flw = name.replace("_views", "_views_flow").replace("_clouds", "_clouds_flow")
+        getattr(L, flw).restype = C.c_int
+        extra = [C.POINTER(CloudFlow)] if "clouds" in name else ([vp, vp] if "backward" in name else [vp])
+        getattr(L, flw).argtypes = getattr(L, pln).argtypes[:len(getattr(L, pln).argtypes) - len(at) + k] + \
+            [C.POINTER(ViewFlow)] + extra + at[k:]
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
                                  i, i, i, i,                        # P D M C
@@ -282,6 +299,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
     "mgs_backward_clouds_distorted", "mgs_lift_views_distorted",
     "mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar",
+    "mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow",
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",

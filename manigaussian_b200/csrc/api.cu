@@ -758,6 +758,118 @@ static int enqueue_normals_bwd(const Cloud& c, const mgs_view* views, const mgs_
 	return 0;
 }
 
+// the flow plane (include/mgs_rasterizer.h, mgs_forward_views_flow) of views [v0, v1) of one cloud: fl NULL or one entry per
+// view of the call, next_means the cloud's next-frame means; it takes the normal plane's tile columns and quad slot
+static bool flow_on(const mgs_view_flow* fl, int v) { return fl && (fl[v].out_flow || fl[v].dL_dpix_flow); }
+// the whole call: flow never beside planar depth or a normal plane (they share the tile's columns 4..7); V views
+static int check_flow_call(const mgs_view_flow* fl, int V, int planar_depth, const mgs_view_normal* normal)
+{
+	bool any = false;
+	for (int v = 0; v < V; v++) any |= flow_on(fl, v);
+	if (!any) return 0;
+	if (planar_depth) return fail(MGS_ERR_INVALID_ARG, "flow cannot be combined with planar_depth (both take columns 4..7 of the tile)");
+	for (int v = 0; v < V && normal; v++)
+		if (normal[v].out_normal || normal[v].dL_dpix_normal)
+			return fail(MGS_ERR_INVALID_ARG, "flow cannot be combined with a normal plane (both take columns 4..7 of the tile)");
+	return 0;
+}
+// views [v0, v1) of one cloud with next-frame means next_means (or NULL); dm: one entry per view of the call, or NULL
+static int check_flow(const mgs_view_flow* fl, const float* next_means, int v0, int v1, const mgs_view_depth_mask* dm)
+{
+	for (int v = v0; v < v1; v++) {
+		if (!flow_on(fl, v)) continue;
+		const mgs_view_flow& f = fl[v];
+		if (dm && (dm[v].target_depth || dm[v].target_mask))
+			return fail(MGS_ERR_INVALID_ARG, "view: the flow plane cannot be combined with the depth / mask heads");
+		if (!f.out_flow) return fail(MGS_ERR_INVALID_ARG, "view: dL_dpix_flow needs out_flow, the plane its forward wrote");
+		if (!next_means) return fail(MGS_ERR_INVALID_ARG, "view: out_flow needs the cloud's next-frame means");
+		if (!f.next_viewmatrix != !f.next_projmatrix)
+			return fail(MGS_ERR_INVALID_ARG, "view: next_viewmatrix and next_projmatrix are given together or not at all");
+	}
+	return 0;
+}
+// the blend's view of a flow plane: the normal plane's arguments (V entries), or `normal` itself when no view has flow
+static const mgs_view_normal* flow_blend_planes(const mgs_view_flow* fl, int V, const mgs_view_normal* normal,
+	std::vector<mgs_view_normal>& keep)
+{
+	bool any = false;
+	for (int v = 0; v < V; v++) any |= flow_on(fl, v);
+	if (!any) return normal;
+	keep.assign(V, mgs_view_normal{ nullptr, nullptr });
+	for (int v = 0; v < V; v++)
+		if (flow_on(fl, v)) keep[v] = mgs_view_normal{ fl[v].out_flow, fl[v].dL_dpix_flow };
+	return keep.data();
+}
+// one end of view w's flow: its model, intrinsics and image size, with the pose (vm, pm)
+static FlowCam flow_cam(const mgs_view& w, const float* tan_fov, int ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc,
+	const float* vm, const float* pm)
+{
+	FlowCam k{};
+	k.viewmatrix = vm; k.projmatrix = pm; k.tan_fov = tan_fov; k.tan_fovx = w.tan_fovx; k.tan_fovy = w.tan_fovy;
+	k.W = w.width; k.H = w.height;
+	k.model = dc ? 3 : fe ? 2 : ortho ? 1 : 0;
+	if (fe) { k.cx = fe->cx; k.cy = fe->cy; k.theta_max = fe->theta_max; k.fe_k = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 }; }
+	if (dc) {
+		k.cx = dc->cx; k.cy = dc->cy; k.r2_max = dc->r_max * dc->r_max;  // +inf stays +inf
+		k.dc_k = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
+	}
+	return k;
+}
+static const float* next_vm(const mgs_view_flow& f, const mgs_view& w) { return f.next_viewmatrix ? f.next_viewmatrix : w.viewmatrix; }
+static const float* next_pm(const mgs_view_flow& f, const mgs_view& w) { return f.next_viewmatrix ? f.next_projmatrix : w.projmatrix; }
+
+// the view's flow quads {dx, dy, 0, 0}, behind its projection on its stream (fl nullable), in the normal plane's quad slot
+static int enqueue_flow_fwd(const Cloud& c, const mgs_view& w, const mgs_view_flow* fl, const float* next_means, const float* tan_fov,
+	int ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, int debug)
+{
+	if (!fl || !fl->out_flow) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+	FlowFwdArgs a{};
+	a.P = c.P; a.means3D = c.means3D; a.next_means3D = next_means;
+	a.cur = flow_cam(w, tan_fov, ortho, fe, dc, w.viewmatrix, w.projmatrix);
+	a.next = flow_cam(w, tan_fov, ortho, fe, dc, next_vm(*fl, w), next_pm(*fl, w));
+	a.radii = w.radii; a.quad = carve_view(w, c.P).nrm;
+	launch_flow_fwd(a, st);
+	MGS_STAGE("flow_fwd");
+	return 0;
+}
+
+// the flow planes' backward for views [v0, v0 + n) of one cloud (n <= MAX_BWD_VIEWS), on `st` behind the blend backward and
+// ahead of the per-Gaussian launch that holds those views: the m path into each view's blend-stage records, the m' path into
+// dL_dnext (written, or added with `accumulate`), and the m' camera terms into the views' camera rows, which one reduce sums
+// into the camera outputs with `accumulate` (the per-Gaussian stage's reduce then adds to them).  Returns whether it enqueued
+// that reduce.
+static int enqueue_flow_bwd(const Cloud& c, const mgs_view* views, const mgs_view_flow* fl, const float* next_means, float* dL_dnext,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const int* ortho, const mgs_view_fisheye* fe,
+	const mgs_view_distortion* dc, int v0, int n, int accumulate_next, int accumulate_cam, int debug, cudaStream_t st, bool& reduced)
+{
+	reduced = false;
+	FlowBwdArgs a{};
+	a.P = c.P; a.V = n; a.next_means3D = next_means; a.dL_dnext_means3D = dL_dnext; a.accumulate = accumulate_next;
+	CamReduceArgs cr{};
+	cr.accumulate = accumulate_cam;
+	for (int u = 0; u < n; u++) {
+		const int v = v0 + u;
+		const mgs_view& w = views[v];
+		FlowBwdView& b = a.view[u];
+		const ViewState s = carve_view(w, c.P);
+		const float* tf = device_fov(intr, v);
+		b.radii = w.radii; b.gb = s.gb;
+		if (flow_on(fl, v) && fl[v].dL_dpix_flow) {
+			b.gn = reinterpret_cast<const float4*>(s.gn);
+			b.cam = flow_cam(w, tf, ortho_of(ortho, v), fisheye_of(fe, v), distortion_of(dc, v), next_vm(fl[v], w), next_pm(fl[v], w));
+			b.own_camera = fl[v].next_viewmatrix ? 0 : 1;
+		}
+		ProjectBwdIntr ki{};
+		camera_view(cam, intr, w, v, c.P, b.cam_rows, ki, cr);
+		b.intr_rows = ki.rows;
+	}
+	launch_flow_bwd(a, st);
+	if (cr.V > 0) { launch_camera_grad_reduce(cr, st); reduced = true; }
+	MGS_STAGE("flow_bwd");
+	return 0;
+}
+
 // launch view u of a backward: a fisheye view sets bit u of the mask and its coefficients
 static void set_fisheye(const mgs_view_fisheye* fe, int u, uint16_t& mask, FisheyeK* k)
 {
@@ -780,9 +892,14 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
 	const mgs_view_normal* nm, const int* ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
-	int accumulate, int stages, int debug, cudaStream_t join)
+	int accumulate, int stages, int debug, cudaStream_t join, const mgs_view_flow* fl = nullptr, const float* flow_means3D = nullptr,
+	float* dL_dflow = nullptr)
 {
 	const int P = c.P, F = c.F;
+	std::vector<mgs_view_normal> flow_planes;
+	const mgs_view_normal* blend_nm = flow_blend_planes(fl, V, nm, flow_planes);  // a flow plane rides in the normal plane's columns
+	bool flow_bwd = false;  // a view has a flow cotangent
+	for (int v = 0; v < V; v++) flow_bwd |= flow_on(fl, v) && fl[v].dL_dpix_flow;
 	if (stages & 1) {
 		if (F > 0 && !accumulate) MGS_CUDA(cudaMemsetAsync(dL_dfeature, 0, (size_t)P * F * sizeof(float), join));
 		int rc = fork_streams(V, views, join);
@@ -792,7 +909,7 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
 			if (rc == 0)
 				rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr,
-					med ? med + v : nullptr, nm ? nm + v : nullptr, debug);
+					med ? med + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 		rc = join_streams(V, views, join);
@@ -823,8 +940,14 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
 		pb.antialias = c.antialias;
 		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
+		bool flow_reduced = false;  // the flow's camera terms already hold the camera outputs
+		if (flow_bwd) {
+			const int rc = enqueue_flow_bwd(c, views, fl, flow_means3D, dL_dflow, cam, intr, ortho, fe, dc, v0, pb.V,
+				(accumulate || v0 > 0) ? 1 : 0, accumulate ? 1 : 0, debug, st, flow_reduced);
+			if (rc < 0) return rc;
+		}
 		CamReduceArgs cr{};
-		cr.accumulate = accumulate ? 1 : 0;
+		cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
 		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
 		for (int u = 0; u < pb.V; u++) pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << u);
 		for (int u = 0; u < pb.V; u++) set_fisheye(fisheye_of(fe, v0 + u), u, pb.fisheye, pb.fe_k);
@@ -912,6 +1035,7 @@ static int check_planar(int planar_depth, const mgs_view_normal* normal, int V)
 			return fail(MGS_ERR_INVALID_ARG, "planar_depth cannot be combined with a normal plane in the same call");
 	return 0;
 }
+
 
 }  // namespace mgs
 
@@ -1154,10 +1278,27 @@ int mgs_forward_views_planar(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_views_flow(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye, distortion,
+		planar_depth, nullptr, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier,
+		rotations, cov3D_precomp, prefiltered, debug, join_stream);
+}
+
+int mgs_forward_views_flow(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	const mgs_view_flow* flow, const float* flow_means3D,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0)
+		return MGS_ERR_INVALID_ARG;
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
@@ -1176,6 +1317,8 @@ int mgs_forward_views_planar(
 	}
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing, planar_depth };
+	std::vector<mgs_view_normal> flow_planes;
+	const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	int rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
@@ -1197,8 +1340,11 @@ int mgs_forward_views_planar(
 					distortion_of(distortion, v))
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
-					median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
+					median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 			if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
+			if (rc == 0 && phase == 0)
+				rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, flow_means3D, device_fov(intr, v), ortho_of(ortho, v),
+					fisheye_of(fisheye, v), distortion_of(distortion, v), debug);
 			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
@@ -1482,8 +1628,27 @@ int mgs_backward_views_planar(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
+	return mgs_backward_views_flow(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho, fisheye,
+		distortion, planar_depth, nullptr, nullptr, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
+		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale,
+		dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
+}
+
+int mgs_backward_views_flow(
+	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
+	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
+	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int planar_depth, const mgs_view_flow* flow, const float* flow_means3D, float* dL_dflow_means3D,
+	int P, int D, int M, int F,
+	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
+	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V > 0 && views && check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (V > 0 && views && (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0))
+		return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
 	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
@@ -1505,7 +1670,7 @@ int mgs_backward_views_planar(
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing, planar_depth };
 	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, fisheye, distortion, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
-		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream));
+		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream), flow, flow_means3D, dL_dflow_means3D);
 }
 
 int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
@@ -1603,6 +1768,19 @@ int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_of
 	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
 	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
+	return mgs_forward_clouds_flow(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho,
+		fisheye, distortion, planar_depth, nullptr, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
+}
+
+// the next-frame means of cloud b (flow_clouds: B entries or NULL)
+static const float* cloud_next(const mgs_cloud_flow* fc, int b) { return fc ? fc[b].means3D : nullptr; }
+
+int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, const mgs_view_flow* flow,
+	const mgs_cloud_flow* flow_clouds, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
+{
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -1611,6 +1789,9 @@ int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_of
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
+	for (int b = 0; b < B; b++)
+		if (check_flow(flow, cloud_next(flow_clouds, b), view_offsets[b], view_offsets[b + 1], depth_mask) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1630,6 +1811,8 @@ int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_of
 		}
 	}
 	const int V = view_offsets[B];
+	std::vector<mgs_view_normal> flow_planes;
+	const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
@@ -1642,8 +1825,11 @@ int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_of
 					distortion_of(distortion, v))
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
-						median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
+						median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 				if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
+				if (rc == 0 && phase == 0)
+					rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, cloud_next(flow_clouds, b), device_fov(intr, v),
+						ortho_of(ortho, v), fisheye_of(fisheye, v), distortion_of(distortion, v), debug);
 				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
@@ -1759,6 +1945,17 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int accumulate, int debug,
 	void* join_stream)
 {
+	return mgs_backward_clouds_flow(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
+		ortho, fisheye, distortion, planar_depth, nullptr, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
+}
+
+int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
+	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
+	const mgs_view_flow* flow, const mgs_cloud_flow* flow_clouds, int D, int M, int F,
+	float scale_modifier, int accumulate, int debug, void* join_stream)
+{
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
@@ -1766,6 +1963,9 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
+	for (int b = 0; b < B; b++)
+		if (check_flow(flow, cloud_next(flow_clouds, b), view_offsets[b], view_offsets[b + 1], depth_mask) < 0) return MGS_ERR_INVALID_ARG;
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
 	for (int b = 0; b < B; b++) {
 		const mgs_cloud& k = clouds[b];
@@ -1792,6 +1992,8 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 		if (F > 0 && k.feature && k.dL_dfeature && !accumulate)
 			MGS_CUDA(cudaMemsetAsync(k.dL_dfeature, 0, (size_t)k.P * F * sizeof(float), join));
 	}
+	std::vector<mgs_view_normal> flow_planes;
+	const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);
 	rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
 	for (int b = 0; b < B; b++) {
@@ -1801,7 +2003,7 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
 			if (rc == 0)
 				rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
-					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, normal ? normal + v : nullptr, debug);
+					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
 	}
@@ -1811,11 +2013,26 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
 	// per-Gaussian stage on `join`: launches of at most MAX_BWD_VIEWS views that pack whole clouds; a cloud with more views
 	// spans launches, and its later launches add to what the earlier ones wrote
 	const cudaStream_t st = join;
+	// the flow planes' backward first, one launch per cloud and MAX_BWD_VIEWS of its views: it adds to the blend-stage records
+	// the per-Gaussian stage reads, and its camera reduce writes the camera outputs the per-Gaussian stage's reduce adds to
+	bool flow_bwd = false, flow_reduced = false;
+	for (int v = 0; v < V; v++) flow_bwd |= flow_on(flow, v) && flow[v].dL_dpix_flow;
+	for (int b = 0; b < B && flow_bwd; b++) {
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			bool red = false;
+			rc = enqueue_flow_bwd(c, views, flow, cloud_next(flow_clouds, b), flow_clouds ? flow_clouds[b].dL_dmeans3D : nullptr, cam, intr,
+				ortho, fisheye, distortion, v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS),
+				(accumulate || v0 > view_offsets[b]) ? 1 : 0, accumulate ? 1 : 0, debug, st, red);
+			if (rc < 0) return rc;
+			flow_reduced |= red;
+		}
+	}
 	// a view's camera rows are summed by the reduce behind the one launch that holds the view
 	ProjectBwdCloudsDistArgs pb{};
 	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
 	CamReduceArgs cr{};
-	cr.accumulate = accumulate ? 1 : 0;
+	cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
 	int nv = 0;  // views in pb
 	auto flush = [&]() -> int {
 		if (pb.B == 0) return 0;

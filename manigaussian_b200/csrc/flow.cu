@@ -1,0 +1,205 @@
+// Per-Gaussian optical flow between a cloud and its paired next-frame means (include/mgs_rasterizer.h, flow plane): the
+// screen displacement delta_i = m'_i - m_i of Gaussian i in one view, m its screen mean and m' the same map applied to its
+// next-frame mean, in pixels, 0 where the next mean fails the projection's cull.  The forward writes the quad
+// {dx, dy, 0, 0} into the view's quad slot, where the normal plane keeps its quads, so the NRM instantiations of the blend
+// carry it in columns 4..7 of the {r,g,b,depth} tile unchanged.  The backward takes the blend's quad gradients gn and
+// chains them through both ends: -gn into the screen-mean slots of the blend-stage records, which the per-Gaussian chain
+// rule then carries to means3D, the camera and the field of view, and (dm'/dmu')^T gn into dL/d(next means), plus the
+// camera terms of m' where a view renders m' with its own camera.
+//
+// Kernels of their own rather than modes of the projection kernels: those compile to pinned instruction sequences (tile ids
+// and sort keys depend on them, DESIGN.md section 4).  Both ends come from one device function, so a next mean equal to the
+// current one under the view's own camera gives delta = 0 bit for bit.
+#include "mgs_common.cuh"
+#include "mgs_kernels.h"
+
+namespace mgs {
+
+namespace {
+
+// the view's screen mean of p in pixels (the projection's expressions for the view's model), and whether p passes the
+// projection's cull of a mean
+__device__ __forceinline__ bool flow_mean(const FlowCam& c, const V3& p, float& px, float& py)
+{
+	const V3 t = xform4x3(p, c.viewmatrix);
+	if (c.model == 0 || c.model == 1) {
+		const float4 h = xform4x4(p, c.projmatrix);
+		const float w = 1.0f / (h.w + 0.0000001f);
+		px = ndc2pix(h.x * w, c.W); py = ndc2pix(h.y * w, c.H);
+		return t.z > NEAR_Z;
+	}
+	px = py = 0.f;
+	if (t.z <= NEAR_Z) return false;
+	const float tanx = c.tan_fov ? c.tan_fov[0] : c.tan_fovx, tany = c.tan_fov ? c.tan_fov[1] : c.tan_fovy;
+	const float fx = c.W / (2.0f * tanx), fy = c.H / (2.0f * tany);
+	if (c.model == 2) {
+		const FisheyeRadial fr = fisheye_radial<false>(t.x, t.y, t.z, c.fe_k);
+		if (fr.theta > c.theta_max) return false;
+		px = fx * fr.a * t.x + c.cx; py = fy * fr.a * t.y + c.cy;
+		return true;
+	}
+	const float iz = 1.0f / t.z;
+	const DistTerms ds = distortion_terms<false>(t.x * iz, t.y * iz, c.dc_k);
+	if (ds.r2 > c.r2_max || fmaf(-ds.d01, ds.d01, ds.d00 * ds.d11) <= 0.f) return false;
+	px = fx * ds.xd + c.cx; py = fy * ds.yd + c.cy;
+	return true;
+}
+
+// the m' chain of one view: g the pixel cotangent of m' at p (valid), into dL/dp (added to gp) and, with cg, the camera terms
+// of the view (CAM_ALL_TERMS, laid out as the per-Gaussian backward's rows: dL/dvm, dL/dpm, dL/dcampos, dL/dtan_fov)
+template <bool CAM>
+__device__ __forceinline__ void flow_mean_bwd(const FlowCam& c, const float p[3], float gx, float gy, float gp[3], float* cg)
+{
+	const float* vm = c.viewmatrix;
+	if (c.model == 0 || c.model == 1) {
+		// ndc = (P p).xy / ((P p).w + 1e-7), pixel = ((ndc + 1) S - 1) / 2: the ndc cotangent is the pixel one times S / 2
+		const float* pm = c.projmatrix;
+		const float dx = gx * (0.5f * c.W), dy = gy * (0.5f * c.H);
+		const float hx = pm[0] * p[0] + pm[4] * p[1] + pm[8] * p[2] + pm[12];
+		const float hy = pm[1] * p[0] + pm[5] * p[1] + pm[9] * p[2] + pm[13];
+		const float hw = pm[3] * p[0] + pm[7] * p[1] + pm[11] * p[2] + pm[15];
+		const float iw = 1.0f / (hw + 0.0000001f);
+		const float kx = hx * iw * iw, ky = hy * iw * iw;
+#pragma unroll
+		for (int k = 0; k < 3; k++) gp[k] += (pm[4 * k] * iw - pm[4 * k + 3] * kx) * dx + (pm[4 * k + 1] * iw - pm[4 * k + 3] * ky) * dy;
+		if constexpr (CAM) {
+			const float ax = dx * iw, ay = dy * iw, aw = -(dx * kx + dy * ky);
+			const float ph[4] = { p[0], p[1], p[2], 1.f };
+#pragma unroll
+			for (int k = 0; k < 4; k++) { cg[12 + 3 * k] = ax * ph[k]; cg[13 + 3 * k] = ay * ph[k]; cg[14 + 3 * k] = aw * ph[k]; }
+		}
+		return;
+	}
+	const float tx = vm[0] * p[0] + vm[4] * p[1] + vm[8] * p[2] + vm[12];
+	const float ty = vm[1] * p[0] + vm[5] * p[1] + vm[9] * p[2] + vm[13];
+	const float tz = vm[2] * p[0] + vm[6] * p[1] + vm[10] * p[2] + vm[14];
+	const float tanx = c.tan_fov ? c.tan_fov[0] : c.tan_fovx, tany = c.tan_fov ? c.tan_fov[1] : c.tan_fovy;
+	const float fx = c.W / (2.0f * tanx), fy = c.H / (2.0f * tany);
+	float dt[3], ftx, fty;  // dL/dt; (u - cx, v - cy) for the field of view
+	if (c.model == 2) {
+		// J = [[fx (a + c x^2), fx c x y, -fx x g], [fy c x y, fy (a + c y^2), -fy y g]] (fisheye.cuh)
+		const FisheyeRadial fr = fisheye_radial<false>(tx, ty, tz, c.fe_k);
+		const float ex = fx * gx, ey = fy * gy, cxy = fr.c * tx * ty;
+		dt[0] = ex * (fr.a + fr.c * tx * tx) + ey * cxy;
+		dt[1] = ex * cxy + ey * (fr.a + fr.c * ty * ty);
+		dt[2] = -(ex * tx + ey * ty) * fr.g;
+		ftx = fx * fr.a * tx; fty = fy * fr.a * ty;
+	} else {
+		// (u, v) = F (xd, yd) + c, d(xd, yd) / d(x, y) = Dd (symmetric), (x, y) = t.xy / t.z
+		const float iz = 1.0f / tz, x = tx * iz, y = ty * iz;
+		const DistTerms ds = distortion_terms<false>(x, y, c.dc_k);
+		const float ex = fx * gx, ey = fy * gy;
+		const float qx = ds.d00 * ex + ds.d01 * ey, qy = ds.d01 * ex + ds.d11 * ey;
+		dt[0] = qx * iz; dt[1] = qy * iz; dt[2] = -(qx * x + qy * y) * iz;
+		ftx = fx * ds.xd; fty = fy * ds.yd;
+	}
+#pragma unroll
+	for (int k = 0; k < 3; k++) gp[k] += vm[4 * k] * dt[0] + vm[4 * k + 1] * dt[1] + vm[4 * k + 2] * dt[2];
+	if constexpr (CAM) {
+		// t = Rv p + tv: dL/dRv[r][k] = dt[r] p[k] at 3k + r, dL/dtv = dt at 9 + r; fx = W / (2 tan_fovx) scales u - cx
+#pragma unroll
+		for (int k = 0; k < 3; k++) { cg[3 * k] = dt[0] * p[k]; cg[3 * k + 1] = dt[1] * p[k]; cg[3 * k + 2] = dt[2] * p[k]; }
+		cg[9] = dt[0]; cg[10] = dt[1]; cg[11] = dt[2];
+		cg[27] = -gx * ftx / tanx; cg[28] = -gy * fty / tany;
+	}
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(256) flow_fwd_kernel(FlowFwdArgs a)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= a.P) return;
+	float dx = 0.f, dy = 0.f;
+	if (a.radii[i] > 0) {
+		const V3 p = { a.means3D[3 * (size_t)i], a.means3D[3 * (size_t)i + 1], a.means3D[3 * (size_t)i + 2] };
+		const V3 q = { a.next_means3D[3 * (size_t)i], a.next_means3D[3 * (size_t)i + 1], a.next_means3D[3 * (size_t)i + 2] };
+		float mx, my, nx, ny;
+		flow_mean(a.cur, p, mx, my);  // passes: the projection kept the Gaussian
+		if (flow_mean(a.next, q, nx, ny)) { dx = nx - mx; dy = ny - my; }
+	}
+	a.quad[i] = make_float4(dx, dy, 0.f, 0.f);
+}
+
+// CAM: the launch writes camera rows.  One thread per Gaussian over the launch's views in order; per view the camera terms are
+// summed over the warp by shuffles in a fixed order, then over the CTA's 4 warps in warp order: deterministic rows.
+template <bool CAM>
+__global__ void __launch_bounds__(FLOW_BWD_THREADS) flow_bwd_kernel(FlowBwdArgs a)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	const bool in = i < a.P;
+	const int id = in ? i : 0;
+	__shared__ float cam_sm[CAM ? FLOW_BWD_THREADS / 32 * CAM_ALL_TERMS : 1];
+	// a cloud without next means (no view of it has flow) still writes its views' camera rows, as zeros
+	const float* nm = a.next_means3D;
+	const float p[3] = { nm ? nm[3 * (size_t)id] : 0.f, nm ? nm[3 * (size_t)id + 1] : 0.f, nm ? nm[3 * (size_t)id + 2] : 0.f };
+	float gp[3] = { 0.f, 0.f, 0.f };
+	for (int v = 0; v < a.V; v++) {
+		const FlowBwdView& w = a.view[v];
+		float cg[CAM ? CAM_ALL_TERMS : 1];
+		if constexpr (CAM) {
+#pragma unroll
+			for (int k = 0; k < CAM_ALL_TERMS; k++) cg[k] = 0.f;
+		}
+		if (in && w.gn && w.radii[id] > 0) {
+			// an invalid pair's delta is 0 whatever m and m' are: it receives nothing through either end
+			const V3 q = { p[0], p[1], p[2] };
+			float nx, ny;
+			if (flow_mean(w.cam, q, nx, ny)) {
+				const float4 g = w.gn[id];
+				// m path: -g onto the blend's screen-mean gradient, in its convention (ndc: pixels times W / 2, H / 2)
+				float* gb = w.gb + (size_t)id * GB_STRIDE;
+				gb[0] -= g.x * (0.5f * w.cam.W);
+				gb[1] -= g.y * (0.5f * w.cam.H);
+				// m' path
+				flow_mean_bwd<CAM>(w.cam, p, g.x, g.y, gp, cg);
+				if constexpr (CAM) {
+					// a next pose is a constant of the loss: its view's camera takes the m path only
+#pragma unroll
+					for (int k = 0; k < CAM_ALL_TERMS; k++) cg[k] = w.own_camera ? cg[k] : 0.f;
+				}
+			}
+		}
+		if constexpr (CAM) {
+			if (w.cam_rows) {
+				const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+				for (int k = 0; k < CAM_ALL_TERMS; k++) {
+					float s = cg[k];
+#pragma unroll
+					for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+					if (lane == 0) cam_sm[warp * CAM_ALL_TERMS + k] = s;
+				}
+				__syncthreads();
+				for (int k = threadIdx.x; k < CAM_ALL_TERMS; k += blockDim.x) {
+					float s = 0.f;
+					for (int u = 0; u < FLOW_BWD_THREADS / 32; u++) s += cam_sm[u * CAM_ALL_TERMS + k];
+					if (k < CAM_TERMS) w.cam_rows[(size_t)blockIdx.x * CAM_TERMS + k] = s;
+					else if (w.intr_rows) w.intr_rows[(size_t)blockIdx.x * CAM_INTR_TERMS + k - CAM_TERMS] = s;
+				}
+				__syncthreads();
+			}
+		}
+	}
+	if (!in || !a.dL_dnext_means3D) return;
+	float* o = a.dL_dnext_means3D + 3 * (size_t)i;
+#pragma unroll
+	for (int k = 0; k < 3; k++) o[k] = a.accumulate ? o[k] + gp[k] : gp[k];
+}
+
+void launch_flow_fwd(const FlowFwdArgs& a, cudaStream_t s)
+{
+	if (a.P > 0) flow_fwd_kernel<<<ceil_div(a.P, 256), 256, 0, s>>>(a);
+}
+
+void launch_flow_bwd(const FlowBwdArgs& a, cudaStream_t s)
+{
+	if (a.P <= 0 || a.V <= 0) return;
+	bool cam = false;
+	for (int v = 0; v < a.V; v++) cam |= a.view[v].cam_rows != nullptr;
+	const int grid = ceil_div(a.P, FLOW_BWD_THREADS);
+	if (cam) flow_bwd_kernel<true><<<grid, FLOW_BWD_THREADS, 0, s>>>(a);
+	else flow_bwd_kernel<false><<<grid, FLOW_BWD_THREADS, 0, s>>>(a);
+}
+
+}  // namespace mgs

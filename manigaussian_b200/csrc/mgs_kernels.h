@@ -462,4 +462,50 @@ cudaError_t field_backward(char* state, char* pair_state, int Q, int P, int C, c
 	const float* scales, const float* rotations, int channel_first, const float* dL_ddensity, const float* dL_dfeatures,
 	float* dL_dpoints, float* dL_dmeans, float* dL_dscales, float* dL_drot, float* dL_dopac, float* dL_dfeat, cudaStream_t st);
 
+// flow.cu: the flow plane's per-Gaussian quads {dx, dy, 0, 0} (include/mgs_rasterizer.h, flow plane) and their backward.
+// FlowCam: the map of one end of a view's flow, the view's model, intrinsics and image size with the pose that end uses.
+struct FlowCam {
+	const float* viewmatrix;
+	const float* projmatrix;     // pinhole and orthographic only
+	const float* tan_fov;        // device {tan_fovx, tan_fovy}, or NULL for the host values
+	float tan_fovx, tan_fovy;
+	int W, H;
+	int model;                   // 0 pinhole, 1 orthographic, 2 fisheye, 3 distorted pinhole
+	float cx, cy;                // fisheye or distorted principal point
+	float theta_max;             // fisheye cull
+	float r2_max;                // distorted cull
+	FisheyeK fe_k;
+	DistK dc_k;
+};
+struct FlowFwdArgs {
+	int P;
+	const float* means3D;
+	const float* next_means3D;
+	FlowCam cur, next;           // the view's camera, and the one its next-frame means are projected with
+	const int* radii;
+	float4* quad;
+};
+void launch_flow_fwd(const FlowFwdArgs& a, cudaStream_t s);
+// the backward runs behind the blend backward and ahead of the per-Gaussian stage, on the same stream, for up to
+// MAX_BWD_VIEWS views of one cloud; CTAs of FLOW_BWD_THREADS, so its camera rows have the per-Gaussian stage's row count
+constexpr int FLOW_BWD_THREADS = 128;
+struct FlowBwdView {
+	FlowCam cam;                 // the camera of the view's next-frame means
+	int own_camera;              // 1: cam is the view's own camera (no next pose), whose gradients take the m' terms
+	const int* radii;
+	const float4* gn;            // [P] blend-stage quad gradients, or NULL (the view has no flow cotangent)
+	float* gb;                   // [P, GB_STRIDE] blend-stage records: the screen-mean slots receive -gn
+	float* cam_rows;             // [CTAs][CAM_TERMS] camera rows, or NULL
+	float* intr_rows;            // [CTAs][CAM_INTR_TERMS] focal-length rows, or NULL
+};
+struct FlowBwdArgs {
+	int P, V;
+	const float* next_means3D;
+	float* dL_dnext_means3D;     // [P,3] or NULL
+	int accumulate;
+	FlowBwdView view[MAX_BWD_VIEWS];
+};
+static_assert(sizeof(FlowBwdArgs) <= 4096, "kernel parameters are limited to 4 KB");
+void launch_flow_bwd(const FlowBwdArgs& a, cudaStream_t s);
+
 }  // namespace mgs

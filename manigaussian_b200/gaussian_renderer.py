@@ -81,7 +81,7 @@ def _with_planar_depth(s):
 
 def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=None, features_color=None,
            features_language=None, return_depth=False, return_alpha=False, antialiasing=False, return_median_depth=False,
-           return_normal=False, planar_depth=False):
+           return_normal=False, planar_depth=False, flow_xyz=None, flow_camera=None):
     """Render view `idx` of data['novel_view'].  Same arguments and result as the reference's render(); with
     return_depth=True the dictionary also holds "depth" [H,W] (view-space z, alpha-blended, no background term), with
     return_alpha=True "alpha" [H,W] (accumulated opacity 1 - final_T; depth / alpha is the expected depth), with
@@ -90,7 +90,8 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
     INTEGRATION.md §7), with return_normal=True "normal" [3,H,W] (each Gaussian's shortest axis in world space, turned to
     face the camera, alpha-blended and not normalised: normal / alpha is the expected normal; differentiable, INTEGRATION.md
     §8).  antialiasing=True renders with the anti-aliased projection (opacity compensation for the 0.3 px^2
-    dilation, INTEGRATION.md §5)."""
+    dilation, INTEGRATION.md §5).  flow_xyz [P,3] (next-frame means paired with pts_xyz) adds "flow" [2,H,W], as
+    render_views' flow_xyz; flow_camera: the next frame's (viewmatrix, projmatrix), or None for the view's own camera."""
     device = pts_xyz.device
     nv = data["novel_view"]
     bg = _background(bg_color, device)
@@ -115,18 +116,71 @@ def render(data, idx, pts_xyz, rotations, scales, opacity, bg_color, pts_rgb=Non
         assert pts_rgb is not None
         colors_precomp = pts_rgb
     feat = normalize_features(features_language) if features_language is not None else None
+    pose = None
+    if flow_xyz is not None:
+        for bad, what in ((return_normal, "return_normal"), (planar_depth, "planar_depth")):
+            if bad:
+                raise ValueError(f"flow_xyz cannot be combined with {what}")
+        nxt = None
+        if flow_camera is not None:
+            nxt = [raster_settings._replace(viewmatrix=flow_camera[0], projmatrix=flow_camera[1])]
+        pose = (_flow_inputs([raster_settings], pts_xyz, flow_xyz, nxt, None, bg, 0, False) or [None])[0]
     out = rasterizer(means3D=pts_xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp,
-                     language_feature_precomp=feat, opacities=opacity, scales=scales, rotations=rotations, cov3D_precomp=None)
+                     language_feature_precomp=feat, opacities=opacity, scales=scales, rotations=rotations, cov3D_precomp=None,
+                     flow_means3D=flow_xyz, flow_pose=pose)
     ret = {"render": out[0], "render_embed": out[1], "viewspace_points": screenspace_points, "radii": out[2]}
+    nf = int(flow_xyz is not None)
+    if flow_xyz is not None:
+        ret["flow"] = out[-1]
     if return_depth:
         ret["depth"] = out[3]
     if return_alpha:
         ret["alpha"] = out[3 + bool(return_depth)]
     if return_median_depth:
-        ret["median_depth"], ret["median_id"] = out[-2 - bool(return_normal)], out[-1 - bool(return_normal)]
+        ret["median_depth"], ret["median_id"] = out[-2 - bool(return_normal) - nf], out[-1 - bool(return_normal) - nf]
     if return_normal:
         ret["normal"] = out[-1]
     return ret
+
+
+def _same_value(a, b):
+    """Whether two settings values agree.  A CUDA tensor (a learnable field of view) is not read back: the flow kernels take
+    every intrinsic from the view itself, so only host values can disagree in a way that matters, and a device comparison
+    would synchronise the host and break CUDA-graph capture."""
+    if (torch.is_tensor(a) and a.is_cuda) or (torch.is_tensor(b) and b.is_cuda):
+        return True
+    return float(a) == float(b)
+
+
+def _flow_inputs(views, pts_xyz, flow_xyz, flow_cameras, view_ids, bg, sh_degree, include):
+    """Checks flow_xyz against the cloud and returns the per-view next-frame poses (None: every view's own camera)."""
+    if not torch.is_tensor(flow_xyz) or tuple(flow_xyz.shape) != (pts_xyz.shape[0], 3) or flow_xyz.dtype != torch.float32 \
+            or flow_xyz.device != pts_xyz.device:
+        raise ValueError(f"flow_xyz: expected [{pts_xyz.shape[0]},3] fp32 on {pts_xyz.device}")
+    if flow_cameras is None:
+        return None
+    if isinstance(flow_cameras, CameraBatch):
+        ids = list(range(len(flow_cameras))) if view_ids is None else list(view_ids)
+        nxt = [flow_cameras.settings(i, bg, sh_degree, include) for i in ids]
+    else:
+        nxt = list(flow_cameras if view_ids is None else [flow_cameras[i] for i in view_ids])
+    if len(nxt) != len(views):
+        raise ValueError(f"flow_cameras: expected {len(views)} views, got {len(nxt)}")
+    poses = []
+    for s, n in zip(views, nxt):
+        for name in ("image_height", "image_width", "tanfovx", "tanfovy"):
+            if not _same_value(getattr(s, name), getattr(n, name)):
+                raise ValueError(f"flow_cameras: {name} differs from the view's (only the pose may change)")
+        if bool(getattr(s, "orthographic", False)) != bool(getattr(n, "orthographic", False)):
+            raise ValueError("flow_cameras: the camera model (orthographic) differs from the view's (only the pose may change)")
+        for name in ("fisheye", "distortion"):
+            a, b = getattr(s, name, None), getattr(n, name, None)
+            if (a is None) != (b is None) or (a is not None and not all(_same_value(x, y) for x, y in zip(tuple(a), tuple(b)))):
+                raise ValueError(f"flow_cameras: the camera model ({name}) differs from the view's (only the pose may change)")
+        if any(torch.is_tensor(t) and t.requires_grad for t in (n.viewmatrix, n.projmatrix)):
+            raise ValueError("flow_cameras: next-frame poses are constants of the loss and must not require grad")
+        poses.append((n.viewmatrix, n.projmatrix))
+    return poses
 
 
 def _device_tan_fov(views):
@@ -182,7 +236,7 @@ class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
                 group, antialiasing=False, return_median=False, return_normal=False, cam_vm=None, cam_pm=None, cam_cp=None,
-                cam_tf=None):
+                cam_tf=None, flow_xyz=None, flow_poses=None):
         dev = means3D.device
         V, P = len(views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -200,13 +254,16 @@ class _RasterizeViews(torch.autograd.Function):
         med_depth = torch.empty((V, H, W), **opts) if return_median else None
         med_id = torch.empty((V, H, W), dtype=torch.int32, device=dev) if return_median else None
         normal = torch.empty((V, 3, H, W), **opts) if return_normal else None
+        flow = torch.empty((V, 3, H, W), **opts) if flow_xyz is not None else None
+        flow_xyz = flow_xyz.detach() if flow_xyz is not None else None
         degree = views[0].sh_degree
         outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
                                             views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
                                             debug=views[0].debug,
-                                            out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal),
+                                            out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal, flow),
                                             return_alpha=return_alpha, antialiasing=antialiasing, tan_fov=cam_tf,
-                                            return_median=return_median, return_normal=return_normal)
+                                            return_median=return_median, return_normal=return_normal, flow_means3D=flow_xyz,
+                                            flow_poses=flow_poses)
         main = torch.cuda.current_stream(dev)
         for st in streams:
             main.wait_stream(st)
@@ -216,20 +273,23 @@ class _RasterizeViews(torch.autograd.Function):
         ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
         ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
         ctx.opac_shape = opacities.shape
+        ctx.flow_poses = flow_poses
         empty = torch.empty(0, device=dev)
         # the id and normal planes are outputs: they reach the backward through save_for_backward (an output on ctx is a
         # reference cycle)
         ctx.save_for_backward(means3D, sh if sh is not None else empty, colors_precomp if colors_precomp is not None else empty,
                               feature if include else empty, scales, rotations, med_id if return_median else empty,
-                              normal if return_normal else empty)
+                              normal if return_normal else empty, flow if flow is not None else empty,
+                              flow_xyz if flow_xyz is not None else empty)
         ctx.mark_non_differentiable(radii, *([med_id] if return_median else []))
         return (color, (feat_img if include else empty), radii, (depth if return_depth else empty),
                 (alpha if return_alpha else empty), (med_depth if return_median else empty),
-                (med_id if return_median else empty), (normal if return_normal else empty))
+                (med_id if return_median else empty), (normal if return_normal else empty),
+                (flow[:, :2] if flow is not None else empty))
 
     @staticmethod
-    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha, g_median, _g_median_id, g_normal):
-        means3D, sh, colors_precomp, feature, scales, rotations, med_id, normal = ctx.saved_tensors
+    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha, g_median, _g_median_id, g_normal, g_flow=None):
+        means3D, sh, colors_precomp, feature, scales, rotations, med_id, normal, flow, flow_xyz = ctx.saved_tensors
         dev = means3D.device
         views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
         H, W = int(views[0].image_height), int(views[0].image_width)
@@ -245,6 +305,9 @@ class _RasterizeViews(torch.autograd.Function):
         g_alpha = _prep(g_alpha, dev) if (ctx.return_alpha and g_alpha is not None and g_alpha.numel()) else None
         g_median = _prep(g_median, dev) if (med_id.numel() and g_median is not None and g_median.numel()) else None
         g_normal = _prep(g_normal, dev) if (normal.numel() and g_normal is not None and g_normal.numel()) else None
+        has_flow = flow_xyz.numel() > 0
+        if has_flow and g_flow is None:
+            g_flow = torch.zeros((V, 2, H, W), dtype=torch.float32, device=dev)
         pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)  # every row is written by the backward
         grp = None if ctx.group in (None, True) else ctx.group
         m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
@@ -256,7 +319,9 @@ class _RasterizeViews(torch.autograd.Function):
                                            after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
                                            antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None,
                                            tan_fov=ctx.tan_fov, grads_median=g_median, median_ids=med_id if g_median is not None else None,
-                                           grads_normal=g_normal, normals=normal if g_normal is not None else None)
+                                           grads_normal=g_normal, normals=normal if g_normal is not None else None,
+                                           flow_means3D=flow_xyz if has_flow else None, flow_poses=ctx.flow_poses,
+                                           grads_flow=list(g_flow) if has_flow else None, flows=list(flow) if has_flow else None)
         if ctx.group is not None:
             # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
             # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields.
@@ -266,7 +331,7 @@ class _RasterizeViews(torch.autograd.Function):
         return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
                 v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
                 v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None,
-                *_camera_outputs(ctx, res[9] if ctx.camera else None, 15))
+                *_camera_outputs(ctx, res[9] if ctx.camera else None, 15), res[-1] if has_flow else None, None)
 
 
 def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
@@ -427,7 +492,7 @@ class _RasterizeViewsLoss(torch.autograd.Function):
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
                  features_language=None, view_ids=None, return_depth=False, sync_gradients=None, normalize_feature=True,
                  targets=None, return_alpha=False, antialiasing=False, ssim=False, return_median_depth=False, return_normal=False,
-                 planar_depth=False):
+                 planar_depth=False, flow_xyz=None, flow_cameras=None):
     """Render several cameras of one Gaussian cloud in one autograd node.
 
     cameras: `cameras.CameraBatch` (or a sequence of GaussianRasterizationSettings); view_ids selects a subset (e.g. this
@@ -476,6 +541,13 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     planar_depth: the depth plane, the depth head (targets["depth"]) and the median depth take each Gaussian's depth along
     the pixel's ray, affine in the pixel offset, instead of its centre depth (include/mgs_rasterizer.h,
     mgs_forward_views_planar); also on when the given settings carry planar_depth=True.  Not with return_normal.
+    flow_xyz: [P,3] next-frame means paired by index with pts_xyz (e.g. the deformed cloud of the dyna step); the result then
+    gains "flow" [V,2,H,W], each Gaussian's screen displacement m' - m in pixels (x right, y down) blended with the colour's
+    weights (flow / alpha is the expected flow; include/mgs_rasterizer.h, flow plane), differentiable in the cloud, the
+    cameras and flow_xyz.  flow_cameras: a CameraBatch or settings aligned with the views (view_ids applies) whose poses
+    project flow_xyz, e.g. a wrist camera that moved; by default each view's own.  Only its view and projection matrices are
+    read; the model, intrinsics and image size must be the view's.  Not with targets, return_normal, planar_depth or
+    sync_gradients.
     Returns {"render" [V,3,H,W], "render_embed" [V,F,H,W] | None, "depth" [V,H,W] (if asked), "alpha" [V,H,W] (if asked),
     "viewspace_points" [V,P,3] (its .grad holds each view's screen-space mean gradients), "radii" [V,P] int32}."""
     device = pts_xyz.device
@@ -504,6 +576,15 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     if ssim and targets is None:
         raise ValueError("ssim=True needs targets (the colour target \"rgb\")")
     cams = _camera_inputs(views, batch=batch)
+    flow_poses = None
+    if flow_xyz is not None:
+        for bad, what in ((targets is not None, "targets"), (return_normal, "return_normal"),
+                          (any(bool(getattr(s, "planar_depth", False)) for s in views), "planar_depth"),
+                          (sync_gradients is not None, "sync_gradients")):
+            if bad:
+                raise ValueError(f"flow_xyz cannot be combined with {what}")
+        flow_poses = _flow_inputs(views, pts_xyz, flow_xyz, flow_cameras, view_ids, _background(bg_color, device), sh_degree,
+                                  include)
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
@@ -527,6 +608,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         if ssim:
             ret["loss_l1"], ret["ssim"] = loss_l1, ssim_v
         return ret
+    flow = None
     if V == 1 and sync_gradients is None and cams[0] is None and cams[3] is None:
         # a single view needs neither side streams nor the packed accumulation buffer: the single-view operator is leaner
         st = GaussianRasterizationSettings(*tuple(views[0])[:13], antialiasing=True,
@@ -538,18 +620,21 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
                                  return_normal=return_normal)(
             means3D=pts_xyz, means2D=screenspace_points[0], shs=features_color,
             colors_precomp=pts_rgb if features_color is None else None, language_feature_precomp=feat, opacities=opacity,
-            scales=scales, rotations=rotations, cov3D_precomp=None)
+            scales=scales, rotations=rotations, cov3D_precomp=None, flow_means3D=flow_xyz,
+            flow_pose=flow_poses[0] if flow_poses is not None else None)
         color, feat_img, radii = out[0].unsqueeze(0), out[1].unsqueeze(0), out[2].unsqueeze(0)
         depth = out[3].unsqueeze(0) if return_depth else None
         alpha = out[3 + bool(return_depth)].unsqueeze(0) if return_alpha else None
-        nn = bool(return_normal)
+        nf = int(flow_xyz is not None)
+        nn = bool(return_normal) + nf
         med_depth, med_id = (out[-2 - nn].unsqueeze(0), out[-1 - nn].unsqueeze(0)) if return_median_depth else (None, None)
-        normal = out[-1].unsqueeze(0) if return_normal else None
+        normal = out[-1 - nf].unsqueeze(0) if return_normal else None
+        flow = out[-1].unsqueeze(0) if flow_xyz is not None else None
     else:
-        color, feat_img, radii, depth, alpha, med_depth, med_id, normal = _RasterizeViews.apply(
+        color, feat_img, radii, depth, alpha, med_depth, med_id, normal, flow = _RasterizeViews.apply(
             pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
             rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa, bool(return_median_depth),
-            bool(return_normal), *cams)
+            bool(return_normal), *cams, flow_xyz, flow_poses)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
@@ -560,6 +645,8 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         ret["median_depth"], ret["median_id"] = med_depth, med_id
     if return_normal:
         ret["normal"] = normal
+    if flow_xyz is not None:
+        ret["flow"] = flow
     return ret
 
 
@@ -734,15 +821,19 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 class _RasterizeClouds(torch.autograd.Function):
     """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha, antialiasing,
-    ssim, camera, return_median, return_normal).  Outputs per cloud: (color, feature image, radii, depth, alpha, median depth,
-    median id, normal), or
+    ssim, camera, return_median, return_normal, flow).  flow: None, or per cloud None or its next-frame poses (a list of
+    (viewmatrix, projmatrix) or None per view, or None for the views' own cameras) with that cloud's flow_xyz among the inputs,
+    behind every other input.  Outputs per cloud: (color, feature image, radii, depth, alpha, median depth, median id, normal,
+    flow), or
     with targets (loss_rgb, loss_embed, color, feature image, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim) with
     gradients through the losses only."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = meta[:9]
+        flows = meta[9]
         B, dev = len(cloud_views), flat[0].device
+        flow_in = [t.detach() if t is not None else None for t in flat[len(flat) - B:]] if flows is not None else [None] * B
         opts = dict(dtype=torch.float32, device=dev)
         clouds, results, frozen, cots, dms, ssims, images = [], [], [], [], [], [], []
         for b, views in enumerate(cloud_views):
@@ -756,12 +847,16 @@ class _RasterizeClouds(torch.autograd.Function):
             med_depth = torch.empty((V, H, W), **opts) if return_median else None
             med_id = torch.empty((V, H, W), dtype=torch.int32, device=dev) if return_median else None
             normal = torch.empty((V, 3, H, W), **opts) if return_normal else None
+            flow = torch.empty((V, 3, H, W), **opts) if flow_in[b] is not None else None
             c = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=feature, opacity=opacities, scales=scales,
-                     rotations=rotations, out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal))
+                     rotations=rotations, out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal, flow))
+            if flow is not None:
+                c["flow_means3D"], c["flow_poses"] = flow_in[b], flows[b]
             if targets is None:
-                # the id and normal planes are outputs: saved for backward, never kept on ctx
+                # the id, normal and flow planes are outputs: saved for backward, never kept on ctx
                 images += [med_id if return_median else torch.empty(0, device=dev),
-                           normal if return_normal else torch.empty(0, device=dev)]
+                           normal if return_normal else torch.empty(0, device=dev),
+                           flow if flow is not None else torch.empty(0, device=dev)]
             if targets is not None:
                 t_rgb = _prep(targets[b]["rgb"], dev)
                 t_emb = _prep(targets[b].get("embed"), dev) if F else None
@@ -785,7 +880,7 @@ class _RasterizeClouds(torch.autograd.Function):
                                              debug=cloud_views[0][0].debug, return_alpha=return_alpha, antialiasing=antialiasing,
                                              return_median=return_median, return_normal=return_normal)
         for b, c in enumerate(clouds):
-            color, feat_img, depth, alpha, med_depth, med_id, normal = c["out_buffers"]
+            color, feat_img, depth, alpha, med_depth, med_id, normal, flow = c["out_buffers"]
             radii = torch.stack([o[3] for o in outs[b]])
             empty = lambda: torch.empty(0, device=dev)
             if targets is not None:
@@ -801,7 +896,8 @@ class _RasterizeClouds(torch.autograd.Function):
             else:
                 results += [color, feat_img if feat_img is not None else empty(), radii, depth if depth is not None else empty(),
                             alpha if alpha is not None else empty(), med_depth if med_depth is not None else empty(),
-                            med_id if med_id is not None else empty(), normal if normal is not None else empty()]
+                            med_id if med_id is not None else empty(), normal if normal is not None else empty(),
+                            flow[:, :2] if flow is not None else empty()]
                 frozen += [radii] + ([med_id] if med_id is not None else [])
         ctx.meta, ctx.streams, ctx.degree, ctx.include, ctx.cots, ctx.dms, ctx.ssims = meta, streams, degree, include, cots, dms, ssims
         # capacity, radii and the state buffers per view -- never an output (an output kept on ctx is a reference cycle)
@@ -809,17 +905,22 @@ class _RasterizeClouds(torch.autograd.Function):
         ctx.opac_shapes = [flat[_CLOUD_INPUTS * b + 5].shape for b in range(B)]
         e = torch.empty(0, device=dev)
         ctx.save_for_backward(*[x if x is not None else e for c in clouds for x in
-                                (c["means3D"], c["sh"], c["colors"], c["feature"], c["scales"], c["rotations"])], *images)
+                                (c["means3D"], c["sh"], c["colors"], c["feature"], c["scales"], c["rotations"])], *images,
+                              *[t if t is not None else e for t in flow_in])
         ctx.mark_non_differentiable(*frozen)  # ONE call: a second one replaces the first
         return tuple(results)
 
     @staticmethod
     def backward(ctx, *grads):
-        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = ctx.meta
+        cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = ctx.meta[:9]
+        flows = ctx.meta[9]
         saved = ctx.saved_tensors
         dev = saved[0].device
-        images = saved[6 * len(cloud_views):]  # per cloud: the image (targets with ssim), or the median ids and the normal plane
-        per = 10 if targets is not None else 8
+        B = len(cloud_views)
+        flow_in = saved[len(saved) - B:]
+        # per cloud: the image (targets with ssim), or the median ids, the normal plane and the flow plane
+        images = saved[6 * B:len(saved) - B]
+        per = 10 if targets is not None else 9
         clouds = []
         for b, views in enumerate(cloud_views):
             means3D, sh, colors, feature, scales, rotations = (t if t.numel() else None for t in saved[6 * b:6 * b + 6])
@@ -846,9 +947,12 @@ class _RasterizeClouds(torch.autograd.Function):
                 if return_alpha and g[4] is not None:
                     c["grad_alpha"] = g[4]
                 if return_median and g[5] is not None:
-                    c["grad_median"], c["median_id"] = g[5], images[2 * b]
+                    c["grad_median"], c["median_id"] = g[5], images[3 * b]
                 if return_normal and g[7] is not None:
-                    c["grad_normal"], c["normal"] = g[7], images[2 * b + 1]
+                    c["grad_normal"], c["normal"] = g[7], images[3 * b + 1]
+                if flow_in[b].numel():
+                    c["flow_means3D"], c["flow_poses"], c["flow"] = flow_in[b], flows[b], images[3 * b + 2]
+                    c["grad_flow"] = g[8] if g[8] is not None else torch.zeros((V, 2, H, W), dtype=torch.float32, device=dev)
             clouds.append(c)
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
@@ -865,6 +969,8 @@ class _RasterizeClouds(torch.autograd.Function):
             for b, r in enumerate(res):
                 cam = (r["dL_dviewmatrix"], r["dL_dprojmatrix"], r["dL_dcampos"], r.get("dL_dtan_fov"))
                 ret += _camera_outputs(ctx, cam, first + 4 * b)
+        if flows is not None:  # every cloud's flow_xyz, behind the camera inputs
+            ret += [r.get("dL_dflow_means3D") for r in res]
         return tuple(ret)
 
 
@@ -887,7 +993,10 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
     ssim: every cloud also returns "loss_l1" and "ssim" [V], as in render_views; needs targets.
     return_median_depth: every cloud also returns "median_depth" and "median_id" [V,H,W], as in render_views; not with targets.
     return_normal: every cloud also returns "normal" [V,3,H,W], as in render_views; not with targets.
-    planar_depth: every cloud's depth follows each Gaussian's tilt, as in render_views."""
+    planar_depth: every cloud's depth follows each Gaussian's tilt, as in render_views.
+    A cloud's optional "flow_xyz" [P,3] (its next-frame means) and "flow_cameras" render its "flow" [V,2,H,W], as
+    render_views' flow_xyz and flow_cameras.  For the dyna pair pass the next cloud's pts_xyz tensor as the current cloud's
+    flow_xyz: autograd sums both of its uses.  Not with targets, return_normal or planar_depth."""
     if not clouds:
         raise ValueError("render_clouds needs at least one cloud")
     with_targets = [c.get("targets") is not None for c in clouds]
@@ -941,6 +1050,22 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         flat += [c["pts_xyz"], vsps[-1], c.get("features_color"), c.get("pts_rgb") if c.get("features_color") is None else None, f,
                  c["opacity"], c["scales"], c["rotations"]]
     targets = [c["targets"] for c in clouds] if all(with_targets) else None
+    flows = None
+    if any(c.get("flow_xyz") is not None for c in clouds):
+        for bad, what in ((targets is not None, "targets"), (return_normal, "return_normal"),
+                          (any(bool(getattr(s, "planar_depth", False)) for views in cloud_views for s in views), "planar_depth")):
+            if bad:
+                raise ValueError(f"flow_xyz cannot be combined with {what}")
+        flows = []
+        for c, views in zip(clouds, cloud_views):
+            if c.get("flow_xyz") is None:
+                flows.append(None)
+                continue
+            sh_degree = 3 if c.get("features_color") is None else 1
+            poses = _flow_inputs(views, c["pts_xyz"], c["flow_xyz"], c.get("flow_cameras"), c.get("view_ids"),
+                                 _background(bg_color, device), sh_degree, c.get("features_language") is not None)
+            flows.append(poses)
+        flows = tuple(flows)
     aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for views in cloud_views for s in views)
     cams = [_camera_inputs(views, batch=bt) for views, bt in zip(cloud_views, batches)]
     camera = any(c[0] is not None for c in cams)
@@ -948,8 +1073,10 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
         cams = [c if c[0] is not None else _camera_inputs(views, force=True, batch=bt)
                 for c, views, bt in zip(cams, cloud_views, batches)]
         flat += [t for c in cams for t in c]
+    if flows is not None:
+        flat += [c.get("flow_xyz") for c in clouds]
     out = _RasterizeClouds.apply((tuple(cloud_views), bool(return_depth), targets, bool(return_alpha), aa, bool(ssim), camera,
-                                  bool(return_median_depth), bool(return_normal)), *flat)
+                                  bool(return_median_depth), bool(return_normal), flows), *flat)
     ret = []
     for b, c in enumerate(clouds):
         include, vsp = c.get("features_language") is not None, vsps[b]
@@ -965,7 +1092,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                 r["loss_l1"], r["ssim"] = loss_l1, ssim_v
             ret.append(r)
         else:
-            color, feat_img, radii, depth, alpha, med_depth, med_id, normal = out[8 * b:8 * b + 8]
+            color, feat_img, radii, depth, alpha, med_depth, med_id, normal, flow = out[9 * b:9 * b + 9]
             r = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": vsp, "radii": radii}
             if return_depth:
                 r["depth"] = depth
@@ -975,5 +1102,7 @@ def render_clouds(clouds, bg_color=(0.0, 0.0, 0.0), return_depth=False, normaliz
                 r["median_depth"], r["median_id"] = med_depth, med_id
             if return_normal:
                 r["normal"] = normal
+            if c.get("flow_xyz") is not None:
+                r["flow"] = flow
             ret.append(r)
     return ret

@@ -263,7 +263,7 @@ def cpu_deep_copy_tuple(input_tuple):
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median_depth=False,
-                        return_normal=False):
+                        return_normal=False, flow_means3D=None, flow_pose=None):
     s = raster_settings
     # camera tensors that require grad become explicit inputs of the node, which then returns their gradients; a field of
     # view held as CUDA tensors (learnable intrinsics) joins them as two more inputs, tanfovx and tanfovy
@@ -274,18 +274,22 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, language_feature_p
         cam = ()
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales,
                                      rotations, cov3Ds_precomp, raster_settings, return_depth, return_alpha,
-                                     bool(return_median_depth), bool(return_normal), *cam)
+                                     bool(return_median_depth), bool(return_normal), flow_means3D, flow_pose, *cam)
 
 
-_CAM_FIRST = 14  # position of the first camera input of _RasterizeGaussians
+_CAM_FIRST = 16  # position of the first camera input of _RasterizeGaussians
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, language_feature_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, return_depth=False, return_alpha=False, return_median=False,
-                return_normal=False, *cam):
+                return_normal=False, flow_means3D=None, flow_pose=None, *cam):
         s = raster_settings
+        ctx.flow = flow_means3D is not None
+        ctx.flow_pose = flow_pose
+        flow_means3D = flow_means3D.detach() if ctx.flow else None
+        flow = None
         args = (s.bg, means3D, colors_precomp, language_feature_precomp, opacities, scales, rotations, s.scale_modifier,
                 cov3Ds_precomp, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.image_height, s.image_width, sh,
                 s.sh_degree, s.campos, s.prefiltered, s.debug, s.include_feature)
@@ -304,7 +308,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         orth = bool(getattr(s, "orthographic", False)) or getattr(s, "fisheye", None) is not None \
             or getattr(s, "distortion", None) is not None or bool(getattr(s, "planar_depth", False))
         ctx.orthographic = orth
-        if (return_alpha or return_median or return_normal or aa or orth or ctx.camera) and views_path:
+        if ctx.flow and not views_path:
+            raise RuntimeError("the flow plane needs a CUDA cloud with at least one Gaussian")
+        if (return_alpha or return_median or return_normal or aa or orth or ctx.camera or ctx.flow) and views_path:
             # the alpha plane, the median planes, the anti-aliased, orthographic, fisheye and distorted projections and the camera
             # gradients exist on
             # the multi-view entry points only: debug renders take them too, with the snapshot dump
@@ -314,7 +320,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                                                     rotations, s.scale_modifier, cov3Ds_precomp, sh, s.sh_degree, s.include_feature,
                                                     return_depth=return_depth, debug=s.debug, return_alpha=return_alpha,
                                                     antialiasing=aa, tan_fov=tf, return_median=return_median,
-                                                    return_normal=return_normal)
+                                                    return_normal=return_normal, flow_means3D=flow_means3D,
+                                                    flow_poses=[flow_pose] if ctx.flow else None)
             except Exception as ex:
                 if s.debug:
                     torch.save(cpu_args, "snapshot_fw.dump")
@@ -323,10 +330,13 @@ class _RasterizeGaussians(torch.autograd.Function):
             out = outs[0]
             planes = 7 + bool(return_depth)
             alpha = out[planes] if return_alpha else None
+            nf = int(ctx.flow)
+            if ctx.flow:
+                flow = out[-1]
             if return_normal:
-                normal = out[-1]
+                normal = out[-1 - nf]
             if return_median:
-                med_depth, med_id = out[-2 - bool(return_normal)], out[-1 - bool(return_normal)]
+                med_depth, med_id = out[-2 - bool(return_normal) - nf], out[-1 - bool(return_normal) - nf]
             ctx.async_view = (int(out[0]), streams)  # as below: never the outputs themselves
         elif s.debug:
             cpu_args = cpu_deep_copy_tuple(args)  # copy before they can be corrupted
@@ -369,13 +379,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         # cycle)
         ctx.save_for_backward(colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii,
                               sh, geomBuffer, binningBuffer, imgBuffer, med_id if return_median else None,
-                              normal if return_normal else None)
+                              normal if return_normal else None, flow, flow_means3D)
         if return_median:
             ctx.mark_non_differentiable(radii, med_id)
         else:
             ctx.mark_non_differentiable(radii)
         return (color, language_feature, radii) + ((depth,) if return_depth else ()) + ((alpha,) if return_alpha else ()) + \
-            ((med_depth, med_id) if return_median else ()) + ((normal,) if return_normal else ())
+            ((med_depth, med_id) if return_median else ()) + ((normal,) if return_normal else ()) + \
+            ((flow[:2],) if ctx.flow else ())
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_out_language_feature, _radii=None, *grad_planes):
@@ -383,11 +394,16 @@ class _RasterizeGaussians(torch.autograd.Function):
         # gradient and the (absent) id gradient when return_median, then the normal gradient when return_normal
         grad_out_depth = grad_planes[0] if ctx.return_depth else None
         grad_out_alpha = grad_planes[int(ctx.return_depth)] if ctx.return_alpha else None
-        grad_out_median = grad_planes[-2 - int(ctx.return_normal)] if ctx.return_median else None
-        grad_out_normal = grad_planes[-1] if ctx.return_normal else None
+        # and the flow gradient, last, with a flow plane
+        nf = int(ctx.flow)
+        grad_out_median = grad_planes[-2 - int(ctx.return_normal) - nf] if ctx.return_median else None
+        grad_out_normal = grad_planes[-1 - nf] if ctx.return_normal else None
+        grad_out_flow = grad_planes[-1] if ctx.flow else None
         s = ctx.raster_settings
         (colors_precomp, language_feature_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-         binningBuffer, imgBuffer, med_id, normal) = ctx.saved_tensors
+         binningBuffer, imgBuffer, med_id, normal, flow, flow_means3D) = ctx.saved_tensors
+        if ctx.flow and grad_out_flow is None:
+            grad_out_flow = torch.zeros((2, s.image_height, s.image_width), dtype=torch.float32, device=means3D.device)
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, s.image_height, s.image_width), dtype=torch.float32, device=means3D.device)
         if s.include_feature and grad_out_language_feature is None:
@@ -413,7 +429,9 @@ class _RasterizeGaussians(torch.autograd.Function):
                     grads_median=[grad_out_median] if grad_out_median is not None else None,
                     median_ids=[med_id] if grad_out_median is not None else None,
                     grads_normal=[grad_out_normal] if (grad_out_normal is not None and normal is not None) else None,
-                    normals=[normal] if (grad_out_normal is not None and normal is not None) else None)
+                    normals=[normal] if (grad_out_normal is not None and normal is not None) else None,
+                    flow_means3D=flow_means3D, flow_poses=[ctx.flow_pose] if ctx.flow else None,
+                    grads_flow=[grad_out_flow] if ctx.flow else None, flows=[flow] if ctx.flow else None)
             except Exception as ex:
                 if cpu_args is not None:
                     torch.save(cpu_args, "snapshot_bw.dump")
@@ -435,7 +453,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.camera:
             # zero gradients when the views path did not run (no Gaussians: nothing depends on the camera)
             z = lambda n: torch.zeros((1, n), device=means3D.device)  # noqa: E731
-            cg = grads[9] if len(grads) > 9 else (z(16), z(16), z(3), z(2))
+            cg = grads[9] if len(grads) > 9 + int(ctx.flow) else (z(16), z(16), z(3), z(2))
             dvm, dpm, dcp = cg[:3]
             gs, ts = [dvm, dpm, dcp], [s.viewmatrix, s.projmatrix, s.campos]
             if _is_device_fov(s):   # tanfovx, tanfovy: the two entries of the view's dL/dtan_fov
@@ -450,7 +468,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, _or_none(grad_sh, sh), _or_none(grad_colors_precomp, colors_precomp),
                 _or_none(grad_language_feature_precomp, language_feature_precomp) if s.include_feature else None,
                 grad_opacities, _or_none(grad_scales, scales), _or_none(grad_rotations, rotations),
-                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None, None, None) + grad_cam
+                _or_none(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None, None, None,
+                grads[-1] if ctx.flow else None, None) + grad_cam
 
 
 class _Settings(NamedTuple):
@@ -577,7 +596,9 @@ class GaussianRasterizer(nn.Module):
             return mark_visible_raw(positions, s.viewmatrix, s.projmatrix)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, language_feature_precomp=None,
-                scales=None, rotations=None, cov3D_precomp=None):
+                scales=None, rotations=None, cov3D_precomp=None, flow_means3D=None, flow_pose=None):
+        """flow_means3D [P,3]: the cloud's next-frame means; the outputs then end with the flow plane [2,H,W] (include/mgs_rasterizer.h,
+        flow plane), with flow_pose (the next frame's (viewmatrix, projmatrix), or None for the view's own camera)."""
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -592,7 +613,7 @@ class GaussianRasterizer(nn.Module):
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, language_feature_precomp, opacities, scales,
                                    rotations, cov3D_precomp, self.raster_settings, self.return_depth, self.return_alpha,
-                                   self.return_median_depth, self.return_normal)
+                                   self.return_median_depth, self.return_normal, flow_means3D, flow_pose)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -701,6 +722,19 @@ def _state_sizes(L, P, W, H, normal=False):
     return s
 
 
+def _check_flow(flow_means3D, normal, planar, depth_mask):
+    """The flow plane's call-wide argument errors (ValueError): it takes the normal plane's tile columns, and has no kernel
+    beside the depth / mask heads."""
+    if flow_means3D is None:
+        return
+    if normal:
+        raise ValueError("flow cannot be combined with a normal plane (return_normal): both take the same tile columns")
+    if planar:
+        raise ValueError("flow cannot be combined with planar_depth: both take the same tile columns")
+    if depth_mask is not None:
+        raise ValueError("flow cannot be combined with the depth / mask heads")
+
+
 def _planar_flag(views, planar_depth=None, normal=False):
     """The call's planar-depth flag: `planar_depth` when given, else the views' `planar_depth` attribute (every view of one
     call must agree).  Raises ValueError beside a normal plane (both take the same columns of the blend's channel tile)."""
@@ -713,6 +747,37 @@ def _planar_flag(views, planar_depth=None, normal=False):
     if planar_depth and normal:
         raise ValueError("planar_depth cannot be combined with a normal plane (return_normal) in the same call")
     return planar_depth
+
+
+def _flow_array(views, flow_means3D, flow_poses, P, dev, keep, planes=None, grads=None):
+    """ViewFlow array of the views' flow planes (C ABI mgs_view_flow), or None without `flow_means3D`.  flow_poses: None, or
+    per view None (the view's own camera) or (viewmatrix, projmatrix) of its next frame.  planes / grads: the backward's
+    forward planes and cotangents (per view [3,H,W] or [2,H,W]).  The tensors that must stay alive go to `keep`."""
+    if flow_means3D is None:
+        return None
+    if tuple(flow_means3D.shape) != (P, 3) or flow_means3D.dtype != torch.float32 or flow_means3D.device != dev:
+        raise ValueError(f"flow_means3D: expected [{P},3] fp32 on {dev}, got {tuple(flow_means3D.shape)} {flow_means3D.dtype} "
+                         f"on {flow_means3D.device}")
+    V = len(views)
+    if flow_poses is not None and len(flow_poses) != V:
+        raise ValueError(f"flow_poses: expected {V} entries, got {len(flow_poses)}")
+    arr = (_b.ViewFlow * V)()
+    for v in range(V):
+        pose = flow_poses[v] if flow_poses is not None else None
+        if pose is not None:
+            vm, pm = (_prep(torch.as_tensor(x, dtype=torch.float32, device=dev).detach().reshape(4, 4), dev) for x in pose)
+            arr[v].next_viewmatrix, arr[v].next_projmatrix = _ptr(vm), _ptr(pm)
+            keep += [vm, pm]
+        if planes is not None:
+            arr[v].out_flow = _ptr(planes[v])
+        if grads is not None and grads[v] is not None:
+            g = grads[v]
+            if g.shape[0] == 2:  # the plane's third channel carries no cotangent
+                g = torch.cat([g, torch.zeros_like(g[:1])])
+            g = _prep(g, dev)
+            arr[v].dL_dpix_flow = _ptr(g)
+            keep.append(g)
+    return arr
 
 
 def _ortho_flags(views, ortho=None):
@@ -833,7 +898,8 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
 def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                         sh, degree, include_feature, return_depth=False, debug=False, out_buffers=None, capacities=None,
                         loss_heads=None, return_alpha=False, depth_mask=None, antialiasing=False, ssim=None, tan_fov=None,
-                        return_median=False, return_normal=False, ortho=None, fisheye=None, distortion=None, planar_depth=None):
+                        return_median=False, return_normal=False, ortho=None, fisheye=None, distortion=None, planar_depth=None,
+                        flow_means3D=None, flow_poses=None):
     """Forward of V views of one Gaussian cloud.  `views` is a sequence of GaussianRasterizationSettings (bg, viewmatrix,
     projmatrix, tanfov*, image size, campos are read per view).  Returns (outs, streams): outs[v] is a ViewOut; all work
     is joined into the caller's current stream before the call returns (`streams` are the per-view streams used).
@@ -864,7 +930,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     `distortion` attribute) marks the distorted-pinhole views, by default each view's `distortion` attribute; with any
     distorted view the call is mgs_forward_views_distorted.  `planar_depth` (default: the views' `planar_depth` attribute):
     each Gaussian's depth follows its tilt across its footprint, in the depth plane, the depth head and the median depth
-    (C ABI mgs_forward_views_planar); it cannot be combined with `return_normal`."""
+    (C ABI mgs_forward_views_planar); it cannot be combined with `return_normal`.  `flow_means3D` [P,3] (the cloud's
+    next-frame means, paired by index) appends, last, every view's flow plane [3,H,W] (channels: x and y screen displacement
+    in pixels, blended with the colour's weights; channel 2 is 0; C ABI mgs_forward_views_flow; out_buffers[7] [V,3,H,W]
+    when given), with `flow_poses` (per view None or the next frame's (viewmatrix, projmatrix)) the pose each view projects
+    the next means with.  Not with `return_normal`, `planar_depth` or `depth_mask`."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -878,6 +948,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
     pln = _planar_flag(views, planar_depth, return_normal)
+    _check_flow(flow_means3D, return_normal, pln, depth_mask)
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
     dcarr = _distortion_array(views, distortion)
@@ -903,6 +974,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
         narr = (_b.ViewNormal * V)() if return_normal else None
         status = _status_slots(V)
         keep, outs = [], []
+        flarr = _flow_array(views, flow_means3D, flow_poses, P, dev, keep)
         for v, s in enumerate(views):
             if darr is not None:
                 _fill_depth_mask(darr[v], depth_mask, v)
@@ -911,7 +983,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
             cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
             o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
                                  aarr[v] if return_alpha else None, marr[v] if return_median else None,
-                                 narr[v] if return_normal else None, quads=pln)
+                                 narr[v] if return_normal else None, quads=pln, wf=flarr[v] if flarr is not None else None)
             arr[v].status = status.data_ptr() + 8 * v
             arr[v].stream = streams[v].cuda_stream
             keep.append(k)
@@ -920,7 +992,11 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if pln:
+        if flarr is not None:
+            _b.check(L.mgs_forward_views_flow(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                              _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                              dcarr, int(pln), flarr, _ptr(flow_means3D), *rest), "mgs_forward_views_flow")
+        elif pln:
             _b.check(L.mgs_forward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                 dcarr, 1, *rest), "mgs_forward_views_planar")
@@ -1069,14 +1145,14 @@ def _fill_ssim(ws, ssim, v, w=None, scale=None):
 
 
 def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads, wa=None, wm=None, wn=None,
-                  quads=False):
+                  quads=False, wf=None):
     """Allocates view v's state buffers and outputs and fills its mgs_view `w` (the caller sets status and stream) and, when
     `wa` (its mgs_view_alpha) is given, its alpha plane, when `wm` (its mgs_view_median) is given, its median planes, and when
     `wn` (its mgs_view_normal) is given, its normal plane.  `quads`: the geometry state also holds per-Gaussian quads (the
-    planar-depth call), as with `wn`.
+    planar-depth call), as with `wn`.  When `wf` (its mgs_view_flow) is given, its flow plane [3,H,W], last.
     Returns the ViewOut and the tensors that must stay alive until the call is enqueued."""
     H, W = int(s.image_height), int(s.image_width)
-    gbytes, ibytes, _ = _state_sizes(L, P, W, H, wn is not None or quads)
+    gbytes, ibytes, _ = _state_sizes(L, P, W, H, wn is not None or quads or wf is not None)
     geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
     img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
     binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
@@ -1118,6 +1194,11 @@ def _forward_view(L, w, s, v, dev, P, F, cap, include_feature, return_depth, out
         normal = ob[v] if ob is not None else torch.empty((3, H, W), dtype=torch.float32, device=dev)
         wn.out_normal = _ptr(normal)
         ret += (normal,)
+    if wf is not None:
+        ob = out_buffers[7] if (out_buffers is not None and len(out_buffers) > 7) else None
+        flow = ob[v] if ob is not None else torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        wf.out_flow = _ptr(flow)
+        ret += (flow,)
     return ViewOut(ret), (bg, vm, pm, cp)
 
 
@@ -1179,7 +1260,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                                  debug=False, accumulate_into=None, means2D_per_view=None, accumulate=False, after_blend=None,
                                  cot_scale=None, grads_alpha=None, depth_mask=None, depth_mask_scale=None, antialiasing=False,
                                  ssim=None, ssim_scale=None, camera_grads=None, tan_fov=None, grads_median=None, median_ids=None,
-                                 grads_normal=None, normals=None, ortho=None, fisheye=None, distortion=None, planar_depth=None):
+                                 grads_normal=None, normals=None, ortho=None, fisheye=None, distortion=None, planar_depth=None,
+                                 flow_means3D=None, flow_poses=None, grads_flow=None, flows=None):
     """Backward of the V views rendered by rasterize_views_raw: every view's blend backward on its stream, then ONE
     per-Gaussian chain-rule kernel that sums over the views (mgs_backward_views).  Returns the 9-tuple of
     rasterize_gaussians_backward_raw holding the SUMS over the views (dL_dmeans2D: `means2D_per_view` [V,P,3] when given,
@@ -1207,7 +1289,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho.
     `fisheye`: as given to the forward (by default the views' `fisheye` attributes); with a fisheye view the call is
     mgs_backward_views_fisheye.  `distortion`: likewise, mgs_backward_views_distorted with a distorted view.  `planar_depth`:
-    as given to the forward (mgs_backward_views_planar)."""
+    as given to the forward (mgs_backward_views_planar).  `flow_means3D` and `flow_poses`: as given to the forward, with
+    `flows` (per view [3,H,W]) the flow planes it returned and `grads_flow` (per view [3,H,W] or [2,H,W], or None) their
+    cotangents (C ABI mgs_backward_views_flow); the return value then gains, last, dL_dflow_means3D [P,3]."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1217,6 +1301,9 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
     V = len(views)
     pln = _planar_flag(views, planar_depth, grads_normal is not None)
+    _check_flow(flow_means3D, grads_normal is not None, pln, depth_mask)
+    if flow_means3D is not None and flows is None:
+        raise ValueError("flow cotangents need the forward's flow planes (flows)")
     oarr = _ortho_flags(views, ortho)
     farr = _fisheye_array(views, fisheye)
     dcarr = _distortion_array(views, distortion)
@@ -1254,6 +1341,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         keep = [dscale, sscale]
         marr = _median_array(grads_median, median_ids, V, dev, keep)
         narr = _normal_array(grads_normal, normals, V, dev, keep)
+        flarr = _flow_array(views, flow_means3D, flow_poses, P, dev, keep, flows, grads_flow)
+        dL_dflow = torch.empty((P, 3), **opts) if flarr is not None else None
         for v, s in enumerate(views):
             w = arr[v]
             if darr is not None:
@@ -1264,7 +1353,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                 keep.append(ga)
             keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
                                        grads_feature[v] if (F and grads_feature is not None) else None,
-                                       grads_depth[v] if grads_depth is not None else None, narr is not None or pln))
+                                       grads_depth[v] if grads_depth is not None else None,
+                                       narr is not None or pln or flarr is not None))
             w.dL_dmean2D = _ptr(m2d) if shared else _ptr(m2d[v])
             w.stream = streams[v].cuda_stream
             if cot_scale is not None:
@@ -1281,7 +1371,11 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if pln:
+            if flarr is not None:
+                _b.check(L.mgs_backward_views_flow(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
+                                                   oarr, farr, dcarr, int(pln), flarr, _ptr(flow_means3D), _ptr(dL_dflow), *rest),
+                         "mgs_backward_views_flow")
+            elif pln:
                 _b.check(L.mgs_backward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
                                                      oarr, farr, dcarr, 1, *rest), "mgs_backward_views_planar")
             elif dcarr is not None:
@@ -1317,7 +1411,8 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
             if stages == 1:
                 after_blend()
     grads = (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
-    return grads + (cam,) if cam is not None else grads
+    grads = grads + (cam,) if cam is not None else grads
+    return grads + (dL_dflow,) if dL_dflow is not None else grads
 
 
 def _median_array(grads, ids, V, dev, keep):
@@ -1452,9 +1547,13 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry.  A cloud's
     optional "fisheye" (V_b entries, each None or parameters; by default its views' `fisheye` attributes) marks its fisheye
     views (C ABI mgs_forward_clouds_fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
-    mgs_forward_clouds_distorted)."""
+    mgs_forward_clouds_distorted).  A cloud's optional "flow_means3D" [P,3] (its next-frame means) and "flow_poses" (as
+    rasterize_views_raw takes them) append, last, its views' flow planes [3,H,W] (out_buffers[7] when given; C ABI
+    mgs_forward_clouds_flow)."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, return_normal)
+    for c in clouds:
+        _check_flow(c.get("flow_means3D"), return_normal, pln, c.get("depth_mask"))
     dev = clouds[0]["means3D"].device
     if not clouds[0]["means3D"].is_cuda:
         raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
@@ -1489,6 +1588,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         narr = (_b.ViewNormal * V)() if return_normal else None
         status = _status_slots(V)
         keep, outs = [], []
+        flarr, cfarr = _clouds_flow(clouds, pc, offsets, dev, keep)
         for b, (c, d) in enumerate(zip(clouds, pc)):
             k = carr[b]
             k.P = d["P"]
@@ -1506,7 +1606,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                     _fill_ssim(sarr[g], c["ssim"], v)
                 o, kp = _forward_view(L, arr[g], s, v, dev, d["P"], F, cap, include_feature, return_depth, c.get("out_buffers"),
                                       c.get("loss_heads"), aarr[g] if return_alpha else None, marr[g] if return_median else None,
-                                      narr[g] if return_normal else None, quads=pln)
+                                      narr[g] if return_normal else None, quads=pln,
+                                      wf=flarr[g] if c.get("flow_means3D") is not None else None)
                 arr[g].status = status.data_ptr() + 8 * g
                 arr[g].stream = streams[g].cuda_stream
                 keep.append(kp)
@@ -1516,7 +1617,11 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
         oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
-        if pln:
+        if flarr is not None:
+            _b.check(L.mgs_forward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
+                                               _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
+                                               dcarr, int(pln), flarr, cfarr, *rest), "mgs_forward_clouds_flow")
+        elif pln:
             _b.check(L.mgs_forward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
                                                  dcarr, 1, *rest), "mgs_forward_clouds_planar")
@@ -1558,6 +1663,31 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         pending = not capturing and all(c.get("capacities") is None for c in clouds)
         _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
     return outs, streams
+
+
+def _clouds_flow(clouds, pc, offsets, dev, keep, backward=False):
+    """(ViewFlow array of every view of the call, CloudFlow array) for clouds with "flow_means3D", or (None, None) without
+    any.  The backward reads each cloud's forward planes "flow" and cotangents "grad_flow" ([V_b,3 or 2,H,W]) and allocates
+    its "dL_dflow_means3D" into pc[b]."""
+    if all(c.get("flow_means3D") is None for c in clouds):
+        return None, None
+    arr, carr = (_b.ViewFlow * offsets[-1])(), (_b.CloudFlow * len(clouds))()
+    for b, (c, d) in enumerate(zip(clouds, pc)):
+        fm = c.get("flow_means3D")
+        if fm is None:
+            continue
+        fm = _prep(fm.detach(), dev)
+        keep.append(fm)
+        planes = c.get("flow") if backward else None
+        grads = c.get("grad_flow") if backward else None
+        one = _flow_array(c["views"], fm, c.get("flow_poses"), d["P"], dev, keep, planes, grads)
+        for v in range(len(c["views"])):
+            ctypes.memmove(ctypes.addressof(arr[offsets[b] + v]), ctypes.addressof(one[v]), ctypes.sizeof(_b.ViewFlow))
+        carr[b].means3D = _ptr(fm)
+        if backward:
+            d["dL_dflow_means3D"] = torch.empty((d["P"], 3), dtype=torch.float32, device=dev)
+            carr[b].dL_dmeans3D = _ptr(d["dL_dflow_means3D"])
+    return arr, carr
 
 
 def _clouds_ortho(clouds):
@@ -1610,9 +1740,15 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
     mgs_backward_clouds_normal).  Clouds with an orthographic view (see rasterize_clouds_raw) make the call
     mgs_backward_clouds_ortho, clouds with a fisheye view mgs_backward_clouds_fisheye, and clouds with a distorted view
-    mgs_backward_clouds_distorted."""
+    mgs_backward_clouds_distorted.  A cloud rendered with "flow_means3D" (and "flow_poses") also takes "flow" [V_b,3,H,W],
+    the planes its forward returned, and "grad_flow" [V_b,2 or 3,H,W], their cotangent (C ABI mgs_backward_clouds_flow);
+    its dict then holds "dL_dflow_means3D" [P,3]."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, any(c.get("grad_normal") is not None for c in clouds))
+    for c in clouds:
+        _check_flow(c.get("flow_means3D"), c.get("grad_normal") is not None, pln, c.get("depth_mask"))
+        if c.get("flow_means3D") is not None and c.get("flow") is None:
+            raise ValueError("flow cotangents need the forward's flow planes (\"flow\")")
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
     F, M, B = pc[0]["F"], pc[0]["M"], len(clouds)
@@ -1639,6 +1775,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             gn = [c["grad_normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
             pl = [c["normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
             narr = _normal_array(gn, pl, V, dev, keep)
+        flarr, cfarr = _clouds_flow(clouds, pc, offsets, dev, keep, backward=True)
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
             has_sr = _nonempty(d["scales"])
@@ -1650,6 +1787,8 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                       dL_dcolors=torch.empty((P, 3), **opts) if _nonempty(d["colors"]) else None,
                       dL_dcov3D=torch.empty((P, 6), **opts) if _nonempty(d["cov3D_precomp"]) else None,
                       dL_dfeature=torch.empty((P, F), **opts) if (F and c.get("want_feature", True)) else None)
+            if "dL_dflow_means3D" in d:
+                gr["dL_dflow_means3D"] = d["dL_dflow_means3D"]
             grads.append(gr)
             k = carr[b]
             k.P = P
@@ -1671,7 +1810,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 keep.append(_backward_view(L, w, s, outs[b][v], dev, P, c["grad_color"][v],
                                            c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
                                            c["grad_depth"][v] if c.get("grad_depth") is not None else None,
-                                           c.get("grad_normal") is not None or pln))
+                                           c.get("grad_normal") is not None or pln or c.get("flow_means3D") is not None))
                 w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
                 w.stream = streams[g].cuda_stream
                 if c.get("grad_alpha") is not None:
@@ -1693,7 +1832,12 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
-        if pln:
+        if flarr is not None:
+            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+            _b.check(L.mgs_backward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
+                                                marr, narr, oarr, farr, dcarr, int(pln), flarr, cfarr, *rest),
+                     "mgs_backward_clouds_flow")
+        elif pln:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
                                                   marr, narr, oarr, farr, dcarr, 1, *rest), "mgs_backward_clouds_planar")
