@@ -1325,6 +1325,45 @@ int mgs_field_query_backward(
 	int debug,
 	void* stream);
 
+/*
+ * Point visibility (no reference counterpart): where Q 3D points land in each view, and how much of the cloud lies between
+ * the camera and each point, with the blend's own tile lists, depth order, thresholds and early stop.  For view v and a
+ * point x, with the expressions the projection and the forward blend already use:
+ *   - Projection: (u, v) is the screen position of x under the view's model (pinhole and orthographic through projmatrix and
+ *     ndc2pix, fisheye and distorted views through their lens maps: the map the projection applies to a Gaussian's mean,
+ *     the same device function as the flow plane's m), d = t.z its view-space depth.  Pixel centres are at integers.
+ *   - in_view: x passes that map's cull (t.z > NEAR_Z; fisheye theta <= theta_max; distorted r2 <= r_max^2 and det Dd > 0)
+ *     and -0.5 <= u < W - 0.5, -0.5 <= v < H - 0.5.
+ *   - Candidates: the instances of the 16x16 tile holding pixel (floor(u + 0.5), floor(v + 0.5)), in the tile list's order
+ *     (depth, then the stable sort's order), restricted to instances with depth z_i < d (strict): a prefix of the list.
+ *   - transmittance: T = prod (1 - alpha_i) over the candidates, alpha_i at the continuous (u, v) with the forward's
+ *     expression min(0.99, o exp(power)) (o the compensated opacity with antialiasing = 1), a candidate skipped where
+ *     power > 0 or alpha < 1/255, accumulated in list order with the forward's stop: the factor that would take T below 1e-4
+ *     is not applied, and the product ends there.
+ *   - Outside the view (in_view false) T = 1.  uv and depth are written wherever the cull passes, NaN where it fails.
+ * Hence at a pixel centre with d behind every Gaussian, T is that pixel's final_T bit for bit (the 8x4 block lists drop only
+ * pairs with alpha < 1/255 at every pixel centre of the block, which contribute nothing); a point in front of every Gaussian
+ * has T = 1; along a ray T does not increase with d.  The outputs are not differentiable.
+ * Arguments are those of mgs_lift_views_distorted with the map arguments replaced by the points and the outputs:
+ *   - points [Q,3]; out_uv [V,Q,2], out_depth [V,Q], out_in_view [V,Q] (uint8 0/1), each NULL to skip it; out_T [V,Q].
+ *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
+ *     (sized as for mgs_forward_views), binning_capacity, status and stream as for the lift, and blend_scratch, the point
+ *     scratch of mgs_visibility_scratch_bytes(Q, width, height) bytes (contents irrelevant on entry).  Every other field is
+ *     ignored.  The view's state afterwards holds its projection and binning; the blend state is not written.
+ *   - Nothing allocates or blocks: a call can be captured in a CUDA graph.  Q = 0 returns 0 and enqueues nothing.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0, Q < 0,
+ * points NULL with Q > 0, out_T NULL, a view without its state buffers, blend_scratch, matrices or radii, the camera-model
+ * errors of the _distorted calls, and the Gaussian-argument errors of mgs_lift_views.
+ */
+size_t mgs_visibility_scratch_bytes(int Q, int width, int height);
+int mgs_visibility_views(
+	int V, const mgs_view* views, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int Q, const float* points,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_uv, float* out_depth, uint8_t* out_in_view, float* out_T, int debug, void* join_stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

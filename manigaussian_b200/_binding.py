@@ -237,6 +237,15 @@ def lib():
     L.mgs_lift_views_distorted.restype = C.c_int
     L.mgs_lift_views_distorted.argtypes = L.mgs_lift_views_fisheye.argtypes[:7] + [C.POINTER(ViewDistortion)] + \
         L.mgs_lift_views_fisheye.argtypes[7:]
+    L.mgs_visibility_scratch_bytes.restype = C.c_size_t
+    L.mgs_visibility_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    L.mgs_visibility_views.restype = C.c_int
+    L.mgs_visibility_views.argtypes = [i, C.POINTER(View), i, C.POINTER(ViewIntrinsics),  # V views aa intr
+                                       C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
+                                       i, i, i, i, vp,                  # P D M Q points
+                                       vp, vp, vp,                      # means3D shs colors
+                                       vp, vp, f, vp, vp,               # opacities scales scale_modifier rotations cov3D_precomp
+                                       vp, vp, vp, vp, i, vp]           # out_uv out_depth out_in_view out_T debug join_stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -301,6 +310,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar",
     "mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow",
     "mgs_field_query", "mgs_field_query_backward",
+    "mgs_visibility_scratch_bytes", "mgs_visibility_views",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -21,7 +21,7 @@ OBJDIR = os.path.join(LIBDIR, "obj" + (("_" + os.environ["MGS_VARIANT"]) if os.e
 VARIANT = os.environ.get("MGS_VARIANT", "")
 EXTRA = os.environ.get("MGS_NVCC_DEFINES", "").split() if VARIANT else []
 LIB = os.path.join(LIBDIR, "libmgs_rasterizer%s.so" % (("_" + VARIANT) if VARIANT else ""))
-SOURCES = ["project.cu", "project_bwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "loss_heads.cu", "ssim.cu", "activate.cu", "normals.cu", "planar.cu", "flow.cu",
+SOURCES = ["project.cu", "project_bwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "loss_heads.cu", "ssim.cu", "activate.cu", "normals.cu", "planar.cu", "flow.cu", "visibility.cu",
            "lift.cu", "field.cu", "api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

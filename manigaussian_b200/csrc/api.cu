@@ -1447,6 +1447,111 @@ int mgs_lift_views_distorted(
 	return join_streams(V, views, join);
 }
 
+}  // extern "C"
+
+namespace mgs {
+// the point scratch of one view of mgs_visibility_views, carved from its blend_scratch
+struct VisScratch {
+	float4* pt; uint32_t* keys; uint32_t* keys_sorted; uint32_t* idx; uint32_t* idx_sorted; uint2* qranges; uint32_t* item_end;
+	char* sort_temp; size_t sort_bytes;
+	static VisScratch carve(char*& chunk, size_t Q, size_t T)
+	{
+		VisScratch s;
+		obtain(chunk, s.pt, Q);
+		obtain(chunk, s.keys, Q);
+		obtain(chunk, s.keys_sorted, Q);
+		obtain(chunk, s.idx, Q);
+		obtain(chunk, s.idx_sorted, Q);
+		obtain(chunk, s.qranges, T);
+		obtain(chunk, s.item_end, T);
+		s.sort_bytes = cached_temp_bytes(1, (int)Q);
+		obtain(chunk, s.sort_temp, s.sort_bytes);
+		return s;
+	}
+};
+}  // namespace mgs
+
+extern "C" {
+
+size_t mgs_visibility_scratch_bytes(int Q, int width, int height)
+{
+	return required([&](char*& p) { VisScratch::carve(p, (size_t)std::max(Q, 0), num_tiles(width, height)); });
+}
+
+int mgs_visibility_views(
+	int V, const mgs_view* views, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int Q, const float* points,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	float* out_uv, float* out_depth, uint8_t* out_in_view, float* out_T, int debug, void* join_stream)
+{
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
+	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (Q < 0) return fail(MGS_ERR_INVALID_ARG, "Q must be >= 0");
+	if (Q > 0 && !points) return fail(MGS_ERR_INVALID_ARG, "points are required with Q > 0");
+	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
+	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
+	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours (never read: they keep the projection the forward's)");
+	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
+	if (!out_T) return fail(MGS_ERR_INVALID_ARG, "out_T is required");
+	for (int v = 0; v < V; v++) {
+		const mgs_view& w = views[v];
+		if (!w.geometry_state || !w.binning_state || !w.image_state)
+			return fail(MGS_ERR_INVALID_ARG, "view: the three state buffers are required");
+		if (!w.blend_scratch) return fail(MGS_ERR_INVALID_ARG, "view: blend_scratch (mgs_visibility_scratch_bytes) is required");
+		if (!w.viewmatrix || !w.projmatrix || !w.radii) return fail(MGS_ERR_INVALID_ARG, "view: matrices and radii are required");
+		if (shs && !colors_precomp && !w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: cam_pos is required with SHs");
+		if (w.width <= 0 || w.height <= 0 || w.binning_capacity < 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size or capacity");
+	}
+	if (Q == 0) return 0;
+	const Cloud c{ P, D, M, 0, means3D, shs, colors_precomp, nullptr, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+		antialiasing };
+	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
+	int rc = fork_streams(V, views, join);
+	if (rc < 0) return rc;
+	// stage by stage across the views, as the lift: the point passes take the blend's place
+	for (int phase = 0; phase < 3; phase++) {
+		for (int v = 0; v < V; v++) {
+			const mgs_view& w = views[v];
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
+					distortion_of(distortion, v));
+			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
+			else {
+				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+				const ViewState s = carve_view(w, P);
+				char* sc = w.blend_scratch;
+				const VisScratch x = VisScratch::carve(sc, (size_t)Q, s.T);
+				const size_t o = (size_t)v * Q;
+				VisArgs a{};
+				a.Q = Q; a.W = w.width; a.H = w.height; a.grid_x = s.gx; a.num_tiles = (int)s.T;
+				a.cam = flow_cam(w, device_fov(intr, v), ortho_of(ortho, v), fisheye_of(fisheye, v), distortion_of(distortion, v),
+					w.viewmatrix, w.projmatrix);
+				a.points = points;
+				a.out_uv = out_uv ? out_uv + 2 * o : nullptr; a.out_depth = out_depth ? out_depth + o : nullptr;
+				a.out_in_view = out_in_view ? out_in_view + o : nullptr; a.out_T = out_T + o;
+				a.pt = x.pt; a.keys = x.keys; a.idx = x.idx; a.keys_sorted = x.keys_sorted; a.idx_sorted = x.idx_sorted;
+				a.qranges = x.qranges; a.item_end = x.item_end;
+				a.ranges = s.img.ranges; a.point_list = s.bin.point_list; a.depths = s.geom.depths; a.recs = s.bin.recs;
+				launch_visibility_points(a, st);
+				MGS_STAGE("visibility_points");
+				// tile ids up to num_tiles (the key of a point outside the view): stable, so a tile's points stay in id order
+				launch_tile_sort(x.sort_temp, x.sort_bytes, x.keys, x.keys_sorted, x.idx, x.idx_sorted, Q, higher_msb((uint32_t)s.T), st);
+				MGS_STAGE("visibility_sort");
+				launch_visibility_group(a, st);
+				MGS_STAGE("visibility_group");
+				launch_visibility_query(a, st);
+				MGS_STAGE("visibility_query");
+			}
+			if (rc < 0) return rc;
+		}
+	}
+	return join_streams(V, views, join);
+}
+
 int mgs_backward_views(
 	int V, const mgs_view* views,
 	int P, int D, int M, int F,

@@ -508,4 +508,33 @@ struct FlowBwdArgs {
 static_assert(sizeof(FlowBwdArgs) <= 4096, "kernel parameters are limited to 4 KB");
 void launch_flow_bwd(const FlowBwdArgs& a, cudaStream_t s);
 
+// visibility.cu: screen position, depth, in_view and transmittance of Q points in one view (include/mgs_rasterizer.h,
+// mgs_visibility_views), behind the view's projection and binning.  The points' tile keys are sorted between the points and
+// the group launches (launch_tile_sort over keys / idx into keys_sorted / idx_sorted).
+struct VisArgs {
+	int Q, W, H, grid_x, num_tiles;
+	FlowCam cam;                 // the view's own camera
+	const float* points;         // [Q,3]
+	float* out_uv;               // [Q,2] or NULL
+	float* out_depth;            // [Q] or NULL
+	uint8_t* out_in_view;        // [Q] or NULL
+	float* out_T;                // [Q]
+	// scratch
+	float4* pt;                  // [Q] {u, v, d, 0}
+	uint32_t* keys;              // [Q] tile of each point, num_tiles outside the view
+	uint32_t* idx;               // [Q] point ids
+	const uint32_t* keys_sorted; // [Q]
+	const uint32_t* idx_sorted;  // [Q]
+	uint2* qranges;              // [num_tiles] range of each tile's points in the sorted order
+	uint32_t* item_end;          // [num_tiles] inclusive scan of the per-tile warp counts
+	// the view's projection and binning
+	const uint2* ranges;
+	const uint32_t* point_list;
+	const float* depths;
+	const InstRec* recs;
+};
+void launch_visibility_points(const VisArgs& a, cudaStream_t s);
+void launch_visibility_group(const VisArgs& a, cudaStream_t s);
+void launch_visibility_query(const VisArgs& a, cudaStream_t s);
+
 }  // namespace mgs

@@ -25,7 +25,7 @@ from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
-                         field_query_raw, lift_views_raw,
+                         field_query_raw, lift_views_raw, visibility_views_raw,
                          rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
@@ -709,6 +709,53 @@ def lift_views(cameras, pts_xyz, rotations, scales, opacity, maps, view_ids=None
     lifted, weight = lift_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0, None, maps,
                                     antialiasing=aa)
     return {"lifted": lifted, "weight": weight}
+
+
+def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_ids=None, antialiasing=False):
+    """Project 3D points into every camera with occlusion (INTEGRATION.md §16).
+
+    cameras / view_ids as `lift_views` (a `cameras.CameraBatch`, including device field-of-view cameras, or a sequence of
+    GaussianRasterizationSettings of any of the four camera models, mixed).  points: [Q,3] fp32 on the cloud's device.  For
+    view v and point x:
+        uv[v, q]            the screen position of x in pixels (pixel centres at integers), through the camera model's own map;
+        depth[v, q]         its view-space depth t.z (uv and depth are NaN where x fails the model's cull, e.g. behind the camera);
+        in_view[v, q]       x passes the cull and lands in [-0.5, W - 0.5) x [-0.5, H - 0.5);
+        transmittance[v, q] prod (1 - alpha_i) over the Gaussians of x's 16x16 tile that lie in front of it (depth < d), in the
+                            blend's order, with the blend's alpha at the continuous uv, its 1/255 cut and its 1e-4 stop; 1 where
+                            x is not in view.
+    At a pixel centre behind the scene the transmittance is the render's final_T (1 - alpha) bit for bit.  Inputs that require
+    grad are detached; the outputs are not differentiable.  Returns {"uv": [V,Q,2], "depth": [V,Q], "in_view": [V,Q] bool,
+    "transmittance": [V,Q]}; raises ValueError on a shape, dtype or device mismatch."""
+    device = pts_xyz.device
+    if isinstance(cameras, CameraBatch):
+        ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
+        bg = _background((0.0, 0.0, 0.0), device)
+        views = tuple(cameras.settings(i, bg, 0, False) for i in ids)
+    else:
+        views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+    if not views:
+        raise ValueError("point_visibility needs at least one view")
+    aa = bool(antialiasing) or any(bool(getattr(s, "antialiasing", False)) for s in views)
+    P = pts_xyz.shape[0] if (torch.is_tensor(pts_xyz) and pts_xyz.dim() == 2) else -1
+    inputs = (("pts_xyz", pts_xyz, (3,)), ("rotations", rotations, (4,)), ("scales", scales, (3,)), ("opacity", opacity, None))
+    for name, t, tail in inputs:
+        if not torch.is_tensor(t):
+            raise ValueError(f"{name}: expected a tensor")
+        shape_ok = tuple(t.shape) in ((P, 1), (P,)) if tail is None else tuple(t.shape) == (P,) + tail
+        if P <= 0 or not shape_ok:
+            raise ValueError(f"{name}: expected [{P},{'1' if tail is None else tail[0]}], got {tuple(t.shape)}")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name}: expected float32, got {t.dtype}")
+    if not torch.is_tensor(points) or points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"points: expected [Q,3], got {tuple(points.shape) if torch.is_tensor(points) else type(points)}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"points: expected float32, got {points.dtype}")
+    for name, t in [(n, x) for n, x, _ in inputs] + [("points", points)]:
+        if t.device != device or not t.is_cuda:
+            raise ValueError(f"{name}: expected a CUDA tensor on {device}, got {t.device}")
+    uv, depth, in_view, T = visibility_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0,
+                                                 None, points.detach(), antialiasing=aa)
+    return {"uv": uv, "depth": depth, "in_view": in_view.bool(), "transmittance": T}
 
 
 class _QueryField(torch.autograd.Function):

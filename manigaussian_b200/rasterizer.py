@@ -1120,6 +1120,82 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
     return lifted, weight
 
 
+def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, points, antialiasing=False,
+                         tan_fov=None, debug=False, ortho=None, fisheye=None, distortion=None):
+    """Project Q points into every view with occlusion (C ABI mgs_visibility_views): per view and point the screen position
+    uv [V,Q,2] (pixel centres at integers), the view-space depth [V,Q], in_view [V,Q] (uint8) and the transmittance [V,Q] the
+    cloud leaves in front of the point, with the blend's own tile lists, depth order, thresholds and early stop.  `points`
+    [Q,3] fp32 on the cloud's device.  `views`, `antialiasing`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in
+    lift_views_raw; the binning state is sized from the same capacity table, so a steady-state call reads nothing back to the
+    host and can be captured in a CUDA graph.  Returns (uv, depth, in_view, T); none is differentiable."""
+    L = _b.lib()
+    dev = means3D.device
+    if not means3D.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    P = means3D.size(0)
+    if P == 0:
+        raise RuntimeError("visibility_views_raw needs at least one Gaussian")
+    means3D, opacity, scales, rotations, cov3D_precomp, points = (
+        _prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp, points))
+    V, Q = len(views), int(points.shape[0])
+    oarr = _ortho_flags(views, ortho)
+    farr = _fisheye_array(views, fisheye)
+    dcarr = _distortion_array(views, distortion)
+    colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
+    main = torch.cuda.current_stream(dev)
+    streams = _view_streams(dev, V) if V > 1 else [main]
+    di = dev.index if dev.index is not None else torch.cuda.current_device()
+    keys = [(di, P, int(s.image_width), int(s.image_height), v) for v, s in enumerate(views)]
+    capturing = torch.cuda.is_current_stream_capturing()
+    uv = torch.empty((V, Q, 2), dtype=torch.float32, device=dev)
+    depth = torch.empty((V, Q), dtype=torch.float32, device=dev)
+    in_view = torch.empty((V, Q), dtype=torch.uint8, device=dev)
+    T = torch.empty((V, Q), dtype=torch.float32, device=dev)
+    if Q == 0:
+        return uv, depth, in_view, T
+    with torch.cuda.device(dev):
+        if not capturing:
+            _poll_status()
+        if any(k not in _CAPACITY for k in keys):
+            if capturing:
+                raise RuntimeError("query the views once before capturing them in a CUDA graph (the binning capacity is learned "
+                                   "from an eager call)")
+            _calibrate(L, views, keys, dev, P, 0, 0, means3D, None, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                       debug, oarr, farr, dcarr)
+        arr = (_b.View * V)()
+        status = _status_slots(V)
+        keep, outs = [colors], []
+        for v, s in enumerate(views):
+            H, W = int(s.image_height), int(s.image_width)
+            gbytes, ibytes, _ = _state_sizes(L, P, W, H)
+            cap = _CAPACITY[keys[v]]
+            geom = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+            img = torch.empty(ibytes, dtype=torch.uint8, device=dev)
+            binb = torch.empty(int(L.mgs_binning_state_bytes(cap)), dtype=torch.uint8, device=dev)
+            scratch = torch.empty(int(L.mgs_visibility_scratch_bytes(Q, W, H)), dtype=torch.uint8, device=dev)
+            radii = torch.empty((P,), dtype=torch.int32, device=dev)
+            vm, pm = _prep(s.viewmatrix, dev), _prep(s.projmatrix, dev)
+            w = arr[v]
+            w.viewmatrix, w.projmatrix = _ptr(vm), _ptr(pm)
+            w.tan_fovx, w.tan_fovy, w.width, w.height = _host_tan(s.tanfovx), _host_tan(s.tanfovy), W, H
+            w.geometry_state, w.binning_state, w.image_state, w.binning_capacity = geom.data_ptr(), binb.data_ptr(), img.data_ptr(), cap
+            w.blend_scratch = scratch.data_ptr()
+            w.radii = radii.data_ptr()
+            w.status = status.data_ptr() + 8 * v
+            w.stream = streams[v].cuda_stream
+            keep += [geom, img, binb, scratch, radii, vm, pm]
+            outs.append(ViewOut((cap,)))
+        tf = _device_fov(views, tan_fov, dev)
+        keep.append(tf)
+        iarr = _intrinsics_array(tf, None) if tf is not None else None
+        _b.check(L.mgs_visibility_views(V, arr, int(bool(antialiasing)), iarr, oarr, farr, dcarr, P, 0, 0, Q, _ptr(points),
+                                        _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier),
+                                        _ptr(rotations), _ptr(cov3D_precomp), _ptr(uv), _ptr(depth), _ptr(in_view), _ptr(T),
+                                        int(bool(debug)), main.cuda_stream), "mgs_visibility_views")
+        _track_status(outs, keys, status, main, not capturing)
+    return uv, depth, in_view, T
+
+
 def _fill_depth_mask(wd, depth_mask, v, scale=None):
     """Fills view v's mgs_view_depth_mask `wd` from a `depth_mask` tuple of rasterize_views_raw (and, for the backward, the
     upstream gradients `scale` [V,2])."""
