@@ -218,6 +218,17 @@ static int higher_msb(uint32_t n)
 	return bits;
 }
 
+// launch view u of a per-Gaussian backward (ProjectBwdViewsArgs or ProjectBwdCloudsDistArgs) with lens l: bit u of its
+// model's mask and, for a fisheye or distorted view, its coefficients
+template <class Args>
+static void bwd_lens(Args& a, int u, const Lens& l)
+{
+	const uint16_t bit = (uint16_t)(1u << u);
+	if (l.model == MODEL_ORTHO) a.ortho |= bit;
+	if (l.model == MODEL_FISHEYE) { a.fisheye |= bit; a.fe_k[u] = l.fe_k; }
+	if (l.model == MODEL_DISTORTED) { a.distorted |= bit; a.dc_k[u] = l.dc_k; }
+}
+
 }  // namespace mgs
 
 using namespace mgs;
@@ -364,56 +375,51 @@ static ViewState carve_view(const mgs_view& w, int P)
 // the view's device {tan_fovx, tan_fovy} (intr: one entry per view, or NULL), or NULL for mgs_view.tan_fovx / tan_fovy
 static const float* device_fov(const mgs_view_intrinsics* intr, int v) { return intr ? intr[v].tan_fov : nullptr; }
 
-// view v's camera model (ortho: one flag per view, or NULL): 1 orthographic, 0 perspective
-static int ortho_of(const int* ortho, int v) { return ortho ? ortho[v] : 0; }
-static int check_ortho(const int* ortho, int V)
+// the views' camera models into lens[0 .. V) (ortho: one flag per view, or NULL; fisheye, distortion: one entry per view, or
+// NULL, an entry whose flag is 0 ignored).  Each model is checked over every view before the next, so a call with several
+// faults reports the same one whatever the views' order.
+static int view_lenses(const int* ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, int V, std::vector<Lens>& lens)
 {
-	for (int v = 0; ortho && v < V; v++)
+	lens.assign(V, Lens{});
+	for (int v = 0; ortho && v < V; v++) {
 		if (ortho[v] != 0 && ortho[v] != 1) return fail(MGS_ERR_INVALID_ARG, "ortho: every entry must be 0 (perspective) or 1 (orthographic)");
-	return 0;
-}
-
-// view v's fisheye parameters (fisheye: one entry per view, or NULL), or NULL for a pinhole or orthographic view
-static const mgs_view_fisheye* fisheye_of(const mgs_view_fisheye* fe, int v) { return fe && fe[v].fisheye ? fe + v : nullptr; }
-static int check_fisheye(const mgs_view_fisheye* fe, const int* ortho, int V)
-{
+		if (ortho[v]) lens[v].model = MODEL_ORTHO;
+	}
 	for (int v = 0; fe && v < V; v++) {
 		const mgs_view_fisheye& f = fe[v];
 		if (f.fisheye != 0 && f.fisheye != 1) return fail(MGS_ERR_INVALID_ARG, "fisheye: every flag must be 0 or 1");
 		if (!f.fisheye) continue;
-		if (ortho_of(ortho, v)) return fail(MGS_ERR_INVALID_ARG, "fisheye: a view cannot be both orthographic and fisheye");
+		if (lens[v].model == MODEL_ORTHO) return fail(MGS_ERR_INVALID_ARG, "fisheye: a view cannot be both orthographic and fisheye");
 		const float x[7] = { f.cx, f.cy, f.k1, f.k2, f.k3, f.k4, f.theta_max };
 		for (float xi : x)
 			if (!std::isfinite(xi)) return fail(MGS_ERR_INVALID_ARG, "fisheye: cx, cy, k1..k4 and theta_max must be finite");
 		if (!(f.theta_max > 0.f && f.theta_max <= 1.57079637f))  // (0, pi/2], pi/2 rounded to float
 			return fail(MGS_ERR_INVALID_ARG, "fisheye: theta_max must lie in (0, pi/2]");
+		Lens& l = lens[v];
+		l.model = MODEL_FISHEYE;
+		l.cx = f.cx; l.cy = f.cy; l.theta_max = f.theta_max; l.fe_k = FisheyeK{ f.k1, f.k2, f.k3, f.k4 };
 	}
-	return 0;
-}
-
-// view v's distortion parameters (dc: one entry per view, or NULL), or NULL for a view without lens distortion
-static const mgs_view_distortion* distortion_of(const mgs_view_distortion* dc, int v) { return dc && dc[v].distorted ? dc + v : nullptr; }
-static int check_distortion(const mgs_view_distortion* dc, const int* ortho, const mgs_view_fisheye* fe, int V)
-{
 	for (int v = 0; dc && v < V; v++) {
 		const mgs_view_distortion& d = dc[v];
 		if (d.distorted != 0 && d.distorted != 1) return fail(MGS_ERR_INVALID_ARG, "distortion: every flag must be 0 or 1");
 		if (!d.distorted) continue;
-		if (ortho_of(ortho, v) || fisheye_of(fe, v))
+		if (lens[v].model != MODEL_PINHOLE)
 			return fail(MGS_ERR_INVALID_ARG, "distortion: a distorted view cannot also be orthographic or fisheye");
 		const float x[10] = { d.cx, d.cy, d.k1, d.k2, d.p1, d.p2, d.k3, d.k4, d.k5, d.k6 };
 		for (float xi : x)
 			if (!std::isfinite(xi)) return fail(MGS_ERR_INVALID_ARG, "distortion: cx, cy and the coefficients must be finite");
 		if (!(d.r_max > 0.f)) return fail(MGS_ERR_INVALID_ARG, "distortion: r_max must be > 0 (+inf for no fold)");
+		Lens& l = lens[v];
+		l.model = MODEL_DISTORTED;
+		l.cx = d.cx; l.cy = d.cy; l.r2_max = d.r_max * d.r_max;  // +inf stays +inf
+		l.dc_k = DistK{ d.k1, d.k2, d.p1, d.p2, d.k3, d.k4, d.k5, d.k6 };
 	}
 	return 0;
 }
 
 // per-Gaussian projection, depth order and instance offsets; the instance count ends up in geom.point_offsets[P - 1].
-// tan_fov: the view's device field of view, or NULL; ortho: 1 for an orthographic view; fe: a fisheye view's parameters,
-// or NULL; dc: a distorted view's parameters, or NULL
-static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, int ortho, int debug,
-	const mgs_view_fisheye* fe = nullptr, const mgs_view_distortion* dc = nullptr)
+// tan_fov: the view's device field of view, or NULL; lens: its camera model
+static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_fov, const Lens& lens, int debug)
 {
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	const ViewState s = carve_view(w, c.P);
@@ -431,27 +437,14 @@ static int enqueue_project(const Cloud& c, const mgs_view& w, const float* tan_f
 	pa.iota = geom.iota;
 	pa.antialias = c.antialias;
 	pa.tan_fov = tan_fov;
-	pa.ortho = ortho;
-	if (fe) {
-		pa.fisheye = 1;
-		pa.fe_cx = fe->cx; pa.fe_cy = fe->cy; pa.fe_k = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 }; pa.fe_theta_max = fe->theta_max;
-	}
-	if (dc) {
-		pa.distorted = 1;
-		pa.dc_cx = dc->cx; pa.dc_cy = dc->cy;
-		pa.dc_k = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
-		pa.dc_r2_max = dc->r_max * dc->r_max;  // +inf stays +inf
-	}
+	pa.lens = lens;
 	{ StageTimer t_(ST_PROJECT_FWD, st); launch_project_fwd(pa, st); }
 	MGS_STAGE("project_fwd");
 	if (c.planar) {
 		// the view's planar-depth quads, where the normal plane keeps its quads (the _normal size queries)
 		PlanarFwdArgs la{};
 		la.P = c.P; la.means3D = c.means3D; la.cov3D = c.cov3D_precomp ? c.cov3D_precomp : geom.cov3D; la.viewmatrix = w.viewmatrix;
-		la.W = w.width; la.H = w.height; la.tan_fovx = w.tan_fovx; la.tan_fovy = w.tan_fovy; la.tan_fov = tan_fov;
-		la.model = dc ? 3 : fe ? 2 : ortho ? 1 : 0;
-		if (fe) la.fe_k = pa.fe_k;
-		if (dc) la.dc_k = pa.dc_k;
+		la.W = w.width; la.H = w.height; la.tan_fovx = w.tan_fovx; la.tan_fovy = w.tan_fovy; la.tan_fov = tan_fov; la.lens = lens;
 		la.radii = w.radii; la.means2D = geom.means2D; la.conic_opacity = geom.conic_opacity; la.quad = s.nrm;
 		launch_planar_fwd(la, st);
 		MGS_STAGE("planar_fwd");
@@ -800,34 +793,24 @@ static const mgs_view_normal* flow_blend_planes(const mgs_view_flow* fl, int V, 
 		if (flow_on(fl, v)) keep[v] = mgs_view_normal{ fl[v].out_flow, fl[v].dL_dpix_flow };
 	return keep.data();
 }
-// one end of view w's flow: its model, intrinsics and image size, with the pose (vm, pm)
-static FlowCam flow_cam(const mgs_view& w, const float* tan_fov, int ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc,
-	const float* vm, const float* pm)
+// view w's camera with the pose (vm, pm): its field of view, image size and lens
+static FlowCam flow_cam(const mgs_view& w, const float* tan_fov, const Lens& lens, const float* vm, const float* pm)
 {
-	FlowCam k{};
-	k.viewmatrix = vm; k.projmatrix = pm; k.tan_fov = tan_fov; k.tan_fovx = w.tan_fovx; k.tan_fovy = w.tan_fovy;
-	k.W = w.width; k.H = w.height;
-	k.model = dc ? 3 : fe ? 2 : ortho ? 1 : 0;
-	if (fe) { k.cx = fe->cx; k.cy = fe->cy; k.theta_max = fe->theta_max; k.fe_k = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 }; }
-	if (dc) {
-		k.cx = dc->cx; k.cy = dc->cy; k.r2_max = dc->r_max * dc->r_max;  // +inf stays +inf
-		k.dc_k = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
-	}
-	return k;
+	return FlowCam{ vm, pm, tan_fov, w.tan_fovx, w.tan_fovy, w.width, w.height, lens };
 }
 static const float* next_vm(const mgs_view_flow& f, const mgs_view& w) { return f.next_viewmatrix ? f.next_viewmatrix : w.viewmatrix; }
 static const float* next_pm(const mgs_view_flow& f, const mgs_view& w) { return f.next_viewmatrix ? f.next_projmatrix : w.projmatrix; }
 
 // the view's flow quads {dx, dy, 0, 0}, behind its projection on its stream (fl nullable), in the normal plane's quad slot
 static int enqueue_flow_fwd(const Cloud& c, const mgs_view& w, const mgs_view_flow* fl, const float* next_means, const float* tan_fov,
-	int ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, int debug)
+	const Lens& lens, int debug)
 {
 	if (!fl || !fl->out_flow) return 0;
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
 	FlowFwdArgs a{};
 	a.P = c.P; a.means3D = c.means3D; a.next_means3D = next_means;
-	a.cur = flow_cam(w, tan_fov, ortho, fe, dc, w.viewmatrix, w.projmatrix);
-	a.next = flow_cam(w, tan_fov, ortho, fe, dc, next_vm(*fl, w), next_pm(*fl, w));
+	a.cur = flow_cam(w, tan_fov, lens, w.viewmatrix, w.projmatrix);
+	a.next = flow_cam(w, tan_fov, lens, next_vm(*fl, w), next_pm(*fl, w));
 	a.radii = w.radii; a.quad = carve_view(w, c.P).nrm;
 	launch_flow_fwd(a, st);
 	MGS_STAGE("flow_fwd");
@@ -840,8 +823,8 @@ static int enqueue_flow_fwd(const Cloud& c, const mgs_view& w, const mgs_view_fl
 // into the camera outputs with `accumulate` (the per-Gaussian stage's reduce then adds to them).  Returns whether it enqueued
 // that reduce.
 static int enqueue_flow_bwd(const Cloud& c, const mgs_view* views, const mgs_view_flow* fl, const float* next_means, float* dL_dnext,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const int* ortho, const mgs_view_fisheye* fe,
-	const mgs_view_distortion* dc, int v0, int n, int accumulate_next, int accumulate_cam, int debug, cudaStream_t st, bool& reduced)
+	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const Lens* lens, int v0, int n, int accumulate_next,
+	int accumulate_cam, int debug, cudaStream_t st, bool& reduced)
 {
 	reduced = false;
 	FlowBwdArgs a{};
@@ -857,7 +840,7 @@ static int enqueue_flow_bwd(const Cloud& c, const mgs_view* views, const mgs_vie
 		b.radii = w.radii; b.gb = s.gb;
 		if (flow_on(fl, v) && fl[v].dL_dpix_flow) {
 			b.gn = reinterpret_cast<const float4*>(s.gn);
-			b.cam = flow_cam(w, tf, ortho_of(ortho, v), fisheye_of(fe, v), distortion_of(dc, v), next_vm(fl[v], w), next_pm(fl[v], w));
+			b.cam = flow_cam(w, tf, lens[v], next_vm(fl[v], w), next_pm(fl[v], w));
 			b.own_camera = fl[v].next_viewmatrix ? 0 : 1;
 		}
 		ProjectBwdIntr ki{};
@@ -870,27 +853,13 @@ static int enqueue_flow_bwd(const Cloud& c, const mgs_view* views, const mgs_vie
 	return 0;
 }
 
-// launch view u of a backward: a fisheye view sets bit u of the mask and its coefficients
-static void set_fisheye(const mgs_view_fisheye* fe, int u, uint16_t& mask, FisheyeK* k)
-{
-	if (!fe) return;
-	mask |= (uint16_t)(1u << u);
-	k[u] = FisheyeK{ fe->k1, fe->k2, fe->k3, fe->k4 };
-}
-// launch view u of a backward: a distorted view sets bit u of the mask and its coefficients
-static void set_distortion(const mgs_view_distortion* dc, int u, uint16_t& mask, DistK* k)
-{
-	if (!dc) return;
-	mask |= (uint16_t)(1u << u);
-	k[u] = DistK{ dc->k1, dc->k2, dc->p1, dc->p2, dc->k3, dc->k4, dc->k5, dc->k6 };
-}
-
 // stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
 // `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
-// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL.
+// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL;
+// lens: V entries.
 static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
 	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
-	const mgs_view_normal* nm, const int* ortho, const mgs_view_fisheye* fe, const mgs_view_distortion* dc, const Cloud& c, float* dL_dmean3D,
+	const mgs_view_normal* nm, const Lens* lens, const Cloud& c, float* dL_dmean3D,
 	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
 	int accumulate, int stages, int debug, cudaStream_t join, const mgs_view_flow* fl = nullptr, const float* flow_means3D = nullptr,
 	float* dL_dflow = nullptr)
@@ -942,16 +911,14 @@ static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* al
 		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
 		bool flow_reduced = false;  // the flow's camera terms already hold the camera outputs
 		if (flow_bwd) {
-			const int rc = enqueue_flow_bwd(c, views, fl, flow_means3D, dL_dflow, cam, intr, ortho, fe, dc, v0, pb.V,
+			const int rc = enqueue_flow_bwd(c, views, fl, flow_means3D, dL_dflow, cam, intr, lens, v0, pb.V,
 				(accumulate || v0 > 0) ? 1 : 0, accumulate ? 1 : 0, debug, st, flow_reduced);
 			if (rc < 0) return rc;
 		}
 		CamReduceArgs cr{};
 		cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
 		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
-		for (int u = 0; u < pb.V; u++) pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << u);
-		for (int u = 0; u < pb.V; u++) set_fisheye(fisheye_of(fe, v0 + u), u, pb.fisheye, pb.fe_k);
-		for (int u = 0; u < pb.V; u++) set_distortion(distortion_of(dc, v0 + u), u, pb.distorted, pb.dc_k);
+		for (int u = 0; u < pb.V; u++) bwd_lens(pb, u, lens[v0 + u]);
 		for (int u = 0; u < pb.V; u++) planar_view(c, views[v0 + u], pb.pl_g[u], pb.pl_q[u], pb.pl_mean[u]);
 		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
 		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
@@ -975,7 +942,7 @@ static int project_single_view(const Cloud& c, mgs_view& w, mgs_alloc_fn geometr
 	w.geometry_state = geometry_alloc(geometry_user, mgs_geometry_state_bytes(c.P));
 	w.image_state = image_alloc(image_user, mgs_image_state_bytes(w.width, w.height));
 	if (!w.geometry_state || !w.image_state) return fail(MGS_ERR_ALLOC, "state allocation failed");
-	int rc = enqueue_project(c, w, nullptr, 0, debug);
+	int rc = enqueue_project(c, w, nullptr, Lens{}, debug);
 	if (rc < 0) return rc;
 	MGS_CUDA(cudaMemcpyAsync(host_count, carve_view(w, c.P).geom.point_offsets + c.P - 1, sizeof(int), cudaMemcpyDeviceToHost,
 		reinterpret_cast<cudaStream_t>(w.stream)));
@@ -1131,7 +1098,8 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
+	const Lens pinhole{};
+	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &pinhole, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -1299,9 +1267,8 @@ int mgs_forward_views_flow(
 	if (check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0)
 		return MGS_ERR_INVALID_ARG;
-	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
 	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours");
@@ -1336,15 +1303,13 @@ int mgs_forward_views_flow(
 			if (rc < 0) return rc;
 		}
 		for (int v = 0; v < V; v++) {
-			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
-					distortion_of(distortion, v))
+			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), lens[v], debug)
 				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 					median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 			if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
 			if (rc == 0 && phase == 0)
-				rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, flow_means3D, device_fov(intr, v), ortho_of(ortho, v),
-					fisheye_of(fisheye, v), distortion_of(distortion, v), debug);
+				rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, flow_means3D, device_fov(intr, v), lens[v], debug);
 			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 			if (rc < 0) return rc;
 		}
@@ -1396,9 +1361,8 @@ int mgs_lift_views_distorted(
 {
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
-	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (C < 0 || C > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, "map channel count must be in [0, " MGS_STR(MGS_MAX_FEATURE_CHANNELS) "]");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
@@ -1427,8 +1391,7 @@ int mgs_lift_views_distorted(
 	for (int phase = 0; phase < 3; phase++) {
 		for (int v = 0; v < V; v++) {
 			const mgs_view& w = views[v];
-			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
-					distortion_of(distortion, v));
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), lens[v], debug);
 			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
 			else {
 				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
@@ -1488,9 +1451,8 @@ int mgs_visibility_views(
 {
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
-	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (Q < 0) return fail(MGS_ERR_INVALID_ARG, "Q must be >= 0");
 	if (Q > 0 && !points) return fail(MGS_ERR_INVALID_ARG, "points are required with Q > 0");
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
@@ -1517,8 +1479,7 @@ int mgs_visibility_views(
 	for (int phase = 0; phase < 3; phase++) {
 		for (int v = 0; v < V; v++) {
 			const mgs_view& w = views[v];
-			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
-					distortion_of(distortion, v));
+			if (phase == 0) rc = enqueue_project(c, w, device_fov(intr, v), lens[v], debug);
 			else if (phase == 1) rc = enqueue_binning(c, w, false, debug);
 			else {
 				cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
@@ -1528,8 +1489,7 @@ int mgs_visibility_views(
 				const size_t o = (size_t)v * Q;
 				VisArgs a{};
 				a.Q = Q; a.W = w.width; a.H = w.height; a.grid_x = s.gx; a.num_tiles = (int)s.T;
-				a.cam = flow_cam(w, device_fov(intr, v), ortho_of(ortho, v), fisheye_of(fisheye, v), distortion_of(distortion, v),
-					w.viewmatrix, w.projmatrix);
+				a.cam = flow_cam(w, device_fov(intr, v), lens[v], w.viewmatrix, w.projmatrix);
 				a.points = points;
 				a.out_uv = out_uv ? out_uv + 2 * o : nullptr; a.out_depth = out_depth ? out_depth + o : nullptr;
 				a.out_in_view = out_in_view ? out_in_view + o : nullptr; a.out_T = out_T + o;
@@ -1756,9 +1716,8 @@ int mgs_backward_views_flow(
 		return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
-	if (check_ortho(ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, V) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
 	if (!means3D || !dL_dmean3D || !dL_dopacity) return fail(MGS_ERR_INVALID_ARG, "means3D, dL_dmean3D and dL_dopacity are required");
 	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
@@ -1774,7 +1733,7 @@ int mgs_backward_views_flow(
 	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
 	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
 		antialiasing, planar_depth };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, ortho, fisheye, distortion, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
+	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, lens.data(), c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream), flow, flow_means3D, dL_dflow_means3D);
 }
 
@@ -1890,9 +1849,8 @@ int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offs
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
-	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, view_offsets[B], lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
 	for (int b = 0; b < B; b++)
@@ -1926,15 +1884,13 @@ int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offs
 		for (int b = 0; b < B; b++) {
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), ortho_of(ortho, v), debug, fisheye_of(fisheye, v),
-					distortion_of(distortion, v))
+				rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), lens[v], debug)
 					: phase == 1 ? enqueue_binning(c, views[v], false, debug)
 					: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
 						median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
 				if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
 				if (rc == 0 && phase == 0)
-					rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, cloud_next(flow_clouds, b), device_fov(intr, v),
-						ortho_of(ortho, v), fisheye_of(fisheye, v), distortion_of(distortion, v), debug);
+					rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, cloud_next(flow_clouds, b), device_fov(intr, v), lens[v], debug);
 				if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
 				if (rc < 0) return rc;
 			}
@@ -2064,9 +2020,8 @@ int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_off
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;
-	if (check_ortho(ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_fisheye(fisheye, ortho, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_distortion(distortion, ortho, fisheye, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, view_offsets[B], lens) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
 	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
 	for (int b = 0; b < B; b++)
@@ -2127,7 +2082,7 @@ int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_off
 		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
 			bool red = false;
 			rc = enqueue_flow_bwd(c, views, flow, cloud_next(flow_clouds, b), flow_clouds ? flow_clouds[b].dL_dmeans3D : nullptr, cam, intr,
-				ortho, fisheye, distortion, v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS),
+				lens.data(), v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS),
 				(accumulate || v0 > view_offsets[b]) ? 1 : 0, accumulate ? 1 : 0, debug, st, red);
 			if (rc < 0) return rc;
 			flow_reduced |= red;
@@ -2170,9 +2125,7 @@ int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_off
 				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
 				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
 				camera_view(cam, intr, views[v0 + u], v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
-				pb.ortho |= (uint16_t)(ortho_of(ortho, v0 + u) << (nv + u));
-				set_fisheye(fisheye_of(fisheye, v0 + u), nv + u, pb.fisheye, pb.fe_k);
-				set_distortion(distortion_of(distortion, v0 + u), nv + u, pb.distorted, pb.dc_k);
+				bwd_lens(pb, nv + u, lens[v0 + u]);
 				planar_view(cloud_of(k, D, M, F, scale_modifier, antialiasing, planar_depth), views[v0 + u], pb.pl_g[nv + u], pb.pl_q[nv + u],
 					pb.pl_mean[nv + u]);
 			}

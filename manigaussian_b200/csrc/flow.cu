@@ -10,19 +10,20 @@
 // Kernels of their own rather than modes of the projection kernels: those compile to pinned instruction sequences (tile ids
 // and sort keys depend on them, DESIGN.md section 4).  Both ends come from one device function, so a next mean equal to the
 // current one under the view's own camera gives delta = 0 bit for bit.
-#include "flow_mean.cuh"
+#include "camera.cuh"
 
 namespace mgs {
 
 namespace {
 
-// the m' chain of one view: g the pixel cotangent of m' at p (valid), into dL/dp (added to gp) and, with cg, the camera terms
-// of the view (CAM_ALL_TERMS, laid out as the per-Gaussian backward's rows: dL/dvm, dL/dpm, dL/dcampos, dL/dtan_fov)
+// the m' chain of one view (the derivative of camera.cuh's screen_mean): g the pixel cotangent of m' at p (valid), into dL/dp
+// (added to gp) and, with cg, the camera terms of the view (CAM_ALL_TERMS, laid out as the per-Gaussian backward's rows:
+// dL/dvm, dL/dpm, dL/dcampos, dL/dtan_fov)
 template <bool CAM>
 __device__ __forceinline__ void flow_mean_bwd(const FlowCam& c, const float p[3], float gx, float gy, float gp[3], float* cg)
 {
 	const float* vm = c.viewmatrix;
-	if (c.model == 0 || c.model == 1) {
+	if (c.lens.model == MODEL_PINHOLE || c.lens.model == MODEL_ORTHO) {
 		// ndc = (P p).xy / ((P p).w + 1e-7), pixel = ((ndc + 1) S - 1) / 2: the ndc cotangent is the pixel one times S / 2
 		const float* pm = c.projmatrix;
 		const float dx = gx * (0.5f * c.W), dy = gy * (0.5f * c.H);
@@ -44,12 +45,12 @@ __device__ __forceinline__ void flow_mean_bwd(const FlowCam& c, const float p[3]
 	const float tx = vm[0] * p[0] + vm[4] * p[1] + vm[8] * p[2] + vm[12];
 	const float ty = vm[1] * p[0] + vm[5] * p[1] + vm[9] * p[2] + vm[13];
 	const float tz = vm[2] * p[0] + vm[6] * p[1] + vm[10] * p[2] + vm[14];
-	const float tanx = c.tan_fov ? c.tan_fov[0] : c.tan_fovx, tany = c.tan_fov ? c.tan_fov[1] : c.tan_fovy;
-	const float fx = c.W / (2.0f * tanx), fy = c.H / (2.0f * tany);
+	const ViewFov f = view_fov(c);
+	const float tanx = f.tanx, tany = f.tany, fx = f.fx, fy = f.fy;
 	float dt[3], ftx, fty;  // dL/dt; (u - cx, v - cy) for the field of view
-	if (c.model == 2) {
+	if (c.lens.model == MODEL_FISHEYE) {
 		// J = [[fx (a + c x^2), fx c x y, -fx x g], [fy c x y, fy (a + c y^2), -fy y g]] (fisheye.cuh)
-		const FisheyeRadial fr = fisheye_radial<false>(tx, ty, tz, c.fe_k);
+		const FisheyeRadial fr = fisheye_radial<false>(tx, ty, tz, c.lens.fe_k);
 		const float ex = fx * gx, ey = fy * gy, cxy = fr.c * tx * ty;
 		dt[0] = ex * (fr.a + fr.c * tx * tx) + ey * cxy;
 		dt[1] = ex * cxy + ey * (fr.a + fr.c * ty * ty);
@@ -58,7 +59,7 @@ __device__ __forceinline__ void flow_mean_bwd(const FlowCam& c, const float p[3]
 	} else {
 		// (u, v) = F (xd, yd) + c, d(xd, yd) / d(x, y) = Dd (symmetric), (x, y) = t.xy / t.z
 		const float iz = 1.0f / tz, x = tx * iz, y = ty * iz;
-		const DistTerms ds = distortion_terms<false>(x, y, c.dc_k);
+		const DistTerms ds = distortion_terms<false>(x, y, c.lens.dc_k);
 		const float ex = fx * gx, ey = fy * gy;
 		const float qx = ds.d00 * ex + ds.d01 * ey, qy = ds.d01 * ex + ds.d11 * ey;
 		dt[0] = qx * iz; dt[1] = qy * iz; dt[2] = -(qx * x + qy * y) * iz;
@@ -86,8 +87,8 @@ __global__ void __launch_bounds__(256) flow_fwd_kernel(FlowFwdArgs a)
 		const V3 p = { a.means3D[3 * (size_t)i], a.means3D[3 * (size_t)i + 1], a.means3D[3 * (size_t)i + 2] };
 		const V3 q = { a.next_means3D[3 * (size_t)i], a.next_means3D[3 * (size_t)i + 1], a.next_means3D[3 * (size_t)i + 2] };
 		float mx, my, nx, ny;
-		flow_mean(a.cur, p, mx, my);  // passes: the projection kept the Gaussian
-		if (flow_mean(a.next, q, nx, ny)) { dx = nx - mx; dy = ny - my; }
+		screen_mean(a.cur, p, mx, my);  // passes: the projection kept the Gaussian
+		if (screen_mean(a.next, q, nx, ny)) { dx = nx - mx; dy = ny - my; }
 	}
 	a.quad[i] = make_float4(dx, dy, 0.f, 0.f);
 }
@@ -116,7 +117,7 @@ __global__ void __launch_bounds__(FLOW_BWD_THREADS) flow_bwd_kernel(FlowBwdArgs 
 			// an invalid pair's delta is 0 whatever m and m' are: it receives nothing through either end
 			const V3 q = { p[0], p[1], p[2] };
 			float nx, ny;
-			if (flow_mean(w.cam, q, nx, ny)) {
+			if (screen_mean(w.cam, q, nx, ny)) {
 				const float4 g = w.gn[id];
 				// m path: -g onto the blend's screen-mean gradient, in its convention (ndc: pixels times W / 2, H / 2)
 				float* gb = w.gb + (size_t)id * GB_STRIDE;

@@ -11,6 +11,21 @@ namespace mgs {
 
 struct InstRec;
 
+// A view's camera model, beside its pose and field of view (include/mgs_rasterizer.h: the ortho flags, mgs_view_fisheye and
+// mgs_view_distortion).  Pinhole and orthographic views take their screen mean through the projection matrix (an
+// orthographic view's tan_fov holds its half extents); fisheye (Kannala-Brandt, fisheye.cuh) and distorted-pinhole (OpenCV,
+// distortion.cuh) views form it from (cx, cy) and their coefficients without it, and cull a mean past theta_max or r2_max.
+// camera.cuh holds the device maths of each model.
+constexpr int MODEL_PINHOLE = 0, MODEL_ORTHO = 1, MODEL_FISHEYE = 2, MODEL_DISTORTED = 3;
+struct Lens {
+	int model;                   // MODEL_*
+	float cx, cy;                // fisheye or distorted principal point
+	float theta_max;             // fisheye cull
+	float r2_max;                // distorted cull: r_max^2
+	FisheyeK fe_k;
+	DistK dc_k;
+};
+
 struct ProjectFwdArgs {
 	int P, D, M;
 	const float* means3D;
@@ -38,26 +53,13 @@ struct ProjectFwdArgs {
 	uint8_t* clamped;  // 3 bits per Gaussian
 	uint32_t* tiles_touched;
 	uint32_t* iota;    // identity permutation (values of the depth sort)
-	int antialias;     // 1: opacity compensation for the 0.3 px^2 low-pass (launcher picks the instantiation; last, so the
-	                   // other members keep their parameter offsets)
 	// device {tan_fovx, tan_fovy}, or NULL: tan_fov* and focal_* above.  Non-NULL picks the instantiation that reads it and
-	// forms the focal lengths as the host does (W / (2 tan_fovx)); behind antialias for the same reason.
+	// forms the focal lengths as the host does (W / (2 tan_fovx)).
 	const float* tan_fov;
-	// 1: an orthographic view (tan_fov* hold its half extents; picks the ORTHO instantiation); behind tan_fov for the same reason
-	int ortho;
-	// 1: a Kannala-Brandt fisheye view (picks the FISHEYE instantiation; projmatrix is not read): principal point, coefficients
-	// and the theta cull of include/mgs_rasterizer.h's mgs_view_fisheye.  Behind ortho for the same reason.
-	int fisheye;
-	float fe_cx, fe_cy;
-	FisheyeK fe_k;
-	float fe_theta_max;
-	// 1: an OpenCV distorted-pinhole view (picks the DISTORTED instantiation; projmatrix is not read): principal point,
-	// coefficients and the squared radius cull of include/mgs_rasterizer.h's mgs_view_distortion.  Behind the fisheye members
-	// for the same reason.
-	int distorted;
-	float dc_cx, dc_cy;
-	DistK dc_k;
-	float dc_r2_max;
+	int antialias;     // 1: opacity compensation for the 0.3 px^2 low-pass (picks the AA instantiation)
+	// the view's camera model (picks the MODEL instantiation).  It starts 4 bytes past an 8-byte boundary, as in FlowCam: the
+	// pairs the kernel reads together ((cx, cy) and the coefficients) then sit on 8-byte boundaries, and are loaded as such.
+	Lens lens;
 };
 
 // project_bwd.cu: per-Gaussian chain rule for up to MAX_BWD_VIEWS views in one launch
@@ -407,9 +409,7 @@ struct PlanarFwdArgs {
 	int W, H;
 	float tan_fovx, tan_fovy;    // host field of view (tan_fov NULL)
 	const float* tan_fov;        // device {tan_fovx, tan_fovy}, or NULL
-	int model;                   // 0 pinhole, 1 orthographic, 2 fisheye, 3 distorted pinhole
-	FisheyeK fe_k;
-	DistK dc_k;
+	Lens lens;
 	const int* radii;
 	const float2* means2D;
 	const float4* conic_opacity;
@@ -463,19 +463,14 @@ cudaError_t field_backward(char* state, char* pair_state, int Q, int P, int C, c
 	float* dL_dpoints, float* dL_dmeans, float* dL_dscales, float* dL_drot, float* dL_dopac, float* dL_dfeat, cudaStream_t st);
 
 // flow.cu: the flow plane's per-Gaussian quads {dx, dy, 0, 0} (include/mgs_rasterizer.h, flow plane) and their backward.
-// FlowCam: the map of one end of a view's flow, the view's model, intrinsics and image size with the pose that end uses.
+// FlowCam: the map of one end of a view's flow, the view's pose, field of view and image size with its lens.
 struct FlowCam {
 	const float* viewmatrix;
 	const float* projmatrix;     // pinhole and orthographic only
 	const float* tan_fov;        // device {tan_fovx, tan_fovy}, or NULL for the host values
 	float tan_fovx, tan_fovy;
 	int W, H;
-	int model;                   // 0 pinhole, 1 orthographic, 2 fisheye, 3 distorted pinhole
-	float cx, cy;                // fisheye or distorted principal point
-	float theta_max;             // fisheye cull
-	float r2_max;                // distorted cull
-	FisheyeK fe_k;
-	DistK dc_k;
+	Lens lens;
 };
 struct FlowFwdArgs {
 	int P;

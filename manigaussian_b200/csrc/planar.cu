@@ -7,8 +7,7 @@
 // A kernel of its own rather than a mode of the projection kernels: those compile to pinned instruction sequences (tile ids
 // and sort keys depend on them, DESIGN.md section 4).  It reads the projection's record (mean, conic) and rebuilds t, J and
 // Sigma_c as the projection forms them.
-#include "mgs_common.cuh"
-#include "mgs_kernels.h"
+#include "camera.cuh"
 
 namespace mgs {
 
@@ -27,23 +26,17 @@ __global__ void __launch_bounds__(256) planar_fwd_kernel(PlanarFwdArgs a)
 	const float tx = Rv[0][0] * p[0] + Rv[0][1] * p[1] + Rv[0][2] * p[2] + vm[12];
 	const float ty = Rv[1][0] * p[0] + Rv[1][1] * p[1] + Rv[1][2] * p[2] + vm[13];
 	const float tz = Rv[2][0] * p[0] + Rv[2][1] * p[1] + Rv[2][2] * p[2] + vm[14];
-	const float tanx = a.tan_fov ? a.tan_fov[0] : a.tan_fovx, tany = a.tan_fov ? a.tan_fov[1] : a.tan_fovy;
-	const float fx = a.W / (2.0f * tanx), fy = a.H / (2.0f * tany);
+	const ViewFov f = view_fov(a);
+	const float tanx = f.tanx, tany = f.tany, fx = f.fx, fy = f.fy;
 	// J (2x3, pixels), as project.cu's cov2d_terms forms it for the view's model
 	float J[2][3];
-	if (a.model == 1) {
-		J[0][0] = fx; J[0][1] = 0.f; J[0][2] = 0.f;
-		J[1][0] = 0.f; J[1][1] = fy; J[1][2] = 0.f;
-	} else if (a.model == 2) {
-		const FisheyeRadial fr = fisheye_radial<false>(tx, ty, tz, a.fe_k);
-		const float cxy = fr.c * tx * ty;
-		J[0][0] = fx * (fr.a + fr.c * tx * tx); J[0][1] = fx * cxy; J[0][2] = -fx * tx * fr.g;
-		J[1][0] = fy * cxy; J[1][1] = fy * (fr.a + fr.c * ty * ty); J[1][2] = -fy * ty * fr.g;
-	} else if (a.model == 3) {
+	if (a.lens.model == MODEL_ORTHO) {
+		ortho_jacobian(fx, fy, J);
+	} else if (a.lens.model == MODEL_FISHEYE) {
+		fisheye_jacobian(fisheye_radial<false>(tx, ty, tz, a.lens.fe_k), tx, ty, fx, fy, J);
+	} else if (a.lens.model == MODEL_DISTORTED) {
 		const float iz = 1.0f / tz, x = tx * iz, y = ty * iz;
-		const DistTerms ds = distortion_terms<false>(x, y, a.dc_k);
-		J[0][0] = fx * ds.d00 * iz; J[0][1] = fx * ds.d01 * iz; J[0][2] = -fx * (ds.d00 * x + ds.d01 * y) * iz;
-		J[1][0] = fy * ds.d01 * iz; J[1][1] = fy * ds.d11 * iz; J[1][2] = -fy * (ds.d01 * x + ds.d11 * y) * iz;
+		distorted_jacobian(distortion_terms<false>(x, y, a.lens.dc_k), x, y, iz, fx, fy, J);
 	} else {
 		// the pinhole Jacobian at the frustum-clamped t.xy
 		const float limx = 1.3f * tanx, limy = 1.3f * tany;

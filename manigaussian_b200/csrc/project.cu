@@ -5,8 +5,7 @@
 //   visible  : checkFrustum (rasterizer_impl.cu:54-66)
 // The forward's expressions keep the reference's shapes (left-to-right sums of products, double-precision ndc2pix): tile
 // ids and sort keys must agree bit for bit, which requires nvcc to contract the same FMAs.
-#include "mgs_common.cuh"
-#include "mgs_kernels.h"
+#include "camera.cuh"
 
 namespace mgs {
 
@@ -38,12 +37,8 @@ struct Cov2DTerms {
 	float txtz, tytz;
 	M3 T, Vrk, W;
 };
-// Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196).
-// MODEL_ORTHO: the orthographic Jacobian J = [[fx, 0, 0], [0, fy, 0]] (fx, fy in pixels per view-space unit), with no frustum
-// clamp.  MODEL_FISHEYE: the Kannala-Brandt Jacobian from the radial terms fr of the unclamped t (fisheye.cuh), no clamp.
-// MODEL_DISTORTED: J = diag(fx, fy) Dd [[1/z, 0, -x/z], [0, 1/z, -y/z]] from the distortion terms ds of the unclamped
-// (x, y) = t.xy / t.z (distortion.cuh), no clamp.
-constexpr int MODEL_PINHOLE = 0, MODEL_ORTHO = 1, MODEL_FISHEYE = 2, MODEL_DISTORTED = 3;
+// Shared by the forward (forward.cu:75-107) and the backward recomputation (backward.cu:163-196).  The orthographic, fisheye
+// and distorted Jacobians are camera.cuh's, at the unclamped t; only the pinhole one clamps t to the frustum.
 template <int MODEL = MODEL_PINHOLE>
 __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, float fy, float tanx, float tany,
 	const float* cov3D, const float* vm, const FisheyeRadial* fr = nullptr, const DistTerms* ds = nullptr)
@@ -52,20 +47,17 @@ __device__ __forceinline__ Cov2DTerms cov2d_terms(const V3& mean, float fx, floa
 	V3 t = xform4x3(mean, vm);
 	M3 J;
 	float txtz = 0.f, tytz = 0.f;
-	if constexpr (MODEL == MODEL_ORTHO) {
-		J = m3(fx, 0.0f, 0.0f, 0.0f, fy, 0.0f, 0.f, 0.f, 0.f);
-	} else if constexpr (MODEL == MODEL_FISHEYE) {
-		const float cxy = fr->c * t.x * t.y;
-		J = m3(
-			fx * (fr->a + fr->c * t.x * t.x), fx * cxy, -fx * t.x * fr->g,
-			fy * cxy, fy * (fr->a + fr->c * t.y * t.y), -fy * t.y * fr->g,
-			0.f, 0.f, 0.f);
-	} else if constexpr (MODEL == MODEL_DISTORTED) {
-		const float iz = 1.0f / t.z, x = t.x * iz, y = t.y * iz;
-		J = m3(
-			fx * ds->d00 * iz, fx * ds->d01 * iz, -fx * (ds->d00 * x + ds->d01 * y) * iz,
-			fy * ds->d01 * iz, fy * ds->d11 * iz, -fy * (ds->d01 * x + ds->d11 * y) * iz,
-			0.f, 0.f, 0.f);
+	if constexpr (MODEL != MODEL_PINHOLE) {
+		float j[2][3];
+		if constexpr (MODEL == MODEL_ORTHO) {
+			ortho_jacobian(fx, fy, j);
+		} else if constexpr (MODEL == MODEL_FISHEYE) {
+			fisheye_jacobian(*fr, t.x, t.y, fx, fy, j);
+		} else {
+			const float iz = 1.0f / t.z;
+			distorted_jacobian(*ds, t.x * iz, t.y * iz, iz, fx, fy, j);
+		}
+		J = m3(j[0][0], j[0][1], j[0][2], j[1][0], j[1][1], j[1][2], 0.f, 0.f, 0.f);
 	} else {
 		const float limx = 1.3f * tanx;
 		const float limy = 1.3f * tany;
@@ -168,14 +160,14 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	if (p_view.z <= NEAR_Z) return;  // near cull only (auxiliary.h:154)
 	FisheyeRadial fr{};
 	if constexpr (MODEL == MODEL_FISHEYE) {
-		fr = fisheye_radial<false>(p_view.x, p_view.y, p_view.z, a.fe_k);
-		if (fr.theta > a.fe_theta_max) return;
+		fr = fisheye_radial<false>(p_view.x, p_view.y, p_view.z, a.lens.fe_k);
+		if (fisheye_culled(fr, a.lens.theta_max)) return;
 	}
 	DistTerms ds{};
 	if constexpr (MODEL == MODEL_DISTORTED) {
 		const float iz = 1.0f / p_view.z;
-		ds = distortion_terms<false>(p_view.x * iz, p_view.y * iz, a.dc_k);
-		if (ds.r2 > a.dc_r2_max || fmaf(-ds.d01, ds.d01, ds.d00 * ds.d11) <= 0.f) return;
+		ds = distortion_terms<false>(p_view.x * iz, p_view.y * iz, a.lens.dc_k);
+		if (distorted_culled(ds, a.lens.r2_max)) return;
 	}
 
 	const float* cov3D;
@@ -189,7 +181,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	float tanx = a.tan_fovx, tany = a.tan_fovy, fx = a.focal_x, fy = a.focal_y;
 	if constexpr (FOV) {
 		tanx = a.tan_fov[0]; tany = a.tan_fov[1];
-		fx = a.W / (2.0f * tanx); fy = a.H / (2.0f * tany);  // as api.cu forms focal_x / focal_y
+		fx = focal_length(a.W, tanx); fy = focal_length(a.H, tany);
 	}
 	Cov2DTerms ct = cov2d_terms<MODEL>(p_orig, fx, fy, tanx, tany, cov3D, a.viewmatrix, &fr, &ds);
 	M3 cov = mul(mul(transpose(ct.T), transpose(ct.Vrk)), ct.T);
@@ -208,14 +200,15 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(ProjectFwdArgs a)
 	float lambda1 = mid + sqrtf(max(0.1f, mid * mid - det));
 	float lambda2 = mid - sqrtf(max(0.1f, mid * mid - det));
 	float my_radius = ceilf(3.f * sqrtf(max(lambda1, lambda2)));
-	float px, py;
+	float2 pm;
 	if constexpr (MODEL == MODEL_FISHEYE) {
-		px = fx * fr.a * p_view.x + a.fe_cx; py = fy * fr.a * p_view.y + a.fe_cy;
+		pm = fisheye_mean(a.lens, fr, p_view.x, p_view.y, fx, fy);
 	} else if constexpr (MODEL == MODEL_DISTORTED) {
-		px = fx * ds.xd + a.dc_cx; py = fy * ds.yd + a.dc_cy;
+		pm = distorted_mean(a.lens, ds, fx, fy);
 	} else {
-		px = ndc2pix(p_proj_x, a.W); py = ndc2pix(p_proj_y, a.H);
+		pm = make_float2(ndc2pix(p_proj_x, a.W), ndc2pix(p_proj_y, a.H));
 	}
+	const float px = pm.x, py = pm.y;
 	uint2 rmin, rmax;
 	tile_rect(px, py, (int)my_radius, rmin, rmax, a.grid_x, a.grid_y);
 	if ((rmax.x - rmin.x) * (rmax.y - rmin.y) == 0) return;
@@ -280,14 +273,11 @@ void launch_project_fwd(const ProjectFwdArgs& a, cudaStream_t s)
 {
 	if (a.P <= 0) return;
 	const int grid = ceil_div(a.P, 256);
-	if (a.distorted) {
-		launch_project_fwd_model<MODEL_DISTORTED>(a, grid, s);
-	} else if (a.fisheye) {
-		launch_project_fwd_model<MODEL_FISHEYE>(a, grid, s);
-	} else if (a.ortho) {
-		launch_project_fwd_model<MODEL_ORTHO>(a, grid, s);
-	} else {
-		launch_project_fwd_model<MODEL_PINHOLE>(a, grid, s);
+	switch (a.lens.model) {
+	case MODEL_DISTORTED: launch_project_fwd_model<MODEL_DISTORTED>(a, grid, s); break;
+	case MODEL_FISHEYE: launch_project_fwd_model<MODEL_FISHEYE>(a, grid, s); break;
+	case MODEL_ORTHO: launch_project_fwd_model<MODEL_ORTHO>(a, grid, s); break;
+	default: launch_project_fwd_model<MODEL_PINHOLE>(a, grid, s);
 	}
 }
 void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t s)

@@ -18,8 +18,7 @@
 // views happens in registers -- no atomics, no zero-fill pass, no per-view gradient tensors.  The multi-view callers
 // (rasterize_views_backward_raw, render_views) write straight into the packed buffer that is the all-reduce message.
 // project_bwd_clouds_kernel runs the same body for several clouds in one launch (mgs_backward_clouds, DESIGN.md section 4).
-#include "mgs_common.cuh"
-#include "mgs_kernels.h"
+#include "camera.cuh"
 
 #include <type_traits>
 
@@ -195,11 +194,11 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			const bool inx = !(ux < -limx || ux > limx), iny = !(uy < -limy || uy > limy);
 			const float cx = fminf(limx, fmaxf(-limx, ux)) * tz, cy = fminf(limy, fmaxf(-limy, uy)) * tz;
 			const float iz = 1.0f / tz, iz2 = iz * iz;
-			const float fx = dfov ? a.intr[v].W / (2.0f * tanx) : w.focal_x, fy = dfov ? a.intr[v].H / (2.0f * tany) : w.focal_y;
+			const float fx = dfov ? focal_length(a.intr[v].W, tanx) : w.focal_x, fy = dfov ? focal_length(a.intr[v].H, tany) : w.focal_y;
 			// M = J Rv: row 0 = (fx / tz) Rv0 - (fx cx / tz^2) Rv2, row 1 likewise with y
 			float m0[3], m1[3], u0[3], u1[3];
 			FisheyeRadial fr{};
-			float j01 = 0.f, j10 = 0.f, fj00 = 0.f, fj11 = 0.f, fj02 = 0.f, fj12 = 0.f;  // FISH: J
+			float J[2][3] = { { 0.f, 0.f, 0.f }, { 0.f, 0.f, 0.f } };  // FISH, DIST: J
 			float du = 0.f, dv = 0.f;  // FISH, DIST: the cotangent of the pixel-space mean (u, v)
 			DistTerms ds{};
 			float nx = 0.f, ny = 0.f;  // DIST: the normalised coordinates t.xy / t.z
@@ -207,25 +206,22 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				du = dm[0] / (0.5f * a.intr[v].W); dv = dm[1] / (0.5f * a.intr[v].H);
 				nx = tx * iz; ny = ty * iz;
 				ds = distortion_terms<true>(nx, ny, a.dc_k[v]);
-				fj00 = fx * ds.d00 * iz; j01 = fx * ds.d01 * iz; fj02 = -fx * (ds.d00 * nx + ds.d01 * ny) * iz;
-				j10 = fy * ds.d01 * iz; fj11 = fy * ds.d11 * iz; fj12 = -fy * (ds.d01 * nx + ds.d11 * ny) * iz;
+				distorted_jacobian(ds, nx, ny, iz, fx, fy, J);
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
-					m0[c] = fj00 * Rv[0][c] + j01 * Rv[1][c] + fj02 * Rv[2][c];
-					m1[c] = j10 * Rv[0][c] + fj11 * Rv[1][c] + fj12 * Rv[2][c];
+					m0[c] = J[0][0] * Rv[0][c] + J[0][1] * Rv[1][c] + J[0][2] * Rv[2][c];
+					m1[c] = J[1][0] * Rv[0][c] + J[1][1] * Rv[1][c] + J[1][2] * Rv[2][c];
 				}
 			} else if (fev) {
 				// dm is the blend's dL/dmean2D, the gradient w.r.t. ndc = (2 u + 1) / W - 1 (the reference's convention: the
 				// blend scales its pixel-space gradient by W / 2, H / 2); the fisheye mean is in pixels
 				du = dm[0] / (0.5f * a.intr[v].W); dv = dm[1] / (0.5f * a.intr[v].H);
 				fr = fisheye_radial<true>(tx, ty, tz, a.fe_k[v]);
-				const float cxy = fr.c * tx * ty;
-				fj00 = fx * (fr.a + fr.c * tx * tx); j01 = fx * cxy; fj02 = -fx * tx * fr.g;
-				j10 = fy * cxy; fj11 = fy * (fr.a + fr.c * ty * ty); fj12 = -fy * ty * fr.g;
+				fisheye_jacobian(fr, tx, ty, fx, fy, J);
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
-					m0[c] = fj00 * Rv[0][c] + j01 * Rv[1][c] + fj02 * Rv[2][c];
-					m1[c] = j10 * Rv[0][c] + fj11 * Rv[1][c] + fj12 * Rv[2][c];
+					m0[c] = J[0][0] * Rv[0][c] + J[0][1] * Rv[1][c] + J[0][2] * Rv[2][c];
+					m1[c] = J[1][0] * Rv[0][c] + J[1][1] * Rv[1][c] + J[1][2] * Rv[2][c];
 				}
 			} else if (orv) {
 #pragma unroll
@@ -302,13 +298,13 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				if (dsv) {
 					// u - cx = fx xd and every entry of J's first row scale with fx
 					const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
-					cg[27] = -(du * fx * ds.xd + dJ00 * fj00 + dJ01 * j01 + dJ02 * fj02) / tanx;
-					cg[28] = -(dv * fy * ds.yd + dJ10 * j10 + dJ11 * fj11 + dJ12 * fj12) / tany;
+					cg[27] = -(du * fx * ds.xd + dJ00 * J[0][0] + dJ01 * J[0][1] + dJ02 * J[0][2]) / tanx;
+					cg[28] = -(dv * fy * ds.yd + dJ10 * J[1][0] + dJ11 * J[1][1] + dJ12 * J[1][2]) / tany;
 				} else if (fev) {
 					// u - cx = fx a t.x and every entry of J's first row scale with fx
 					const float dJ01 = dot3(q0, Rv[1]), dJ10 = dot3(q1, Rv[0]);
-					cg[27] = -(du * fx * fr.a * tx + dJ00 * fj00 + dJ01 * j01 + dJ02 * fj02) / tanx;
-					cg[28] = -(dv * fy * fr.a * ty + dJ10 * j10 + dJ11 * fj11 + dJ12 * fj12) / tany;
+					cg[27] = -(du * fx * fr.a * tx + dJ00 * J[0][0] + dJ01 * J[0][1] + dJ02 * J[0][2]) / tanx;
+					cg[28] = -(dv * fy * fr.a * ty + dJ10 * J[1][0] + dJ11 * J[1][1] + dJ12 * J[1][2]) / tany;
 				} else if (orv) {
 					cg[27] = -(fx / tanx) * dJ00;
 					cg[28] = -(fy / tany) * dJ11;
@@ -343,9 +339,9 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				dt[1] = A * ty * cx2 + Bs * tx * cy2 + Ee * ty * (2.f * fr.c + cy2) + Cc * fr.cz * tx * ty - Ff * (fr.g - fr.cz * ty * ty);
 				dt[2] = A * (fr.cz * tx * tx - fr.g) + Bs * fr.cz * tx * ty + Ee * (fr.cz * ty * ty - fr.g) - (Cc * tx + Ff * ty) * fr.gz
 					+ ddepth;
-				dt[0] += fj00 * du + j10 * dv;
-				dt[1] += j01 * du + fj11 * dv;
-				dt[2] += fj02 * du + fj12 * dv;
+				dt[0] += J[0][0] * du + J[1][0] * dv;
+				dt[1] += J[0][1] * du + J[1][1] * dv;
+				dt[2] += J[0][2] * du + J[1][2] * dv;
 			} else if (orv) {
 				dt[0] = 0.f; dt[1] = 0.f; dt[2] = ddepth;
 			} else {
@@ -369,14 +365,14 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 			if constexpr (CAM) {
 				// t = Rv p + tv and M = J Rv with J held: dL/dRv = dt p^T + J^T dL/dM, dL/dtv = dt
 				const bool full = fev || dsv;  // J has all six entries
-				const float j00 = full ? fj00 : orv ? fx : fx * iz, j11 = full ? fj11 : orv ? fy : fy * iz;
-				const float j02 = full ? fj02 : orv ? 0.f : -fx * cx * iz2, j12 = full ? fj12 : orv ? 0.f : -fy * cy * iz2;
+				const float j00 = full ? J[0][0] : orv ? fx : fx * iz, j11 = full ? J[1][1] : orv ? fy : fy * iz;
+				const float j02 = full ? J[0][2] : orv ? 0.f : -fx * cx * iz2, j12 = full ? J[1][2] : orv ? 0.f : -fy * cy * iz2;
 #pragma unroll
 				for (int c = 0; c < 3; c++) {
 					cg[3 * c] = dt[0] * p[c] + j00 * q0[c];
 					cg[3 * c + 1] = dt[1] * p[c] + j11 * q1[c];
 					cg[3 * c + 2] = dt[2] * p[c] + j02 * q0[c] + j12 * q1[c];
-					if (full) { cg[3 * c] += j10 * q1[c]; cg[3 * c + 1] += j01 * q0[c]; }
+					if (full) { cg[3 * c] += J[1][0] * q1[c]; cg[3 * c + 1] += J[0][1] * q0[c]; }
 				}
 				if constexpr (PLN) {
 #pragma unroll

@@ -1,5 +1,5 @@
 // Point visibility: where query points land in a view and how much of the cloud lies in front of them
-// (include/mgs_rasterizer.h, mgs_visibility_views).  For point x: (u, v) and d = t.z from flow_mean (the projection's own map
+// (include/mgs_rasterizer.h, mgs_visibility_views).  For point x: (u, v) and d = t.z from screen_mean (camera.cuh: the projection's own map
 // of a mean, every camera model), in_view, and T = prod (1 - alpha_i) over the instances of the 16x16 tile holding pixel
 // (floor(u + 0.5), floor(v + 0.5)) in tile-list order with depth z_i < d, alpha_i at the continuous (u, v) with walk_alphas
 // and the forward's T_STOP rule.  At a pixel centre with d behind the scene that is the pixel's final_T bit for bit.
@@ -18,7 +18,7 @@
 // hundreds of independent warps, so the time follows points x cut, not points per tile.
 #include <cub/block/block_scan.cuh>
 #include "blend_common.cuh"
-#include "flow_mean.cuh"
+#include "camera.cuh"
 
 namespace mgs {
 
@@ -32,8 +32,8 @@ __global__ void __launch_bounds__(256) vis_points_kernel(VisArgs a)
 	if (q >= a.Q) return;
 	const V3 p = { a.points[3 * (size_t)q], a.points[3 * (size_t)q + 1], a.points[3 * (size_t)q + 2] };
 	float u, v;
-	const bool ok = flow_mean(a.cam, p, u, v);
-	float d = xform4x3(p, a.cam.viewmatrix).z;  // flow_mean's t.z
+	const bool ok = screen_mean(a.cam, p, u, v);
+	float d = xform4x3(p, a.cam.viewmatrix).z;  // screen_mean's t.z
 	const float nan = __int_as_float(0x7fffffff);
 	if (!ok) u = v = d = nan;
 	const bool in = ok && u >= -0.5f && u < a.W - 0.5f && v >= -0.5f && v < a.H - 0.5f;

@@ -824,6 +824,11 @@ def _distortion_array(views, distortion=None):
     return arr
 
 
+def _lens_arrays(views, ortho=None, fisheye=None, distortion=None):
+    """The views' camera models as the C ABI takes them: (_ortho_flags, _fisheye_array, _distortion_array)"""
+    return _ortho_flags(views, ortho), _fisheye_array(views, fisheye), _distortion_array(views, distortion)
+
+
 def _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, debug,
                ortho=None, fisheye=None, distortion=None):
     """First call for a (cloud size, image size): one projection + scan per view with a host read of the instance count
@@ -949,9 +954,7 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     V = len(views)
     pln = _planar_flag(views, planar_depth, return_normal)
     _check_flow(flow_means3D, return_normal, pln, depth_mask)
-    oarr = _ortho_flags(views, ortho)
-    farr = _fisheye_array(views, fisheye)
-    dcarr = _distortion_array(views, distortion)
+    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]  # a single view needs no side stream
     di = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -1055,9 +1058,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         raise RuntimeError("lift_views_raw needs at least one Gaussian")
     means3D, opacity, scales, rotations, cov3D_precomp = (_prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp))
     V = len(views)
-    oarr = _ortho_flags(views, ortho)
-    farr = _fisheye_array(views, fisheye)
-    dcarr = _distortion_array(views, distortion)
+    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
     C = int(maps[0].shape[0]) if maps is not None else 0
     colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
     main = torch.cuda.current_stream(dev)
@@ -1138,9 +1139,7 @@ def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modif
     means3D, opacity, scales, rotations, cov3D_precomp, points = (
         _prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp, points))
     V, Q = len(views), int(points.shape[0])
-    oarr = _ortho_flags(views, ortho)
-    farr = _fisheye_array(views, fisheye)
-    dcarr = _distortion_array(views, distortion)
+    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
     colors = torch.zeros((P, 3), dtype=torch.float32, device=dev)
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]
@@ -1380,9 +1379,7 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     _check_flow(flow_means3D, grads_normal is not None, pln, depth_mask)
     if flow_means3D is not None and flows is None:
         raise ValueError("flow cotangents need the forward's flow planes (flows)")
-    oarr = _ortho_flags(views, ortho)
-    farr = _fisheye_array(views, fisheye)
-    dcarr = _distortion_array(views, distortion)
+    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
     main = torch.cuda.current_stream(dev)
     opts = dict(dtype=torch.float32, device=dev)
     acc = accumulate_into or {}
@@ -1654,8 +1651,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                     raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is "
                                        "learned from an eager call) or pass `capacities`")
                 _calibrate(L, c["views"], keys[b], dev, d["P"], degree, M, d["means3D"], d["sh"], d["colors"], d["opacity"],
-                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug, _ortho_flags(c["views"], c.get("ortho")),
-                           _fisheye_array(c["views"], c.get("fisheye")), _distortion_array(c["views"], c.get("distortion")))
+                           d["scales"], d["rotations"], scale_modifier, d["cov3D_precomp"], debug,
+                           *_lens_arrays(c["views"], c.get("ortho"), c.get("fisheye"), c.get("distortion")))
         arr, carr, offs = (_b.View * V)(), (_b.Cloud * B)(), (ctypes.c_int * (B + 1))(*offsets)
         aarr = (_b.ViewAlpha * V)() if return_alpha else None
         darr = (_b.ViewDepthMask * V)() if any(c.get("depth_mask") is not None for c in clouds) else None
@@ -1692,7 +1689,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
+        oarr, farr, dcarr = _clouds_lens(clouds)
         if flarr is not None:
             _b.check(L.mgs_forward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
@@ -1766,24 +1763,19 @@ def _clouds_flow(clouds, pc, offsets, dev, keep, backward=False):
     return arr, carr
 
 
-def _clouds_ortho(clouds):
-    """The _ortho calls' int array over every view of the clouds in order, or None when every view is perspective"""
-    flags = [f for c in clouds for f in (_ortho_flags(c["views"], c.get("ortho")) or [0] * len(c["views"]))]
-    return (ctypes.c_int * len(flags))(*flags) if any(flags) else None
-
-
-def _clouds_fisheye(clouds):
-    """The _fisheye calls' ViewFisheye array over every view of the clouds in order, or None when no view is fisheye"""
-    fe = [f for c in clouds for f in ([_fisheye_params(x) for x in c["fisheye"]] if c.get("fisheye") is not None
-                                      else [getattr(s, "fisheye", None) for s in c["views"]])]
-    return _fisheye_array([None] * len(fe), fe)
-
-
-def _clouds_distortion(clouds):
-    """The _distorted calls' ViewDistortion array over every view of the clouds in order, or None when no view is distorted"""
-    dc = [d for c in clouds for d in ([_distortion_params(x) for x in c["distortion"]] if c.get("distortion") is not None
-                                      else [getattr(s, "distortion", None) for s in c["views"]])]
-    return _distortion_array([None] * len(dc), dc)
+def _clouds_lens(clouds):
+    """_lens_arrays over every view of the clouds in order: each cloud's "ortho", "fisheye" and "distortion" entries, or its
+    views' attributes"""
+    def entries(key, attr):
+        out = []
+        for c in clouds:
+            e = list(c[key]) if c.get(key) is not None else [getattr(s, attr, None) for s in c["views"]]
+            if len(e) != len(c["views"]):
+                raise ValueError(f"{key}: expected {len(c['views'])} entries, got {len(e)}")
+            out += e
+        return out
+    return _lens_arrays([s for c in clouds for s in c["views"]], entries("ortho", "orthographic"), entries("fisheye", "fisheye"),
+                        entries("distortion", "distortion"))
 
 
 def _clouds_fov(clouds, dev):
@@ -1907,7 +1899,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                 for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
-        oarr, farr, dcarr = _clouds_ortho(clouds), _clouds_fisheye(clouds), _clouds_distortion(clouds)
+        oarr, farr, dcarr = _clouds_lens(clouds)
         if flarr is not None:
             iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
             _b.check(L.mgs_backward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
