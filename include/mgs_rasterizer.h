@@ -1364,6 +1364,33 @@ int mgs_visibility_views(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_uv, float* out_depth, uint8_t* out_in_view, float* out_T, int debug, void* join_stream);
 
+/*
+ * k nearest neighbours (no reference counterpart; simple-knn's distCUDA2 is the mean of the first three d2 of each point):
+ * for each of Q queries, its k nearest of N reference points by the fp32 squared distance
+ *   d2 = (qx - px)^2 + (qy - py)^2 + (qz - pz)^2,
+ * the exact k-nearest set for those distances (there is no approximate mode).
+ *   - queries [Q,3], or NULL: the points themselves (Q must equal N), and then query i never returns index i (a duplicate
+ *     of point i at distance 0 is returned).
+ *   - Order: each query's results ascend by (d2, index), so ties go to the lower index; the results are deterministic.
+ *   - A point with a non-finite coordinate is never a neighbour; a non-finite query has every slot padded.  Where fewer
+ *     than k neighbours exist, the remaining slots are index -1, d2 = +inf.
+ *   - out_index [Q,k] (long long: usable as a torch index without a conversion), out_dist2 [Q,k], both fully written.
+ *   - state: mgs_knn_state_bytes(N, Q) bytes of device memory on the device current at the call (contents irrelevant on
+ *     entry); the size depends on the device, so query it with the same device current as mgs_knn.  0 means CUDA's size
+ *     query failed (mgs_last_error says why).
+ *   - k is 1 .. 32 (larger k returns MGS_ERR_UNSUPPORTED).  Q = 0 returns 0 and enqueues nothing; N = 0 pads every slot.
+ * Method: a grid over the points' bounding box whose resolution is chosen on the device from the occupied cells, the points
+ * and queries sorted by cell, and one warp per 32 queries of a cell searching shells of cells until the distance to the
+ * unvisited cells exceeds each query's k-th d2.  Nothing allocates, blocks or reads back to the host: a call can be
+ * captured in a CUDA graph.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for k > 32;
+ * MGS_ERR_INVALID_ARG for k < 1, N < 0, Q < 0, queries NULL with Q != N (Q > 0), and a NULL state, points (N > 0) or
+ * output (Q > 0).
+ */
+size_t mgs_knn_state_bytes(int N, int Q);
+int mgs_knn(void* state, int N, int Q, int k, const float* points, const float* queries, long long* out_index, float* out_dist2,
+	int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

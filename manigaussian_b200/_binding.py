@@ -246,6 +246,10 @@ def lib():
                                        vp, vp, vp,                      # means3D shs colors
                                        vp, vp, f, vp, vp,               # opacities scales scale_modifier rotations cov3D_precomp
                                        vp, vp, vp, vp, i, vp]           # out_uv out_depth out_in_view out_T debug join_stream
+    L.mgs_knn_state_bytes.restype = C.c_size_t
+    L.mgs_knn_state_bytes.argtypes = [C.c_int, C.c_int]
+    L.mgs_knn.restype = C.c_int
+    L.mgs_knn.argtypes = [vp, i, i, i, vp, vp, vp, vp, i, vp]  # state N Q k points queries out_index out_dist2 debug stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -311,6 +315,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow",
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_visibility_scratch_bytes", "mgs_visibility_views",
+    "mgs_knn_state_bytes", "mgs_knn",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -2381,3 +2381,31 @@ int mgs_field_query_backward(
 	MGS_STAGE("field_backward");
 	return 0;
 }
+
+size_t mgs_knn_state_bytes(int N, int Q)
+{
+	size_t bytes = 0;
+	const cudaError_t e = mgs::knn_state_bytes(std::max(N, 0), std::max(Q, 0), &bytes);
+	if (e != cudaSuccess) {
+		mgs::fail(MGS_ERR_CUDA, std::string("mgs_knn_state_bytes: ") + cudaGetErrorString(e));
+		return 0;
+	}
+	return bytes;
+}
+
+int mgs_knn(void* state, int N, int Q, int k, const float* points, const float* queries, long long* out_index, float* out_dist2,
+	int debug, void* stream)
+{
+	using namespace mgs;
+	if (k > KNN_MAX_K) return fail(MGS_ERR_UNSUPPORTED, "k must be at most 32");
+	if (k < 1) return fail(MGS_ERR_INVALID_ARG, "k must be >= 1");
+	if (N < 0 || Q < 0) return fail(MGS_ERR_INVALID_ARG, "N and Q must be >= 0");
+	if (Q == 0) return 0;
+	if (!queries && Q != N) return fail(MGS_ERR_INVALID_ARG, "without queries the points are the queries: Q must equal N");
+	if (!state || !out_index || !out_dist2) return fail(MGS_ERR_INVALID_ARG, "state, out_index and out_dist2 are required");
+	if (N > 0 && !points) return fail(MGS_ERR_INVALID_ARG, "points are required with N > 0");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(knn_run(static_cast<char*>(state), N, Q, k, points, queries, out_index, out_dist2, st));
+	MGS_STAGE("knn");
+	return 0;
+}

@@ -40,14 +40,7 @@ constexpr int FQ_WS = 36;      // forward weight tile [query][Gaussian] row stri
 constexpr int FQ_FS_FWD = 40;  // forward feature rows [Gaussian][channel]: B fragments (k = Gaussian) hit 32 banks
 constexpr int FQ_FS_BWD = 36;  // backward feature rows: GEMM 1's B fragments (k = channel) hit 32 banks
 
-// ---- bounding box of the finite queries, as order-preserving unsigned keys ----
-__device__ __forceinline__ uint32_t fkey(float f)
-{
-	const uint32_t b = __float_as_uint(f);
-	return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float funkey(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
-
+// ---- bounding box of the finite queries, as order-preserving unsigned keys (fkey / funkey, mgs_common.cuh) ----
 __global__ void __launch_bounds__(256) field_bbox_kernel(int Q, const float* __restrict__ pts, uint32_t* __restrict__ box)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;

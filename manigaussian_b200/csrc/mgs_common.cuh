@@ -132,4 +132,12 @@ __device__ __forceinline__ float4 ldg_nc_v4(const float4* p)
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// order-preserving unsigned keys of floats: a bounding box as atomicMin / atomicMax of keys (field.cu, knn.cu)
+__device__ __forceinline__ uint32_t fkey(float f)
+{
+	const uint32_t b = __float_as_uint(f);
+	return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float funkey(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
 }  // namespace mgs

@@ -461,6 +461,25 @@ cudaError_t field_forward(char* state, char* pair_state, int Q, int P, int C, co
 cudaError_t field_backward(char* state, char* pair_state, int Q, int P, int C, const float* points, const float* features,
 	const float* scales, const float* rotations, int channel_first, const float* dL_ddensity, const float* dL_dfeatures,
 	float* dL_dpoints, float* dL_dmeans, float* dL_dscales, float* dL_drot, float* dL_dopac, float* dL_dfeat, cudaStream_t st);
+// the field's front-end kernels that knn.cu runs as well (launched with 256 threads per CTA):
+//   field_bbox_kernel       box[0..2] = min, box[3..5] = max of the finite points' fkey (box preset to ~0 / 0);
+//   field_ranges_kernel     range[key] = [first, last + 1) of each run of equal sorted keys (range zeroed by the caller);
+//   field_warp_count_kernel wcnt[b] = warps of 32 over range b;
+//   field_items_kernel      items[woff[b] - wcnt[b] + w] = {first, end, b, 0} of warp w of range b (woff the inclusive scan
+//                           of wcnt), *nitems = woff[nb - 1].
+__global__ void __launch_bounds__(256) field_bbox_kernel(int Q, const float* __restrict__ pts, uint32_t* __restrict__ box);
+__global__ void __launch_bounds__(256) field_ranges_kernel(int n, const uint32_t* __restrict__ keys, uint2* __restrict__ range);
+__global__ void __launch_bounds__(256) field_warp_count_kernel(int nb, const uint2* __restrict__ qrange, uint32_t* __restrict__ wcnt);
+__global__ void __launch_bounds__(256) field_items_kernel(int nb, const uint2* __restrict__ qrange, const uint32_t* __restrict__ wcnt,
+	const uint32_t* __restrict__ woff, uint4* __restrict__ items, int* __restrict__ nitems);
+
+// knn.cu: the k nearest of N points to each of Q queries (include/mgs_rasterizer.h, mgs_knn); queries NULL: the points
+// themselves, each without its own index.  The state (knn_state_bytes) holds the grid, the sorted points and queries and the
+// warp items; nothing is read back to the host.  Both functions size the state for the current device.
+constexpr int KNN_MAX_K = 32;
+cudaError_t knn_state_bytes(int N, int Q, size_t* bytes);
+cudaError_t knn_run(char* state, int N, int Q, int k, const float* points, const float* queries, long long* out_index,
+	float* out_dist2, cudaStream_t st);
 
 // flow.cu: the flow plane's per-Gaussian quads {dx, dy, 0, 0} (include/mgs_rasterizer.h, flow plane) and their backward.
 // FlowCam: the map of one end of a view's flow, the view's pose, field of view and image size with its lens.

@@ -25,7 +25,7 @@ from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
-                         field_query_raw, lift_views_raw, visibility_views_raw,
+                         field_query_raw, knn_raw, lift_views_raw, visibility_views_raw,
                          rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
@@ -756,6 +756,33 @@ def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_
     uv, depth, in_view, T = visibility_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0,
                                                  None, points.detach(), antialiasing=aa)
     return {"uv": uv, "depth": depth, "in_view": in_view.bool(), "transmittance": T}
+
+
+def knn(points, k, queries=None):
+    """The k nearest neighbours of each query among `points` (INTEGRATION.md §17), by the fp32 squared distance
+    d2 = (qx - px)^2 + (qy - py)^2 + (qz - pz)^2; the exact k-nearest set, with no approximate mode.
+    points [N,3] float32 on a CUDA device; queries [Q,3] float32 on the same device, or None for the points themselves (each
+    point's own index is then never returned; a duplicate of it at distance 0 is).  k is 1 .. 32.
+    Returns {"index": [Q,k] int64, "dist2": [Q,k] float32} on the points' device, each row ascending by (d2, index), so ties
+    go to the lower index.  A point with a non-finite coordinate is never a neighbour and a non-finite query gets only
+    padding; where fewer than k neighbours exist the remaining slots hold index -1 and d2 = +inf.
+    Neither output is differentiable (inputs that require grad are detached).  A loss that needs the gradient of a
+    distance recomputes it from the index with autograd, e.g. ((points[index] - points[:, None]) ** 2).sum(-1).
+    Nothing is read back to the host, so a call can be captured in a CUDA graph.  Raises ValueError for a non-float32 or
+    non-[.,3] input, inputs on different devices and k outside 1 .. 32."""
+    for name, t in (("points", points), ("queries", queries)):
+        if t is None and name == "queries":
+            continue
+        if not torch.is_tensor(t) or t.dim() != 2 or t.shape[1] != 3:
+            raise ValueError(f"knn: {name}: expected [.,3], got {tuple(t.shape) if torch.is_tensor(t) else type(t)}")
+        if t.dtype != torch.float32:
+            raise ValueError(f"knn: {name}: expected float32, got {t.dtype}")
+    if queries is not None and queries.device != points.device:
+        raise ValueError(f"knn: queries: expected a tensor on {points.device}, got {queries.device}")
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 32:
+        raise ValueError(f"knn: k must be an int in 1 .. 32, got {k!r}")
+    index, dist2 = knn_raw(points.detach(), k, None if queries is None else queries.detach())
+    return {"index": index, "dist2": dist2}
 
 
 class _QueryField(torch.autograd.Function):

@@ -1993,3 +1993,30 @@ def field_query_backward_raw(state, pair_state, points, scales, rotations, featu
                                             _ptr(features), int(bool(channel_first)), _ptr(grad_density), _ptr(grad_features),
                                             *[_ptr(o) for o in outs], int(bool(debug)), _stream(dev)), "mgs_field_query_backward")
     return tuple(outs)
+
+
+def knn_raw(points, k, queries=None, debug=False):
+    """The k nearest of `points` [N,3] to each query (C ABI mgs_knn; definition in include/mgs_rasterizer.h): `queries` [Q,3],
+    or None for the points themselves (each without its own index).  Returns (index [Q,k] int64, dist2 [Q,k] float32) on the
+    points' device, each query's entries ascending by (d2, index), padded with index -1 and d2 = +inf.  The state is
+    allocated with torch and nothing is read back, so a call can be captured in a CUDA graph.  Not differentiable."""
+    if not points.is_cuda or (queries is not None and not queries.is_cuda):
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = points.device
+    points = _prep(points, dev)
+    queries = _prep(queries, dev)
+    N = points.size(0)
+    Q = N if queries is None else queries.size(0)
+    index = torch.empty((Q, k), dtype=torch.int64, device=dev)
+    dist2 = torch.empty((Q, k), dtype=torch.float32, device=dev)
+    if Q == 0:
+        return index, dist2
+    with torch.cuda.device(dev):  # the state's size depends on the device it is used on
+        nbytes = int(L.mgs_knn_state_bytes(N, Q))
+        if nbytes == 0:
+            raise RuntimeError("mgs_knn_state_bytes: " + _b.last_error())
+        state = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _b.check(L.mgs_knn(_ptr(state), N, Q, int(k), _ptr(points), _ptr(queries), _ptr(index), _ptr(dist2), int(bool(debug)),
+                           _stream(dev)), "mgs_knn")
+    return index, dist2
