@@ -1391,6 +1391,38 @@ size_t mgs_knn_state_bytes(int N, int Q);
 int mgs_knn(void* state, int N, int Q, int k, const float* points, const float* queries, long long* out_index, float* out_dist2,
 	int debug, void* stream);
 
+/*
+ * Neighbour regularisers of a dynamic field (Dynamic 3D Gaussians, Luiten et al.; no reference counterpart): local rigidity,
+ * rotation similarity and isometry between a cloud (xyz [P,3], rot [P,4]) and its deformed next frame (xyz_next [P,3],
+ * rot_next [P,4]) over fixed neighbour lists index [P,k] (as mgs_knn returns them) with constant weights weight [P,k]
+ * (callers pass exp(-lambda dist2) from the same mgs_knn call).  Quaternions are (r, x, y, z), real part first.  Per Gaussian i:
+ *   q_i = rot_i / max(|rot_i|, 1e-12),  qn_i = rot_next_i / max(|rot_next_i|, 1e-12)            (F.normalize)
+ *   rel_i = qn_i (x) conj(q_i)                                                                    (Hamilton product)
+ *   R_i = qrot(rel_i)   (INTEGRATION.md section 17's formula; rel is not renormalised)
+ * Per slot (i, s) with j = index[i,s], w = weight[i,s]: the slot is valid iff 0 <= j < P (padding -1 and out-of-range
+ * indices are skipped before anything is read; j = i gives zero offsets); o = xyz_j - xyz_i, o' = xyz_next_j - xyz_next_i;
+ *   rigid    = 1/(P k) sum_valid w |o' - R_i o|
+ *   rotation = 1/(P k) sum_valid w |rel_j - rel_i|
+ *   isometry = 1/(P k) sum_valid w | |o'| - |o| |
+ * written to out_loss[0..2] (device memory).  P = 0 writes three zeros.  The losses are bitwise identical from call to call.
+ * Backward: dL_dloss [3] in device memory (never read by the host); gradients, each NULL to skip it and fully written
+ * otherwise, to xyz [P,3], rot [P,4], xyz_next [P,3] and rot_next [P,4], none to weight or index.  Conventions as torch:
+ * d|v|/dv = v/|v| and 0 at v = 0; d|a|/da = sign(a), 0 at 0; below the 1e-12 clamp the normalisation's gradient is that
+ * of x / 1e-12.  The backward's float atomics make its last bits depend on the order of the reductions.
+ *   - state: mgs_neighbour_reg_state_bytes(P, k) bytes of device memory, any alignment; the backward reads what the forward
+ *     with the same inputs left there (the offsets and rel of every Gaussian), so it takes the forward's arguments unchanged.
+ *   - k is 1 .. 32 (larger k returns MGS_ERR_UNSUPPORTED).
+ * Nothing allocates, blocks or reads back to the host: both calls can be captured in a CUDA graph.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for k > 32;
+ * MGS_ERR_INVALID_ARG for k < 1, P < 0, and a NULL state, out_loss / dL_dloss, or input (P > 0).
+ */
+size_t mgs_neighbour_reg_state_bytes(int P, int k);
+int mgs_neighbour_reg(void* state, int P, int k, const float* xyz, const float* rot, const float* xyz_next,
+	const float* rot_next, const long long* index, const float* weight, float* out_loss, int debug, void* stream);
+int mgs_neighbour_reg_backward(void* state, int P, int k, const float* xyz, const float* rot, const float* xyz_next,
+	const float* rot_next, const long long* index, const float* weight, const float* dL_dloss, float* dL_dxyz, float* dL_drot,
+	float* dL_dxyz_next, float* dL_drot_next, int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

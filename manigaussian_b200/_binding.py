@@ -250,6 +250,14 @@ def lib():
     L.mgs_knn_state_bytes.argtypes = [C.c_int, C.c_int]
     L.mgs_knn.restype = C.c_int
     L.mgs_knn.argtypes = [vp, i, i, i, vp, vp, vp, vp, i, vp]  # state N Q k points queries out_index out_dist2 debug stream
+    L.mgs_neighbour_reg_state_bytes.restype = C.c_size_t
+    L.mgs_neighbour_reg_state_bytes.argtypes = [C.c_int, C.c_int]
+    L.mgs_neighbour_reg.restype = C.c_int
+    L.mgs_neighbour_reg.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp,  # state P k xyz rot xyz_next rot_next index weight
+                                    vp, i, vp]                         # out_loss debug stream
+    L.mgs_neighbour_reg_backward.restype = C.c_int
+    L.mgs_neighbour_reg_backward.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp,  # state P k xyz rot xyz_next rot_next index weight
+                                             vp, vp, vp, vp, vp, i, vp]         # dL_dloss dL_d{xyz,rot,xyz_next,rot_next} debug stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -316,6 +324,7 @@ EXPORTED_SYMBOLS = (
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_visibility_scratch_bytes", "mgs_visibility_views",
     "mgs_knn_state_bytes", "mgs_knn",
+    "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

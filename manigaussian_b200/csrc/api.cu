@@ -2409,3 +2409,51 @@ int mgs_knn(void* state, int N, int Q, int k, const float* points, const float* 
 	MGS_STAGE("knn");
 	return 0;
 }
+
+size_t mgs_neighbour_reg_state_bytes(int P, int /*k*/)
+{
+	return mgs::neighbour_reg_state_bytes(std::max(P, 0));
+}
+
+// the argument checks both directions share (include/mgs_rasterizer.h, mgs_neighbour_reg)
+static int neighbour_reg_args(const char* where, void* state, int P, int k, const float* xyz, const float* rot,
+	const float* xyz_next, const float* rot_next, const long long* index, const float* weight, const void* loss)
+{
+	using namespace mgs;
+	const std::string w(where);
+	if (k > NEIGHBOUR_REG_MAX_K) return fail(MGS_ERR_UNSUPPORTED, w + ": k must be at most 32");
+	if (k < 1) return fail(MGS_ERR_INVALID_ARG, w + ": k must be >= 1");
+	if (P < 0) return fail(MGS_ERR_INVALID_ARG, w + ": P must be >= 0");
+	if (!state || !loss) return fail(MGS_ERR_INVALID_ARG, w + ": state and the [3] loss buffer are required");
+	if (P > 0 && (!xyz || !rot || !xyz_next || !rot_next || !index || !weight))
+		return fail(MGS_ERR_INVALID_ARG, w + ": xyz, rot, xyz_next, rot_next, index and weight are required with P > 0");
+	return 0;
+}
+
+int mgs_neighbour_reg(void* state, int P, int k, const float* xyz, const float* rot, const float* xyz_next,
+	const float* rot_next, const long long* index, const float* weight, float* out_loss, int debug, void* stream)
+{
+	using namespace mgs;
+	if (int r = neighbour_reg_args("mgs_neighbour_reg", state, P, k, xyz, rot, xyz_next, rot_next, index, weight, out_loss))
+		return r;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(neighbour_reg_forward(state, P, k, xyz, rot, xyz_next, rot_next, index, weight, out_loss, st));
+	MGS_STAGE("neighbour_reg");
+	return 0;
+}
+
+int mgs_neighbour_reg_backward(void* state, int P, int k, const float* xyz, const float* rot, const float* xyz_next,
+	const float* rot_next, const long long* index, const float* weight, const float* dL_dloss, float* dL_dxyz, float* dL_drot,
+	float* dL_dxyz_next, float* dL_drot_next, int debug, void* stream)
+{
+	using namespace mgs;
+	if (int r = neighbour_reg_args("mgs_neighbour_reg_backward", state, P, k, xyz, rot, xyz_next, rot_next, index, weight,
+	                               dL_dloss))
+		return r;
+	if (P == 0) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(neighbour_reg_backward(state, P, k, rot, rot_next, index, weight, dL_dloss, dL_dxyz, dL_drot, dL_dxyz_next,
+	                                dL_drot_next, st));
+	MGS_STAGE("neighbour_reg_bwd");
+	return 0;
+}

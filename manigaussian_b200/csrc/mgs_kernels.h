@@ -551,4 +551,16 @@ void launch_visibility_points(const VisArgs& a, cudaStream_t s);
 void launch_visibility_group(const VisArgs& a, cudaStream_t s);
 void launch_visibility_query(const VisArgs& a, cudaStream_t s);
 
+// neighbour_reg.cu: the dynamic field's local-rigidity, rotation-similarity and isometry terms over [P,k] neighbour lists
+// (include/mgs_rasterizer.h, mgs_neighbour_reg).  The state (neighbour_reg_state_bytes, any alignment) holds the per-Gaussian
+// records and R_i the forward writes, its CTA partials and the backward's gradient rows; the backward reads the records of
+// the forward with the same inputs.  Nothing is read back to the host.
+constexpr int NEIGHBOUR_REG_MAX_K = 32;
+size_t neighbour_reg_state_bytes(int P);
+cudaError_t neighbour_reg_forward(void* state, int P, int k, const float* xyz, const float* rot, const float* xyz_next,
+	const float* rot_next, const long long* index, const float* weight, float* out_loss, cudaStream_t st);
+cudaError_t neighbour_reg_backward(void* state, int P, int k, const float* rot, const float* rot_next, const long long* index,
+	const float* weight, const float* dL_dloss, float* dL_dxyz, float* dL_drot, float* dL_dxyz_next, float* dL_drot_next,
+	cudaStream_t st);
+
 }  // namespace mgs

@@ -25,7 +25,7 @@ from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
-                         field_query_raw, knn_raw, lift_views_raw, visibility_views_raw,
+                         field_query_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
                          rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
@@ -783,6 +783,64 @@ def knn(points, k, queries=None):
         raise ValueError(f"knn: k must be an int in 1 .. 32, got {k!r}")
     index, dist2 = knn_raw(points.detach(), k, None if queries is None else queries.detach())
     return {"index": index, "dist2": dist2}
+
+
+class _NeighbourReg(torch.autograd.Function):
+    """the three neighbour regularisers: one node, differentiable in xyz, rot, xyz_next and rot_next"""
+
+    @staticmethod
+    def forward(ctx, xyz, rot, xyz_next, rot_next, index, weight):
+        loss, state = neighbour_reg_raw(xyz.detach(), rot.detach(), xyz_next.detach(), rot_next.detach(), index, weight)
+        ctx.save_for_backward(xyz, rot, xyz_next, rot_next, index, weight, state)
+        return tuple(loss.unbind(0))
+
+    @staticmethod
+    def backward(ctx, g_rigid, g_rotation, g_isometry):
+        xyz, rot, xyz_next, rot_next, index, weight, state = ctx.saved_tensors
+        needs = tuple(ctx.needs_input_grad[:4])
+        if not any(needs):
+            return (None,) * 6
+        zero = torch.zeros((), dtype=torch.float32, device=xyz.device)
+        grad = torch.stack([zero if g is None else g.float() for g in (g_rigid, g_rotation, g_isometry)])
+        g = neighbour_reg_backward_raw(state, xyz.detach(), rot.detach(), xyz_next.detach(), rot_next.detach(), index, weight,
+                                       grad, needs=needs)
+        return g + (None, None)
+
+
+def neighbour_regularisers(xyz, rot, xyz_next, rot_next, index, weight):
+    """The neighbour regularisers of Dynamic 3D Gaussians (Luiten et al.; INTEGRATION.md §18) between a cloud and its
+    deformed next frame, fused (definition in include/mgs_rasterizer.h, mgs_neighbour_reg).
+    xyz, xyz_next [P,3] and rot, rot_next [P,4] (quaternions (r, x, y, z), real part first, normalised inside) float32 on one
+    CUDA device; index [P,k] int64 with k = 1 .. 32, as knn returns it (slots outside 0 .. P-1, such as knn's -1 padding,
+    are skipped); weight [P,k] float32, a constant, e.g. torch.exp(-lam * dist2) from the same knn call.  With
+    rel_i = normalize(rot_next_i) * conj(normalize(rot_i)), R_i its rotation matrix, o = xyz_j - xyz_i and
+    o' = xyz_next_j - xyz_next_i, the three terms are 1/(P k) times the sums over the valid slots of
+        rigid: w |o' - R_i o|,   rotation: w |rel_j - rel_i|,   isometry: w | |o'| - |o| |.
+    Returns {"rigid", "rotation", "isometry"}, three 0-dim tensors of one autograd node, differentiable in xyz, rot, xyz_next
+    and rot_next (only the gradients autograd asks for are computed).  Nothing is read back to the host.  Raises ValueError
+    for a shape, dtype or device mismatch, index not int64 [P,k], k outside 1 .. 32 and a weight that requires grad."""
+    where = "neighbour_regularisers"
+    tensors = (("xyz", xyz, 3), ("rot", rot, 4), ("xyz_next", xyz_next, 3), ("rot_next", rot_next, 4),
+               ("index", index, None), ("weight", weight, None))
+    for name, t, _ in tensors:
+        if not torch.is_tensor(t):
+            raise ValueError(f"{where}: {name}: expected a tensor, got {type(t)}")
+    P = xyz.shape[0] if xyz.dim() == 2 else -1
+    k = index.shape[1] if index.dim() == 2 else -1
+    for name, t, c in tensors:
+        want = (P, c if c is not None else k)
+        if tuple(t.shape) != want or P < 0:
+            raise ValueError(f"{where}: {name}: expected [{P},{c if c is not None else 'k'}], got {tuple(t.shape)}")
+        if t.dtype != (torch.int64 if name == "index" else torch.float32):
+            raise ValueError(f"{where}: {name}: expected {'int64' if name == 'index' else 'float32'}, got {t.dtype}")
+        if t.device != xyz.device:
+            raise ValueError(f"{where}: {name}: expected a tensor on {xyz.device}, got {t.device}")
+    if not 1 <= k <= 32:
+        raise ValueError(f"{where}: k must be in 1 .. 32, got {k}")
+    if weight.requires_grad:
+        raise ValueError(f"{where}: weight requires grad, but no gradient flows to it: pass weight.detach()")
+    rigid, rotation, isometry = _NeighbourReg.apply(xyz, rot, xyz_next, rot_next, index, weight)
+    return {"rigid": rigid, "rotation": rotation, "isometry": isometry}
 
 
 class _QueryField(torch.autograd.Function):

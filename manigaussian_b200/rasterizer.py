@@ -2020,3 +2020,41 @@ def knn_raw(points, k, queries=None, debug=False):
         _b.check(L.mgs_knn(_ptr(state), N, Q, int(k), _ptr(points), _ptr(queries), _ptr(index), _ptr(dist2), int(bool(debug)),
                            _stream(dev)), "mgs_knn")
     return index, dist2
+
+
+def neighbour_reg_raw(xyz, rot, xyz_next, rot_next, index, weight, debug=False):
+    """The neighbour regularisers (C ABI mgs_neighbour_reg; definition in include/mgs_rasterizer.h) of a cloud xyz [P,3],
+    rot [P,4] and its next frame xyz_next [P,3], rot_next [P,4] over index [P,k] int64 with constant weight [P,k].
+    Returns (loss [3] = {rigid, rotation, isometry}, state) on xyz's device; the state is what neighbour_reg_backward_raw
+    reads.  Nothing is read back to the host, so a call can be captured in a CUDA graph.  Not differentiable."""
+    if not all(t.is_cuda for t in (xyz, rot, xyz_next, rot_next, index, weight)):
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = xyz.device
+    xyz, rot, xyz_next, rot_next, weight = (_prep(t, dev) for t in (xyz, rot, xyz_next, rot_next, weight))
+    index = index.to(device=dev, dtype=torch.int64).contiguous()
+    P, k = index.shape
+    loss = torch.empty(3, dtype=torch.float32, device=dev)
+    state = torch.empty(int(L.mgs_neighbour_reg_state_bytes(P, k)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_neighbour_reg(_ptr(state), P, k, _ptr(xyz), _ptr(rot), _ptr(xyz_next), _ptr(rot_next), _ptr(index),
+                                     _ptr(weight), _ptr(loss), int(bool(debug)), _stream(dev)), "mgs_neighbour_reg")
+    return loss, state
+
+
+def neighbour_reg_backward_raw(state, xyz, rot, xyz_next, rot_next, index, weight, grad_loss, needs=(True,) * 4, debug=False):
+    """Backward of neighbour_reg_raw (C ABI mgs_neighbour_reg_backward) with the state its forward returned for the same
+    inputs: grad_loss [3] on the device (read there, never by the host).  Returns (dL_dxyz, dL_drot, dL_dxyz_next,
+    dL_drot_next), each None where `needs` is False."""
+    L = _b.lib()
+    dev = xyz.device
+    xyz, rot, xyz_next, rot_next, weight = (_prep(t, dev) for t in (xyz, rot, xyz_next, rot_next, weight))
+    index = index.to(device=dev, dtype=torch.int64).contiguous()
+    grad_loss = _prep(grad_loss, dev)
+    P, k = index.shape
+    outs = [torch.empty((P, c), dtype=torch.float32, device=dev) if n else None for n, c in zip(needs, (3, 4, 3, 4))]
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_neighbour_reg_backward(_ptr(state), P, k, _ptr(xyz), _ptr(rot), _ptr(xyz_next), _ptr(rot_next),
+                                              _ptr(index), _ptr(weight), _ptr(grad_loss), *[_ptr(o) for o in outs],
+                                              int(bool(debug)), _stream(dev)), "mgs_neighbour_reg_backward")
+    return tuple(outs)
