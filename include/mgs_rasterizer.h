@@ -1343,13 +1343,14 @@ int mgs_field_query_backward(
  *   - Outside the view (in_view false) T = 1.  uv and depth are written wherever the cull passes, NaN where it fails.
  * Hence at a pixel centre with d behind every Gaussian, T is that pixel's final_T bit for bit (the 8x4 block lists drop only
  * pairs with alpha < 1/255 at every pixel centre of the block, which contribute nothing); a point in front of every Gaussian
- * has T = 1; along a ray T does not increase with d.  The outputs are not differentiable.
+ * has T = 1; along a ray T does not increase with d.  mgs_visibility_views_backward below differentiates them.
  * Arguments are those of mgs_lift_views_distorted with the map arguments replaced by the points and the outputs:
  *   - points [Q,3]; out_uv [V,Q,2], out_depth [V,Q], out_in_view [V,Q] (uint8 0/1), each NULL to skip it; out_T [V,Q].
  *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
  *     (sized as for mgs_forward_views), binning_capacity, status and stream as for the lift, and blend_scratch, the point
  *     scratch of mgs_visibility_scratch_bytes(Q, width, height) bytes (contents irrelevant on entry).  Every other field is
- *     ignored.  The view's state afterwards holds its projection and binning; the blend state is not written.
+ *     ignored (dL_dmean2D carries the backward's scratch).  The view's state afterwards holds its projection and binning;
+ *     the blend state is not written.
  *   - Nothing allocates or blocks: a call can be captured in a CUDA graph.  Q = 0 returns 0 and enqueues nothing.
  * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0, Q < 0,
  * points NULL with Q > 0, out_T NULL, a view without its state buffers, blend_scratch, matrices or radii, the camera-model
@@ -1363,6 +1364,49 @@ int mgs_visibility_views(
 	const float* means3D, const float* shs, const float* colors_precomp,
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* out_uv, float* out_depth, uint8_t* out_in_view, float* out_T, int debug, void* join_stream);
+
+/*
+ * Point visibility backward (no reference counterpart): the chain of cotangents dL_dT, dL_duv and dL_ddepth of the outputs of
+ * mgs_visibility_views into the points, the cloud and the cameras.  With uv, d, in_view and T those outputs for view v and
+ * point x:
+ *   - Transmittance, where in_view only.  A, the accepted candidates, are the candidates in tile-list order with power <= 0
+ *     and alpha >= 1/255 before the factor that would take T below 1e-4.  dT/dalpha_i = -T / (1 - alpha_i) for i in A, 0
+ *     for every other instance, with alpha_i = min(0.99, o_i G_i(uv)).  As in the blend backward, dL/dG = o dL/dalpha with
+ *     no mask for the 0.99 clamp and dL/do = G dL/dalpha (o the compensated opacity with antialiasing = 1).  The tile, the
+ *     candidate set, the depth cut, the 1/255 cut and the stop are constants: d receives nothing through T.  Through G_i(uv)
+ *     T reaches the Gaussian's screen mean, conic and opacity, and uv, with dG/duv = -dG/dmean.
+ *   - uv and depth, where the view's cull passes: uv through the projection's map of a mean, d = t.z through row 2 of the
+ *     view matrix, to the point and the view's camera.  Where the cull fails (uv and depth NaN) their cotangents are ignored.
+ *   - Outputs, each NULL to skip it and fully written otherwise (sums over the V views): dL_dpoints [Q,3]; dL_dmean3D [P,3],
+ *     dL_dopacity [P], dL_dscale [P,3], dL_drot [P,4] (zeros without scales and rotations) and dL_dcov3D [P,6] (with
+ *     cov3D_precomp) through the per-Gaussian chain of the render's backward; per view through `cam` (one
+ *     mgs_view_camera_grad per view, or NULL; its scratch field is ignored) dL_dviewmatrix, dL_dprojmatrix and dL_dcampos
+ *     (0: no SHs), and through intr (as the _intr calls take it) dL_dtan_fov with a device field of view.  A camera's gradient
+ *     sums the Gaussian path and the point path, with the definitions of the camera-gradient and intrinsics sections.
+ *   - Arguments: those of mgs_visibility_views, unchanged since that call (its views' state buffers and point scratch in
+ *     blend_scratch are read as it left them), with its outputs replaced by out_T [V,Q] (its T; needed with dL_dT), the
+ *     cotangents dL_dT [V,Q], dL_duv [V,Q,2] and dL_ddepth [V,Q] (each nullable), the outputs and `cam`.  Each view also
+ *     carries its backward scratch of mgs_visibility_backward_scratch_bytes(P, Q) bytes (contents irrelevant on entry) in
+ *     mgs_view.dL_dmean2D, cast; mgs_visibility_views ignores that field.
+ *   - The per-Gaussian chain runs when a cloud or camera output is asked for, the point chain when dL_dpoints or a camera
+ *     output is.  The blend-stage rows of the Gaussians are summed with float reductions, so their last bits may vary from
+ *     call to call, as the render backward's; dL_dpoints and the point path's camera sums are deterministic (each point sums
+ *     its views in order; the camera rows are fixed-order partial sums).
+ *   - Nothing allocates, blocks or reads back to the host: a call can be captured in a CUDA graph.  Q = 0 returns 0 and
+ *     enqueues nothing.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for those of
+ * mgs_visibility_views (out_T only with dL_dT), a view without its backward scratch, and dL_dcov3D without cov3D_precomp.
+ */
+size_t mgs_visibility_backward_scratch_bytes(int P, int Q);
+int mgs_visibility_views_backward(
+	int V, const mgs_view* views, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int Q, const float* points,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	const float* out_T, const float* dL_dT, const float* dL_duv, const float* dL_ddepth,
+	float* dL_dpoints, float* dL_dmean3D, float* dL_dopacity, float* dL_dscale, float* dL_drot, float* dL_dcov3D,
+	const mgs_view_camera_grad* cam, int debug, void* join_stream);
 
 /*
  * k nearest neighbours (no reference counterpart; simple-knn's distCUDA2 is the mean of the first three d2 of each point):

@@ -246,6 +246,13 @@ def lib():
                                        vp, vp, vp,                      # means3D shs colors
                                        vp, vp, f, vp, vp,               # opacities scales scale_modifier rotations cov3D_precomp
                                        vp, vp, vp, vp, i, vp]           # out_uv out_depth out_in_view out_T debug join_stream
+    L.mgs_visibility_backward_scratch_bytes.restype = C.c_size_t
+    L.mgs_visibility_backward_scratch_bytes.argtypes = [C.c_int, C.c_int]
+    L.mgs_visibility_views_backward.restype = C.c_int
+    L.mgs_visibility_views_backward.argtypes = L.mgs_visibility_views.argtypes[:20] + [
+        vp, vp, vp, vp,                  # out_T dL_dT dL_duv dL_ddepth
+        vp, vp, vp, vp, vp, vp,          # dL_dpoints dL_dmean3D dL_dopacity dL_dscale dL_drot dL_dcov3D
+        C.POINTER(ViewCameraGrad), i, vp]  # cam debug join_stream
     L.mgs_knn_state_bytes.restype = C.c_size_t
     L.mgs_knn_state_bytes.argtypes = [C.c_int, C.c_int]
     L.mgs_knn.restype = C.c_int
@@ -323,6 +330,7 @@ EXPORTED_SYMBOLS = (
     "mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow",
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_visibility_scratch_bytes", "mgs_visibility_views",
+    "mgs_visibility_backward_scratch_bytes", "mgs_visibility_views_backward",
     "mgs_knn_state_bytes", "mgs_knn",
     "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
     "mgs_activate", "mgs_activate_backward",

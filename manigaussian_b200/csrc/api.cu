@@ -1432,6 +1432,37 @@ struct VisScratch {
 		return s;
 	}
 };
+// the query arguments of one view of mgs_visibility_views over its state s and point scratch x (outputs left NULL)
+static VisArgs vis_args(const mgs_view& w, const ViewState& s, const VisScratch& x, const FlowCam& cam, int Q, const float* points)
+{
+	VisArgs a{};
+	a.Q = Q; a.W = w.width; a.H = w.height; a.grid_x = s.gx; a.num_tiles = (int)s.T;
+	a.cam = cam;
+	a.points = points;
+	a.pt = x.pt; a.keys = x.keys; a.idx = x.idx; a.keys_sorted = x.keys_sorted; a.idx_sorted = x.idx_sorted;
+	a.qranges = x.qranges; a.item_end = x.item_end;
+	a.ranges = s.img.ranges; a.point_list = s.bin.point_list; a.depths = s.geom.depths; a.recs = s.bin.recs;
+	return a;
+}
+// the backward scratch of one view of mgs_visibility_views_backward, carved from its dL_dmean2D: the blend-stage rows gb, the
+// T path's uv cotangents, the point path's camera and focal-length rows (one per VIS_PTS_BWD_THREADS points), the Gaussian
+// path's camera rows, and the two cloud outputs the per-Gaussian chain always writes, for a call that asks only for cameras
+struct VisBwdScratch {
+	float* gb; float* duv; float* pt_rows; float* pt_intr; float* g_rows; float* mean3D; float* opacity;
+	static VisBwdScratch carve(char*& chunk, size_t P, size_t Q)
+	{
+		VisBwdScratch s;
+		const size_t qb = (Q + VIS_PTS_BWD_THREADS - 1) / VIS_PTS_BWD_THREADS;
+		obtain(chunk, s.gb, P * GB_STRIDE);
+		obtain(chunk, s.duv, 2 * Q);
+		obtain(chunk, s.pt_rows, qb * CAM_TERMS);
+		obtain(chunk, s.pt_intr, qb * CAM_INTR_TERMS);
+		obtain(chunk, s.g_rows, camera_rows_bytes((int)P) / sizeof(float));
+		obtain(chunk, s.mean3D, 3 * P);
+		obtain(chunk, s.opacity, P);
+		return s;
+	}
+};
 }  // namespace mgs
 
 extern "C" {
@@ -1487,15 +1518,9 @@ int mgs_visibility_views(
 				char* sc = w.blend_scratch;
 				const VisScratch x = VisScratch::carve(sc, (size_t)Q, s.T);
 				const size_t o = (size_t)v * Q;
-				VisArgs a{};
-				a.Q = Q; a.W = w.width; a.H = w.height; a.grid_x = s.gx; a.num_tiles = (int)s.T;
-				a.cam = flow_cam(w, device_fov(intr, v), lens[v], w.viewmatrix, w.projmatrix);
-				a.points = points;
+				VisArgs a = vis_args(w, s, x, flow_cam(w, device_fov(intr, v), lens[v], w.viewmatrix, w.projmatrix), Q, points);
 				a.out_uv = out_uv ? out_uv + 2 * o : nullptr; a.out_depth = out_depth ? out_depth + o : nullptr;
 				a.out_in_view = out_in_view ? out_in_view + o : nullptr; a.out_T = out_T + o;
-				a.pt = x.pt; a.keys = x.keys; a.idx = x.idx; a.keys_sorted = x.keys_sorted; a.idx_sorted = x.idx_sorted;
-				a.qranges = x.qranges; a.item_end = x.item_end;
-				a.ranges = s.img.ranges; a.point_list = s.bin.point_list; a.depths = s.geom.depths; a.recs = s.bin.recs;
 				launch_visibility_points(a, st);
 				MGS_STAGE("visibility_points");
 				// tile ids up to num_tiles (the key of a point outside the view): stable, so a tile's points stay in id order
@@ -1510,6 +1535,149 @@ int mgs_visibility_views(
 		}
 	}
 	return join_streams(V, views, join);
+}
+
+size_t mgs_visibility_backward_scratch_bytes(int P, int Q)
+{
+	return required([&](char*& p) { VisBwdScratch::carve(p, (size_t)std::max(P, 0), (size_t)std::max(Q, 0)); });
+}
+
+int mgs_visibility_views_backward(
+	int V, const mgs_view* views, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int Q, const float* points,
+	const float* means3D, const float* shs, const float* colors_precomp,
+	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
+	const float* out_T, const float* dL_dT, const float* dL_duv, const float* dL_ddepth,
+	float* dL_dpoints, float* dL_dmean3D, float* dL_dopacity, float* dL_dscale, float* dL_drot, float* dL_dcov3D,
+	const mgs_view_camera_grad* cam, int debug, void* join_stream)
+{
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
+	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
+	if (Q < 0) return fail(MGS_ERR_INVALID_ARG, "Q must be >= 0");
+	if (Q > 0 && !points) return fail(MGS_ERR_INVALID_ARG, "points are required with Q > 0");
+	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
+	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
+	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours (never read: they keep the projection the forward's)");
+	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
+	if (dL_dT && !out_T) return fail(MGS_ERR_INVALID_ARG, "dL_dT needs out_T, the transmittance the forward wrote");
+	if (dL_dcov3D && !cov3D_precomp) return fail(MGS_ERR_INVALID_ARG, "dL_dcov3D needs cov3D_precomp");
+	for (int v = 0; v < V; v++) {
+		const mgs_view& w = views[v];
+		if (!w.geometry_state || !w.binning_state || !w.image_state)
+			return fail(MGS_ERR_INVALID_ARG, "view: the three state buffers are required");
+		if (!w.blend_scratch) return fail(MGS_ERR_INVALID_ARG, "view: blend_scratch (mgs_visibility_scratch_bytes) is required");
+		if (!w.dL_dmean2D)
+			return fail(MGS_ERR_INVALID_ARG, "view: dL_dmean2D must carry the backward scratch (mgs_visibility_backward_scratch_bytes)");
+		if (!w.viewmatrix || !w.projmatrix || !w.radii) return fail(MGS_ERR_INVALID_ARG, "view: matrices and radii are required");
+		if (shs && !colors_precomp && !w.cam_pos) return fail(MGS_ERR_INVALID_ARG, "view: cam_pos is required with SHs");
+		if (w.width <= 0 || w.height <= 0 || w.binning_capacity < 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size or capacity");
+	}
+	if (Q == 0) return 0;
+	const Cloud c{ P, D, M, 0, means3D, shs, colors_precomp, nullptr, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+		antialiasing };
+	bool any_cam = false;
+	for (int v = 0; v < V; v++) any_cam |= camera_on(cam, intr, v);
+	const bool gauss = dL_dmean3D || dL_dopacity || dL_dscale || dL_drot || dL_dcov3D || any_cam;  // the per-Gaussian chain
+	const bool chain = dL_dpoints || any_cam;                                                      // the point chain
+	const bool tpath = dL_dT && (gauss || chain);
+	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
+	// the views' scratch, carved once
+	std::vector<VisBwdScratch> ys(V);
+	for (int v = 0; v < V; v++) {
+		char* bc = reinterpret_cast<char*>(views[v].dL_dmean2D);
+		ys[v] = VisBwdScratch::carve(bc, (size_t)P, (size_t)Q);
+	}
+	// per view on its stream: the T path's replay into gb and duv
+	int rc = fork_streams(V, views, join);
+	if (rc < 0) return rc;
+	for (int v = 0; v < V; v++) {
+		const mgs_view& w = views[v];
+		cudaStream_t st = reinterpret_cast<cudaStream_t>(w.stream);
+		const VisBwdScratch& y = ys[v];
+		if (gauss) MGS_CUDA(cudaMemsetAsync(y.gb, 0, (size_t)P * GB_STRIDE * sizeof(float), st));
+		if (!tpath) continue;
+		if (chain) MGS_CUDA(cudaMemsetAsync(y.duv, 0, 2 * (size_t)Q * sizeof(float), st));
+		const ViewState s = carve_view(w, P);
+		char* sc = w.blend_scratch;
+		const VisScratch x = VisScratch::carve(sc, (size_t)Q, s.T);
+		VisQueryBwdArgs b{};
+		b.f = vis_args(w, s, x, flow_cam(w, device_fov(intr, v), lens[v], w.viewmatrix, w.projmatrix), Q, points);
+		b.f.out_T = const_cast<float*>(out_T + (size_t)v * Q);  // read only
+		b.dL_dT = dL_dT + (size_t)v * Q;
+		b.gb = gauss ? y.gb : nullptr;
+		b.duv = chain ? y.duv : nullptr;
+		launch_visibility_query_bwd(b, st);
+		MGS_STAGE("visibility_query_bwd");
+	}
+	rc = join_streams(V, views, join);
+	if (rc < 0) return rc;
+	cudaStream_t st = join;
+	// the point chain on the join stream, MAX_BWD_VIEWS views per launch; its camera sums are written, the Gaussian path's added
+	for (int v0 = 0; chain && v0 < V; v0 += MAX_BWD_VIEWS) {
+		VisPointsBwdArgs pa{};
+		pa.Q = Q; pa.V = std::min(V - v0, (int)MAX_BWD_VIEWS); pa.points = points; pa.dL_dpoints = dL_dpoints; pa.accumulate = v0 > 0;
+		CamReduceArgs cr{};
+		for (int u = 0; u < pa.V; u++) {
+			const int v = v0 + u;
+			const mgs_view& w = views[v];
+			VisPointsBwdView& pv = pa.view[u];
+			pv.cam = flow_cam(w, device_fov(intr, v), lens[v], w.viewmatrix, w.projmatrix);
+			pv.dL_duv = dL_duv ? dL_duv + 2 * (size_t)v * Q : nullptr;
+			pv.dL_ddepth = dL_ddepth ? dL_ddepth + (size_t)v * Q : nullptr;
+			pv.duv = tpath ? ys[v].duv : nullptr;
+			if (!camera_on(cam, intr, v)) continue;
+			float* dtf = tan_fov_grad(intr, v);
+			pv.cam_rows = ys[v].pt_rows;
+			pv.intr_rows = dtf ? ys[v].pt_intr : nullptr;
+			const mgs_view_camera_grad* e = cam ? cam + v : nullptr;
+			cr.view[cr.V++] = CamReduceView{ pv.cam_rows, ceil_div(Q, VIS_PTS_BWD_THREADS), e ? e->dL_dviewmatrix : nullptr,
+				e ? e->dL_dprojmatrix : nullptr, e ? e->dL_dcampos : nullptr, pv.intr_rows, dtf };
+		}
+		launch_visibility_points_bwd(pa, st);
+		if (cr.V > 0) launch_camera_grad_reduce(cr, st);
+		MGS_STAGE("visibility_points_bwd");
+	}
+	if (!gauss) return 0;
+	// the per-Gaussian chain of the render's backward (backward_views' stage 2) over the views' gb
+	const bool have_sr = c.scales && c.rotations && (dL_dscale || dL_drot);
+	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
+		ProjectBwdViewsArgs pb{};
+		pb.P = P; pb.D = c.D; pb.M = c.M; pb.V = std::min(V - v0, (int)MAX_BWD_VIEWS);
+		pb.means3D = c.means3D; pb.shs = c.shs;
+		pb.scales = have_sr ? c.scales : nullptr; pb.rotations = c.rotations; pb.scale_modifier = c.scale_modifier;
+		pb.cov3D_precomp = c.cov3D_precomp;
+		if (!have_sr && !c.cov3D_precomp) pb.cov3D_precomp = carve_view(views[0], P).geom.cov3D;
+		pb.accumulate = v0 > 0;
+		// with camera outputs only, the two rows the chain always writes go to view 0's scratch
+		pb.dL_dmean3D = dL_dmean3D ? dL_dmean3D : ys[0].mean3D;
+		pb.dL_dopacity = dL_dopacity ? dL_dopacity : ys[0].opacity;
+		pb.dL_dcov3D = dL_dcov3D; pb.dL_dscale = dL_dscale; pb.dL_drot = dL_drot;
+		pb.antialias = c.antialias;
+		CamReduceArgs cr{};
+		cr.accumulate = 1;  // the point chain wrote every camera output
+		for (int u = 0; u < pb.V; u++) {
+			const int v = v0 + u;
+			const mgs_view& w = views[v];
+			const ViewState s = carve_view(w, P);
+			pb.view[u] = bwd_view(w, P, nullptr);
+			pb.view[u].gb = ys[v].gb;
+			if (c.antialias) pb.conic_opacity[u] = s.geom.conic_opacity;
+			float* dtf = tan_fov_grad(intr, v);
+			pb.intr[u] = ProjectBwdIntr{ device_fov(intr, v), w.width, w.height, dtf ? s.geom.cam_intr : nullptr };
+			bwd_lens(pb, u, lens[v]);
+			if (!camera_on(cam, intr, v)) continue;
+			pb.cam_rows[u] = ys[v].g_rows;
+			const mgs_view_camera_grad* e = cam ? cam + v : nullptr;
+			cr.view[cr.V++] = CamReduceView{ ys[v].g_rows, (P + 127) / 128, e ? e->dL_dviewmatrix : nullptr,
+				e ? e->dL_dprojmatrix : nullptr, e ? e->dL_dcampos : nullptr, pb.intr[u].rows, dtf };
+		}
+		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
+		MGS_STAGE("visibility_project_bwd");
+	}
+	return 0;
 }
 
 int mgs_backward_views(

@@ -550,6 +550,38 @@ struct VisArgs {
 void launch_visibility_points(const VisArgs& a, cudaStream_t s);
 void launch_visibility_group(const VisArgs& a, cudaStream_t s);
 void launch_visibility_query(const VisArgs& a, cudaStream_t s);
+// the backward (include/mgs_rasterizer.h, mgs_visibility_views_backward).  The query backward replays one view's query over
+// the forward's point scratch (f, with f.out_T the forward's T): per accepted pair the cotangent dL_dT[q] of the point's T goes
+// into the Gaussian's blend-stage record (gb, zeroed by the caller, or NULL) and into dL/duv of the point (duv [Q,2], zeroed
+// by the caller, or NULL).
+struct VisQueryBwdArgs {
+	VisArgs f;
+	const float* dL_dT;          // [Q]
+	float* gb;                   // [P, GB_STRIDE] or NULL
+	float* duv;                  // [Q,2] or NULL
+};
+void launch_visibility_query_bwd(const VisQueryBwdArgs& a, cudaStream_t s);
+// the point chain: one thread per point over the launch's views in order, uv's cotangent (dL_duv plus the T path's duv) through
+// screen_mean's derivative and depth's through row 2 of the view matrix, where the view's cull passes; camera rows as the
+// flow backward's.  CTAs of VIS_PTS_BWD_THREADS.
+constexpr int VIS_PTS_BWD_THREADS = 128;
+struct VisPointsBwdView {
+	FlowCam cam;
+	const float* dL_duv;         // [Q,2] or NULL
+	const float* dL_ddepth;      // [Q] or NULL
+	const float* duv;            // [Q,2] the T path's uv cotangent, or NULL
+	float* cam_rows;             // [CTAs][CAM_TERMS] or NULL
+	float* intr_rows;            // [CTAs][CAM_INTR_TERMS] or NULL
+};
+struct VisPointsBwdArgs {
+	int Q, V;
+	const float* points;
+	float* dL_dpoints;           // [Q,3] or NULL
+	int accumulate;              // 0: dL_dpoints written, 1: added to
+	VisPointsBwdView view[MAX_BWD_VIEWS];
+};
+static_assert(sizeof(VisPointsBwdArgs) <= 4096, "kernel parameters are limited to 4 KB");
+void launch_visibility_points_bwd(const VisPointsBwdArgs& a, cudaStream_t s);
 
 // neighbour_reg.cu: the dynamic field's local-rigidity, rotation-similarity and isometry terms over [P,k] neighbour lists
 // (include/mgs_rasterizer.h, mgs_neighbour_reg).  The state (neighbour_reg_state_bytes, any alignment) holds the per-Gaussian

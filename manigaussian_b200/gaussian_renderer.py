@@ -26,7 +26,7 @@ from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
                          field_query_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
-                         rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
+                         visibility_views_backward_raw, rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
 MIN_DENOMINATOR = 1e-12  # gaussian_renderer/__init__.py:67; compiled into the kernel (activate.cu FEAT_EPS)
@@ -711,7 +711,43 @@ def lift_views(cameras, pts_xyz, rotations, scales, opacity, maps, view_ids=None
     return {"lifted": lifted, "weight": weight}
 
 
-def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_ids=None, antialiasing=False):
+class _PointVisibility(torch.autograd.Function):
+    """point_visibility(differentiable=True): uv, depth and transmittance as outputs of one node, differentiable in the points,
+    the cloud and the cameras' explicit inputs (_camera_inputs); in_view is not differentiable"""
+
+    @staticmethod
+    def forward(ctx, points, pts_xyz, rotations, scales, opacity, views, aa, cam_vm=None, cam_pm=None, cam_cp=None, cam_tf=None):
+        uv, depth, in_view, T, state = visibility_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(),
+                                                            rotations.detach(), 1.0, None, points.detach(), antialiasing=aa,
+                                                            tan_fov=cam_tf, keep_state=True)
+        in_view = in_view.bool()
+        ctx.state, ctx.opac_shape, ctx.camera = state, opacity.shape, cam_vm is not None
+        # T is an output: it reaches the backward through save_for_backward (an output kept on ctx is a reference cycle)
+        ctx.save_for_backward(points, pts_xyz, rotations, scales, opacity, T)
+        ctx.mark_non_differentiable(in_view)
+        return uv, depth, in_view, T
+
+    @staticmethod
+    def backward(ctx, g_uv, g_depth, _g_in_view, g_T):
+        points, pts_xyz, rotations, scales, opacity, T = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        want_points, want_cloud, want_cam = need[0], any(need[1:5]), ctx.camera and any(need[7:11])
+        if ctx.state is None or not (want_points or want_cloud or want_cam):  # Q = 0: nothing depends on the cloud
+            zero = lambda t, n: torch.zeros_like(t) if n else None  # noqa: E731
+            cam = None
+            if ctx.camera:
+                V = T.shape[0]
+                cam = tuple(torch.zeros(s, dtype=torch.float32, device=T.device) for s in ((V, 16), (V, 16), (V, 3), (V, 2)))
+            return (zero(points, need[0]), zero(pts_xyz, need[1]), zero(rotations, need[2]), zero(scales, need[3]),
+                    zero(opacity, need[4]), None, None, *_camera_outputs(ctx, cam, 7))
+        dpts, dmeans, dop, dscales, drot, cam = visibility_views_backward_raw(
+            ctx.state, points, pts_xyz, opacity, scales, rotations, 1.0, None, T, g_T, g_uv, g_depth, want_points=want_points,
+            want_cloud=(need[1], need[4], need[3], need[2]), camera_grads=want_cam)
+        return (dpts, dmeans, drot, dscales, dop.view(ctx.opac_shape) if dop is not None else None, None, None,
+                *_camera_outputs(ctx, cam if want_cam else None, 7))
+
+
+def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_ids=None, antialiasing=False, differentiable=False):
     """Project 3D points into every camera with occlusion (INTEGRATION.md §16).
 
     cameras / view_ids as `lift_views` (a `cameras.CameraBatch`, including device field-of-view cameras, or a sequence of
@@ -723,14 +759,25 @@ def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_
         transmittance[v, q] prod (1 - alpha_i) over the Gaussians of x's 16x16 tile that lie in front of it (depth < d), in the
                             blend's order, with the blend's alpha at the continuous uv, its 1/255 cut and its 1e-4 stop; 1 where
                             x is not in view.
-    At a pixel centre behind the scene the transmittance is the render's final_T (1 - alpha) bit for bit.  Inputs that require
-    grad are detached; the outputs are not differentiable.  Returns {"uv": [V,Q,2], "depth": [V,Q], "in_view": [V,Q] bool,
-    "transmittance": [V,Q]}; raises ValueError on a shape, dtype or device mismatch."""
+    At a pixel centre behind the scene the transmittance is the render's final_T (1 - alpha) bit for bit.  By default inputs
+    that require grad are detached and the outputs are not differentiable.  differentiable=True makes uv, depth and
+    transmittance outputs of one autograd node (include/mgs_rasterizer.h, mgs_visibility_views_backward), with the same
+    forward values: differentiable in points, pts_xyz, rotations, scales, opacity and, for a `cameras.CameraBatch` with a
+    learnable w2c or intr, its tensors.  The transmittance reaches the Gaussians of its product and uv (the tile, the depth cut,
+    the 1/255 cut and the stop are constants; dT/dalpha_i = -T / (1 - alpha_i) with the blend's convention at the 0.99 clamp),
+    uv and depth reach the point and the camera where the camera model's cull passes; in_view has no gradient.  Only the
+    gradients autograd asks for are computed.  Returns {"uv": [V,Q,2], "depth": [V,Q], "in_view": [V,Q] bool,
+    "transmittance": [V,Q]}; raises ValueError on a shape, dtype or device mismatch, and on a `differentiable` that is not a
+    bool (a tensor or a string would silently pick a path)."""
+    if not isinstance(differentiable, bool):
+        raise ValueError(f"differentiable: expected True or False, got {type(differentiable).__name__}")
     device = pts_xyz.device
+    batch = None
     if isinstance(cameras, CameraBatch):
         ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
         bg = _background((0.0, 0.0, 0.0), device)
         views = tuple(cameras.settings(i, bg, 0, False) for i in ids)
+        batch = _batch_cameras(cameras, ids) if (ids and differentiable) else None
     else:
         views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
     if not views:
@@ -753,6 +800,10 @@ def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_
     for name, t in [(n, x) for n, x, _ in inputs] + [("points", points)]:
         if t.device != device or not t.is_cuda:
             raise ValueError(f"{name}: expected a CUDA tensor on {device}, got {t.device}")
+    if differentiable:
+        uv, depth, in_view, T = _PointVisibility.apply(points, pts_xyz, rotations, scales, opacity, views, aa,
+                                                       *_camera_inputs(views, batch=batch))
+        return {"uv": uv, "depth": depth, "in_view": in_view, "transmittance": T}
     uv, depth, in_view, T = visibility_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0,
                                                  None, points.detach(), antialiasing=aa)
     return {"uv": uv, "depth": depth, "in_view": in_view.bool(), "transmittance": T}

@@ -1122,13 +1122,15 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
 
 
 def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, points, antialiasing=False,
-                         tan_fov=None, debug=False, ortho=None, fisheye=None, distortion=None):
+                         tan_fov=None, debug=False, ortho=None, fisheye=None, distortion=None, keep_state=False):
     """Project Q points into every view with occlusion (C ABI mgs_visibility_views): per view and point the screen position
     uv [V,Q,2] (pixel centres at integers), the view-space depth [V,Q], in_view [V,Q] (uint8) and the transmittance [V,Q] the
     cloud leaves in front of the point, with the blend's own tile lists, depth order, thresholds and early stop.  `points`
     [Q,3] fp32 on the cloud's device.  `views`, `antialiasing`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in
     lift_views_raw; the binning state is sized from the same capacity table, so a steady-state call reads nothing back to the
-    host and can be captured in a CUDA graph.  Returns (uv, depth, in_view, T); none is differentiable."""
+    host and can be captured in a CUDA graph.  Returns (uv, depth, in_view, T); none is differentiable.  `keep_state`: also
+    return, fifth, what visibility_views_backward_raw needs (the views' state buffers, point scratch and streams; None for
+    Q = 0)."""
     L = _b.lib()
     dev = means3D.device
     if not means3D.is_cuda:
@@ -1151,7 +1153,7 @@ def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modif
     in_view = torch.empty((V, Q), dtype=torch.uint8, device=dev)
     T = torch.empty((V, Q), dtype=torch.float32, device=dev)
     if Q == 0:
-        return uv, depth, in_view, T
+        return (uv, depth, in_view, T) + ((None,) if keep_state else ())
     with torch.cuda.device(dev):
         if not capturing:
             _poll_status()
@@ -1192,7 +1194,59 @@ def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modif
                                         _ptr(rotations), _ptr(cov3D_precomp), _ptr(uv), _ptr(depth), _ptr(in_view), _ptr(T),
                                         int(bool(debug)), main.cuda_stream), "mgs_visibility_views")
         _track_status(outs, keys, status, main, not capturing)
-    return uv, depth, in_view, T
+    if not keep_state:
+        return uv, depth, in_view, T
+    state = dict(arr=arr, keep=keep, tf=tf, lens=(oarr, farr, dcarr), P=P, Q=Q, aa=bool(antialiasing), debug=bool(debug),
+                 colors=colors, streams=streams)
+    return uv, depth, in_view, T, state
+
+
+def visibility_views_backward_raw(state, points, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, T, grad_T,
+                                  grad_uv, grad_depth, want_points=True, want_cloud=True, camera_grads=False):
+    """Backward of visibility_views_raw (C ABI mgs_visibility_views_backward).  `state`: the fifth result of that call with
+    keep_state=True; points, the cloud and `T` (its transmittance) as given to and returned by it.  grad_T [V,Q], grad_uv
+    [V,Q,2] and grad_depth [V,Q]: the cotangents, each None for none.  Returns (dL_dpoints [Q,3], dL_dmeans3D [P,3],
+    dL_dopacity [P,1], dL_dscales [P,3], dL_drotations [P,4], camera), each gradient None where not wanted: `want_points`, and
+    `want_cloud`, a bool or four in that order (scales and rotations are None without scales too).  camera is None, or with
+    camera_grads=True (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16], dL_dcampos [V,3], dL_dtan_fov [V,2], None without a
+    device field of view).  Nothing is read back to the host."""
+    L = _b.lib()
+    dev = means3D.device
+    P, Q = state["P"], state["Q"]
+    arr = state["arr"]
+    V = len(arr)
+    means3D, opacity, scales, rotations, cov3D_precomp, points, T = (
+        _prep(x, dev) for x in (means3D, opacity, scales, rotations, cov3D_precomp, points, T))
+    grad_T, grad_uv, grad_depth = (_prep(x, dev) if x is not None else None for x in (grad_T, grad_uv, grad_depth))
+    opts = dict(dtype=torch.float32, device=dev)
+    main = torch.cuda.current_stream(dev)
+    dpts = torch.empty((Q, 3), **opts) if want_points else None
+    has_sr = scales is not None and scales.numel() != 0
+    want = tuple(want_cloud) if isinstance(want_cloud, (tuple, list)) else (bool(want_cloud),) * 4
+    cloud = tuple(torch.empty(shape, **opts) if (w and (has_sr or i < 2)) else None
+                  for i, (w, shape) in enumerate(zip(want, ((P, 3), (P, 1), (P, 3), (P, 4)))))
+    tf = state["tf"]
+    cam, carr = None, None
+    if camera_grads:
+        cam = (torch.empty((V, 16), **opts), torch.empty((V, 16), **opts), torch.empty((V, 3), **opts),
+               torch.empty((V, 2), **opts) if tf is not None else None)
+        carr = (_b.ViewCameraGrad * V)()
+        for v in range(V):
+            carr[v].dL_dviewmatrix = cam[0].data_ptr() + 64 * v
+            carr[v].dL_dprojmatrix = cam[1].data_ptr() + 64 * v
+            carr[v].dL_dcampos = cam[2].data_ptr() + 12 * v
+    iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+    scratch = torch.empty((V, int(L.mgs_visibility_backward_scratch_bytes(P, Q))), dtype=torch.uint8, device=dev)
+    for v in range(V):
+        arr[v].dL_dmean2D = scratch[v].data_ptr()
+    oarr, farr, dcarr = state["lens"]
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_visibility_views_backward(
+            V, arr, int(state["aa"]), iarr, oarr, farr, dcarr, P, 0, 0, Q, _ptr(points), _ptr(means3D), None, _ptr(state["colors"]),
+            _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(T), _ptr(grad_T),
+            _ptr(grad_uv), _ptr(grad_depth), _ptr(dpts), _ptr(cloud[0]), _ptr(cloud[1]), _ptr(cloud[2]), _ptr(cloud[3]), None,
+            carr, int(state["debug"]), main.cuda_stream), "mgs_visibility_views_backward")
+    return (dpts,) + tuple(cloud) + (cam,)
 
 
 def _fill_depth_mask(wd, depth_mask, v, scale=None):
