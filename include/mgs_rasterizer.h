@@ -1409,6 +1409,57 @@ int mgs_visibility_views_backward(
 	const mgs_view_camera_grad* cam, int debug, void* join_stream);
 
 /*
+ * Camera rays (no reference counterpart): the inverse of the map the projection applies to a mean (screen_mean, as in point
+ * visibility), from a pixel to the world points it is the image of.  For view v and pixel position (u, v) (pixel centres at
+ * integers), the ray is the set of points p whose screen position is (u, v); each is labelled by its view-space depth z = t.z,
+ * the quantity the depth plane holds, and for every camera model that set is the line
+ *   p(z) = origin + z direction,   direction's view-space z component exactly 1 (not unit length),
+ * so origin + depth direction unprojects a z-depth image, or the renderer's own depth / alpha.
+ *   - Pinhole and orthographic: with (nx, ny) = ((2u + 1) / W - 1, (2v + 1) / H - 1) (ndc2pix's inverse) and Pk, Vk the rows
+ *     of projmatrix and viewmatrix, the rows (P0 - nx P3) (p, 1) = nx 1e-7, (P1 - ny P3) (p, 1) = ny 1e-7 and V2 (p, 1) = z:
+ *     a 3x3 system A p = b + z e3, so origin = A^-1 b and direction = A^-1 e3.  An off-centre principal point baked into
+ *     projmatrix and the orthographic origin that moves with the pixel are covered.  Valid where det A is finite and non-zero.
+ *   - Fisheye: (xd, yd) = ((u - cx) / fx, (v - cy) / fy), theta_d = |(xd, yd)|, theta in [0, theta_max] the root of
+ *     theta rho(theta) = theta_d (safeguarded Newton, FISHEYE_RAY_ITERS = 16 steps at most; monotone there by
+ *     cameras.fisheye_theta_max), t = z (tan theta xd / theta_d, tan theta yd / theta_d, 1), p = Rv^T (t - tv).  The axis pixel
+ *     takes tan(theta) / theta from its series.  Valid iff theta_d <= theta_max rho(theta_max) (and tan theta finite, >= 0).
+ *   - Distorted pinhole: Newton's method with Dd on distort(x, y) = (xd, yd) from (xd, yd), DIST_RAY_ITERS = 20 steps at
+ *     most; t = z (x, y, 1).  Valid iff the iterate passes the projection's cull (r2 <= r_max^2, det Dd > 0) and
+ *     |distort(x, y) - (xd, yd)| <= 1e-6 (1 + |(xd, yd)|): fp32 evaluates distort at |x| <~ 2 to a few ulps of 2.4e-7, so a
+ *     converged iterate passes it; at fx = 500 px the bound is 5e-4 px.
+ *   - fx = W / (2 tan_fovx), fy = H / (2 tan_fovy) (or the device field of view, as for the projection).
+ *   - For a valid ray and z > NEAR_Z, p(z) passes the model's cull and projects back to (u, v) up to fp32 rounding.  An invalid
+ *     ray (the pixel is not the image of points the projection keeps, or is not finite) has origin and direction NaN.
+ * Arguments: views, intr, ortho, fisheye and distortion as mgs_visibility_views takes them; of each view only viewmatrix,
+ * projmatrix (both required), tan_fovx, tan_fovy, width and height are read.  pixels [V,Q,2], or NULL for every pixel centre
+ * of the W x H grid, ray i at (i % W, i / W): then Q must equal width * height of every view.  Outputs out_origin [V,Q,3],
+ * out_direction [V,Q,3] and out_valid [V,Q] (uint8 0/1), all required with Q > 0.  One stream for every view.
+ * Backward, by implicit differentiation of those maps (the 3x3 solve, the inverse of the fisheye forward Jacobian, Dd^-1): the
+ * forward's inputs unchanged, the cotangents dL_dorigin and dL_ddirection ([V,Q,3], each NULL for zero), and the outputs
+ * dL_dpixels [V,Q,2] (NULL to skip; needs pixels) and, per view through `cam` (one mgs_view_camera_grad per view, or NULL),
+ * dL_dviewmatrix, dL_dprojmatrix (pinhole and orthographic only) and dL_dcampos (always 0), and through intr dL_dtan_fov
+ * (fisheye and distorted views: fx enters no pinhole or orthographic term, as in screen_mean).  A view with a camera output
+ * needs its entry's scratch of mgs_camera_rays_scratch_bytes(Q) bytes.  The principal point, the coefficients, theta_max,
+ * r_max and NEAR_Z are constants, valid has no gradient, and an invalid ray's cotangents are ignored (its pixel gradient is
+ * 0).  Every output is written.  The camera sums are fixed-order partial sums (one row per CTA of RAYS_THREADS rays, summed
+ * by the camera-gradient reduce): the backward is deterministic.
+ * Nothing allocates, blocks or reads back to the host: both calls can be captured in a CUDA graph.  Q = 0 returns 0 and
+ * enqueues nothing (no output is written).  The ABI version stays 300.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0 or views
+ * NULL, the camera-model errors of the _distorted calls, Q < 0, a view without its matrices or with a size <= 0, pixels NULL
+ * with Q != width * height of a view, a NULL output (forward, Q > 0), dL_dpixels without pixels, and a camera output without
+ * its entry's scratch.
+ */
+size_t mgs_camera_rays_scratch_bytes(int Q);
+int mgs_camera_rays(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int Q, const float* pixels,
+	float* out_origin, float* out_direction, uint8_t* out_valid, int debug, void* stream);
+int mgs_camera_rays_backward(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int Q, const float* pixels,
+	const float* dL_dorigin, const float* dL_ddirection, float* dL_dpixels, const mgs_view_camera_grad* cam, int debug,
+	void* stream);
+
+/*
  * k nearest neighbours (no reference counterpart; simple-knn's distCUDA2 is the mean of the first three d2 of each point):
  * for each of Q queries, its k nearest of N reference points by the fp32 squared distance
  *   d2 = (qx - px)^2 + (qy - py)^2 + (qz - pz)^2,

@@ -253,6 +253,15 @@ def lib():
         vp, vp, vp, vp,                  # out_T dL_dT dL_duv dL_ddepth
         vp, vp, vp, vp, vp, vp,          # dL_dpoints dL_dmean3D dL_dopacity dL_dscale dL_drot dL_dcov3D
         C.POINTER(ViewCameraGrad), i, vp]  # cam debug join_stream
+    L.mgs_camera_rays_scratch_bytes.restype = C.c_size_t
+    L.mgs_camera_rays_scratch_bytes.argtypes = [C.c_int]
+    L.mgs_camera_rays.restype = C.c_int
+    L.mgs_camera_rays.argtypes = [i, C.POINTER(View), C.POINTER(ViewIntrinsics),  # V views intr
+                                  C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
+                                  i, vp, vp, vp, vp, i, vp]  # Q pixels out_origin out_direction out_valid debug stream
+    L.mgs_camera_rays_backward.restype = C.c_int
+    L.mgs_camera_rays_backward.argtypes = L.mgs_camera_rays.argtypes[:8] + [
+        vp, vp, vp, C.POINTER(ViewCameraGrad), i, vp]  # dL_dorigin dL_ddirection dL_dpixels cam debug stream
     L.mgs_knn_state_bytes.restype = C.c_size_t
     L.mgs_knn_state_bytes.argtypes = [C.c_int, C.c_int]
     L.mgs_knn.restype = C.c_int
@@ -331,6 +340,7 @@ EXPORTED_SYMBOLS = (
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_visibility_scratch_bytes", "mgs_visibility_views",
     "mgs_visibility_backward_scratch_bytes", "mgs_visibility_views_backward",
+    "mgs_camera_rays_scratch_bytes", "mgs_camera_rays", "mgs_camera_rays_backward",
     "mgs_knn_state_bytes", "mgs_knn",
     "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
     "mgs_activate", "mgs_activate_backward",

@@ -1680,6 +1680,105 @@ int mgs_visibility_views_backward(
 	return 0;
 }
 
+}  // extern "C"
+
+namespace mgs {
+// the argument checks shared by mgs_camera_rays and its backward; the views' camera models into lens
+static int check_rays(int V, const mgs_view* views, const int* ortho, const mgs_view_fisheye* fisheye,
+	const mgs_view_distortion* distortion, int Q, const float* pixels, std::vector<Lens>& lens)
+{
+	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
+	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
+	if (Q < 0) return fail(MGS_ERR_INVALID_ARG, "Q must be >= 0");
+	for (int v = 0; v < V; v++) {
+		const mgs_view& w = views[v];
+		if (!w.viewmatrix || !w.projmatrix) return fail(MGS_ERR_INVALID_ARG, "view: matrices are required");
+		if (w.width <= 0 || w.height <= 0) return fail(MGS_ERR_INVALID_ARG, "view: bad size");
+		if (!pixels && Q > 0 && (long long)w.width * w.height != Q)
+			return fail(MGS_ERR_INVALID_ARG, "pixels NULL (every pixel centre): Q must equal width * height of every view");
+	}
+	return 0;
+}
+// the launch over views [v0, v0 + MAX_BWD_VIEWS) of a call with Q rays per view (outputs and cotangents left NULL)
+static RaysArgs rays_args(const mgs_view* views, const mgs_view_intrinsics* intr, const std::vector<Lens>& lens, int v0, int V,
+	int Q, const float* pixels)
+{
+	RaysArgs a{};
+	a.V = std::min(V - v0, (int)MAX_BWD_VIEWS);
+	a.N = Q;
+	a.grid_w = views[v0].width;
+	a.pixels = pixels ? pixels + 2 * (size_t)v0 * Q : nullptr;
+	for (int u = 0; u < a.V; u++) {
+		const mgs_view& w = views[v0 + u];
+		a.cam[u] = flow_cam(w, device_fov(intr, v0 + u), lens[v0 + u], w.viewmatrix, w.projmatrix);
+	}
+	return a;
+}
+}  // namespace mgs
+
+extern "C" {
+
+size_t mgs_camera_rays_scratch_bytes(int Q)
+{
+	return (size_t)ceil_div(std::max(Q, 0), RAYS_THREADS) * (CAM_TERMS + CAM_INTR_TERMS) * sizeof(float);
+}
+
+int mgs_camera_rays(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int Q, const float* pixels,
+	float* out_origin, float* out_direction, uint8_t* out_valid, int debug, void* stream)
+{
+	std::vector<Lens> lens;
+	if (check_rays(V, views, ortho, fisheye, distortion, Q, pixels, lens) < 0) return MGS_ERR_INVALID_ARG;
+	if (Q == 0) return 0;
+	if (!out_origin || !out_direction || !out_valid)
+		return fail(MGS_ERR_INVALID_ARG, "out_origin, out_direction and out_valid are required");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
+		RaysArgs a = rays_args(views, intr, lens, v0, V, Q, pixels);
+		const size_t o = (size_t)v0 * Q;
+		a.origin = out_origin + 3 * o; a.direction = out_direction + 3 * o; a.valid = out_valid + o;
+		launch_rays_fwd(a, st);
+		MGS_STAGE("camera_rays");
+	}
+	return 0;
+}
+
+int mgs_camera_rays_backward(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int Q, const float* pixels,
+	const float* dL_dorigin, const float* dL_ddirection, float* dL_dpixels, const mgs_view_camera_grad* cam, int debug,
+	void* stream)
+{
+	std::vector<Lens> lens;
+	if (check_rays(V, views, ortho, fisheye, distortion, Q, pixels, lens) < 0) return MGS_ERR_INVALID_ARG;
+	if (dL_dpixels && !pixels) return fail(MGS_ERR_INVALID_ARG, "dL_dpixels needs pixels (the grid's pixel centres are constants)");
+	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
+	if (Q == 0) return 0;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const int nrows = ceil_div(Q, RAYS_THREADS);
+	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
+		RaysArgs a = rays_args(views, intr, lens, v0, V, Q, pixels);
+		const size_t o = (size_t)v0 * Q;
+		a.dL_dorigin = dL_dorigin ? dL_dorigin + 3 * o : nullptr;
+		a.dL_ddirection = dL_ddirection ? dL_ddirection + 3 * o : nullptr;
+		a.dL_dpixels = dL_dpixels ? dL_dpixels + 2 * o : nullptr;
+		CamReduceArgs cr{};
+		for (int u = 0; u < a.V; u++) {
+			const int v = v0 + u;
+			if (!camera_on(cam, intr, v)) continue;
+			float* dtf = tan_fov_grad(intr, v);
+			a.cam_rows[u] = cam[v].scratch;
+			a.intr_rows[u] = dtf ? cam[v].scratch + (size_t)nrows * CAM_TERMS : nullptr;
+			cr.view[cr.V++] = CamReduceView{ a.cam_rows[u], nrows, cam[v].dL_dviewmatrix, cam[v].dL_dprojmatrix, cam[v].dL_dcampos,
+				a.intr_rows[u], dtf };
+		}
+		if (!a.dL_dpixels && cr.V == 0) continue;
+		launch_rays_bwd(a, st);
+		if (cr.V > 0) launch_camera_grad_reduce(cr, st);
+		MGS_STAGE("camera_rays_backward");
+	}
+	return 0;
+}
+
 int mgs_backward_views(
 	int V, const mgs_view* views,
 	int P, int D, int M, int F,

@@ -583,6 +583,28 @@ struct VisPointsBwdArgs {
 static_assert(sizeof(VisPointsBwdArgs) <= 4096, "kernel parameters are limited to 4 KB");
 void launch_visibility_points_bwd(const VisPointsBwdArgs& a, cudaStream_t s);
 
+// rays.cu: the ray of each pixel of up to MAX_BWD_VIEWS views per launch (include/mgs_rasterizer.h, mgs_camera_rays), one
+// thread per (view, pixel): blockIdx.y is the view of the launch, CTAs of RAYS_THREADS pixels.  Every pointer is that of the
+// launch's first view; view u's rays start at u N.
+constexpr int RAYS_THREADS = 128;
+struct RaysArgs {
+	int V, N;                    // views of the launch, rays per view
+	int grid_w;                  // pixels NULL: ray i is pixel centre (i % grid_w, i / grid_w)
+	const float* pixels;         // [V,N,2] or NULL
+	float* origin;               // forward: [V,N,3]
+	float* direction;            // forward: [V,N,3]
+	uint8_t* valid;              // forward: [V,N]
+	const float* dL_dorigin;     // backward: [V,N,3] or NULL
+	const float* dL_ddirection;  // backward: [V,N,3] or NULL
+	float* dL_dpixels;           // backward: [V,N,2] or NULL
+	float* cam_rows[MAX_BWD_VIEWS];   // backward: view u's [CTAs][CAM_TERMS] or NULL (the launcher picks CAM when any is set)
+	float* intr_rows[MAX_BWD_VIEWS];  // backward: view u's [CTAs][CAM_INTR_TERMS] or NULL
+	FlowCam cam[MAX_BWD_VIEWS];
+};
+static_assert(sizeof(RaysArgs) <= 4096, "kernel parameters are limited to 4 KB");
+void launch_rays_fwd(const RaysArgs& a, cudaStream_t s);
+void launch_rays_bwd(const RaysArgs& a, cudaStream_t s);
+
 // neighbour_reg.cu: the dynamic field's local-rigidity, rotation-similarity and isometry terms over [P,k] neighbour lists
 // (include/mgs_rasterizer.h, mgs_neighbour_reg).  The state (neighbour_reg_state_bytes, any alignment) holds the per-Gaussian
 // records and R_i the forward writes, its CTA partials and the backward's gradient rows; the backward reads the records of

@@ -24,7 +24,8 @@ import torch
 from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, field_query_backward_raw,
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, camera_rays_backward_raw,
+                         camera_rays_raw, field_query_backward_raw,
                          field_query_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
                          visibility_views_backward_raw, rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
@@ -807,6 +808,87 @@ def point_visibility(cameras, points, pts_xyz, rotations, scales, opacity, view_
     uv, depth, in_view, T = visibility_views_raw(views, pts_xyz.detach(), opacity.detach(), scales.detach(), rotations.detach(), 1.0,
                                                  None, points.detach(), antialiasing=aa)
     return {"uv": uv, "depth": depth, "in_view": in_view.bool(), "transmittance": T}
+
+
+class _CameraRays(torch.autograd.Function):
+    """camera_rays with a pixel or camera tensor that requires grad: origin and direction as outputs of one node,
+    differentiable in the pixels and the cameras' explicit inputs (_camera_inputs); valid is not differentiable"""
+
+    @staticmethod
+    def forward(ctx, pixels, views, shape, cam_vm=None, cam_pm=None, cam_cp=None, cam_tf=None):
+        origin, direction, valid = camera_rays_raw(views, pixels.detach() if pixels is not None else None,
+                                                   tan_fov=cam_tf.detach() if cam_tf is not None else None)
+        valid = valid.bool().view(shape)
+        ctx.views, ctx.camera = views, cam_vm is not None
+        ctx.save_for_backward(pixels, cam_tf)
+        ctx.mark_non_differentiable(valid)
+        return origin.view(shape + (3,)), direction.view(shape + (3,)), valid
+
+    @staticmethod
+    def backward(ctx, g_origin, g_direction, _g_valid):
+        pixels, tf = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        want_cam = ctx.camera and any(need[3:7])
+        V = len(ctx.views)
+        flat = lambda g: g.reshape(V, -1, 3) if g is not None else None  # noqa: E731
+        dpix, cam = camera_rays_backward_raw(ctx.views, pixels.detach() if pixels is not None else None, flat(g_origin),
+                                             flat(g_direction), tan_fov=tf.detach() if tf is not None else None,
+                                             want_pixels=need[0], camera_grads=want_cam)
+        return (dpix if need[0] else None, None, None, *_camera_outputs(ctx, cam if want_cam else None, 3))
+
+
+def camera_rays(cameras, pixels=None, view_ids=None):
+    """The ray of each pixel through every camera's own lens model (INTEGRATION.md §19): the inverse of the map the renderer
+    projects with, for all four camera models (include/mgs_rasterizer.h, mgs_camera_rays).
+
+    cameras / view_ids as `point_visibility` (a `cameras.CameraBatch`, including a learnable w2c or intr, or a sequence of
+    GaussianRasterizationSettings of any of the four camera models, mixed).  pixels: None for every pixel centre of the
+    views' shared H x W image, or [V,Q,2] fp32 pixel positions (u, v) on the cameras' device, pixel centres at integers.  For
+    view v and a pixel, the world points p(z) = origin + z * direction are those whose screen position is the pixel, z their
+    view-space depth: direction's view-space z component is 1 (it is not unit length), so `origin + depth[..., None] *
+    direction` unprojects a z-depth image, or the renderer's own depth / alpha.  valid is False where the pixel is not the image
+    of points the projection keeps (past a fisheye's theta_max, a distorted lens's r_max or fold, or a non-finite pixel); origin
+    and direction are NaN there.  Returns {"origin", "direction": [V,H,W,3] or [V,Q,3], "valid": [V,H,W] or [V,Q] bool}.
+    One autograd node exactly when pixels or a camera tensor requires grad: origin and direction are then differentiable in
+    the pixels, the view and projection matrices and the field of view (fisheye and distorted views), by implicit
+    differentiation of the lens maps; the principal point and distortion coefficients are constants.  Raises ValueError on a
+    shape, dtype or device mismatch, and on the grid with views of different sizes."""
+    batch = None
+    if isinstance(cameras, CameraBatch):
+        ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
+        dev = cameras.world_view_transform.device
+        bg = _background((0.0, 0.0, 0.0), dev)
+        views = tuple(cameras.settings(i, bg, 0, False) for i in ids)
+        batch = _batch_cameras(cameras, ids) if ids else None
+    else:
+        views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+    if not views:
+        raise ValueError("camera_rays needs at least one view")
+    device = torch.as_tensor(views[0].viewmatrix).device
+    for v, s in enumerate(views):
+        if not (torch.is_tensor(s.viewmatrix) and s.viewmatrix.is_cuda and s.viewmatrix.device == device):
+            raise ValueError(f"cameras[{v}]: expected a CUDA viewmatrix on {device}")
+    V = len(views)
+    if pixels is None:
+        sizes = {(int(s.image_height), int(s.image_width)) for s in views}
+        if len(sizes) != 1:
+            raise ValueError(f"pixels=None (every pixel centre) needs views of one size, got {sorted(sizes)}")
+        shape = (V,) + sizes.pop()
+    else:
+        if not torch.is_tensor(pixels) or pixels.dim() != 3 or tuple(pixels.shape[::2]) != (V, 2):
+            raise ValueError(f"pixels: expected [{V},Q,2], got {tuple(pixels.shape) if torch.is_tensor(pixels) else type(pixels)}")
+        if pixels.dtype != torch.float32:
+            raise ValueError(f"pixels: expected float32, got {pixels.dtype}")
+        if pixels.device != device:
+            raise ValueError(f"pixels: expected a CUDA tensor on {device}, got {pixels.device}")
+        shape = (V, int(pixels.shape[1]))
+    cam = _camera_inputs(views, batch=batch)
+    if (pixels is not None and pixels.requires_grad) or cam[0] is not None:
+        origin, direction, valid = _CameraRays.apply(pixels, views, shape, *cam)
+        return {"origin": origin, "direction": direction, "valid": valid}
+    tf = cam[3].detach() if cam[3] is not None else None
+    origin, direction, valid = camera_rays_raw(views, pixels, tan_fov=tf)
+    return {"origin": origin.view(shape + (3,)), "direction": direction.view(shape + (3,)), "valid": valid.bool().view(shape)}
 
 
 def knn(points, k, queries=None):

@@ -1249,6 +1249,86 @@ def visibility_views_backward_raw(state, points, means3D, opacity, scales, rotat
     return (dpts,) + tuple(cloud) + (cam,)
 
 
+def _ray_call(views, pixels, tan_fov, ortho, fisheye, distortion):
+    """(device, Q, pixels or None, mgs_view array, intrinsics array or None, lens arrays, tensors to keep alive) of a camera_rays
+    call: every view's viewmatrix, projmatrix, field of view and size"""
+    dev = pixels.device if pixels is not None else torch.as_tensor(views[0].viewmatrix).device
+    if not dev.type == "cuda":
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    V = len(views)
+    Q = int(pixels.shape[1]) if pixels is not None else int(views[0].image_width) * int(views[0].image_height)
+    pixels = _prep(pixels, dev) if pixels is not None else None
+    arr = (_b.View * V)()
+    keep = [pixels]
+    for v, s in enumerate(views):
+        vm, pm = _prep(s.viewmatrix, dev), _prep(s.projmatrix, dev)
+        w = arr[v]
+        w.viewmatrix, w.projmatrix = _ptr(vm), _ptr(pm)
+        w.tan_fovx, w.tan_fovy = _host_tan(s.tanfovx), _host_tan(s.tanfovy)
+        w.width, w.height = int(s.image_width), int(s.image_height)
+        keep += [vm, pm]
+    tf = _device_fov(views, tan_fov, dev)
+    keep.append(tf)
+    return dev, Q, pixels, arr, tf, _lens_arrays(views, ortho, fisheye, distortion), keep
+
+
+def camera_rays_raw(views, pixels=None, tan_fov=None, ortho=None, fisheye=None, distortion=None, debug=False):
+    """The ray of each pixel of every view (C ABI mgs_camera_rays): the world points p(z) = origin + z direction whose screen
+    position under the view's camera model is the pixel, z their view-space depth (direction's view-space z is 1).  pixels
+    [V,Q,2] fp32 on the views' device (pixel centres at integers), or None for every pixel centre of the views' shared
+    W x H grid, ray i at (i % W, i // W).  `views`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in
+    visibility_views_raw.  Returns (origin [V,N,3], direction [V,N,3], valid [V,N] uint8), origin and direction NaN where
+    invalid; not differentiable (camera_rays_backward_raw is the backward).  Nothing is read back to the host."""
+    L = _b.lib()
+    dev, Q, pixels, arr, tf, (oarr, farr, dcarr), keep = _ray_call(views, pixels, tan_fov, ortho, fisheye, distortion)
+    V = len(views)
+    origin = torch.empty((V, Q, 3), dtype=torch.float32, device=dev)
+    direction = torch.empty((V, Q, 3), dtype=torch.float32, device=dev)
+    valid = torch.empty((V, Q), dtype=torch.uint8, device=dev)
+    iarr = _intrinsics_array(tf, None) if tf is not None else None
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_camera_rays(V, arr, iarr, oarr, farr, dcarr, Q, _ptr(pixels), _ptr(origin), _ptr(direction), _ptr(valid),
+                                   int(bool(debug)), torch.cuda.current_stream(dev).cuda_stream), "mgs_camera_rays")
+    return origin, direction, valid
+
+
+def camera_rays_backward_raw(views, pixels, grad_origin, grad_direction, tan_fov=None, ortho=None, fisheye=None, distortion=None,
+                             want_pixels=True, camera_grads=False, debug=False):
+    """Backward of camera_rays_raw (C ABI mgs_camera_rays_backward) with the same views, pixels and camera models.
+    grad_origin / grad_direction [V,N,3]: the cotangents, each None for zero.  Returns (dL_dpixels [V,Q,2] or None (with
+    want_pixels and pixels), camera): camera is None, or with camera_grads=True (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16],
+    dL_dcampos [V,3] (zeros), dL_dtan_fov [V,2], None without a device field of view).  Deterministic; nothing is read back
+    to the host."""
+    L = _b.lib()
+    dev, Q, pixels, arr, tf, (oarr, farr, dcarr), keep = _ray_call(views, pixels, tan_fov, ortho, fisheye, distortion)
+    V = len(views)
+    opts = dict(dtype=torch.float32, device=dev)
+    go, gd = (_prep(g, dev) if g is not None else None for g in (grad_origin, grad_direction))
+    dpix = torch.empty((V, Q, 2), **opts) if (want_pixels and pixels is not None) else None
+    cam, carr = None, None
+    if camera_grads:
+        cam = (torch.empty((V, 16), **opts), torch.empty((V, 16), **opts), torch.empty((V, 3), **opts),
+               torch.empty((V, 2), **opts) if tf is not None else None)
+        rows = int(L.mgs_camera_rays_scratch_bytes(Q))
+        scratch = torch.empty((V, max(rows, 4) // 4), **opts)
+        carr = (_b.ViewCameraGrad * V)()
+        for v in range(V):
+            carr[v].dL_dviewmatrix = cam[0].data_ptr() + 64 * v
+            carr[v].dL_dprojmatrix = cam[1].data_ptr() + 64 * v
+            carr[v].dL_dcampos = cam[2].data_ptr() + 12 * v
+            carr[v].scratch = scratch[v].data_ptr()
+        keep.append(scratch)
+        if Q == 0:  # the call enqueues nothing: the gradients of no rays are zero
+            for t in cam:
+                if t is not None:
+                    t.zero_()
+    iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_camera_rays_backward(V, arr, iarr, oarr, farr, dcarr, Q, _ptr(pixels), _ptr(go), _ptr(gd), _ptr(dpix), carr,
+                                            int(bool(debug)), torch.cuda.current_stream(dev).cuda_stream), "mgs_camera_rays_backward")
+    return dpix, cam
+
+
 def _fill_depth_mask(wd, depth_mask, v, scale=None):
     """Fills view v's mgs_view_depth_mask `wd` from a `depth_mask` tuple of rasterize_views_raw (and, for the backward, the
     upstream gradients `scale` [V,2])."""
