@@ -1155,7 +1155,8 @@ int mgs_lift_views_distorted(
  * col3 + px col4 + py col5 + col6; the quads live where the normal plane's do, so the geometry state must be sized by
  * mgs_geometry_state_bytes_normal and the backward scratch by mgs_backward_scratch_bytes_normal.
  * Backward: the depth cotangent g (including the depth head's) enters the blend as the column cotangents (g, g px, g py, g),
- * which makes dL/dalpha that of the planar depth; the blend returns dL/d(a, b, e) per Gaussian and view, and the per-Gaussian
+ * which makes dL/dalpha that of the planar depth; the blend returns dL/d(a, b, e) per Gaussian and view (formed relative to
+ * each Gaussian's screen mean, so its precision does not depend on the pixel coordinates), and the per-Gaussian
  * stage chains them through e to mu (added to dL/dmean2D in its convention), through Q (added to the conic's gradient) and
  * through k to Sigma_c, J and the third row of Rv, and from there to means3D, scales, rotations (or cov3D), the camera
  * gradients and dL_dtan_fov for all four models.  The median depth's cotangent reaches z, a, b and mu of its contributor.
@@ -1584,6 +1585,11 @@ int mgs_activate_backward(int P, int F,
  *             ties by tile id: the launch order of the blend CTAs; no reference counterpart), "block_count" u32[8T]
  *             (entries of block s's list of tile t at 8 t + s), "block_nwalk" u32[8T] (block-list entries up to and
  *             including the block's last contributor, written by the forward blend for blocks with a pixel in the image)
+ *   scratch : a view's blend_scratch after a backward, P_or_R_or_width = P: "gb" f32[P][12], the blend-stage record of each
+ *             Gaussian {dL/dmean2D x, y, dL/dconic a, b | c, dL/dopacity, dL/dcolour r, g | b, dL/ddepth, 0, 0} (dL/dmean2D
+ *             with the 0.5 W / 0.5 H factors, dL/dconic b the half-weight off-diagonal term), "gn" f32[P][4] (scratch sized
+ *             by mgs_backward_scratch_bytes_normal only: the normal plane's dL/dn {x, y, z, 0}, or planar depth's quad
+ *             gradient, or flow's)
  * Returns 0, or MGS_ERR_INVALID_ARG for an unknown name.
  */
 int mgs_state_array(const char* which_state, const char* name, char* state, int P_or_R_or_width, int height,

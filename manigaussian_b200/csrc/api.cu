@@ -356,6 +356,12 @@ struct ViewState {
 	float4* nrm;
 	float* gn;
 };
+// the blend-stage records in a view's blend_scratch: gb [P, GB_STRIDE], then (buffers sized by the _normal queries) gn [P,4]
+static void carve_scratch(char* sc, int P, float*& gb, float*& gn)
+{
+	obtain(sc, gb, (size_t)P * GB_STRIDE);
+	obtain(sc, gn, (size_t)P * 4);
+}
 static ViewState carve_view(const mgs_view& w, int P)
 {
 	ViewState s;
@@ -366,9 +372,8 @@ static ViewState carve_view(const mgs_view& w, int P)
 	s.geom = GeomState::carve(g, (size_t)P);
 	s.img = ImageState::carve(i, (size_t)w.width * w.height, s.T);
 	s.bin = BinState::carve(b, (size_t)w.binning_capacity);
-	obtain(sc, s.gb, (size_t)P * GB_STRIDE);
 	obtain(g, s.nrm, (size_t)P);
-	obtain(sc, s.gn, (size_t)P * 4);
+	carve_scratch(sc, P, s.gb, s.gn);
 	return s;
 }
 
@@ -666,7 +671,7 @@ static int enqueue_blend_bwd(const Cloud& c, const mgs_view& w, float* dL_dfeatu
 	if (c.planar) MGS_CUDA(cudaMemsetAsync(s.gn, 0, (size_t)c.P * 4 * sizeof(float), st));
 	if (med && med->dL_dpix_median_depth) {
 		launch_median_depth_bwd(w.width * w.height, med->median_id, med->dL_dpix_median_depth, s.gb, st, w.width,
-			c.planar ? s.gn : nullptr);
+			c.planar ? s.gn : nullptr, s.geom.means2D);
 		MGS_STAGE("median_depth_bwd");
 	}
 	BlendArgs ba = blend_args(s, w, F, c.feature);
@@ -2589,6 +2594,10 @@ int mgs_state_array(const char* which_state, const char* name, char* state, int 
 		if (n == "final_T") p = s.final_T; else if (n == "n_contrib") p = s.n_contrib; else if (n == "ranges") p = s.ranges;
 		else if (n == "tile_order") p = s.tile_order; else if (n == "block_count") p = s.block_count;
 		else if (n == "block_nwalk") p = s.block_nwalk;
+	} else if (w == "scratch") {
+		float* gb; float* gn;
+		carve_scratch(state, a0, gb, gn);
+		if (n == "gb") p = gb; else if (n == "gn") p = gn;
 	}
 	if (!p) return fail(MGS_ERR_INVALID_ARG, "unknown state array " + w + "/" + n);
 	*out_ptr = p;

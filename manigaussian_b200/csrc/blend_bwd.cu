@@ -105,12 +105,28 @@ __device__ __forceinline__ void depth_mask_cotangents(const BlendArgs& a, size_t
 	if (a.tgt_mask) h += (a.dm_scale ? a.dm_scale[1] : 1.f) * a.cot_alpha_mask[pix];
 }
 
+// PLN: the gathered quads {a, b, e, 0} of a chunk's cnt survivors (rows of stride rs from q4, records rec) get e_b =
+// -(a (mu_x - bx0) + b (mu_y - by0)) in place of e, the offset of the planar depth relative to the block origin.  Lane j < cnt
+// rewrites row j.
+__device__ __forceinline__ void planar_block_offset(float* q4, int rs, const float4* rec, int cnt, int lane, float fbx0, float fby0)
+{
+	if (lane < cnt) {
+		const float4 r0 = rec[2 * lane];
+		float* q = q4 + lane * rs;
+		q[2] = -fmaf(q[0], r0.x - fbx0, q[1] * (r0.y - fby0));
+	}
+}
+
 // F <= 32 (one channel group); channel groups run blend_bwd_groups_kernel below.  DM: the depth / mask heads
 // (BlendArgs::tgt_depth / tgt_mask); the instantiations without them keep their registers.  NRM: the normal plane
 // (BlendArgs::nrm / dL_dnormal / gn): the quad {nx, ny, nz, 0} and its cotangent fill columns 4..7 of the {r,g,b,depth} tile,
 // so GEMM 1 and GEMM 2 carry them as issued, and the flush adds dL/dn into gn; likewise.  PLN: planar depth
-// (BlendArgs::planar): the quad {a, b, e, 0} fills the same columns and the depth cotangent g enters them as {g px, g py, g, 0},
-// so dL/dalpha is that of the planar depth, and the flush adds {dL/da, dL/db, dL/de, 0} into gn; likewise.
+// (BlendArgs::planar): in block-local pixel coordinates (lx, ly) = (px - bx0, py - by0) the depth is z + a lx + b ly + e_b
+// with e_b = -(a (mu_x - bx0) + b (mu_y - by0)); the quad {a, b, e_b, 0} fills the same columns (e_b replaces the gathered e
+// once the rows are in) and the depth cotangent g enters them as {g lx, g ly, g, 0}, so dL/dalpha is that of the planar
+// depth.  The flush adds {sum w g (px - mu_x), sum w g (py - mu_y), sum w g, 0} = {dn.x - u dn.z, dn.y - v dn.z, dn.z, 0}
+// (u, v: the mean relative to the block) into gn: dL/d(a, b) with e's share included, and dL/de.  Every term is
+// footprint-sized, whatever the pixel coordinates; likewise.
 template <int NFT, bool VEC, bool DM, bool NRM, bool PLN>
 __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendArgs a)
 {
@@ -182,7 +198,7 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			grow[2 * (RGBD + c)] = g4[c];
 			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
 			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside) ? a.dL_dnormal[c * HW + pix] : 0.f;
-			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)pxi : c == 1 ? g4[3] * (float)pyi : c == 2 ? g4[3] : 0.f;
+			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)(lane >> 2) : c == 1 ? g4[3] * (float)(lane & 3) : c == 2 ? g4[3] : 0.f;
 		}
 		if (NFT > 0) {
 #pragma unroll
@@ -551,7 +567,9 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 				red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}
 				if (NRM || PLN) {
 					const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
-					red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
+					float* gn = a.gn + (size_t)__float_as_uint(r1.w) * 4;
+					if (PLN) red_add_v4(gn, fmaf(-u, dn.z, dn.x), fmaf(-v, dn.z, dn.y), dn.z, 0.f);  // mean-relative
+					else red_add_v4(gn, dn.x, dn.y, dn.z, 0.f);
 				}
 			}
 			BWD_PH_LAP(ph, BWD_PH_FLUSH);
@@ -578,6 +596,10 @@ __global__ void __launch_bounds__(64, MGS_BWD_MIN_CTAS) blend_bwd_kernel(BlendAr
 			const int rn = r == BWD_NREC - 1 ? 0 : r + 1;
 			if (cnt > 0) {
 				cp_async_wait<0>();  // this chunk's channel rows
+				if (PLN) {  // the quad's offset relative to the block origin (see above)
+					__syncwarp();
+					planar_block_offset(s_rows[s] + RGBD + 4, RS, s_rec[r], cnt, lane, fbx0, fby0);
+				}
 				if (!W_GEMM1) {
 					__syncwarp();
 					BWD_PH_LAP(ph, BWD_PH_ROW_WAIT);
@@ -686,7 +708,7 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 			// NRM: the normal plane's cotangent in columns 4..6, unscaled (the plane has no background term either)
 			grow[2 * (RGBD + 4 + c)] = (NRM && c < 3 && inside && first) ? a.dL_dnormal[c * HW + pix] : 0.f;
 			// PLN: g4 is zero outside the image and in groups >= 1
-			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)pxi : c == 1 ? g4[3] * (float)pyi : c == 2 ? g4[3] : 0.f;
+			if (PLN) grow[2 * (RGBD + 4 + c)] = c == 0 ? g4[3] * (float)(lane >> 2) : c == 1 ? g4[3] * (float)(lane & 3) : c == 2 ? g4[3] : 0.f;
 		}
 		if (NFT > 0) {
 #pragma unroll
@@ -791,6 +813,10 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 		cnt_next = next_chunk(buf ^ 1);  // the next chunk's records travel while this chunk runs
 		cp_async_wait<1>();              // the channel rows
 		__syncwarp();
+		if (PLN && first) {  // the quad's offset relative to the block origin (blend_bwd_kernel)
+			planar_block_offset(s_rows + RGBD + 4, RS, s_q, cnt, lane, fbx0, fby0);
+			__syncwarp();
+		}
 		// ---- 2. GEMM 1: Wd[p][j] = Gpx[p][:] . C[j][:]   (M = pixels (2 tiles), N = survivors, K = channels) ----
 		{
 			float wd[2][BWD_CH / 8][4];
@@ -935,7 +961,9 @@ __global__ void __launch_bounds__(32, 12) blend_bwd_groups_kernel(BlendArgs a)
 			if (first) red_add_v4(gb + 8, m2.x, m2.y, 0.f, 0.f);  // {db, ddepth}: zero in the other groups
 			if ((NRM || PLN) && first) {
 				const float4 dn = *reinterpret_cast<const float4*>(s_m + BWD_CH * 12 + lane * 4);
-				red_add_v4(a.gn + (size_t)__float_as_uint(r1.w) * 4, dn.x, dn.y, dn.z, 0.f);
+				float* gn = a.gn + (size_t)__float_as_uint(r1.w) * 4;
+				if (PLN) red_add_v4(gn, fmaf(-u, dn.z, dn.x), fmaf(-v, dn.z, dn.y), dn.z, 0.f);  // mean-relative
+				else red_add_v4(gn, dn.x, dn.y, dn.z, 0.f);
 			}
 		}
 	};
@@ -995,10 +1023,11 @@ void launch_blend_bwd(const BlendArgs& a, cudaStream_t s)
 
 // The median depth is the view-space z of one Gaussian per pixel, chosen by a piecewise-constant rule: its cotangent goes to
 // that Gaussian's depth slot of the blend-stage records and nowhere else.  One thread per pixel.  PLN (planar depth): the
-// median depth is z + a px + b py + e, so the cotangent also goes to the contributor's quad gradients gn.
+// median depth is z + a (px - mu_x) + b (py - mu_y), so the cotangent also goes to the contributor's quad gradients gn, in
+// gn's mean-relative form (blend_bwd_kernel).
 template <bool PLN>
 __global__ void median_depth_bwd_kernel(int N, const int* __restrict__ median_id, const float* __restrict__ dL_dmedian, float* gb, int W,
-	float* gn)
+	float* gn, const float2* __restrict__ means2D)
 {
 	const int p = blockIdx.x * blockDim.x + threadIdx.x;
 	if (p >= N) return;
@@ -1007,15 +1036,17 @@ __global__ void median_depth_bwd_kernel(int N, const int* __restrict__ median_id
 	if (id >= 0 && g != 0.f) red_add(gb + (size_t)id * GB_STRIDE + 9, g);
 	if (PLN && id >= 0 && g != 0.f) {
 		const int py = p / W, px = p - py * W;
-		red_add_v4(gn + (size_t)id * 4, g * (float)px, g * (float)py, g, 0.f);
+		const float2 mu = means2D[id];
+		red_add_v4(gn + (size_t)id * 4, g * ((float)px - mu.x), g * ((float)py - mu.y), g, 0.f);
 	}
 }
 
-void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s, int W, float* gn)
+void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s, int W, float* gn,
+	const float2* means2D)
 {
 	if (N <= 0) return;
-	if (gn) median_depth_bwd_kernel<true><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn);
-	else median_depth_bwd_kernel<false><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn);
+	if (gn) median_depth_bwd_kernel<true><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn, means2D);
+	else median_depth_bwd_kernel<false><<<ceil_div(N, 256), 256, 0, s>>>(N, median_id, dL_dmedian, gb, W, gn, means2D);
 }
 
 }  // namespace mgs

@@ -266,7 +266,9 @@ struct BlendArgs {
 	float* gn;
 	// planar depth (the launchers pick the PLN instantiations when set): nrm holds the view's planar quads {a, b, e, 0}
 	// (planar.cu) instead, and the depth plane, the depth / mask heads and the median depth take each Gaussian's depth
-	// z + a px + b py + e at pixel (px, py).  Backward: gn receives {dL/da, dL/db, dL/de, 0}.  Behind gn for the same reason.
+	// z + a px + b py + e at pixel (px, py).  Backward: gn receives {dL/da, dL/db, dL/de, 0} with e's share folded into dL/da
+	// and dL/db (e = -(a mu_x + b mu_y)): {sum w g (px - mu_x), sum w g (py - mu_y), sum w g, 0}, formed in block-local
+	// coordinates so that no term grows with the pixel coordinates.  Behind gn for the same reason.
 	int planar;
 #ifdef MGS_CTA_LOG
 	// measurement build only (tools/cta_timeline.py): every blend CTA appends {t0, t1 (globaltimer ns), kind | sub << 8, entries of
@@ -358,9 +360,10 @@ int blend_groups(int F);  // channel groups of 32 (BlendArgs::groups)
 void launch_blend_fwd(const BlendArgs& a, cudaStream_t s);
 void launch_blend_bwd(const BlendArgs& a, cudaStream_t s);
 // the median depth's backward: gb[median_id[p] * GB_STRIDE + 9] += dL_dmedian[p] for every pixel p with median_id[p] >= 0;
-// with gn (planar depth, W the image width) also gn[median_id[p]] += dL_dmedian[p] {px, py, 1, 0}
+// with gn (planar depth, W the image width, means2D the view's screen means) also gn[median_id[p]] += dL_dmedian[p]
+// {px - mu_x, py - mu_y, 1, 0} (gn's mean-relative form, BlendArgs::planar)
 void launch_median_depth_bwd(int N, const int* median_id, const float* dL_dmedian, float* gb, cudaStream_t s, int W = 0,
-	float* gn = nullptr);
+	float* gn = nullptr, const float2* means2D = nullptr);
 
 // lift.cu: lifted[id][c] += sum_p w_p,id map[c][p] and weight[id] += sum_p w_p,id over one view's pixels, w = alpha T the
 // forward blend's weights (include/mgs_rasterizer.h, mgs_lift_views).  The tile grid, lists and records are the view's, as

@@ -89,8 +89,9 @@ __device__ __forceinline__ void warp_halve(float* x, const int lane)
 // dL/dJ : dJ/dt = (G P^T) : dDd/d(x, y) chained through P, plus (Dd G) : dP/dt (Dd is symmetric); J^T (du, dv) enters through
 // the same chain.  The camera terms and dL/dtan_fov are the fisheye ones with u - cx = fx xd.
 //
-// PLN (DIST, FISH, ORTHO and CAM only): planar depth on the views with a.pl_g[v] set.  The blend's quad gradients {ga, gb, ge}
-// of (a, b, e = -(a mu_x + b mu_y)) give dL/d(a, b) = (ga - mu_x ge, gb - mu_y ge) and, through e, the screen mean's cotangent
+// PLN (DIST, FISH, ORTHO and CAM only): planar depth on the views with a.pl_g[v] set.  The blend's quad gradients of
+// (a, b, e = -(a mu_x + b mu_y)) arrive with e's share folded in, {ga - mu_x ge, gb - mu_y ge, ge} = dL/d(a, b) and ge (formed
+// relative to the mean in the blend, where its terms stay footprint-sized); through e, the screen mean's cotangent is
 // -(a, b) ge in pixels, added to dm in its convention.  With (a, b) = k Q, k_j = Rv2^T S m_j (m_j row j of M = J Rv):
 // dL/dQ = k^T dL/d(a, b) joins G, dk = dL/d(a, b) Q, and dk reaches S (sym(Rv2 n^T), n = dk_0 m_0 + dk_1 m_1), M (dL/dm_j +=
 // dk_j S Rv2, so the existing chain carries it through J to t, the camera and the field of view) and the third row of Rv
@@ -165,8 +166,7 @@ __device__ __forceinline__ void project_bwd_gaussian(const Args& a, const int id
 				plv = a.pl_g[v] != nullptr;
 				if (plv) {
 					const float4 g = a.pl_g[v][idx], q = a.pl_q[v][idx];
-					const float2 mu = a.pl_mean[v][idx];
-					pga = g.x - mu.x * g.z; pgb = g.y - mu.y * g.z;
+					pga = g.x; pgb = g.y;  // the blend formed them relative to the mean (mgs_kernels.h, BlendArgs::planar)
 					dm[0] -= q.x * g.z * (0.5f * a.intr[v].W); dm[1] -= q.y * g.z * (0.5f * a.intr[v].H);
 				}
 			}

@@ -15,6 +15,16 @@ colours, depth, features) and re-does only the blend:
 
 Per tile everything is a (256 pixels x L entries) array: transmittances come from cumulative products, the suffix sums of
 the backward from reversed cumulative sums.
+
+Extra columns (columns 4..7 of the kernels' {r,g,b,depth} tile): `st["quad"]` [P,4] per-Gaussian quads blended as four more
+channels without a background term and without `cot_scale`.  With `st["planar"]` false (the normal plane, the flow plane) the
+cotangent planes are `st["g_quad"]` [3 or 4,H,W]; `blend` returns the plane `quad` [4,H,W] and `dL_dquad` [P,4] = w^T g_quad.
+With `st["planar"]` true the quad is {a, b, e, 0} and each pair's depth is per pixel, D = z + a px + b py + e: the depth
+plane is col3 + px col4 + py col5 + col6, the cotangent columns are {g px, g py, g, 0} with g the depth cotangent, so dot,
+S and dL/dalpha are those of the planar depth, and `dL_dquad` = {sum w g (px - mu_x), sum w g (py - mu_y), sum w g, 0}:
+dL/d(a, b) with the share of e = -(a mu_x + b mu_y) folded in, the kernels' gn, whose terms are footprint-sized wherever the
+pixels lie (its bound: |px - mu_x| + 16 per term, the block-local columns and the mean's offset from the block origin).
+`median_planar` adds the planar median depth and its gradient.
 """
 import numpy as np
 
@@ -29,6 +39,11 @@ U = 2.0 ** -24
 # measured against the C oracle's blend with the depth as a feature channel (test_depth_cotangent_matches_oracle_per_element).
 KAPPA = dict(color=14.5, feature=24.0, depth=11.1, final_T=7.1, alpha=2.0,
              dL_dmeans2D=0.23, dL_dconic=0.012, dL_dopacity=0.7, dL_dcolors=1.6, dL_ddepth=0.26, dL_dfeature=5.3)
+# the extra columns (tests/test_blend_planes_gpu.py, measured on the near-origin scenes); planar_depth covers the planar depth
+# plane, median_planar the planar median depth
+KAPPA.update(normal=9.0, planar_depth=8.7, median_planar=2.6, dL_dquad=1.0)
+# dL_dconic with the depth / mask heads folded into the cotangents (their term64 case: 0.0151, past the plain scenes' 0.003)
+KAPPA["dL_dconic_heads"] = 0.061
 
 
 def tile_pixels(W, H, tile):
@@ -121,13 +136,19 @@ def decide_fp32(st, tile):
     return ok & (np.arange(L)[None, :] < first_stop[:, None]) & inside[:, None]
 
 
+def _nfeat(st):
+    return st["feature"].shape[1] if (st.get("feature") is not None and st["feature"].ndim == 2) else 0
+
+
 def _channels(st, ids):
-    """[L, C] channel rows {r, g, b, depth?, features...} of the entries and the matching cotangent plane list."""
+    """[L, C] channel rows {r, g, b, depth?, features..., quad?} of the entries."""
     cols = [st["colors"][ids].astype(np.float64)]
     if st.get("depth") is not None:
         cols.append(st["depth"][ids].astype(np.float64)[:, None])
     if st.get("feature") is not None and st["feature"].ndim == 2 and st["feature"].shape[1]:
         cols.append(st["feature"][ids].astype(np.float64))
+    if st.get("quad") is not None:
+        cols.append(st["quad"][ids].astype(np.float64))
     return np.concatenate(cols, 1)
 
 
@@ -140,6 +161,14 @@ def _cot(st, px, py, inside):
         g.append((gd[y, x] if gd is not None else np.zeros(256))[:, None].astype(np.float64))
     if st.get("feature") is not None and st["feature"].ndim == 2 and st["feature"].shape[1]:
         g.append(st["g_feature"][:, y, x].T.astype(np.float64))
+    if st.get("quad") is not None:
+        if st.get("planar"):
+            gd = g[1][:, 0]
+            g.append(np.stack([gd * px, gd * py, gd, np.zeros(256)], 1))
+        else:
+            gq = np.zeros((256, 4))
+            gq[:, :st["g_quad"].shape[0]] = st["g_quad"][:, y, x].T
+            g.append(gq)
     ga = st.get("g_alpha")
     h = ga[y, x].astype(np.float64) if ga is not None else np.zeros(256)
     g = np.concatenate(g, 1)
@@ -168,6 +197,10 @@ def new_out(st):
     out = {k: np.zeros(s) for k, s in (("color", (3, H, W)), ("color_B", (3, H, W)), ("feature", (F, H, W)),
                                        ("feature_B", (F, H, W)), ("depth", (H, W)), ("depth_B", (H, W)),
                                        ("final_T", (H, W)), ("final_T_B", (H, W)), ("alpha", (H, W)), ("alpha_B", (H, W)))}
+    if st.get("quad") is not None:
+        for k, s in (("quad", (4, H, W)), ("dL_dquad", (P, 4))):
+            out[k] = np.zeros(s)
+            out[k + "_B"] = np.zeros(s)
     out["n_contrib"] = np.zeros((H, W), np.int64)
     for k, s in (("dL_dmeans2D", (P, 2)), ("dL_dconic", (P, 3)), ("dL_dopacity", (P,)), ("dL_dcolors", (P, 3)),
                  ("dL_ddepth", (P,)), ("dL_dfeature", (P, F))):
@@ -216,8 +249,19 @@ def blend_tile(st, tile, m, out, backward=True):
         out["depth"][y, x] = vals[inside, 3]
         out["depth_B"][y, x] = vB[inside, 3]
     if F:
-        out["feature"][:, y, x] = vals[inside, nch:].T
-        out["feature_B"][:, y, x] = vB[inside, nch:].T
+        out["feature"][:, y, x] = vals[inside, nch:nch + F].T
+        out["feature_B"][:, y, x] = vB[inside, nch:nch + F].T
+    if st.get("quad") is not None:
+        q0 = nch + F
+        out["quad"][:, y, x] = vals[inside, q0:q0 + 4].T
+        out["quad_B"][:, y, x] = vB[inside, q0:q0 + 4].T
+        if st.get("planar"):
+            # col3 + px col4 + py col5 + col6: each term's bound, plus the magnitude of every term for the products and the
+            # three fp32 additions
+            terms = (vals[:, 3], px * vals[:, q0], py * vals[:, q0 + 1], vals[:, q0 + 2])
+            mag = sum(np.abs(t) for t in terms)
+            out["depth"][y, x] = sum(terms)[inside]
+            out["depth_B"][y, x] = (vB[:, 3] + px * vB[:, q0] + py * vB[:, q0 + 1] + vB[:, q0 + 2] + 4.0 * mag)[inside]
     out["final_T"][y, x] = Tf[inside]
     out["final_T_B"][y, x] = (Tf * (relTf + 1.0))[inside]
     out["alpha"][y, x] = 1.0 - Tf[inside]
@@ -268,8 +312,52 @@ def blend_tile(st, tile, m, out, backward=True):
         np.add.at(out["dL_ddepth"], ids, w.T @ g[:, 3])
         np.add.at(out["dL_ddepth_B"], ids, ge.T @ np.abs(g[:, 3]))
     if F:
-        np.add.at(out["dL_dfeature"], ids, w.T @ g[:, nch:])
-        np.add.at(out["dL_dfeature_B"], ids, ge.T @ np.abs(g[:, nch:]))
+        np.add.at(out["dL_dfeature"], ids, w.T @ g[:, nch:nch + F])
+        np.add.at(out["dL_dfeature_B"], ids, ge.T @ np.abs(g[:, nch:nch + F]))
+    if st.get("quad") is not None:
+        gq = g[:, nch + F:nch + F + 4]
+        dq, dqB = w.T @ gq, ge.T @ np.abs(gq)
+        if st.get("planar"):
+            # relative to each pair's mean: dx = mu_x - px
+            gd = np.abs(gq[:, 2])[:, None]
+            dq[:, 0] = (w * gq[:, 2][:, None] * -dx).sum(0)
+            dq[:, 1] = (w * gq[:, 2][:, None] * -dy).sum(0)
+            dqB[:, 0] = (ge * gd * (np.abs(dx) + 16.0)).sum(0)
+            dqB[:, 1] = (ge * gd * (np.abs(dy) + 16.0)).sum(0)
+        np.add.at(out["dL_dquad"], ids, dq)
+        np.add.at(out["dL_dquad_B"], ids, dqB)
+
+
+def median_planar(st, median_id, g_median, out):
+    """The median depth of each pixel's median contributor (`median_id` [H,W], -1: none) with its bound -- z, or with
+    st["planar"] z + a px + b py + e -- and its gradient: `g_median` [H,W] (or None) added to that Gaussian's dL_ddepth and,
+    planar, as g {px - mu_x, py - mu_y, 1, 0} to its dL_dquad in `out`.  The kernels add one term per pixel into the blend's sums with
+    fp32 atomics, each rounding its running sum: n terms on a Gaussian add n (|its blend sum| + sum |g|) to the bound.
+    Returns (plane, bound)."""
+    H, W = median_id.shape
+    py, px = np.mgrid[0:H, 0:W].astype(np.float64)
+    has = median_id >= 0
+    ids = np.where(has, median_id, 0)
+    z = st["depth"][ids].astype(np.float64)
+    planar = bool(st.get("planar"))
+    q = st["quad"][ids].astype(np.float64) if planar else None
+    terms = (z, q[..., 0] * px, q[..., 1] * py, q[..., 2]) if planar else (z,)
+    plane = np.where(has, sum(terms), 0.0)
+    B = np.where(has, 4.0 * sum(np.abs(t) for t in terms), 0.0)
+    if g_median is not None:
+        g = np.where(has, g_median.astype(np.float64), 0.0)
+        i = ids[has]
+        n = np.bincount(i, minlength=out["dL_ddepth"].shape[0]).astype(np.float64)
+        cols = [(out["dL_ddepth"], out["dL_ddepth_B"], g)]
+        if planar:
+            mu = st["means2D"][ids].astype(np.float64)
+            cols += [(out["dL_dquad"][:, c], out["dL_dquad_B"][:, c], g * f)
+                     for c, f in enumerate((px - mu[..., 0], py - mu[..., 1], np.ones_like(px)))]
+        for v, vB, x in cols:
+            sabs = np.bincount(i, np.abs(x[has]), minlength=len(n))
+            vB += n * (np.abs(v) + sabs) + sabs
+            np.add.at(v, i, x[has])
+    return plane, B
 
 
 def masks_from_blocks(st, block_lists, pixel_masks, block_nwalk):

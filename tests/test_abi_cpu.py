@@ -44,6 +44,13 @@ def test_invalid_arguments_return_error_codes_without_touching_a_gpu():
     assert L.mgs_mark_visible(-1, None, None, None, None, None) == -1
     out = ctypes.c_void_p()
     assert L.mgs_state_array(b"geometry", b"nope", ctypes.c_void_p(4096), 10, 0, ctypes.byref(out)) < 0
+    assert L.mgs_state_array(b"scratch", b"nope", ctypes.c_void_p(4096), 10, 0, ctypes.byref(out)) < 0
+    # the blend-stage records: gb [P][12] at the start of the scratch, gn [P][4] behind it (no device access)
+    base = 1 << 20
+    assert L.mgs_state_array(b"scratch", b"gb", ctypes.c_void_p(base), 10, 0, ctypes.byref(out)) == 0 and out.value == base
+    assert L.mgs_state_array(b"scratch", b"gn", ctypes.c_void_p(base), 10, 0, ctypes.byref(out)) == 0
+    assert out.value >= base + 10 * 12 * 4 and out.value % 16 == 0
+    assert out.value - base + 10 * 4 * 4 <= L.mgs_backward_scratch_bytes_normal(10)
 
 
 def test_python_surface_matches_reference():

@@ -4,7 +4,10 @@ Per scene: (a) every pair the reference puts surely inside the alpha >= 1/255 fo
 cull in binning.cu / project.cu is sound); (b) our pixel masks equal the float64 decisions wherever no decision is
 borderline, and block_nwalk ends at the block's last contributor; (c) with our masks as the decisions every pixel of
 colour / features / depth / final_T / alpha is within its bound and n_contrib is exact; (d) every Gaussian's dL_dmeans2D,
-dL_dopacity, dL_dcolors and dL_dfeature is within its bound (F <= 32: the two-warp kernel; F > 32: blend_bwd_groups).
+dL_dopacity, dL_dcolors and dL_dfeature, and the blend-stage record's dL_dconic and dL_ddepth (read from the backward
+scratch), is within its bound (F <= 32: the two-warp kernel; F > 32: blend_bwd_groups).  F = 12 and 28 take the padded
+NFT = 2 / 4 paths, F = 16 the vectorised NFT = 2 one, and `ragged_off4` (F = 32 with the feature rows 4 bytes off a 16-byte
+boundary) the NFT = 4 path without vector loads.
 
 The scenes are built in screen space (`place`: target pixel centres and depths unprojected through the camera, shapes
 given as 2D covariances through cov3D_precomp) to reach the kernels' structural edges, and each asserts the edge it was
@@ -24,10 +27,13 @@ these and of the CPU-side ratios, per quantity):
 | ragged (F 0-67) | 2.89 | 1.78 | 0.10 | 0.48 | 2.49 | 0.011 | 0.030 | 0.065 | 0.14 | 0 |
 | ragged_f32 | 3.63 | 2.77 | 0.11 | 0.48 | 1.60 | 0.0054 | 0.010 | - | 0.072 | - |
 | sh3_big | 1.48 | 1.23 | 0.19 | 0.22 | 1.60 | 0.0100 | 0.017 | - | 0.12 | - |
+| ragged F 12 / 16 / 28, ragged_off4 (H100 80GB HBM3, 700 W) | 2.89 | 1.78 | 0.10 | 0.48 | 2.47 | 0.0051 | 0.016 | 0.065 | 0.14 | 0 |
+
+gb dL_dconic / dL_ddepth (the blend-stage record) on the same H100 80GB HBM3 (700 W), all cases: at most 0.0060 / 0.15.
 
 dcov3D: project_ref64.cov3d_grad, the raw ratio of the part the inherited conic bound does not cover, over u e.
 No cull violation in any scene; borderline pixels 0.12 % (needles), 0.10 % (opacity), 0.09 % (ragged_f32), 0 elsewhere.
-All 17 cases take about 10 s.
+All 21 cases take about 15 s.
 """
 import numpy as np
 import pytest
@@ -203,6 +209,7 @@ SCENES = {
     "offscreen": lambda F: scene_offscreen(F),
     "opacity": lambda F: scene_opacity(F),
     "ragged": lambda F: scene_ragged(F),
+    "ragged_off4": lambda F: dict(scene_ragged(F), feature_offset=1),
     # the existing random parity cases, so the per-element bars also cover realistic density
     "ragged_f32": lambda F: _random(dict(P=5000, W=200, H=120, F=F, seed=3, bg=(0.3, 0.6, 0.9))),
     "sh3_big": lambda F: _random(dict(P=1500, W=128, H=96, F=F, seed=5, sh_degree=3, scale0=0.04, bg=(1.0, 1.0, 1.0))),
@@ -216,27 +223,92 @@ def _random(kw):
 
 
 # --------------------------------------------------------------------------- running the kernels
-def run_kernels(inp):
+class scratch_capture:
+    """Keeps every backward view's blend_scratch alive (in call order) while in effect, so that its blend-stage records
+    can be read after the call: `records(i, P)` = (gb [P,12], gn [P,4] or None) of the i-th view's scratch."""
+    def __enter__(self):
+        from manigaussian_b200 import rasterizer as R
+        self.R, self.orig, self.views = R, R._backward_view, []
+
+        def wrapped(*a, **kw):
+            keep = self.orig(*a, **kw)
+            self.views.append((keep[-1], bool(a[-1]) if len(a) > 9 else bool(kw.get("normal", False))))
+            return keep
+        R._backward_view = wrapped
+        return self
+
+    def __exit__(self, *exc):
+        self.R._backward_view = self.orig
+
+    def records(self, i, P):
+        import torch
+        torch.cuda.synchronize()
+        sc, normal = self.views[i]
+        out = []
+        for name, n in (("gb", 12), ("gn", 4)):
+            if name == "gn" and not normal:
+                out.append(None)
+                continue
+            off = self.R.state_array("scratch", name, sc, P) - sc.data_ptr()
+            out.append(sc[off:off + 4 * n * P].view(torch.float32).reshape(P, n).cpu().numpy())
+        return out
+
+
+def feature_tensor(feature, offset=0):
+    """The feature rows as a CUDA tensor whose data start `offset` floats past a 16-byte boundary (offset 0: util._t)."""
+    import torch
+    if not offset:
+        return util._t(feature)
+    n = feature.size
+    buf = torch.zeros(n + offset, dtype=torch.float32, device="cuda")
+    buf[offset:] = torch.from_numpy(np.ascontiguousarray(feature, np.float32).ravel()).cuda()
+    return buf[offset:].view(feature.shape)
+
+
+def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False):
+    """One forward and backward of the scene `inp`, and everything the checks read back.  The options (for
+    tests/test_blend_planes_gpu.py): planar depth, the normal plane (cotangent inp["ct"]["dL_dnormal"]), the median depth
+    (cotangent inp["ct"]["dL_dmedian"]) and the depth / mask heads (targets inp["dm_targets"], upstream gradients
+    inp["dm_scale"]).  inp["lens"]: a distortion tuple for a distorted-pinhole view, inp["tanfov"] its (tan_fovx, tan_fovy)."""
     import torch
     from manigaussian_b200 import rasterizer as R
     t = util._t
     cam, g, ct = inp["cam"], inp["g"], inp["ct"]
     P, W, H, F = inp["P"], inp["W"], inp["H"], inp["F"]
-    s = R.GaussianRasterizationSettings(H, W, cam["tanfovx"], cam["tanfovy"], t(inp["bg"]), 1.0, t(cam["viewmatrix"]),
-                                        t(cam["projmatrix"]), g["sh_degree"], t(cam["campos"]), False, False, F > 0)
-    args = (t(g["means3D"]), t(g["colors_precomp"]), t(g["feature"]) if F else None, t(g["opacities"]), t(g["scales"]),
+    tfx, tfy = inp.get("tanfov", (cam["tanfovx"], cam["tanfovy"]))
+    s = R.GaussianRasterizationSettings(H, W, tfx, tfy, t(inp["bg"]), 1.0, t(cam["viewmatrix"]),
+                                        t(cam["projmatrix"]), g["sh_degree"], t(cam["campos"]), False, False, F > 0,
+                                        distortion=inp.get("lens"), planar_depth=planar)
+    feat = feature_tensor(g["feature"], inp.get("feature_offset", 0)) if F else None
+    if feat is not None and inp.get("feature_offset"):
+        assert feat.data_ptr() % 16 == 4 * inp["feature_offset"]
+    args = (t(g["means3D"]), t(g["colors_precomp"]), feat, t(g["opacities"]), t(g["scales"]),
             t(g["rotations"]), 1.0, t(g["cov3D_precomp"]), t(g["shs"]), g["sh_degree"], F > 0)
-    outs, streams = R.rasterize_views_raw([s], *args, return_depth=True, return_alpha=True)
+    heads = dm = dm_scale = None
+    if depth_mask:
+        from manigaussian_b200.gaussian_renderer import _depth_mask_heads
+        opts = dict(dtype=torch.float32, device="cuda")
+        heads = (torch.zeros((1, 3, H, W), **opts), None, torch.empty((1, 3, H, W), **opts), None, torch.empty((1, 2), **opts))
+        dm = _depth_mask_heads(t(inp["dm_targets"][0][None]), t(inp["dm_targets"][1][None]), 1, H, W, torch.device("cuda"))
+        dm_scale = t(np.asarray(inp["dm_scale"], np.float32)[None])
+    outs, streams = R.rasterize_views_raw([s], *args, return_depth=True, return_alpha=True, return_median=median,
+                                          return_normal=normal, loss_heads=heads, depth_mask=dm)
     o = outs[0]
     Rn = o.num_rendered()
     assert not o.overflowed()
     cap = int(o[0])
     gc = [t(ct["dL_dcolor"])]
     gf = [t(ct["dL_dfeature"])] if F else None
-    grads = R.rasterize_views_backward_raw([s], outs, streams, gc, gf, args[0], args[1], args[2], args[4], args[5], 1.0,
-                                           args[7], args[8], g["sh_degree"], F > 0, grads_depth=[t(ct["dL_ddepth"])],
-                                           grads_alpha=[t(ct["dL_dalpha"])])
+    med = (o[-2 - int(normal)], o[-1 - int(normal)]) if median else None
+    with scratch_capture() as cap_sc:
+        grads = R.rasterize_views_backward_raw(
+            [s], outs, streams, gc, gf, args[0], args[1], args[2], args[4], args[5], 1.0, args[7], args[8], g["sh_degree"], F > 0,
+            grads_depth=[t(ct["dL_ddepth"])], grads_alpha=[t(ct["dL_dalpha"])],
+            grads_median=[t(ct["dL_dmedian"])] if median else None, median_ids=[med[1]] if median else None,
+            grads_normal=[t(ct["dL_dnormal"])] if normal else None, normals=[o[-1]] if normal else None,
+            depth_mask=dm, depth_mask_scale=dm_scale)
     torch.cuda.synchronize()
+    gb, gn = cap_sc.records(0, P)
     geomB, binB, imgB = o[4], o[5], o[6]
     T = ((W + 15) // 16) * ((H + 15) // 16)
     S = (cap + 11) & ~3
@@ -264,6 +336,17 @@ def run_kernels(inp):
     for n, v in zip(names, grads[:4]):
         k[n] = None if v is None else v.cpu().numpy()
     k["radii"] = o[3].cpu().numpy()
+    k["gb"], k["gn"] = gb, gn
+    k["dL_dmeans3D"] = grads[4].cpu().numpy()
+    if planar or normal:
+        k["nrm"] = arr("geometry", "nrm", geomB, P, 0, torch.float32, 4 * P).reshape(P, 4)
+    if normal:
+        k["normal"] = o[-1].cpu().numpy()
+    if median:
+        k["median_depth"], k["median_id"] = med[0].cpu().numpy(), med[1].cpu().numpy()
+    if depth_mask:
+        k["dm_planes"] = [None if x is None else x[0].cpu().numpy() for x in dm[2:5]]
+        k["dm_acc"] = dm[5][0].cpu().numpy()
     k["dL_dcov3D"] = None if grads[5] is None else grads[5].cpu().numpy()
     return k
 
@@ -321,8 +404,9 @@ def _check(name, got, ref, B, where, report):
 
 # --------------------------------------------------------------------------- the test
 CASES = [("lists", 3), ("lists", 40), ("term32", 0), ("term64", 32), ("empty_run", 3), ("empty_run", 67),
-         ("needles", 3), ("offscreen", 3), ("opacity", 32), ("opacity", 67), ("ragged", 0), ("ragged", 3),
-         ("ragged", 32), ("ragged", 40), ("ragged", 67), ("ragged_f32", 32), ("sh3_big", 8)]
+         ("needles", 3), ("offscreen", 3), ("opacity", 32), ("opacity", 67), ("ragged", 0), ("ragged", 3), ("ragged", 12),
+         ("ragged", 16), ("ragged", 28), ("ragged", 32), ("ragged_off4", 32), ("ragged", 40), ("ragged", 67), ("ragged_f32", 32),
+         ("sh3_big", 8)]
 
 
 @pytest.mark.parametrize("scene,F", CASES, ids=[f"{s}-F{f}" for s, f in CASES])
@@ -330,18 +414,35 @@ def test_blend_pairs(scene, F):
     inp = SCENES[scene](F)
     k = run_kernels(inp)
     st = state_of(inp, k)
+    ours, ref, problems, report = check_blend(k, st, inp)
+    print(f"[{scene} F={F}] " + " ".join(f"{a}={b:.3g}" for a, b in report.items()))
+    _assert_edge(scene, k, st, ours)
+    problems = [p for p in problems if p]
+    assert not problems, "\n".join(problems)
+
+
+def check_blend(k, st, inp, depth="depth", cov3d=True, records=True):
+    """Checks (a) to (d) of one render `k` (run_kernels) against the reference state `st`.  Returns (our masks, the reference's
+    blend(), the list of problems (None for a passed check), the report of worst ratios).  depth: the KAPPA entry of the depth
+    plane; cov3d: also check dL_dcov3D (cov3D_precomp renders through a pinhole view); records: also check the blend-stage
+    record's dL_dconic and dL_ddepth."""
+    F = k["F"]
     W, H = k["W"], k["H"]
     T = k["ranges"].shape[0]
     ours = R64.masks_from_blocks(st, k["block_lists"], k["pixel_masks"], k["block_nwalk"])
     problems, report = [], {}
     cull_bad, border_px, mask_bad, npix = [], 0, [], 0
     for t in range(T):
-        d = R64.decide(st, t)
         r0, r1 = (int(v) for v in k["ranges"][t])
         L = r1 - r0
         px, py, inside = R64.tile_pixels(W, H, t)
         lx, ly = np.arange(256) % 16, np.arange(256) // 16
         s, _ = R64.pixel_block_bit(lx, ly)
+        if L == 0:  # an empty tile: nothing to decide, and no block walks
+            npix += int(inside.sum())
+            assert all(int(k["block_nwalk"][t, b]) == 0 for b in range(8) if (inside & (s == b)).any()), t
+            continue
+        d = R64.decide(st, t)
         bits = k["block_bits"][r0:r1].astype(np.int64)
         listed = ((bits[None, :] >> s[:, None]) & 1).astype(bool)
         # (a) cull soundness
@@ -384,16 +485,22 @@ def test_blend_pairs(scene, F):
     pix = lambda u: _where_pixel(k, u[-1], u[-2])  # noqa: E731
     for name, got in (("color", k["color"]), ("depth", k["depth"]), ("final_T", k["final_T"]), ("alpha", k["alpha"])) + \
             ((("feature", k["feature"]),) if F else ()):
-        problems.append(_check("(c) " + name, got, ref[name], ref[name + "_B"], pix, report))
+        q = depth if name == "depth" else name
+        problems.append(_check("(c) " + q, got, ref[name], ref[name + "_B"], pix, report))
     # (d) backward, per Gaussian
     gw = lambda u: _where_gaussian(k, u[0])  # noqa: E731
-    problems.append(_check("(d) dL_dmeans2D", k["dL_dmeans2D"][:, :2], ref["dL_dmeans2D"], ref["dL_dmeans2D_B"], gw, report))
+    if not st.get("planar"):  # with planar depth the returned dL_dmeans2D also holds the quad's share through e
+        problems.append(_check("(d) dL_dmeans2D", k["dL_dmeans2D"][:, :2], ref["dL_dmeans2D"], ref["dL_dmeans2D_B"], gw, report))
     problems.append(_check("(d) dL_dopacity", k["dL_dopacity"][:, 0], ref["dL_dopacity"], ref["dL_dopacity_B"], gw, report))
     if k["dL_dcolors"] is not None:
         problems.append(_check("(d) dL_dcolors", k["dL_dcolors"], ref["dL_dcolors"], ref["dL_dcolors_B"], gw, report))
     if F:
         problems.append(_check("(d) dL_dfeature", k["dL_dfeature"], ref["dL_dfeature"], ref["dL_dfeature_B"], gw, report))
-    if k["dL_dcov3D"] is not None:
+    if records:
+        # the blend-stage record (gb) itself: dL_dconic {a, b, c} in slots 2..4, dL_ddepth in slot 9
+        problems.append(_check("(d) gb dL_dconic", k["gb"][:, [2, 3, 4]], ref["dL_dconic"], ref["dL_dconic_B"], gw, report))
+        problems.append(_check("(d) gb dL_ddepth", k["gb"][:, 9], ref["dL_ddepth"], ref["dL_ddepth_B"], gw, report))
+    if cov3d and k["dL_dcov3D"] is not None:
         # the conic gradients (GEMM 3's six moments) through the output the ABI returns for cov3D_precomp
         cam, g = inp["cam"], inp["g"]
         c3, bd = P64.cov3d_grad(ref, g, cam, live=k["radii"] > 0)
@@ -404,10 +511,7 @@ def test_blend_pairs(scene, F):
             i = np.argsort(r.max(1))[::-1][:5]
             problems.append(f"(d) dL_dcov3D: {int((r > P64.KAPPA['dL_dcov3D']).any(1).sum())} Gaussians out of bound; worst "
                             f"{[(_where_gaussian(k, np.nonzero(ok)[0][j]), float(r[j].max())) for j in i]}")
-    print(f"[{scene} F={F}] " + " ".join(f"{a}={b:.3g}" for a, b in report.items()))
-    _assert_edge(scene, k, st, ours)
-    problems = [p for p in problems if p]
-    assert not problems, "\n".join(problems)
+    return ours, ref, problems, report
 
 
 def _assert_edge(scene, k, st, ours):
