@@ -1519,6 +1519,41 @@ int mgs_neighbour_reg_backward(void* state, int P, int k, const float* xyz, cons
 	const float* rot_next, const long long* index, const float* weight, const float* dL_dloss, float* dL_dxyz, float* dL_drot,
 	float* dL_dxyz_next, float* dL_drot_next, int debug, void* stream);
 
+/*
+ * Deformation by a sparse control graph (embedded deformation, Sumner et al.; SC-GS; no reference counterpart): a cloud
+ * (xyz [P,3], rot [P,4]) moved by N control nodes (node_xyz [N,3], node_rot [N,4], node_t [N,3]), each Gaussian blending
+ * the rigid motions of the nodes its row of index [P,k] names (as mgs_knn returns it for the nodes, queried at xyz) with
+ * weights weight [P,k], used exactly as given (not normalised).  Quaternions are (r, x, y, z), real part first.  Per node j:
+ *   q^_j = node_rot_j / max(|node_rot_j|, 1e-12), negated where its real part is below 0 (kept at exactly 0)
+ *   R_j = qrot(q^_j)   (INTEGRATION.md section 17's formula),   c_j = node_xyz_j + node_t_j - R_j node_xyz_j
+ * so node j moves a point x to R_j x + c_j, a rotation about the node followed by its translation.  Per Gaussian i, summed
+ * over its valid slots s (0 <= j = index[i,s] < N; padding -1 and out-of-range indices are skipped before anything is read),
+ * w = weight[i,s] and e = (1, 0, 0, 0):
+ *   out_xyz_i = xyz_i + sum_s w (R_j xyz_i + c_j - xyz_i)
+ *   r_i = e + sum_s w (q^_j - e),   out_rot_i = normalize(r_i) (x) rot_i     (Hamilton product; rot_i used as given)
+ * Weight missing from 1 goes to the identity motion: a row without a valid slot, or with zero weights, is copied unchanged.
+ * The outputs are bitwise identical from call to call.
+ * Backward: dL_dout_xyz [P,3] and dL_dout_rot [P,4] (each NULL: zero); gradients, each NULL to skip it and fully written
+ * otherwise, to xyz [P,3], rot [P,4], node_xyz [N,3], node_rot [N,4], node_t [N,3] and weight [P,k] (0 in invalid slots).
+ * Conventions as torch: below the 1e-12 clamp the normalisation's gradient is that of x / 1e-12, and the sign of q^_j passes
+ * the gradient through.  The node gradients are float atomics: their last bits depend on the order of the reductions.
+ *   - state: mgs_deform_state_bytes(P, N, k) bytes of device memory, any alignment (k does not change it); the backward
+ *     reads what the forward with the same inputs left there (the node records and each r_i), so it takes the forward's
+ *     arguments unchanged.
+ *   - k is 1 .. 32 (larger k returns MGS_ERR_UNSUPPORTED).  P = 0 or N = 0 is allowed.
+ * Nothing allocates, blocks or reads back to the host: both calls can be captured in a CUDA graph.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for k > 32;
+ * MGS_ERR_INVALID_ARG for k < 1, P < 0, N < 0, a NULL state, a NULL xyz, rot, index or weight (P > 0), a NULL node_xyz,
+ * node_rot or node_t (N > 0), and a NULL out_xyz or out_rot of the forward (P > 0).
+ */
+size_t mgs_deform_state_bytes(int P, int N, int k);
+int mgs_deform(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz, const float* node_rot,
+	const float* node_t, const long long* index, const float* weight, float* out_xyz, float* out_rot, int debug, void* stream);
+int mgs_deform_backward(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz,
+	const float* node_rot, const float* node_t, const long long* index, const float* weight, const float* dL_dout_xyz,
+	const float* dL_dout_rot, float* dL_dxyz, float* dL_drot, float* dL_dnode_xyz, float* dL_dnode_rot, float* dL_dnode_t,
+	float* dL_dweight, int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -274,6 +274,16 @@ def lib():
     L.mgs_neighbour_reg_backward.restype = C.c_int
     L.mgs_neighbour_reg_backward.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp,  # state P k xyz rot xyz_next rot_next index weight
                                              vp, vp, vp, vp, vp, i, vp]         # dL_dloss dL_d{xyz,rot,xyz_next,rot_next} debug stream
+    L.mgs_deform_state_bytes.restype = C.c_size_t
+    L.mgs_deform_state_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    L.mgs_deform.restype = C.c_int
+    L.mgs_deform.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, vp,  # state P N k xyz rot node_xyz node_rot node_t index weight
+                             vp, vp, i, vp]                          # out_xyz out_rot debug stream
+    L.mgs_deform_backward.restype = C.c_int
+    L.mgs_deform_backward.argtypes = L.mgs_deform.argtypes[:11] + [
+        vp, vp,                  # dL_dout_xyz dL_dout_rot
+        vp, vp, vp, vp, vp, vp,  # dL_d{xyz,rot,node_xyz,node_rot,node_t,weight}
+        i, vp]                   # debug stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -343,6 +353,7 @@ EXPORTED_SYMBOLS = (
     "mgs_camera_rays_scratch_bytes", "mgs_camera_rays", "mgs_camera_rays_backward",
     "mgs_knn_state_bytes", "mgs_knn",
     "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
+    "mgs_deform_state_bytes", "mgs_deform", "mgs_deform_backward",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

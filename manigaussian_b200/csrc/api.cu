@@ -2733,3 +2733,51 @@ int mgs_neighbour_reg_backward(void* state, int P, int k, const float* xyz, cons
 	MGS_STAGE("neighbour_reg_bwd");
 	return 0;
 }
+
+size_t mgs_deform_state_bytes(int P, int N, int /*k*/)
+{
+	return mgs::deform_state_bytes(std::max(P, 0), std::max(N, 0));
+}
+
+// the argument checks both directions share (include/mgs_rasterizer.h, mgs_deform)
+static int deform_args(const char* where, void* state, int P, int N, int k, const float* xyz, const float* rot,
+	const float* node_xyz, const float* node_rot, const float* node_t, const long long* index, const float* weight)
+{
+	using namespace mgs;
+	const std::string w(where);
+	if (k > DEFORM_MAX_K) return fail(MGS_ERR_UNSUPPORTED, w + ": k must be at most 32");
+	if (k < 1) return fail(MGS_ERR_INVALID_ARG, w + ": k must be >= 1");
+	if (P < 0 || N < 0) return fail(MGS_ERR_INVALID_ARG, w + ": P and N must be >= 0");
+	if (!state) return fail(MGS_ERR_INVALID_ARG, w + ": state is required");
+	if (P > 0 && (!xyz || !rot || !index || !weight))
+		return fail(MGS_ERR_INVALID_ARG, w + ": xyz, rot, index and weight are required with P > 0");
+	if (N > 0 && (!node_xyz || !node_rot || !node_t))
+		return fail(MGS_ERR_INVALID_ARG, w + ": node_xyz, node_rot and node_t are required with N > 0");
+	return 0;
+}
+
+int mgs_deform(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz, const float* node_rot,
+	const float* node_t, const long long* index, const float* weight, float* out_xyz, float* out_rot, int debug, void* stream)
+{
+	using namespace mgs;
+	if (int r = deform_args("mgs_deform", state, P, N, k, xyz, rot, node_xyz, node_rot, node_t, index, weight)) return r;
+	if (P > 0 && (!out_xyz || !out_rot)) return fail(MGS_ERR_INVALID_ARG, "mgs_deform: out_xyz and out_rot are required with P > 0");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(deform_forward(state, P, N, k, xyz, rot, node_xyz, node_rot, node_t, index, weight, out_xyz, out_rot, st));
+	MGS_STAGE("deform");
+	return 0;
+}
+
+int mgs_deform_backward(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz,
+	const float* node_rot, const float* node_t, const long long* index, const float* weight, const float* dL_dout_xyz,
+	const float* dL_dout_rot, float* dL_dxyz, float* dL_drot, float* dL_dnode_xyz, float* dL_dnode_rot, float* dL_dnode_t,
+	float* dL_dweight, int debug, void* stream)
+{
+	using namespace mgs;
+	if (int r = deform_args("mgs_deform_backward", state, P, N, k, xyz, rot, node_xyz, node_rot, node_t, index, weight)) return r;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(deform_backward(state, P, N, k, xyz, rot, node_xyz, node_rot, index, weight, dL_dout_xyz, dL_dout_rot, dL_dxyz,
+	                         dL_drot, dL_dnode_xyz, dL_dnode_rot, dL_dnode_t, dL_dweight, st));
+	MGS_STAGE("deform_bwd");
+	return 0;
+}

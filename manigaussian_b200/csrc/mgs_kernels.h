@@ -620,4 +620,18 @@ cudaError_t neighbour_reg_backward(void* state, int P, int k, const float* rot, 
 	const float* weight, const float* dL_dloss, float* dL_dxyz, float* dL_drot, float* dL_dxyz_next, float* dL_drot_next,
 	cudaStream_t st);
 
+// deform.cu: a cloud deformed by a sparse control graph, each Gaussian blending the rigid motions of the nodes of its [P,k]
+// index row (include/mgs_rasterizer.h, mgs_deform).  The state (deform_state_bytes, any alignment) holds the node records the
+// forward writes, each Gaussian's unnormalised quaternion blend, and the backward's node accumulators; the backward reads
+// what the forward with the same inputs left there.  Nothing is read back to the host.
+constexpr int DEFORM_MAX_K = 32;
+size_t deform_state_bytes(int P, int N);
+cudaError_t deform_forward(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz,
+	const float* node_rot, const float* node_t, const long long* index, const float* weight, float* out_xyz, float* out_rot,
+	cudaStream_t st);
+cudaError_t deform_backward(void* state, int P, int N, int k, const float* xyz, const float* rot, const float* node_xyz,
+	const float* node_rot, const long long* index, const float* weight, const float* dL_dout_xyz, const float* dL_dout_rot,
+	float* dL_dxyz, float* dL_drot, float* dL_dnode_xyz, float* dL_dnode_rot, float* dL_dnode_t, float* dL_dweight,
+	cudaStream_t st);
+
 }  // namespace mgs

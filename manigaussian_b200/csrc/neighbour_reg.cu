@@ -19,12 +19,12 @@
 #include "../../include/mgs_rasterizer.h"
 #include "mgs_common.cuh"
 #include "mgs_kernels.h"
+#include "quat.cuh"
 
 namespace mgs {
 
 constexpr int NR_WARPS = 8;        // Gaussians (warps) per pair-kernel CTA
 constexpr int NR_REDUCE = 256;     // threads of the final reduce
-constexpr float NR_EPS = 1e-12f;   // F.normalize's clamp of the norm
 
 static_assert(NEIGHBOUR_REG_MAX_K == 32, "one lane per slot");
 
@@ -61,33 +61,6 @@ size_t neighbour_reg_state_bytes(int P) { return NrState::at(nullptr, P).end + 2
 
 static char* align_state(void* state) { return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(state) + 255) & ~uintptr_t(255)); }
 
-struct Quat { float r, x, y, z; };
-
-__device__ __forceinline__ Quat qmul(const Quat& a, const Quat& b)  // Hamilton product (r, x, y, z), as INTEGRATION.md's qmul
-{
-	return {a.r * b.r - a.x * b.x - a.y * b.y - a.z * b.z, a.r * b.x + a.x * b.r + a.y * b.z - a.z * b.y,
-	        a.r * b.y - a.x * b.z + a.y * b.r + a.z * b.x, a.r * b.z + a.x * b.y - a.y * b.x + a.z * b.r};
-}
-__device__ __forceinline__ Quat conj(const Quat& a) { return {a.r, -a.x, -a.y, -a.z}; }
-__device__ __forceinline__ float qnorm(const float4& v) { return sqrtf(v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w); }
-__device__ __forceinline__ Quat normalized(const float4& v, float n)  // F.normalize: v / max(|v|, 1e-12)
-{
-	const float d = fmaxf(n, NR_EPS);
-	return {v.x / d, v.y / d, v.z / d, v.w / d};
-}
-// the backward of F.normalize: dL/dv from dL/dq, q = v / max(n, eps); the norm's gradient only where the clamp is not active
-__device__ __forceinline__ float4 normalize_bwd(const float4& v, float n, const Quat& q, const Quat& g)
-{
-	if (n >= NR_EPS) {
-		const float qg = q.r * g.r + q.x * g.x + q.y * g.y + q.z * g.z;
-		return make_float4((g.r - q.r * qg) / n, (g.x - q.x * qg) / n, (g.y - q.y * qg) / n, (g.z - q.z * qg) / n);
-	}
-	return make_float4(g.r / NR_EPS, g.x / NR_EPS, g.y / NR_EPS, g.z / NR_EPS);
-}
-// scalar accesses: a [P,4] tensor need not start on a 16-byte boundary (a slice of a larger one)
-__device__ __forceinline__ float4 ld4(const float* p) { return make_float4(p[0], p[1], p[2], p[3]); }
-__device__ __forceinline__ void st4(float* p, const float4& v) { p[0] = v.x; p[1] = v.y; p[2] = v.z; p[3] = v.w; }
-
 __device__ __forceinline__ Quat rel_of(const float* rot, const float* rot_next, int i)
 {
 	const float4 a = ld4(rot + 4 * (size_t)i), b = ld4(rot_next + 4 * (size_t)i);
@@ -105,10 +78,11 @@ __global__ void __launch_bounds__(256) nr_prologue_kernel(int P, const float* __
 	rec[3 * i + 0] = make_float4(p[0], p[1], p[2], n[0]);
 	rec[3 * i + 1] = make_float4(n[1], n[2], q.r, q.x);
 	rec[3 * i + 2] = make_float4(q.y, q.z, 0.f, 0.f);
-	const float r = q.r, x = q.x, y = q.y, z = q.z;  // INTEGRATION.md's qrot, rel not renormalised
-	rmat[3 * i + 0] = make_float4(1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y), 0.f);
-	rmat[3 * i + 1] = make_float4(2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x), 0.f);
-	rmat[3 * i + 2] = make_float4(2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y), 0.f);
+	float4 R[3];  // INTEGRATION.md's qrot, rel not renormalised
+	qrot_rows(q, R);
+	rmat[3 * i + 0] = R[0];
+	rmat[3 * i + 1] = R[1];
+	rmat[3 * i + 2] = R[2];
 }
 
 // One slot's geometry: the offsets o = xyz_j - xyz_i, o' = xyz_next_j - xyz_next_i, d = o' - R_i o and v = rel_j - rel_i.
@@ -245,22 +219,15 @@ __global__ void __launch_bounds__(32 * NR_WARPS) nr_bwd_pairs_kernel(int P, int 
 		if (need & 2) red_add_v4(reinterpret_cast<float*>(gxn + j), dxn[0], dxn[1], dxn[2], 0.f);
 		if (need & 4) red_add_v4(reinterpret_cast<float*>(grel + j), e[0], e[1], e[2], e[3]);
 		// dL/dR_i = -u o^T, chained to rel_i = (r, x, y, z) through qrot: dL/drel_c = sum_ab G_ab dR_ab/drel_c
-		const float r = ri[1].z, x = ri[1].w, y = ri[2].x, z = ri[2].y;
 		float G[3][3];
 #pragma unroll
 		for (int aa = 0; aa < 3; aa++)
 #pragma unroll
 			for (int b = 0; b < 3; b++) G[aa][b] = -u[aa] * s.o[b];
-		const float gr = 2.f * (-z * G[0][1] + y * G[0][2] + z * G[1][0] - x * G[1][2] - y * G[2][0] + x * G[2][1]);
-		const float gx_ = 2.f * (y * G[0][1] + z * G[0][2] + y * G[1][0] - 2.f * x * G[1][1] - r * G[1][2] + z * G[2][0]
-		                         + r * G[2][1] - 2.f * x * G[2][2]);
-		const float gy = 2.f * (-2.f * y * G[0][0] + x * G[0][1] + r * G[0][2] + x * G[1][0] + z * G[1][2] - r * G[2][0]
-		                        + z * G[2][1] - 2.f * y * G[2][2]);
-		const float gz = 2.f * (-2.f * z * G[0][0] - r * G[0][1] + x * G[0][2] + r * G[1][0] - 2.f * z * G[1][1] + y * G[1][2]
-		                        + x * G[2][0] + y * G[2][1]);
+		const Quat gq = qrot_bwd({ri[1].z, ri[1].w, ri[2].x, ri[2].y}, G);
 		gi[0] = -dx[0]; gi[1] = -dx[1]; gi[2] = -dx[2];
 		gi[3] = -dxn[0]; gi[4] = -dxn[1]; gi[5] = -dxn[2];
-		gi[6] = gr - e[0]; gi[7] = gx_ - e[1]; gi[8] = gy - e[2]; gi[9] = gz - e[3];
+		gi[6] = gq.r - e[0]; gi[7] = gq.x - e[1]; gi[8] = gq.y - e[2]; gi[9] = gq.z - e[3];
 	}
 #pragma unroll
 	for (int m = 16; m > 0; m >>= 1)

@@ -25,7 +25,7 @@ from . import gaussian_params as _gp
 from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, camera_rays_backward_raw,
-                         camera_rays_raw, field_query_backward_raw,
+                         camera_rays_raw, deform_backward_raw, deform_raw, field_query_backward_raw,
                          field_query_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
                          visibility_views_backward_raw, rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
@@ -974,6 +974,66 @@ def neighbour_regularisers(xyz, rot, xyz_next, rot_next, index, weight):
         raise ValueError(f"{where}: weight requires grad, but no gradient flows to it: pass weight.detach()")
     rigid, rotation, isometry = _NeighbourReg.apply(xyz, rot, xyz_next, rot_next, index, weight)
     return {"rigid": rigid, "rotation": rotation, "isometry": isometry}
+
+
+class _Deform(torch.autograd.Function):
+    """a cloud deformed by a control graph: one node, differentiable in xyz, rot, node_xyz, node_rot, node_t and weight"""
+
+    @staticmethod
+    def forward(ctx, xyz, rot, node_xyz, node_rot, node_t, index, weight):
+        out_xyz, out_rot, state = deform_raw(xyz.detach(), rot.detach(), node_xyz.detach(), node_rot.detach(), node_t.detach(),
+                                             index, weight.detach())
+        ctx.save_for_backward(xyz, rot, node_xyz, node_rot, node_t, index, weight, state)
+        return out_xyz, out_rot
+
+    @staticmethod
+    def backward(ctx, g_xyz, g_rot):
+        xyz, rot, node_xyz, node_rot, node_t, index, weight, state = ctx.saved_tensors
+        n = ctx.needs_input_grad
+        needs = (n[0], n[1], n[2], n[3], n[4], n[6])
+        if not any(needs):
+            return (None,) * 7
+        g = deform_backward_raw(state, xyz.detach(), rot.detach(), node_xyz.detach(), node_rot.detach(), node_t.detach(), index,
+                                weight.detach(), g_xyz, g_rot, needs=needs)
+        return g[:5] + (None, g[5])
+
+
+def deform_gaussians(xyz, rot, node_xyz, node_rot, node_t, index, weight):
+    """A cloud deformed by a sparse control graph (embedded deformation, SC-GS; INTEGRATION.md §20), fused (definition in
+    include/mgs_rasterizer.h, mgs_deform).  xyz [P,3] and rot [P,4] are the cloud, node_xyz [N,3], node_rot [N,4] and
+    node_t [N,3] the control nodes (N >= 0), all float32 on one CUDA device, quaternions (r, x, y, z), real part first;
+    index [P,k] int64 with k = 1 .. 32, as knn(node_xyz, k, queries=xyz) returns it (slots outside 0 .. N-1, such as knn's
+    -1 padding, are skipped); weight [P,k] float32, used exactly as given.  With q^_j = normalize(node_rot_j) (negated where
+    its real part is below 0), R_j its rotation matrix and c_j = node_xyz_j + node_t_j - R_j node_xyz_j, each Gaussian moves to
+        xyz'_i = xyz_i + sum_s w (R_j xyz_i + c_j - xyz_i),   rot'_i = normalize(e + sum_s w (q^_j - e)) (x) rot_i
+    over its valid slots, e = (1, 0, 0, 0).  Weight missing from 1 goes to the identity motion.  Returns {"xyz": [P,3],
+    "rot": [P,4]}, both outputs of one autograd node, differentiable in xyz, rot, node_xyz, node_rot, node_t and weight (only
+    the gradients autograd asks for are computed).  Nothing is read back to the host.  Raises ValueError for a shape, dtype
+    or device mismatch, index not int64 [P,k] and k outside 1 .. 32."""
+    where = "deform_gaussians"
+    tensors = (("xyz", xyz), ("rot", rot), ("node_xyz", node_xyz), ("node_rot", node_rot), ("node_t", node_t),
+               ("index", index), ("weight", weight))
+    for name, t in tensors:
+        if not torch.is_tensor(t):
+            raise ValueError(f"{where}: {name}: expected a tensor, got {type(t)}")
+    P = xyz.shape[0] if xyz.dim() == 2 else -1
+    N = node_xyz.shape[0] if node_xyz.dim() == 2 else -1
+    k = index.shape[1] if index.dim() == 2 else -1
+    want = {"xyz": (P, 3), "rot": (P, 4), "node_xyz": (N, 3), "node_rot": (N, 4), "node_t": (N, 3), "index": (P, k),
+            "weight": (P, k)}
+    for name, t in tensors:
+        rows, cols = want[name]
+        if tuple(t.shape) != want[name] or rows < 0:
+            raise ValueError(f"{where}: {name}: expected [{rows},{'k' if name in ('index', 'weight') else cols}], "
+                             f"got {tuple(t.shape)}")
+        if t.dtype != (torch.int64 if name == "index" else torch.float32):
+            raise ValueError(f"{where}: {name}: expected {'int64' if name == 'index' else 'float32'}, got {t.dtype}")
+        if t.device != xyz.device:
+            raise ValueError(f"{where}: {name}: expected a tensor on {xyz.device}, got {t.device}")
+    if not 1 <= k <= 32:
+        raise ValueError(f"{where}: k must be in 1 .. 32, got {k}")
+    out_xyz, out_rot = _Deform.apply(xyz, rot, node_xyz, node_rot, node_t, index, weight)
+    return {"xyz": out_xyz, "rot": out_rot}
 
 
 class _QueryField(torch.autograd.Function):

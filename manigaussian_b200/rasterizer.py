@@ -2192,3 +2192,47 @@ def neighbour_reg_backward_raw(state, xyz, rot, xyz_next, rot_next, index, weigh
                                               _ptr(index), _ptr(weight), _ptr(grad_loss), *[_ptr(o) for o in outs],
                                               int(bool(debug)), _stream(dev)), "mgs_neighbour_reg_backward")
     return tuple(outs)
+
+
+def deform_raw(xyz, rot, node_xyz, node_rot, node_t, index, weight, debug=False):
+    """A cloud xyz [P,3], rot [P,4] deformed by control nodes node_xyz [N,3], node_rot [N,4], node_t [N,3] over index [P,k]
+    int64 with weight [P,k] (C ABI mgs_deform; definition in include/mgs_rasterizer.h).  Returns (out_xyz [P,3],
+    out_rot [P,4], state) on xyz's device; the state is what deform_backward_raw reads.  Nothing is read back to the host,
+    so a call can be captured in a CUDA graph.  Not differentiable."""
+    if not all(t.is_cuda for t in (xyz, rot, node_xyz, node_rot, node_t, index, weight)):
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = xyz.device
+    xyz, rot, node_xyz, node_rot, node_t, weight = (_prep(t, dev) for t in (xyz, rot, node_xyz, node_rot, node_t, weight))
+    index = index.to(device=dev, dtype=torch.int64).contiguous()
+    P, k = index.shape
+    N = node_xyz.shape[0]
+    out_xyz = torch.empty((P, 3), dtype=torch.float32, device=dev)
+    out_rot = torch.empty((P, 4), dtype=torch.float32, device=dev)
+    state = torch.empty(int(L.mgs_deform_state_bytes(P, N, k)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_deform(_ptr(state), P, N, k, _ptr(xyz), _ptr(rot), _ptr(node_xyz), _ptr(node_rot), _ptr(node_t),
+                              _ptr(index), _ptr(weight), _ptr(out_xyz), _ptr(out_rot), int(bool(debug)), _stream(dev)),
+                 "mgs_deform")
+    return out_xyz, out_rot, state
+
+
+def deform_backward_raw(state, xyz, rot, node_xyz, node_rot, node_t, index, weight, grad_xyz, grad_rot, needs=(True,) * 6,
+                        debug=False):
+    """Backward of deform_raw (C ABI mgs_deform_backward) with the state its forward returned for the same inputs:
+    grad_xyz [P,3] and grad_rot [P,4], each None for zero.  Returns (dL_dxyz, dL_drot, dL_dnode_xyz, dL_dnode_rot,
+    dL_dnode_t, dL_dweight), each None where `needs` is False."""
+    L = _b.lib()
+    dev = xyz.device
+    xyz, rot, node_xyz, node_rot, node_t, weight, grad_xyz, grad_rot = (
+        _prep(t, dev) for t in (xyz, rot, node_xyz, node_rot, node_t, weight, grad_xyz, grad_rot))
+    index = index.to(device=dev, dtype=torch.int64).contiguous()
+    P, k = index.shape
+    N = node_xyz.shape[0]
+    shapes = ((P, 3), (P, 4), (N, 3), (N, 4), (N, 3), (P, k))
+    outs = [torch.empty(s, dtype=torch.float32, device=dev) if n else None for n, s in zip(needs, shapes)]
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_deform_backward(_ptr(state), P, N, k, _ptr(xyz), _ptr(rot), _ptr(node_xyz), _ptr(node_rot),
+                                       _ptr(node_t), _ptr(index), _ptr(weight), _ptr(grad_xyz), _ptr(grad_rot),
+                                       *[_ptr(o) for o in outs], int(bool(debug)), _stream(dev)), "mgs_deform_backward")
+    return tuple(outs)
