@@ -1554,6 +1554,34 @@ int mgs_deform_backward(void* state, int P, int N, int k, const float* xyz, cons
 	const float* dL_dout_rot, float* dL_dxyz, float* dL_drot, float* dL_dnode_xyz, float* dL_dnode_rot, float* dL_dnode_t,
 	float* dL_dweight, int debug, void* stream);
 
+/*
+ * Farthest-point sampling (no reference counterpart; SC-GS control nodes, point-cloud policy inputs): n picks from each of
+ * B clouds points [B,P,3].  Cloud b is points[b, :L_b] with L_b = lengths[b] clamped to 0 .. P (P when lengths is NULL).
+ *   - Only points with three finite coordinates can be picked.  Each starts with d_i = +inf.
+ *   - Pick 0 is start[b] when start is given and start[b] is a finite point in 0 .. L_b - 1; otherwise the lowest-index
+ *     finite point (which the argmax rule below gives when every d is +inf).
+ *   - After each pick s, every unpicked finite point i takes d_i = min(d_i, D(i, s)), and s is never picked again.  D is
+ *     the fp32 squared distance in a fixed order with every operation rounded to float32 and no FMA contraction:
+ *       dx = x_i - x_s, dy = y_i - y_s, dz = z_i - z_s,   D = ((dx*dx) + (dy*dy)) + (dz*dz)
+ *   - Pick t >= 1 is the unpicked finite point with the largest d; ties go to the lower index.
+ *   - out_index [B,n] is each pick as an index into its cloud; out_dist2 [B,n] is its d at the time of the pick, the squared
+ *     distance to the nearest earlier pick (out_dist2[b,0] = +inf).  Where fewer than n finite points exist, the rest of
+ *     the row is index -1, d2 = +inf.  So the picks of a row are distinct, out_dist2[b,1:] never increases along the valid
+ *     picks, and duplicate points are picked at d2 = 0 in ascending index once every distinct position is taken.
+ *   - The outputs are bitwise identical from call to call.
+ *   - lengths [B] and start [B] (each NULL to omit) are in device memory and never read by the host.
+ *   - state: mgs_fps_state_bytes(B, P) bytes of device memory (contents irrelevant on entry).
+ *   - B = 0 or n = 0 returns 0 and enqueues nothing; P = 0 pads every slot.
+ * Method: one thread-block cluster per cloud, its CTAs holding the cloud's points and their d in registers (clouds above
+ * 131,072 points stream a packed copy kept in the state), one cluster-wide argmax through distributed shared memory per
+ * pick.  Nothing allocates, blocks or reads back to the host: a call can be captured in a CUDA graph.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_INVALID_ARG for B, P or n < 0,
+ * and for a NULL state, out_index or out_dist2 (B > 0 and n > 0) or points (also P > 0).
+ */
+size_t mgs_fps_state_bytes(int B, int P);
+int mgs_fps(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
+	long long* out_index, float* out_dist2, int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

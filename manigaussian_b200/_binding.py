@@ -284,6 +284,11 @@ def lib():
         vp, vp,                  # dL_dout_xyz dL_dout_rot
         vp, vp, vp, vp, vp, vp,  # dL_d{xyz,rot,node_xyz,node_rot,node_t,weight}
         i, vp]                   # debug stream
+    L.mgs_fps_state_bytes.restype = C.c_size_t
+    L.mgs_fps_state_bytes.argtypes = [C.c_int, C.c_int]
+    L.mgs_fps.restype = C.c_int
+    L.mgs_fps.argtypes = [vp, i, i, i, vp, vp, vp,  # state B P n points lengths start
+                          vp, vp, i, vp]            # out_index out_dist2 debug stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -354,6 +359,7 @@ EXPORTED_SYMBOLS = (
     "mgs_knn_state_bytes", "mgs_knn",
     "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
     "mgs_deform_state_bytes", "mgs_deform", "mgs_deform_backward",
+    "mgs_fps_state_bytes", "mgs_fps",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

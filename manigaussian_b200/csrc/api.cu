@@ -2781,3 +2781,22 @@ int mgs_deform_backward(void* state, int P, int N, int k, const float* xyz, cons
 	MGS_STAGE("deform_bwd");
 	return 0;
 }
+
+size_t mgs_fps_state_bytes(int B, int P)
+{
+	return mgs::fps_state_bytes(std::max(B, 0), std::max(P, 0));
+}
+
+int mgs_fps(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
+	long long* out_index, float* out_dist2, int debug, void* stream)
+{
+	using namespace mgs;
+	if (B < 0 || P < 0 || n < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_fps: B, P and n must be >= 0");
+	if (B == 0 || n == 0) return 0;
+	if (!state || !out_index || !out_dist2) return fail(MGS_ERR_INVALID_ARG, "mgs_fps: state, out_index and out_dist2 are required");
+	if (P > 0 && !points) return fail(MGS_ERR_INVALID_ARG, "mgs_fps: points are required with P > 0");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(fps_run(state, B, P, n, points, lengths, start, out_index, out_dist2, st));
+	MGS_STAGE("fps");
+	return 0;
+}

@@ -634,4 +634,11 @@ cudaError_t deform_backward(void* state, int P, int N, int k, const float* xyz, 
 	float* dL_dxyz, float* dL_drot, float* dL_dnode_xyz, float* dL_dnode_rot, float* dL_dnode_t, float* dL_dweight,
 	cudaStream_t st);
 
+// fps.cu: farthest-point sampling of B clouds [B,P,3], n picks each (include/mgs_rasterizer.h, mgs_fps); one thread-block
+// cluster per cloud, the cluster size and the points-per-thread tier chosen on the host from P.  The state
+// (fps_state_bytes) holds the packed {x, y, z, d} copy of the streaming tier; nothing is read back to the host.
+size_t fps_state_bytes(int B, int P);
+cudaError_t fps_run(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
+	long long* out_index, float* out_dist2, cudaStream_t st);
+
 }  // namespace mgs

@@ -26,7 +26,7 @@ from .cameras import CameraBatch
 from .parallel import PackedGradients
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, _prep, _prep_clouds, camera_rays_backward_raw,
                          camera_rays_raw, deform_backward_raw, deform_raw, field_query_backward_raw,
-                         field_query_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
+                         field_query_raw, fps_raw, knn_raw, lift_views_raw, neighbour_reg_backward_raw, neighbour_reg_raw, visibility_views_raw,
                          visibility_views_backward_raw, rasterize_clouds_backward_raw, rasterize_clouds_raw, rasterize_views_backward_raw, rasterize_views_raw)
 
 _BG_CACHE = {}
@@ -915,6 +915,46 @@ def knn(points, k, queries=None):
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 32:
         raise ValueError(f"knn: k must be an int in 1 .. 32, got {k!r}")
     index, dist2 = knn_raw(points.detach(), k, None if queries is None else queries.detach())
+    return {"index": index, "dist2": dist2}
+
+
+def farthest_point_sample(points, n, lengths=None, start=None):
+    """Farthest-point sampling (INTEGRATION.md §21): n picks from a cloud, each the unpicked finite point farthest from the
+    picks before it by the fp32 squared distance D = ((dx*dx) + (dy*dy)) + (dz*dz), every operation rounded to float32
+    (no FMA), ties to the lower index.  Pick 0 is `start` when it names a finite point of the cloud, else the lowest-index
+    finite point.  Only points with three finite coordinates are picked.
+    points [P,3] or [B,P,3] float32 on a CUDA device; lengths int64 [B] on the same device (cloud b is points[b, :lengths[b]],
+    clamped to 0 .. P), or None; start int64 [B] on the same device ([] or [1] for a [P,3] cloud), or None.  n >= 0.
+    Returns {"index": int64, "dist2": float32}, each [n] or [B,n]: the picks as indices into their cloud, and each pick's
+    squared distance to the nearest earlier pick (+inf for pick 0).  Where fewer than n finite points exist the rest of the
+    row holds index -1 and d2 = +inf.  The outputs are bitwise identical from call to call.
+    Neither output is differentiable (inputs that require grad are detached): gather points[index] for gradients.
+    Nothing is read back to the host, so a call can be captured in a CUDA graph.  Raises ValueError for a non-float32 or
+    non-[.,3] / [.,.,3] points, a non-int64 or misshapen lengths or start, tensors on different devices and an n that is not
+    an int >= 0."""
+    if not torch.is_tensor(points) or points.dim() not in (2, 3) or points.shape[-1] != 3:
+        got = tuple(points.shape) if torch.is_tensor(points) else type(points)
+        raise ValueError(f"farthest_point_sample: points: expected [P,3] or [B,P,3], got {got}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"farthest_point_sample: points: expected float32, got {points.dtype}")
+    batched = points.dim() == 3
+    B = points.shape[0] if batched else 1
+    for name, t in (("lengths", lengths), ("start", start)):
+        if t is None:
+            continue
+        if not torch.is_tensor(t) or t.dtype != torch.int64:
+            raise ValueError(f"farthest_point_sample: {name}: expected int64, got {t.dtype if torch.is_tensor(t) else type(t)}")
+        if tuple(t.shape) not in (((B,),) if batched else ((), (1,))):
+            raise ValueError(f"farthest_point_sample: {name}: expected [{B if batched else '] or [1'}], got {tuple(t.shape)}")
+        if t.device != points.device:
+            raise ValueError(f"farthest_point_sample: {name}: expected a tensor on {points.device}, got {t.device}")
+    if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+        raise ValueError(f"farthest_point_sample: n must be an int >= 0, got {n!r}")
+    p = points.detach() if batched else points.detach()[None]
+    lengths, start = (None if t is None else t.reshape(B) for t in (lengths, start))
+    index, dist2 = fps_raw(p, n, lengths, start)
+    if not batched:
+        index, dist2 = index[0], dist2[0]
     return {"index": index, "dist2": dist2}
 
 

@@ -2236,3 +2236,27 @@ def deform_backward_raw(state, xyz, rot, node_xyz, node_rot, node_t, index, weig
                                        _ptr(node_t), _ptr(index), _ptr(weight), _ptr(grad_xyz), _ptr(grad_rot),
                                        *[_ptr(o) for o in outs], int(bool(debug)), _stream(dev)), "mgs_deform_backward")
     return tuple(outs)
+
+
+def fps_raw(points, n, lengths=None, start=None, debug=False):
+    """Farthest-point sampling of n picks from each cloud of `points` [B,P,3] (C ABI mgs_fps; definition in
+    include/mgs_rasterizer.h), each cloud cut to lengths[b] points ([B] int64, or None for all P) and started at start[b]
+    ([B] int64, or None).  Returns (index [B,n] int64, dist2 [B,n] float32) on the points' device, padded with index -1 and
+    d2 = +inf.  The state is allocated with torch and nothing is read back, so a call can be captured in a CUDA graph.  Not
+    differentiable."""
+    if not points.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = points.device
+    points = _prep(points, dev)
+    lengths, start = (None if t is None else t.to(device=dev, dtype=torch.int64).contiguous() for t in (lengths, start))
+    B, P = points.shape[0], points.shape[1]
+    index = torch.empty((B, n), dtype=torch.int64, device=dev)
+    dist2 = torch.empty((B, n), dtype=torch.float32, device=dev)
+    if B == 0 or n == 0:
+        return index, dist2
+    state = torch.empty(int(L.mgs_fps_state_bytes(B, P)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):  # the cluster sizes are looked up for the device current at the call
+        _b.check(L.mgs_fps(_ptr(state), B, P, int(n), _ptr(points), _ptr(lengths), _ptr(start), _ptr(index), _ptr(dist2),
+                           int(bool(debug)), _stream(dev)), "mgs_fps")
+    return index, dist2
