@@ -200,6 +200,9 @@ int mgs_backward(
  * which is summed into views[0].dL_dmean2D (shared_mean2D = 1).  Output NULL-ability as in mgs_backward.
  * `stages` splits the call in two so that a multi-GPU caller can start the all-reduce of dL_dfeature -- more than half of
  * the message, final after the blend stage -- while the per-Gaussian stage computes the remaining fields.
+ * Every optional input of these calls and of the multi-cloud calls (extra planes, loss heads, camera models, gradients of
+ * the camera) is a field of one mgs_render_options record, declared below after the structs it points to; the sections
+ * between here and there describe each field.  A NULL record turns every one of them off.
  */
 typedef struct mgs_view {
 	const float* viewmatrix;     /* device, 16 floats */
@@ -240,45 +243,6 @@ typedef struct mgs_view {
 	const float* cot_scale;
 } mgs_view;
 
-int mgs_forward_views(
-	int V, const mgs_view* views,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views(
-	int V, const mgs_view* views,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,            /* 1: blend stage of every view (dL_dfeature is final afterwards), 2: the per-Gaussian stage, 3: both */
-	int debug,
-	void* join_stream);
 
 /*
  * Several clouds in one step (no reference counterpart).  A ManiGaussian training step with the dynamic field renders two
@@ -307,16 +271,11 @@ typedef struct mgs_cloud {
 	float *dL_dmean3D, *dL_dopacity, *dL_dcolor, *dL_dfeature, *dL_dcov3D, *dL_dsh, *dL_dscale, *dL_drot;
 } mgs_cloud;
 
-int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
  * Alpha plane (no reference counterpart): the pixel's accumulated opacity alpha = 1 - final_T, e.g. for a mask loss or for
  * the expected depth out_depth / alpha (out_depth has no background term and falls to 0 where nothing covers the pixel).
- * The four calls below are the multi-view and multi-cloud calls above with one more argument, `alpha`: one mgs_view_alpha
- * per view (V entries, or view_offsets[B] for clouds), or NULL for none; the calls above are these with alpha == NULL.
+ * mgs_render_options.alpha: one mgs_view_alpha per view, or NULL for none.
  * Forward: out_alpha [H,W] is fully overwritten.  Backward: dL_dpix_alpha [H,W] adds T_final / (1 - a_k) * dL_dalpha to
  * every contributor's dL/da_k (cot_scale does not scale it); a pixel nothing blended into has no alpha gradient.
  * Either pointer may be NULL per view.  mgs_view and mgs_cloud keep their layouts: existing arrays of them stay valid.
@@ -326,49 +285,6 @@ typedef struct mgs_view_alpha {
 	const float* dL_dpix_alpha;  /* backward input [H,W], or NULL */
 } mgs_view_alpha;
 
-int mgs_forward_views_alpha(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_alpha(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
  * Depth and mask heads (no reference counterpart; INTEGRATION.md §4): two more loss heads beside the fused colour and
@@ -378,9 +294,8 @@ int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_of
  *   depth  valid = (target_depth > 0) && (A > 0.5), d = D / A, n = sum valid:  loss_depth = sum_valid |d - target_depth| / n
  *          (0 when n = 0);
  *   mask   loss_mask = mean_px BCE(clamp(A, 1e-4, 1 - 1e-4), target_mask) as torch.nn.functional.binary_cross_entropy.
- * The calls below are the _alpha calls with one more argument, `depth_mask`: one mgs_view_depth_mask per view (V entries,
- * or view_offsets[B] for clouds), or NULL for none; the _alpha calls are these with depth_mask == NULL.  Pass the same
- * array to the forward and the backward.  A view whose two targets are NULL has no depth or mask head.
+ * mgs_render_options.depth_mask: one mgs_view_depth_mask per view, or NULL for none.  Pass the same array to the forward
+ * and the backward.  A view whose two targets are NULL has no depth or mask head.
  * Forward: the heads need the colour head (the view's target_color).  loss_acc (device, 3 floats, zeroed by the call)
  * receives {sum_valid |d - g|, n, sum_px BCE}: loss_depth = loss_acc[0] / max(loss_acc[1], 1), loss_mask = loss_acc[2] / N.
  * With target_depth, cot_depth and cot_alpha_depth [H,W] receive the unscaled cotangents sign(d - g) / A and
@@ -400,51 +315,6 @@ typedef struct mgs_view_depth_mask {
 	const float* cot_scale;        /* device, 2 floats, or NULL */
 } mgs_view_depth_mask;
 
-int mgs_forward_views_depth_mask(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_depth_mask(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int prefiltered,
-	int debug, void* join_stream);
-int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
-	int debug, void* join_stream);
 
 /*
  * Anti-aliased projection (Mip-Splatting's "2D filter"; the `antialiasing` setting of the 3DGS authors' current rasterizer,
@@ -454,55 +324,9 @@ int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* vi
  * so that the dilated splat carries the energy of the undilated one: the blend sees o_eff = o s.  The conic, radius, screen
  * mean, depth, tiles, instance count and sort keys are those of antialiasing = 0, bit for bit.  The backward chains dL/do_eff
  * to dL/do and, through s, to the covariance (and so to means, scales, rotations or cov3D).
- * The calls below are the _depth_mask calls with one more argument, `antialiasing` (0 or 1); the _depth_mask calls are these
- * with 0.  Pass the same value to the forward and the backward: the backward reads o_eff back from the forward's geometry
+ * mgs_render_options.antialiasing: 0 or 1, for every view of the call.  Pass the same value to the forward and the backward: the backward reads o_eff back from the forward's geometry
  * state.  Any other value returns MGS_ERR_INVALID_ARG before anything is enqueued.
  */
-int mgs_forward_views_aa(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_aa(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
-	int accumulate, int debug, void* join_stream);
 
 /*
  * L1 + SSIM photometric loss (no reference counterpart in the rasterizer; the objective 3DGS trains with,
@@ -520,8 +344,7 @@ int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offse
  *   dS/dmu_x = 2 mu_g (B - A) / (C D) - 2 mu_x S (1/C - 1/D),  dS/dE[x^2] = -S / D,  dS/dE[xg] = 2 A / (C D),
  *   d ssim / dx = (G(*)dS/dmu_x + 2 x G(*)dS/dE[x^2] + g G(*)dS/dE[xg]) / N.
  * Images smaller than the window (down to 1x1) are valid.
- * The calls below are the _aa calls with one more argument, `ssim`: one mgs_view_ssim per view (V entries, or view_offsets[B]
- * for clouds), or NULL for none; the _aa calls are these with ssim == NULL.  Every entry of a non-NULL array is an SSIM head.
+ * mgs_render_options.ssim: one mgs_view_ssim per view, or NULL for none.  Every entry of a non-NULL array is an SSIM head.
  * Forward: behind the view's blend, on its stream, the head reads out_color and target_color, zeroes loss_acc and adds
  * {sum |x - g|, sum S} into loss_acc[0..1] (loss_l1 = loss_acc[0] / N, ssim = loss_acc[1] / N), and writes the unscaled
  * partials {dS/dmu_x, dS/dE[x^2], dS/dE[xg]} of every pixel into ssim_terms [3 partials x 3 channels, H, W].
@@ -540,58 +363,10 @@ typedef struct mgs_view_ssim {
 	float* cot_color;              /* [3,H,W]: receives the combined colour cotangent in the backward */
 } mgs_view_ssim;
 
-int mgs_forward_views_ssim(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_ssim(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
-	int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
-	int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
- * Camera gradients (no reference counterpart: the reference's backward returns None for the camera).  The calls below are
- * the _ssim backward calls with one more argument, `cam`: one mgs_view_camera_grad per view (V entries, or view_offsets[B]
- * for clouds), or NULL; the _ssim backward calls are these with cam == NULL.  An entry asks for the gradients of its view
+ * Camera gradients (no reference counterpart: the reference's backward returns None for the camera).
+ * mgs_render_options.camera_grad, read by the backward calls only: one mgs_view_camera_grad per view, or NULL.  An entry asks for the gradients of its view
  * when any of its three outputs is non-NULL; each output is written (accumulate = 0) or added to (accumulate = 1) by the
  * per-Gaussian stage (stage 2), a NULL output is skipped.  An entry with an output but no scratch returns
  * MGS_ERR_INVALID_ARG before anything is enqueued.
@@ -612,11 +387,11 @@ int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_off
  * The gradient of a 16-float array is the gradient with respect to those 16 floats, so as a torch [4,4] it is directly the
  * gradient of world_view_transform / full_proj_transform.  In these calls tan_fov, the focal lengths, the 1.3 tan_fov clamp
  * limit, the near-plane cull, the radii and the tiles are constants: a projmatrix built from a learnable focal length
- * receives only the screen-mean path.  The _intr calls below add the focal-length path through J and the clamp limit.
+ * receives only the screen-mean path.  mgs_render_options.intrinsics below adds the focal-length path through J and the
+ * clamp limit.
  * The sums are deterministic: every CTA of the per-Gaussian kernel writes one row of 27 partial sums per view into the
  * entry's scratch in a fixed order, and a reduce kernel on join_stream sums each view's rows in a fixed tree.  A view's rows
- * all come from one launch of at most 16 views.  These calls leave mgs_abi_version() at 300: they only add symbols, and a
- * caller detects them by symbol, as the _ssim calls.
+ * all come from one launch of at most 16 views.
  */
 typedef struct mgs_view_camera_grad {
 	float* dL_dviewmatrix;   /* device, 16 floats, or NULL */
@@ -626,39 +401,10 @@ typedef struct mgs_view_camera_grad {
 } mgs_view_camera_grad;
 
 size_t mgs_camera_grad_scratch_bytes(int P);
-int mgs_backward_views_cam(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
- * Learnable intrinsics (no reference counterpart).  The _intr calls are the _ssim forward and the _cam backward calls with one
- * more argument, `intr`: one mgs_view_intrinsics per view (V entries, or view_offsets[B] for clouds), or NULL; the older calls
- * are these with intr == NULL, and the calls above keep the definition given there.
+ * Learnable intrinsics (no reference counterpart).  mgs_render_options.intrinsics: one mgs_view_intrinsics per view, or NULL;
+ * without it the camera gradients keep the definition given above.
  *
  * Device field of view.  An entry's tan_fov, when set, points at the view's {tan_fovx, tan_fovy} in device memory, and the
  * projection forward and backward read it there in place of mgs_view.tan_fovx / tan_fovy: a value an optimizer step has just
@@ -677,66 +423,17 @@ int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offs
  *                  - [|t.x / tz| > 1.3 tan_fovx] fx dJ02 (+-1.3) / tz      (the clamp cx = +-1.3 tan_fovx tz, sign of t.x / tz)
  * and likewise dL/dtan_fovy with fy, dJ11, dJ12, cy.  The near-plane cull, the radii, the tiles and the sort stay constants.
  * The projection-matrix path of the focal lengths and the principal point is dL/dprojmatrix above, to be chained by the
- * caller (for a projmatrix built from K).  With intrinsics on, the 27 other camera terms are those the _cam calls write.
+ * caller (for a projmatrix built from K).  With intrinsics on, the 27 other camera terms are those camera_grad alone writes.
  */
 typedef struct mgs_view_intrinsics {
 	const float* tan_fov;    /* device, 2 floats, or NULL: use mgs_view.tan_fovx / tan_fovy */
 	float* dL_dtan_fov;      /* device, 2 floats, or NULL */
 } mgs_view_intrinsics;
 
-int mgs_forward_views_intr(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_intr(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
-	int debug, void* join_stream);
 
 /*
- * Median depth and surface Gaussian (no reference counterpart; 2DGS's median_contributor).  The _median calls are the _intr
- * calls with one more argument, `median`: one mgs_view_median per view (V entries, or view_offsets[B] for clouds), or NULL;
- * the _intr calls are these with median == NULL.
+ * Median depth and surface Gaussian (no reference counterpart; 2DGS's median_contributor).
+ * mgs_render_options.median: one mgs_view_median per view, or NULL.
  *
  * Definition.  For pixel p, walk its contributors front to back with the forward blend's own decisions (the pairs whose
  * pixel-mask bit is set, "pixel_masks" of mgs_state_array) and its fp32 transmittance T before each pair:
@@ -759,60 +456,10 @@ typedef struct mgs_view_median {
 	const float* dL_dpix_median_depth;    /* backward input [H,W], or NULL */
 } mgs_view_median;
 
-int mgs_forward_views_median(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_median(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F, float scale_modifier, int prefiltered,
-	int debug, void* join_stream);
-int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
- * Surface normals (no reference counterpart; the rend_normal plane of 2DGS / RaDe-GS / GaussianShader).  The _normal calls are
- * the _median calls with one more argument, `normal`: one mgs_view_normal per view (V entries, or view_offsets[B] for clouds),
- * or NULL; the _median calls are these with normal == NULL.
+ * Surface normals (no reference counterpart; the rend_normal plane of 2DGS / RaDe-GS / GaussianShader).
+ * mgs_render_options.normal: one mgs_view_normal per view, or NULL.
  *
  * Definition.  Per Gaussian i and view v, from scales [P,3] and rotations [P,4] (r, x, y, z):
  *   - k = argmin_j scales[i][j], the lowest index on ties (scale_modifier does not change it);
@@ -844,108 +491,11 @@ typedef struct mgs_view_normal {
 size_t mgs_geometry_state_bytes_normal(int P);
 size_t mgs_backward_scratch_bytes_normal(int P);
 
-int mgs_forward_views_normal(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	int prefiltered,
-	int debug,
-	void* join_stream);
-int mgs_backward_views_normal(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal,
-	int P, int D, int M, int F,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* feature_precomp,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* dL_dmean3D,
-	float* dL_dopacity,
-	float* dL_dcolor,
-	float* dL_dfeature,
-	float* dL_dcov3D,
-	float* dL_dsh,
-	float* dL_dscale,
-	float* dL_drot,
-	int shared_mean2D,
-	int accumulate,
-	int stages,
-	int debug,
-	void* join_stream);
-int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, int D, int M, int F,
-	float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
-
-/*
- * Lifting 2D maps onto the Gaussians (no reference counterpart; the lift of Gaussian Grouping, SAGA, Feature Splatting and
- * LUDVIG).  Given one map per view, mgs_lift_views computes per Gaussian g
- *   lifted[g][c] = sum_v sum_p w_vpg map_v[c][p],     weight[g] = sum_v sum_p w_vpg,
- * so lifted / weight is the Gaussian's blend-weighted average of the maps and weight alone its visibility over the views.
- * Definition.  For each view the contributors and weights are the forward blend's own: the same expf, the same skip tests
- * (power > 0, alpha < 1/255), the same 0.99 clamp, the same T (1 - alpha) < 1e-4 stop, and T the running product, so
- * w_vpg is bit for bit the weight with which the colour image of that view blends Gaussian g into pixel p (alpha with the
- * compensated opacity o_eff when antialiasing = 1).  There is no background term; pixels outside the image do not count.
- * lifted is dL/dfeature of a feature render (normalize_feature off) with cotangent map_v, without the backward's geometry.
- *   - map_v (mgs_view_lift.map) is [C,H,W] fp32, planar like the feature images; C in [0, MGS_MAX_FEATURE_CHANNELS] is the
- *     same for every view; with C = 0 only weight is computed and lift may be NULL.
- *   - out_lifted [P,C] (NULL allowed with C = 0) and out_weight [P] are zero-filled by the call on join_stream, then every
- *     view of the call is summed into them (float atomics: the order of the sums is not fixed).
- *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
- *     (sized as for mgs_forward_views) and binning_capacity, status and stream are used; background and every image,
- *     backward and loss-head field are ignored.  The view's state afterwards holds its projection and binning; the blend
- *     state (final_T, n_contrib, pixel masks, block_nwalk) is not written, so it cannot serve a backward.
- *   - shs or colors_precomp must be given as in mgs_forward_views, and are never read for the lift: the projection stage
- *     is the forward's own.  intr (NULL, or one mgs_view_intrinsics per view) gives device fields of view; its dL_dtan_fov
- *     is not used.  The outputs are not differentiable.
- * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for C outside
- * [0, MGS_MAX_FEATURE_CHANNELS]; MGS_ERR_INVALID_ARG for V <= 0, P <= 0, a NULL map while C > 0, a NULL output, a view
- * without its state buffers, matrices or radii, and the Gaussian-argument errors of mgs_forward_views.
- */
-typedef struct mgs_view_lift {
-	const float* map;               /* [C,H,W] fp32, or NULL with C = 0 */
-} mgs_view_lift;
-
-int mgs_lift_views(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int C,
-	const float* means3D,
-	const float* shs,
-	const float* colors_precomp,
-	const float* opacities,
-	const float* scales,
-	float scale_modifier,
-	const float* rotations,
-	const float* cov3D_precomp,
-	float* out_lifted,
-	float* out_weight,
-	int debug,
-	void* join_stream);
-
 /*
  * Orthographic views (no reference counterpart; gsplat's camera_model="ortho", the virtual views of RVT / RVT-2 and the
- * top-down colour and height maps of Transporter / CLIPort).  The _ortho calls are the _normal calls (and mgs_lift_views)
- * with one more argument, `ortho`: a host array of one int per view (V entries, or view_offsets[B] for clouds), 0 for a
- * perspective view and 1 for an orthographic one, or NULL for all perspective.  The older calls are the _ortho calls with
- * ortho = NULL.  One call may mix both kinds, also among the views of one cloud; the backward sums them in one pass.
+ * top-down colour and height maps of Transporter / CLIPort).  mgs_render_options.ortho
+ * (and the `ortho` argument of mgs_lift_views, mgs_visibility_views and mgs_camera_rays): a host array of one int per view,
+ * 0 for a perspective view and 1 for an orthographic one, or NULL for all perspective.  One call may mix both kinds, also among the views of one cloud; the backward sums them in one pass.
  * Definition, for an orthographic view, with t = Rv p + tv as for a pinhole view:
  *   - tan_fovx / tan_fovy (mgs_view, or mgs_view_intrinsics.tan_fov on the device) hold the half-width and half-height of
  *     the view volume in view-space units.  fx = W / (2 tan_fovx) and fy = H / (2 tan_fovy), the same float expressions as
@@ -961,44 +511,12 @@ int mgs_lift_views(
  *     the gradient of a learnable half extent.
  * Argument errors: an ortho entry other than 0 or 1 returns MGS_ERR_INVALID_ARG before anything is enqueued.
  */
-int mgs_forward_views_ortho(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_views_ortho(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
-int mgs_forward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho, int D, int M,
-	int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
-int mgs_lift_views_ortho(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
 /*
  * Fisheye views (gsplat's camera_model="fisheye"; OpenCV's cv::fisheye model, Kannala-Brandt with four coefficients, all
- * k = 0 being the equidistant fisheye).  The _fisheye calls are the _ortho calls with one more argument, `fisheye`: a host
- * array of one mgs_view_fisheye per view (V entries, or view_offsets[B] for clouds), or NULL for none.  An entry with
- * fisheye = 0 is ignored (the view is perspective or, by its ortho flag, orthographic).  The _ortho calls are the _fisheye
- * calls with fisheye = NULL.  One call may mix all three models, also among the views of one cloud.
+ * k = 0 being the equidistant fisheye).  mgs_render_options.fisheye (and the `fisheye` argument of the lift, visibility and
+ * ray calls): a host array of one mgs_view_fisheye per view, or NULL for none.  An entry with fisheye = 0 is ignored (the
+ * view is perspective or, by its ortho flag, orthographic).  One call may mix all three models, also among the views of one cloud.
  * Definition, for a fisheye view, with t = Rv p + tv as for a pinhole view:
  *   - r = sqrt(t.x^2 + t.y^2), theta = atan2(r, t.z), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8).
  *   - Screen mean: u = fx theta_d t.x / r + cx, v = fy theta_d t.y / r + cy ((cx, cy) at r = 0).  (cx, cy) are in the blend's
@@ -1032,46 +550,12 @@ typedef struct mgs_view_fisheye {
 	float k1, k2, k3, k4;           /* Kannala-Brandt coefficients */
 	float theta_max;                /* cull: theta of the mean above it, in (0, pi/2] */
 } mgs_view_fisheye;
-int mgs_forward_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
-int mgs_forward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int accumulate, int debug,
-	void* join_stream);
-int mgs_lift_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
-	const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
 /*
  * Distorted-pinhole views (OpenCV's cv::projectPoints with the 8-coefficient D = (k1, k2, p1, p2, k3, k4, k5, k6);
- * COLMAP's OPENCV / FULL_OPENCV).  The _distorted calls are the _fisheye calls with one more argument, `distortion`: a host
- * array of one mgs_view_distortion per view (V entries, or view_offsets[B] for clouds), or NULL for none.  An entry with
- * distorted = 0 is ignored (the view's model is then given by its ortho flag and fisheye entry).  The _fisheye calls are the
- * _distorted calls with distortion = NULL.  One call may mix all four models, also among the views of one cloud.
+ * COLMAP's OPENCV / FULL_OPENCV).  mgs_render_options.distortion (and the `distortion` argument of the lift, visibility and
+ * ray calls): a host array of one mgs_view_distortion per view, or NULL for none.  An entry with distorted = 0 is ignored
+ * (the view's model is then given by its ortho flag and fisheye entry).  One call may mix all four models, also among the views of one cloud.
  * Definition, for a distorted view, with t = Rv p + tv as for every view:
  *   - x = t.x / t.z, y = t.y / t.z, r2 = x^2 + y^2,
  *     R = (1 + k1 r2 + k2 r2^2 + k3 r2^3) / (1 + k4 r2 + k5 r2^2 + k6 r2^3),
@@ -1102,44 +586,9 @@ typedef struct mgs_view_distortion {
 	float k1, k2, p1, p2, k3, k4, k5, k6;  /* OpenCV's D, in its order; 4 or 5 coefficients: the rest 0 */
 	float r_max;                    /* cull: sqrt(x^2 + y^2) of the mean above it, > 0 or +inf */
 } mgs_view_distortion;
-int mgs_forward_views_distorted(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_views_distorted(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
-int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream);
-int mgs_lift_views_distorted(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
 /*
- * Planar depth.  The _planar calls are the _distorted calls with one more argument, `planar_depth` (0 or 1, for every view of
- * the call, like antialiasing); the _distorted calls are the _planar calls with planar_depth = 0.  Without it each Gaussian
+ * Planar depth.  mgs_render_options.planar_depth: 0 or 1, for every view of the call, like antialiasing.  Without it each Gaussian
  * paints its centre depth z = t.z over its whole footprint; with it, Gaussian i's depth at pixel p is its depth along the
  * pixel's ray, affine in the pixel offset (RaDe-GS, PGSR).  Definition, for Gaussian i in view v, with t = Rv p + tv:
  *   - Sigma_c = Rv S Rv^T, S the world-space covariance (from scales and rotations, or cov3D_precomp);
@@ -1164,39 +613,12 @@ int mgs_lift_views_distorted(
  * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: planar_depth other than 0 or 1; planar_depth together
  * with a normal plane in the same call (both need columns 4..6 of the tile; a fourth column tile for both is left for later).
  */
-int mgs_forward_views_planar(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_views_planar(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int planar_depth,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
-int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F,
-	float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream);
 
 /*
- * Optical flow.  The _flow calls are the _planar calls with the flow arguments after planar_depth; the _planar calls are the
- * _flow calls with NULL for them.  The flow plane relates a cloud to its deformed next frame: for one view v of a cloud with
- * means mu_i and paired next-frame means mu'_i (flow_means3D [P,3], the same P, paired by index):
+ * Optical flow.  mgs_render_options.flow: one mgs_view_flow per view, or NULL; mgs_render_options.flow_next: one
+ * mgs_cloud_flow per cloud (one for a views call), or NULL.  The flow plane relates a cloud to its deformed next frame: for
+ * one view v of a cloud with means mu_i and paired next-frame means mu'_i (flow_next[b].means3D [P,3], the same P, paired
+ * by index):
  *   - m_i is Gaussian i's screen mean in pixels, as the projection forms it: through projmatrix and ndc2pix for pinhole and
  *     orthographic views, the lens map for fisheye and distorted views;
  *   - m'_i is the same map applied to mu'_i, with the view's own camera, or with the view's next-frame pose when one is given
@@ -1214,12 +636,12 @@ int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_o
  * channel (opacity, conic and means2D of the current frame, with the anti-aliased compensation where it is on); with
  * gd_i = sum_p w_{p,i} g[:, p], -gd_i joins view v's dL/dmean2D in the blend's convention (pixels times W / 2, H / 2), from
  * where the per-Gaussian stage carries it to means3D, the camera gradients and dL_dtan_fov; (dm'/dmu')^T gd_i, summed over
- * the views, is dL_dflow_means3D (written, or added with accumulate = 1; NULL skips it), and where the view has no next pose
+ * the cloud's views, is flow_next[b].dL_dmeans3D (written, or added with accumulate = 1; NULL skips it), and where the view has no next pose
  * (dm'/dcamera)^T gd_i joins its dL_dviewmatrix, dL_dprojmatrix and dL_dtan_fov.  Invalid pairs receive nothing through delta.
  * Flow needs no rotations (cov3D_precomp works), and adds no host synchronisation.
  * Argument errors, MGS_ERR_INVALID_ARG before anything is enqueued: flow beside a normal plane or planar_depth (they share the
- * tile's columns 4..7), or beside the depth / mask heads of the same view; out_flow without next means (flow_means3D, or the
- * cloud's mgs_cloud_flow.means3D); dL_dpix_flow without out_flow, the plane that view's forward wrote; only one of
+ * tile's columns 4..7), or beside the depth / mask heads of the same view; out_flow without next means (the cloud's
+ * mgs_cloud_flow.means3D); dL_dpix_flow without out_flow, the plane that view's forward wrote; only one of
  * next_viewmatrix and next_projmatrix.
  */
 typedef struct mgs_view_flow {
@@ -1233,36 +655,113 @@ typedef struct mgs_cloud_flow {
 	const float* means3D;
 	float* dL_dmeans3D;
 } mgs_cloud_flow;
-int mgs_forward_views_flow(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	const mgs_view_flow* flow, const float* flow_means3D,
+
+/*
+ * The optional inputs of mgs_forward_views, mgs_backward_views, mgs_forward_clouds and mgs_backward_clouds, each described in
+ * its section above.  Per-view arrays have V entries (views calls) or view_offsets[B] entries (clouds calls); NULL turns the
+ * input off.  A NULL record means the same as a record with every field zero.  The forward ignores the backward-only fields
+ * (camera_grad, flow_next[.].dL_dmeans3D and the gradient fields of the per-view structs), as it does those of mgs_view.
+ * A new optional per-view input becomes a field of this record; a change of its layout changes mgs_abi_version().
+ */
+typedef struct mgs_render_options {
+	/* per-view arrays: V entries (views calls) or view_offsets[B] entries (clouds calls), or NULL for none */
+	const mgs_view_alpha* alpha;
+	const mgs_view_depth_mask* depth_mask;
+	const mgs_view_ssim* ssim;
+	const mgs_view_camera_grad* camera_grad;   /* read by the backward only */
+	const mgs_view_intrinsics* intrinsics;
+	const mgs_view_median* median;
+	const mgs_view_normal* normal;
+	const int* ortho;
+	const mgs_view_fisheye* fisheye;
+	const mgs_view_distortion* distortion;
+	const mgs_view_flow* flow;
+	/* next-frame means of the flow planes: 1 entry for a views call, B for a clouds call, or NULL */
+	const mgs_cloud_flow* flow_next;
+	int antialiasing;                          /* 0 or 1 */
+	int planar_depth;                          /* 0 or 1 */
+} mgs_render_options;
+
+int mgs_forward_views(
+	int V, const mgs_view* views, const mgs_render_options* options,
 	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* opacities,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	int prefiltered,
+	int debug,
+	void* join_stream);
+int mgs_backward_views(
+	int V, const mgs_view* views, const mgs_render_options* options,
+	int P, int D, int M, int F,
+	const float* means3D,
+	const float* shs,
+	const float* colors_precomp,
+	const float* feature_precomp,
+	const float* scales,
+	float scale_modifier,
+	const float* rotations,
+	const float* cov3D_precomp,
+	float* dL_dmean3D,
+	float* dL_dopacity,
+	float* dL_dcolor,
+	float* dL_dfeature,
+	float* dL_dcov3D,
+	float* dL_dsh,
+	float* dL_dscale,
+	float* dL_drot,
+	int shared_mean2D,
+	int accumulate,
+	int stages,            /* 1: blend stage of every view (dL_dfeature is final afterwards), 2: the per-Gaussian stage, 3: both */
+	int debug,
+	void* join_stream);
+int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
+int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream);
+
+/*
+ * Lifting 2D maps onto the Gaussians (no reference counterpart; the lift of Gaussian Grouping, SAGA, Feature Splatting and
+ * LUDVIG).  Given one map per view, mgs_lift_views computes per Gaussian g
+ *   lifted[g][c] = sum_v sum_p w_vpg map_v[c][p],     weight[g] = sum_v sum_p w_vpg,
+ * so lifted / weight is the Gaussian's blend-weighted average of the maps and weight alone its visibility over the views.
+ * Definition.  For each view the contributors and weights are the forward blend's own: the same expf, the same skip tests
+ * (power > 0, alpha < 1/255), the same 0.99 clamp, the same T (1 - alpha) < 1e-4 stop, and T the running product, so
+ * w_vpg is bit for bit the weight with which the colour image of that view blends Gaussian g into pixel p (alpha with the
+ * compensated opacity o_eff when antialiasing = 1).  There is no background term; pixels outside the image do not count.
+ * lifted is dL/dfeature of a feature render (normalize_feature off) with cotangent map_v, without the backward's geometry.
+ *   - map_v (mgs_view_lift.map) is [C,H,W] fp32, planar like the feature images; C in [0, MGS_MAX_FEATURE_CHANNELS] is the
+ *     same for every view; with C = 0 only weight is computed and lift may be NULL.
+ *   - out_lifted [P,C] (NULL allowed with C = 0) and out_weight [P] are zero-filled by the call on join_stream, then every
+ *     view of the call is summed into them (float atomics: the order of the sums is not fixed).
+ *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
+ *     (sized as for mgs_forward_views) and binning_capacity, status and stream are used; background and every image,
+ *     backward and loss-head field are ignored.  The view's state afterwards holds its projection and binning; the blend
+ *     state (final_T, n_contrib, pixel masks, block_nwalk) is not written, so it cannot serve a backward.
+ *   - shs or colors_precomp must be given as in mgs_forward_views, and are never read for the lift: the projection stage
+ *     is the forward's own.  intr (NULL, or one mgs_view_intrinsics per view) gives device fields of view; its dL_dtan_fov
+ *     is not used.  The outputs are not differentiable.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued: MGS_ERR_UNSUPPORTED for C outside
+ * [0, MGS_MAX_FEATURE_CHANNELS]; MGS_ERR_INVALID_ARG for V <= 0, P <= 0, a NULL map while C > 0, a NULL output, a view
+ * without its state buffers, matrices or radii, and the Gaussian-argument errors of mgs_forward_views.
+ */
+typedef struct mgs_view_lift {
+	const float* map;               /* [C,H,W] fp32, or NULL with C = 0 */
+} mgs_view_lift;
+
+int mgs_lift_views(
+	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
+	int P, int D, int M, int C,
+	const float* means3D, const float* shs, const float* colors_precomp,
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream);
-int mgs_backward_views_flow(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int planar_depth, const mgs_view_flow* flow, const float* flow_means3D, float* dL_dflow_means3D,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream);
-int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, const mgs_view_flow* flow,
-	const mgs_cloud_flow* flow_clouds, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream);
-int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	const mgs_view_flow* flow, const mgs_cloud_flow* flow_clouds, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream);
+	float* out_lifted, float* out_weight, int debug, void* join_stream);
 
 /*
  * Field queries (no reference counterpart): the cloud's density and features at Q arbitrary 3D points, with no camera.
@@ -1345,7 +844,7 @@ int mgs_field_query_backward(
  * Hence at a pixel centre with d behind every Gaussian, T is that pixel's final_T bit for bit (the 8x4 block lists drop only
  * pairs with alpha < 1/255 at every pixel centre of the block, which contribute nothing); a point in front of every Gaussian
  * has T = 1; along a ray T does not increase with d.  mgs_visibility_views_backward below differentiates them.
- * Arguments are those of mgs_lift_views_distorted with the map arguments replaced by the points and the outputs:
+ * Arguments are those of mgs_lift_views with the map arguments replaced by the points and the outputs:
  *   - points [Q,3]; out_uv [V,Q,2], out_depth [V,Q], out_in_view [V,Q] (uint8 0/1), each NULL to skip it; out_T [V,Q].
  *   - Per view: viewmatrix, projmatrix, cam_pos (with SHs), radii (written, as by the forward), the three state buffers
  *     (sized as for mgs_forward_views), binning_capacity, status and stream as for the lift, and blend_scratch, the point
@@ -1355,7 +854,7 @@ int mgs_field_query_backward(
  *   - Nothing allocates or blocks: a call can be captured in a CUDA graph.  Q = 0 returns 0 and enqueues nothing.
  * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0, Q < 0,
  * points NULL with Q > 0, out_T NULL, a view without its state buffers, blend_scratch, matrices or radii, the camera-model
- * errors of the _distorted calls, and the Gaussian-argument errors of mgs_lift_views.
+ * errors of the distortion section, and the Gaussian-argument errors of mgs_lift_views.
  */
 size_t mgs_visibility_scratch_bytes(int Q, int width, int height);
 int mgs_visibility_views(
@@ -1382,7 +881,7 @@ int mgs_visibility_views(
  *     dL_dopacity [P], dL_dscale [P,3], dL_drot [P,4] (zeros without scales and rotations) and dL_dcov3D [P,6] (with
  *     cov3D_precomp) through the per-Gaussian chain of the render's backward; per view through `cam` (one
  *     mgs_view_camera_grad per view, or NULL; its scratch field is ignored) dL_dviewmatrix, dL_dprojmatrix and dL_dcampos
- *     (0: no SHs), and through intr (as the _intr calls take it) dL_dtan_fov with a device field of view.  A camera's gradient
+ *     (0: no SHs), and through intr (as mgs_render_options.intrinsics) dL_dtan_fov with a device field of view.  A camera's gradient
  *     sums the Gaussian path and the point path, with the definitions of the camera-gradient and intrinsics sections.
  *   - Arguments: those of mgs_visibility_views, unchanged since that call (its views' state buffers and point scratch in
  *     blend_scratch are read as it left them), with its outputs replaced by out_T [V,Q] (its T; needed with dL_dT), the
@@ -1445,9 +944,9 @@ int mgs_visibility_views_backward(
  * 0).  Every output is written.  The camera sums are fixed-order partial sums (one row per CTA of RAYS_THREADS rays, summed
  * by the camera-gradient reduce): the backward is deterministic.
  * Nothing allocates, blocks or reads back to the host: both calls can be captured in a CUDA graph.  Q = 0 returns 0 and
- * enqueues nothing (no output is written).  The ABI version stays 300.
+ * enqueues nothing (no output is written).
  * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0 or views
- * NULL, the camera-model errors of the _distorted calls, Q < 0, a view without its matrices or with a size <= 0, pixels NULL
+ * NULL, the camera-model errors of the distortion section, Q < 0, a view without its matrices or with a size <= 0, pixels NULL
  * with Q != width * height of a view, a NULL output (forward, Q > 0), dL_dpixels without pixels, and a camera output without
  * its entry's scratch.
  */

@@ -86,6 +86,16 @@ class ViewDistortion(C.Structure):
         [(n, C.c_float) for n in ("cx", "cy", "k1", "k2", "p1", "p2", "k3", "k4", "k5", "k6", "r_max")]
 
 
+class RenderOptions(C.Structure):
+    """mirror of `mgs_render_options` (include/mgs_rasterizer.h): every optional input of the render calls; the array
+    fields take ctypes arrays (kept alive by the record) or None"""
+    _fields_ = [("alpha", C.POINTER(ViewAlpha)), ("depth_mask", C.POINTER(ViewDepthMask)), ("ssim", C.POINTER(ViewSsim)),
+                ("camera_grad", C.POINTER(ViewCameraGrad)), ("intrinsics", C.POINTER(ViewIntrinsics)),
+                ("median", C.POINTER(ViewMedian)), ("normal", C.POINTER(ViewNormal)), ("ortho", C.POINTER(C.c_int)),
+                ("fisheye", C.POINTER(ViewFisheye)), ("distortion", C.POINTER(ViewDistortion)), ("flow", C.POINTER(ViewFlow)),
+                ("flow_next", C.POINTER(CloudFlow)), ("antialiasing", C.c_int), ("planar_depth", C.c_int)]
+
+
 class ViewLift(C.Structure):
     """mirror of `mgs_view_lift` (include/mgs_rasterizer.h): the 2D map [C,H,W] one view lifts onto the Gaussians"""
     _fields_ = [("map", C.c_void_p)]
@@ -142,101 +152,33 @@ def lib():
                                vp, vp, vp, vp, vp,   # dL_dmean2D dL_dconic dL_dopacity dL_dcolor dL_dfeature
                                vp, vp, vp, vp, vp,   # dL_dmean3D dL_dcov3D dL_dsh dL_dscale dL_drot
                                vp, i, i, vp]         # scratch accumulate debug stream
+    opts = C.POINTER(RenderOptions)
     L.mgs_forward_views.restype = C.c_int
-    L.mgs_forward_views.argtypes = [i, C.POINTER(View), i, i, i, i,     # V views P D M F
+    L.mgs_forward_views.argtypes = [i, C.POINTER(View), opts, i, i, i, i,  # V views options P D M F
                                     vp, vp, vp, vp,                     # means3D shs colors feature
                                     vp, vp, f, vp, vp,                  # opacities scales scale_modifier rotations cov3D_precomp
                                     i, i, vp]                           # prefiltered debug join_stream
     L.mgs_backward_views.restype = C.c_int
-    L.mgs_backward_views.argtypes = [i, C.POINTER(View), i, i, i, i,    # V views P D M F
+    L.mgs_backward_views.argtypes = [i, C.POINTER(View), opts, i, i, i, i,  # V views options P D M F
                                      vp, vp, vp, vp,                    # means3D shs colors feature
                                      vp, f, vp, vp,                     # scales scale_modifier rotations cov3D_precomp
                                      vp, vp, vp, vp, vp, vp, vp, vp,    # dL: mean3D opacity color feature cov3D sh scale rot
                                      i, i, i, i, vp]                    # shared_mean2D accumulate stages debug join_stream
-    for name in ("mgs_forward_clouds", "mgs_backward_clouds"):
-        getattr(L, name).restype = C.c_int
-        getattr(L, name).argtypes = [i, C.POINTER(Cloud), C.POINTER(C.c_int), C.POINTER(View),  # B clouds view_offsets views
-                                     i, i, i, f,                                                 # D M F scale_modifier
-                                     i, i, vp]  # prefiltered (forward) or accumulate (backward), debug, join_stream
-    # the same four calls with the alpha planes (one ViewAlpha per view, or NULL) after the views
-    for name in ("mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds"):
-        at = list(getattr(L, name).argtypes)
-        k = 4 if "clouds" in name else 2
-        getattr(L, name + "_alpha").restype = C.c_int
-        getattr(L, name + "_alpha").argtypes = at[:k] + [C.POINTER(ViewAlpha)] + at[k:]
-        # ... and with the depth / mask heads (one ViewDepthMask per view, or NULL) after the alpha planes
-        getattr(L, name + "_depth_mask").restype = C.c_int
-        getattr(L, name + "_depth_mask").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask)] + at[k:]
-        # ... and with the anti-aliased projection switch (int antialiasing) after the depth / mask heads
-        getattr(L, name + "_aa").restype = C.c_int
-        getattr(L, name + "_aa").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i] + at[k:]
-        # ... and with the L1 + SSIM heads (one ViewSsim per view, or NULL) after the switch
-        getattr(L, name + "_ssim").restype = C.c_int
-        getattr(L, name + "_ssim").argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + at[k:]
-        # ... and the backward with the camera gradients (one ViewCameraGrad per view, or NULL) after the L1 + SSIM heads
-        if "backward" in name:
-            cam = name.replace("_views", "_views_cam").replace("_clouds", "_clouds_cam")
-            getattr(L, cam).restype = C.c_int
-            getattr(L, cam).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim),
-                                                 C.POINTER(ViewCameraGrad)] + at[k:]
-        # ... and the device field of view (one ViewIntrinsics per view, or NULL): after the L1 + SSIM heads in the forward,
-        # after the camera gradients in the backward
-        intr = name.replace("_views", "_views_intr").replace("_clouds", "_clouds_intr")
-        getattr(L, intr).restype = C.c_int
-        getattr(L, intr).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
-            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics)] + at[k:]
-        # ... and the median planes (one ViewMedian per view, or NULL) after the field of view
-        med = name.replace("_views", "_views_median").replace("_clouds", "_clouds_median")
-        getattr(L, med).restype = C.c_int
-        getattr(L, med).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
-            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian)] + at[k:]
-        # ... and the normal plane (one ViewNormal per view, or NULL) after the median planes
-        nrm = name.replace("_views", "_views_normal").replace("_clouds", "_clouds_normal")
-        getattr(L, nrm).restype = C.c_int
-        getattr(L, nrm).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
-            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
-            [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal)] + at[k:]
-        # ... and the camera models (int ortho[] per view, or NULL) after the normal planes
-        orth = name.replace("_views", "_views_ortho").replace("_clouds", "_clouds_ortho")
-        getattr(L, orth).restype = C.c_int
-        getattr(L, orth).argtypes = at[:k] + [C.POINTER(ViewAlpha), C.POINTER(ViewDepthMask), i, C.POINTER(ViewSsim)] + \
-            ([C.POINTER(ViewCameraGrad)] if "backward" in name else []) + \
-            [C.POINTER(ViewIntrinsics), C.POINTER(ViewMedian), C.POINTER(ViewNormal), C.POINTER(C.c_int)] + at[k:]
-        # ... and the fisheye parameters (one ViewFisheye per view, or NULL) after the camera models
-        fish = name.replace("_views", "_views_fisheye").replace("_clouds", "_clouds_fisheye")
-        getattr(L, fish).restype = C.c_int
-        getattr(L, fish).argtypes = getattr(L, orth).argtypes[:len(getattr(L, orth).argtypes) - len(at) + k] + \
-            [C.POINTER(ViewFisheye)] + at[k:]
-        # ... and the distortion parameters (one ViewDistortion per view, or NULL) after the fisheye parameters
-        dist = name.replace("_views", "_views_distorted").replace("_clouds", "_clouds_distorted")
-        getattr(L, dist).restype = C.c_int
-        getattr(L, dist).argtypes = getattr(L, fish).argtypes[:len(getattr(L, fish).argtypes) - len(at) + k] + \
-            [C.POINTER(ViewDistortion)] + at[k:]
-        # ... and the planar_depth flag after the distortion parameters
-        pln = name.replace("_views", "_views_planar").replace("_clouds", "_clouds_planar")
-        getattr(L, pln).restype = C.c_int
-        getattr(L, pln).argtypes = getattr(L, dist).argtypes[:len(getattr(L, dist).argtypes) - len(at) + k] + [i] + at[k:]
-        # ... and the flow planes after the planar_depth flag: views calls take the next-frame means (and the backward their
-        # gradient), clouds calls one CloudFlow per cloud
-        flw = name.replace("_views", "_views_flow").replace("_clouds", "_clouds_flow")
-        getattr(L, flw).restype = C.c_int
-        extra = [C.POINTER(CloudFlow)] if "clouds" in name else ([vp, vp] if "backward" in name else [vp])
-        getattr(L, flw).argtypes = getattr(L, pln).argtypes[:len(getattr(L, pln).argtypes) - len(at) + k] + \
-            [C.POINTER(ViewFlow)] + extra + at[k:]
+    L.mgs_forward_clouds.restype = C.c_int
+    L.mgs_forward_clouds.argtypes = [i, C.POINTER(Cloud), C.POINTER(C.c_int), C.POINTER(View),  # B clouds view_offsets views
+                                     opts, i, i, i, f,                  # options D M F scale_modifier
+                                     i, i, vp]                          # prefiltered debug join_stream
+    L.mgs_backward_clouds.restype = C.c_int
+    L.mgs_backward_clouds.argtypes = [i, C.POINTER(Cloud), C.POINTER(C.c_int), C.POINTER(View),  # B clouds view_offsets views
+                                      opts, i, i, i, f,                 # options D M F scale_modifier
+                                      i, i, vp]                         # accumulate debug join_stream
     L.mgs_lift_views.restype = C.c_int
     L.mgs_lift_views.argtypes = [i, C.POINTER(View), C.POINTER(ViewLift), i, C.POINTER(ViewIntrinsics),  # V views lift aa intr
+                                 C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
                                  i, i, i, i,                        # P D M C
                                  vp, vp, vp,                        # means3D shs colors
                                  vp, vp, f, vp, vp,                 # opacities scales scale_modifier rotations cov3D_precomp
                                  vp, vp, i, vp]                     # out_lifted out_weight debug join_stream
-    L.mgs_lift_views_ortho.restype = C.c_int
-    L.mgs_lift_views_ortho.argtypes = L.mgs_lift_views.argtypes[:5] + [C.POINTER(C.c_int)] + L.mgs_lift_views.argtypes[5:]
-    L.mgs_lift_views_fisheye.restype = C.c_int
-    L.mgs_lift_views_fisheye.argtypes = L.mgs_lift_views_ortho.argtypes[:6] + [C.POINTER(ViewFisheye)] + \
-        L.mgs_lift_views_ortho.argtypes[6:]
-    L.mgs_lift_views_distorted.restype = C.c_int
-    L.mgs_lift_views_distorted.argtypes = L.mgs_lift_views_fisheye.argtypes[:7] + [C.POINTER(ViewDistortion)] + \
-        L.mgs_lift_views_fisheye.argtypes[7:]
     L.mgs_visibility_scratch_bytes.restype = C.c_size_t
     L.mgs_visibility_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     L.mgs_visibility_views.restype = C.c_int
@@ -322,7 +264,7 @@ def lib():
                                         vp, vp, vp, vp, vp,             # g_means g_rot g_scales g_opac g_feature
                                         vp, vp, vp, vp, vp, vp, vp, vp, # dL: means d_means rot d_rot scales d_scales opac feature
                                         vp]
-    if L.mgs_abi_version() != 300:
+    if L.mgs_abi_version() != 400:
         raise ImportError("manigaussian_b200: ABI version mismatch")
     _lib = L
     return L
@@ -332,26 +274,9 @@ EXPORTED_SYMBOLS = (
     "mgs_abi_version", "mgs_last_error", "mgs_geometry_state_bytes", "mgs_image_state_bytes",
     "mgs_binning_state_bytes", "mgs_backward_scratch_bytes", "mgs_forward", "mgs_forward_begin",
     "mgs_backward", "mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds", "mgs_loss_heads",
-    "mgs_forward_views_alpha", "mgs_backward_views_alpha", "mgs_forward_clouds_alpha", "mgs_backward_clouds_alpha",
-    "mgs_forward_views_depth_mask", "mgs_backward_views_depth_mask", "mgs_forward_clouds_depth_mask",
-    "mgs_backward_clouds_depth_mask",
-    "mgs_forward_views_aa", "mgs_backward_views_aa", "mgs_forward_clouds_aa", "mgs_backward_clouds_aa",
-    "mgs_forward_views_ssim", "mgs_backward_views_ssim", "mgs_forward_clouds_ssim", "mgs_backward_clouds_ssim",
-    "mgs_ssim", "mgs_ssim_backward",
-    "mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam",
-    "mgs_forward_views_intr", "mgs_backward_views_intr", "mgs_forward_clouds_intr", "mgs_backward_clouds_intr",
-    "mgs_forward_views_median", "mgs_backward_views_median", "mgs_forward_clouds_median", "mgs_backward_clouds_median",
-    "mgs_forward_views_normal", "mgs_backward_views_normal", "mgs_forward_clouds_normal", "mgs_backward_clouds_normal",
+    "mgs_ssim", "mgs_ssim_backward", "mgs_camera_grad_scratch_bytes",
     "mgs_geometry_state_bytes_normal", "mgs_backward_scratch_bytes_normal",
     "mgs_lift_views",
-    "mgs_forward_views_ortho", "mgs_backward_views_ortho", "mgs_forward_clouds_ortho", "mgs_backward_clouds_ortho",
-    "mgs_lift_views_ortho",
-    "mgs_forward_views_fisheye", "mgs_backward_views_fisheye", "mgs_forward_clouds_fisheye", "mgs_backward_clouds_fisheye",
-    "mgs_lift_views_fisheye",
-    "mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
-    "mgs_backward_clouds_distorted", "mgs_lift_views_distorted",
-    "mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar",
-    "mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow",
     "mgs_field_query", "mgs_field_query_backward",
     "mgs_visibility_scratch_bytes", "mgs_visibility_views",
     "mgs_visibility_backward_scratch_bytes", "mgs_visibility_views_backward",

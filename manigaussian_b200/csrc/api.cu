@@ -235,7 +235,7 @@ using namespace mgs;
 
 extern "C" {
 
-int mgs_abi_version(void) { return 300; }
+int mgs_abi_version(void) { return 400; }
 const char* mgs_last_error(void) { return g_err.c_str(); }
 
 size_t mgs_geometry_state_bytes(int P) { return required([&](char*& p) { GeomState::carve(p, (size_t)P); }); }
@@ -342,7 +342,7 @@ struct Cloud {
 	const float* means3D; const float* shs; const float* colors_precomp; const float* feature; const float* opacities;
 	const float* scales; float scale_modifier; const float* rotations; const float* cov3D_precomp;
 	int antialias;  // 1: the anti-aliased projection (opacity compensation); 0 where an initialiser leaves it out
-	int planar;     // 1: planar depth (include/mgs_rasterizer.h, mgs_forward_views_planar); 0 where an initialiser leaves it out
+	int planar;     // 1: planar depth (include/mgs_rasterizer.h, mgs_render_options.planar_depth); 0 where an initialiser leaves it out
 };
 
 // a view's tile grid and its state buffers, carved (pointers into a buffer the view does not provide are never used)
@@ -756,7 +756,7 @@ static int enqueue_normals_bwd(const Cloud& c, const mgs_view* views, const mgs_
 	return 0;
 }
 
-// the flow plane (include/mgs_rasterizer.h, mgs_forward_views_flow) of views [v0, v1) of one cloud: fl NULL or one entry per
+// the flow plane (include/mgs_rasterizer.h, mgs_render_options.flow) of views [v0, v1) of one cloud: fl NULL or one entry per
 // view of the call, next_means the cloud's next-frame means; it takes the normal plane's tile columns and quad slot
 static bool flow_on(const mgs_view_flow* fl, int v) { return fl && (fl[v].out_flow || fl[v].dL_dpix_flow); }
 // the whole call: flow never beside planar depth or a normal plane (they share the tile's columns 4..7); V views
@@ -1108,164 +1108,24 @@ int mgs_backward(
 		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// NULL options: every optional input off
+static const mgs_render_options no_options{};
+// the next-frame means of cloud b (flow_next: one entry per cloud, or NULL)
+static const float* cloud_next(const mgs_cloud_flow* fc, int b) { return fc ? fc[b].means3D : nullptr; }
+
 int mgs_forward_views(
-	int V, const mgs_view* views,
+	int V, const mgs_view* views, const mgs_render_options* options,
 	int P, int D, int M, int F,
 	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
-	return mgs_forward_views_alpha(V, views, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales,
-		scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_alpha(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_depth_mask(V, views, alpha, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities,
-		scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_depth_mask(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_aa(V, views, alpha, depth_mask, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities,
-		scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_aa(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_ssim(V, views, alpha, depth_mask, antialiasing, nullptr, P, D, M, F, means3D, shs, colors_precomp,
-		feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_ssim(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_intr(V, views, alpha, depth_mask, antialiasing, ssim, nullptr, P, D, M, F, means3D, shs, colors_precomp,
-		feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_intr(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_median(V, views, alpha, depth_mask, antialiasing, ssim, intr, nullptr, P, D, M, F, means3D, shs,
-		colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_median(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_normal(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, nullptr, P, D, M, F, means3D, shs,
-		colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_normal(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_ortho(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, nullptr, P, D, M, F, means3D,
-		shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_ortho(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_fisheye(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, nullptr, P, D, M, F,
-		means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, prefiltered, debug,
-		join_stream);
-}
-
-int mgs_forward_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_distorted(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye,
-		nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations,
-		cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_distorted(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_planar(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye,
-		distortion, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations,
-		cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_planar(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_views_flow(V, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho, fisheye, distortion,
-		planar_depth, nullptr, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier,
-		rotations, cov3D_precomp, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_views_flow(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	const mgs_view_flow* flow, const float* flow_means3D,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	int prefiltered, int debug, void* join_stream)
-{
+	const mgs_render_options& o = options ? *options : no_options;
+	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
+	const mgs_view_intrinsics* intr = o.intrinsics; const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
+	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye; const mgs_view_distortion* distortion = o.distortion;
+	const mgs_view_flow* flow = o.flow; const float* flow_means3D = cloud_next(o.flow_next, 0);
+	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
@@ -1323,40 +1183,6 @@ int mgs_forward_views_flow(
 }
 
 int mgs_lift_views(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream)
-{
-	return mgs_lift_views_ortho(V, views, lift, antialiasing, intr, nullptr, P, D, M, C, means3D, shs, colors_precomp, opacities, scales,
-		scale_modifier, rotations, cov3D_precomp, out_lifted, out_weight, debug, join_stream);
-}
-
-int mgs_lift_views_ortho(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream)
-{
-	return mgs_lift_views_fisheye(V, views, lift, antialiasing, intr, ortho, nullptr, P, D, M, C, means3D, shs, colors_precomp, opacities,
-		scales, scale_modifier, rotations, cov3D_precomp, out_lifted, out_weight, debug, join_stream);
-}
-
-int mgs_lift_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
-	const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int C,
-	const float* means3D, const float* shs, const float* colors_precomp,
-	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* out_lifted, float* out_weight, int debug, void* join_stream)
-{
-	return mgs_lift_views_distorted(V, views, lift, antialiasing, intr, ortho, fisheye, nullptr, P, D, M, C, means3D, shs,
-		colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, out_lifted, out_weight, debug, join_stream);
-}
-
-int mgs_lift_views_distorted(
 	int V, const mgs_view* views, const mgs_view_lift* lift, int antialiasing, const mgs_view_intrinsics* intr, const int* ortho,
 	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
 	int P, int D, int M, int C,
@@ -1392,7 +1218,7 @@ int mgs_lift_views_distorted(
 	if (C > 0) MGS_CUDA(cudaMemsetAsync(out_lifted, 0, (size_t)P * C * sizeof(float), join));
 	int rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
-	// stage by stage across the views, as mgs_forward_views_normal: the lift takes the forward blend's place
+	// stage by stage across the views, as mgs_forward_views: the lift takes the forward blend's place
 	for (int phase = 0; phase < 3; phase++) {
 		for (int v = 0; v < V; v++) {
 			const mgs_view& w = views[v];
@@ -1785,203 +1611,22 @@ int mgs_camera_rays_backward(int V, const mgs_view* views, const mgs_view_intrin
 }
 
 int mgs_backward_views(
-	int V, const mgs_view* views,
+	int V, const mgs_view* views, const mgs_render_options* options,
 	int P, int D, int M, int F,
 	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
 	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
-	return mgs_backward_views_alpha(V, views, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier,
-		rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D,
-		accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_alpha(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_depth_mask(V, views, alpha, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
-		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot,
-		shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_depth_mask(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_aa(V, views, alpha, depth_mask, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
-		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot,
-		shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_aa(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_ssim(V, views, alpha, depth_mask, antialiasing, nullptr, P, D, M, F, means3D, shs, colors_precomp,
-		feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D,
-		dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_ssim(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_cam(V, views, alpha, depth_mask, antialiasing, ssim, nullptr, P, D, M, F, means3D, shs, colors_precomp,
-		feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D,
-		dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_cam(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_intr(V, views, alpha, depth_mask, antialiasing, ssim, cam, nullptr, P, D, M, F, means3D, shs,
-		colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
-		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_intr(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_median(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, nullptr, P, D, M, F, means3D, shs,
-		colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
-		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_median(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_normal(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, nullptr, P, D, M, F, means3D,
-		shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor,
-		dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_normal(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_ortho(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, nullptr, P, D, M, F,
-		means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity,
-		dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_ortho(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_fisheye(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho, nullptr, P, D,
-		M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity,
-		dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_fisheye(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_distorted(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho,
-		fisheye, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp,
-		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages,
-		debug, join_stream);
-}
-
-int mgs_backward_views_distorted(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_planar(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho, fisheye,
-		distortion, 0, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales, scale_modifier, rotations, cov3D_precomp,
-		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, shared_mean2D, accumulate, stages,
-		debug, join_stream);
-}
-
-int mgs_backward_views_planar(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int planar_depth,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
-	return mgs_backward_views_flow(V, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal, ortho, fisheye,
-		distortion, planar_depth, nullptr, nullptr, nullptr, P, D, M, F, means3D, shs, colors_precomp, feature_precomp, scales,
-		scale_modifier, rotations, cov3D_precomp, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale,
-		dL_drot, shared_mean2D, accumulate, stages, debug, join_stream);
-}
-
-int mgs_backward_views_flow(
-	int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median,
-	const mgs_view_normal* normal, const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion,
-	int planar_depth, const mgs_view_flow* flow, const float* flow_means3D, float* dL_dflow_means3D,
-	int P, int D, int M, int F,
-	const float* means3D, const float* shs, const float* colors_precomp, const float* feature_precomp,
-	const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
-	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
-	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
-{
+	const mgs_render_options& o = options ? *options : no_options;
+	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
+	const mgs_view_camera_grad* cam = o.camera_grad; const mgs_view_intrinsics* intr = o.intrinsics;
+	const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
+	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye;
+	const mgs_view_distortion* distortion = o.distortion; const mgs_view_flow* flow = o.flow;
+	const float* flow_means3D = cloud_next(o.flow_next, 0);
+	float* dL_dflow_means3D = o.flow_next ? o.flow_next[0].dL_dmeans3D : nullptr;
+	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V > 0 && views && check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
 	if (V > 0 && views && (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0))
@@ -2009,114 +1654,15 @@ int mgs_backward_views_flow(
 		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream), flow, flow_means3D, dL_dflow_means3D);
 }
 
-int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
-	float scale_modifier, int prefiltered, int debug, void* join_stream)
+int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
 {
-	return mgs_forward_clouds_alpha(B, clouds, view_offsets, views, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
-	int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_depth_mask(B, clouds, view_offsets, views, alpha, nullptr, D, M, F, scale_modifier, prefiltered, debug,
-		join_stream);
-}
-
-int mgs_forward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int prefiltered,
-	int debug, void* join_stream)
-{
-	return mgs_forward_clouds_aa(B, clouds, view_offsets, views, alpha, depth_mask, 0, D, M, F, scale_modifier, prefiltered, debug,
-		join_stream);
-}
-
-int mgs_forward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
-	int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_ssim(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, nullptr, D, M, F, scale_modifier,
-		prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
-	int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_intr(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, nullptr, D, M, F,
-		scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_median(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, nullptr, D, M, F,
-		scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F, float scale_modifier, int prefiltered,
-	int debug, void* join_stream)
-{
-	return mgs_forward_clouds_normal(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, nullptr, D, M,
-		F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, int D, int M, int F,
-	float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_ortho(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, nullptr,
-		D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho, int D, int M,
-	int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_fisheye(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho,
-		nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_distorted(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median,
-		normal, ortho, fisheye, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_planar(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho,
-		fisheye, distortion, 0, D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-int mgs_forward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
-	return mgs_forward_clouds_flow(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, intr, median, normal, ortho,
-		fisheye, distortion, planar_depth, nullptr, nullptr, D, M, F, scale_modifier, prefiltered, debug, join_stream);
-}
-
-// the next-frame means of cloud b (flow_clouds: B entries or NULL)
-static const float* cloud_next(const mgs_cloud_flow* fc, int b) { return fc ? fc[b].means3D : nullptr; }
-
-int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal, const int* ortho,
-	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, const mgs_view_flow* flow,
-	const mgs_cloud_flow* flow_clouds, int D, int M, int F, float scale_modifier, int prefiltered, int debug, void* join_stream)
-{
+	const mgs_render_options& o = options ? *options : no_options;
+	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
+	const mgs_view_intrinsics* intr = o.intrinsics; const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
+	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye; const mgs_view_distortion* distortion = o.distortion;
+	const mgs_view_flow* flow = o.flow; const mgs_cloud_flow* flow_clouds = o.flow_next;
+	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
 	(void)prefiltered;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
@@ -2171,124 +1717,17 @@ int mgs_forward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offs
 	return join_streams(V, views, join);
 }
 
-int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream)
+int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
-	return mgs_backward_clouds_alpha(B, clouds, view_offsets, views, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_alpha(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views, const mgs_view_alpha* alpha,
-	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_depth_mask(B, clouds, view_offsets, views, alpha, nullptr, D, M, F, scale_modifier, accumulate, debug,
-		join_stream);
-}
-
-int mgs_backward_clouds_depth_mask(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int D, int M, int F, float scale_modifier, int accumulate,
-	int debug, void* join_stream)
-{
-	return mgs_backward_clouds_aa(B, clouds, view_offsets, views, alpha, depth_mask, 0, D, M, F, scale_modifier, accumulate, debug,
-		join_stream);
-}
-
-int mgs_backward_clouds_aa(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, int D, int M, int F, float scale_modifier,
-	int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_ssim(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, nullptr, D, M, F, scale_modifier,
-		accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_ssim(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim, int D, int M,
-	int F, float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_cam(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, nullptr, D, M, F,
-		scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_cam(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_intr(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, nullptr, D, M, F,
-		scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_intr(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, int D, int M, int F, float scale_modifier, int accumulate,
-	int debug, void* join_stream)
-{
-	return mgs_backward_clouds_median(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, nullptr, D, M,
-		F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_median(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_normal(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, nullptr,
-		D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_normal(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_ortho(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
-		nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_ortho(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
-{
-	return mgs_backward_clouds_fisheye(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
-		ortho, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_fisheye(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, int D, int M, int F, float scale_modifier, int accumulate, int debug,
-	void* join_stream)
-{
-	return mgs_backward_clouds_distorted(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median,
-		normal, ortho, fisheye, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_distorted(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int D, int M, int F, float scale_modifier, int accumulate, int debug,
-	void* join_stream)
-{
-	return mgs_backward_clouds_planar(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
-		ortho, fisheye, distortion, 0, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_planar(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth, int D, int M, int F, float scale_modifier, int accumulate, int debug,
-	void* join_stream)
-{
-	return mgs_backward_clouds_flow(B, clouds, view_offsets, views, alpha, depth_mask, antialiasing, ssim, cam, intr, median, normal,
-		ortho, fisheye, distortion, planar_depth, nullptr, nullptr, D, M, F, scale_modifier, accumulate, debug, join_stream);
-}
-
-int mgs_backward_clouds_flow(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
-	const mgs_view_alpha* alpha, const mgs_view_depth_mask* depth_mask, int antialiasing, const mgs_view_ssim* ssim,
-	const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* median, const mgs_view_normal* normal,
-	const int* ortho, const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, int planar_depth,
-	const mgs_view_flow* flow, const mgs_cloud_flow* flow_clouds, int D, int M, int F,
-	float scale_modifier, int accumulate, int debug, void* join_stream)
-{
+	const mgs_render_options& o = options ? *options : no_options;
+	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
+	const mgs_view_camera_grad* cam = o.camera_grad; const mgs_view_intrinsics* intr = o.intrinsics;
+	const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
+	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye;
+	const mgs_view_distortion* distortion = o.distortion; const mgs_view_flow* flow = o.flow;
+	const mgs_cloud_flow* flow_clouds = o.flow_next;
+	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
 	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	int rc = check_clouds(B, clouds, view_offsets, views);
 	if (rc < 0) return rc;

@@ -126,13 +126,13 @@ __device__ __forceinline__ void sh_to_rgb(int idx, int deg, int max_coeffs, cons
 // Only conic_opacity.w and the extent's opacity change; the conic, radius, tiles and keys are those of AA = false.
 // FOV: the field of view is read from the device ({tan_fovx, tan_fovy} at a.tan_fov) and the focal lengths are formed here
 // with the host's float expression, so equal values give the host path's results bit for bit.
-// MODEL_ORTHO: an orthographic view (include/mgs_rasterizer.h, mgs_forward_views_ortho): tan_fov holds the view volume's half
+// MODEL_ORTHO: an orthographic view (include/mgs_rasterizer.h, mgs_render_options.ortho): tan_fov holds the view volume's half
 // extents, fx = W / (2 tan_fovx) is in pixels per unit, and J does not depend on t.  The screen mean still goes through the
 // caller's projmatrix (w = 1 for an orthographic matrix), and everything after the covariance is the perspective path's.
-// MODEL_FISHEYE: a Kannala-Brandt view (mgs_forward_views_fisheye): projmatrix is not read; the screen mean is
+// MODEL_FISHEYE: a Kannala-Brandt view (mgs_render_options.fisheye): projmatrix is not read; the screen mean is
 // (fx a t.x + cx, fy a t.y + cy), J the map's Jacobian (fisheye.cuh), and a mean with theta > theta_max is culled like one
 // behind the near plane.  Everything after the covariance is the perspective path's.
-// MODEL_DISTORTED: an OpenCV distorted-pinhole view (mgs_forward_views_distorted): projmatrix is not read; the screen mean
+// MODEL_DISTORTED: an OpenCV distorted-pinhole view (mgs_render_options.distortion): projmatrix is not read; the screen mean
 // is (fx xd + cx, fy yd + cy), J = diag(fx, fy) Dd (d(x, y) / dt) (distortion.cuh), and a mean past the first fold
 // (r2 > r2_max) or on a local fold (det Dd <= 0) is culled like one behind the near plane.
 template <bool AA, bool FOV, int MODEL>

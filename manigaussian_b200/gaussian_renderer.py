@@ -74,7 +74,7 @@ def _camera_scalars(nv, idx):
 
 
 def _with_planar_depth(s):
-    """The settings `s` with planar_depth=True (include/mgs_rasterizer.h, mgs_forward_views_planar), its other attributes kept."""
+    """The settings `s` with planar_depth=True (include/mgs_rasterizer.h, mgs_render_options.planar_depth), its other attributes kept."""
     return GaussianRasterizationSettings(*tuple(s)[:13], antialiasing=getattr(s, "antialiasing", False),
                                          orthographic=getattr(s, "orthographic", False), fisheye=getattr(s, "fisheye", None),
                                          distortion=getattr(s, "distortion", None), planar_depth=True)
@@ -541,7 +541,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
     the depth / mask heads have no kernel beside it.
     planar_depth: the depth plane, the depth head (targets["depth"]) and the median depth take each Gaussian's depth along
     the pixel's ray, affine in the pixel offset, instead of its centre depth (include/mgs_rasterizer.h,
-    mgs_forward_views_planar); also on when the given settings carry planar_depth=True.  Not with return_normal.
+    mgs_render_options.planar_depth); also on when the given settings carry planar_depth=True.  Not with return_normal.
     flow_xyz: [P,3] next-frame means paired by index with pts_xyz (e.g. the deformed cloud of the dyna step); the result then
     gains "flow" [V,2,H,W], each Gaussian's screen displacement m' - m in pixels (x right, y down) blended with the colour's
     weights (flow / alpha is the expected flow; include/mgs_rasterizer.h, flow plane), differentiable in the cloud, the

@@ -495,18 +495,18 @@ class GaussianRasterizationSettings(_Settings):
     the settings still unpack into the reference's own 13-field NamedTuple, and `_fields` is the reference's.
     `orthographic` (default False; keyword, or positional after antialiasing) is an attribute in the same way: True makes the
     view orthographic, with tanfovx / tanfovy its half-width and half-height in view-space units and projmatrix an
-    orthographic matrix (cameras.projection_orthographic; include/mgs_rasterizer.h, mgs_forward_views_ortho).
+    orthographic matrix (cameras.projection_orthographic; include/mgs_rasterizer.h, mgs_render_options.ortho).
     `fisheye` (default None; keyword, or positional after orthographic) is an attribute in the same way: the view's
     Kannala-Brandt parameters (cx, cy, k1, k2, k3, k4, theta_max), or a dict with those keys, make it a fisheye view, with
     tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (fx, fy in pixels per radian; include/mgs_rasterizer.h,
-    mgs_forward_views_fisheye; cameras.build_fisheye_cameras).  It cannot be combined with orthographic=True.
+    mgs_render_options.fisheye; cameras.build_fisheye_cameras).  It cannot be combined with orthographic=True.
     `distortion` (default None; keyword, or positional after fisheye) is an attribute in the same way: the view's OpenCV
     parameters (cx, cy, k1, k2, p1, p2, k3, k4, k5, k6, r_max), or a dict with those keys, make it a distorted-pinhole view,
-    with tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (include/mgs_rasterizer.h, mgs_forward_views_distorted;
+    with tanfovx / tanfovy holding W / (2 fx) and H / (2 fy) (include/mgs_rasterizer.h, mgs_render_options.distortion;
     cameras.build_distorted_cameras).  It cannot be combined with orthographic=True or fisheye.
     `planar_depth` (default False; keyword, or positional after distortion) is an attribute in the same way: True makes the
     depth plane, the depth head and the median depth take each Gaussian's depth along the pixel's ray, affine in the pixel
-    offset, instead of its centre depth (include/mgs_rasterizer.h, mgs_forward_views_planar).  It is a per-call setting: the
+    offset, instead of its centre depth (include/mgs_rasterizer.h, mgs_render_options.planar_depth).  It is a per-call setting: the
     views of one call must agree."""
     antialiasing = False
     orthographic = False
@@ -782,7 +782,7 @@ def _flow_array(views, flow_means3D, flow_poses, P, dev, keep, planes=None, grad
 
 def _ortho_flags(views, ortho=None):
     """Per-view camera models: `ortho` (V truthy values) when given, else each view's `orthographic` attribute; a ctypes int
-    array for the _ortho calls, or None when every view is perspective (the calls without the argument then serve)."""
+    array for mgs_render_options.ortho, or None when every view is perspective."""
     flags = [bool(o) for o in ortho] if ortho is not None else [bool(getattr(s, "orthographic", False)) for s in views]
     if len(flags) != len(views):
         raise ValueError(f"ortho: expected {len(views)} flags, got {len(flags)}")
@@ -791,7 +791,7 @@ def _ortho_flags(views, ortho=None):
 
 def _fisheye_array(views, fisheye=None):
     """Per-view fisheye parameters: `fisheye` (V entries, each None or parameters) when given, else each view's `fisheye`
-    attribute; a ctypes ViewFisheye array for the _fisheye calls, or None when no view is fisheye."""
+    attribute; a ctypes ViewFisheye array for mgs_render_options.fisheye, or None when no view is fisheye."""
     fe = [_fisheye_params(f) for f in fisheye] if fisheye is not None else [getattr(s, "fisheye", None) for s in views]
     if len(fe) != len(views):
         raise ValueError(f"fisheye: expected {len(views)} entries, got {len(fe)}")
@@ -808,7 +808,7 @@ def _fisheye_array(views, fisheye=None):
 
 def _distortion_array(views, distortion=None):
     """Per-view distortion parameters: `distortion` (V entries, each None or parameters) when given, else each view's
-    `distortion` attribute; a ctypes ViewDistortion array for the _distorted calls, or None when no view is distorted."""
+    `distortion` attribute; a ctypes ViewDistortion array for mgs_render_options.distortion, or None when no view is distorted."""
     dc = [_distortion_params(d) for d in distortion] if distortion is not None else \
         [getattr(s, "distortion", None) for s in views]
     if len(dc) != len(views):
@@ -890,13 +890,10 @@ def _count_ortho(L, s, dev, P, means3D, colors, opacity, scales, rotations, scal
     iarr = _intrinsics_array(tf, None) if tf is not None else None
     rest = (P, 0, 0, 0, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
             _ptr(cov3D_precomp), None, _ptr(weight), int(bool(debug)), st.cuda_stream)
-    if distortion is not None:
-        _b.check(L.mgs_lift_views_distorted(1, w, None, 0, iarr, None, None, (_b.ViewDistortion * 1)(distortion), *rest),
-                 "mgs_lift_views_distorted")
-    elif fisheye is not None:
-        _b.check(L.mgs_lift_views_fisheye(1, w, None, 0, iarr, None, (_b.ViewFisheye * 1)(fisheye), *rest), "mgs_lift_views_fisheye")
-    else:
-        _b.check(L.mgs_lift_views_ortho(1, w, None, 0, iarr, (ctypes.c_int * 1)(1), *rest), "mgs_lift_views_ortho")
+    dcarr = (_b.ViewDistortion * 1)(distortion) if distortion is not None else None
+    farr = (_b.ViewFisheye * 1)(fisheye) if fisheye is not None and dcarr is None else None
+    oarr = (ctypes.c_int * 1)(1) if farr is None and dcarr is None else None
+    _b.check(L.mgs_lift_views(1, w, None, 0, iarr, oarr, farr, dcarr, *rest), "mgs_lift_views")
     return status, (geom, img, binb, radii, weight, vm, pm, tf, colors)
 
 
@@ -918,26 +915,26 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     [V,H,W] or None, cot_depth, cot_alpha_depth (both [V,H,W], with target_depth), cot_alpha_mask [V,H,W] (with target_mask),
     loss_acc [V,3]), with `loss_heads` only: the same epilogue also evaluates the expected-depth L1 head and the alpha mask
     head (C ABI mgs_view_depth_mask), leaving {sum |d - g|, valid pixels, sum BCE} in loss_acc.  `antialiasing`: the
-    anti-aliased projection (C ABI mgs_forward_views_aa); pass the same value to the backward.  `ssim` = (ssim_terms
+    anti-aliased projection (C ABI mgs_render_options.antialiasing); pass the same value to the backward.  `ssim` = (ssim_terms
     [V,9,H,W], loss_acc [V,4], cot_color [V,3,H,W]), with `loss_heads` only: behind each view's blend, the L1 + SSIM head
     (C ABI mgs_view_ssim) leaves {sum |x - g|, sum S} in loss_acc[:, :2] and the partials of S in ssim_terms.  `tan_fov`
     [V,2] (device): every view's {tan_fovx, tan_fovy}, read by the kernels in place of the settings' host floats (C ABI
-    mgs_forward_views_intr); views whose tanfovx / tanfovy are CUDA tensors use it without being asked.  Pass the same to
+    mgs_render_options.intrinsics); views whose tanfovx / tanfovy are CUDA tensors use it without being asked.  Pass the same to
     the backward.  `return_median` appends the median-depth plane [H,W] and the median contributor's Gaussian id [H,W] int32
     (-1 where nothing covers the pixel) to every ViewOut, behind the other planes (C ABI mgs_view_median); with `out_buffers`
     they go to out_buffers[4] and out_buffers[5] ([V,H,W] each) when those are given.  `return_normal` appends, last, the
     surface-normal plane [3,H,W] to every ViewOut (C ABI mgs_view_normal; out_buffers[6] [V,3,H,W] when given); it needs scales
     and rotations, and cannot be combined with `depth_mask`.  `ortho` (V flags) marks the orthographic views; by default each
-    view's `orthographic` attribute does.  With any orthographic view the call is mgs_forward_views_ortho; pass the same
+    view's `orthographic` attribute does.  They go to mgs_render_options.ortho; pass the same
     flags (or views) to the backward.  `fisheye` (V entries, each None or a view's fisheye parameters, as the settings'
-    `fisheye` attribute) marks the fisheye views, by default each view's `fisheye` attribute; with any fisheye view the call
-    is mgs_forward_views_fisheye.  `distortion` (V entries, each None or a view's distortion parameters, as the settings'
-    `distortion` attribute) marks the distorted-pinhole views, by default each view's `distortion` attribute; with any
-    distorted view the call is mgs_forward_views_distorted.  `planar_depth` (default: the views' `planar_depth` attribute):
+    `fisheye` attribute) marks the fisheye views, by default each view's `fisheye` attribute; they go to
+    mgs_render_options.fisheye.  `distortion` (V entries, each None or a view's distortion parameters, as the settings'
+    `distortion` attribute) marks the distorted-pinhole views, by default each view's `distortion` attribute; they go to
+    mgs_render_options.distortion.  `planar_depth` (default: the views' `planar_depth` attribute):
     each Gaussian's depth follows its tilt across its footprint, in the depth plane, the depth head and the median depth
-    (C ABI mgs_forward_views_planar); it cannot be combined with `return_normal`.  `flow_means3D` [P,3] (the cloud's
+    (C ABI mgs_render_options.planar_depth); it cannot be combined with `return_normal`.  `flow_means3D` [P,3] (the cloud's
     next-frame means, paired by index) appends, last, every view's flow plane [3,H,W] (channels: x and y screen displacement
-    in pixels, blended with the colour's weights; channel 2 is 0; C ABI mgs_forward_views_flow; out_buffers[7] [V,3,H,W]
+    in pixels, blended with the colour's weights; channel 2 is 0; C ABI mgs_render_options.flow; out_buffers[7] [V,3,H,W]
     when given), with `flow_poses` (per view None or the next frame's (viewmatrix, projmatrix)) the pose each view projects
     the next means with.  Not with `return_normal`, `planar_depth` or `depth_mask`."""
     L = _b.lib()
@@ -995,47 +992,12 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
                 _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
         tf = _device_fov(views, tan_fov, dev)
         keep.append(tf)
-        if flarr is not None:
-            _b.check(L.mgs_forward_views_flow(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                              _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                              dcarr, int(pln), flarr, _ptr(flow_means3D), *rest), "mgs_forward_views_flow")
-        elif pln:
-            _b.check(L.mgs_forward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                dcarr, 1, *rest), "mgs_forward_views_planar")
-        elif dcarr is not None:
-            _b.check(L.mgs_forward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                   _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                   dcarr, *rest), "mgs_forward_views_distorted")
-        elif farr is not None:
-            _b.check(L.mgs_forward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                 *rest), "mgs_forward_views_fisheye")
-        elif oarr is not None:
-            _b.check(L.mgs_forward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                               _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
-                     "mgs_forward_views_ortho")
-        elif narr is not None:
-            _b.check(L.mgs_forward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
-                     "mgs_forward_views_normal")
-        elif marr is not None:
-            _b.check(L.mgs_forward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
-                     "mgs_forward_views_median")
-        elif tf is not None:
-            _b.check(L.mgs_forward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None), *rest),
-                     "mgs_forward_views_intr")
-        elif sarr is not None:
-            _b.check(L.mgs_forward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_forward_views_ssim")
-        elif antialiasing:
-            _b.check(L.mgs_forward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_forward_views_aa")
-        elif darr is not None:
-            _b.check(L.mgs_forward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_forward_views_depth_mask")
-        elif return_alpha:
-            _b.check(L.mgs_forward_views_alpha(V, arr, aarr, *rest), "mgs_forward_views_alpha")
-        else:
-            _b.check(L.mgs_forward_views(V, arr, *rest), "mgs_forward_views")
+        iarr = _intrinsics_array(tf, None) if tf is not None else None
+        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, intrinsics=iarr, median=marr, normal=narr,
+                                ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
+                                flow_next=(_b.CloudFlow * 1)((_ptr(flow_means3D), None)) if flarr is not None else None,
+                                antialiasing=int(bool(antialiasing)), planar_depth=int(pln))
+        _b.check(L.mgs_forward_views(V, arr, opts, *rest), "mgs_forward_views")
         _track_status(outs, keys, status, main, capacities is None and not capturing)
     return outs, streams
 
@@ -1045,9 +1007,8 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
     """Lift one 2D map per view onto the Gaussians (C ABI mgs_lift_views): lifted [P,C] = sum over the views and pixels of
     the forward blend's weights w = alpha T times the map, weight [P] = the sum of the weights.  `maps`: [V,C,H,W] or a
     sequence of V [C,H,W] fp32 tensors on the cloud's device (each view's own H, W), or None for weight only.  `views`,
-    `antialiasing`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in rasterize_views_raw (C ABI mgs_lift_views_ortho with
-    an orthographic view, mgs_lift_views_fisheye with a fisheye one, mgs_lift_views_distorted with a distorted one); the binning state is sized from the same capacity table (a
-    steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
+    `antialiasing`, `tan_fov`, `ortho`, `fisheye` and `distortion` as in rasterize_views_raw; the binning state is sized
+    from the same capacity table (a steady-state call reads nothing back to the host).  Returns (lifted, weight); neither is differentiable.  The projection
     needs colours, which the lift never reads: a zero [P,3] buffer stands in for them."""
     L = _b.lib()
     dev = means3D.device
@@ -1108,15 +1069,7 @@ def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, c
         iarr = _intrinsics_array(tf, None) if tf is not None else None
         rest = (P, 0, 0, C, _ptr(means3D), None, _ptr(colors), _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations),
                 _ptr(cov3D_precomp), _ptr(lifted) if C else None, _ptr(weight), int(bool(debug)), main.cuda_stream)
-        if dcarr is not None:
-            _b.check(L.mgs_lift_views_distorted(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, dcarr, *rest),
-                     "mgs_lift_views_distorted")
-        elif farr is not None:
-            _b.check(L.mgs_lift_views_fisheye(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, *rest), "mgs_lift_views_fisheye")
-        elif oarr is not None:
-            _b.check(L.mgs_lift_views_ortho(V, arr, larr, int(bool(antialiasing)), iarr, oarr, *rest), "mgs_lift_views_ortho")
-        else:
-            _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), iarr, *rest), "mgs_lift_views")
+        _b.check(L.mgs_lift_views(V, arr, larr, int(bool(antialiasing)), iarr, oarr, farr, dcarr, *rest), "mgs_lift_views")
         _track_status(outs, keys, status, main, not capturing)
     return lifted, weight
 
@@ -1482,25 +1435,25 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     are loaded.  `grads_alpha` (per view [H,W] or None): cotangents of the alpha planes of a `return_alpha` forward.  The
     caller's current stream holds the result on return.  `depth_mask`: the tuple given to the forward, whose cotangent planes
     are read back with `depth_mask_scale` [V,2] (device; the upstream gradients {g_depth, g_mask} of the depth and mask losses,
-    or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_backward_views_aa).  `ssim`: the tuple given to
+    or None for 1).  `antialiasing`: the value the forward was given (C ABI mgs_render_options.antialiasing).  `ssim`: the tuple given to
     the forward plus the forward's images and colour targets (both [V,3,H,W]); each view's L1 + SSIM head then writes its
     complete colour cotangent, with `ssim_scale` [V,2] (device; the upstream gradients {g_l1, g_ssim}, or None for 1), before
     its blend backward reads it.  `camera_grads`: True, or a tuple (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16], dL_dcampos
     [V,3]) of fp32 device tensors or None each, asks for the gradients with respect to each view's viewmatrix, projmatrix and
-    campos (C ABI mgs_backward_views_cam; written, or added to with accumulate=True); the return value then gains that tuple
+    campos (C ABI mgs_render_options.camera_grad; written, or added to with accumulate=True); the return value then gains that tuple
     (allocated for True) as a 10th element.  `tan_fov`: as given to the forward (views with CUDA-tensor tanfov* imply it);
-    with it the call is mgs_backward_views_intr, and `camera_grads` gains a 4th entry, dL_dtan_fov [V,2] (the gradient with
+    it goes to mgs_render_options.intrinsics, and `camera_grads` gains a 4th entry, dL_dtan_fov [V,2] (the gradient with
     respect to each view's {tan_fovx, tan_fovy}; allocated for True, or named in a 4-tuple).  `grads_median` (per view [H,W]
     or None): cotangents of the median-depth planes of a `return_median` forward, with `median_ids` (per view [H,W] int32)
-    the id planes that forward returned (C ABI mgs_backward_views_median).  `grads_normal` (per view [3,H,W] or None):
+    the id planes that forward returned (C ABI mgs_view_median).  `grads_normal` (per view [3,H,W] or None):
     cotangents of the normal planes of a `return_normal` forward, with `normals` (per view [3,H,W]) the planes that forward
-    returned (C ABI mgs_backward_views_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
-    forward (by default the views' `orthographic` attributes); with an orthographic view the call is mgs_backward_views_ortho.
-    `fisheye`: as given to the forward (by default the views' `fisheye` attributes); with a fisheye view the call is
-    mgs_backward_views_fisheye.  `distortion`: likewise, mgs_backward_views_distorted with a distorted view.  `planar_depth`:
-    as given to the forward (mgs_backward_views_planar).  `flow_means3D` and `flow_poses`: as given to the forward, with
+    returned (C ABI mgs_view_normal); their rotation gradient is added to dL_drotations.  `ortho`: as given to the
+    forward (by default the views' `orthographic` attributes); C ABI mgs_render_options.ortho.
+    `fisheye`: as given to the forward (by default the views' `fisheye` attributes); C ABI
+    mgs_render_options.fisheye.  `distortion`: likewise, mgs_render_options.distortion.  `planar_depth`:
+    as given to the forward (mgs_render_options.planar_depth).  `flow_means3D` and `flow_poses`: as given to the forward, with
     `flows` (per view [3,H,W]) the flow planes it returned and `grads_flow` (per view [3,H,W] or [2,H,W], or None) their
-    cotangents (C ABI mgs_backward_views_flow); the return value then gains, last, dL_dflow_means3D [P,3]."""
+    cotangents (C ABI mgs_render_options.flow and flow_next); the return value then gains, last, dL_dflow_means3D [P,3]."""
     L = _b.lib()
     dev = means3D.device
     P = means3D.size(0)
@@ -1572,49 +1525,17 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
         cam, carr = _camera_grads(L, camera_grads, [P] * V, dev, keep, tf is not None)
         iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
         keep.append(tf)
+        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, camera_grad=carr, intrinsics=iarr, median=marr,
+                                normal=narr, ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
+                                flow_next=(_b.CloudFlow * 1)((_ptr(flow_means3D), _ptr(dL_dflow))) if flarr is not None else None,
+                                antialiasing=int(bool(antialiasing)), planar_depth=int(pln))
         for stages in ((1, 2) if after_blend is not None else (3,)):
             rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
                     _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
                     _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
                     _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
                     int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            if flarr is not None:
-                _b.check(L.mgs_backward_views_flow(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
-                                                   oarr, farr, dcarr, int(pln), flarr, _ptr(flow_means3D), _ptr(dL_dflow), *rest),
-                         "mgs_backward_views_flow")
-            elif pln:
-                _b.check(L.mgs_backward_views_planar(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
-                                                     oarr, farr, dcarr, 1, *rest), "mgs_backward_views_planar")
-            elif dcarr is not None:
-                _b.check(L.mgs_backward_views_distorted(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr,
-                                                        oarr, farr, dcarr, *rest), "mgs_backward_views_distorted")
-            elif farr is not None:
-                _b.check(L.mgs_backward_views_fisheye(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
-                                                      farr, *rest), "mgs_backward_views_fisheye")
-            elif oarr is not None:
-                _b.check(L.mgs_backward_views_ortho(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, oarr,
-                                                    *rest), "mgs_backward_views_ortho")
-            elif narr is not None:
-                _b.check(L.mgs_backward_views_normal(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, narr, *rest),
-                         "mgs_backward_views_normal")
-            elif marr is not None:
-                _b.check(L.mgs_backward_views_median(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, marr, *rest),
-                         "mgs_backward_views_median")
-            elif iarr is not None:
-                _b.check(L.mgs_backward_views_intr(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, iarr, *rest),
-                         "mgs_backward_views_intr")
-            elif carr is not None:
-                _b.check(L.mgs_backward_views_cam(V, arr, aarr, darr, int(bool(antialiasing)), sarr, carr, *rest), "mgs_backward_views_cam")
-            elif sarr is not None:
-                _b.check(L.mgs_backward_views_ssim(V, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest), "mgs_backward_views_ssim")
-            elif antialiasing:
-                _b.check(L.mgs_backward_views_aa(V, arr, aarr, darr, 1, *rest), "mgs_backward_views_aa")
-            elif darr is not None:
-                _b.check(L.mgs_backward_views_depth_mask(V, arr, aarr, darr, *rest), "mgs_backward_views_depth_mask")
-            elif aarr is not None:
-                _b.check(L.mgs_backward_views_alpha(V, arr, aarr, *rest), "mgs_backward_views_alpha")
-            else:
-                _b.check(L.mgs_backward_views(V, arr, *rest), "mgs_backward_views")
+            _b.check(L.mgs_backward_views(V, arr, opts, *rest), "mgs_backward_views")
             if stages == 1:
                 after_blend()
     grads = (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
@@ -1746,17 +1667,17 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
     Capacity history is kept per (device, P, W, H, cloud slot, view slot).  `antialiasing`: the anti-aliased projection for
-    every cloud (C ABI mgs_forward_clouds_aa); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
-    (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_forward_clouds_intr).
+    every cloud (C ABI mgs_render_options.antialiasing); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
+    (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_render_options.intrinsics).
     `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
-    mgs_forward_clouds_median).  `return_normal` appends, last, every view's normal plane [3,H,W], as in rasterize_views_raw
-    (C ABI mgs_forward_clouds_normal).  A cloud's optional "ortho" (V_b flags; by default its views' `orthographic`
-    attributes) marks its orthographic views (C ABI mgs_forward_clouds_ortho); the backward reads the same entry.  A cloud's
+    mgs_view_median).  `return_normal` appends, last, every view's normal plane [3,H,W], as in rasterize_views_raw
+    (C ABI mgs_view_normal).  A cloud's optional "ortho" (V_b flags; by default its views' `orthographic`
+    attributes) marks its orthographic views (C ABI mgs_render_options.ortho); the backward reads the same entry.  A cloud's
     optional "fisheye" (V_b entries, each None or parameters; by default its views' `fisheye` attributes) marks its fisheye
-    views (C ABI mgs_forward_clouds_fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
-    mgs_forward_clouds_distorted).  A cloud's optional "flow_means3D" [P,3] (its next-frame means) and "flow_poses" (as
+    views (C ABI mgs_render_options.fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
+    mgs_render_options.distortion).  A cloud's optional "flow_means3D" [P,3] (its next-frame means) and "flow_poses" (as
     rasterize_views_raw takes them) append, last, its views' flow planes [3,H,W] (out_buffers[7] when given; C ABI
-    mgs_forward_clouds_flow)."""
+    mgs_render_options.flow)."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, return_normal)
     for c in clouds:
@@ -1824,48 +1745,12 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
         oarr, farr, dcarr = _clouds_lens(clouds)
-        if flarr is not None:
-            _b.check(L.mgs_forward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                               _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                               dcarr, int(pln), flarr, cfarr, *rest), "mgs_forward_clouds_flow")
-        elif pln:
-            _b.check(L.mgs_forward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                 dcarr, 1, *rest), "mgs_forward_clouds_planar")
-        elif dcarr is not None:
-            _b.check(L.mgs_forward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                    _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                    dcarr, *rest), "mgs_forward_clouds_distorted")
-        elif farr is not None:
-            _b.check(L.mgs_forward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                  _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, farr,
-                                                  *rest), "mgs_forward_clouds_fisheye")
-        elif oarr is not None:
-            _b.check(L.mgs_forward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                _intrinsics_array(tf, None) if tf is not None else None, marr, narr, oarr, *rest),
-                     "mgs_forward_clouds_ortho")
-        elif narr is not None:
-            _b.check(L.mgs_forward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, narr, *rest),
-                     "mgs_forward_clouds_normal")
-        elif marr is not None:
-            _b.check(L.mgs_forward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr,
-                                                 _intrinsics_array(tf, None) if tf is not None else None, marr, *rest),
-                     "mgs_forward_clouds_median")
-        elif tf is not None:
-            _b.check(L.mgs_forward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, _intrinsics_array(tf, None),
-                                               *rest), "mgs_forward_clouds_intr")
-        elif sarr is not None:
-            _b.check(L.mgs_forward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
-                     "mgs_forward_clouds_ssim")
-        elif antialiasing:
-            _b.check(L.mgs_forward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_forward_clouds_aa")
-        elif darr is not None:
-            _b.check(L.mgs_forward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_forward_clouds_depth_mask")
-        elif return_alpha:
-            _b.check(L.mgs_forward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_forward_clouds_alpha")
-        else:
-            _b.check(L.mgs_forward_clouds(B, carr, offs, arr, *rest), "mgs_forward_clouds")
+        iarr = _intrinsics_array(tf, None) if tf is not None else None
+        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, intrinsics=iarr, median=marr, normal=narr,
+                                ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
+                                flow_next=cfarr if flarr is not None else None, antialiasing=int(bool(antialiasing)),
+                                planar_depth=int(pln))
+        _b.check(L.mgs_forward_clouds(B, carr, offs, arr, opts, *rest), "mgs_forward_clouds")
         flat = [o for co in outs for o in co]
         pending = not capturing and all(c.get("capacities") is None for c in clouds)
         _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
@@ -1933,17 +1818,16 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     as rasterize_views_backward_raw takes them.  Returns one dict per cloud
     holding the sums over its views: dL_dmeans3D [P,3], dL_dmeans2D [V_b,P,3] (per view), dL_dopacity [P,1], dL_dscales,
     dL_drotations, dL_dsh [P,M,3], dL_dcolors, dL_dcov3D, dL_dfeature (None where not computed).  `antialiasing`: the value
-    the forward was given (C ABI mgs_backward_clouds_aa).  `camera_grads=True`: every cloud's dict also holds the gradients
+    the forward was given (C ABI mgs_render_options.antialiasing).  `camera_grads=True`: every cloud's dict also holds the gradients
     with respect to its views' viewmatrix, projmatrix and campos, "dL_dviewmatrix" [V_b,16], "dL_dprojmatrix" [V_b,16] and
-    "dL_dcampos" [V_b,3] (C ABI mgs_backward_clouds_cam).  Clouds with a device field of view (see rasterize_clouds_raw)
-    make the call mgs_backward_clouds_intr, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict.  A cloud's
+    "dL_dcampos" [V_b,3] (C ABI mgs_render_options.camera_grad).  Clouds with a device field of view (see rasterize_clouds_raw)
+    pass it as mgs_render_options.intrinsics, and `camera_grads=True` then adds "dL_dtan_fov" [V_b,2] to every dict.  A cloud's
     "grad_median" [V_b,H,W] is the cotangent of a `return_median` forward's median-depth planes, with "median_id" [V_b,H,W]
-    int32 the id planes that forward returned (C ABI mgs_backward_clouds_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
+    int32 the id planes that forward returned (C ABI mgs_view_median).  A cloud's "grad_normal" [V_b,3,H,W] is the
     cotangent of a `return_normal` forward's normal planes, with "normal" [V_b,3,H,W] the planes that forward returned (C ABI
-    mgs_backward_clouds_normal).  Clouds with an orthographic view (see rasterize_clouds_raw) make the call
-    mgs_backward_clouds_ortho, clouds with a fisheye view mgs_backward_clouds_fisheye, and clouds with a distorted view
-    mgs_backward_clouds_distorted.  A cloud rendered with "flow_means3D" (and "flow_poses") also takes "flow" [V_b,3,H,W],
-    the planes its forward returned, and "grad_flow" [V_b,2 or 3,H,W], their cotangent (C ABI mgs_backward_clouds_flow);
+    mgs_view_normal).  The camera models of the clouds (see rasterize_clouds_raw) go to mgs_render_options.ortho, fisheye
+    and distortion.  A cloud rendered with "flow_means3D" (and "flow_poses") also takes "flow" [V_b,3,H,W],
+    the planes its forward returned, and "grad_flow" [V_b,2 or 3,H,W], their cotangent (C ABI mgs_render_options.flow and flow_next);
     its dict then holds "dL_dflow_means3D" [P,3]."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, any(c.get("grad_normal") is not None for c in clouds))
@@ -2034,53 +1918,12 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                     gr[name] = t[offsets[b]:offsets[b + 1]]
         rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
         oarr, farr, dcarr = _clouds_lens(clouds)
-        if flarr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_flow(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
-                                                marr, narr, oarr, farr, dcarr, int(pln), flarr, cfarr, *rest),
-                     "mgs_backward_clouds_flow")
-        elif pln:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_planar(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
-                                                  marr, narr, oarr, farr, dcarr, 1, *rest), "mgs_backward_clouds_planar")
-        elif dcarr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_distorted(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr,
-                                                     marr, narr, oarr, farr, dcarr, *rest), "mgs_backward_clouds_distorted")
-        elif farr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_fisheye(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
-                                                   narr, oarr, farr, *rest), "mgs_backward_clouds_fisheye")
-        elif oarr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_ortho(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
-                                                 narr, oarr, *rest), "mgs_backward_clouds_ortho")
-        elif narr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_normal(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
-                                                  narr, *rest), "mgs_backward_clouds_normal")
-        elif marr is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-            _b.check(L.mgs_backward_clouds_median(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, marr,
-                                                  *rest), "mgs_backward_clouds_median")
-        elif tf is not None:
-            iarr = _intrinsics_array(tf, cam[3] if cam is not None else None)
-            _b.check(L.mgs_backward_clouds_intr(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, iarr, *rest),
-                     "mgs_backward_clouds_intr")
-        elif camarr is not None:
-            _b.check(L.mgs_backward_clouds_cam(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, camarr, *rest),
-                     "mgs_backward_clouds_cam")
-        elif sarr is not None:
-            _b.check(L.mgs_backward_clouds_ssim(B, carr, offs, arr, aarr, darr, int(bool(antialiasing)), sarr, *rest),
-                     "mgs_backward_clouds_ssim")
-        elif antialiasing:
-            _b.check(L.mgs_backward_clouds_aa(B, carr, offs, arr, aarr, darr, 1, *rest), "mgs_backward_clouds_aa")
-        elif darr is not None:
-            _b.check(L.mgs_backward_clouds_depth_mask(B, carr, offs, arr, aarr, darr, *rest), "mgs_backward_clouds_depth_mask")
-        elif aarr is not None:
-            _b.check(L.mgs_backward_clouds_alpha(B, carr, offs, arr, aarr, *rest), "mgs_backward_clouds_alpha")
-        else:
-            _b.check(L.mgs_backward_clouds(B, carr, offs, arr, *rest), "mgs_backward_clouds")
+        iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
+        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, camera_grad=camarr, intrinsics=iarr, median=marr,
+                                normal=narr, ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
+                                flow_next=cfarr if flarr is not None else None, antialiasing=int(bool(antialiasing)),
+                                planar_depth=int(pln))
+        _b.check(L.mgs_backward_clouds(B, carr, offs, arr, opts, *rest), "mgs_backward_clouds")
     return grads
 
 

@@ -1,4 +1,4 @@
-"""Float64 restatement of planar depth (include/mgs_rasterizer.h, mgs_forward_views_planar), in torch so that its gradients
+"""Float64 restatement of planar depth (include/mgs_rasterizer.h, mgs_render_options.planar_depth), in torch so that its gradients
 come from autograd rather than from the hand chain of project_bwd.cu.
 
 For Gaussian i in a view with t = Rv p + tv: Sigma_c = Rv S Rv^T, J the view model's 2x3 screen Jacobian in pixels, Q the

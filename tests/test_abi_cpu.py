@@ -11,7 +11,7 @@ import util  # noqa: F401  (sys.path)
 from manigaussian_b200 import _binding
 
 
-def test_library_exports_every_declared_symbol_of_abi_300():
+def test_library_exports_every_declared_symbol_of_abi_400():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     declared = set(re.findall(r"\b(mgs_[a-z_]+)\s*\(", hdr)) - {"mgs_alloc_fn"}
@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol_of_abi_300():
     for sym in sorted(declared):
         assert hasattr(L, sym), f"{sym} declared in include/mgs_rasterizer.h but not exported"
     assert declared == set(_binding.EXPORTED_SYMBOLS)
-    assert L.mgs_abi_version() == 300
+    assert L.mgs_abi_version() == 400
 
 
 def test_state_size_queries_are_monotone_and_aligned():

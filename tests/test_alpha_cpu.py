@@ -1,4 +1,4 @@
-"""The alpha plane (accumulated opacity 1 - final_T) without a GPU: the C ABI declares and exports its four entry points while
+"""The alpha plane (accumulated opacity 1 - final_T) without a GPU: the C ABI declares its struct and options field while
 the existing view and cloud structs keep their layouts, and the alpha expectations built from the C oracle
 (tests/alpha_oracle.py) are right: the plane against the reference's stored final_T, the gradient against central
 differences of the oracle's own 1 - final_T."""
@@ -15,7 +15,6 @@ import util
 from manigaussian_b200 import _binding
 import alpha_oracle as A
 
-ALPHA_CALLS = ("mgs_forward_views_alpha", "mgs_backward_views_alpha", "mgs_forward_clouds_alpha", "mgs_backward_clouds_alpha")
 # mgs_view as C callers compiled against ABI 300 hold it: the alpha plane must not move a field
 VIEW_FIELDS = ("viewmatrix", "projmatrix", "cam_pos", "background", "tan_fovx", "tan_fovy", "width", "height", "geometry_state",
                "binning_state", "image_state", "binning_capacity", "out_color", "out_feature", "out_depth", "radii", "status",
@@ -23,17 +22,13 @@ VIEW_FIELDS = ("viewmatrix", "projmatrix", "cam_pos", "background", "tan_fovx", 
                "cot_color", "cot_feature", "loss_acc", "cot_scale")
 
 
-def test_header_declares_and_library_exports_the_alpha_calls():
+def test_header_declares_the_alpha_struct_and_option():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     code = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     assert re.search(r"typedef struct mgs_view_alpha \{\s*float\* out_alpha;\s*const float\* dL_dpix_alpha;\s*\} mgs_view_alpha;", code)
-    L = _binding.lib()
-    for name in ALPHA_CALLS:
-        assert re.search(r"\b%s\s*\(" % name, code), name
-        assert name in _binding.EXPORTED_SYMBOLS and hasattr(L, name), name
+    assert re.search(r"typedef struct mgs_render_options \{[^}]*const mgs_view_alpha\* alpha;", code)
     assert [f for f, _ in _binding.ViewAlpha._fields_] == ["out_alpha", "dL_dpix_alpha"]
     assert ctypes.sizeof(_binding.ViewAlpha) == 2 * ctypes.sizeof(ctypes.c_void_p)
-    assert L.mgs_abi_version() == 300
 
 
 def test_view_and_cloud_layouts_are_unchanged():
@@ -44,19 +39,19 @@ def test_view_and_cloud_layouts_are_unchanged():
     assert ctypes.sizeof(_binding.Cloud) == 17 * ptr
 
 
-def test_alpha_calls_check_their_arguments_without_a_gpu():
+def test_alpha_option_checks_its_arguments_without_a_gpu():
     L = _binding.lib()
     views = (_binding.View * 1)()
-    alpha = (_binding.ViewAlpha * 1)()
-    rc = L.mgs_forward_views_alpha(0, views, alpha, 10, 1, 4, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None)
+    alpha = _binding.RenderOptions(alpha=(_binding.ViewAlpha * 1)())
+    rc = L.mgs_forward_views(0, views, alpha, 10, 1, 4, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None)
     assert rc < 0 and _binding.last_error()
-    rc = L.mgs_backward_views_alpha(1, views, alpha, 0, 1, 4, 0, None, None, None, None, None, 1.0, None, None,
-                                    None, None, None, None, None, None, None, None, 1, 0, 3, 0, None)
+    rc = L.mgs_backward_views(1, views, alpha, 0, 1, 4, 0, None, None, None, None, None, 1.0, None, None,
+                              None, None, None, None, None, None, None, None, 1, 0, 3, 0, None)
     assert rc < 0
     offs = (ctypes.c_int * 2)(0, 1)
     clouds = (_binding.Cloud * 1)()
-    assert L.mgs_forward_clouds_alpha(0, clouds, offs, views, alpha, 1, 4, 0, 1.0, 0, 0, None) < 0
-    assert L.mgs_backward_clouds_alpha(1, clouds, offs, views, None, 1, 4, 0, 1.0, 0, 0, None) < 0  # P = 0
+    assert L.mgs_forward_clouds(0, clouds, offs, views, alpha, 1, 4, 0, 1.0, 0, 0, None) < 0
+    assert L.mgs_backward_clouds(1, clouds, offs, views, None, 1, 4, 0, 1.0, 0, 0, None) < 0  # P = 0
 
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "g[0-9]*.npz")))

@@ -1,4 +1,4 @@
-"""The anti-aliased projection without a GPU: the C ABI declares and exports its four entry points and rejects an
+"""The anti-aliased projection without a GPU: the C ABI declares its switch in the render options and rejects an
 out-of-range switch before enqueueing anything, the settings keep the reference's 13 fields with `antialiasing` as a 14th
 argument, and the expectations of tests/aa_oracle.py (the unmodified C oracle plus a float64 compensation) are right: mode
 on changes only the opacity the blend sees and keeps the oracle's own chain, the float64 screen covariance is the oracle's,
@@ -18,45 +18,35 @@ from manigaussian_b200 import _binding
 import aa_oracle as A
 from oracle import gs_oracle as O
 
-AA_CALLS = ("mgs_forward_views_aa", "mgs_backward_views_aa", "mgs_forward_clouds_aa", "mgs_backward_clouds_aa")
+AA_CALLS = ("mgs_forward_views", "mgs_backward_views", "mgs_forward_clouds", "mgs_backward_clouds")
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "g[0-9]*.npz")))
 MGS_ERR_INVALID_ARG = -1
 
 
-def test_header_declares_and_library_exports_the_aa_calls():
+def test_header_declares_the_aa_option():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     code = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
-    L = _binding.lib()
-    for name in AA_CALLS:
-        m = re.search(r"\bint\s+%s\s*\(([^;]*)\);" % name, code)
-        assert m, name
-        params = [p.strip() for p in m.group(1).split(",")]
-        base = re.search(r"\bint\s+%s\s*\(([^;]*)\);" % name.replace("_aa", "_depth_mask"), code).group(1).split(",")
-        # the _depth_mask call's parameters with `int antialiasing` right after depth_mask
-        k = [i for i, p in enumerate(params) if p.endswith("depth_mask")][0]
-        assert params[k + 1] == "int antialiasing" and len(params) == len(base) + 1, name
-        assert name in _binding.EXPORTED_SYMBOLS and hasattr(L, name), name
-        at, bt = getattr(L, name).argtypes, getattr(L, name.replace("_aa", "_depth_mask")).argtypes
-        assert len(at) == len(params) and at[:k + 1] == bt[:k + 1] and at[k + 1] is C.c_int and at[k + 2:] == bt[k + 1:], name
-    assert L.mgs_abi_version() == 300
+    assert re.search(r"typedef struct mgs_render_options \{[^}]*\bint antialiasing;", code)
+    assert dict(_binding.RenderOptions._fields_)["antialiasing"] is C.c_int
     hm = re.search(r"#define\s+MGS_ERR_INVALID_ARG\s+\(?(-?\d+)\)?", hdr)
     assert hm and int(hm.group(1)) == MGS_ERR_INVALID_ARG
 
 
 @pytest.mark.parametrize("value", [-1, 2, 7])
-def test_out_of_range_switch_is_rejected_before_anything_runs(value):
+def test_out_of_range_aa_option_is_rejected_before_anything_runs(value):
     """Every other argument is valid-looking or NULL: the switch is checked first, so no stream or pointer is touched."""
     L = _binding.lib()
     views = (_binding.View * 1)()
     offs = (C.c_int * 2)(0, 1)
     clouds = (_binding.Cloud * 1)()
     clouds[0].P = 10
+    opts = _binding.RenderOptions(antialiasing=value)
     rcs = [
-        L.mgs_forward_views_aa(1, views, None, None, value, 10, 1, 4, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None),
-        L.mgs_backward_views_aa(1, views, None, None, value, 10, 1, 4, 0, None, None, None, None, None, 1.0, None, None,
-                                None, None, None, None, None, None, None, None, 1, 0, 3, 0, None),
-        L.mgs_forward_clouds_aa(1, clouds, offs, views, None, None, value, 1, 4, 0, 1.0, 0, 0, None),
-        L.mgs_backward_clouds_aa(1, clouds, offs, views, None, None, value, 1, 4, 0, 1.0, 0, 0, None),
+        L.mgs_forward_views(1, views, opts, 10, 1, 4, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None),
+        L.mgs_backward_views(1, views, opts, 10, 1, 4, 0, None, None, None, None, None, 1.0, None, None,
+                             None, None, None, None, None, None, None, None, 1, 0, 3, 0, None),
+        L.mgs_forward_clouds(1, clouds, offs, views, opts, 1, 4, 0, 1.0, 0, 0, None),
+        L.mgs_backward_clouds(1, clouds, offs, views, opts, 1, 4, 0, 1.0, 0, 0, None),
     ]
     for name, rc in zip(AA_CALLS, rcs):
         assert rc == MGS_ERR_INVALID_ARG, name

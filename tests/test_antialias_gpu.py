@@ -67,16 +67,18 @@ def _run(inp, aa, scale_modifier=1.0, prefiltered=False, capacity=None, backward
     return k
 
 
-def test_mode_off_through_the_aa_calls_is_the_existing_path(monkeypatch):
-    """The _aa calls with 0 in place of mgs_forward_views / mgs_backward_views: images, radii and instance counts bit for bit,
-    gradients within the run-to-run spread of the blend's float atomics."""
+def test_mode_off_through_a_null_options_record_is_the_same_path(monkeypatch):
+    """mgs_forward_views / mgs_backward_views with a NULL options record in place of the all-zero record (antialiasing 0) the
+    Python layer passes: images, radii and instance counts bit for bit, gradients within the run-to-run spread of the blend's
+    float atomics."""
     from manigaussian_b200 import _binding
     inp = util.make_inputs(P=20000, W=128, H=96, F=32, seed=31, bg=(0.2, 0.3, 0.4))
     a = _run(inp, False)
     a2 = _run(inp, False, capacity=a["cap"])
     L = _binding.lib()
-    monkeypatch.setattr(L, "mgs_forward_views", lambda V, arr, *rest: L.mgs_forward_views_aa(V, arr, None, None, 0, *rest), raising=False)
-    monkeypatch.setattr(L, "mgs_backward_views", lambda V, arr, *rest: L.mgs_backward_views_aa(V, arr, None, None, 0, *rest), raising=False)
+    fwd, bwd = L.mgs_forward_views, L.mgs_backward_views
+    monkeypatch.setattr(L, "mgs_forward_views", lambda V, arr, opts, *rest: fwd(V, arr, None, *rest), raising=False)
+    monkeypatch.setattr(L, "mgs_backward_views", lambda V, arr, opts, *rest: bwd(V, arr, None, *rest), raising=False)
     b = _run(inp, False, capacity=a["cap"])
     for key in ("color", "feature", "radii", "R", "point_list", "final_T"):
         assert np.array_equal(a[key], b[key]), key

@@ -53,10 +53,9 @@ def test_camera_batch_is_differentiable_in_w2c():
     assert cb.world_view_transform.requires_grad and cb.camera_center.requires_grad
 
 
-def test_camera_symbols_are_exported_and_check_their_arguments():
+def test_camera_option_checks_its_arguments():
     L = _binding.lib()
-    for name in ("mgs_camera_grad_scratch_bytes", "mgs_backward_views_cam", "mgs_backward_clouds_cam"):
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
+    assert hasattr(L, "mgs_camera_grad_scratch_bytes") and "mgs_camera_grad_scratch_bytes" in _binding.EXPORTED_SYMBOLS
     assert L.mgs_camera_grad_scratch_bytes(1) == 27 * 4
     assert L.mgs_camera_grad_scratch_bytes(16384) == 128 * 27 * 4
     assert L.mgs_camera_grad_scratch_bytes(16385) == 129 * 27 * 4
@@ -69,14 +68,15 @@ def test_camera_symbols_are_exported_and_check_their_arguments():
     v.binning_capacity = 1
     cam = (_binding.ViewCameraGrad * 1)()
     cam[0].dL_dviewmatrix = 4096   # an output without scratch
-    rc = L.mgs_backward_views_cam(1, views, None, None, 0, None, cam, 4, 0, 0, 0, 4096, None, 4096, None, None, 1.0, None, 4096,
-                                  4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
+    cam = _binding.RenderOptions(camera_grad=cam)
+    rc = L.mgs_backward_views(1, views, cam, 4, 0, 0, 0, 4096, None, 4096, None, None, 1.0, None, 4096,
+                              4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
     assert rc == -1 and "scratch" in _binding.last_error()
     clouds = (_binding.Cloud * 1)()
     c = clouds[0]
     c.P, c.means3D, c.colors_precomp, c.dL_dmean3D, c.dL_dopacity = 4, 4096, 4096, 4096, 4096
     offs = (ctypes.c_int * 2)(0, 1)
-    rc = L.mgs_backward_clouds_cam(1, clouds, offs, views, None, None, 0, None, cam, 0, 0, 0, 1.0, 0, 0, None)
+    rc = L.mgs_backward_clouds(1, clouds, offs, views, cam, 0, 0, 0, 1.0, 0, 0, None)
     assert rc == -1 and "scratch" in _binding.last_error()
 
 

@@ -396,7 +396,7 @@ def test_every_camera_entry_is_within_the_float64_bound(kind, deg, aa, nv):
     assert not problems, problems[:3]
 
 
-def test_stage_two_with_and_without_cameras_on_the_same_records():
+def test_stage_two_with_and_without_the_camera_option_on_the_same_records():
     """Stage 1 (the blend backward) once, then stage 2 (the per-Gaussian kernel) without cam, with cam, and with cam again on
     the same blend-stage records: the two CAM runs are bit-identical in every output, camera gradients included; without
     cam the per-Gaussian outputs agree to the last bits (a separately compiled instantiation)."""
@@ -416,15 +416,16 @@ def test_stage_two_with_and_without_cameras_on_the_same_records():
             def __getattr__(self, name):
                 return getattr(real, name)
 
-            def mgs_backward_views_cam(self, *args):
+            def mgs_backward_views(self, *args):
                 stages = args[-3]
                 if stages != 2:
-                    return real.mgs_backward_views_cam(*args)
+                    return real.mgs_backward_views(*args)
                 for with_cam in (False, True, True):
                     a = list(args)
                     if not with_cam:
-                        a[6] = None
-                    rc = real.mgs_backward_views_cam(*a)
+                        a[2] = B.RenderOptions.from_buffer_copy(args[2])
+                        a[2].camera_grad = None
+                    rc = real.mgs_backward_views(*a)
                     if rc < 0:
                         return rc
                     torch.cuda.synchronize()

@@ -39,15 +39,15 @@ def _offsets(*o):
 
 def _both(B, clouds, offsets, views):
     L = _binding.lib()
-    rf = L.mgs_forward_clouds(B, clouds, offsets, views, 1, 4, 3, 1.0, 0, 0, None)
+    rf = L.mgs_forward_clouds(B, clouds, offsets, views, None, 1, 4, 3, 1.0, 0, 0, None)
     ef = _binding.last_error()
-    rb = L.mgs_backward_clouds(B, clouds, offsets, views, 1, 4, 3, 1.0, 0, 0, None)
+    rb = L.mgs_backward_clouds(B, clouds, offsets, views, None, 1, 4, 3, 1.0, 0, 0, None)
     eb = _binding.last_error()
     return (rf, ef), (rb, eb)
 
 
 @pytest.mark.parametrize("case", ["B=0", "offsets_not_from_0", "offsets_not_increasing", "P=0", "P<0"])
-def test_malformed_clouds_are_refused_by_both_directions(case):
+def test_malformed_clouds_are_refused_by_both_clouds_calls(case):
     B, clouds, offsets, views = 2, _clouds(2), _offsets(0, 1, 3), _views(3)
     if case == "B=0":
         B = 0
@@ -63,7 +63,7 @@ def test_malformed_clouds_are_refused_by_both_directions(case):
         assert rc == MGS_ERR_INVALID_ARG and msg, msg
 
 
-def test_missing_pointers_are_refused():
+def test_missing_cloud_pointers_are_refused():
     L = _binding.lib()
     views, offs = _views(3), _offsets(0, 1, 3)
     c = _clouds(2)
@@ -72,30 +72,30 @@ def test_missing_pointers_are_refused():
         assert rc == MGS_ERR_INVALID_ARG and "means3D" in msg
     c = _clouds(2)
     c[0].opacities = None
-    assert L.mgs_forward_clouds(2, c, offs, views, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
+    assert L.mgs_forward_clouds(2, c, offs, views, None, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
     c = _clouds(2)
     c[1].shs = None  # neither SHs nor precomputed colours
-    assert L.mgs_forward_clouds(2, c, offs, views, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
+    assert L.mgs_forward_clouds(2, c, offs, views, None, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
     c = _clouds(2)
     c[0].scales = None  # neither scales+rotations nor a covariance
-    assert L.mgs_forward_clouds(2, c, offs, views, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
+    assert L.mgs_forward_clouds(2, c, offs, views, None, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
     c = _clouds(2)
     c[1].dL_dopacity = None
-    assert L.mgs_backward_clouds(2, c, offs, views, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
+    assert L.mgs_backward_clouds(2, c, offs, views, None, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG
     # a view of the second cloud without its state buffers / without its feature cotangents
     for field, direction in (("image_state", "mgs_forward_clouds"), ("image_state", "mgs_backward_clouds"),
                              ("dL_dpix_F", "mgs_backward_clouds")):
         v = _views(3)
         setattr(v[2], field, None)
-        assert getattr(L, direction)(2, _clouds(2), offs, v, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG, (field, direction)
+        assert getattr(L, direction)(2, _clouds(2), offs, v, None, 1, 4, 3, 1.0, 0, 0, None) == MGS_ERR_INVALID_ARG, (field, direction)
         assert "view" in _binding.last_error()
 
 
-def test_shs_without_their_gradient_are_refused():
+def test_cloud_shs_without_their_gradient_are_refused():
     """dL_dsh carries the view-direction term of dL_dmean3D: without it that term would be dropped silently."""
     c = _clouds(2)
     c[1].dL_dsh = None
-    rc = _binding.lib().mgs_backward_clouds(2, c, _offsets(0, 1, 3), _views(3), 1, 4, 3, 1.0, 0, 0, None)
+    rc = _binding.lib().mgs_backward_clouds(2, c, _offsets(0, 1, 3), _views(3), None, 1, 4, 3, 1.0, 0, 0, None)
     assert rc == MGS_ERR_INVALID_ARG and "dL_dsh" in _binding.last_error()
 
 

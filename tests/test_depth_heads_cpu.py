@@ -12,8 +12,6 @@ import util
 from manigaussian_b200 import _binding
 import depth_heads_oracle as O
 
-CALLS = ("mgs_forward_views_depth_mask", "mgs_backward_views_depth_mask", "mgs_forward_clouds_depth_mask",
-         "mgs_backward_clouds_depth_mask")
 FIELDS = ("target_depth", "target_mask", "cot_depth", "cot_alpha_depth", "cot_alpha_mask", "loss_acc", "cot_scale")
 
 
@@ -69,18 +67,14 @@ def test_oracle_matches_torch_recipe(seed, empty):
     assert cd.flat[0] == 0 and ca.flat[0] == 0
 
 
-def test_header_declares_and_library_exports_the_depth_mask_calls():
+def test_header_declares_the_depth_mask_struct_and_option():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     code = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     m = re.search(r"typedef struct mgs_view_depth_mask \{(.*?)\} mgs_view_depth_mask;", code, flags=re.S)
     assert m
     fields = re.findall(r"\*\s*(\w+);", m.group(1))
     assert tuple(fields) == FIELDS
-    L = _binding.lib()
-    for name in CALLS:
-        assert re.search(r"\b%s\s*\(" % name, code), name
-        assert name in _binding.EXPORTED_SYMBOLS and hasattr(L, name), name
-    assert L.mgs_abi_version() == 300
+    assert re.search(r"typedef struct mgs_render_options \{[^}]*const mgs_view_depth_mask\* depth_mask;", code)
 
 
 def test_struct_layout_matches_the_header():
@@ -101,7 +95,7 @@ def _view(**kw):
 
 
 @pytest.mark.parametrize("case", ["depth_without_planes", "mask_without_plane", "no_accumulator", "no_colour_head"])
-def test_depth_mask_calls_check_their_arguments_without_a_gpu(case):
+def test_depth_mask_option_checks_its_arguments_without_a_gpu(case):
     L = _binding.lib()
     colour = dict(target_color=16, cot_color=16, loss_acc=16)
     views = (_binding.View * 1)(_view(**({} if case == "no_colour_head" else colour)))
@@ -115,18 +109,19 @@ def test_depth_mask_calls_check_their_arguments_without_a_gpu(case):
         dm[0].target_depth, dm[0].cot_depth, dm[0].cot_alpha_depth, dm[0].loss_acc = 16, 16, 16, None
     else:
         dm[0].target_mask, dm[0].cot_alpha_mask = 16, 16
-    rc = L.mgs_forward_views_depth_mask(1, views, None, dm, 10, 1, 4, 0, 16, 16, None, None, 16, 16, 1.0, 16, None, 0, 0, None)
+    dm = _binding.RenderOptions(depth_mask=dm)
+    rc = L.mgs_forward_views(1, views, dm, 10, 1, 4, 0, 16, 16, None, None, 16, 16, 1.0, 16, None, 0, 0, None)
     assert rc == -1  # MGS_ERR_INVALID_ARG
     assert ("colour head" if case == "no_colour_head" else "target" if case != "no_accumulator" else "loss_acc") in _binding.last_error()
     offs = (ctypes.c_int * 2)(0, 1)
     clouds = (_binding.Cloud * 1)()
     clouds[0].P, clouds[0].means3D, clouds[0].opacities, clouds[0].shs, clouds[0].scales, clouds[0].rotations = 10, 16, 16, 16, 16, 16
-    rc = L.mgs_forward_clouds_depth_mask(1, clouds, offs, views, None, dm, 1, 4, 0, 1.0, 0, 0, None)
+    rc = L.mgs_forward_clouds(1, clouds, offs, views, dm, 1, 4, 0, 1.0, 0, 0, None)
     assert rc == -1
     if case != "no_colour_head":  # the backward does not need the colour head's targets
-        rc = L.mgs_backward_views_depth_mask(1, views, None, dm, 10, 1, 4, 0, 16, 16, None, None, 16, 1.0, 16, None,
-                                             16, 16, None, None, None, 16, 16, 16, 1, 0, 3, 0, None)
+        rc = L.mgs_backward_views(1, views, dm, 10, 1, 4, 0, 16, 16, None, None, 16, 1.0, 16, None,
+                                  16, 16, None, None, None, 16, 16, 16, 1, 0, 3, 0, None)
         assert rc == -1
         clouds[0].dL_dmean3D, clouds[0].dL_dopacity, clouds[0].dL_dsh = 16, 16, 16
-        rc = L.mgs_backward_clouds_depth_mask(1, clouds, offs, views, None, dm, 1, 4, 0, 1.0, 0, 0, None)
+        rc = L.mgs_backward_clouds(1, clouds, offs, views, dm, 1, 4, 0, 1.0, 0, 0, None)
         assert rc == -1

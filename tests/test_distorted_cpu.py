@@ -9,7 +9,7 @@ distortion_r_max and the C ABI's checks.
 * With all coefficients 0 the records and per-Gaussian gradients are the pinhole reference's inside the clamp region.
 * distortion_r_max: the fold of k1 < 0 alone, a zero of the rational denominator, monotone coefficients, 4- and 5-entry D.
 * Each broken convention of distorted_ref64.MUTATIONS moves a checked element past twice its bound.
-* The _distorted symbols are exported; bad parameters return MGS_ERR_INVALID_ARG before anything is enqueued.
+* Bad distortion parameters in the render options and the lift return MGS_ERR_INVALID_ARG before anything is enqueued.
 """
 import ctypes
 import math
@@ -365,11 +365,8 @@ BAD = [("flag", dict(distorted=2)), ("ortho", dict()), ("fisheye", dict()), ("na
 
 
 @pytest.mark.parametrize("what,bad", BAD, ids=[b[0] for b in BAD])
-def test_distorted_symbols_check_their_parameters(what, bad):
+def test_distortion_option_checks_its_parameters(what, bad):
     L = _binding.lib()
-    for name in ("mgs_forward_views_distorted", "mgs_backward_views_distorted", "mgs_forward_clouds_distorted",
-                 "mgs_backward_clouds_distorted", "mgs_lift_views_distorted"):
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
     views = (_binding.View * 2)()
     for v in views:
         v.width, v.height, v.tan_fovx, v.tan_fovy = 8, 8, 0.5, 0.5
@@ -386,23 +383,20 @@ def test_distorted_symbols_check_their_parameters(what, bad):
     if what == "fisheye":
         fe = (_binding.ViewFisheye * 2)()
         fe[1].fisheye, fe[1].cx, fe[1].cy, fe[1].theta_max = 1, 3.5, 3.5, 1.5
+    opts = _binding.RenderOptions(ortho=ortho, fisheye=fe, distortion=dc)
     # pointers are never dereferenced: the parameters are checked before anything is enqueued
     rcs = [
-        L.mgs_forward_views_distorted(2, views, None, None, 0, None, None, None, None, ortho, fe, dc, 4, 0, 0, 0, 4096, None, 4096,
-                                      None, 4096, 4096, 1.0, 4096, None, 0, 0, None),
-        L.mgs_backward_views_distorted(2, views, None, None, 0, None, None, None, None, None, ortho, fe, dc, 4, 0, 0, 0, 4096, None,
-                                       4096, None, 4096, 1.0, 4096, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0,
-                                       None),
-        L.mgs_lift_views_distorted(2, views, None, 0, None, ortho, fe, dc, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None,
+        L.mgs_forward_views(2, views, opts, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096, 1.0, 4096, None, 0, 0, None),
+        L.mgs_backward_views(2, views, opts, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 1.0, 4096, None, 4096, 4096, None, None, None,
+                             None, None, None, 0, 0, 3, 0, None),
+        L.mgs_lift_views(2, views, None, 0, None, ortho, fe, dc, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None,
                                    None, 4096, 0, None)]
     clouds = (_binding.Cloud * 1)()
     c = clouds[0]
     c.P, c.means3D, c.colors_precomp, c.opacities, c.scales, c.rotations = 4, 4096, 4096, 4096, 4096, 4096
     c.dL_dmean3D, c.dL_dopacity = 4096, 4096
     offs = (ctypes.c_int * 2)(0, 2)
-    rcs.append(L.mgs_forward_clouds_distorted(1, clouds, offs, views, None, None, 0, None, None, None, None, ortho, fe, dc, 0, 0, 0,
-                                              1.0, 0, 0, None))
-    rcs.append(L.mgs_backward_clouds_distorted(1, clouds, offs, views, None, None, 0, None, None, None, None, None, ortho, fe, dc, 0,
-                                               0, 0, 1.0, 0, 0, None))
+    rcs.append(L.mgs_forward_clouds(1, clouds, offs, views, opts, 0, 0, 0, 1.0, 0, 0, None))
+    rcs.append(L.mgs_backward_clouds(1, clouds, offs, views, opts, 0, 0, 0, 1.0, 0, 0, None))
     for rc in rcs:
         assert rc == -1 and "distortion" in _binding.last_error(), (what, rc, _binding.last_error())

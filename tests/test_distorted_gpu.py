@@ -11,8 +11,8 @@
   precomputed colours and covariances, and 20 clouds (the clouds kernels' large parameter block).
 * A zero-coefficient distorted view renders the pinhole view of the same K, and one loss's gradients agree.
 * Mixed pinhole + orthographic + fisheye + distorted batches: images, radii, sort keys and instance counts bit-identical to
-  each view rendered alone, gradients the sum over the views within 1e-5 relative L2.  All-zero distortion entries through
-  the _distorted calls match the _fisheye calls bit for bit (gradients within 1e-5: the float atomics' order).
+  each view rendered alone, gradients the sum over the views within 1e-5 relative L2.  All-zero distortion entries match
+  a NULL distortion array bit for bit (gradients within 1e-5: the float atomics' order).
 * Public paths: render_views with every option, render_clouds, lift_views, GaussianRasterizer, a CUDA-graph replay and no
   device memory growth.
 
@@ -462,13 +462,12 @@ def test_mixed_views_of_one_cloud_in_render_clouds():
 
 
 def test_zero_entries_match_the_fisheye_calls(monkeypatch):
-    """All-zero distortion entries through the _distorted calls give the _fisheye calls' results (which are the _distorted
-    calls with NULL): the entries' other fields are ignored, and the launches run the FISH kernels."""
+    """All-zero distortion entries give the results of a NULL distortion array: the entries' other fields are ignored, and the launches run the FISH kernels."""
     from manigaussian_b200 import _binding as B
     from manigaussian_b200 import rasterizer as R
     g = TP._cloud_g(3000, 1, 13)
     views = [TP.settings(TO._pcam(0, 3), 1), TO.osettings(TO.ocam(1, 3), 1), fsettings(fcam(2, 3, k=UMI_K), 1)]
-    o0, g0, _, _ = _render_raw(views, g, camera=True)   # the _fisheye calls
+    o0, g0, _, _ = _render_raw(views, g, camera=True)   # no distortion array
     calls = []
     real = R._distortion_array
 

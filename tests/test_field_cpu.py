@@ -14,13 +14,12 @@ from manigaussian_b200 import _binding
 from manigaussian_b200 import gaussian_renderer as GR
 
 
-def test_header_declares_and_the_library_exports_the_field_calls():
+def test_field_calls_are_declared_and_exported():
     hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read(), flags=re.S)
     L = _binding.lib()
     for name in ("mgs_field_query", "mgs_field_query_backward"):
         assert re.search(r"\b%s\s*\(" % name, hdr), name
         assert name in _binding.EXPORTED_SYMBOLS and hasattr(L, name)
-    assert L.mgs_abi_version() == 300
 
 
 _CB = _binding.ALLOC_FN(lambda u, n: 0)  # never called: every case fails before anything is allocated

@@ -8,7 +8,7 @@
 * With k = 0 and a small-angle scene, the fisheye records converge to the pinhole records as the angles shrink.
 * Builders: tan_fov = W / (2 fx), theta_max against the root of rho', learnable focal lengths; the errors.
 * Each broken convention of fisheye_ref64.MUTATIONS moves a checked element past twice its bound.
-* The _fisheye symbols are exported; bad parameters return MGS_ERR_INVALID_ARG before anything is enqueued.
+* Bad fisheye parameters in the render options and the lift return MGS_ERR_INVALID_ARG before anything is enqueued.
 """
 import ctypes
 import math
@@ -366,11 +366,8 @@ BAD = [("flag", dict(fisheye=2)), ("ortho", dict()), ("nan", dict(k2=float("nan"
 
 
 @pytest.mark.parametrize("what,bad", BAD, ids=[b[0] for b in BAD])
-def test_fisheye_symbols_check_their_parameters(what, bad):
+def test_fisheye_option_checks_its_parameters(what, bad):
     L = _binding.lib()
-    for name in ("mgs_forward_views_fisheye", "mgs_backward_views_fisheye", "mgs_forward_clouds_fisheye",
-                 "mgs_backward_clouds_fisheye", "mgs_lift_views_fisheye"):
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
     views = (_binding.View * 2)()
     for v in views:
         v.width, v.height, v.tan_fovx, v.tan_fovy = 8, 8, 0.5, 0.5
@@ -383,22 +380,20 @@ def test_fisheye_symbols_check_their_parameters(what, bad):
     for k, x in bad.items():
         setattr(fe[1], k, x)
     ortho = (ctypes.c_int * 2)(0, 1) if what == "ortho" else None
+    opts = _binding.RenderOptions(ortho=ortho, fisheye=fe)
     # pointers are never dereferenced: the parameters are checked before anything is enqueued
     rcs = [
-        L.mgs_forward_views_fisheye(2, views, None, None, 0, None, None, None, None, ortho, fe, 4, 0, 0, 0, 4096, None, 4096, None,
-                                    4096, 4096, 1.0, 4096, None, 0, 0, None),
-        L.mgs_backward_views_fisheye(2, views, None, None, 0, None, None, None, None, None, ortho, fe, 4, 0, 0, 0, 4096, None, 4096,
-                                     None, 4096, 1.0, 4096, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None),
-        L.mgs_lift_views_fisheye(2, views, None, 0, None, ortho, fe, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None, None,
+        L.mgs_forward_views(2, views, opts, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096, 1.0, 4096, None, 0, 0, None),
+        L.mgs_backward_views(2, views, opts, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 1.0, 4096, None, 4096, 4096, None, None, None,
+                             None, None, None, 0, 0, 3, 0, None),
+        L.mgs_lift_views(2, views, None, 0, None, ortho, fe, None, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None, None,
                                  4096, 0, None)]
     clouds = (_binding.Cloud * 1)()
     c = clouds[0]
     c.P, c.means3D, c.colors_precomp, c.opacities, c.scales, c.rotations = 4, 4096, 4096, 4096, 4096, 4096
     c.dL_dmean3D, c.dL_dopacity = 4096, 4096
     offs = (ctypes.c_int * 2)(0, 2)
-    rcs.append(L.mgs_forward_clouds_fisheye(1, clouds, offs, views, None, None, 0, None, None, None, None, ortho, fe, 0, 0, 0, 1.0,
-                                            0, 0, None))
-    rcs.append(L.mgs_backward_clouds_fisheye(1, clouds, offs, views, None, None, 0, None, None, None, None, None, ortho, fe, 0, 0, 0,
-                                             1.0, 0, 0, None))
+    rcs.append(L.mgs_forward_clouds(1, clouds, offs, views, opts, 0, 0, 0, 1.0, 0, 0, None))
+    rcs.append(L.mgs_backward_clouds(1, clouds, offs, views, opts, 0, 0, 0, 1.0, 0, 0, None))
     for rc in rcs:
         assert rc == -1 and "fisheye" in _binding.last_error(), (what, rc, _binding.last_error())

@@ -9,8 +9,8 @@
   KAPPA_FISHEYE_CAM (u e + d) and dL/dtan_fov within KAPPA_FISHEYE_INTR (u e + d), over 1 to 33 views, SH degrees 0-3,
   precomputed colours and covariances, and 20 clouds.  Each instantiation is launched.
 * Mixed pinhole + orthographic + fisheye batches: images, radii, sort keys and instance counts bit-identical to each view
-  rendered alone, gradients the sum over the views within 1e-5 relative L2.  All-zero fisheye entries through the _fisheye
-  calls match the _ortho calls (the _fisheye calls with NULL) bit for bit (gradients within 1e-5: the float atomics' order).
+  rendered alone, gradients the sum over the views within 1e-5 relative L2.  All-zero fisheye entries match a NULL fisheye
+  array bit for bit (gradients within 1e-5: the float atomics' order).
 * Public paths: render_views with every option, render_clouds, lift_views, GaussianRasterizer, a CUDA-graph replay and no
   device memory growth.
 
@@ -404,13 +404,12 @@ def test_mixed_views_of_one_cloud_in_render_clouds():
 
 
 def test_zero_entries_match_the_ortho_calls(monkeypatch):
-    """All-zero fisheye entries through the _fisheye calls give the _ortho calls' results (which are the _fisheye calls with
-    NULL): the entries' other fields are ignored, and the launches run the ORTHO kernels."""
+    """All-zero fisheye entries give the results of a NULL fisheye array: the entries' other fields are ignored, and the launches run the ORTHO kernels."""
     from manigaussian_b200 import _binding as B
     from manigaussian_b200 import rasterizer as R
     g = TP._cloud_g(3000, 1, 13)
     views = [TP.settings(TO._pcam(0, 3), 1), TO.osettings(TO.ocam(1, 3), 1), TP.settings(TO._pcam(2, 3), 1)]
-    o0, g0, _, _ = _render_raw(views, g)   # the _ortho calls
+    o0, g0, _, _ = _render_raw(views, g)   # no fisheye array
     calls = []
     real = R._fisheye_array
 

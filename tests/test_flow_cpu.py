@@ -100,16 +100,9 @@ def test_same_mean_gives_exactly_zero():
         assert float(d.abs().max()) == 0.0
 
 
-def test_abi_exports_and_argument_checks():
+def test_flow_option_argument_checks():
     from manigaussian_b200 import _binding as B
-    names = ("mgs_forward_views_flow", "mgs_backward_views_flow", "mgs_forward_clouds_flow", "mgs_backward_clouds_flow")
-    for n in names:
-        assert n in B.EXPORTED_SYMBOLS
     L = B.lib()
-    assert len(L.mgs_forward_views_flow.argtypes) == len(L.mgs_forward_views_planar.argtypes) + 2
-    assert len(L.mgs_backward_views_flow.argtypes) == len(L.mgs_backward_views_planar.argtypes) + 3
-    assert len(L.mgs_forward_clouds_flow.argtypes) == len(L.mgs_forward_clouds_planar.argtypes) + 2
-    assert len(L.mgs_backward_clouds_flow.argtypes) == len(L.mgs_backward_clouds_planar.argtypes) + 2
     views = (B.View * 1)()
     buf = (C.c_float * 16)()
     means = C.addressof(buf)
@@ -135,7 +128,8 @@ def test_abi_exports_and_argument_checks():
         (None, None, 0, flow(vm=True), means, b"next_projmatrix"),
     ]
     for nrm, d, pln, fl, nxt, what in cases:
-        rc = L.mgs_forward_views_flow(1, views, None, d, 0, None, None, None, nrm, None, None, None, pln, fl, nxt, *rest)
+        opts = B.RenderOptions(depth_mask=d, normal=nrm, planar_depth=pln, flow=fl, flow_next=(B.CloudFlow * 1)((nxt, None)))
+        rc = L.mgs_forward_views(1, views, opts, *rest)
         assert rc == -1, what
         assert what in L.mgs_last_error(), (what, L.mgs_last_error())
 

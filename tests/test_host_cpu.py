@@ -153,7 +153,7 @@ def test_binning_capacity_estimator():
         R._PENDING_STATUS[:] = saved_pending
 
 
-def test_allocator_callback_errors_reach_the_caller():
+def test_allocator_and_library_errors_reach_the_caller():
     """An exception inside the C library's allocation callback (ctypes would print and swallow it) is stashed on the allocator
     and re-raised by the call that triggered it; the allocators are released on every error path."""
     import pytest
@@ -175,7 +175,7 @@ def test_allocator_callback_errors_reach_the_caller():
     # a library error code without a stashed exception raises the binding's error and releases too
     c = R._Alloc("cpu")
     with pytest.raises(Exception):
-        R._checked((c,), B.lib().mgs_forward_views(0, None, 0, 0, 0, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None), "unit")
+        R._checked((c,), B.lib().mgs_forward_views(0, None, None, 0, 0, 0, 0, None, None, None, None, None, None, 1.0, None, None, 0, 0, None), "unit")
     assert c.key not in R._Alloc._live
     d = R._Alloc("cpu")
     assert R._checked((d,), 7, "unit") == 7 and d.key in R._Alloc._live

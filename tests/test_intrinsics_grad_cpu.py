@@ -7,7 +7,7 @@
   moves an entry past twice its bound.
 * cameras.camera_batch with an intr that requires grad builds the matrices of build_cameras (float32 rounding), a [B,2]
   device-side tan_fov, and passes a float64 gradcheck from intr and w2c to all four camera tensors.
-* The _intr symbols are exported, and their argument errors return MGS_ERR_INVALID_ARG before anything is enqueued.
+* The argument errors of the intrinsics option return MGS_ERR_INVALID_ARG before anything is enqueued.
 """
 import ctypes
 import os
@@ -175,11 +175,8 @@ def test_other_intr_forms_are_unchanged():
 
 
 # --------------------------------------------------------------------------- the C ABI
-def test_intrinsics_symbols_are_exported_and_check_their_arguments():
+def test_intrinsics_option_checks_its_arguments():
     L = _binding.lib()
-    for name in ("mgs_forward_views_intr", "mgs_backward_views_intr", "mgs_forward_clouds_intr", "mgs_backward_clouds_intr"):
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
-    assert L.mgs_abi_version() == 300
     views = (_binding.View * 1)()
     v = views[0]
     v.width, v.height, v.tan_fovx, v.tan_fovy = 8, 8, 0.5, 0.5
@@ -191,21 +188,22 @@ def test_intrinsics_symbols_are_exported_and_check_their_arguments():
     intr[0].tan_fov, intr[0].dL_dtan_fov = 4096, 4096
     # dL_dtan_fov with no camera entry, then with a camera entry that has no scratch
     for cam in (None, (_binding.ViewCameraGrad * 1)()):
-        rc = L.mgs_backward_views_intr(1, views, None, None, 0, None, cam, intr, 4, 0, 0, 0, 4096, None, 4096, None, None, 1.0, None,
-                                       4096, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
+        opts = _binding.RenderOptions(camera_grad=cam, intrinsics=intr)
+        rc = L.mgs_backward_views(1, views, opts, 4, 0, 0, 0, 4096, None, 4096, None, None, 1.0, None,
+                                  4096, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
         assert rc == -1 and "scratch" in _binding.last_error()
         clouds = (_binding.Cloud * 1)()
         c = clouds[0]
         c.P, c.means3D, c.colors_precomp, c.dL_dmean3D, c.dL_dopacity = 4, 4096, 4096, 4096, 4096
         offs = (ctypes.c_int * 2)(0, 1)
-        rc = L.mgs_backward_clouds_intr(1, clouds, offs, views, None, None, 0, None, cam, intr, 0, 0, 0, 1.0, 0, 0, None)
+        rc = L.mgs_backward_clouds(1, clouds, offs, views, opts, 0, 0, 0, 1.0, 0, 0, None)
         assert rc == -1 and "scratch" in _binding.last_error()
-    # the forward checks its arguments as the _ssim forward does, before reading intr
-    rc = L.mgs_forward_views_intr(0, views, None, None, 0, None, intr, 4, 0, 0, 0, 4096, None, 4096, None, 4096, None, 1.0, None,
-                                  None, 0, 0, None)
+    # the forward checks its other arguments before reading intr
+    rc = L.mgs_forward_views(0, views, _binding.RenderOptions(intrinsics=intr), 4, 0, 0, 0, 4096, None, 4096, None, 4096, None, 1.0,
+                             None, None, 0, 0, None)
     assert rc == -1
-    rc = L.mgs_forward_views_intr(1, views, None, None, 2, None, intr, 4, 0, 0, 0, 4096, None, 4096, None, 4096, None, 1.0, None,
-                                  None, 0, 0, None)
+    rc = L.mgs_forward_views(1, views, _binding.RenderOptions(intrinsics=intr, antialiasing=2), 4, 0, 0, 0, 4096, None, 4096, None,
+                             4096, None, 1.0, None, None, 0, 0, None)
     assert rc == -1 and "antialiasing" in _binding.last_error()
     # the camera-grad scratch keeps its size: the focal-length rows live in the geometry state
     assert L.mgs_camera_grad_scratch_bytes(16385) == 129 * 27 * 4

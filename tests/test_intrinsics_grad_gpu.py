@@ -133,7 +133,7 @@ def test_device_fov_through_the_renderers(kind, aa):
 
 
 @pytest.mark.parametrize("aa", [False, True])
-def test_same_records_give_the_same_outputs_with_and_without_the_device_fov(aa):
+def test_same_records_give_the_same_outputs_with_and_without_the_intrinsics_option(aa):
     """Stage 2 four times on one set of blend-stage records: {host, device} field of view x {without, with} dL_dtan_fov.
     Every per-Gaussian output and the 27 camera entries are bit-identical; dL_dtan_fov is bit-identical with the host or
     the device field of view."""
@@ -160,19 +160,20 @@ def test_same_records_give_the_same_outputs_with_and_without_the_device_fov(aa):
         def __getattr__(self, name):
             return getattr(real, name)
 
-        def mgs_backward_views_intr(self, *args):
+        def mgs_backward_views(self, *args):
             if args[-3] != 2:
-                return real.mgs_backward_views_intr(*args)
-            iarr = args[7]
+                return real.mgs_backward_views(*args)
+            iarr = args[2].intrinsics
             for dev_fov, want in ((False, False), (True, False), (True, True), (False, True)):
                 a = list(args)
                 ia = (B.ViewIntrinsics * V)()
                 for v in range(V):
                     ia[v].tan_fov = iarr[v].tan_fov if dev_fov else None
                     ia[v].dL_dtan_fov = iarr[v].dL_dtan_fov if want else None
-                a[7] = ia
+                a[2] = B.RenderOptions.from_buffer_copy(args[2])
+                a[2].intrinsics = ia
                 cam[3].fill_(float("nan"))
-                rc = real.mgs_backward_views_intr(*a)
+                rc = real.mgs_backward_views(*a)
                 if rc < 0:
                     return rc
                 torch.cuda.synchronize()

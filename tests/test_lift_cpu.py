@@ -50,7 +50,7 @@ def _call(V=1, views=None, lift="ok", aa=0, P=4, C=3, colors=4096, out_lifted=40
         lift = (_binding.ViewLift * max(V, 1))()
         for i in range(max(V, 1)):
             lift[i].map = 4096
-    return L.mgs_lift_views(V, views, lift, aa, None, P, 0, 0, C, 4096, None, colors, 4096, 4096, 1.0, 4096, None,
+    return L.mgs_lift_views(V, views, lift, aa, None, None, None, None, P, 0, 0, C, 4096, None, colors, 4096, 4096, 1.0, 4096, None,
                             out_lifted, out_weight, 0, None)
 
 
@@ -68,7 +68,7 @@ def _call(V=1, views=None, lift="ok", aa=0, P=4, C=3, colors=4096, out_lifted=40
     ("no_colors", -1, "colours"),
     ("aa", -1, "antialiasing"),
 ])
-def test_argument_errors_return_their_code_without_touching_a_gpu(case, code, msg):
+def test_lift_argument_errors_return_their_code_without_touching_a_gpu(case, code, msg):
     views = _views()
     kw = {}
     if case == "V0":
@@ -96,7 +96,7 @@ def test_argument_errors_return_their_code_without_touching_a_gpu(case, code, ms
     assert rc == code and msg in _binding.last_error(), (rc, _binding.last_error())
 
 
-def test_weights_only_needs_no_map_or_lifted_output():
+def test_lift_of_weights_only_needs_no_map_or_lifted_output():
     # C = 0 with no lift array and no lifted output passes every argument check; with V = 0 the call still fails on V,
     # so no work is enqueued
     rc = _call(V=0, lift=None, C=0, out_lifted=None)

@@ -3,7 +3,7 @@
 * tests/median_ref64.py, the vectorised float64 statement of the rule (last contributor whose incoming T > 0.5), agrees with a
   pixel-by-pixel walk on random small scenes with random contributor masks, picks the pixel's last contributor where T never
   falls to 0.5, -1 where there is no contributor, and its fp32 band always contains the exact choice.
-* The _median symbols are exported, and a median-depth output or cotangent without median_id returns MGS_ERR_INVALID_ARG
+* A median-depth output or cotangent without median_id returns MGS_ERR_INVALID_ARG
   before anything is enqueued (no device is touched: the pointers are never dereferenced).
 """
 import ctypes
@@ -74,11 +74,8 @@ def _view():
     return views
 
 
-def test_median_symbols_are_exported_and_check_their_arguments():
+def test_median_option_checks_its_arguments():
     L = _binding.lib()
-    for name in ("mgs_forward_views_median", "mgs_backward_views_median", "mgs_forward_clouds_median", "mgs_backward_clouds_median"):
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
-    assert L.mgs_abi_version() == 300
     views = _view()
     clouds = (_binding.Cloud * 1)()
     c = clouds[0]
@@ -88,20 +85,21 @@ def test_median_symbols_are_exported_and_check_their_arguments():
     for field in ("out_median_depth", "dL_dpix_median_depth"):
         med = (_binding.ViewMedian * 1)()
         setattr(med[0], field, 4096)  # without median_id
+        med = _binding.RenderOptions(median=med)
         if field == "out_median_depth":
-            rc = L.mgs_forward_views_median(1, views, None, None, 0, None, None, med, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096,
-                                            1.0, 4096, None, 0, 0, None)
+            rc = L.mgs_forward_views(1, views, med, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096,
+                                     1.0, 4096, None, 0, 0, None)
             assert rc == -1 and "median_id" in _binding.last_error()
-            rc = L.mgs_forward_clouds_median(1, clouds, offs, views, None, None, 0, None, None, med, 0, 0, 0, 1.0, 0, 0, None)
+            rc = L.mgs_forward_clouds(1, clouds, offs, views, med, 0, 0, 0, 1.0, 0, 0, None)
             assert rc == -1 and "median_id" in _binding.last_error()
         else:
-            rc = L.mgs_backward_views_median(1, views, None, None, 0, None, None, None, med, 4, 0, 0, 0, 4096, None, 4096, None, None,
-                                             1.0, None, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
+            rc = L.mgs_backward_views(1, views, med, 4, 0, 0, 0, 4096, None, 4096, None, None,
+                                      1.0, None, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
             assert rc == -1 and "median_id" in _binding.last_error()
-            rc = L.mgs_backward_clouds_median(1, clouds, offs, views, None, None, 0, None, None, None, med, 0, 0, 0, 1.0, 0, 0, None)
+            rc = L.mgs_backward_clouds(1, clouds, offs, views, med, 0, 0, 0, 1.0, 0, 0, None)
             assert rc == -1 and "median_id" in _binding.last_error()
     # the other argument checks still come first
-    med = (_binding.ViewMedian * 1)()
-    rc = L.mgs_forward_views_median(1, views, None, None, 2, None, None, med, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096, 1.0,
-                                    4096, None, 0, 0, None)
+    med = _binding.RenderOptions(median=(_binding.ViewMedian * 1)(), antialiasing=2)
+    rc = L.mgs_forward_views(1, views, med, 4, 0, 0, 0, 4096, None, 4096, None, 4096, 4096, 1.0,
+                             4096, None, 0, 0, None)
     assert rc == -1 and "antialiasing" in _binding.last_error()

@@ -138,7 +138,8 @@ def test_state_queries_grow_only_with_normals():
 
 
 def _views_call(L, forward, normal, cov3D=False, cam_pos=True, depth_mask=None):
-    """mgs_{forward,backward}_views_normal with fake non-NULL pointers: every refusal happens before anything is enqueued"""
+    """mgs_forward_views / mgs_backward_views with a normal plane and fake non-NULL pointers: every refusal happens before
+    anything is enqueued"""
     p = ctypes.c_void_p(4096)
     w = (_binding.View * 1)()
     v = w[0]
@@ -148,14 +149,15 @@ def _views_call(L, forward, normal, cov3D=False, cam_pos=True, depth_mask=None):
     v.width = v.height = 16
     v.tan_fovx = v.tan_fovy = 0.5
     geo = (p, p, None, None, p, None if cov3D else p, 1.0, None if cov3D else p, p if cov3D else None)
+    opts = _binding.RenderOptions(depth_mask=depth_mask, normal=normal)
     if forward:
-        return L.mgs_forward_views_normal(1, w, None, depth_mask, 0, None, None, None, normal, 10, 1, 4, 0, *geo, 0, 0, None)
+        return L.mgs_forward_views(1, w, opts, 10, 1, 4, 0, *geo, 0, 0, None)
     geo = (p, p, None, None, None if cov3D else p, 1.0, None if cov3D else p, p if cov3D else None)
-    return L.mgs_backward_views_normal(1, w, None, depth_mask, 0, None, None, None, None, normal, 10, 1, 4, 0, *geo,
-                                       p, p, None, None, None, p, p, p, 1, 0, 3, 0, None)
+    return L.mgs_backward_views(1, w, opts, 10, 1, 4, 0, *geo,
+                                p, p, None, None, None, p, p, p, 1, 0, 3, 0, None)
 
 
-def test_argument_errors_before_anything_is_enqueued():
+def test_normal_option_errors_before_anything_is_enqueued():
     L = _binding.lib()
     n = (_binding.ViewNormal * 1)()
     n[0].out_normal = 4096

@@ -6,7 +6,7 @@
 * A pinhole camera pulled back to distance D with tan_fov = h / D converges to the orthographic conic as D grows.
 * The builders' matrices give d px / d t.x = fx and d py / d t.y = fy, the Jacobian's entries, and top_down_camera maps
   the workspace box onto the image.
-* The _ortho symbols are exported; a flag other than 0 or 1 returns MGS_ERR_INVALID_ARG before anything is enqueued.
+* An ortho flag other than 0 or 1 returns MGS_ERR_INVALID_ARG before anything is enqueued.
 * GaussianRasterizationSettings.orthographic: default, _replace and repr; CameraBatch.as_novel_view refuses orthographic
   cameras.
 """
@@ -292,12 +292,8 @@ def test_as_novel_view_refuses_orthographic_cameras():
         cb.as_novel_view()
 
 
-def test_ortho_symbols_are_exported_and_check_their_flags():
+def test_ortho_option_checks_its_flags():
     L = _binding.lib()
-    names = ("mgs_forward_views_ortho", "mgs_backward_views_ortho", "mgs_forward_clouds_ortho", "mgs_backward_clouds_ortho",
-             "mgs_lift_views_ortho")
-    for name in names:
-        assert hasattr(L, name) and name in _binding.EXPORTED_SYMBOLS
     views = (_binding.View * 2)()
     for v in views:
         v.width, v.height, v.tan_fovx, v.tan_fovy = 8, 8, 0.5, 0.5
@@ -307,13 +303,13 @@ def test_ortho_symbols_are_exported_and_check_their_flags():
         v.binning_capacity = 1
     bad = (ctypes.c_int * 2)(0, 2)
     # pointers are never dereferenced: the flags are checked before anything is enqueued
-    rc = L.mgs_forward_views_ortho(2, views, None, None, 0, None, None, None, None, bad, 4, 0, 0, 0, 4096, None, 4096, None, 4096,
-                                   4096, 1.0, 4096, None, 0, 0, None)
+    rc = L.mgs_forward_views(2, views, _binding.RenderOptions(ortho=bad), 4, 0, 0, 0, 4096, None, 4096, None, 4096,
+                             4096, 1.0, 4096, None, 0, 0, None)
     assert rc == -1 and "ortho" in _binding.last_error()
-    rc = L.mgs_backward_views_ortho(2, views, None, None, 0, None, None, None, None, None, bad, 4, 0, 0, 0, 4096, None, 4096, None,
-                                    4096, 1.0, 4096, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
+    rc = L.mgs_backward_views(2, views, _binding.RenderOptions(ortho=bad), 4, 0, 0, 0, 4096, None, 4096, None,
+                              4096, 1.0, 4096, None, 4096, 4096, None, None, None, None, None, None, 0, 0, 3, 0, None)
     assert rc == -1 and "ortho" in _binding.last_error()
-    rc = L.mgs_lift_views_ortho(2, views, None, 0, None, bad, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None, None,
+    rc = L.mgs_lift_views(2, views, None, 0, None, bad, None, None, 4, 0, 0, 0, 4096, None, 4096, 4096, 4096, 1.0, 4096, None, None,
                                 4096, 0, None)
     assert rc == -1 and "ortho" in _binding.last_error()
     clouds = (_binding.Cloud * 1)()
@@ -322,8 +318,7 @@ def test_ortho_symbols_are_exported_and_check_their_flags():
     c.dL_dmean3D, c.dL_dopacity = 4096, 4096
     offs = (ctypes.c_int * 2)(0, 2)
     neg = (ctypes.c_int * 2)(-1, 0)
-    rc = L.mgs_forward_clouds_ortho(1, clouds, offs, views, None, None, 0, None, None, None, None, neg, 0, 0, 0, 1.0, 0, 0, None)
+    rc = L.mgs_forward_clouds(1, clouds, offs, views, _binding.RenderOptions(ortho=neg), 0, 0, 0, 1.0, 0, 0, None)
     assert rc == -1 and "ortho" in _binding.last_error()
-    rc = L.mgs_backward_clouds_ortho(1, clouds, offs, views, None, None, 0, None, None, None, None, None, neg, 0, 0, 0, 1.0, 0, 0,
-                                     None)
+    rc = L.mgs_backward_clouds(1, clouds, offs, views, _binding.RenderOptions(ortho=neg), 0, 0, 0, 1.0, 0, 0, None)
     assert rc == -1 and "ortho" in _binding.last_error()

@@ -10,8 +10,7 @@
 * Images: the blend of the orthographic records against blend_ref64.
 * Mixed batches: each view's image, radii and instance count are bit-identical to the view rendered alone, and the
   gradients are the sum over the views within float-atomic order.
-* All flags zero through the _ortho calls: bit-identical images, radii, sort keys and counts to the calls without the
-  argument, gradients within 1e-5 relative L2 (the float atomics' order).  The renders compared bit for bit take explicit
+* An all-zero ortho array: bit-identical images, radii, sort keys and counts to a NULL one, gradients within 1e-5 relative L2 (the float atomics' order).  The renders compared bit for bit take explicit
   binning capacities and are checked not to overflow.
 * Public paths: render_views / render_clouds / lift_views / GaussianRasterizer with every option, a CUDA-graph replay, and
   no device memory growth over steps.
@@ -412,7 +411,7 @@ def test_all_zero_flags_match_the_calls_without_them(monkeypatch):
         return (ctypes.c_int * len(vs))(*([0] * len(vs)))
     monkeypatch.setattr(R, "_ortho_flags", zeros)
     o1, g1, _, _ = _render_raw(views, g)
-    assert calls   # the _ortho symbols ran
+    assert calls   # the all-zero flag arrays reached the calls
     for a, b in zip(o0, o1):
         assert torch.equal(a[1], b[1]) and torch.equal(a[3], b[3]) and torch.equal(a[7], b[7])
         assert a.num_rendered() == b.num_rendered()

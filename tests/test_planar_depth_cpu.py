@@ -1,5 +1,5 @@
 """Planar depth without a GPU: the float64 reference (tests/planar_ref64.py) against finite differences and geometry, and the
-C ABI's argument checks (include/mgs_rasterizer.h, mgs_forward_views_planar)."""
+C ABI's argument checks (include/mgs_rasterizer.h, mgs_render_options.planar_depth)."""
 import ctypes as C
 
 import numpy as np
@@ -93,21 +93,17 @@ def test_thin_tilted_gaussian_follows_its_plane():
     assert errs[2.0] < errs[4.0] / 3  # second order: halving the offset quarters the error (up to the dilation's share)
 
 
-def test_abi_exports_and_argument_checks():
+def test_planar_depth_option_argument_checks():
     from manigaussian_b200 import _binding as B
     from manigaussian_b200 import rasterizer as R
-    for n in ("mgs_forward_views_planar", "mgs_backward_views_planar", "mgs_forward_clouds_planar", "mgs_backward_clouds_planar"):
-        assert n in B.EXPORTED_SYMBOLS
     L = B.lib()
-    assert len(L.mgs_forward_views_planar.argtypes) == len(L.mgs_forward_views_distorted.argtypes) + 1
-    assert len(L.mgs_backward_clouds_planar.argtypes) == len(L.mgs_backward_clouds_distorted.argtypes) + 1
     views = (B.View * 1)()
     normal = (B.ViewNormal * 1)()
     buf = (C.c_float * 4)()
     normal[0].out_normal = C.addressof(buf)
     rest = (1, 0, 0, 0) + (None,) * 4 + (None, None, 1.0, None, None, 0, 0, None)
     for flag, nrm in ((2, None), (1, normal)):
-        rc = L.mgs_forward_views_planar(1, views, None, None, 0, None, None, None, nrm, None, None, None, flag, *rest)
+        rc = L.mgs_forward_views(1, views, B.RenderOptions(normal=nrm, planar_depth=flag), *rest)
         assert rc == B.MGS_ERR_INVALID_ARG if hasattr(B, "MGS_ERR_INVALID_ARG") else rc != 0
         assert b"planar_depth" in L.mgs_last_error()
     s = R.GaussianRasterizationSettings(4, 4, 0.5, 0.5, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0, torch.zeros(3), False,

@@ -1,4 +1,4 @@
-"""Planar depth on the GPU (include/mgs_rasterizer.h, mgs_forward_views_planar).
+"""Planar depth on the GPU (include/mgs_rasterizer.h, mgs_render_options.planar_depth).
 
 * Per-Gaussian quad: {a, b, e} read back from the geometry state equals the float64 reference (tests/planar_ref64.py) for
   pinhole, orthographic, fisheye and distorted views.

@@ -419,7 +419,7 @@ P64_QNORMS = QNORMS
 
 @pytest.mark.parametrize("scene", ["aa1", "aa2", "aa3"])
 def test_antialiased_view_per_gaussian(scene):
-    """The anti-aliased projection (one view through mgs_forward_views_aa / mgs_backward_views_aa, depth cotangents on):
+    """The anti-aliased projection (one view through mgs_forward_views / mgs_backward_views with antialiasing = 1, depth cotangents on):
     every record, o_eff included, against project_ref64.forward(antialias=True), and every per-Gaussian output against the
     AA chain fed blend_ref64's cotangents, on needles both sides of the 2.5e-5 clamp."""
     import test_project_ref64_cpu as CPU
@@ -741,7 +741,7 @@ VIEWS_NULLABLE = ("dL_dcolor", "dL_dcov3D", "dL_dsh", "dL_dscale", "dL_drot")
 
 
 @pytest.mark.parametrize("scene", ["near", "precomp_cov", "sh2"])
-def test_mgs_backward_views_writes_every_output_it_is_given(scene):
+def test_backward_views_call_writes_every_output_it_is_given(scene):
     """mgs_backward_views over two views (shared dL_dmean2D), each nullable output NULL in turn and every other output
     prefilled with NaN: every output given is fully written and equals the all-outputs call up to the reordering of the
     blend's atomic sums.  dL_dmean3D keeps its SH view-direction term without dL_dsh, dL_dscale / dL_drot are written on
@@ -774,7 +774,7 @@ def test_mgs_backward_views_writes_every_output_it_is_given(scene):
             keep.append(R._backward_view(L, arr[v], s, outs[v], torch.device("cuda"), P, gc[v], None, None))
             arr[v].dL_dmean2D = ptr(out["dL_dmean2D"])
             arr[v].stream = streams[v].cuda_stream
-        rc = L.mgs_backward_views(len(views), arr, P, deg, M, 0, ptr(a["means3D"]), ptr(a["sh"]) if M else None,
+        rc = L.mgs_backward_views(len(views), arr, None, P, deg, M, 0, ptr(a["means3D"]), ptr(a["sh"]) if M else None,
                                   ptr(a["colors"]) if g["colors_precomp"] is not None else None, None,
                                   ptr(a["scales"]) if g["scales"] is not None else None, float(mod),
                                   ptr(a["rotations"]) if g["rotations"] is not None else None,

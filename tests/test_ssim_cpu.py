@@ -13,8 +13,7 @@ import util
 from manigaussian_b200 import _binding
 import ssim_oracle as O
 
-CALLS = ("mgs_forward_views_ssim", "mgs_backward_views_ssim", "mgs_forward_clouds_ssim", "mgs_backward_clouds_ssim",
-         "mgs_ssim", "mgs_ssim_backward")
+CALLS = ("mgs_ssim", "mgs_ssim_backward")
 FIELDS = ("ssim_terms", "loss_acc", "cot_scale", "cot_color")
 
 
@@ -92,7 +91,7 @@ def test_oracle_terms_and_batches():
     assert np.array_equal(O.ssim_map(x2, g2)[0][1], O.ssim_map(x[::-1], g[::-1])[0])
 
 
-def test_header_declares_and_library_exports_the_ssim_calls():
+def test_header_declares_the_ssim_struct_option_and_calls():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     code = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     m = re.search(r"typedef struct mgs_view_ssim \{(.*?)\} mgs_view_ssim;", code, flags=re.S)
@@ -102,7 +101,7 @@ def test_header_declares_and_library_exports_the_ssim_calls():
     for name in CALLS:
         assert re.search(r"\b%s\s*\(" % name, code), name
         assert name in _binding.EXPORTED_SYMBOLS and hasattr(L, name), name
-    assert L.mgs_abi_version() == 300
+    assert re.search(r"typedef struct mgs_render_options \{[^}]*const mgs_view_ssim\* ssim;", code)
     names = [L.mgs_profile_stage_name(i).decode() for i in range(L.mgs_profile_num_stages())]
     assert names[-2:] == ["ssim_fwd", "ssim_bwd"] and names[:3] == ["project_fwd", "depth_sort", "scan"]
 
@@ -125,7 +124,7 @@ def _view(**kw):
 
 
 @pytest.mark.parametrize("case", ["no_target_color", "no_terms", "no_loss_acc", "no_cot_color", "no_out_color"])
-def test_ssim_calls_check_their_arguments_without_a_gpu(case):
+def test_ssim_option_checks_its_arguments_without_a_gpu(case):
     L = _binding.lib()
     views = (_binding.View * 1)(_view(**{"no_target_color": dict(target_color=None),
                                          "no_out_color": dict(out_color=None)}.get(case, {})))
@@ -141,16 +140,17 @@ def test_ssim_calls_check_their_arguments_without_a_gpu(case):
     clouds = (_binding.Cloud * 1)()
     clouds[0].P, clouds[0].means3D, clouds[0].opacities, clouds[0].shs, clouds[0].scales, clouds[0].rotations = 10, 16, 16, 16, 16, 16
     clouds[0].dL_dmean3D, clouds[0].dL_dopacity, clouds[0].dL_dsh = 16, 16, 16
+    ss = _binding.RenderOptions(ssim=ss)
     if case != "no_out_color":  # out_color is required of every forward view anyway
-        rc = L.mgs_forward_views_ssim(1, views, None, None, 0, ss, 10, 1, 4, 0, 16, 16, None, None, 16, 16, 1.0, 16, None, 0, 0, None)
+        rc = L.mgs_forward_views(1, views, ss, 10, 1, 4, 0, 16, 16, None, None, 16, 16, 1.0, 16, None, 0, 0, None)
         assert rc == -1  # MGS_ERR_INVALID_ARG
         assert "SSIM" in _binding.last_error()
-        rc = L.mgs_forward_clouds_ssim(1, clouds, offs, views, None, None, 0, ss, 1, 4, 0, 1.0, 0, 0, None)
+        rc = L.mgs_forward_clouds(1, clouds, offs, views, ss, 1, 4, 0, 1.0, 0, 0, None)
         assert rc == -1 and "SSIM" in _binding.last_error()
-    rc = L.mgs_backward_views_ssim(1, views, None, None, 0, ss, 10, 1, 4, 0, 16, 16, None, None, 16, 1.0, 16, None,
-                                   16, 16, None, None, None, 16, 16, 16, 1, 0, 3, 0, None)
+    rc = L.mgs_backward_views(1, views, ss, 10, 1, 4, 0, 16, 16, None, None, 16, 1.0, 16, None,
+                              16, 16, None, None, None, 16, 16, 16, 1, 0, 3, 0, None)
     assert rc == -1 and "SSIM" in _binding.last_error()
-    rc = L.mgs_backward_clouds_ssim(1, clouds, offs, views, None, None, 0, ss, 1, 4, 0, 1.0, 0, 0, None)
+    rc = L.mgs_backward_clouds(1, clouds, offs, views, ss, 1, 4, 0, 1.0, 0, 0, None)
     assert rc == -1 and "SSIM" in _binding.last_error()
 
 

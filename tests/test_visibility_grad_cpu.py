@@ -76,7 +76,7 @@ def test_reference_T_is_the_product_over_the_accepted_candidates():
     assert torch.allclose(d, VG.F64.view_space(t(pts), view)[:, 2])
 
 
-def test_symbols_are_declared_and_exported():
+def test_visibility_backward_symbols_are_declared_and_exported():
     hdr = open(os.path.join(util.ROOT, "include", "mgs_rasterizer.h")).read()
     L = _binding.lib()
     for sym in ("mgs_visibility_views_backward", "mgs_visibility_backward_scratch_bytes"):
@@ -84,7 +84,6 @@ def test_symbols_are_declared_and_exported():
     # gb, the uv cotangents and the camera rows of both paths grow with P and Q
     a, b, c = (L.mgs_visibility_backward_scratch_bytes(P, Q) for P, Q in ((1000, 1000), (2000, 1000), (1000, 2000)))
     assert b - a >= 1000 * 12 * 4 and c - a >= 1000 * 2 * 4
-    assert L.mgs_abi_version() == 300
 
 
 def _bcall(V=1, views=None, P=4, Q=3, out_T=4096, dT=4096, dcov=None, cov=None):

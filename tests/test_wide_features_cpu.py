@@ -21,7 +21,7 @@ def test_feature_width_limit_is_512_and_documented_in_python():
     assert "0..512" in rasterizer.__doc__
 
 
-def test_too_wide_features_are_refused_without_touching_a_gpu():
+def test_too_wide_features_are_refused_by_every_call_without_touching_a_gpu():
     L = _binding.lib()
     F = _max_channels() + 1
     fake = ctypes.c_void_p(4096)  # a non-NULL device address: the width check comes first, nothing reads it
@@ -42,8 +42,8 @@ def test_too_wide_features_are_refused_without_touching_a_gpu():
                         fake, 0, 0, None)                    # scratch accumulate debug stream
     assert rc == MGS_ERR_UNSUPPORTED, _binding.last_error()
     views = (_binding.View * 1)()
-    rc = L.mgs_forward_views(1, views, 10, 1, 4, F, fake, fake, None, fake, fake, fake, 1.0, fake, None, 0, 0, None)
+    rc = L.mgs_forward_views(1, views, None, 10, 1, 4, F, fake, fake, None, fake, fake, fake, 1.0, fake, None, 0, 0, None)
     assert rc == MGS_ERR_UNSUPPORTED, _binding.last_error()
-    rc = L.mgs_backward_views(1, views, 10, 1, 4, F, fake, fake, None, fake, fake, 1.0, fake, None,
+    rc = L.mgs_backward_views(1, views, None, 10, 1, 4, F, fake, fake, None, fake, fake, 1.0, fake, None,
                               fake, fake, None, fake, None, fake, fake, fake, 1, 0, 3, 0, None)
     assert rc == MGS_ERR_UNSUPPORTED, _binding.last_error()
