@@ -1081,6 +1081,68 @@ size_t mgs_fps_state_bytes(int B, int P);
 int mgs_fps(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
 	long long* out_index, float* out_dist2, int debug, void* stream);
 
+/*
+ * TSDF fusion (no reference counterpart; KinectFusion's and Open3D's rule with unit weights, no bitwise parity with Open3D
+ * claimed): V depth images fused into a truncated signed-distance volume over the [X,Y,Z] grid of bounds (host double[6],
+ * x0 y0 z0 x1 y1 z1).  Voxel (i, j, k) sits at voxel_centres' point: per axis lo + (i + 1/2) ((hi - lo) / n) evaluated in
+ * double (no FMA), rounded once to float.  For each voxel centre x, over the views v = 0 .. V-1 in order:
+ *   1. (px, py) and z = t.z from the projection's map of a mean (screen_mean, as in point visibility), with its cull
+ *      (NEAR_Z, a fisheye's theta_max, a distorted lens's r_max and fold); a culled view is skipped;
+ *   2. the pixel is (i, j) = (floor(px + 0.5), floor(py + 0.5)), pixel centres at integers; a view is skipped unless
+ *      (px, py) lies in [-0.5, W - 0.5) x [-0.5, H - 0.5) (point visibility's bounds; i and j are clamped to W - 1, H - 1);
+ *   3. d = depth[v, j, i]; a view is skipped where d is not finite or d <= 0 (no return);
+ *   4. s = d - z; a view is skipped where s < -trunc (the voxel is occluded);
+ *   5. f = min(1, s / trunc), tsdf <- (tsdf w + f) / (w + 1), for each channel c <- (c w + color[v, :, j, i]) / (w + 1),
+ *      then w <- w + 1, every operation rounded to float32 in this order (no FMA).
+ * Arguments: views, intr, ortho, fisheye and distortion as mgs_camera_rays takes them (of each view viewmatrix, projmatrix,
+ * tan_fovx, tan_fovy, width and height are read; every view has the same width W and height H).  depth [V,H,W] view-space z;
+ * color [V,C,H,W] or NULL with C = 0, C in 0 .. 32; trunc > 0 in world units.  tsdf [X,Y,Z], weight [X,Y,Z] and
+ * color_volume [C,X,Y,Z] (NULL with C = 0) are read and updated in place: a fresh volume holds tsdf 1, weight 0, colour 0.
+ *   - The result is bitwise repeatable, one call over V views is bitwise equal to successive calls over any split of the
+ *     same views in order, and a voxel no view updates is left bitwise unchanged (it is not written).
+ *   - Views run in launches of up to 64, each reading and writing the volume once.
+ * Nothing allocates, blocks or reads back to the host: a call can be captured in a CUDA graph.  Not differentiable.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V <= 0 or views
+ * NULL, the camera-model errors of the distortion section, a view without its matrices or with a size <= 0, views of
+ * different sizes, X, Y or Z <= 0, trunc <= 0 or not finite, C outside 0 .. 32, bounds NULL, not finite or not increasing,
+ * and a NULL depth, tsdf or weight, or color or color_volume with C > 0.
+ */
+int mgs_tsdf_fuse(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho,
+	const mgs_view_fisheye* fisheye, const mgs_view_distortion* distortion, const float* depth, int C, const float* color,
+	const double* bounds, int X, int Y, int Z, float trunc, float* tsdf, float* weight, float* color_volume, int debug,
+	void* stream);
+
+/*
+ * Marching cubes (no reference counterpart): the level surface of values [X,Y,Z] (a TSDF at level 0, or a density) as an
+ * indexed triangle mesh.  Grid point (i, j, k) sits at its voxel centre over bounds, as in mgs_tsdf_fuse.
+ *   - A grid point is valid when its value is finite and, with weight [X,Y,Z] (NULL for none), its weight is > 0.  The
+ *     cells are the (X-1)(Y-1)(Z-1) cubes of 8 neighbouring points; a cell with an invalid corner emits nothing.  Corner c
+ *     of the cell with lower corner (i, j, k) is the point (i + (c & 1), j + ((c >> 1) & 1), k + ((c >> 2) & 1)), below when
+ *     value < level; the case index has bit c set for a below corner (csrc/mc_table.cuh holds the table and its numbering).
+ *   - Each crossed cell edge (exactly one endpoint below) that an emitted triangle uses gets exactly one vertex, shared by
+ *     every cell around the edge: no vertex is duplicated or unused.  With a the edge's lower endpoint (first in x-major
+ *     order) and b the other, t = (level - v_a) / (v_b - v_a) and p = c_a + t (c_b - c_a) per coordinate, each operation
+ *     rounded to float32 (no FMA); colours (color [C,X,Y,Z], C in 0 .. 32) are interpolated with the same t.  Vertices are
+ *     ordered by (a in x-major order, then the edge's axis x < y < z).
+ *   - Faces follow the table's triangles, cells in x-major order.  Each normal (v1 - v0) x (v2 - v0) points toward
+ *     increasing value.  An ambiguous face always cuts off its below corners, from both cells that share it, so a level
+ *     set inside the valid region gives a closed mesh.  Zero-area triangles (a value exactly at the level) are kept.
+ *   - The mesh is bitwise repeatable (no atomics).
+ * Two calls: mgs_marching_cubes_count fills the state (mgs_marching_cubes_state_bytes(X, Y, Z) bytes of device memory,
+ * contents irrelevant on entry: 18 bytes per grid point and CUB's scan space) and writes out_counts (device, 2 long long)
+ * = {vertex count Nv, face count Nf}; the caller reads them back and sizes out_vertices [Nv,3], out_faces [Nf,3] (long long)
+ * and out_colors [Nv,C] (NULL with C = 0) for mgs_marching_cubes_emit, which takes the same state, values and level.
+ * A grid with a side below 2 has no cell: both calls return 0 and enqueue nothing (out_counts is not written).
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: X, Y or Z < 0,
+ * C outside 0 .. 32, bounds NULL, not finite or not increasing (emit), and a NULL state, values, out_counts, out_vertices or
+ * out_faces, or color or out_colors with C > 0.
+ */
+size_t mgs_marching_cubes_state_bytes(int X, int Y, int Z);
+int mgs_marching_cubes_count(void* state, int X, int Y, int Z, const float* values, const float* weight, float level,
+	long long* out_counts, int debug, void* stream);
+int mgs_marching_cubes_emit(void* state, int X, int Y, int Z, const float* values, float level, const double* bounds, int C,
+	const float* color, float* out_vertices, long long* out_faces, float* out_colors, int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -231,6 +231,18 @@ def lib():
     L.mgs_fps.restype = C.c_int
     L.mgs_fps.argtypes = [vp, i, i, i, vp, vp, vp,  # state B P n points lengths start
                           vp, vp, i, vp]            # out_index out_dist2 debug stream
+    L.mgs_tsdf_fuse.restype = C.c_int
+    L.mgs_tsdf_fuse.argtypes = [i, C.POINTER(View), C.POINTER(ViewIntrinsics),  # V views intr
+                                C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
+                                vp, i, vp, C.POINTER(C.c_double),  # depth C color bounds
+                                i, i, i, f, vp, vp, vp, i, vp]     # X Y Z trunc tsdf weight color_volume debug stream
+    L.mgs_marching_cubes_state_bytes.restype = C.c_size_t
+    L.mgs_marching_cubes_state_bytes.argtypes = [i, i, i]
+    L.mgs_marching_cubes_count.restype = C.c_int
+    L.mgs_marching_cubes_count.argtypes = [vp, i, i, i, vp, vp, f, vp, i, vp]  # state X Y Z values weight level out_counts debug stream
+    L.mgs_marching_cubes_emit.restype = C.c_int
+    L.mgs_marching_cubes_emit.argtypes = [vp, i, i, i, vp, f, C.POINTER(C.c_double), i, vp,  # state X Y Z values level bounds C color
+                                          vp, vp, vp, i, vp]  # out_vertices out_faces out_colors debug stream
     L.mgs_field_query.restype = C.c_int
     L.mgs_field_query.argtypes = [ALLOC_FN, vp, ALLOC_FN, vp, i, i, i,    # state and pair allocators, Q P C
                                   vp, vp, vp, vp, vp, vp, i,            # points means3D scales rotations opacities features channel_first
@@ -285,6 +297,7 @@ EXPORTED_SYMBOLS = (
     "mgs_neighbour_reg_state_bytes", "mgs_neighbour_reg", "mgs_neighbour_reg_backward",
     "mgs_deform_state_bytes", "mgs_deform", "mgs_deform_backward",
     "mgs_fps_state_bytes", "mgs_fps",
+    "mgs_tsdf_fuse", "mgs_marching_cubes_state_bytes", "mgs_marching_cubes_count", "mgs_marching_cubes_emit",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

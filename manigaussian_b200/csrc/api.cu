@@ -2239,3 +2239,99 @@ int mgs_fps(void* state, int B, int P, int n, const float* points, const long lo
 	MGS_STAGE("fps");
 	return 0;
 }
+
+// the grid of bounds (host double[6], x0 y0 z0 x1 y1 z1) with n points per axis: lower corner and voxel size per axis
+static int grid_of(const char* where, const double* bounds, const int n[3], double lo[3], double step[3])
+{
+	using namespace mgs;
+	const std::string w(where);
+	if (!bounds) return fail(MGS_ERR_INVALID_ARG, w + ": bounds are required");
+	for (int k = 0; k < 3; k++) {
+		if (!(std::isfinite(bounds[k]) && std::isfinite(bounds[k + 3]) && bounds[k + 3] > bounds[k]))
+			return fail(MGS_ERR_INVALID_ARG, w + ": bounds must be finite and increasing (x1 > x0, y1 > y0, z1 > z0)");
+		lo[k] = bounds[k];
+		step[k] = (bounds[k + 3] - bounds[k]) / n[k];
+	}
+	return 0;
+}
+
+int mgs_tsdf_fuse(int V, const mgs_view* views, const mgs_view_intrinsics* intr, const int* ortho, const mgs_view_fisheye* fisheye,
+	const mgs_view_distortion* distortion, const float* depth, int C, const float* color, const double* bounds, int X, int Y, int Z,
+	float trunc, float* tsdf, float* weight, float* color_volume, int debug, void* stream)
+{
+	using namespace mgs;
+	std::vector<Lens> lens;
+	if (check_rays(V, views, ortho, fisheye, distortion, 0, nullptr, lens) < 0) return MGS_ERR_INVALID_ARG;
+	for (int v = 1; v < V; v++)
+		if (views[v].width != views[0].width || views[v].height != views[0].height)
+			return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: every view must have the same width and height");
+	if (X <= 0 || Y <= 0 || Z <= 0) return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: X, Y and Z must be > 0");
+	if (!(trunc > 0.f) || !std::isfinite(trunc)) return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: trunc must be finite and > 0");
+	if (C < 0 || C > TSDF_MAX_CHANNELS) return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: C must be in [0, 32]");
+	const int n[3] = { X, Y, Z };
+	double lo[3], step[3];
+	if (grid_of("mgs_tsdf_fuse", bounds, n, lo, step) < 0) return MGS_ERR_INVALID_ARG;
+	if (!depth || !tsdf || !weight) return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: depth, tsdf and weight are required");
+	if (C > 0 && (!color || !color_volume))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_tsdf_fuse: color and color_volume are required with C > 0");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const size_t plane = (size_t)views[0].width * views[0].height;
+	for (int v0 = 0; v0 < V; v0 += TSDF_CHUNK) {
+		TsdfArgs a{};
+		a.V = std::min(V - v0, TSDF_CHUNK);
+		a.C = C; a.W = views[0].width; a.H = views[0].height;
+		a.X = X; a.Y = Y; a.Z = Z;
+		for (int k = 0; k < 3; k++) { a.lo[k] = lo[k]; a.step[k] = step[k]; }
+		a.trunc = trunc;
+		a.depth = depth + (size_t)v0 * plane;
+		a.color = C > 0 ? color + (size_t)v0 * C * plane : nullptr;
+		a.tsdf = tsdf; a.weight = weight; a.color_volume = C > 0 ? color_volume : nullptr;
+		for (int u = 0; u < a.V; u++) {
+			const mgs_view& w = views[v0 + u];
+			a.cam[u] = flow_cam(w, device_fov(intr, v0 + u), lens[v0 + u], w.viewmatrix, w.projmatrix);
+		}
+		launch_tsdf_fuse(a, st);
+		MGS_STAGE("tsdf_fuse");
+	}
+	return 0;
+}
+
+size_t mgs_marching_cubes_state_bytes(int X, int Y, int Z)
+{
+	return mgs::mc_state_bytes(std::max(X, 0), std::max(Y, 0), std::max(Z, 0));
+}
+
+int mgs_marching_cubes_count(void* state, int X, int Y, int Z, const float* values, const float* weight, float level,
+	long long* out_counts, int debug, void* stream)
+{
+	using namespace mgs;
+	if (X < 0 || Y < 0 || Z < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_count: X, Y and Z must be >= 0");
+	if (X < 2 || Y < 2 || Z < 2) return 0;  // no cell: an empty mesh
+	if (!state || !values || !out_counts)
+		return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_count: state, values and out_counts are required");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(mc_count(state, X, Y, Z, values, weight, level, out_counts, st));
+	MGS_STAGE("marching_cubes_count");
+	return 0;
+}
+
+int mgs_marching_cubes_emit(void* state, int X, int Y, int Z, const float* values, float level, const double* bounds, int C,
+	const float* color, float* out_vertices, long long* out_faces, float* out_colors, int debug, void* stream)
+{
+	using namespace mgs;
+	if (X < 0 || Y < 0 || Z < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_emit: X, Y and Z must be >= 0");
+	if (C < 0 || C > TSDF_MAX_CHANNELS) return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_emit: C must be in [0, 32]");
+	if (X < 2 || Y < 2 || Z < 2) return 0;
+	const int n[3] = { X, Y, Z };
+	double lo[3], step[3];
+	if (grid_of("mgs_marching_cubes_emit", bounds, n, lo, step) < 0) return MGS_ERR_INVALID_ARG;
+	if (!state || !values || !out_vertices || !out_faces)
+		return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_emit: state, values, out_vertices and out_faces are required");
+	if (C > 0 && (!color || !out_colors))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_marching_cubes_emit: color and out_colors are required with C > 0");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(mc_emit(state, X, Y, Z, values, level, lo, step, C, C > 0 ? color : nullptr, out_vertices, out_faces,
+	                 C > 0 ? out_colors : nullptr, st));
+	MGS_STAGE("marching_cubes_emit");
+	return 0;
+}

@@ -641,4 +641,33 @@ size_t fps_state_bytes(int B, int P);
 cudaError_t fps_run(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
 	long long* out_index, float* out_dist2, cudaStream_t st);
 
+// tsdf.cu: depth images fused into an [X,Y,Z] volume (include/mgs_rasterizer.h, mgs_tsdf_fuse), one thread per voxel over
+// the up to TSDF_CHUNK views of one launch, in order.  Every pointer is that of the launch's first view; view u's depth
+// starts at u H W and its colour at u C H W.  The kernel parameters exceed 4 KB (CUDA 12.1+ accepts up to 32,764 bytes).
+constexpr int TSDF_CHUNK = 64;
+constexpr int TSDF_MAX_CHANNELS = 32;
+struct TsdfArgs {
+	int V, C, W, H;              // views of the launch, colour channels, image size shared by every view
+	int X, Y, Z;
+	double lo[3], step[3];       // voxel (i, j, k) sits at lo + (idx + 1/2) step per axis, in double, rounded to float
+	float trunc;
+	const float* depth;          // [V,H,W]
+	const float* color;          // [V,C,H,W] or NULL (C = 0)
+	float* tsdf;                 // [X,Y,Z]
+	float* weight;               // [X,Y,Z]
+	float* color_volume;         // [C,X,Y,Z] or NULL (C = 0)
+	FlowCam cam[TSDF_CHUNK];
+};
+static_assert(sizeof(TsdfArgs) <= 32764, "large kernel parameters are limited to 32,764 bytes");
+void launch_tsdf_fuse(const TsdfArgs& a, cudaStream_t s);
+
+// marching_cubes.cu: the level surface of an [X,Y,Z] grid (include/mgs_rasterizer.h, mgs_marching_cubes_count / _emit).
+// The state holds per grid point its cell's case byte and its 3 edge-used bits, and the inclusive scans of the vertex and
+// triangle counts; mc_count fills it and writes the two totals, mc_emit reads it.
+size_t mc_state_bytes(int X, int Y, int Z);
+cudaError_t mc_count(void* state, int X, int Y, int Z, const float* values, const float* weight, float level, long long* out_counts,
+	cudaStream_t st);
+cudaError_t mc_emit(void* state, int X, int Y, int Z, const float* values, float level, const double lo[3], const double step[3],
+	int C, const float* color, float* out_vertices, long long* out_faces, float* out_colors, cudaStream_t st);
+
 }  // namespace mgs

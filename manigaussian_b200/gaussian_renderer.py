@@ -1149,13 +1149,13 @@ def query_field(points, pts_xyz, rotations, scales, opacity, features=None):
     return {"density": density, "features": out if features is not None else None}
 
 
-def _grid(bounds, resolution):
+def _grid(bounds, resolution, where="voxelize"):
     b = [float(v) for v in bounds]
     if len(b) != 6 or not all(b[k + 3] > b[k] for k in range(3)):
-        raise ValueError(f"voxelize: bounds must be (x0, y0, z0, x1, y1, z1) with x1 > x0, y1 > y0, z1 > z0, got {bounds}")
+        raise ValueError(f"{where}: bounds must be (x0, y0, z0, x1, y1, z1) with x1 > x0, y1 > y0, z1 > z0, got {bounds}")
     n = [int(resolution)] * 3 if isinstance(resolution, int) else [int(r) for r in resolution]
     if len(n) != 3 or min(n) <= 0:
-        raise ValueError(f"voxelize: resolution must be a positive int or three of them, got {resolution}")
+        raise ValueError(f"{where}: resolution must be a positive int or three of them, got {resolution}")
     return b, n
 
 
@@ -1179,6 +1179,129 @@ def voxelize(bounds, resolution, pts_xyz, rotations, scales, opacity, features=N
     points, n = voxel_centres(bounds, resolution, pts_xyz.device)
     density, out = _QueryField.apply(True, points, pts_xyz, rotations, scales, opacity, features)
     return {"density": density.view(*n), "features": out.view(-1, *n) if features is not None else None}
+
+
+def _views_of(where, cameras, view_ids):
+    """the GaussianRasterizationSettings of `cameras` (a CameraBatch or a sequence of settings) picked by view_ids, and
+    their device; ValueError without a view or with a viewmatrix that is not a tensor on the first view's device (the caller
+    checks that it is a CUDA device after its other checks)"""
+    if isinstance(cameras, CameraBatch):
+        ids = list(range(len(cameras))) if view_ids is None else list(view_ids)
+        bg = _background((0.0, 0.0, 0.0), cameras.world_view_transform.device)
+        views = tuple(cameras.settings(i, bg, 0, False) for i in ids)
+    else:
+        views = tuple(cameras if view_ids is None else [cameras[i] for i in view_ids])
+    if not views:
+        raise ValueError(f"{where} needs at least one view")
+    device = torch.as_tensor(views[0].viewmatrix).device
+    for v, s in enumerate(views):
+        if not (torch.is_tensor(s.viewmatrix) and s.viewmatrix.device == device):
+            raise ValueError(f"{where}: cameras[{v}]: expected a viewmatrix on {device}")
+    return views, device
+
+
+def _check_tensor(where, name, t, shape, device):
+    """ValueError unless t is a float32 tensor of `shape` (None entries free) on `device`"""
+    if not torch.is_tensor(t) or t.dim() != len(shape) or any(n is not None and int(m) != n for m, n in zip(t.shape, shape)):
+        want = "[" + ",".join("." if n is None else str(n) for n in shape) + "]"
+        raise ValueError(f"{where}: {name}: expected {want}, got {tuple(t.shape) if torch.is_tensor(t) else type(t)}")
+    if t.dtype != torch.float32:
+        raise ValueError(f"{where}: {name}: expected float32, got {t.dtype}")
+    if t.device != device:
+        raise ValueError(f"{where}: {name}: expected a tensor on {device}, got {t.device}")
+
+
+def tsdf_fuse(cameras, depth, bounds, resolution, trunc, color=None, view_ids=None, volume=None):
+    """Fuse depth images into a truncated signed-distance volume (INTEGRATION.md §22), through every camera's own lens model
+    (include/mgs_rasterizer.h, mgs_tsdf_fuse): each voxel centre is projected with the renderer's map of a mean and its
+    cull, takes the depth d of the pixel it lands on (floor(px + 0.5), floor(py + 0.5)), and with s = d - z (z its view-space
+    depth) and views in order: skipped where d is not finite, d <= 0 or s < -trunc, else f = min(1, s / trunc) and
+    tsdf <- (tsdf w + f) / (w + 1), colour likewise, w <- w + 1, in float32 with no FMA.
+    cameras / view_ids as `camera_rays` (a CameraBatch or a sequence of settings of any of the four camera models, mixed;
+    learnable camera tensors are detached).  depth [V,H,W] float32 view-space z (the renderer's depth / alpha, or a sensor's
+    z-depth image; 0 where there is no return), every view H x W.  color [V,C,H,W] float32 (1 <= C <= 32) or None.  bounds
+    and resolution as `voxelize` (voxel (i, j, k) at voxel_centres' point); trunc > 0 the truncation distance in world units.
+    volume: an earlier result, fused into in place (a long stream can be fused in batches of views: one call over V views is
+    bitwise equal to successive calls over any split of them in order), or None for a fresh volume (tsdf 1, weight 0,
+    colour 0).  Returns {"tsdf": [X,Y,Z], "weight": [X,Y,Z], "color": [C,X,Y,Z] or None}; a voxel no view updates keeps its
+    bits, and the result is bitwise repeatable.  Not differentiable (inputs that require grad are detached).  Nothing is read
+    back to the host, so a call can be captured in a CUDA graph.  Raises ValueError on a bad shape, dtype, device, size
+    mismatch, trunc, channel count, bounds or resolution."""
+    where = "tsdf_fuse"
+    views, device = _views_of(where, cameras, view_ids)
+    V = len(views)
+    sizes = {(int(s.image_height), int(s.image_width)) for s in views}
+    if len(sizes) != 1:
+        raise ValueError(f"{where}: every view must have the same size, got {sorted(sizes)}")
+    H, W = sizes.pop()
+    b, n = _grid(bounds, resolution, where)
+    if isinstance(trunc, bool) or not isinstance(trunc, (int, float)) or not math.isfinite(trunc) or not trunc > 0:
+        raise ValueError(f"{where}: trunc must be a finite number > 0, got {trunc!r}")
+    _check_tensor(where, "depth", depth, (V, H, W), device)
+    C = 0
+    if color is not None:
+        _check_tensor(where, "color", color, (V, None, H, W), device)
+        C = int(color.shape[1])
+        if not 1 <= C <= 32:
+            raise ValueError(f"{where}: color: expected 1 to 32 channels, got {C}")
+    vol = None
+    if volume is not None:
+        if not isinstance(volume, dict) or not {"tsdf", "weight"} <= set(volume):
+            raise ValueError(f"{where}: volume: expected an earlier result (a dict with tsdf, weight and color)")
+        _check_tensor(where, "volume['tsdf']", volume["tsdf"], tuple(n), device)
+        _check_tensor(where, "volume['weight']", volume["weight"], tuple(n), device)
+        vc = volume.get("color")
+        if (vc is None) != (color is None):
+            raise ValueError(f"{where}: volume: its colour and color must both be given or both be None")
+        if vc is not None:
+            _check_tensor(where, "volume['color']", vc, (C,) + tuple(n), device)
+        for key in ("tsdf", "weight", "color"):
+            if volume.get(key) is not None and not volume[key].is_contiguous():
+                raise ValueError(f"{where}: volume['{key}']: expected a contiguous tensor (it is updated in place)")
+        vol = (volume["tsdf"].detach(), volume["weight"].detach(), vc.detach() if vc is not None else None)
+    if device.type != "cuda":
+        raise ValueError(f"{where}: cameras: expected a CUDA viewmatrix, got one on {device}")
+    from .rasterizer import tsdf_fuse_raw
+    tsdf, weight, cvol = tsdf_fuse_raw(views, depth.detach(), b, n, float(trunc), None if color is None else color.detach(),
+                                       volume=vol)
+    if volume is not None:
+        return volume
+    return {"tsdf": tsdf, "weight": weight, "color": cvol}
+
+
+def marching_cubes(values, level, bounds, weight=None, color=None):
+    """The level surface of a scalar grid as an indexed triangle mesh (INTEGRATION.md §22; include/mgs_rasterizer.h,
+    mgs_marching_cubes_count): values [X,Y,Z] float32 (a TSDF at level 0, or voxelize's density at a density level), grid
+    point (i, j, k) at its voxel centre over bounds (as `voxelize`).  weight [X,Y,Z] or None: a grid point is valid where its
+    value is finite and its weight is > 0 (unobserved TSDF voxels produce nothing); a cell with an invalid corner emits no
+    triangle.  color [C,X,Y,Z] (1 <= C <= 32) or None gives per-vertex attributes.
+    Returns {"vertices": [Nv,3] float32, "faces": [Nf,3] int64, "colors": [Nv,C] or None}.  Each crossed edge a triangle uses
+    has one vertex, shared by the cells around it, interpolated linearly at the level (t = (level - v_a) / (v_b - v_a), float32,
+    no FMA); each face's normal (v1 - v0) x (v2 - v0) points toward increasing value: out of a TSDF surface, into a density
+    blob (use faces[:, [0, 2, 1]] for outward faces there).  Ambiguous faces are split the same way from both sides, so a
+    level set inside the valid region gives a closed mesh; zero-area triangles are kept; a side below 2 gives an empty mesh.
+    The mesh is bitwise repeatable.  One device->host synchronisation per call reads the two totals that size the outputs,
+    so the call cannot be captured in a CUDA graph.  Not differentiable.  Raises ValueError on a bad shape, dtype, device,
+    channel count or bounds."""
+    where = "marching_cubes"
+    if not torch.is_tensor(values) or values.dim() != 3:
+        raise ValueError(f"{where}: values: expected [X,Y,Z], got {tuple(values.shape) if torch.is_tensor(values) else type(values)}")
+    device = values.device
+    _check_tensor(where, "values", values, (None, None, None), device)
+    n = tuple(int(x) for x in values.shape)
+    if isinstance(level, bool) or not isinstance(level, (int, float)) or not math.isfinite(level):
+        raise ValueError(f"{where}: level must be a finite number, got {level!r}")
+    b, _ = _grid(bounds, 1, where)
+    if weight is not None:
+        _check_tensor(where, "weight", weight, n, device)
+    if color is not None:
+        _check_tensor(where, "color", color, (None,) + n, device)
+        if not 1 <= color.shape[0] <= 32:
+            raise ValueError(f"{where}: color: expected 1 to 32 channels, got {color.shape[0]}")
+    from .rasterizer import marching_cubes_raw
+    vertices, faces, colors = marching_cubes_raw(values.detach(), float(level), b, None if weight is None else weight.detach(),
+                                                 None if color is None else color.detach())
+    return {"vertices": vertices, "faces": faces, "colors": colors}
 
 
 _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations

@@ -2103,3 +2103,57 @@ def fps_raw(points, n, lengths=None, start=None, debug=False):
         _b.check(L.mgs_fps(_ptr(state), B, P, int(n), _ptr(points), _ptr(lengths), _ptr(start), _ptr(index), _ptr(dist2),
                            int(bool(debug)), _stream(dev)), "mgs_fps")
     return index, dist2
+
+
+def tsdf_fuse_raw(views, depth, bounds, resolution, trunc, color=None, volume=None, tan_fov=None, ortho=None, fisheye=None,
+                  distortion=None, debug=False):
+    """Depth images fused into a TSDF volume (C ABI mgs_tsdf_fuse; definition in include/mgs_rasterizer.h).  depth [V,H,W]
+    view-space z on the views' device, every view W x H; color [V,C,H,W] or None; bounds (x0, y0, z0, x1, y1, z1) and
+    resolution (X, Y, Z) as voxel_centres takes them; trunc > 0.  volume: (tsdf [X,Y,Z], weight [X,Y,Z], color [C,X,Y,Z] or
+    None), updated in place, or None for a fresh one (tsdf 1, weight 0, colour 0).  `views`, `tan_fov`, `ortho`, `fisheye`
+    and `distortion` as in camera_rays_raw.  Returns (tsdf, weight, color or None).  Nothing is read back to the host."""
+    L = _b.lib()
+    dev, _, _, arr, tf, (oarr, farr, dcarr), keep = _ray_call(views, None, tan_fov, ortho, fisheye, distortion)
+    V = len(views)
+    X, Y, Z = (int(n) for n in resolution)
+    C = 0 if color is None else int(color.shape[1])
+    depth, color = _prep(depth, dev), _prep(color, dev)
+    if volume is None:
+        volume = (torch.ones((X, Y, Z), dtype=torch.float32, device=dev), torch.zeros((X, Y, Z), dtype=torch.float32, device=dev),
+                  torch.zeros((C, X, Y, Z), dtype=torch.float32, device=dev) if C else None)
+    tsdf, weight, cvol = volume
+    iarr = _intrinsics_array(tf, None) if tf is not None else None
+    b = (ctypes.c_double * 6)(*[float(x) for x in bounds])
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_tsdf_fuse(V, arr, iarr, oarr, farr, dcarr, _ptr(depth), C, _ptr(color), b, X, Y, Z, float(trunc), _ptr(tsdf),
+                                 _ptr(weight), _ptr(cvol) if C else None, int(bool(debug)), _stream(dev)), "mgs_tsdf_fuse")
+    return tsdf, weight, cvol
+
+
+def marching_cubes_raw(values, level, bounds, weight=None, color=None, debug=False):
+    """The level surface of values [X,Y,Z] (C ABI mgs_marching_cubes_count / _emit; definition in include/mgs_rasterizer.h),
+    grid point (i, j, k) at its voxel centre over bounds; weight [X,Y,Z] or None (a point is valid where its weight is > 0),
+    color [C,X,Y,Z] or None.  Returns (vertices [Nv,3] float32, faces [Nf,3] int64, colors [Nv,C] or None).  One
+    device->host read of the two totals sizes the outputs."""
+    if not values.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = values.device
+    values, weight, color = _prep(values, dev), _prep(weight, dev), _prep(color, dev)
+    X, Y, Z = values.shape
+    C = 0 if color is None else int(color.shape[0])
+    counts = torch.zeros(2, dtype=torch.int64, device=dev)
+    state = torch.empty(int(L.mgs_marching_cubes_state_bytes(X, Y, Z)), dtype=torch.uint8, device=dev)
+    lvl = float(level)
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_marching_cubes_count(_ptr(state), X, Y, Z, _ptr(values), _ptr(weight), lvl, _ptr(counts), int(bool(debug)),
+                                            _stream(dev)), "mgs_marching_cubes_count")
+        nv, nf = (int(n) for n in counts.cpu())
+        vertices = torch.empty((nv, 3), dtype=torch.float32, device=dev)
+        faces = torch.empty((nf, 3), dtype=torch.int64, device=dev)
+        colors = torch.empty((nv, C), dtype=torch.float32, device=dev) if C else None
+        if nv or nf:
+            b = (ctypes.c_double * 6)(*[float(x) for x in bounds])
+            _b.check(L.mgs_marching_cubes_emit(_ptr(state), X, Y, Z, _ptr(values), lvl, b, C, _ptr(color), _ptr(vertices), _ptr(faces),
+                                               _ptr(colors), int(bool(debug)), _stream(dev)), "mgs_marching_cubes_emit")
+    return vertices, faces, colors
