@@ -223,6 +223,10 @@ def _random(kw):
 
 
 # --------------------------------------------------------------------------- running the kernels
+GRAD_NAMES = ("dL_dmeans2D", "dL_dcolors", "dL_dfeature", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dsh", "dL_dscales",
+              "dL_drotations")
+
+
 class scratch_capture:
     """Keeps every backward view's blend_scratch alive (in call order) while in effect, so that its blend-stage records
     can be read after the call: `records(i, P)` = (gb [P,12], gn [P,4] or None) of the i-th view's scratch."""
@@ -265,11 +269,13 @@ def feature_tensor(feature, offset=0):
     return buf[offset:].view(feature.shape)
 
 
-def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False):
+def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False, capacity=None):
     """One forward and backward of the scene `inp`, and everything the checks read back.  The options (for
     tests/test_blend_planes_gpu.py): planar depth, the normal plane (cotangent inp["ct"]["dL_dnormal"]), the median depth
     (cotangent inp["ct"]["dL_dmedian"]) and the depth / mask heads (targets inp["dm_targets"], upstream gradients
-    inp["dm_scale"]).  inp["lens"]: a distortion tuple for a distorted-pinhole view, inp["tanfov"] its (tan_fovx, tan_fovy)."""
+    inp["dm_scale"]).  inp["lens"]: a distortion tuple for a distorted-pinhole view, inp["tanfov"] its (tan_fovx, tan_fovy).
+    capacity: the binning state's instance capacity (default: the history's, which must hold every instance); below the
+    instance count R the view keeps the first `capacity` instances it emits.  k["R"] is the true count, k["n"] the kept one."""
     import torch
     from manigaussian_b200 import rasterizer as R
     t = util._t
@@ -292,11 +298,16 @@ def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False)
         dm = _depth_mask_heads(t(inp["dm_targets"][0][None]), t(inp["dm_targets"][1][None]), 1, H, W, torch.device("cuda"))
         dm_scale = t(np.asarray(inp["dm_scale"], np.float32)[None])
     outs, streams = R.rasterize_views_raw([s], *args, return_depth=True, return_alpha=True, return_median=median,
-                                          return_normal=normal, loss_heads=heads, depth_mask=dm)
+                                          return_normal=normal, loss_heads=heads, depth_mask=dm,
+                                          capacities=None if capacity is None else [capacity])
     o = outs[0]
     Rn = o.num_rendered()
-    assert not o.overflowed()
     cap = int(o[0])
+    if capacity is None:
+        assert not o.overflowed()
+    else:
+        assert cap == capacity and o.overflowed() == (Rn > capacity), (Rn, capacity, o.overflowed())
+    n = min(Rn, cap)
     gc = [t(ct["dL_dcolor"])]
     gf = [t(ct["dL_dfeature"])] if F else None
     med = (o[-2 - int(normal)], o[-1 - int(normal)]) if median else None
@@ -318,13 +329,14 @@ def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False)
         nbytes = count * torch.empty((), dtype=dtype).element_size()
         return state[off:off + nbytes].view(dtype).cpu().numpy()
 
-    k = dict(W=W, H=H, F=F, R=Rn, color=o[1].cpu().numpy(), feature=o[2].cpu().numpy() if F else None,
-             depth=o[7].cpu().numpy(), alpha=o[8].cpu().numpy())
+    k = dict(W=W, H=H, F=F, R=Rn, n=n, cap=cap, status=o.status.numpy().copy(), color=o[1].cpu().numpy(),
+             feature=o[2].cpu().numpy() if F else None, depth=o[7].cpu().numpy(), alpha=o[8].cpu().numpy())
     k["means2D"] = arr("geometry", "means2D", geomB, P, 0, torch.float32, 2 * P).reshape(P, 2)
     k["conic_opacity"] = arr("geometry", "conic_opacity", geomB, P, 0, torch.float32, 4 * P).reshape(P, 4)
     k["rgbd"] = arr("geometry", "rgbd", geomB, P, 0, torch.float32, 4 * P).reshape(P, 4)
-    k["point_list"] = arr("binning", "point_list", binB, cap, 0, torch.int32, Rn).view(np.uint32)
-    k["block_bits"] = arr("binning", "block_bits", binB, cap, 0, torch.uint8, Rn)
+    k["point_list"] = arr("binning", "point_list", binB, cap, 0, torch.int32, n).view(np.uint32)
+    k["tile_ids"] = arr("binning", "tile_ids", binB, cap, 0, torch.int32, n).view(np.uint32)
+    k["block_bits"] = arr("binning", "block_bits", binB, cap, 0, torch.uint8, n)
     k["block_lists"] = arr("binning", "block_lists", binB, cap, 0, torch.int32, 8 * S).view(np.uint32).reshape(8, S)
     k["pixel_masks"] = arr("binning", "pixel_masks", binB, cap, 0, torch.int32, 8 * S).view(np.uint32).reshape(8, S)
     k["ranges"] = arr("image", "ranges", imgB, W, H, torch.int32, 2 * T).view(np.uint32).reshape(T, 2)
@@ -336,8 +348,11 @@ def run_kernels(inp, planar=False, normal=False, median=False, depth_mask=False)
     for n, v in zip(names, grads[:4]):
         k[n] = None if v is None else v.cpu().numpy()
     k["radii"] = o[3].cpu().numpy()
+    k["depths"] = arr("geometry", "depths", geomB, P, 0, torch.float32, P)
     k["gb"], k["gn"] = gb, gn
     k["dL_dmeans3D"] = grads[4].cpu().numpy()
+    k["grads"] = {n: (None if v is None else v.cpu().numpy()) for n, v in zip(GRAD_NAMES, grads)}
+    k["clamped"] = arr("geometry", "clamped", geomB, P, 0, torch.uint8, P)
     if planar or normal:
         k["nrm"] = arr("geometry", "nrm", geomB, P, 0, torch.float32, 4 * P).reshape(P, 4)
     if normal:

@@ -42,9 +42,17 @@ def test_block_lists_match_block_bits(W, H, F):
     n_contrib = arr("image", "n_contrib", imgB, W, H, torch.int32, W * H).view(np.uint32).reshape(H, W)
 
     assert np.array_equal(bits, recs[:, 6].astype(np.uint8)), "block_bits must be the records' block masks"
+    assert check_block_lists(W, H, ranges, bits, lists, masks, count, nwalk, n_contrib) > 0
+
+
+def check_block_lists(W, H, ranges, bits, lists, masks, count, nwalk, n_contrib):
+    """The block-list invariants of one view's binning state (numpy arrays as read back from its states): every 8x4 block's
+    list is exactly the positions of its tile's list whose block bit is set, in order; block_nwalk ends at the block's last
+    contributor, and the mask stored there names each pixel's last contributor.  Returns the number of blocks walked."""
+    gx = (W + 15) // 16
     walked = 0
-    for tile in range(T):
-        x0, x1 = ranges[tile]
+    for tile in range(ranges.shape[0]):
+        x0, x1 = (int(v) for v in ranges[tile])
         tb = bits[x0:x1]
         tx, ty = tile % gx, tile // gx
         for s in range(8):
@@ -72,4 +80,4 @@ def test_block_lists_match_block_bits(W, H, F):
                     e = np.nonzero(got[:k] == c - 1)[0]
                     assert len(e) == 1, (tile, s, xx, yy)
                     assert (masks[s, x0 + e[0]] >> (xx * 4 + yy)) & 1, (tile, s, xx, yy)
-    assert walked > 0
+    return walked
