@@ -1143,6 +1143,69 @@ int mgs_marching_cubes_count(void* state, int X, int Y, int Z, const float* valu
 int mgs_marching_cubes_emit(void* state, int X, int Y, int Z, const float* values, float level, const double* bounds, int C,
 	const float* color, float* out_vertices, long long* out_faces, float* out_colors, int debug, void* stream);
 
+/*
+ * MCMC density control (3DGS as Markov chain Monte Carlo, Kheradmand et al. 2024; gsplat's MCMCStrategy; no reference
+ * counterpart).  Parameters are raw, in 3DGS's parameterisation, fp32, contiguous, on one device: means [P,3], quats [P,4]
+ * (r, x, y, z; not necessarily unit), log_scales [P,3] (s = exp(log_scales)), opacity_logit [P] (o = sigmoid(x)).  Further
+ * per-Gaussian rows (SH [P,K,3], features [P,F], ...) travel as host arrays rows[num_rows] of device pointers with
+ * row_widths[num_rows] floats per Gaussian; optimizer moments (exp_avg, exp_avg_sq, max_exp_avg_sq of every parameter,
+ * the four above included) likewise as moments[num_moments] with moment_widths.
+ *
+ * Random numbers: Philox4x32-10 (Random123) with key {seed lo, seed hi} and counter {slot, offset lo, offset hi, tag}, tag 0
+ * for relocation and 1 for perturbation.  rng is device int64 [2] = {seed, offset}; each call reads it on the device and
+ * then advances offset by one there, so a replayed CUDA graph draws fresh numbers and equals the same eager calls.  Of the
+ * four output words w0..w3: a uniform 64-bit draw is r64 = w0 + 2^32 w1; normals are Box-Muller in fp32 with
+ * u1 = (float(w) + 1) 2^-32 and u2 = float(w') 2^-32: z0 = sqrt(-2 ln u1) cos(2 pi u2) and z1 = ... sin(2 pi u2) from
+ * (w0, w1), z2 = the cosine of (w2, w3).
+ *
+ * Relocation and growth, mgs_mcmc_relocate: rows [P_old, P) are newly appended rows.
+ *   - t = fp32(logit(min_opacity)).  Gaussian i < P_old is dead iff x_i <= t.  The destinations are the dead slots and every
+ *     slot in [P_old, P).
+ *   - w_i = floor(2^24 sigmoid_f64(x_i)) for alive i, 0 otherwise (also for a NaN x_i, which is neither dead nor a source);
+ *     S is their inclusive uint64 scan, T = S[P_old - 1].
+ *   - Destination j draws r64_j (slot j), u = mulhi64(r64_j, T), and takes src_j = min{i : S_i > u}: integer-exact, so it
+ *     does not depend on the scan's order.
+ *   - m_i = the number of destinations that picked i; n_i = min(m_i + 1, 51) (gsplat's clamp).  A source (m_i > 0) gets, in
+ *     fp64, o' = -expm1(log1p(-o) / n) and s' = s o / sum_{j=1..n} C(n,j) (-1)^(j-1) o'^j / sqrt(j) (gsplat's double sum
+ *     collapsed by the hockey-stick identity); o' is then clamped to [min_opacity, 1 - 2^-23], and the source's x and
+ *     log_scales become fp32(logit(o')) and fp32(log(s')).  The alternating sum loses about log10 of its largest term in
+ *     digits: 3 at o = 1 - 5e-5 (x = 10) and n = 51, all of them as o -> 1.
+ *   - Every destination becomes a copy of its source's new row: means, quats, log_scales, opacity_logit and every listed
+ *     row.  Every listed moment row is zeroed at every source and every destination (gsplat zeroes only the sources, which
+ *     leaves a copy with the dead Gaussian's stale moments).
+ *   - out_relocated: device int64 [1], the number of destinations filled; out_source: device int64 [P], src_j or -1 where
+ *     there is none, so callers can carry their own non-float state (labels, neighbour rows).
+ *   - T = 0 (nothing alive) writes no row, and out_relocated is 0.
+ *   - The result is bitwise repeatable (integer atomics count, and the per-source maths has no reduction), so the ranks of a
+ *     view-parallel run stay identical without a broadcast.
+ *   - state: mgs_mcmc_state_bytes(P_old) bytes of device memory on the device current at the call (contents irrelevant on
+ *     entry: the weights' scan, the counts and CUB's scan space; 12 bytes per Gaussian and the scan space).  0 means CUDA's
+ *     size query failed (mgs_last_error says why).
+ * Method: CUB's scan over the weights, then one thread per slot (dead test, draw, binary search, count), one per source
+ * (fp64 maths, moments), and one per (slot, tensor) for the copies; the tensors go to the kernels by value.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: P_old < 0 or
+ * P < P_old, min_opacity outside (0, 1), a NULL state, rng or out_relocated, a NULL out_source or parameter with P > 0,
+ * num_rows outside 0 .. MGS_MCMC_MAX_ROWS or num_moments outside 0 .. MGS_MCMC_MAX_MOMENTS, a NULL pointer or width array
+ * with a count > 0, a width <= 0, and a NULL row or moment pointer with P > 0.
+ *
+ * Position noise, mgs_mcmc_perturb: per Gaussian i, means_i += Sigma_i z_i g(o_i) scale with
+ *   Sigma_i = R(q^) diag(s^2) R(q^)^T, q^ = q / max(|q|, 1e-12)   (the projection's covariance formula, fp32)
+ *   z_i ~ N(0, I3) from slot i,   g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))),
+ * scale (device float [1]) = lr_means * noise_lr (gsplat: noise_lr = 5e5), read on the device so a captured graph follows
+ * the learning-rate schedule.  Only means is written.  quats must be 16-byte aligned.  P = 0 only advances the offset.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: P < 0, a NULL
+ * rng, a NULL means, quats, log_scales, opacity_logit or scale with P > 0, and misaligned quats.
+ * Neither call allocates, blocks or reads back to the host: both can be captured in a CUDA graph.  Not differentiable.
+ */
+#define MGS_MCMC_MAX_ROWS 16
+#define MGS_MCMC_MAX_MOMENTS 64
+size_t mgs_mcmc_state_bytes(int P);
+int mgs_mcmc_relocate(void* state, int P_old, int P, float min_opacity, float* means, float* quats, float* log_scales,
+	float* opacity_logit, int num_rows, float* const* rows, const int* row_widths, int num_moments, float* const* moments,
+	const int* moment_widths, long long* rng, long long* out_source, long long* out_relocated, int debug, void* stream);
+int mgs_mcmc_perturb(int P, float* means, const float* quats, const float* log_scales, const float* opacity_logit,
+	const float* scale, long long* rng, int debug, void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

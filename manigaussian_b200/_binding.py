@@ -231,6 +231,15 @@ def lib():
     L.mgs_fps.restype = C.c_int
     L.mgs_fps.argtypes = [vp, i, i, i, vp, vp, vp,  # state B P n points lengths start
                           vp, vp, i, vp]            # out_index out_dist2 debug stream
+    L.mgs_mcmc_state_bytes.restype = C.c_size_t
+    L.mgs_mcmc_state_bytes.argtypes = [C.c_int]
+    fpp, ip = C.POINTER(C.c_void_p), C.POINTER(C.c_int)
+    L.mgs_mcmc_relocate.restype = C.c_int
+    L.mgs_mcmc_relocate.argtypes = [vp, i, i, f, vp, vp, vp, vp,  # state P_old P min_opacity means quats log_scales opacity_logit
+                                    i, fpp, ip, i, fpp, ip,       # num_rows rows row_widths num_moments moments moment_widths
+                                    vp, vp, vp, i, vp]            # rng out_source out_relocated debug stream
+    L.mgs_mcmc_perturb.restype = C.c_int
+    L.mgs_mcmc_perturb.argtypes = [i, vp, vp, vp, vp, vp, vp, i, vp]  # P means quats log_scales opacity_logit scale rng debug stream
     L.mgs_tsdf_fuse.restype = C.c_int
     L.mgs_tsdf_fuse.argtypes = [i, C.POINTER(View), C.POINTER(ViewIntrinsics),  # V views intr
                                 C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
@@ -298,6 +307,7 @@ EXPORTED_SYMBOLS = (
     "mgs_deform_state_bytes", "mgs_deform", "mgs_deform_backward",
     "mgs_fps_state_bytes", "mgs_fps",
     "mgs_tsdf_fuse", "mgs_marching_cubes_state_bytes", "mgs_marching_cubes_count", "mgs_marching_cubes_emit",
+    "mgs_mcmc_state_bytes", "mgs_mcmc_relocate", "mgs_mcmc_perturb",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

@@ -2240,6 +2240,66 @@ int mgs_fps(void* state, int B, int P, int n, const float* points, const long lo
 	return 0;
 }
 
+size_t mgs_mcmc_state_bytes(int P)
+{
+	size_t bytes = 0;
+	const cudaError_t e = mgs::mcmc_state_bytes(std::max(P, 0), &bytes);
+	if (e != cudaSuccess) {
+		mgs::fail(MGS_ERR_CUDA, std::string("mgs_mcmc_state_bytes: ") + cudaGetErrorString(e));
+		return 0;
+	}
+	return bytes;
+}
+
+// a generic row list: count in 0 .. max, and with P > 0 a non-NULL pointer and a width > 0 for each
+static int mcmc_list(const char* what, int count, int max, float* const* ptrs, const int* widths, int P)
+{
+	using namespace mgs;
+	const std::string w = std::string("mgs_mcmc_relocate: ") + what;
+	if (count < 0 || count > max) return fail(MGS_ERR_INVALID_ARG, w + ": the count must be in [0, " + std::to_string(max) + "]");
+	if (count > 0 && (!ptrs || !widths)) return fail(MGS_ERR_INVALID_ARG, w + ": the pointer and width arrays are required");
+	for (int k = 0; k < count; k++) {
+		if (widths[k] <= 0) return fail(MGS_ERR_INVALID_ARG, w + ": every width must be > 0");
+		if (P > 0 && !ptrs[k]) return fail(MGS_ERR_INVALID_ARG, w + ": every pointer is required with P > 0");
+	}
+	return 0;
+}
+
+int mgs_mcmc_relocate(void* state, int P_old, int P, float min_opacity, float* means, float* quats, float* log_scales,
+	float* opacity_logit, int num_rows, float* const* rows, const int* row_widths, int num_moments, float* const* moments,
+	const int* moment_widths, long long* rng, long long* out_source, long long* out_relocated, int debug, void* stream)
+{
+	using namespace mgs;
+	if (P_old < 0 || P < P_old) return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: need 0 <= P_old <= P");
+	if (!(min_opacity > 0.f && min_opacity < 1.f)) return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: min_opacity must be in (0, 1)");
+	if (!state || !rng || !out_relocated || (P > 0 && !out_source))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: state, rng, out_relocated and out_source are required");
+	if (P > 0 && (!means || !quats || !log_scales || !opacity_logit))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: means, quats, log_scales and opacity_logit are required with P > 0");
+	if (mcmc_list("rows", num_rows, MGS_MCMC_MAX_ROWS, rows, row_widths, P) < 0) return MGS_ERR_INVALID_ARG;
+	if (mcmc_list("moments", num_moments, MGS_MCMC_MAX_MOMENTS, moments, moment_widths, P) < 0) return MGS_ERR_INVALID_ARG;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(mcmc_relocate(state, P_old, P, min_opacity, means, quats, log_scales, opacity_logit, num_rows, rows, row_widths,
+	                       num_moments, moments, moment_widths, rng, out_source, out_relocated, st));
+	MGS_STAGE("mcmc_relocate");
+	return 0;
+}
+
+int mgs_mcmc_perturb(int P, float* means, const float* quats, const float* log_scales, const float* opacity_logit, const float* scale,
+	long long* rng, int debug, void* stream)
+{
+	using namespace mgs;
+	if (P < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_perturb: P must be >= 0");
+	if (!rng) return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_perturb: rng is required");
+	if (P > 0 && (!means || !quats || !log_scales || !opacity_logit || !scale))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_perturb: means, quats, log_scales, opacity_logit and scale are required with P > 0");
+	if (reinterpret_cast<uintptr_t>(quats) & 15) return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_perturb: quats must be 16-byte aligned");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(mcmc_perturb(P, means, quats, log_scales, opacity_logit, scale, rng, st));
+	MGS_STAGE("mcmc_perturb");
+	return 0;
+}
+
 // the grid of bounds (host double[6], x0 y0 z0 x1 y1 z1) with n points per axis: lower corner and voxel size per axis
 static int grid_of(const char* where, const double* bounds, const int n[3], double lo[3], double step[3])
 {

@@ -70,6 +70,20 @@ __device__ __forceinline__ M3 transpose(const M3& a)
 			r.m[j][i] = a.m[i][j];
 	return r;
 }
+// Sigma = (S R)^T (S R) from scale and (un-normalised) quaternion; forward.cu:119-153 (project.cu, mcmc.cu)
+__device__ __forceinline__ void cov3d_from_scale_rot(const float* scale, float mod, const float* rot, float* cov3D)
+{
+	M3 S = m3(mod * scale[0], 0.f, 0.f, 0.f, mod * scale[1], 0.f, 0.f, 0.f, mod * scale[2]);
+	float r = rot[0], x = rot[1], y = rot[2], z = rot[3];
+	M3 R = m3(
+		1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y),
+		2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x),
+		2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y));
+	M3 Mx = mul(S, R);
+	M3 Sigma = mul(transpose(Mx), Mx);
+	cov3D[0] = Sigma.m[0][0]; cov3D[1] = Sigma.m[0][1]; cov3D[2] = Sigma.m[0][2];
+	cov3D[3] = Sigma.m[1][1]; cov3D[4] = Sigma.m[1][2]; cov3D[5] = Sigma.m[2][2];
+}
 __device__ __forceinline__ float dot(const float* a, const float* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
 __device__ __forceinline__ V3 xform4x3(const V3& p, const float* m)

@@ -641,6 +641,15 @@ size_t fps_state_bytes(int B, int P);
 cudaError_t fps_run(void* state, int B, int P, int n, const float* points, const long long* lengths, const long long* start,
 	long long* out_index, float* out_dist2, cudaStream_t st);
 
+// mcmc.cu: MCMC density control (include/mgs_rasterizer.h, mgs_mcmc_relocate / mgs_mcmc_perturb).  The state
+// (mcmc_state_bytes) holds the weights' inclusive scan, the per-source counts and CUB's scan scratch; nothing is read back.
+cudaError_t mcmc_state_bytes(int P, size_t* bytes);
+cudaError_t mcmc_relocate(void* state, int P_old, int P, float min_opacity, float* means, float* quats, float* log_scales,
+	float* opacity_logit, int num_rows, float* const* rows, const int* row_widths, int num_moments, float* const* moments,
+	const int* moment_widths, long long* rng, long long* out_source, long long* out_relocated, cudaStream_t st);
+cudaError_t mcmc_perturb(int P, float* means, const float* quats, const float* log_scales, const float* opacity_logit,
+	const float* scale, long long* rng, cudaStream_t st);
+
 // tsdf.cu: depth images fused into an [X,Y,Z] volume (include/mgs_rasterizer.h, mgs_tsdf_fuse), one thread per voxel over
 // the up to TSDF_CHUNK views of one launch, in order.  Every pointer is that of the launch's first view; view u's depth
 // starts at u H W and its colour at u C H W.  The kernel parameters exceed 4 KB (CUDA 12.1+ accepts up to 32,764 bytes).

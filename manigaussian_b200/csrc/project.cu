@@ -17,21 +17,6 @@ __device__ const float kSH_C2[] = { 1.0925484305920792f, -1.0925484305920792f, 0
 __device__ const float kSH_C3[] = { -0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
 	0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f, -0.5900435899266435f };
 
-// Sigma = (S R)^T (S R) from scale and (un-normalised) quaternion; forward.cu:119-153
-__device__ __forceinline__ void cov3d_from_scale_rot(const float* scale, float mod, const float* rot, float* cov3D)
-{
-	M3 S = m3(mod * scale[0], 0.f, 0.f, 0.f, mod * scale[1], 0.f, 0.f, 0.f, mod * scale[2]);
-	float r = rot[0], x = rot[1], y = rot[2], z = rot[3];
-	M3 R = m3(
-		1.f - 2.f * (y * y + z * z), 2.f * (x * y - r * z), 2.f * (x * z + r * y),
-		2.f * (x * y + r * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - r * x),
-		2.f * (x * z - r * y), 2.f * (y * z + r * x), 1.f - 2.f * (x * x + y * y));
-	M3 Mx = mul(S, R);
-	M3 Sigma = mul(transpose(Mx), Mx);
-	cov3D[0] = Sigma.m[0][0]; cov3D[1] = Sigma.m[0][1]; cov3D[2] = Sigma.m[0][2];
-	cov3D[3] = Sigma.m[1][1]; cov3D[4] = Sigma.m[1][2]; cov3D[5] = Sigma.m[2][2];
-}
-
 struct Cov2DTerms {
 	V3 t;
 	float txtz, tytz;

@@ -1304,6 +1304,154 @@ def marching_cubes(values, level, bounds, weight=None, color=None):
     return {"vertices": vertices, "faces": faces, "colors": colors}
 
 
+_MCMC_BASE = (("pts_xyz", 3), ("rotations", 4), ("scales", 3), ("opacity", 1))
+_MCMC_MAX_ROWS, _MCMC_MAX_MOMENTS = 16, 64  # MGS_MCMC_MAX_ROWS / MGS_MCMC_MAX_MOMENTS (include/mgs_rasterizer.h)
+
+
+def _mcmc_tensor(where, name, t, P, device, width=None):
+    """ValueError unless t is a contiguous float32 [P, ...] tensor on `device`; with a width, [P,width] (or [P] for width 1)"""
+    got = tuple(t.shape) if torch.is_tensor(t) else type(t)
+    if width is None:
+        ok = torch.is_tensor(t) and t.dim() >= 1 and (P is None or t.shape[0] == P)
+        want = f"[{'P' if P is None else P}, ...]"
+    else:
+        shapes = ((P, width),) + (((P,),) if width == 1 else ())
+        ok = torch.is_tensor(t) and (tuple(t.shape) in shapes if P is not None else (t.dim() == 2 and t.shape[1] == width))
+        want = " or ".join("[" + ",".join(str(x) for x in s) + "]" for s in shapes) if P is not None else f"[P,{width}]"
+    if not ok:
+        raise ValueError(f"{where}: {name}: expected {want}, got {got}")
+    if t.dtype != torch.float32:
+        raise ValueError(f"{where}: {name}: expected float32, got {t.dtype}")
+    if device is not None and t.device != device:
+        raise ValueError(f"{where}: {name}: expected a tensor on {device}, got {t.device}")
+    if not t.is_contiguous():
+        raise ValueError(f"{where}: {name}: expected a contiguous tensor (it is read and written in place)")
+
+
+def _mcmc_rng(where, rng, device):
+    if not torch.is_tensor(rng) or rng.dtype != torch.int64 or tuple(rng.shape) != (2,) or not rng.is_contiguous():
+        got = (rng.dtype, tuple(rng.shape)) if torch.is_tensor(rng) else type(rng)
+        raise ValueError(f"{where}: rng: expected a contiguous int64 [2] tensor {{seed, offset}}, got {got}")
+    if rng.device != device:
+        raise ValueError(f"{where}: rng: expected a tensor on {device}, got {rng.device}")
+
+
+def _mcmc_logit(min_opacity):
+    """t = fp32(logit(min_opacity)): a Gaussian whose opacity logit is <= t is dead"""
+    return float(torch.tensor(math.log(min_opacity / (1.0 - min_opacity)), dtype=torch.float32))
+
+
+def mcmc_relocate(params, optimizer=None, n=None, min_opacity=0.005, *, rng):
+    """MCMC relocation and growth (3DGS as Markov chain Monte Carlo, Kheradmand et al. 2024, as gsplat's MCMCStrategy runs it;
+    INTEGRATION.md §23; definition in include/mgs_rasterizer.h, mgs_mcmc_relocate), in place on the device.
+    params: a dict of float32 contiguous tensors on one CUDA device, in 3DGS's raw parameterisation: "pts_xyz" [P,3],
+    "rotations" [P,4] (r, x, y, z), "scales" [P,3] (log scales), "opacity" [P] or [P,1] (logits), plus up to 16 further
+    per-Gaussian rows [P, ...] (SH, features).  n: the new count (None: P); n > P appends n - P rows.
+    Dead Gaussians (opacity logit <= fp32(logit(min_opacity))) and the appended rows are the destinations.  Each draws a
+    live source with probability proportional to floor(2^24 opacity); each source that k destinations picked splits its
+    opacity o and scales s over its n = min(k + 1, 51) copies (o' = 1 - (1 - o)^(1/n), s' from gsplat's formula in fp64),
+    and every destination becomes a copy of its source's new row.
+    optimizer: a torch.optim optimizer over (some of) the params, or None.  Every state tensor shaped like its parameter
+    (Adam's exp_avg, exp_avg_sq, max_exp_avg_sq) is zeroed at every source and destination (gsplat zeroes the sources
+    only).  On growth, the params dict, the optimizer's param groups and its state get new, longer tensors (as gsplat's
+    _update_param_with_optimizer does); without growth every tensor is updated in place.
+    rng: int64 [2] = {seed, offset} on the params' device; the offset advances by one on the device per call.
+    Returns {"source": [n] int64, each slot's source or -1, "relocated": [1] int64, the destinations filled} on the device.
+    With nothing alive no row is written (appended rows are zero with a dead opacity).  The result is bitwise repeatable.
+    Nothing is read back to the host: without growth a call can be captured in a CUDA graph.  Not differentiable.
+    Raises ValueError on a missing key, a bad shape, dtype, device or contiguity, rows of different lengths, n < P, too
+    many rows or moments, min_opacity outside (0, 1), a bad rng, and non-leaf params with an optimizer."""
+    where = "mcmc_relocate"
+    if not isinstance(params, dict) or any(k not in params for k, _ in _MCMC_BASE):
+        raise ValueError(f"{where}: params: expected a dict with keys {', '.join(k for k, _ in _MCMC_BASE)} (and any further rows)")
+    x = params["pts_xyz"]
+    _mcmc_tensor(where, "params['pts_xyz']", x, None, None, 3)
+    P, device = int(x.shape[0]), x.device
+    widths = dict(_MCMC_BASE)
+    for name, t in params.items():
+        _mcmc_tensor(where, f"params[{name!r}]", t, P, device, widths.get(name))
+    extra = [k for k in params if k not in widths]
+    if len(extra) > _MCMC_MAX_ROWS:
+        raise ValueError(f"{where}: params: at most {_MCMC_MAX_ROWS} rows besides the four parameters, got {len(extra)}")
+    n = P if n is None else n
+    if isinstance(n, bool) or not isinstance(n, int) or n < P:
+        raise ValueError(f"{where}: n must be an int >= P = {P}, got {n!r}")
+    if isinstance(min_opacity, bool) or not isinstance(min_opacity, (int, float)) or not 0.0 < min_opacity < 1.0:
+        raise ValueError(f"{where}: min_opacity must be a number in (0, 1), got {min_opacity!r}")
+    _mcmc_rng(where, rng, device)
+    names = {}
+    if optimizer is not None:
+        for name, t in params.items():
+            if not t.is_leaf:
+                raise ValueError(f"{where}: params[{name!r}] is not a leaf tensor: an optimizer can only hold leaves")
+            names[id(t)] = name
+    if n > P:
+        grown = {}
+        for name, p in params.items():
+            ext = torch.zeros((n - P,) + tuple(p.shape[1:]), dtype=p.dtype, device=device)
+            if name == "opacity":
+                ext.fill_(_mcmc_logit(min_opacity))
+            q = torch.cat([p.detach(), ext])
+            grown[name] = torch.nn.Parameter(q, p.requires_grad) if isinstance(p, torch.nn.Parameter) else q.requires_grad_(p.requires_grad)
+        if optimizer is not None:
+            for group in optimizer.param_groups:
+                for k, p in enumerate(group["params"]):
+                    name = names.get(id(p))
+                    if name is None:
+                        continue
+                    q = grown[name]
+                    state = optimizer.state.pop(p, None)
+                    if state is not None:
+                        for key, v in state.items():
+                            if torch.is_tensor(v) and v.shape == p.shape:
+                                state[key] = torch.cat([v, torch.zeros((n - P,) + tuple(v.shape[1:]), dtype=v.dtype, device=v.device)])
+                        optimizer.state[q] = state
+                    group["params"][k] = q
+        params.update(grown)
+    moments = []
+    if optimizer is not None:
+        for name, p in params.items():
+            for key, v in optimizer.state.get(p, {}).items():
+                if torch.is_tensor(v) and v.shape == p.shape:
+                    _mcmc_tensor(where, f"optimizer state {key!r} of params[{name!r}]", v, n, device)
+                    moments.append(v)
+    if len(moments) > _MCMC_MAX_MOMENTS:
+        raise ValueError(f"{where}: optimizer: at most {_MCMC_MAX_MOMENTS} moment tensors, got {len(moments)}")
+    from .rasterizer import mcmc_relocate_raw
+    d = {k: v.detach() for k, v in params.items()}
+    source, relocated = mcmc_relocate_raw(P, d["pts_xyz"], d["rotations"], d["scales"], d["opacity"], [d[k] for k in extra],
+                                          moments, rng, float(min_opacity))
+    return {"source": source, "relocated": relocated}
+
+
+def mcmc_perturb(pts_xyz, rotations, scales, opacity, scale, rng):
+    """MCMC position noise (INTEGRATION.md §23; include/mgs_rasterizer.h, mgs_mcmc_perturb), in place: per Gaussian,
+    pts_xyz += Sigma z g(o) scale with Sigma = R(q/|q|) diag(exp(scales)^2) R^T, z ~ N(0, I3) from rng, o = sigmoid(opacity)
+    and g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))), so only nearly transparent Gaussians move far.  Raw parameters as
+    mcmc_relocate takes them: pts_xyz [P,3] (written), rotations [P,4], scales [P,3] (log), opacity [P] or [P,1] (logits).
+    scale: lr_means * noise_lr (gsplat: noise_lr = 5e5) as a float32 tensor of one element on the device (a captured
+    graph then follows the learning-rate schedule), or a number.  rng: int64 [2] = {seed, offset}, advanced by one on the
+    device.  Only pts_xyz is written.  Nothing is read back to the host, so a call can be captured in a CUDA graph.  Not
+    differentiable.  Returns pts_xyz.  Raises ValueError on a bad shape, dtype, device, contiguity, scale or rng."""
+    where = "mcmc_perturb"
+    _mcmc_tensor(where, "pts_xyz", pts_xyz, None, None, 3)
+    P, device = int(pts_xyz.shape[0]), pts_xyz.device
+    for name, t, w in (("rotations", rotations, 4), ("scales", scales, 3), ("opacity", opacity, 1)):
+        _mcmc_tensor(where, name, t, P, device, w)
+    if torch.is_tensor(scale):
+        if scale.dtype != torch.float32 or scale.numel() != 1 or scale.device != device:
+            raise ValueError(f"{where}: scale: expected a float32 tensor of one element on {device}, got "
+                             f"{scale.dtype} {tuple(scale.shape)} on {scale.device}")
+    elif isinstance(scale, bool) or not isinstance(scale, (int, float)) or not math.isfinite(scale):
+        raise ValueError(f"{where}: scale: expected a finite number or a device tensor, got {scale!r}")
+    else:
+        scale = torch.full((1,), float(scale), dtype=torch.float32, device=device)
+    _mcmc_rng(where, rng, device)
+    from .rasterizer import mcmc_perturb_raw
+    mcmc_perturb_raw(pts_xyz.detach(), rotations.detach(), scales.detach(), opacity.detach(), scale.detach(), rng)
+    return pts_xyz
+
+
 _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations
 
 

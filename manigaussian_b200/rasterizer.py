@@ -2157,3 +2157,53 @@ def marching_cubes_raw(values, level, bounds, weight=None, color=None, debug=Fal
             _b.check(L.mgs_marching_cubes_emit(_ptr(state), X, Y, Z, _ptr(values), lvl, b, C, _ptr(color), _ptr(vertices), _ptr(faces),
                                                _ptr(colors), int(bool(debug)), _stream(dev)), "mgs_marching_cubes_emit")
     return vertices, faces, colors
+
+
+def _pointer_list(tensors):
+    """host arrays (device pointers, floats per row) of a list of [P, ...] tensors, for the C ABI's generic row lists"""
+    n = len(tensors)
+    ptrs = (ctypes.c_void_p * max(n, 1))(*[t.data_ptr() for t in tensors])
+    widths = (ctypes.c_int * max(n, 1))(*[t.numel() // max(t.shape[0], 1) for t in tensors])
+    return n, ptrs, widths
+
+
+def mcmc_relocate_raw(P_old, means, quats, log_scales, opacity_logit, rows, moments, rng, min_opacity=0.005, debug=False):
+    """MCMC relocation and growth in place (C ABI mgs_mcmc_relocate; definition in include/mgs_rasterizer.h): means [P,3],
+    quats [P,4], log_scales [P,3], opacity_logit [P] or [P,1], every tensor of `rows` and `moments` [P, ...], all float32,
+    contiguous and on one device; rows [P_old, P) are newly appended.  rng: device int64 [2] = {seed, offset}, advanced by
+    one on the device.  Returns (source [P] int64, relocated [1] int64) on the same device.  Nothing is read back to the
+    host, so a call can be captured in a CUDA graph."""
+    if not means.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = means.device
+    P = means.shape[0]
+    source = torch.empty(P, dtype=torch.int64, device=dev)
+    relocated = torch.empty(1, dtype=torch.int64, device=dev)
+    nr, rp, rw = _pointer_list(rows)
+    nm, mp, mw = _pointer_list(moments)
+    with torch.cuda.device(dev):  # the state's size depends on the device it is used on
+        nbytes = int(L.mgs_mcmc_state_bytes(int(P_old)))
+        if nbytes == 0:
+            raise RuntimeError("mgs_mcmc_state_bytes: " + _b.last_error())
+        state = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _b.check(L.mgs_mcmc_relocate(_ptr(state), int(P_old), P, float(min_opacity), _ptr(means), _ptr(quats), _ptr(log_scales),
+                                     _ptr(opacity_logit), nr, rp, rw, nm, mp, mw, _ptr(rng), _ptr(source), _ptr(relocated),
+                                     int(bool(debug)), _stream(dev)), "mgs_mcmc_relocate")
+    return source, relocated
+
+
+def mcmc_perturb_raw(means, quats, log_scales, opacity_logit, scale, rng, debug=False):
+    """MCMC position noise in place (C ABI mgs_mcmc_perturb; definition in include/mgs_rasterizer.h): means [P,3] += the
+    covariance-shaped noise of quats [P,4], log_scales [P,3] and opacity_logit [P], times scale (device float32 [1]).  rng:
+    device int64 [2] = {seed, offset}, advanced by one on the device.  Only means is written; nothing is read back."""
+    if not means.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = means.device
+    if quats.data_ptr() % 16:  # the kernel reads each quaternion as one 16-byte load
+        quats = quats.clone()
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_mcmc_perturb(means.shape[0], _ptr(means), _ptr(quats), _ptr(log_scales), _ptr(opacity_logit), _ptr(scale),
+                                    _ptr(rng), int(bool(debug)), _stream(dev)), "mgs_mcmc_perturb")
+    return means
