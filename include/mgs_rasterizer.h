@@ -1206,6 +1206,72 @@ int mgs_mcmc_relocate(void* state, int P_old, int P, float min_opacity, float* m
 int mgs_mcmc_perturb(int P, float* means, const float* quats, const float* log_scales, const float* opacity_logit,
 	const float* scale, long long* rng, int debug, void* stream);
 
+/*
+ * Default density control (3DGS's adaptive density control as gsplat's DefaultStrategy runs it; no reference counterpart).
+ * Parameters, extra rows and moments as in the MCMC section above.
+ *
+ * Statistics, mgs_densify_stats: for each Gaussian i, over the views v = 0 .. V-1 in order, where radii[v,i] > 0:
+ *   n = sqrt(gx gx + gy gy) with (gx, gy) the first two components of viewspace_grad[v,i];
+ *   grad2d_i += n scale;   count_i += 1;   radius_i = max(radius_i, float(radii[v,i]) / float(sizes[v]))
+ * every operation rounded to fp32 without FMA, so the result is bitwise equal to a float32 restatement.
+ *   - viewspace_grad [V,P,3] fp32 (each view's screen-space mean gradient, the reference's viewspace_points.grad);
+ *     radii [V,P] int32; sizes host int[V], each view's max(W, H) > 0; grad2d [P] fp32, count [P] int32 and radius [P]
+ *     fp32 are read and updated in place (zero for fresh statistics).
+ *   - scale: scale_device (device float [1]) when not NULL, else the host value scale.  A loss averaged over V views has
+ *     per-view gradients 1/V as large; scale = V undoes that, as gsplat's n_cameras factor does.
+ *   - One thread per Gaussian, no atomics: bitwise repeatable.  Views run in launches of up to 64.  V = 0 or P = 0
+ *     enqueues nothing.
+ * Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for: V or P < 0,
+ * a NULL viewspace_grad, radii, sizes, grad2d, count or radius with V, P > 0, a size <= 0, and a scale that is not finite
+ * with a NULL scale_device.
+ *
+ * Refinement, mgs_densify_count then mgs_densify_emit (gsplat's duplicate, then split, then prune).  The thresholds move
+ * into the log / logit domain once, in fp64, rounded to fp32:
+ *   t_opa = fp32(logit(prune_opacity)),  t_small = fp32(log(grow_scale3d scene_scale)),  t_big = fp32(log(prune_scale3d scene_scale)).
+ * Per Gaussian i, with L_i = fmaxf(fmaxf(ls0, ls1), ls2) its largest log scale (a NaN operand is ignored) and r_i = radius_i:
+ *   - high_i = grad2d_i / max(count_i, 1) > grad_threshold (fp32 division);  small_i = L_i <= t_small;
+ *   - clone_i = high_i && small_i;  split_i = (high_i && !small_i) || r_i > grow_scale2d (a Gaussian can be both);
+ *   - a row with logit x, largest log scale L and radius r is pruned when
+ *     x < t_opa || (prune_too_big && (L > t_big || r > prune_scale2d));
+ *   - the kept original: present when !split_i and not pruned; all its rows and moment rows are copied;
+ *   - the clone: present when clone_i and the original's row is not pruned; its rows are copied, its moments zero;
+ *   - the children b = 0, 1 of a split i, present when not pruned by their own L (their logit and radius are the parent's):
+ *     log scales fp32((double)ls - log(1.6)) per axis; means mu + R(q^) diag(exp(ls)) z_{i,b} in fp32 with the parent's
+ *     log scales ls and q^ = q / max(|q|, 1e-12); quats, opacity and every extra row copied; moments zero.
+ *   - z_{i,b}: the normals z0, z1, z2 of the MCMC section's Box-Muller from Philox counter {i, offset lo, offset hi, 2 + b}.
+ *   - Output order (gsplat's concatenation): [kept originals] ++ [kept clones] ++ [kept first children] ++ [kept second
+ *     children], each segment in ascending i.
+ * grow_scale2d and prune_scale2d take INFINITY to turn their test off (gsplat's None).
+ * mgs_densify_count classifies, scans the three per-Gaussian flags (original kept, clone kept, children kept) with CUB and
+ * writes out_counts (device int64 [4]) = {n_new, cloned, split, pruned}: cloned and split count clone_i and split_i, and
+ * n_new = P + cloned + split - pruned.  state: mgs_densify_state_bytes(P) bytes of device memory (17 bytes per Gaussian
+ * and CUB's scan space; contents irrelevant on entry; 0 means CUDA's size query failed).  The caller reads out_counts back
+ * (the one host read of a refinement), allocates the n_new-row tensors and calls mgs_densify_emit with the same state, P
+ * and old tensors; the new tensors have n_new rows of the same widths (new_rows[k] and new_moments[k] beside rows[k] and
+ * moments[k]).  emit writes every new row and out_source (device int64 [n_new], each row's parent i), reads rng = {seed,
+ * offset} (device int64 [2]) on the device and advances the offset by one there.  Both calls are bitwise repeatable
+ * (integer atomics count; the scan and the rows have no float reduction).  P = 0 writes zero totals; n_new = 0 writes
+ * no row.  Argument errors return, with mgs_last_error set and before anything is enqueued, MGS_ERR_INVALID_ARG for:
+ *   count: P < 0, a NULL state or out_counts, a NULL input with P > 0, scene_scale, grow_scale3d or prune_scale3d not
+ *     finite and > 0, prune_opacity outside (0, 1), and a NaN grad_threshold, grow_scale2d or prune_scale2d;
+ *   emit: P or n_new < 0, n_new > 0 with P = 0, a NULL state or rng, a NULL old parameter with P > 0, a NULL new parameter
+ *     or out_source with n_new > 0, the row-list errors of mgs_mcmc_relocate (at most MGS_MCMC_MAX_ROWS rows and
+ *     MGS_MCMC_MAX_MOMENTS moments), and a NULL new_rows / new_moments array or entry with n_new > 0.
+ * Not differentiable.
+ */
+int mgs_densify_stats(int V, int P, const float* viewspace_grad, const int* radii, const int* sizes, float scale,
+	const float* scale_device, float* grad2d, int* count, float* radius, int debug, void* stream);
+size_t mgs_densify_state_bytes(int P);
+int mgs_densify_count(void* state, int P, const float* log_scales, const float* opacity_logit, const float* grad2d,
+	const int* count, const float* radius, double scene_scale, float grad_threshold, double grow_scale3d, float grow_scale2d,
+	double prune_opacity, double prune_scale3d, float prune_scale2d, int prune_too_big, long long* out_counts, int debug,
+	void* stream);
+int mgs_densify_emit(void* state, int P, int n_new, const float* means, const float* quats, const float* log_scales,
+	const float* opacity_logit, int num_rows, const float* const* rows, const int* row_widths, int num_moments,
+	const float* const* moments, const int* moment_widths, float* new_means, float* new_quats, float* new_log_scales,
+	float* new_opacity_logit, float* const* new_rows, float* const* new_moments, long long* rng, long long* out_source, int debug,
+	void* stream);
+
 /* The same two loss heads for V images that already sit in device memory (planar color [V,3,N], feature [V,F,N] or NULL,
  * N = H*W): loss_acc [V,2] (zeroed by the call) and the cotangent planes as above, one launch. */
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

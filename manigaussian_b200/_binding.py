@@ -240,6 +240,22 @@ def lib():
                                     vp, vp, vp, i, vp]            # rng out_source out_relocated debug stream
     L.mgs_mcmc_perturb.restype = C.c_int
     L.mgs_mcmc_perturb.argtypes = [i, vp, vp, vp, vp, vp, vp, i, vp]  # P means quats log_scales opacity_logit scale rng debug stream
+    d = C.c_double
+    L.mgs_densify_stats.restype = C.c_int
+    L.mgs_densify_stats.argtypes = [i, i, vp, vp, ip, f, vp,  # V P viewspace_grad radii sizes scale scale_device
+                                    vp, vp, vp, i, vp]        # grad2d count radius debug stream
+    L.mgs_densify_state_bytes.restype = C.c_size_t
+    L.mgs_densify_state_bytes.argtypes = [C.c_int]
+    L.mgs_densify_count.restype = C.c_int
+    L.mgs_densify_count.argtypes = [vp, i, vp, vp, vp, vp, vp,  # state P log_scales opacity_logit grad2d count radius
+                                    d, f, d, f,                 # scene_scale grad_threshold grow_scale3d grow_scale2d
+                                    d, d, f, i,                 # prune_opacity prune_scale3d prune_scale2d prune_too_big
+                                    vp, i, vp]                  # out_counts debug stream
+    L.mgs_densify_emit.restype = C.c_int
+    L.mgs_densify_emit.argtypes = [vp, i, i, vp, vp, vp, vp,    # state P n_new means quats log_scales opacity_logit
+                                   i, fpp, ip, i, fpp, ip,      # num_rows rows row_widths num_moments moments moment_widths
+                                   vp, vp, vp, vp, fpp, fpp,    # new_{means,quats,log_scales,opacity_logit,rows,moments}
+                                   vp, vp, i, vp]               # rng out_source debug stream
     L.mgs_tsdf_fuse.restype = C.c_int
     L.mgs_tsdf_fuse.argtypes = [i, C.POINTER(View), C.POINTER(ViewIntrinsics),  # V views intr
                                 C.POINTER(C.c_int), C.POINTER(ViewFisheye), C.POINTER(ViewDistortion),  # ortho fisheye distortion
@@ -308,6 +324,7 @@ EXPORTED_SYMBOLS = (
     "mgs_fps_state_bytes", "mgs_fps",
     "mgs_tsdf_fuse", "mgs_marching_cubes_state_bytes", "mgs_marching_cubes_count", "mgs_marching_cubes_emit",
     "mgs_mcmc_state_bytes", "mgs_mcmc_relocate", "mgs_mcmc_perturb",
+    "mgs_densify_stats", "mgs_densify_state_bytes", "mgs_densify_count", "mgs_densify_emit",
     "mgs_activate", "mgs_activate_backward",
     "mgs_mark_visible", "mgs_state_array", "mgs_profile_enable", "mgs_profile_num_stages",
     "mgs_profile_stage_name", "mgs_profile_read",

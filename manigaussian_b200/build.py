@@ -22,7 +22,7 @@ VARIANT = os.environ.get("MGS_VARIANT", "")
 EXTRA = os.environ.get("MGS_NVCC_DEFINES", "").split() if VARIANT else []
 LIB = os.path.join(LIBDIR, "libmgs_rasterizer%s.so" % (("_" + VARIANT) if VARIANT else ""))
 SOURCES = ["project.cu", "project_bwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "loss_heads.cu", "ssim.cu", "activate.cu", "normals.cu", "planar.cu", "flow.cu", "visibility.cu",
-           "lift.cu", "field.cu", "knn.cu", "neighbour_reg.cu", "deform.cu", "rays.cu", "fps.cu", "tsdf.cu", "marching_cubes.cu", "mcmc.cu", "api.cu"]
+           "lift.cu", "field.cu", "knn.cu", "neighbour_reg.cu", "deform.cu", "rays.cu", "fps.cu", "tsdf.cu", "marching_cubes.cu", "mcmc.cu", "densify.cu", "api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

@@ -2252,10 +2252,11 @@ size_t mgs_mcmc_state_bytes(int P)
 }
 
 // a generic row list: count in 0 .. max, and with P > 0 a non-NULL pointer and a width > 0 for each
-static int mcmc_list(const char* what, int count, int max, float* const* ptrs, const int* widths, int P)
+template <class T>
+static int row_list(const char* where, const char* what, int count, int max, T* const* ptrs, const int* widths, int P)
 {
 	using namespace mgs;
-	const std::string w = std::string("mgs_mcmc_relocate: ") + what;
+	const std::string w = std::string(where) + ": " + what;
 	if (count < 0 || count > max) return fail(MGS_ERR_INVALID_ARG, w + ": the count must be in [0, " + std::to_string(max) + "]");
 	if (count > 0 && (!ptrs || !widths)) return fail(MGS_ERR_INVALID_ARG, w + ": the pointer and width arrays are required");
 	for (int k = 0; k < count; k++) {
@@ -2276,8 +2277,8 @@ int mgs_mcmc_relocate(void* state, int P_old, int P, float min_opacity, float* m
 		return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: state, rng, out_relocated and out_source are required");
 	if (P > 0 && (!means || !quats || !log_scales || !opacity_logit))
 		return fail(MGS_ERR_INVALID_ARG, "mgs_mcmc_relocate: means, quats, log_scales and opacity_logit are required with P > 0");
-	if (mcmc_list("rows", num_rows, MGS_MCMC_MAX_ROWS, rows, row_widths, P) < 0) return MGS_ERR_INVALID_ARG;
-	if (mcmc_list("moments", num_moments, MGS_MCMC_MAX_MOMENTS, moments, moment_widths, P) < 0) return MGS_ERR_INVALID_ARG;
+	if (row_list("mgs_mcmc_relocate", "rows", num_rows, MGS_MCMC_MAX_ROWS, rows, row_widths, P) < 0) return MGS_ERR_INVALID_ARG;
+	if (row_list("mgs_mcmc_relocate", "moments", num_moments, MGS_MCMC_MAX_MOMENTS, moments, moment_widths, P) < 0) return MGS_ERR_INVALID_ARG;
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	MGS_CUDA(mcmc_relocate(state, P_old, P, min_opacity, means, quats, log_scales, opacity_logit, num_rows, rows, row_widths,
 	                       num_moments, moments, moment_widths, rng, out_source, out_relocated, st));
@@ -2297,6 +2298,99 @@ int mgs_mcmc_perturb(int P, float* means, const float* quats, const float* log_s
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	MGS_CUDA(mcmc_perturb(P, means, quats, log_scales, opacity_logit, scale, rng, st));
 	MGS_STAGE("mcmc_perturb");
+	return 0;
+}
+
+int mgs_densify_stats(int V, int P, const float* viewspace_grad, const int* radii, const int* sizes, float scale,
+	const float* scale_device, float* grad2d, int* count, float* radius, int debug, void* stream)
+{
+	using namespace mgs;
+	if (V < 0 || P < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_stats: V and P must be >= 0");
+	if (V == 0 || P == 0) return 0;
+	if (!viewspace_grad || !radii || !sizes || !grad2d || !count || !radius)
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_stats: viewspace_grad, radii, sizes, grad2d, count and radius are required");
+	for (int v = 0; v < V; v++)
+		if (sizes[v] <= 0) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_stats: every size must be > 0");
+	if (!scale_device && !std::isfinite(scale)) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_stats: scale must be finite");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(densify_stats(V, P, viewspace_grad, radii, sizes, scale, scale_device, grad2d, count, radius, st));
+	MGS_STAGE("densify_stats");
+	return 0;
+}
+
+size_t mgs_densify_state_bytes(int P)
+{
+	size_t bytes = 0;
+	const cudaError_t e = mgs::densify_state_bytes(std::max(P, 0), &bytes);
+	if (e != cudaSuccess) {
+		mgs::fail(MGS_ERR_CUDA, std::string("mgs_densify_state_bytes: ") + cudaGetErrorString(e));
+		return 0;
+	}
+	return bytes;
+}
+
+static bool positive_finite(double v) { return std::isfinite(v) && v > 0.0; }
+
+int mgs_densify_count(void* state, int P, const float* log_scales, const float* opacity_logit, const float* grad2d,
+	const int* count, const float* radius, double scene_scale, float grad_threshold, double grow_scale3d, float grow_scale2d,
+	double prune_opacity, double prune_scale3d, float prune_scale2d, int prune_too_big, long long* out_counts, int debug,
+	void* stream)
+{
+	using namespace mgs;
+	if (P < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: P must be >= 0");
+	if (!state || !out_counts) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: state and out_counts are required");
+	if (P > 0 && (!log_scales || !opacity_logit || !grad2d || !count || !radius))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: log_scales, opacity_logit, grad2d, count and radius are required with P > 0");
+	if (!positive_finite(scene_scale) || !positive_finite(grow_scale3d) || !positive_finite(prune_scale3d))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: scene_scale, grow_scale3d and prune_scale3d must be finite and > 0");
+	if (!(prune_opacity > 0.0 && prune_opacity < 1.0))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: prune_opacity must be in (0, 1)");
+	if (std::isnan(grad_threshold) || std::isnan(grow_scale2d) || std::isnan(prune_scale2d))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_count: grad_threshold, grow_scale2d and prune_scale2d must not be NaN");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(densify_count(state, P, log_scales, opacity_logit, grad2d, count, radius, scene_scale, grad_threshold, grow_scale3d,
+	                       grow_scale2d, prune_opacity, prune_scale3d, prune_scale2d, prune_too_big, out_counts, st));
+	MGS_STAGE("densify_count");
+	return 0;
+}
+
+// the new tensors of a row list: with n_new > 0 the array and every pointer are required
+static int new_list(const char* what, int count, float* const* ptrs, int n_new)
+{
+	using namespace mgs;
+	if (count <= 0 || n_new == 0) return 0;
+	const std::string w = std::string("mgs_densify_emit: ") + what + ": every new pointer is required with n_new > 0";
+	if (!ptrs) return fail(MGS_ERR_INVALID_ARG, w);
+	for (int k = 0; k < count; k++)
+		if (!ptrs[k]) return fail(MGS_ERR_INVALID_ARG, w);
+	return 0;
+}
+
+int mgs_densify_emit(void* state, int P, int n_new, const float* means, const float* quats, const float* log_scales,
+	const float* opacity_logit, int num_rows, const float* const* rows, const int* row_widths, int num_moments,
+	const float* const* moments, const int* moment_widths, float* new_means, float* new_quats, float* new_log_scales,
+	float* new_opacity_logit, float* const* new_rows, float* const* new_moments, long long* rng, long long* out_source, int debug,
+	void* stream)
+{
+	using namespace mgs;
+	if (P < 0 || n_new < 0) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_emit: P and n_new must be >= 0");
+	if (P == 0 && n_new > 0) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_emit: n_new must be 0 with P = 0");
+	if (!state || !rng) return fail(MGS_ERR_INVALID_ARG, "mgs_densify_emit: state and rng are required");
+	if (P > 0 && (!means || !quats || !log_scales || !opacity_logit))
+		return fail(MGS_ERR_INVALID_ARG, "mgs_densify_emit: means, quats, log_scales and opacity_logit are required with P > 0");
+	if (n_new > 0 && (!new_means || !new_quats || !new_log_scales || !new_opacity_logit || !out_source))
+		return fail(MGS_ERR_INVALID_ARG,
+		            "mgs_densify_emit: new_means, new_quats, new_log_scales, new_opacity_logit and out_source are required with n_new > 0");
+	if (row_list("mgs_densify_emit", "rows", num_rows, MGS_MCMC_MAX_ROWS, rows, row_widths, P) < 0) return MGS_ERR_INVALID_ARG;
+	if (row_list("mgs_densify_emit", "moments", num_moments, MGS_MCMC_MAX_MOMENTS, moments, moment_widths, P) < 0)
+		return MGS_ERR_INVALID_ARG;
+	if (new_list("rows", num_rows, new_rows, n_new) < 0 || new_list("moments", num_moments, new_moments, n_new) < 0)
+		return MGS_ERR_INVALID_ARG;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	MGS_CUDA(densify_emit(state, P, means, quats, log_scales, opacity_logit, num_rows, rows, row_widths, num_moments, moments,
+	                      moment_widths, new_means, new_quats, new_log_scales, new_opacity_logit, new_rows, new_moments, rng, out_source,
+	                      st));
+	MGS_STAGE("densify_emit");
 	return 0;
 }
 

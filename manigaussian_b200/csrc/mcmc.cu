@@ -19,6 +19,7 @@
 #include "../../include/mgs_rasterizer.h"
 #include "mgs_common.cuh"
 #include "mgs_kernels.h"
+#include "philox.cuh"
 
 namespace mgs {
 
@@ -27,26 +28,6 @@ constexpr int MCMC_MAX_TENSORS = 4 + MGS_MCMC_MAX_ROWS + MGS_MCMC_MAX_MOMENTS;
 constexpr int MCMC_N_MAX = 51;            // gsplat's clamp of n = m + 1
 constexpr uint32_t MCMC_TAG_RELOCATE = 0;  // counter word 3: relocation and perturbation never share a draw
 constexpr uint32_t MCMC_TAG_PERTURB = 1;
-
-// ---------------------------------------------------------------------------------------------------------------- Philox
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1)
-{
-#pragma unroll
-	for (int r = 0; r < 10; r++) {
-		if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-		const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-		const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-		c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-	}
-	return c;
-}
-
-// the words of slot `slot` at the generator state rng = {seed, offset} (device int64 [2])
-__device__ __forceinline__ uint4 mcmc_draw(const long long* rng, uint32_t slot, uint32_t tag)
-{
-	const unsigned long long seed = (unsigned long long)rng[0], off = (unsigned long long)rng[1];
-	return philox4x32_10(make_uint4(slot, (uint32_t)off, (uint32_t)(off >> 32), tag), (uint32_t)seed, (uint32_t)(seed >> 32));
-}
 
 // ---------------------------------------------------------------------------------------------------------------- relocation
 struct McmcTensors {
@@ -81,7 +62,7 @@ __global__ void __launch_bounds__(MCMC_THREADS) mcmc_draw_kernel(int P_old, int 
 	long long src = -1;
 	const unsigned long long T = P_old > 0 ? S[P_old - 1] : 0ull;
 	if (j < P && T > 0 && mcmc_dest(j, P_old, x, t)) {
-		const uint4 w = mcmc_draw(rng, (uint32_t)j, MCMC_TAG_RELOCATE);
+		const uint4 w = philox_draw(rng, (uint32_t)j, MCMC_TAG_RELOCATE);
 		const unsigned long long u = __umul64hi(((unsigned long long)w.y << 32) | w.x, T);  // u < T
 		int lo = 0, hi = P_old - 1;  // S[hi] = T > u
 		while (lo < hi) {
@@ -230,14 +211,8 @@ __global__ void __launch_bounds__(MCMC_THREADS) mcmc_perturb_kernel(int P, float
 {
 	const int i = blockIdx.x * MCMC_THREADS + threadIdx.x;
 	if (i >= P) return;
-	const uint4 w = mcmc_draw(rng, (uint32_t)i, MCMC_TAG_PERTURB);
-	// Box-Muller in fp32: (w0, w1) give z0 and z1, (w2, w3) give z2
-	const float r0 = sqrtf(-2.f * logf(((float)w.x + 1.f) * 2.3283064365386963e-10f));
-	const float r1 = sqrtf(-2.f * logf(((float)w.z + 1.f) * 2.3283064365386963e-10f));
-	float s0, c0, s1, c1;
-	sincospif(2.f * ((float)w.y * 2.3283064365386963e-10f), &s0, &c0);
-	sincospif(2.f * ((float)w.w * 2.3283064365386963e-10f), &s1, &c1);
-	const float z0 = r0 * c0, z1 = r0 * s0, z2 = r1 * c1;
+	float z0, z1, z2;
+	philox_normals(philox_draw(rng, (uint32_t)i, MCMC_TAG_PERTURB), z0, z1, z2);
 
 	float4 q = quats[i];
 	const float inv = 1.f / fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);

@@ -650,6 +650,26 @@ cudaError_t mcmc_relocate(void* state, int P_old, int P, float min_opacity, floa
 cudaError_t mcmc_perturb(int P, float* means, const float* quats, const float* log_scales, const float* opacity_logit,
 	const float* scale, long long* rng, cudaStream_t st);
 
+// densify.cu: default density control (include/mgs_rasterizer.h, mgs_densify_stats / _count / _emit).  The statistics
+// take the views in launches of up to DENSIFY_VIEW_CHUNK, each view's max(W, H) by value.  The state (densify_state_bytes)
+// holds each Gaussian's flags, their inclusive int4 scan and CUB's scan scratch; emit reads what count left there.
+constexpr int DENSIFY_VIEW_CHUNK = 64;
+struct DensifyViews {
+	int V;
+	float size[DENSIFY_VIEW_CHUNK];  // max(W, H) of each view of the launch
+};
+cudaError_t densify_stats(int V, int P, const float* viewspace_grad, const int* radii, const int* sizes, float scale,
+	const float* scale_device, float* grad2d, int* count, float* radius, cudaStream_t st);
+cudaError_t densify_state_bytes(int P, size_t* bytes);
+cudaError_t densify_count(void* state, int P, const float* log_scales, const float* opacity_logit, const float* grad2d,
+	const int* count, const float* radius, double scene_scale, float grad_threshold, double grow_scale3d, float grow_scale2d,
+	double prune_opacity, double prune_scale3d, float prune_scale2d, int prune_too_big, long long* out_counts, cudaStream_t st);
+cudaError_t densify_emit(void* state, int P, const float* means, const float* quats, const float* log_scales,
+	const float* opacity_logit, int num_rows, const float* const* rows, const int* row_widths, int num_moments,
+	const float* const* moments, const int* moment_widths, float* new_means, float* new_quats, float* new_log_scales,
+	float* new_opacity_logit, float* const* new_rows, float* const* new_moments, long long* rng, long long* out_source,
+	cudaStream_t st);
+
 // tsdf.cu: depth images fused into an [X,Y,Z] volume (include/mgs_rasterizer.h, mgs_tsdf_fuse), one thread per voxel over
 // the up to TSDF_CHUNK views of one launch, in order.  Every pointer is that of the launch's first view; view u's depth
 // starts at u H W and its colour at u C H W.  The kernel parameters exceed 4 KB (CUDA 12.1+ accepts up to 32,764 bytes).

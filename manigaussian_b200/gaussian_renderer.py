@@ -1341,6 +1341,39 @@ def _mcmc_logit(min_opacity):
     return float(torch.tensor(math.log(min_opacity / (1.0 - min_opacity)), dtype=torch.float32))
 
 
+def _check_leaves(where, params):
+    for name, t in params.items():
+        if not t.is_leaf:
+            raise ValueError(f"{where}: params[{name!r}] is not a leaf tensor: an optimizer can only hold leaves")
+
+
+def _swap_params(params, optimizer, new, new_moment):
+    """Put the tensors of `new` ({name: tensor}, a new row count) into `params` in place of the tensors of the same names,
+    as Parameters where those were and with their requires_grad, and into the optimizer's param groups and state: each
+    state tensor shaped like its parameter becomes new_moment(name, key, old tensor), every other entry (Adam's step) is
+    kept.  This is what gsplat's _update_param_with_optimizer does."""
+    wrapped = {}
+    for name, q in new.items():
+        p = params[name]
+        wrapped[name] = torch.nn.Parameter(q, p.requires_grad) if isinstance(p, torch.nn.Parameter) else q.requires_grad_(p.requires_grad)
+    if optimizer is not None:
+        names = {id(p): name for name, p in params.items()}
+        for group in optimizer.param_groups:
+            for k, p in enumerate(group["params"]):
+                name = names.get(id(p))
+                if name not in wrapped:
+                    continue
+                q = wrapped[name]
+                state = optimizer.state.pop(p, None)
+                if state is not None:
+                    for key, v in state.items():
+                        if torch.is_tensor(v) and v.shape == p.shape:
+                            state[key] = new_moment(name, key, v)
+                    optimizer.state[q] = state
+                group["params"][k] = q
+    params.update(wrapped)
+
+
 def mcmc_relocate(params, optimizer=None, n=None, min_opacity=0.005, *, rng):
     """MCMC relocation and growth (3DGS as Markov chain Monte Carlo, Kheradmand et al. 2024, as gsplat's MCMCStrategy runs it;
     INTEGRATION.md §23; definition in include/mgs_rasterizer.h, mgs_mcmc_relocate), in place on the device.
@@ -1379,35 +1412,17 @@ def mcmc_relocate(params, optimizer=None, n=None, min_opacity=0.005, *, rng):
     if isinstance(min_opacity, bool) or not isinstance(min_opacity, (int, float)) or not 0.0 < min_opacity < 1.0:
         raise ValueError(f"{where}: min_opacity must be a number in (0, 1), got {min_opacity!r}")
     _mcmc_rng(where, rng, device)
-    names = {}
     if optimizer is not None:
-        for name, t in params.items():
-            if not t.is_leaf:
-                raise ValueError(f"{where}: params[{name!r}] is not a leaf tensor: an optimizer can only hold leaves")
-            names[id(t)] = name
+        _check_leaves(where, params)
     if n > P:
         grown = {}
         for name, p in params.items():
             ext = torch.zeros((n - P,) + tuple(p.shape[1:]), dtype=p.dtype, device=device)
             if name == "opacity":
                 ext.fill_(_mcmc_logit(min_opacity))
-            q = torch.cat([p.detach(), ext])
-            grown[name] = torch.nn.Parameter(q, p.requires_grad) if isinstance(p, torch.nn.Parameter) else q.requires_grad_(p.requires_grad)
-        if optimizer is not None:
-            for group in optimizer.param_groups:
-                for k, p in enumerate(group["params"]):
-                    name = names.get(id(p))
-                    if name is None:
-                        continue
-                    q = grown[name]
-                    state = optimizer.state.pop(p, None)
-                    if state is not None:
-                        for key, v in state.items():
-                            if torch.is_tensor(v) and v.shape == p.shape:
-                                state[key] = torch.cat([v, torch.zeros((n - P,) + tuple(v.shape[1:]), dtype=v.dtype, device=v.device)])
-                        optimizer.state[q] = state
-                    group["params"][k] = q
-        params.update(grown)
+            grown[name] = torch.cat([p.detach(), ext])
+        _swap_params(params, optimizer, grown, lambda name, key, v: torch.cat(
+            [v, torch.zeros((n - P,) + tuple(v.shape[1:]), dtype=v.dtype, device=v.device)]))
     moments = []
     if optimizer is not None:
         for name, p in params.items():
@@ -1450,6 +1465,191 @@ def mcmc_perturb(pts_xyz, rotations, scales, opacity, scale, rng):
     from .rasterizer import mcmc_perturb_raw
     mcmc_perturb_raw(pts_xyz.detach(), rotations.detach(), scales.detach(), opacity.detach(), scale.detach(), rng)
     return pts_xyz
+
+
+def densify_state(P, device):
+    """Zeroed statistics for densify_stats / densify_and_prune: {"grad2d": [P] float32, "count": [P] int32, "radius": [P]
+    float32} on `device`."""
+    return {"grad2d": torch.zeros(P, dtype=torch.float32, device=device),
+            "count": torch.zeros(P, dtype=torch.int32, device=device),
+            "radius": torch.zeros(P, dtype=torch.float32, device=device)}
+
+
+_DENSIFY_STATS = (("grad2d", torch.float32), ("count", torch.int32), ("radius", torch.float32))
+
+
+def _densify_check_stats(where, stats, P, device):
+    if not isinstance(stats, dict) or any(k not in stats for k, _ in _DENSIFY_STATS):
+        raise ValueError(f"{where}: stats: expected a dict with keys grad2d, count and radius (densify_state makes one)")
+    for k, dt in _DENSIFY_STATS:
+        t = stats[k]
+        if not torch.is_tensor(t) or tuple(t.shape) != (P,) or t.dtype != dt or t.device != device or not t.is_contiguous():
+            got = (t.dtype, tuple(t.shape), str(t.device)) if torch.is_tensor(t) else type(t)
+            raise ValueError(f"{where}: stats[{k!r}]: expected a contiguous {dt} [{P}] tensor on {device}, got {got}")
+
+
+def _densify_sizes(where, sizes, V):
+    """each view's max(W, H) as V host ints, from ints, a CameraBatch or a sequence of rasterization settings"""
+    if isinstance(sizes, CameraBatch):
+        out = [max(int(sizes.width), int(sizes.height))] * len(sizes)
+    elif isinstance(sizes, int) and not isinstance(sizes, bool):
+        out = [sizes] * V
+    else:
+        try:
+            out = [max(int(s.image_width), int(s.image_height)) if hasattr(s, "image_width") else s for s in sizes]
+        except TypeError:
+            raise ValueError(f"{where}: sizes: expected ints, a CameraBatch or a sequence of settings, got {type(sizes)}") from None
+    if len(out) != V or any(isinstance(s, bool) or not isinstance(s, int) or s <= 0 for s in out):
+        raise ValueError(f"{where}: sizes: expected {V} positive ints (each view's max(W, H)), got {out!r}")
+    return out
+
+
+def densify_stats(stats, viewspace_grad, radii, sizes, scale=1.0):
+    """Accumulate the statistics of default density control (3DGS's adaptive density control as gsplat's DefaultStrategy
+    runs it; INTEGRATION.md §24; definition in include/mgs_rasterizer.h, mgs_densify_stats), in place, once per step.
+    stats: densify_state(P, device)'s dict.  viewspace_grad: [V,P,3] (render_views' viewspace_points.grad) or [P,3]
+    (render's), float32; radii: [V,P] or [P] int32, the renders' "radii".  sizes: each view's max(W, H): ints (one int for
+    every view), a CameraBatch, or a sequence of GaussianRasterizationSettings.  For each Gaussian, over the views in order
+    where its radius is > 0: grad2d += |(gx, gy)| scale, count += 1, radius = max(radius, radii / max(W, H)), every
+    operation in fp32 without FMA.  scale: a number or a float32 device tensor of one element; a loss averaged over V
+    views has per-view gradients 1/V as large, so pass V (gsplat's n_cameras factor).
+    One thread per Gaussian and no atomics: bitwise repeatable.  Nothing is read back to the host, so the call can be
+    captured in a CUDA graph beside the training step.  Returns stats.  Raises ValueError on a bad stats dict, shape,
+    dtype, device, size or scale."""
+    where = "densify_stats"
+    if not torch.is_tensor(viewspace_grad) or viewspace_grad.dim() not in (2, 3) or viewspace_grad.shape[-1] != 3:
+        got = tuple(viewspace_grad.shape) if torch.is_tensor(viewspace_grad) else type(viewspace_grad)
+        raise ValueError(f"{where}: viewspace_grad: expected [V,P,3] or [P,3] (viewspace_points.grad), got {got}")
+    if viewspace_grad.dtype != torch.float32:
+        raise ValueError(f"{where}: viewspace_grad: expected float32, got {viewspace_grad.dtype}")
+    g = viewspace_grad.detach()
+    g = g if g.dim() == 3 else g[None]
+    V, P, device = int(g.shape[0]), int(g.shape[1]), g.device
+    if not torch.is_tensor(radii) or tuple(radii.shape) not in ((V, P),) + (((P,),) if viewspace_grad.dim() == 2 else ()):
+        got = tuple(radii.shape) if torch.is_tensor(radii) else type(radii)
+        raise ValueError(f"{where}: radii: expected [{V},{P}]" + (f" or [{P}]" if viewspace_grad.dim() == 2 else "") + f", got {got}")
+    if radii.dtype != torch.int32 or radii.device != device:
+        raise ValueError(f"{where}: radii: expected int32 on {device}, got {radii.dtype} on {radii.device}")
+    _densify_check_stats(where, stats, P, device)
+    sz = _densify_sizes(where, sizes, V)
+    if torch.is_tensor(scale):
+        if scale.dtype != torch.float32 or scale.numel() != 1 or scale.device != device:
+            raise ValueError(f"{where}: scale: expected a float32 tensor of one element on {device}, got "
+                             f"{scale.dtype} {tuple(scale.shape)} on {scale.device}")
+        scale = scale.detach()
+    elif isinstance(scale, bool) or not isinstance(scale, (int, float)) or not math.isfinite(scale):
+        raise ValueError(f"{where}: scale: expected a finite number or a device tensor, got {scale!r}")
+    from .rasterizer import densify_stats_raw
+    densify_stats_raw(g.contiguous(), radii.detach().reshape(V, P).contiguous(), sz, stats["grad2d"], stats["count"],
+                      stats["radius"], scale)
+    return stats
+
+
+def _positive(where, name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not (math.isfinite(v) and v > 0):
+        raise ValueError(f"{where}: {name} must be a finite number > 0, got {v!r}")
+
+
+def densify_and_prune(params, stats, optimizer=None, *, scene_scale, grad_threshold=2e-4, grow_scale3d=0.01, grow_scale2d=None,
+                      prune_opacity=0.005, prune_scale3d=0.1, prune_scale2d=None, prune_too_big=False, rng):
+    """One refinement of default density control (INTEGRATION.md §24; definition in include/mgs_rasterizer.h,
+    mgs_densify_count / mgs_densify_emit): gsplat's DefaultStrategy duplicate, then split, then prune, on the device.
+    params: mcmc_relocate's dict ("pts_xyz" [P,3], "rotations" [P,4], "scales" [P,3] log, "opacity" [P] or [P,1] logits,
+    plus up to 16 further rows [P, ...]); stats: densify_stats' dict for the same P.
+    With L the largest log scale and g = grad2d / max(count, 1): g > grad_threshold clones a Gaussian whose
+    exp(L) <= grow_scale3d * scene_scale and splits the others; with grow_scale2d (None: off) a radius above it also splits.
+    A split Gaussian is replaced by two children with scales / 1.6 and means drawn from its own Gaussian (Philox from rng).
+    Every row (original, clone, child) with opacity below prune_opacity is removed, and with prune_too_big also one with
+    exp(L) > prune_scale3d * scene_scale or (with prune_scale2d) a radius above prune_scale2d.  Rows come out as
+    [kept originals] ++ [kept clones] ++ [kept first children] ++ [kept second children], each in ascending index.
+    optimizer: a torch.optim optimizer over (some of) the params, or None: each state tensor shaped like its parameter
+    (Adam's moments) keeps its rows for the kept originals and is zero for new rows; the params dict, the optimizer's param
+    groups and state and `stats` get new tensors of the new length, and `stats` is zeroed (gsplat resets it after each
+    refinement).  When nothing is cloned, split or pruned no tensor is replaced and only `stats` is zeroed.
+    rng: int64 [2] = {seed, offset} on the params' device; the offset advances by one on the device per call.
+    Returns {"source": [n_new] int64, each row's parent index (for labels and neighbour lists), "counts": {"n_new",
+    "cloned", "split", "pruned"} host ints} with n_new = P + cloned + split - pruned.  The result is bitwise repeatable,
+    so the ranks of a view-parallel run that reduce their statistics (INTEGRATION.md §24) make the same refinement.
+    One device->host read per call, of the four totals that size the new tensors.  Not differentiable.
+    Raises ValueError on a bad params or stats dict, shape, dtype, device or contiguity, a threshold out of range, too many
+    rows or moments, a bad rng, and non-leaf params with an optimizer; RuntimeError when n_new would exceed 2^31 - 1."""
+    where = "densify_and_prune"
+    if not isinstance(params, dict) or any(k not in params for k, _ in _MCMC_BASE):
+        raise ValueError(f"{where}: params: expected a dict with keys {', '.join(k for k, _ in _MCMC_BASE)} (and any further rows)")
+    x = params["pts_xyz"]
+    _mcmc_tensor(where, "params['pts_xyz']", x, None, None, 3)
+    P, device = int(x.shape[0]), x.device
+    widths = dict(_MCMC_BASE)
+    for name, t in params.items():
+        _mcmc_tensor(where, f"params[{name!r}]", t, P, device, widths.get(name))
+    extra = [k for k in params if k not in widths]
+    if len(extra) > _MCMC_MAX_ROWS:
+        raise ValueError(f"{where}: params: at most {_MCMC_MAX_ROWS} rows besides the four parameters, got {len(extra)}")
+    _densify_check_stats(where, stats, P, device)
+    for name, v in (("scene_scale", scene_scale), ("grow_scale3d", grow_scale3d), ("prune_scale3d", prune_scale3d)):
+        _positive(where, name, v)
+    if isinstance(prune_opacity, bool) or not isinstance(prune_opacity, (int, float)) or not 0.0 < prune_opacity < 1.0:
+        raise ValueError(f"{where}: prune_opacity must be a number in (0, 1), got {prune_opacity!r}")
+    if isinstance(grad_threshold, bool) or not isinstance(grad_threshold, (int, float)) or math.isnan(grad_threshold):
+        raise ValueError(f"{where}: grad_threshold must be a number, got {grad_threshold!r}")
+    for name, v in (("grow_scale2d", grow_scale2d), ("prune_scale2d", prune_scale2d)):
+        if v is not None and (isinstance(v, bool) or not isinstance(v, (int, float)) or math.isnan(v)):
+            raise ValueError(f"{where}: {name} must be a number or None, got {v!r}")
+    _mcmc_rng(where, rng, device)
+    if optimizer is not None:
+        _check_leaves(where, params)
+    moments, keys = [], []
+    if optimizer is not None:
+        for name, p in params.items():
+            for key, v in optimizer.state.get(p, {}).items():
+                if torch.is_tensor(v) and v.shape == p.shape:
+                    _mcmc_tensor(where, f"optimizer state {key!r} of params[{name!r}]", v, P, device)
+                    moments.append(v)
+                    keys.append((name, key))
+    if len(moments) > _MCMC_MAX_MOMENTS:
+        raise ValueError(f"{where}: optimizer: at most {_MCMC_MAX_MOMENTS} moment tensors, got {len(moments)}")
+    from .rasterizer import densify_and_prune_raw
+    d = {k: v.detach() for k, v in params.items()}
+    totals, out = densify_and_prune_raw(
+        d["pts_xyz"], d["rotations"], d["scales"], d["opacity"], [d[k] for k in extra], moments, stats["grad2d"],
+        stats["count"], stats["radius"], rng, float(scene_scale), float(grad_threshold), float(grow_scale3d),
+        math.inf if grow_scale2d is None else float(grow_scale2d), float(prune_opacity), float(prune_scale3d),
+        math.inf if prune_scale2d is None else float(prune_scale2d), bool(prune_too_big))
+    counts = dict(zip(("n_new", "cloned", "split", "pruned"), totals))
+    if out is None:
+        rng[1:].add_(1)  # what the emit would have done
+        for t in stats.values():
+            t.zero_()
+        return {"source": torch.arange(P, dtype=torch.int64, device=device), "counts": counts}
+    means, quats, log_scales, opacity, new_rows, new_moments, source = out
+    new = dict(zip(("pts_xyz", "rotations", "scales", "opacity"), (means, quats, log_scales, opacity)))
+    new.update(zip(extra, new_rows))
+    by_key = dict(zip(keys, new_moments))
+    _swap_params(params, optimizer, new, lambda name, key, v: by_key[(name, key)])
+    stats.update(densify_state(counts["n_new"], device))
+    return {"source": source, "counts": counts}
+
+
+def densify_reset_opacity(params, optimizer=None, value=0.01):
+    """Default density control's opacity reset (INTEGRATION.md §24), in place: params["opacity"] (logits) becomes
+    min(opacity, fp32(logit(value))) and that parameter's optimizer moments (state tensors shaped like it) are zeroed, as
+    gsplat's reset_opa does.  Two torch ops per tensor, no kernel of its own and no host read.  Returns params["opacity"].
+    Raises ValueError on a missing or bad "opacity" tensor and a value outside (0, 1)."""
+    where = "densify_reset_opacity"
+    if not isinstance(params, dict) or "opacity" not in params:
+        raise ValueError(f"{where}: params: expected a dict with key opacity")
+    x = params["opacity"]
+    if not torch.is_tensor(x) or x.dtype != torch.float32:
+        raise ValueError(f"{where}: params['opacity']: expected a float32 tensor, got {x.dtype if torch.is_tensor(x) else type(x)}")
+    if isinstance(value, bool) or not isinstance(value, (int, float)) or not 0.0 < value < 1.0:
+        raise ValueError(f"{where}: value must be a number in (0, 1), got {value!r}")
+    with torch.no_grad():
+        x.clamp_(max=_mcmc_logit(value))
+    if optimizer is not None:
+        for v in optimizer.state.get(x, {}).values():
+            if torch.is_tensor(v) and v.shape == x.shape:
+                v.zero_()
+    return x
 
 
 _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, opacities, scales, rotations

@@ -16,6 +16,7 @@ median-depth plane and each pixel's surface Gaussian, and `return_normal=True` t
 from typing import NamedTuple
 
 import ctypes
+import math
 import os
 
 import torch
@@ -2207,3 +2208,69 @@ def mcmc_perturb_raw(means, quats, log_scales, opacity_logit, scale, rng, debug=
         _b.check(L.mgs_mcmc_perturb(means.shape[0], _ptr(means), _ptr(quats), _ptr(log_scales), _ptr(opacity_logit), _ptr(scale),
                                     _ptr(rng), int(bool(debug)), _stream(dev)), "mgs_mcmc_perturb")
     return means
+
+
+def densify_stats_raw(viewspace_grad, radii, sizes, grad2d, count, radius, scale=1.0, debug=False):
+    """Density-control statistics in place (C ABI mgs_densify_stats; definition in include/mgs_rasterizer.h):
+    viewspace_grad [V,P,3] float32, radii [V,P] int32, sizes: V host ints (each view's max(W, H)), grad2d [P] float32,
+    count [P] int32 and radius [P] float32 (updated), all contiguous on one device.  scale: a number, or a float32 tensor of
+    one element on the device.  Nothing is read back to the host, so a call can be captured in a CUDA graph."""
+    if not viewspace_grad.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = viewspace_grad.device
+    V, P = int(viewspace_grad.shape[0]), int(viewspace_grad.shape[1])
+    sz = (ctypes.c_int * max(V, 1))(*[int(s) for s in sizes])
+    dscale = scale if torch.is_tensor(scale) else None
+    with torch.cuda.device(dev):
+        _b.check(L.mgs_densify_stats(V, P, _ptr(viewspace_grad), _ptr(radii), sz, 1.0 if dscale is not None else float(scale),
+                                     _ptr(dscale), _ptr(grad2d), _ptr(count), _ptr(radius), int(bool(debug)), _stream(dev)),
+                 "mgs_densify_stats")
+
+
+def densify_and_prune_raw(means, quats, log_scales, opacity_logit, rows, moments, grad2d, count, radius, rng, scene_scale,
+                          grad_threshold=2e-4, grow_scale3d=0.01, grow_scale2d=math.inf, prune_opacity=0.005,
+                          prune_scale3d=0.1, prune_scale2d=math.inf, prune_too_big=False, debug=False):
+    """Clone, split and prune (C ABI mgs_densify_count / mgs_densify_emit; definition in include/mgs_rasterizer.h): means
+    [P,3], quats [P,4], log_scales [P,3], opacity_logit [P] or [P,1], every tensor of `rows` and `moments` [P, ...], all
+    float32 and contiguous, and the statistics grad2d [P], count [P] int32, radius [P] on one device; grow_scale2d and
+    prune_scale2d take math.inf for no test.  rng: device int64 [2] = {seed, offset}; emit advances the offset by one on
+    the device.  One device->host read of the four totals sizes the outputs.  Returns (counts (n_new, cloned, split,
+    pruned) as host ints, or None when nothing is cloned, split or pruned (then nothing is enqueued after the count),
+    else (new means, quats, log_scales, opacity_logit, [new rows], [new moments], source [n_new] int64))."""
+    if not means.is_cuda:
+        raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
+    L = _b.lib()
+    dev = means.device
+    P = int(means.shape[0])
+    counts = torch.empty(4, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):  # the state's size depends on the device it is used on
+        nbytes = int(L.mgs_densify_state_bytes(P))
+        if nbytes == 0:
+            raise RuntimeError("mgs_densify_state_bytes: " + _b.last_error())
+        state = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _b.check(L.mgs_densify_count(_ptr(state), P, _ptr(log_scales), _ptr(opacity_logit), _ptr(grad2d), _ptr(count),
+                                     _ptr(radius), float(scene_scale), float(grad_threshold), float(grow_scale3d),
+                                     float(grow_scale2d), float(prune_opacity), float(prune_scale3d), float(prune_scale2d),
+                                     int(bool(prune_too_big)), _ptr(counts), int(bool(debug)), _stream(dev)), "mgs_densify_count")
+        totals = tuple(int(n) for n in counts.cpu())
+        n_new, cloned, split, pruned = totals
+        if cloned == 0 and split == 0 and pruned == 0:
+            return totals, None
+        if n_new > 2 ** 31 - 1:
+            raise RuntimeError(f"densify_and_prune: {n_new} Gaussians after refinement exceed the 2^31 - 1 the kernels index")
+
+        def grown(t):
+            return torch.empty((n_new,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+
+        new = [grown(t) for t in (means, quats, log_scales, opacity_logit)]
+        new_rows, new_moments = [grown(t) for t in rows], [grown(t) for t in moments]
+        source = torch.empty(n_new, dtype=torch.int64, device=dev)
+        nr, rp, rw = _pointer_list(rows)
+        nm, mp, mw = _pointer_list(moments)
+        _, nrp, _ = _pointer_list(new_rows)
+        _, nmp, _ = _pointer_list(new_moments)
+        _b.check(L.mgs_densify_emit(_ptr(state), P, n_new, _ptr(means), _ptr(quats), _ptr(log_scales), _ptr(opacity_logit),
+                                    nr, rp, rw, nm, mp, mw, *[_ptr(t) for t in new], nrp, nmp, _ptr(rng), _ptr(source),
+                                    int(bool(debug)), _stream(dev)), "mgs_densify_emit")
+    return totals, (*new, new_rows, new_moments, source)
