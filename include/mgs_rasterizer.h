@@ -194,6 +194,9 @@ int mgs_backward(
  * and `join_stream` waits for every view stream before the call returns, so the caller needs no stream logic of its own
  * (a view whose stream IS join_stream is simply serialised).  Nothing in these calls allocates or blocks: a step built
  * from them can be captured in a CUDA graph.
+ * mgs_forward_views and mgs_backward_views are the one-cloud form of mgs_forward_clouds and mgs_backward_clouds (below):
+ * the same code runs them with view_offsets = {0, V}.  Only the views backward has `stages` and `shared_mean2D`, and its
+ * per-Gaussian launches run their own kernel, built for more blocks per SM than the clouds kernel.
  * mgs_backward_views runs the blend backward of every view on its stream, joins, and runs ONE per-Gaussian chain-rule
  * kernel that sums over the views in registers: outputs are the SUMS over the V views (the packed buffer of the
  * multi-GPU all-reduce can be passed directly), except dL_dmean2D which each view owns ([P,3], shared_mean2D = 0) or

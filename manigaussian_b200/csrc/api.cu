@@ -858,82 +858,6 @@ static int enqueue_flow_bwd(const Cloud& c, const mgs_view* views, const mgs_vie
 	return 0;
 }
 
-// stages bit 0: the blend backward of every view on its stream, then the join; bit 1: the per-Gaussian chain rule on
-// `join`, one launch per MAX_BWD_VIEWS views summed in registers.  dL_dconic (or NULL) is written only by a launch that
-// does not accumulate, i.e. the first one when `accumulate` is 0: single-view callers only.  alpha, dm, ssim: V entries or NULL;
-// lens: V entries.
-static int backward_views(int V, const mgs_view* views, const mgs_view_alpha* alpha, const mgs_view_depth_mask* dm,
-	const mgs_view_ssim* ssim, const mgs_view_camera_grad* cam, const mgs_view_intrinsics* intr, const mgs_view_median* med,
-	const mgs_view_normal* nm, const Lens* lens, const Cloud& c, float* dL_dmean3D,
-	float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dconic, int shared_mean2D,
-	int accumulate, int stages, int debug, cudaStream_t join, const mgs_view_flow* fl = nullptr, const float* flow_means3D = nullptr,
-	float* dL_dflow = nullptr)
-{
-	const int P = c.P, F = c.F;
-	std::vector<mgs_view_normal> flow_planes;
-	const mgs_view_normal* blend_nm = flow_blend_planes(fl, V, nm, flow_planes);  // a flow plane rides in the normal plane's columns
-	bool flow_bwd = false;  // a view has a flow cotangent
-	for (int v = 0; v < V; v++) flow_bwd |= flow_on(fl, v) && fl[v].dL_dpix_flow;
-	if (stages & 1) {
-		if (F > 0 && !accumulate) MGS_CUDA(cudaMemsetAsync(dL_dfeature, 0, (size_t)P * F * sizeof(float), join));
-		int rc = fork_streams(V, views, join);
-		if (rc < 0) return rc;
-		for (int v = 0; v < V; v++) {
-			mgs_view w = views[v];
-			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
-			if (rc == 0)
-				rc = enqueue_blend_bwd(c, w, dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr, dm ? dm + v : nullptr,
-					med ? med + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
-			if (rc < 0) return rc;
-		}
-		rc = join_streams(V, views, join);
-		if (rc < 0) return rc;
-	}  // blend stage: dL_dfeature is final here -- a caller may start exchanging it while the per-Gaussian stage runs
-	if (!(stages & 2)) return 0;
-	// the chain to scale / rotation runs when either gradient is asked for; without scales (cov3D_precomp) the rows
-	// asked for are written as zeros.  shs are read whether or not dL_dsh is asked for: they carry the view-direction
-	// term of dL_dmean3D.
-	const bool have_sr = c.scales && c.rotations && (dL_dscale || dL_drot);
-	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
-		cudaStream_t st = join;
-		ProjectBwdViewsArgs pb{};
-		pb.P = P; pb.D = c.D; pb.M = c.M; pb.V = std::min(V - v0, (int)MAX_BWD_VIEWS);
-		pb.means3D = c.means3D; pb.shs = c.shs;
-		pb.scales = have_sr ? c.scales : nullptr; pb.rotations = c.rotations; pb.scale_modifier = c.scale_modifier;
-		pb.cov3D_precomp = c.cov3D_precomp;
-		if (!have_sr && !c.cov3D_precomp) {
-			// gradients w.r.t. scale/rotation not requested: the forward's own covariance (any view's copy) serves
-			pb.cov3D_precomp = carve_view(views[0], P).geom.cov3D;
-		}
-		pb.accumulate = (accumulate || v0 > 0) ? 1 : 0;
-		pb.shared_mean2D = shared_mean2D;
-		pb.dL_dmean3D = dL_dmean3D; pb.dL_dopacity = dL_dopacity; pb.dL_dcolor = dL_dcolor; pb.dL_dcov3D = dL_dcov3D;
-		pb.dL_dsh = dL_dsh; pb.dL_dscale = dL_dscale; pb.dL_drot = dL_drot;
-		pb.dL_dconic = pb.accumulate ? nullptr : dL_dconic;
-		for (int u = 0; u < pb.V; u++)
-			pb.view[u] = bwd_view(views[v0 + u], P, shared_mean2D ? views[0].dL_dmean2D : views[v0 + u].dL_dmean2D);
-		pb.antialias = c.antialias;
-		for (int u = 0; u < pb.V && c.antialias; u++) pb.conic_opacity[u] = carve_view(views[v0 + u], P).geom.conic_opacity;
-		bool flow_reduced = false;  // the flow's camera terms already hold the camera outputs
-		if (flow_bwd) {
-			const int rc = enqueue_flow_bwd(c, views, fl, flow_means3D, dL_dflow, cam, intr, lens, v0, pb.V,
-				(accumulate || v0 > 0) ? 1 : 0, accumulate ? 1 : 0, debug, st, flow_reduced);
-			if (rc < 0) return rc;
-		}
-		CamReduceArgs cr{};
-		cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
-		for (int u = 0; u < pb.V; u++) camera_view(cam, intr, views[v0 + u], v0 + u, P, pb.cam_rows[u], pb.intr[u], cr);
-		for (int u = 0; u < pb.V; u++) bwd_lens(pb, u, lens[v0 + u]);
-		for (int u = 0; u < pb.V; u++) planar_view(c, views[v0 + u], pb.pl_g[u], pb.pl_q[u], pb.pl_mean[u]);
-		// the camera reduce is timed with the launch it completes: the stage list ends with the SSIM stages
-		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_views(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
-		MGS_STAGE("project_bwd");
-		const int rc = enqueue_normals_bwd(c, views, nm, v0, pb.V, dL_drot, debug, st);
-		if (rc < 0) return rc;
-	}
-	return 0;
-}
-
 // first half of a single-view forward (P > 0): checks the projection inputs, allocates the geometry and image state,
 // enqueues the projection stage and copies the instance count to *host_count asynchronously on the view's stream
 static int project_single_view(const Cloud& c, mgs_view& w, mgs_alloc_fn geometry_alloc, void* geometry_user, mgs_alloc_fn image_alloc,
@@ -1008,6 +932,185 @@ static int check_planar(int planar_depth, const mgs_view_normal* normal, int V)
 	return 0;
 }
 
+
+// NULL options: every optional input off
+static const mgs_render_options no_options{};
+// the next-frame means of cloud b (flow_next: one entry per cloud, or NULL)
+static const float* cloud_next(const mgs_cloud_flow* fc, int b) { return fc ? fc[b].means3D : nullptr; }
+
+// one per-Gaussian launch of the backward.  A views call (one cloud) runs the views kernel: it is built for more blocks per SM
+// than the clouds kernel, and only it takes shared_mean2D and dL_dconic (written when the launch does not accumulate)
+static void launch_project_bwd(const ProjectBwdCloudsDistArgs& pb, bool views_call, int shared_mean2D, float* dL_dconic,
+	cudaStream_t st)
+{
+	if (!views_call) { launch_project_bwd_clouds(pb, st); return; }
+	const ProjectBwdCloud& k = pb.cloud[0];
+	ProjectBwdViewsArgs a{};
+	a.P = k.P; a.D = pb.D; a.M = pb.M; a.V = k.V;
+	a.means3D = k.means3D; a.shs = k.shs; a.scales = k.scales; a.rotations = k.rotations; a.scale_modifier = pb.scale_modifier;
+	a.cov3D_precomp = k.cov3D_precomp; a.accumulate = k.accumulate; a.shared_mean2D = shared_mean2D;
+	a.dL_dmean3D = k.dL_dmean3D; a.dL_dopacity = k.dL_dopacity; a.dL_dcolor = k.dL_dcolor; a.dL_dcov3D = k.dL_dcov3D;
+	a.dL_dsh = k.dL_dsh; a.dL_dscale = k.dL_dscale; a.dL_drot = k.dL_drot; a.dL_dconic = k.accumulate ? nullptr : dL_dconic;
+	a.antialias = pb.antialias; a.ortho = pb.ortho; a.fisheye = pb.fisheye; a.distorted = pb.distorted;
+	for (int u = 0; u < k.V; u++) {
+		a.view[u] = pb.view[u]; a.conic_opacity[u] = pb.conic_opacity[u]; a.cam_rows[u] = pb.cam_rows[u]; a.intr[u] = pb.intr[u];
+		a.fe_k[u] = pb.fe_k[u]; a.dc_k[u] = pb.dc_k[u]; a.pl_g[u] = pb.pl_g[u]; a.pl_q[u] = pb.pl_q[u]; a.pl_mean[u] = pb.pl_mean[u];
+	}
+	launch_project_bwd_views(a, st);
+}
+
+// the backward of mgs_backward_clouds, and of mgs_backward_views and mgs_backward as its one-cloud form.  views_call: the
+// one-cloud form, whose per-Gaussian launches run the views kernel, which keeps the view-direction term of dL_dmean3D
+// without dL_dsh (the clouds kernel needs dL_dsh with shs).  Inputs only a views call has: stages (bit 0: the blend backward
+// of every view on its stream, then the join; bit 1: the per-Gaussian stage on join_stream), shared_mean2D (every view's
+// dL_dmean2D is summed into the first view's) and dL_dconic (single-view callers).
+static int backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
+	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream,
+	bool views_call, int stages = 3, int shared_mean2D = 0, float* dL_dconic = nullptr)
+{
+	const mgs_render_options& o = options ? *options : no_options;
+	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
+	const mgs_view_camera_grad* cam = o.camera_grad; const mgs_view_intrinsics* intr = o.intrinsics;
+	const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
+	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye;
+	const mgs_view_distortion* distortion = o.distortion; const mgs_view_flow* flow = o.flow;
+	const mgs_cloud_flow* flow_clouds = o.flow_next;
+	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
+	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
+	int rc = check_clouds(B, clouds, view_offsets, views);
+	if (rc < 0) return rc;
+	std::vector<Lens> lens;
+	if (view_lenses(ortho, fisheye, distortion, view_offsets[B], lens) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
+	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
+	for (int b = 0; b < B; b++)
+		if (check_flow(flow, cloud_next(flow_clouds, b), view_offsets[b], view_offsets[b + 1], depth_mask) < 0) return MGS_ERR_INVALID_ARG;
+	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		if (!k.means3D || !k.dL_dmean3D || !k.dL_dopacity)
+			return fail(MGS_ERR_INVALID_ARG, "cloud: means3D, dL_dmean3D and dL_dopacity are required");
+		if (!views_call && k.shs && !k.dL_dsh)
+			return fail(MGS_ERR_INVALID_ARG, "cloud: dL_dsh is required with SHs (it carries the view-direction term of dL_dmean3D)");
+		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+			rc = check_bwd_view(views[v], F > 0 && k.feature);
+			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
+			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
+			if (rc == 0) rc = check_median(median ? median + v : nullptr);
+			if (rc == 0)
+				rc = check_normal(views[v], normal ? normal + v : nullptr, k.scales, k.rotations, k.cov3D_precomp,
+					depth_mask ? depth_mask + v : nullptr);
+			if (rc < 0) return rc;
+		}
+	}
+	const int V = view_offsets[B];
+	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
+	const cudaStream_t st = reinterpret_cast<cudaStream_t>(join_stream);
+	if (stages & 1) {
+		for (int b = 0; b < B; b++) {
+			const mgs_cloud& k = clouds[b];
+			if (F > 0 && k.feature && k.dL_dfeature && !accumulate)
+				MGS_CUDA(cudaMemsetAsync(k.dL_dfeature, 0, (size_t)k.P * F * sizeof(float), st));
+		}
+		std::vector<mgs_view_normal> flow_planes;
+		const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);  // a flow plane rides in the normal plane's columns
+		rc = fork_streams(V, views, st);
+		if (rc < 0) return rc;
+		for (int b = 0; b < B; b++) {
+			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
+			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
+				mgs_view w = views[v];
+				rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
+				if (rc == 0)
+					rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
+						depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
+				if (rc < 0) return rc;
+			}
+		}
+		rc = join_streams(V, views, st);
+		if (rc < 0) return rc;
+	}  // blend stage: dL_dfeature is final here -- a caller may start exchanging it while the per-Gaussian stage runs
+	if (!(stages & 2)) return 0;
+
+	// per-Gaussian stage on the join stream: launches of at most MAX_BWD_VIEWS views that pack whole clouds; a cloud with more
+	// views spans launches, and its later launches add to what the earlier ones wrote.
+	// The flow planes' backward first, one launch per cloud and MAX_BWD_VIEWS of its views: it adds to the blend-stage records
+	// the per-Gaussian stage reads, and its camera reduce writes the camera outputs the per-Gaussian stage's reduce adds to
+	bool flow_bwd = false, flow_reduced = false;
+	for (int v = 0; v < V; v++) flow_bwd |= flow_on(flow, v) && flow[v].dL_dpix_flow;
+	for (int b = 0; b < B && flow_bwd; b++) {
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			bool red = false;
+			rc = enqueue_flow_bwd(c, views, flow, cloud_next(flow_clouds, b), flow_clouds ? flow_clouds[b].dL_dmeans3D : nullptr, cam, intr,
+				lens.data(), v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS),
+				(accumulate || v0 > view_offsets[b]) ? 1 : 0, accumulate ? 1 : 0, debug, st, red);
+			if (rc < 0) return rc;
+			flow_reduced |= red;
+		}
+	}
+	// a view's camera rows are summed by the reduce behind the one launch that holds the view
+	ProjectBwdCloudsDistArgs pb{};
+	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
+	CamReduceArgs cr{};
+	cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
+	int nv = 0;  // views in pb
+	auto flush = [&]() -> int {
+		if (pb.B == 0) return 0;
+		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd(pb, views_call, shared_mean2D, dL_dconic, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
+		MGS_STAGE("project_bwd");
+		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0; pb.fisheye = 0; pb.distorted = 0;
+		for (float*& r : pb.cam_rows) r = nullptr;
+		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
+		for (int u = 0; u < MAX_BWD_VIEWS; u++) { pb.pl_g[u] = nullptr; pb.pl_q[u] = nullptr; pb.pl_mean[u] = nullptr; }
+		return 0;
+	};
+	for (int b = 0; b < B; b++) {
+		const mgs_cloud& k = clouds[b];
+		// the chain to scale / rotation runs when either gradient is asked for; without scales (cov3D_precomp) the rows asked
+		// for are written as zeros.  shs are read whether or not dL_dsh is asked for: they carry the view-direction term of
+		// dL_dmean3D.
+		const bool have_sr = k.scales && k.rotations && (k.dL_dscale || k.dL_drot);
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			const int n = std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS);
+			if (nv + n > MAX_BWD_VIEWS) {
+				rc = flush();
+				if (rc < 0) return rc;
+			}
+			ProjectBwdCloud& pc = pb.cloud[pb.B++];
+			pc.P = k.P; pc.V = n; pc.view0 = nv;
+			pc.means3D = k.means3D; pc.shs = k.shs; pc.scales = have_sr ? k.scales : nullptr; pc.rotations = k.rotations;
+			// gradients w.r.t. scale/rotation not requested: the forward's own covariance (any view's copy) serves
+			pc.cov3D_precomp = (have_sr || k.cov3D_precomp) ? k.cov3D_precomp : carve_view(views[view_offsets[b]], k.P).geom.cov3D;
+			pc.accumulate = (accumulate || v0 > view_offsets[b]) ? 1 : 0;
+			pc.dL_dmean3D = k.dL_dmean3D; pc.dL_dopacity = k.dL_dopacity; pc.dL_dcolor = k.dL_dcolor; pc.dL_dcov3D = k.dL_dcov3D;
+			pc.dL_dsh = k.dL_dsh; pc.dL_dscale = k.dL_dscale; pc.dL_drot = k.dL_drot;
+			for (int u = 0; u < n; u++) {
+				const mgs_view& w = views[v0 + u];
+				pb.view[nv + u] = bwd_view(w, k.P, shared_mean2D ? views[view_offsets[b]].dL_dmean2D : w.dL_dmean2D);
+				pb.conic_opacity[nv + u] = antialiasing ? carve_view(w, k.P).geom.conic_opacity : nullptr;
+				camera_view(cam, intr, w, v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
+				bwd_lens(pb, nv + u, lens[v0 + u]);
+				planar_view(cloud_of(k, D, M, F, scale_modifier, antialiasing, planar_depth), w, pb.pl_g[nv + u], pb.pl_q[nv + u],
+					pb.pl_mean[nv + u]);
+			}
+			nv += n;
+		}
+	}
+	rc = flush();
+	if (rc < 0) return rc;
+	// the normal planes' share of every cloud's dL_drot, behind the launches that wrote it: one launch per cloud and
+	// MAX_BWD_VIEWS of its views
+	for (int b = 0; b < B && normal; b++) {
+		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
+		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
+			rc = enqueue_normals_bwd(c, views, normal, v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS), clouds[b].dL_drot,
+				debug, st);
+			if (rc < 0) return rc;
+		}
+	}
+	return 0;
+}
 
 }  // namespace mgs
 
@@ -1095,7 +1198,8 @@ int mgs_backward(
 		return fail(MGS_ERR_INVALID_ARG, "state buffers and scratch are required");
 	if (!dL_dpix || !dL_dmean2D || !dL_dopacity || !dL_dmean3D || !means3D || !radii || !background)
 		return fail(MGS_ERR_INVALID_ARG, "required pointer is NULL");
-	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp };
+	const mgs_cloud k{ P, means3D, shs, colors_precomp, F > 0 ? feature_precomp : nullptr, nullptr, scales, rotations, cov3D_precomp,
+		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot };
 	mgs_view w{};
 	w.viewmatrix = viewmatrix; w.projmatrix = projmatrix; w.cam_pos = campos; w.background = background;
 	w.tan_fovx = tan_fovx; w.tan_fovy = tan_fovy; w.width = width; w.height = height;
@@ -1103,16 +1207,11 @@ int mgs_backward(
 	w.radii = const_cast<int*>(radii);  // read only by the backward
 	w.dL_dpix = dL_dpix; w.dL_dpix_F = dL_dpix_F; w.dL_dpix_depth = dL_dpix_depth;
 	w.blend_scratch = blend_scratch; w.dL_dmean2D = dL_dmean2D; w.stream = stream;
-	const Lens pinhole{};
-	return backward_views(1, &w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &pinhole, c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dconic,
-		1, accumulate, 3, debug, reinterpret_cast<cudaStream_t>(stream));
+	const int view_offsets[2] = { 0, 1 };
+	return backward_clouds(1, &k, view_offsets, &w, nullptr, D, M, F, scale_modifier, accumulate, debug, stream, true, 3, 1, dL_dconic);
 }
 
-// NULL options: every optional input off
-static const mgs_render_options no_options{};
-// the next-frame means of cloud b (flow_next: one entry per cloud, or NULL)
-static const float* cloud_next(const mgs_cloud_flow* fc, int b) { return fc ? fc[b].means3D : nullptr; }
-
+// the one-cloud form of mgs_forward_clouds
 int mgs_forward_views(
 	int V, const mgs_view* views, const mgs_render_options* options,
 	int P, int D, int M, int F,
@@ -1120,66 +1219,10 @@ int mgs_forward_views(
 	const float* opacities, const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp,
 	int prefiltered, int debug, void* join_stream)
 {
-	const mgs_render_options& o = options ? *options : no_options;
-	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
-	const mgs_view_intrinsics* intr = o.intrinsics; const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
-	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye; const mgs_view_distortion* distortion = o.distortion;
-	const mgs_view_flow* flow = o.flow; const float* flow_means3D = cloud_next(o.flow_next, 0);
-	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
-	(void)prefiltered;
-	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
-	if (check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0)
-		return MGS_ERR_INVALID_ARG;
-	std::vector<Lens> lens;
-	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
-	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
-	if (!means3D || !opacities) return fail(MGS_ERR_INVALID_ARG, "means3D/opacities are required");
-	if (!colors_precomp && !shs) return fail(MGS_ERR_INVALID_ARG, "provide SHs or precomputed colours");
-	if (!cov3D_precomp && (!scales || !rotations)) return fail(MGS_ERR_INVALID_ARG, "provide scales+rotations or a precomputed 3D covariance");
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS || !blend_supported(F)) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
-	for (int v = 0; v < V; v++) {
-		int rc = check_fwd_view(views[v], !colors_precomp);
-		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, true);
-		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, true);
-		if (rc == 0) rc = check_median(median ? median + v : nullptr);
-		if (rc == 0) rc = check_normal(views[v], normal ? normal + v : nullptr, scales, rotations, cov3D_precomp, depth_mask ? depth_mask + v : nullptr);
-		if (rc < 0) return rc;
-	}
-	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-		antialiasing, planar_depth };
-	std::vector<mgs_view_normal> flow_planes;
-	const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);
-	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
-	int rc = fork_streams(V, views, join);
-	if (rc < 0) return rc;
-	// stage by stage across the views: the short per-Gaussian and binning kernels of every view are enqueued before any
-	// view's long blend kernel, so no view's chain queues behind another view's blend
-	for (int phase = 0; phase < 3; phase++) {
-		// MGS_BLEND_BARRIER=1: all blends start together, after the binning chain of EVERY view.  A blend launch is one
-		// wave of small CTAs that takes every shared-memory slot of the GPU, and the short binning kernels of the
-		// other views crawl behind it (CTA timeline, tools/cta_timeline.py: blends 0 and 1 each run alone, 790 us for the
-		// four forward blends of the bench step; started together 590 us) -- but four binning chains side by side take
-		// 0.38 ms instead of 0.22 ms for the first alone, and the step time comes out the same (2.21 ms either way,
-		// DESIGN.md section 7), so the default keeps the dependency-free schedule.
-		if (phase == 2 && barrier_before_blend()) {
-			rc = cross_wait_streams(V, views);
-			if (rc < 0) return rc;
-		}
-		for (int v = 0; v < V; v++) {
-			rc = phase == 0 ? enqueue_project(c, views[v], device_fov(intr, v), lens[v], debug)
-				: phase == 1 ? enqueue_binning(c, views[v], false, debug)
-				: enqueue_blend_fwd(c, views[v], alpha ? alpha[v].out_alpha : nullptr, depth_mask ? depth_mask + v : nullptr,
-					median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
-			if (rc == 0 && phase == 0) rc = enqueue_normals_fwd(c, views[v], normal ? normal + v : nullptr, debug);
-			if (rc == 0 && phase == 0)
-				rc = enqueue_flow_fwd(c, views[v], flow ? flow + v : nullptr, flow_means3D, device_fov(intr, v), lens[v], debug);
-			if (rc == 0 && phase == 2) rc = enqueue_ssim_fwd(views[v], ssim ? ssim + v : nullptr, debug);
-			if (rc < 0) return rc;
-		}
-	}
-	return join_streams(V, views, join);
+	const mgs_cloud k{ P, means3D, shs, colors_precomp, feature_precomp, opacities, scales, rotations, cov3D_precomp };
+	const int view_offsets[2] = { 0, V };
+	return mgs_forward_clouds(1, &k, view_offsets, views, options, D, M, F, scale_modifier, prefiltered, debug, join_stream);
 }
 
 int mgs_lift_views(
@@ -1472,7 +1515,7 @@ int mgs_visibility_views_backward(
 		MGS_STAGE("visibility_points_bwd");
 	}
 	if (!gauss) return 0;
-	// the per-Gaussian chain of the render's backward (backward_views' stage 2) over the views' gb
+	// the per-Gaussian chain of the render's backward (backward_clouds' per-Gaussian stage) over the views' gb
 	const bool have_sr = c.scales && c.rotations && (dL_dscale || dL_drot);
 	for (int v0 = 0; v0 < V; v0 += MAX_BWD_VIEWS) {
 		ProjectBwdViewsArgs pb{};
@@ -1610,6 +1653,8 @@ int mgs_camera_rays_backward(int V, const mgs_view* views, const mgs_view_intrin
 	return 0;
 }
 
+// the one-cloud form of mgs_backward_clouds, with the stage split and the shared dL_dmean2D.  Features are off for the whole
+// call without feature_precomp or dL_dfeature, and shs need no dL_dsh.
 int mgs_backward_views(
 	int V, const mgs_view* views, const mgs_render_options* options,
 	int P, int D, int M, int F,
@@ -1618,40 +1663,13 @@ int mgs_backward_views(
 	float* dL_dmean3D, float* dL_dopacity, float* dL_dcolor, float* dL_dfeature, float* dL_dcov3D, float* dL_dsh,
 	float* dL_dscale, float* dL_drot, int shared_mean2D, int accumulate, int stages, int debug, void* join_stream)
 {
-	const mgs_render_options& o = options ? *options : no_options;
-	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
-	const mgs_view_camera_grad* cam = o.camera_grad; const mgs_view_intrinsics* intr = o.intrinsics;
-	const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
-	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye;
-	const mgs_view_distortion* distortion = o.distortion; const mgs_view_flow* flow = o.flow;
-	const float* flow_means3D = cloud_next(o.flow_next, 0);
-	float* dL_dflow_means3D = o.flow_next ? o.flow_next[0].dL_dmeans3D : nullptr;
-	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
-	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
-	if (V > 0 && views && check_planar(planar_depth, normal, V) < 0) return MGS_ERR_INVALID_ARG;
-	if (V > 0 && views && (check_flow_call(flow, V, planar_depth, normal) < 0 || check_flow(flow, flow_means3D, 0, V, depth_mask) < 0))
-		return MGS_ERR_INVALID_ARG;
 	if (!(stages & 3)) return fail(MGS_ERR_INVALID_ARG, "stages must name the blend stage (1), the per-Gaussian stage (2) or both (3)");
 	if (V <= 0 || !views) return fail(MGS_ERR_INVALID_ARG, "need at least one view");
-	std::vector<Lens> lens;
-	if (view_lenses(ortho, fisheye, distortion, V, lens) < 0) return MGS_ERR_INVALID_ARG;
-	if (P <= 0) return fail(MGS_ERR_INVALID_ARG, "P must be > 0");
-	if (!means3D || !dL_dmean3D || !dL_dopacity) return fail(MGS_ERR_INVALID_ARG, "means3D, dL_dmean3D and dL_dopacity are required");
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
-	if (F > 0 && (!feature_precomp || !dL_dfeature)) F = 0;
-	for (int v = 0; v < V; v++) {
-		int rc = check_bwd_view(views[v], F > 0);
-		if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
-		if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
-		if (rc == 0) rc = check_median(median ? median + v : nullptr);
-		if (rc == 0) rc = check_normal(views[v], normal ? normal + v : nullptr, scales, rotations, cov3D_precomp, depth_mask ? depth_mask + v : nullptr);
-		if (rc < 0) return rc;
-	}
-	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
-	const Cloud c{ P, D, M, F, means3D, shs, colors_precomp, feature_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp,
-		antialiasing, planar_depth };
-	return backward_views(V, views, alpha, depth_mask, ssim, cam, intr, median, normal, lens.data(), c, dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, nullptr,
-		shared_mean2D, accumulate, stages, debug, reinterpret_cast<cudaStream_t>(join_stream), flow, flow_means3D, dL_dflow_means3D);
+	const mgs_cloud k{ P, means3D, shs, colors_precomp, dL_dfeature ? feature_precomp : nullptr, nullptr, scales, rotations, cov3D_precomp,
+		dL_dmean3D, dL_dopacity, dL_dcolor, dL_dfeature, dL_dcov3D, dL_dsh, dL_dscale, dL_drot };
+	const int view_offsets[2] = { 0, V };
+	return backward_clouds(1, &k, view_offsets, views, options, D, M, F, scale_modifier, accumulate, debug, join_stream, true, stages,
+		shared_mean2D, nullptr);
 }
 
 int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
@@ -1697,8 +1715,19 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
 	rc = fork_streams(V, views, join);
 	if (rc < 0) return rc;
-	// stage by stage across the views of every cloud, as in mgs_forward_views
+	// stage by stage across the views of every cloud: the short per-Gaussian and binning kernels of every view are enqueued
+	// before any view's long blend kernel, so no view's chain queues behind another view's blend
 	for (int phase = 0; phase < 3; phase++) {
+		// MGS_BLEND_BARRIER=1: all blends start together, after the binning chain of EVERY view.  A blend launch is one
+		// wave of small CTAs that takes every shared-memory slot of the GPU, and the short binning kernels of the
+		// other views crawl behind it (CTA timeline, tools/cta_timeline.py: blends 0 and 1 each run alone, 790 us for the
+		// four forward blends of the bench step; started together 590 us) -- but four binning chains side by side take
+		// 0.38 ms instead of 0.22 ms for the first alone, and the step time comes out the same (2.21 ms either way,
+		// DESIGN.md section 7), so the default keeps the dependency-free schedule.
+		if (phase == 2 && barrier_before_blend()) {
+			rc = cross_wait_streams(V, views);
+			if (rc < 0) return rc;
+		}
 		for (int b = 0; b < B; b++) {
 			const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
 			for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
@@ -1720,142 +1749,7 @@ int mgs_forward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, 
 int mgs_backward_clouds(int B, const mgs_cloud* clouds, const int* view_offsets, const mgs_view* views,
 	const mgs_render_options* options, int D, int M, int F, float scale_modifier, int accumulate, int debug, void* join_stream)
 {
-	const mgs_render_options& o = options ? *options : no_options;
-	const mgs_view_alpha* alpha = o.alpha; const mgs_view_depth_mask* depth_mask = o.depth_mask; const mgs_view_ssim* ssim = o.ssim;
-	const mgs_view_camera_grad* cam = o.camera_grad; const mgs_view_intrinsics* intr = o.intrinsics;
-	const mgs_view_median* median = o.median; const mgs_view_normal* normal = o.normal;
-	const int* ortho = o.ortho; const mgs_view_fisheye* fisheye = o.fisheye;
-	const mgs_view_distortion* distortion = o.distortion; const mgs_view_flow* flow = o.flow;
-	const mgs_cloud_flow* flow_clouds = o.flow_next;
-	const int antialiasing = o.antialiasing, planar_depth = o.planar_depth;
-	if (check_antialias(antialiasing) < 0) return MGS_ERR_INVALID_ARG;
-	int rc = check_clouds(B, clouds, view_offsets, views);
-	if (rc < 0) return rc;
-	std::vector<Lens> lens;
-	if (view_lenses(ortho, fisheye, distortion, view_offsets[B], lens) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_planar(planar_depth, normal, view_offsets[B]) < 0) return MGS_ERR_INVALID_ARG;
-	if (check_flow_call(flow, view_offsets[B], planar_depth, normal) < 0) return MGS_ERR_INVALID_ARG;
-	for (int b = 0; b < B; b++)
-		if (check_flow(flow, cloud_next(flow_clouds, b), view_offsets[b], view_offsets[b + 1], depth_mask) < 0) return MGS_ERR_INVALID_ARG;
-	if (F < 0 || F > MGS_MAX_FEATURE_CHANNELS) return fail(MGS_ERR_UNSUPPORTED, bad_width_msg);
-	for (int b = 0; b < B; b++) {
-		const mgs_cloud& k = clouds[b];
-		if (!k.means3D || !k.dL_dmean3D || !k.dL_dopacity)
-			return fail(MGS_ERR_INVALID_ARG, "cloud: means3D, dL_dmean3D and dL_dopacity are required");
-		if (k.shs && !k.dL_dsh)
-			return fail(MGS_ERR_INVALID_ARG, "cloud: dL_dsh is required with SHs (it carries the view-direction term of dL_dmean3D)");
-		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-			rc = check_bwd_view(views[v], F > 0 && k.feature);
-			if (rc == 0) rc = check_depth_mask(views[v], depth_mask ? depth_mask + v : nullptr, false);
-			if (rc == 0) rc = check_ssim(views[v], ssim ? ssim + v : nullptr, false);
-			if (rc == 0) rc = check_median(median ? median + v : nullptr);
-			if (rc == 0)
-				rc = check_normal(views[v], normal ? normal + v : nullptr, k.scales, k.rotations, k.cov3D_precomp,
-					depth_mask ? depth_mask + v : nullptr);
-			if (rc < 0) return rc;
-		}
-	}
-	const int V = view_offsets[B];
-	if (check_camera(cam, intr, V) < 0) return MGS_ERR_INVALID_ARG;
-	cudaStream_t join = reinterpret_cast<cudaStream_t>(join_stream);
-	for (int b = 0; b < B; b++) {
-		const mgs_cloud& k = clouds[b];
-		if (F > 0 && k.feature && k.dL_dfeature && !accumulate)
-			MGS_CUDA(cudaMemsetAsync(k.dL_dfeature, 0, (size_t)k.P * F * sizeof(float), join));
-	}
-	std::vector<mgs_view_normal> flow_planes;
-	const mgs_view_normal* blend_nm = flow_blend_planes(flow, V, normal, flow_planes);
-	rc = fork_streams(V, views, join);
-	if (rc < 0) return rc;
-	for (int b = 0; b < B; b++) {
-		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing, planar_depth);
-		for (int v = view_offsets[b]; v < view_offsets[b + 1]; v++) {
-			mgs_view w = views[v];
-			rc = enqueue_ssim_bwd(w, ssim ? ssim + v : nullptr, debug);
-			if (rc == 0)
-				rc = enqueue_blend_bwd(c, w, clouds[b].dL_dfeature, alpha ? alpha[v].dL_dpix_alpha : nullptr,
-					depth_mask ? depth_mask + v : nullptr, median ? median + v : nullptr, blend_nm ? blend_nm + v : nullptr, debug);
-			if (rc < 0) return rc;
-		}
-	}
-	rc = join_streams(V, views, join);
-	if (rc < 0) return rc;
-
-	// per-Gaussian stage on `join`: launches of at most MAX_BWD_VIEWS views that pack whole clouds; a cloud with more views
-	// spans launches, and its later launches add to what the earlier ones wrote
-	const cudaStream_t st = join;
-	// the flow planes' backward first, one launch per cloud and MAX_BWD_VIEWS of its views: it adds to the blend-stage records
-	// the per-Gaussian stage reads, and its camera reduce writes the camera outputs the per-Gaussian stage's reduce adds to
-	bool flow_bwd = false, flow_reduced = false;
-	for (int v = 0; v < V; v++) flow_bwd |= flow_on(flow, v) && flow[v].dL_dpix_flow;
-	for (int b = 0; b < B && flow_bwd; b++) {
-		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
-		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
-			bool red = false;
-			rc = enqueue_flow_bwd(c, views, flow, cloud_next(flow_clouds, b), flow_clouds ? flow_clouds[b].dL_dmeans3D : nullptr, cam, intr,
-				lens.data(), v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS),
-				(accumulate || v0 > view_offsets[b]) ? 1 : 0, accumulate ? 1 : 0, debug, st, red);
-			if (rc < 0) return rc;
-			flow_reduced |= red;
-		}
-	}
-	// a view's camera rows are summed by the reduce behind the one launch that holds the view
-	ProjectBwdCloudsDistArgs pb{};
-	pb.D = D; pb.M = M; pb.scale_modifier = scale_modifier; pb.antialias = antialiasing;
-	CamReduceArgs cr{};
-	cr.accumulate = (accumulate || flow_reduced) ? 1 : 0;
-	int nv = 0;  // views in pb
-	auto flush = [&]() -> int {
-		if (pb.B == 0) return 0;
-		{ StageTimer t_(ST_PROJECT_BWD, st); launch_project_bwd_clouds(pb, st); if (cr.V > 0) launch_camera_grad_reduce(cr, st); }
-		MGS_STAGE("project_bwd");
-		pb.B = 0; nv = 0; cr.V = 0; pb.ortho = 0; pb.fisheye = 0; pb.distorted = 0;
-		for (float*& r : pb.cam_rows) r = nullptr;
-		for (ProjectBwdIntr& ki : pb.intr) ki = ProjectBwdIntr{};
-		for (int u = 0; u < MAX_BWD_VIEWS; u++) { pb.pl_g[u] = nullptr; pb.pl_q[u] = nullptr; pb.pl_mean[u] = nullptr; }
-		return 0;
-	};
-	for (int b = 0; b < B; b++) {
-		const mgs_cloud& k = clouds[b];
-		const bool have_sr = k.scales && k.rotations && (k.dL_dscale || k.dL_drot);  // as in backward_views
-		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
-			const int n = std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS);
-			if (nv + n > MAX_BWD_VIEWS) {
-				rc = flush();
-				if (rc < 0) return rc;
-			}
-			ProjectBwdCloud& pc = pb.cloud[pb.B++];
-			pc.P = k.P; pc.V = n; pc.view0 = nv;
-			pc.means3D = k.means3D; pc.shs = k.shs; pc.scales = have_sr ? k.scales : nullptr; pc.rotations = k.rotations;
-			// gradients w.r.t. scale/rotation not requested: the forward's own covariance (any view's copy) serves
-			pc.cov3D_precomp = (have_sr || k.cov3D_precomp) ? k.cov3D_precomp : carve_view(views[view_offsets[b]], k.P).geom.cov3D;
-			pc.accumulate = (accumulate || v0 > view_offsets[b]) ? 1 : 0;
-			pc.dL_dmean3D = k.dL_dmean3D; pc.dL_dopacity = k.dL_dopacity; pc.dL_dcolor = k.dL_dcolor; pc.dL_dcov3D = k.dL_dcov3D;
-			pc.dL_dsh = k.dL_dsh; pc.dL_dscale = k.dL_dscale; pc.dL_drot = k.dL_drot;
-			for (int u = 0; u < n; u++) {
-				pb.view[nv + u] = bwd_view(views[v0 + u], k.P, views[v0 + u].dL_dmean2D);
-				pb.conic_opacity[nv + u] = antialiasing ? carve_view(views[v0 + u], k.P).geom.conic_opacity : nullptr;
-				camera_view(cam, intr, views[v0 + u], v0 + u, k.P, pb.cam_rows[nv + u], pb.intr[nv + u], cr);
-				bwd_lens(pb, nv + u, lens[v0 + u]);
-				planar_view(cloud_of(k, D, M, F, scale_modifier, antialiasing, planar_depth), views[v0 + u], pb.pl_g[nv + u], pb.pl_q[nv + u],
-					pb.pl_mean[nv + u]);
-			}
-			nv += n;
-		}
-	}
-	rc = flush();
-	if (rc < 0) return rc;
-	// the normal planes' share of every cloud's dL_drot, behind the launches that wrote it: one launch per cloud and
-	// MAX_BWD_VIEWS of its views
-	for (int b = 0; b < B && normal; b++) {
-		const Cloud c = cloud_of(clouds[b], D, M, F, scale_modifier, antialiasing);
-		for (int v0 = view_offsets[b]; v0 < view_offsets[b + 1]; v0 += MAX_BWD_VIEWS) {
-			rc = enqueue_normals_bwd(c, views, normal, v0, std::min(view_offsets[b + 1] - v0, (int)MAX_BWD_VIEWS), clouds[b].dL_drot,
-				debug, st);
-			if (rc < 0) return rc;
-		}
-	}
-	return 0;
+	return backward_clouds(B, clouds, view_offsets, views, options, D, M, F, scale_modifier, accumulate, debug, join_stream, false);
 }
 
 int mgs_loss_heads(int V, int F, int N, const float* color, const float* feature, const float* target_color,

@@ -233,108 +233,6 @@ def _camera_outputs(ctx, cam, first):
                  for i, (g, shape) in enumerate(zip(cam, shapes)))
 
 
-class _RasterizeViews(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, return_depth, return_alpha,
-                group, antialiasing=False, return_median=False, return_normal=False, cam_vm=None, cam_pm=None, cam_cp=None,
-                cam_tf=None, flow_xyz=None, flow_poses=None):
-        dev = means3D.device
-        V, P = len(views), means3D.shape[0]
-        H, W = int(views[0].image_height), int(views[0].image_width)
-        if any((int(s.image_height), int(s.image_width)) != (H, W) for s in views):
-            raise ValueError("render_views needs one image size for all views")
-        include = feature is not None and feature.numel() > 0
-        F = int(feature.shape[1]) if include else 0
-        means3D, sh, colors_precomp, feature = (_prep(t, dev) for t in (means3D, sh, colors_precomp, feature))
-        opacities, scales, rotations = (_prep(t, dev) for t in (opacities, scales, rotations))
-        opts = dict(dtype=torch.float32, device=dev)
-        color = torch.empty((V, 3, H, W), **opts)
-        feat_img = torch.empty((V, F, H, W), **opts) if include else None
-        depth = torch.empty((V, H, W), **opts) if return_depth else None
-        alpha = torch.empty((V, H, W), **opts) if return_alpha else None
-        med_depth = torch.empty((V, H, W), **opts) if return_median else None
-        med_id = torch.empty((V, H, W), dtype=torch.int32, device=dev) if return_median else None
-        normal = torch.empty((V, 3, H, W), **opts) if return_normal else None
-        flow = torch.empty((V, 3, H, W), **opts) if flow_xyz is not None else None
-        flow_xyz = flow_xyz.detach() if flow_xyz is not None else None
-        degree = views[0].sh_degree
-        outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
-                                            views[0].scale_modifier, None, sh, degree, include, return_depth=return_depth,
-                                            debug=views[0].debug,
-                                            out_buffers=(color, feat_img, depth, alpha, med_depth, med_id, normal, flow),
-                                            return_alpha=return_alpha, antialiasing=antialiasing, tan_fov=cam_tf,
-                                            return_median=return_median, return_normal=return_normal, flow_means3D=flow_xyz,
-                                            flow_poses=flow_poses)
-        main = torch.cuda.current_stream(dev)
-        for st in streams:
-            main.wait_stream(st)
-        radii = torch.stack([o[3] for o in outs])
-        ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
-        ctx.camera, ctx.tan_fov = cam_vm is not None, (cam_tf.detach() if cam_tf is not None else None)
-        ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]   # R, radii, geometry / binning / image state per view
-        ctx.include, ctx.F, ctx.return_depth, ctx.return_alpha, ctx.degree = include, F, return_depth, return_alpha, degree
-        ctx.opac_shape = opacities.shape
-        ctx.flow_poses = flow_poses
-        empty = torch.empty(0, device=dev)
-        # the id and normal planes are outputs: they reach the backward through save_for_backward (an output on ctx is a
-        # reference cycle)
-        ctx.save_for_backward(means3D, sh if sh is not None else empty, colors_precomp if colors_precomp is not None else empty,
-                              feature if include else empty, scales, rotations, med_id if return_median else empty,
-                              normal if return_normal else empty, flow if flow is not None else empty,
-                              flow_xyz if flow_xyz is not None else empty)
-        ctx.mark_non_differentiable(radii, *([med_id] if return_median else []))
-        return (color, (feat_img if include else empty), radii, (depth if return_depth else empty),
-                (alpha if return_alpha else empty), (med_depth if return_median else empty),
-                (med_id if return_median else empty), (normal if return_normal else empty),
-                (flow[:, :2] if flow is not None else empty))
-
-    @staticmethod
-    def backward(ctx, g_color, g_feat, _g_radii, g_depth, g_alpha, g_median, _g_median_id, g_normal, g_flow=None):
-        means3D, sh, colors_precomp, feature, scales, rotations, med_id, normal, flow, flow_xyz = ctx.saved_tensors
-        dev = means3D.device
-        views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
-        H, W = int(views[0].image_height), int(views[0].image_width)
-        M = sh.shape[1] if sh.numel() else 0
-        use_colors = colors_precomp.numel() > 0
-        if g_color is None:
-            g_color = torch.zeros((V, 3, H, W), dtype=torch.float32, device=dev)
-        if ctx.include and g_feat is None:
-            g_feat = torch.zeros((V, ctx.F, H, W), dtype=torch.float32, device=dev)
-        g_color = _prep(g_color, dev)
-        g_feat = _prep(g_feat, dev) if ctx.include else None
-        g_depth = _prep(g_depth, dev) if (ctx.return_depth and g_depth is not None and g_depth.numel()) else None
-        g_alpha = _prep(g_alpha, dev) if (ctx.return_alpha and g_alpha is not None and g_alpha.numel()) else None
-        g_median = _prep(g_median, dev) if (med_id.numel() and g_median is not None and g_median.numel()) else None
-        g_normal = _prep(g_normal, dev) if (normal.numel() and g_normal is not None and g_normal.numel()) else None
-        has_flow = flow_xyz.numel() > 0
-        if has_flow and g_flow is None:
-            g_flow = torch.zeros((V, 2, H, W), dtype=torch.float32, device=dev)
-        pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)  # every row is written by the backward
-        grp = None if ctx.group in (None, True) else ctx.group
-        m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
-        outs = [(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in ctx.state]
-        res = rasterize_views_backward_raw(views, outs, ctx.streams, g_color, g_feat, means3D, colors_precomp if use_colors else None,
-                                           feature if ctx.include else None, scales, rotations, views[0].scale_modifier, None,
-                                           sh if M else None, ctx.degree, ctx.include, grads_depth=g_depth, debug=views[0].debug,
-                                           accumulate_into=pk.views, means2D_per_view=m2d, grads_alpha=g_alpha,
-                                           after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
-                                           antialiasing=ctx.antialiasing, camera_grads=True if ctx.camera else None,
-                                           tan_fov=ctx.tan_fov, grads_median=g_median, median_ids=med_id if g_median is not None else None,
-                                           grads_normal=g_normal, normals=normal if g_normal is not None else None,
-                                           flow_means3D=flow_xyz if has_flow else None, flow_poses=ctx.flow_poses,
-                                           grads_flow=list(g_flow) if has_flow else None, flows=list(flow) if has_flow else None)
-        if ctx.group is not None:
-            # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
-            # (final after the blend stage) is already travelling while the per-Gaussian kernel produced the other fields.
-            # A view's camera gradients are complete on the rank that rendered it.
-            pk.all_reduce_finish(grp)
-        v = pk.views
-        return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
-                v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None,
-                *_camera_outputs(ctx, res[9] if ctx.camera else None, 15), res[-1] if has_flow else None, None)
-
-
 def _depth_mask_heads(t_depth, t_mask, V, H, W, dev, where="targets"):
     """The depth / mask heads' `depth_mask` tuple for the raw calls (targets [V,H,W], their cotangent planes, the [V,3]
     accumulator), or None when neither target is given."""
@@ -389,105 +287,6 @@ def _depth_mask_scale(dm, g_depth, g_mask, V, dev):
     z = torch.zeros((V,), dtype=torch.float32, device=dev)
     return torch.stack([g_depth if (dm[0] is not None and g_depth is not None) else z,
                         g_mask if (dm[1] is not None and g_mask is not None) else z], 1).contiguous()
-
-
-class _RasterizeViewsLoss(torch.autograd.Function):
-    """render_views with the loss heads fused into the forward blend's epilogue (SURVEY.md 8(f) row f4): returns the per-view
-    L2 colour loss and cosine embedding loss of NeuralRenderer.forward (neural_rendering.py:300-318, loss.py:12-23) and,
-    with depth / mask targets (row f7), the expected-depth L1 loss, the alpha mask BCE loss and the valid-pixel counts, and
-    with ssim (row f9) the L1 loss and the SSIM of the colour image; the images come back too, but gradients flow through the
-    losses only."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, feature, opacities, scales, rotations, views, target_rgb, target_embed, group,
-                target_depth=None, target_mask=None, antialiasing=False, ssim=False, cam_vm=None, cam_pm=None, cam_cp=None,
-                cam_tf=None):
-        dev = means3D.device
-        V, P = len(views), means3D.shape[0]
-        H, W = int(views[0].image_height), int(views[0].image_width)
-        if any((int(s.image_height), int(s.image_width)) != (H, W) for s in views):
-            raise ValueError("render_views needs one image size for all views")
-        include = feature is not None and feature.numel() > 0
-        F = int(feature.shape[1]) if include else 0
-        means3D, sh, colors_precomp, feature = (_prep(t, dev) for t in (means3D, sh, colors_precomp, feature))
-        opacities, scales, rotations = (_prep(t, dev) for t in (opacities, scales, rotations))
-        target_rgb = _prep(target_rgb, dev)
-        target_embed = _prep(target_embed, dev) if (include and target_embed is not None) else None
-        if tuple(target_rgb.shape) != (V, 3, H, W) or (target_embed is not None and tuple(target_embed.shape) != (V, F, H, W)):
-            raise ValueError("targets must be [V,3,H,W] and [V,F,H,W]")
-        opts = dict(dtype=torch.float32, device=dev)
-        color = torch.empty((V, 3, H, W), **opts)
-        feat_img = torch.empty((V, F, H, W), **opts) if include else None
-        cot_rgb = torch.empty((V, 3, H, W), **opts)
-        cot_embed = torch.empty((V, F, H, W), **opts) if target_embed is not None else (torch.zeros((V, F, H, W), **opts) if include else None)
-        loss_acc = torch.empty((V, 2), **opts)
-        dm = _depth_mask_heads(target_depth, target_mask, V, H, W, dev)
-        ssim_head = _ssim_head(V, H, W, dev) if ssim else None
-        degree = views[0].sh_degree
-        outs, streams = rasterize_views_raw(views, means3D, colors_precomp, feature, opacities, scales, rotations,
-                                            views[0].scale_modifier, None, sh, degree, include, debug=views[0].debug,
-                                            out_buffers=(color, feat_img, None),
-                                            loss_heads=(target_rgb, target_embed, cot_rgb, cot_embed, loss_acc), depth_mask=dm,
-                                            antialiasing=antialiasing, ssim=ssim_head, tan_fov=cam_tf)
-        N = float(H * W)
-        loss_rgb = loss_acc[:, 0] / (3.0 * N)
-        loss_embed = 1.0 - loss_acc[:, 1] / N if target_embed is not None else torch.zeros((V,), **opts)
-        radii = torch.stack([o[3] for o in outs])
-        ctx.views, ctx.streams, ctx.group, ctx.antialiasing = views, streams, group, antialiasing
-        ctx.camera, ctx.tan_fov = cam_vm is not None, (cam_tf.detach() if cam_tf is not None else None)
-        # capacity, radii and the three state buffers per view -- never the images: they are views of this node's outputs, and an
-        # output kept on ctx is a reference cycle (output -> grad_fn -> ctx -> output) that leaks the whole step
-        ctx.state = [(o[0], o[3], o[4], o[5], o[6]) for o in outs]
-        ctx.include, ctx.F, ctx.degree = include, F, degree
-        ctx.opac_shape = opacities.shape
-        ctx.cots = (cot_rgb, cot_embed)
-        ctx.dm = dm  # the targets, cotangent planes and accumulator of the depth / mask heads: none of them is an output
-        # the SSIM head's planes and accumulator, and the colour target (an input); the backward also reads the image, an
-        # output, which therefore goes through save_for_backward
-        ctx.ssim, ctx.target_rgb = ssim_head, (target_rgb if ssim else None)
-        ctx.save_for_backward(means3D, sh if sh is not None else torch.empty(0, device=dev),
-                              colors_precomp if colors_precomp is not None else torch.empty(0, device=dev),
-                              feature if include else torch.empty(0, device=dev), scales, rotations,
-                              color if ssim else torch.empty(0, device=dev))
-        empty = torch.empty(0, device=dev)
-        loss_depth, loss_mask, depth_pixels = _depth_mask_losses(dm, N, dev)
-        loss_l1, ssim_v = _ssim_losses(ssim_head, 3.0 * N, dev)
-        # ONE call: a second mark_non_differentiable replaces the first
-        ctx.mark_non_differentiable(radii, color, *([feat_img] if include else []), depth_pixels)
-        return (loss_rgb, loss_embed, color, (feat_img if include else empty), radii, loss_depth, loss_mask, depth_pixels, loss_l1,
-                ssim_v)
-
-    @staticmethod
-    def backward(ctx, g_rgb, g_embed, _gc, _gf, _gr, g_depth, g_mask, _gn, g_l1, g_ssim):
-        means3D, sh, colors_precomp, feature, scales, rotations, color = ctx.saved_tensors
-        dev = means3D.device
-        views, V, P = ctx.views, len(ctx.views), means3D.shape[0]
-        M = sh.shape[1] if sh.numel() else 0
-        use_colors = colors_precomp.numel() > 0
-        scale = _pair_scale(g_rgb, g_embed, V, dev)
-        cot_rgb, cot_embed = ctx.cots
-        pk = PackedGradients(P, ctx.F, M, dev, colors=use_colors, zero=False)
-        grp = None if ctx.group in (None, True) else ctx.group
-        m2d = torch.empty((V, P, 3), dtype=torch.float32, device=dev)
-        outs = [(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in ctx.state]
-        res = rasterize_views_backward_raw(views, outs, ctx.streams, cot_rgb, cot_embed if ctx.include else None, means3D,
-                                     colors_precomp if use_colors else None, feature if ctx.include else None, scales, rotations,
-                                     views[0].scale_modifier, None, sh if M else None, ctx.degree, ctx.include, debug=views[0].debug,
-                                     accumulate_into=pk.views, means2D_per_view=m2d, cot_scale=scale,
-                                     after_blend=(lambda: pk.all_reduce_begin(grp)) if ctx.group is not None else None,
-                                     depth_mask=ctx.dm,
-                                     depth_mask_scale=_depth_mask_scale(ctx.dm, g_depth, g_mask, V, dev) if ctx.dm is not None else None,
-                                     antialiasing=ctx.antialiasing,
-                                     ssim=ctx.ssim + (color, ctx.target_rgb) if ctx.ssim is not None else None,
-                                     ssim_scale=_pair_scale(g_l1, g_ssim, V, dev) if ctx.ssim is not None else None,
-                                     camera_grads=True if ctx.camera else None, tan_fov=ctx.tan_fov)
-        if ctx.group is not None:
-            pk.all_reduce_finish(grp)
-        v = pk.views
-        return (v["dL_dmeans3D"], m2d, v.get("dL_dsh").view(P, M, 3) if M else None, v.get("dL_dcolors"),
-                v.get("dL_dfeature") if ctx.include else None, v["dL_dopacity"].view(ctx.opac_shape),
-                v["dL_dscales"], v["dL_drotations"], None, None, None, None, None, None, None, None,
-                *_camera_outputs(ctx, res[9] if ctx.camera else None, 16))
 
 
 def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.0, 0.0), pts_rgb=None, features_color=None,
@@ -586,6 +385,19 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
                 raise ValueError(f"flow_xyz cannot be combined with {what}")
         flow_poses = _flow_inputs(views, pts_xyz, flow_xyz, flow_cameras, view_ids, _background(bg_color, device), sh_degree,
                                   include)
+    H, W = int(views[0].image_height), int(views[0].image_width)
+    if any((int(s.image_height), int(s.image_width)) != (H, W) for s in views):
+        raise ValueError("render_views needs one image size for all views")
+    camera = cams[0] is not None
+    flat = [pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
+            rotations] + (list(cams) if camera else []) + ([flow_xyz] if flow_xyz is not None else [])
+
+    def node(tgt):  # render_clouds' node, one cloud rendered by the views calls
+        if P == 0:
+            raise RuntimeError("render_views needs at least one Gaussian")
+        meta = ((views,), bool(return_depth), tgt, bool(return_alpha), aa, bool(ssim), camera, bool(return_median_depth),
+                bool(return_normal), (flow_poses,) if flow_xyz is not None else None, True, sync_gradients)
+        return _RasterizeClouds.apply(meta, *flat)
     if targets is not None:
         if return_depth:
             raise ValueError("targets and return_depth cannot be combined")
@@ -595,11 +407,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
             raise ValueError("targets and return_median_depth cannot be combined")
         if return_normal:
             raise ValueError("targets and return_normal cannot be combined")
-        (loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels, loss_l1,
-         ssim_v) = _RasterizeViewsLoss.apply(
-            pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, targets["rgb"], targets.get("embed"), sync_gradients, targets.get("depth"), targets.get("mask"), aa,
-            bool(ssim), *cams)
+        loss_rgb, loss_embed, color, feat_img, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim_v = node([targets])
         ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
                "radii": radii, "loss_rgb": loss_rgb, "loss_embed": loss_embed}
         if targets.get("depth") is not None:
@@ -632,10 +440,7 @@ def render_views(cameras, pts_xyz, rotations, scales, opacity, bg_color=(0.0, 0.
         normal = out[-1 - nf].unsqueeze(0) if return_normal else None
         flow = out[-1].unsqueeze(0) if flow_xyz is not None else None
     else:
-        color, feat_img, radii, depth, alpha, med_depth, med_id, normal, flow = _RasterizeViews.apply(
-            pts_xyz, screenspace_points, features_color, pts_rgb if features_color is None else None, feat, opacity, scales,
-            rotations, views, bool(return_depth), bool(return_alpha), sync_gradients, aa, bool(return_median_depth),
-            bool(return_normal), *cams, flow_xyz, flow_poses)
+        color, feat_img, radii, depth, alpha, med_depth, med_id, normal, flow = node(None)
     ret = {"render": color, "render_embed": feat_img if include else None, "viewspace_points": screenspace_points,
            "radii": radii}
     if return_depth:
@@ -1657,12 +1462,15 @@ _CLOUD_INPUTS = 8  # per cloud: means3D, means2D [V,P,3], sh, colors, feature, o
 
 class _RasterizeClouds(torch.autograd.Function):
     """render_clouds' node.  meta = (views per cloud, return_depth, targets per cloud or None, return_alpha, antialiasing,
-    ssim, camera, return_median, return_normal, flow).  flow: None, or per cloud None or its next-frame poses (a list of
+    ssim, camera, return_median, return_normal, flow[, views_call, sync_gradients]).  flow: None, or per cloud None or its next-frame poses (a list of
     (viewmatrix, projmatrix) or None per view, or None for the views' own cameras) with that cloud's flow_xyz among the inputs,
     behind every other input.  Outputs per cloud: (color, feature image, radii, depth, alpha, median depth, median id, normal,
     flow), or
     with targets (loss_rgb, loss_embed, color, feature image, radii, loss_depth, loss_mask, depth_pixels, loss_l1, ssim) with
-    gradients through the losses only."""
+    gradients through the losses only.  views_call: one cloud, rendered by the views calls (render_views').
+    sync_gradients (with views_call): None, True or a process group; the
+    backward then sums the per-Gaussian gradients over the ranks in one packed all-reduce, started as soon as the blend stage
+    has made the feature gradients final."""
 
     @staticmethod
     def forward(ctx, meta, *flat):
@@ -1714,7 +1522,8 @@ class _RasterizeClouds(torch.autograd.Function):
         include = clouds[0]["feature"] is not None
         outs, streams = rasterize_clouds_raw(clouds, degree, include, cloud_views[0][0].scale_modifier, return_depth=return_depth,
                                              debug=cloud_views[0][0].debug, return_alpha=return_alpha, antialiasing=antialiasing,
-                                             return_median=return_median, return_normal=return_normal)
+                                             return_median=return_median, return_normal=return_normal,
+                                             views_call=len(meta) > 10 and meta[10])
         for b, c in enumerate(clouds):
             color, feat_img, depth, alpha, med_depth, med_id, normal, flow = c["out_buffers"]
             radii = torch.stack([o[3] for o in outs[b]])
@@ -1750,6 +1559,7 @@ class _RasterizeClouds(torch.autograd.Function):
     def backward(ctx, *grads):
         cloud_views, return_depth, targets, return_alpha, antialiasing, ssim, camera, return_median, return_normal = ctx.meta[:9]
         flows = ctx.meta[9]
+        views_call, group = ctx.meta[10:] if len(ctx.meta) > 10 else (False, None)
         saved = ctx.saved_tensors
         dev = saved[0].device
         B = len(cloud_views)
@@ -1792,8 +1602,23 @@ class _RasterizeClouds(torch.autograd.Function):
             clouds.append(c)
         # the raw call reads only the blend inputs of the views, their capacity and state (`outs`)
         outs = [[(R, None, None, radii, geom, binb, img) for (R, radii, geom, binb, img) in st] for st in ctx.state]
+        after_blend = None
+        if group is not None:
+            # view-parallel multi-GPU: the one exchange of the path, a SUM all-reduce of the packed buffer; the feature field
+            # (final after the blend stage) is already travelling while the per-Gaussian kernel produces the other fields.
+            # A view's camera gradients are complete on the rank that rendered it.
+            c = clouds[0]
+            P, M = c["means3D"].shape[0], c["sh"].shape[1] if c["sh"] is not None else 0
+            F = int(c["feature"].shape[1]) if c["feature"] is not None else 0
+            pk = PackedGradients(P, F, M, dev, colors=c["colors"] is not None, zero=False)  # every row is written
+            grp = None if group is True else group
+            c["accumulate_into"] = pk.views
+            after_blend = lambda: pk.all_reduce_begin(grp)  # noqa: E731
         res = rasterize_clouds_backward_raw(clouds, outs, ctx.streams, ctx.degree, ctx.include, cloud_views[0][0].scale_modifier,
-                                            debug=cloud_views[0][0].debug, antialiasing=antialiasing, camera_grads=camera)
+                                            debug=cloud_views[0][0].debug, antialiasing=antialiasing, camera_grads=camera,
+                                            after_blend=after_blend, views_call=views_call)
+        if group is not None:
+            pk.all_reduce_finish(grp)
         ret = [None]
         for b, r in enumerate(res):
             P = clouds[b]["means3D"].shape[0]

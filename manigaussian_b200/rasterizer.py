@@ -938,69 +938,17 @@ def rasterize_views_raw(views, means3D, colors, language_feature, opacity, scale
     in pixels, blended with the colour's weights; channel 2 is 0; C ABI mgs_render_options.flow; out_buffers[7] [V,3,H,W]
     when given), with `flow_poses` (per view None or the next frame's (viewmatrix, projmatrix)) the pose each view projects
     the next means with.  Not with `return_normal`, `planar_depth` or `depth_mask`."""
-    L = _b.lib()
-    dev = means3D.device
     if not means3D.is_cuda:
         raise RuntimeError("manigaussian_b200 runs on CUDA tensors only (there is no CPU path)")
-    P = means3D.size(0)
-    if P == 0:
+    if means3D.size(0) == 0:
         raise RuntimeError("rasterize_views_raw needs at least one Gaussian")
-    means3D, colors, language_feature, opacity = (_prep(x, dev) for x in (means3D, colors, language_feature, opacity))
-    scales, rotations, cov3D_precomp, sh = (_prep(x, dev) for x in (scales, rotations, cov3D_precomp, sh))
-    F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
-    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
-    V = len(views)
-    pln = _planar_flag(views, planar_depth, return_normal)
-    _check_flow(flow_means3D, return_normal, pln, depth_mask)
-    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
-    main = torch.cuda.current_stream(dev)
-    streams = _view_streams(dev, V) if V > 1 else [main]  # a single view needs no side stream
-    di = dev.index if dev.index is not None else torch.cuda.current_device()
-    keys = [(di, P, int(s.image_width), int(s.image_height), v) for v, s in enumerate(views)]
-    capturing = torch.cuda.is_current_stream_capturing()  # inside a CUDA-graph capture: no event queries, no calibration
-    with torch.cuda.device(dev):
-        if not capturing:
-            _poll_status()
-        if capacities is None and any(k not in _CAPACITY for k in keys):
-            if capturing:
-                raise RuntimeError("render the views once before capturing them in a CUDA graph (the binning capacity is learned "
-                                   "from an eager call) or pass `capacities`")
-            _calibrate(L, views, keys, dev, P, degree, M, means3D, sh, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                       debug, oarr, farr, dcarr)
-        arr = (_b.View * V)()
-        aarr = (_b.ViewAlpha * V)() if return_alpha else None
-        darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
-        sarr = (_b.ViewSsim * V)() if ssim is not None else None
-        marr = (_b.ViewMedian * V)() if return_median else None
-        narr = (_b.ViewNormal * V)() if return_normal else None
-        status = _status_slots(V)
-        keep, outs = [], []
-        flarr = _flow_array(views, flow_means3D, flow_poses, P, dev, keep)
-        for v, s in enumerate(views):
-            if darr is not None:
-                _fill_depth_mask(darr[v], depth_mask, v)
-            if sarr is not None:
-                _fill_ssim(sarr[v], ssim, v)
-            cap = int(capacities[v]) if capacities is not None else _CAPACITY[keys[v]]
-            o, k = _forward_view(L, arr[v], s, v, dev, P, F, cap, include_feature, return_depth, out_buffers, loss_heads,
-                                 aarr[v] if return_alpha else None, marr[v] if return_median else None,
-                                 narr[v] if return_normal else None, quads=pln, wf=flarr[v] if flarr is not None else None)
-            arr[v].status = status.data_ptr() + 8 * v
-            arr[v].stream = streams[v].cuda_stream
-            keep.append(k)
-            outs.append(o)
-        rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(language_feature) if F else None, _ptr(opacity),
-                _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), 0, int(bool(debug)), main.cuda_stream)
-        tf = _device_fov(views, tan_fov, dev)
-        keep.append(tf)
-        iarr = _intrinsics_array(tf, None) if tf is not None else None
-        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, intrinsics=iarr, median=marr, normal=narr,
-                                ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
-                                flow_next=(_b.CloudFlow * 1)((_ptr(flow_means3D), None)) if flarr is not None else None,
-                                antialiasing=int(bool(antialiasing)), planar_depth=int(pln))
-        _b.check(L.mgs_forward_views(V, arr, opts, *rest), "mgs_forward_views")
-        _track_status(outs, keys, status, main, capacities is None and not capturing)
-    return outs, streams
+    cloud = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=language_feature, opacity=opacity, scales=scales,
+                 rotations=rotations, cov3D_precomp=cov3D_precomp, out_buffers=out_buffers, capacities=capacities,
+                 loss_heads=loss_heads, depth_mask=depth_mask, ssim=ssim, tan_fov=tan_fov, ortho=ortho, fisheye=fisheye,
+                 distortion=distortion, flow_means3D=flow_means3D, flow_poses=flow_poses)
+    outs, streams = rasterize_clouds_raw([cloud], degree, include_feature, scale_modifier, return_depth, debug, return_alpha,
+                                         antialiasing, return_median, return_normal, planar_depth, views_call=True)
+    return outs[0], streams
 
 
 def lift_views_raw(views, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, maps, antialiasing=False,
@@ -1455,93 +1403,25 @@ def rasterize_views_backward_raw(views, outs, streams, grads_color, grads_featur
     as given to the forward (mgs_render_options.planar_depth).  `flow_means3D` and `flow_poses`: as given to the forward, with
     `flows` (per view [3,H,W]) the flow planes it returned and `grads_flow` (per view [3,H,W] or [2,H,W], or None) their
     cotangents (C ABI mgs_render_options.flow and flow_next); the return value then gains, last, dL_dflow_means3D [P,3]."""
-    L = _b.lib()
-    dev = means3D.device
-    P = means3D.size(0)
-    means3D, colors, language_feature = (_prep(x, dev) for x in (means3D, colors, language_feature))
-    scales, rotations, cov3D_precomp, sh = (_prep(x, dev) for x in (scales, rotations, cov3D_precomp, sh))
-    F = language_feature.size(1) if (include_feature and language_feature is not None and language_feature.numel() > 0) else 0
-    M = sh.size(1) if (sh is not None and sh.numel() != 0) else 0
-    V = len(views)
-    pln = _planar_flag(views, planar_depth, grads_normal is not None)
-    _check_flow(flow_means3D, grads_normal is not None, pln, depth_mask)
     if flow_means3D is not None and flows is None:
         raise ValueError("flow cotangents need the forward's flow planes (flows)")
-    oarr, farr, dcarr = _lens_arrays(views, ortho, fisheye, distortion)
-    main = torch.cuda.current_stream(dev)
-    opts = dict(dtype=torch.float32, device=dev)
-    acc = accumulate_into or {}
-    has_sr = scales is not None and scales.numel() != 0
-    use_colors = colors is not None and colors.numel() != 0
+    cloud = dict(views=views, means3D=means3D, sh=sh, colors=colors, feature=language_feature, scales=scales, rotations=rotations,
+                 cov3D_precomp=cov3D_precomp, grad_color=grads_color, grad_feature=grads_feature, grad_depth=grads_depth,
+                 grad_alpha=grads_alpha, cot_scale=cot_scale, depth_mask=depth_mask, depth_mask_scale=depth_mask_scale, ssim=ssim,
+                 ssim_scale=ssim_scale, tan_fov=tan_fov, grad_median=grads_median, median_id=median_ids, grad_normal=grads_normal,
+                 normal=normals, ortho=ortho, fisheye=fisheye, distortion=distortion, flow_means3D=flow_means3D,
+                 flow_poses=flow_poses, flow=flows, grad_flow=grads_flow, accumulate_into=accumulate_into,
+                 means2D_per_view=means2D_per_view, shared_mean2D=means2D_per_view is None)
+    r = rasterize_clouds_backward_raw([cloud], [outs], streams, degree, include_feature, scale_modifier, debug, antialiasing,
+                                      camera_grads, planar_depth, accumulate=accumulate, after_blend=after_blend, views_call=True)[0]
+    grads = tuple(r[k] for k in ("dL_dmeans2D", "dL_dcolors", "dL_dfeature", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dsh",
+                                 "dL_dscales", "dL_drotations"))
+    if camera_grads is not None and camera_grads is not False:
+        grads += (tuple(r[k] for k in _CAMERA_GRADS if k in r),)
+    return grads + (r["dL_dflow_means3D"],) if flow_means3D is not None else grads
 
-    def out(name, shape, need=True):
-        t = acc.get(name)
-        if t is None and need:
-            if accumulate_into is not None and name not in ("dL_dmeans2D", "dL_dcov3D"):
-                raise ValueError(f"accumulate_into lacks '{name}', the gradient of an input of this render")
-            t = torch.empty(shape, **opts)
-        return t
 
-    dL_dmeans3D = out("dL_dmeans3D", (P, 3))
-    dL_dopacity = out("dL_dopacity", (P, 1))
-    dL_dscales = out("dL_dscales", (P, 3), has_sr)
-    dL_drotations = out("dL_drotations", (P, 4), has_sr)
-    dL_dsh = out("dL_dsh", (P, M, 3), M > 0)
-    dL_dfeature = out("dL_dfeature", (P, F), F > 0)
-    dL_dcolors = out("dL_dcolors", (P, 3), use_colors)
-    dL_dcov3D = out("dL_dcov3D", (P, 6), cov3D_precomp is not None and cov3D_precomp.numel() != 0)
-    shared = means2D_per_view is None
-    m2d = out("dL_dmeans2D", (P, 3)) if shared else means2D_per_view
-    with torch.cuda.device(dev):
-        arr = (_b.View * V)()
-        aarr = (_b.ViewAlpha * V)() if grads_alpha is not None else None
-        darr = (_b.ViewDepthMask * V)() if depth_mask is not None else None
-        dscale = _prep(depth_mask_scale, dev)
-        sarr = (_b.ViewSsim * V)() if ssim is not None else None
-        sscale = _prep(ssim_scale, dev)
-        keep = [dscale, sscale]
-        marr = _median_array(grads_median, median_ids, V, dev, keep)
-        narr = _normal_array(grads_normal, normals, V, dev, keep)
-        flarr = _flow_array(views, flow_means3D, flow_poses, P, dev, keep, flows, grads_flow)
-        dL_dflow = torch.empty((P, 3), **opts) if flarr is not None else None
-        for v, s in enumerate(views):
-            w = arr[v]
-            if darr is not None:
-                _fill_depth_mask(darr[v], depth_mask, v, dscale)
-            if aarr is not None:
-                ga = _prep(grads_alpha[v], dev)
-                aarr[v].dL_dpix_alpha = _ptr(ga)
-                keep.append(ga)
-            keep.append(_backward_view(L, w, s, outs[v], dev, P, grads_color[v],
-                                       grads_feature[v] if (F and grads_feature is not None) else None,
-                                       grads_depth[v] if grads_depth is not None else None,
-                                       narr is not None or pln or flarr is not None))
-            w.dL_dmean2D = _ptr(m2d) if shared else _ptr(m2d[v])
-            w.stream = streams[v].cuda_stream
-            if cot_scale is not None:
-                w.cot_scale = cot_scale.data_ptr() + 8 * v
-            if sarr is not None:
-                _fill_ssim(sarr[v], ssim, v, w, sscale)
-        tf = _device_fov(views, tan_fov, dev)
-        cam, carr = _camera_grads(L, camera_grads, [P] * V, dev, keep, tf is not None)
-        iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
-        keep.append(tf)
-        opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, camera_grad=carr, intrinsics=iarr, median=marr,
-                                normal=narr, ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
-                                flow_next=(_b.CloudFlow * 1)((_ptr(flow_means3D), _ptr(dL_dflow))) if flarr is not None else None,
-                                antialiasing=int(bool(antialiasing)), planar_depth=int(pln))
-        for stages in ((1, 2) if after_blend is not None else (3,)):
-            rest = (P, int(degree), M, F, _ptr(means3D), _ptr(sh) if M else None, _ptr(colors), _ptr(language_feature) if F else None,
-                    _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(dL_dmeans3D), _ptr(dL_dopacity),
-                    _ptr(dL_dcolors), _ptr(dL_dfeature) if F else None, _ptr(dL_dcov3D), _ptr(dL_dsh) if M else None,
-                    _ptr(dL_dscales) if has_sr else None, _ptr(dL_drotations) if has_sr else None,
-                    int(shared), int(bool(accumulate)), stages, int(bool(debug)), main.cuda_stream)
-            _b.check(L.mgs_backward_views(V, arr, opts, *rest), "mgs_backward_views")
-            if stages == 1:
-                after_blend()
-    grads = (m2d, dL_dcolors, dL_dfeature, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)
-    grads = grads + (cam,) if cam is not None else grads
-    return grads + (dL_dflow,) if dL_dflow is not None else grads
+_CAMERA_GRADS = ("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov")
 
 
 def _median_array(grads, ids, V, dev, keep):
@@ -1658,7 +1538,7 @@ def _prep_clouds(clouds, dev, include_feature):
 
 
 def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, return_depth=False, debug=False, return_alpha=False,
-                         antialiasing=False, return_median=False, return_normal=False, planar_depth=None):
+                         antialiasing=False, return_median=False, return_normal=False, planar_depth=None, views_call=False):
     """Forward of several Gaussian clouds, each with its own views, in one C call.  clouds[b] is a dict: "views" (a sequence
     of GaussianRasterizationSettings, one image size per cloud), the tensors "means3D", "sh" or "colors", "feature"
     (optional), "opacity", "scales" + "rotations" or "cov3D_precomp", and optionally "out_buffers", "loss_heads" and
@@ -1667,7 +1547,7 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     colour and covariance modes are shared.  `return_alpha`
     appends every view's alpha plane to its ViewOut, as in rasterize_views_raw.  Returns
     (outs, streams): outs[b][v] is the ViewOut of view v of cloud b; streams are the per-view streams of all views in order.
-    Capacity history is kept per (device, P, W, H, cloud slot, view slot).  `antialiasing`: the anti-aliased projection for
+    Capacity history is kept per (device, P, W, H, view slot across the call).  `antialiasing`: the anti-aliased projection for
     every cloud (C ABI mgs_render_options.antialiasing); pass the same value to the backward.  A cloud's optional "tan_fov" [V_b,2]
     (device) is its views' field of view, as rasterize_views_raw's `tan_fov` (C ABI mgs_render_options.intrinsics).
     `return_median` appends every view's median-depth and median-id planes to its ViewOut, as in rasterize_views_raw (C ABI
@@ -1678,7 +1558,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     views (C ABI mgs_render_options.fisheye), likewise, and its optional "distortion" its distorted-pinhole views (C ABI
     mgs_render_options.distortion).  A cloud's optional "flow_means3D" [P,3] (its next-frame means) and "flow_poses" (as
     rasterize_views_raw takes them) append, last, its views' flow planes [3,H,W] (out_buffers[7] when given; C ABI
-    mgs_render_options.flow)."""
+    mgs_render_options.flow).  `views_call`: one cloud, rendered by mgs_forward_views, the C ABI's one-cloud form (the
+    backward then takes `views_call` too)."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, return_normal)
     for c in clouds:
@@ -1695,7 +1576,8 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
     main = torch.cuda.current_stream(dev)
     streams = _view_streams(dev, V) if V > 1 else [main]
     di = dev.index if dev.index is not None else torch.cuda.current_device()
-    keys = [[(di, d["P"], int(s.image_width), int(s.image_height), b, v) for v, s in enumerate(c["views"])]
+    # capacity history per view of the call, g its index across the clouds: a one-cloud call keys its views as v
+    keys = [[(di, d["P"], int(s.image_width), int(s.image_height), offsets[b] + v) for v, s in enumerate(c["views"])]
             for b, (c, d) in enumerate(zip(clouds, pc))]
     capturing = torch.cuda.is_current_stream_capturing()
     with torch.cuda.device(dev):
@@ -1751,7 +1633,13 @@ def rasterize_clouds_raw(clouds, degree, include_feature, scale_modifier=1.0, re
                                 ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
                                 flow_next=cfarr if flarr is not None else None, antialiasing=int(bool(antialiasing)),
                                 planar_depth=int(pln))
-        _b.check(L.mgs_forward_clouds(B, carr, offs, arr, opts, *rest), "mgs_forward_clouds")
+        if views_call:
+            k = carr[0]
+            _b.check(L.mgs_forward_views(V, arr, opts, k.P, int(degree), M, F, k.means3D, k.shs, k.colors_precomp, k.feature,
+                                         k.opacities, k.scales, float(scale_modifier), k.rotations, k.cov3D_precomp, *rest[4:]),
+                     "mgs_forward_views")
+        else:
+            _b.check(L.mgs_forward_clouds(B, carr, offs, arr, opts, *rest), "mgs_forward_clouds")
         flat = [o for co in outs for o in co]
         pending = not capturing and all(c.get("capacities") is None for c in clouds)
         _track_status(flat, [k for ks in keys for k in ks], status, main, pending)
@@ -1808,7 +1696,8 @@ def _clouds_fov(clouds, dev):
 
 
 def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature, scale_modifier=1.0, debug=False,
-                                  antialiasing=False, camera_grads=False, planar_depth=None):
+                                  antialiasing=False, camera_grads=False, planar_depth=None, accumulate=False, after_blend=None,
+                                  views_call=False):
     """Backward of the clouds rendered by rasterize_clouds_raw: every view's blend backward on its stream, one join, then the
     per-Gaussian stage in launches that pack whole clouds (mgs_backward_clouds).  clouds[b]: the dict given to the forward
     plus "grad_color" [V_b,3,H,W], "grad_feature" [V_b,F,H,W] (with features), optionally "grad_depth" [V_b,H,W] and
@@ -1829,13 +1718,20 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
     mgs_view_normal).  The camera models of the clouds (see rasterize_clouds_raw) go to mgs_render_options.ortho, fisheye
     and distortion.  A cloud rendered with "flow_means3D" (and "flow_poses") also takes "flow" [V_b,3,H,W],
     the planes its forward returned, and "grad_flow" [V_b,2 or 3,H,W], their cotangent (C ABI mgs_render_options.flow and flow_next);
-    its dict then holds "dL_dflow_means3D" [P,3]."""
+    its dict then holds "dL_dflow_means3D" [P,3].  A cloud's "accumulate_into" (a dict as rasterize_views_backward_raw takes it)
+    receives its sums, overwritten or, with `accumulate`, added to.  Its "means2D_per_view" [V_b,P,3] receives the per-view
+    dL_dmeans2D, or with "shared_mean2D" True its dict holds their sum [P,3].  `camera_grads` may also be a tuple of
+    caller-given outputs over every view of the call, as rasterize_views_backward_raw takes it.  `views_call`: one cloud,
+    run by mgs_backward_views, the C ABI's one-cloud form, which always computes the feature gradient; only such a call takes
+    `after_blend` (called when the feature gradients are final) and a shared dL_dmeans2D."""
     L = _b.lib()
     pln = _planar_flag([s for c in clouds for s in c["views"]], planar_depth, any(c.get("grad_normal") is not None for c in clouds))
     for c in clouds:
         _check_flow(c.get("flow_means3D"), c.get("grad_normal") is not None, pln, c.get("depth_mask"))
         if c.get("flow_means3D") is not None and c.get("flow") is None:
             raise ValueError("flow cotangents need the forward's flow planes (\"flow\")")
+    if not views_call and (after_blend is not None or any(c.get("shared_mean2D") for c in clouds)):
+        raise ValueError("after_blend and a shared dL_dmeans2D need a one-cloud views call")
     dev = clouds[0]["means3D"].device
     pc = _prep_clouds(clouds, dev, include_feature)
     F, M, B = pc[0]["F"], pc[0]["M"], len(clouds)
@@ -1855,25 +1751,37 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
         marr = None
         if any(c.get("grad_median") is not None for c in clouds):
             gm = [c["grad_median"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
-            ids = [c["median_id"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
+            ids = None if any(c.get("grad_median") is not None and c.get("median_id") is None for c in clouds) else \
+                [c["median_id"][v] if c.get("grad_median") is not None else None for c in clouds for v in range(len(c["views"]))]
             marr = _median_array(gm, ids, V, dev, keep)
         narr = None
         if any(c.get("grad_normal") is not None for c in clouds):
             gn = [c["grad_normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
-            pl = [c["normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
+            pl = None if any(c.get("grad_normal") is not None and c.get("normal") is None for c in clouds) else \
+                [c["normal"][v] if c.get("grad_normal") is not None else None for c in clouds for v in range(len(c["views"]))]
             narr = _normal_array(gn, pl, V, dev, keep)
         flarr, cfarr = _clouds_flow(clouds, pc, offsets, dev, keep, backward=True)
         for b, (c, d) in enumerate(zip(clouds, pc)):
             P, Vb = d["P"], len(c["views"])
             has_sr = _nonempty(d["scales"])
-            gr = dict(dL_dmeans3D=torch.empty((P, 3), **opts), dL_dmeans2D=torch.empty((Vb, P, 3), **opts),
-                      dL_dopacity=torch.empty((P, 1), **opts),
-                      dL_dscales=torch.empty((P, 3), **opts) if has_sr else None,
-                      dL_drotations=torch.empty((P, 4), **opts) if has_sr else None,
-                      dL_dsh=torch.empty((P, M, 3), **opts) if M else None,
-                      dL_dcolors=torch.empty((P, 3), **opts) if _nonempty(d["colors"]) else None,
-                      dL_dcov3D=torch.empty((P, 6), **opts) if _nonempty(d["cov3D_precomp"]) else None,
-                      dL_dfeature=torch.empty((P, F), **opts) if (F and c.get("want_feature", True)) else None)
+            acc = c.get("accumulate_into")
+
+            def out(name, shape, need=True):
+                t = acc.get(name) if acc is not None else None
+                if t is None and need:
+                    if acc is not None and name not in ("dL_dmeans2D", "dL_dcov3D"):
+                        raise ValueError(f"accumulate_into lacks '{name}', the gradient of an input of this render")
+                    t = torch.empty(shape, **opts)
+                return t
+
+            shared = bool(c.get("shared_mean2D"))
+            m2d = out("dL_dmeans2D", (P, 3)) if shared else c.get("means2D_per_view")
+            gr = dict(dL_dmeans3D=out("dL_dmeans3D", (P, 3)), dL_dmeans2D=m2d if m2d is not None else torch.empty((Vb, P, 3), **opts),
+                      dL_dopacity=out("dL_dopacity", (P, 1)), dL_dscales=out("dL_dscales", (P, 3), has_sr),
+                      dL_drotations=out("dL_drotations", (P, 4), has_sr), dL_dsh=out("dL_dsh", (P, M, 3), M > 0),
+                      dL_dcolors=out("dL_dcolors", (P, 3), _nonempty(d["colors"])),
+                      dL_dcov3D=out("dL_dcov3D", (P, 6), _nonempty(d["cov3D_precomp"])),
+                      dL_dfeature=out("dL_dfeature", (P, F), views_call or c.get("want_feature", True)) if F else None)
             if "dL_dflow_means3D" in d:
                 gr["dL_dflow_means3D"] = d["dL_dflow_means3D"]
             grads.append(gr)
@@ -1883,8 +1791,9 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             k.feature = _ptr(d["feature"]) if F else None
             k.scales, k.rotations, k.cov3D_precomp = _ptr(d["scales"]), _ptr(d["rotations"]), _ptr(d["cov3D_precomp"])
             k.dL_dmean3D, k.dL_dopacity, k.dL_dcolor = _ptr(gr["dL_dmeans3D"]), _ptr(gr["dL_dopacity"]), _ptr(gr["dL_dcolors"])
-            k.dL_dfeature, k.dL_dcov3D, k.dL_dsh = _ptr(gr["dL_dfeature"]), _ptr(gr["dL_dcov3D"]), _ptr(gr["dL_dsh"])
-            k.dL_dscale, k.dL_drot = _ptr(gr["dL_dscales"]), _ptr(gr["dL_drotations"])
+            k.dL_dfeature, k.dL_dcov3D, k.dL_dsh = _ptr(gr["dL_dfeature"]), _ptr(gr["dL_dcov3D"]), _ptr(gr["dL_dsh"]) if M else None
+            k.dL_dscale = _ptr(gr["dL_dscales"]) if has_sr else None
+            k.dL_drot = _ptr(gr["dL_drotations"]) if has_sr else None
             cot = _prep(c.get("cot_scale"), dev)
             dscale = _prep(c.get("depth_mask_scale"), dev)
             sscale = _prep(c.get("ssim_scale"), dev)
@@ -1898,7 +1807,7 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
                                            c["grad_feature"][v] if (F and c.get("grad_feature") is not None) else None,
                                            c["grad_depth"][v] if c.get("grad_depth") is not None else None,
                                            c.get("grad_normal") is not None or pln or c.get("flow_means3D") is not None))
-                w.dL_dmean2D = _ptr(gr["dL_dmeans2D"][v])
+                w.dL_dmean2D = _ptr(gr["dL_dmeans2D"]) if shared else _ptr(gr["dL_dmeans2D"][v])
                 w.stream = streams[g].cuda_stream
                 if c.get("grad_alpha") is not None:
                     ga = _prep(c["grad_alpha"][v], dev)
@@ -1911,20 +1820,31 @@ def rasterize_clouds_backward_raw(clouds, outs, streams, degree, include_feature
             keep.append(cot)
         tf = _clouds_fov(clouds, dev)
         keep.append(tf)
-        cam, camarr = _camera_grads(L, bool(camera_grads), [d["P"] for d, c in zip(pc, clouds) for _ in c["views"]], dev, keep,
+        cam, camarr = _camera_grads(L, camera_grads, [d["P"] for d, c in zip(pc, clouds) for _ in c["views"]], dev, keep,
                                     tf is not None)
         if cam is not None:
             for b, gr in enumerate(grads):
-                for name, t in zip(("dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos", "dL_dtan_fov"), cam):
-                    gr[name] = t[offsets[b]:offsets[b + 1]]
-        rest = (int(degree), M, F, float(scale_modifier), 0, int(bool(debug)), main.cuda_stream)
+                for name, t in zip(_CAMERA_GRADS, cam):
+                    gr[name] = t[offsets[b]:offsets[b + 1]] if (t is not None and not views_call) else t
+        rest = (int(degree), M, F, float(scale_modifier), int(bool(accumulate)), int(bool(debug)), main.cuda_stream)
         oarr, farr, dcarr = _clouds_lens(clouds)
         iarr = _intrinsics_array(tf, cam[3] if cam is not None else None) if tf is not None else None
         opts = _b.RenderOptions(alpha=aarr, depth_mask=darr, ssim=sarr, camera_grad=camarr, intrinsics=iarr, median=marr,
                                 normal=narr, ortho=oarr, fisheye=farr, distortion=dcarr, flow=flarr,
                                 flow_next=cfarr if flarr is not None else None, antialiasing=int(bool(antialiasing)),
                                 planar_depth=int(pln))
-        _b.check(L.mgs_backward_clouds(B, carr, offs, arr, opts, *rest), "mgs_backward_clouds")
+        if views_call:
+            k = carr[0]
+            for stages in ((1, 2) if after_blend is not None else (3,)):
+                _b.check(L.mgs_backward_views(V, arr, opts, k.P, int(degree), M, F, k.means3D, k.shs if M else None, k.colors_precomp,
+                                              k.feature, k.scales, float(scale_modifier), k.rotations, k.cov3D_precomp, k.dL_dmean3D,
+                                              k.dL_dopacity, k.dL_dcolor, k.dL_dfeature, k.dL_dcov3D, k.dL_dsh, k.dL_dscale, k.dL_drot,
+                                              int(bool(clouds[0].get("shared_mean2D"))), *rest[4:5], stages, *rest[5:]),
+                         "mgs_backward_views")
+                if stages == 1:
+                    after_blend()
+        else:
+            _b.check(L.mgs_backward_clouds(B, carr, offs, arr, opts, *rest), "mgs_backward_clouds")
     return grads
 
 
