@@ -1346,6 +1346,10 @@ int mgs_activate_backward(int P, int F,
  *             with the 0.5 W / 0.5 H factors, dL/dconic b the half-weight off-diagonal term), "gn" f32[P][4] (scratch sized
  *             by mgs_backward_scratch_bytes_normal only: the normal plane's dL/dn {x, y, z, 0}, or planar depth's quad
  *             gradient, or flow's)
+ *   visibility_backward : one view's backward scratch of mgs_visibility_views_backward (its dL_dmean2D) after the call,
+ *             P_or_R_or_width = P, height = Q: "gb" f32[P][12] (the blend-stage records as in scratch, slots 0..5 written
+ *             where the call asks for a cloud or camera gradient), "duv" f32[Q][2] (each point's dL/duv through T, written
+ *             where it asks for a point or camera gradient)
  * Returns 0, or MGS_ERR_INVALID_ARG for an unknown name.
  */
 int mgs_state_array(const char* which_state, const char* name, char* state, int P_or_R_or_width, int height,

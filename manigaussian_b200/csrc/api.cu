@@ -1931,6 +1931,9 @@ int mgs_state_array(const char* which_state, const char* name, char* state, int 
 		float* gb; float* gn;
 		carve_scratch(state, a0, gb, gn);
 		if (n == "gb") p = gb; else if (n == "gn") p = gn;
+	} else if (w == "visibility_backward") {
+		VisBwdScratch s = VisBwdScratch::carve(state, (size_t)a0, (size_t)a1);
+		if (n == "gb") p = s.gb; else if (n == "duv") p = s.duv;
 	}
 	if (!p) return fail(MGS_ERR_INVALID_ARG, "unknown state array " + w + "/" + n);
 	*out_ptr = p;

@@ -1104,14 +1104,16 @@ def visibility_views_raw(views, means3D, opacity, scales, rotations, scale_modif
 
 
 def visibility_views_backward_raw(state, points, means3D, opacity, scales, rotations, scale_modifier, cov3D_precomp, T, grad_T,
-                                  grad_uv, grad_depth, want_points=True, want_cloud=True, camera_grads=False):
+                                  grad_uv, grad_depth, want_points=True, want_cloud=True, camera_grads=False,
+                                  return_scratch=False):
     """Backward of visibility_views_raw (C ABI mgs_visibility_views_backward).  `state`: the fifth result of that call with
     keep_state=True; points, the cloud and `T` (its transmittance) as given to and returned by it.  grad_T [V,Q], grad_uv
     [V,Q,2] and grad_depth [V,Q]: the cotangents, each None for none.  Returns (dL_dpoints [Q,3], dL_dmeans3D [P,3],
     dL_dopacity [P,1], dL_dscales [P,3], dL_drotations [P,4], camera), each gradient None where not wanted: `want_points`, and
     `want_cloud`, a bool or four in that order (scales and rotations are None without scales too).  camera is None, or with
     camera_grads=True (dL_dviewmatrix [V,16], dL_dprojmatrix [V,16], dL_dcampos [V,3], dL_dtan_fov [V,2], None without a
-    device field of view).  Nothing is read back to the host."""
+    device field of view).  Nothing is read back to the host.  `return_scratch`: also return, seventh, the per-view backward
+    scratch [V, bytes] the call wrote (its "visibility_backward" arrays of state_array)."""
     L = _b.lib()
     dev = means3D.device
     P, Q = state["P"], state["Q"]
@@ -1148,7 +1150,7 @@ def visibility_views_backward_raw(state, points, means3D, opacity, scales, rotat
             _ptr(opacity), _ptr(scales), float(scale_modifier), _ptr(rotations), _ptr(cov3D_precomp), _ptr(T), _ptr(grad_T),
             _ptr(grad_uv), _ptr(grad_depth), _ptr(dpts), _ptr(cloud[0]), _ptr(cloud[1]), _ptr(cloud[2]), _ptr(cloud[3]), None,
             carr, int(state["debug"]), main.cuda_stream), "mgs_visibility_views_backward")
-    return (dpts,) + tuple(cloud) + (cam,)
+    return (dpts,) + tuple(cloud) + (cam,) + ((scratch,) if return_scratch else ())
 
 
 def _ray_call(views, pixels, tan_fov, ortho, fisheye, distortion):

@@ -91,13 +91,19 @@ def outputs(points, means3D, opacities, view, accepted, scales=None, rotations=N
     depth = F64.view_space(points, view)[:, 2]
     S = P64.covariance(scales, rotations) if cov3D is None else P64.packed_cov(cov3D)
     mu, conic, s = _screen_conic(means3D, S, view, antialias)
+    return uv, depth, screen_transmittance(uv, mu, conic, opacities.reshape(-1) * s, accepted)
+
+
+def screen_transmittance(uv, mu, conic, opacity, accepted):
+    """T [Q] = prod (1 - alpha_i) over each point's accepted Gaussians, from the points' uv [Q,2] and the Gaussians' screen
+    means [P,2], conics (A, B, C) [P,3] and (effective) opacities [P]: the screen-space half of `outputs`"""
     qi = np.concatenate([np.full(len(a), q, np.int64) for q, a in enumerate(accepted)] + [np.zeros(0, np.int64)])
     gi = np.concatenate(list(accepted) + [np.zeros(0, np.int64)])
     qi, gi = torch.as_tensor(qi), torch.as_tensor(gi)
     d = mu[gi] - uv[qi]
     A, B, C = conic[gi].unbind(-1)
     power = -0.5 * (A * d[:, 0] ** 2 + C * d[:, 1] ** 2) - B * d[:, 0] * d[:, 1]
-    a = opacities.reshape(-1)[gi] * s[gi] * torch.exp(power)
+    a = opacity[gi] * torch.exp(power)
     alpha = a - (a - torch.clamp(a, max=R64.ALPHA_MAX)).detach()  # the 0.99 clamp passes the gradient through
-    logT = torch.zeros(points.shape[0], dtype=D64).index_add(0, qi, torch.log1p(-alpha))
-    return uv, depth, torch.exp(logT)
+    logT = torch.zeros(uv.shape[0], dtype=D64).index_add(0, qi, torch.log1p(-alpha))
+    return torch.exp(logT)
